@@ -260,19 +260,22 @@ int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, 
 
 /* logits[M,d_out] = W3·relu(W2·relu(W1·obs^T)) with bf16 storage, fp32 accumulation on wgmma
  * tensor cores (TMA-fed warp-specialised CTAs), activations rounded to bf16 between layers.
- * W_l is [d_l, d_{l-1}] row-major (nn.Linear layout).  This build: M % 128 == 0, d_in % 64 == 0,
- * d_hidden % 256 == 0, d_out == 64 (KTB_ERR_UNSUPPORTED otherwise).  Rows are processed in chunks;
- * for chunks with rows % 256 == 0 layer 2 and the head run as ONE kernel (the second hidden activation
- * never leaves the SM), other chunks use three GEMM launches — results agree within one bf16 ulp.
- * `scratch` holds 2*M_chunk*d_hidden bf16 (see ktb_mlp_scratch_bytes).  Replaces the user's
- * nn.Sequential policy inside execute_callable_async (kt/serving/http_server.py:1845-1891). */
+ * W_l is [d_l, d_{l-1}] row-major (nn.Linear layout).  This build: any M, d_in % 64 == 0,
+ * d_hidden % 256 == 0 (KTB_ERR_ARG otherwise), d_out == 64 (KTB_ERR_UNSUPPORTED otherwise); every
+ * pointer 16-byte aligned (KTB_ERR_ARG).  Rows are processed in chunks (16 896 rows by default), each
+ * layer of a chunk as one GEMM launch over 128-row tiles; a tile is computed the same way whatever the
+ * chunking, so every chunk size and every form below give bit-identical logits.  Each layer's result
+ * is act(fp32 sum of the exact bf16 products) rounded to nearest-even bf16.  Writes stay inside
+ * logits[M*d_out] and `scratch`, which holds 2*min(M, chunk)*d_hidden bf16 (ktb_mlp_scratch_bytes).
+ * Replaces the user's nn.Sequential policy inside execute_callable_async
+ * (kt/serving/http_server.py:1845-1891). */
 size_t ktb_mlp_scratch_bytes(size_t M, int d_hidden);
 int ktb_mlp_bf16(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
                  const void* W1, const void* W2, const void* W3, void* logits, void* scratch,
                  uintptr_t stream);
 /* Scatter-fused form for a rank whose observations live on the ROOT GPU: row chunks are pulled
- * peer → local into `stage` (ktb_mlp_stage_bytes, double-buffered) on a library side stream while
- * the previous chunk computes; `logits` may be a peer pointer (fused gather). */
+ * peer → local into `stage` (ktb_mlp_stage_bytes, double-buffered; NULL is KTB_ERR_ARG) on a library
+ * side stream while the previous chunk computes; `logits` may be a peer pointer (fused gather). */
 size_t ktb_mlp_stage_bytes(size_t M, int d_in);
 int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d_hidden, int d_out,
                         const void* W1, const void* W2, const void* W3, void* logits, void* scratch,
@@ -282,7 +285,11 @@ int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d
  * chunk_elems = chunk_rows * d_in into stage_local, double-buffered by call parity with stride stage_stride):
  * before each row chunk's GEMMs a one-warp kernel waits in-stream for ready[chunk] >= seq; the logits are stored
  * straight into `logits` (a peer pointer into the root's result: fused gather) and ack[rank] = seq is published in
- * the root's control block behind the last chunk.  Root NVLink egress carries posted writes only. */
+ * the root's control block behind the last chunk.  Root NVLink egress carries posted writes only.
+ * Requires M % 128 == 0 (a root routes other shards to the staged form), chunk_rows a positive multiple
+ * of 128, ceil(M / chunk_rows) <= 64 and M*d_in*2 <= stage_stride (KTB_ERR_ARG otherwise).  `scratch`
+ * holds 2*min(chunk_rows, M)*d_hidden bf16: it follows this call's chunk_rows, not the chunk of
+ * ktb_mlp_scratch_bytes. */
 int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
                         int d_out, const void* W1, const void* W2, const void* W3, void* logits, void* scratch,
                         void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,

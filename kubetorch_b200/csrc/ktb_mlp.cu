@@ -109,11 +109,13 @@ struct MlpSmem {
 };
 
 // C[m0:m0+128, n0:n0+BLOCK_N] = act(A[m0:.., :K] · B[n0:.., :K]ᵀ), one output tile per CTA.  blockIdx.x walks N, so
-// the CTAs of one 128-row block run side by side and read their A tile from L2 once.
+// the CTAs of one 128-row block run side by side and read their A tile from L2 once.  A has `rows` rows (the outer
+// dimension of map_a): TMA zero-fills the rows of the last row block past the end (and still counts the whole box
+// toward complete_tx), and the epilogue stores only rows < rows.
 template <int BLOCK_N, int STAGES, bool RELU>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     gemm_bf16_tn_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                              __nv_bfloat16* __restrict__ C, int ldc, int K) {
+                              __nv_bfloat16* __restrict__ C, int ldc, int K, int rows) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must be 1024-byte aligned
@@ -179,6 +181,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   // ===== epilogue: registers → (ReLU) → bf16 → global =====
   // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
   const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const bool st0 = row < rows, st1 = row + 8 < rows;
   __nv_bfloat16* c0 = C + (size_t)row * ldc + n0 + 2 * (lane & 3);
   __nv_bfloat16* c1 = c0 + (size_t)8 * ldc;
 #pragma unroll
@@ -188,8 +191,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
 #pragma unroll
       for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
     }
-    *reinterpret_cast<__nv_bfloat162*>(c0 + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
-    *reinterpret_cast<__nv_bfloat162*>(c1 + 8 * j) = __floats2bfloat162_rn(v[2], v[3]);
+    if (st0) *reinterpret_cast<__nv_bfloat162*>(c0 + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
+    if (st1) *reinterpret_cast<__nv_bfloat162*>(c1 + 8 * j) = __floats2bfloat162_rn(v[2], v[3]);
   }
 }
 
@@ -286,8 +289,8 @@ static int launch_gemm(int dev, const void* A, const void* B, void* C, size_t M,
   static std::atomic<unsigned> attr_done{0};
   rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
   if (rc) return rc;
-  dim3 grid((unsigned)(N / BLOCK_N), (unsigned)(M / kMlpBlockM));
-  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<__nv_bfloat16*>(C), ldc, K);
+  dim3 grid((unsigned)(N / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
+  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<__nv_bfloat16*>(C), ldc, K, (int)M);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
@@ -316,7 +319,6 @@ static int mlp_run(int dev, const void* obs, size_t M, int d_in, int d_hidden, i
   if (rc) return rc;
   if (M == 0) return KTB_OK;
   KTB_REQUIRE(obs && W1 && W2 && W3 && logits && scratch, KTB_ERR_ARG, "ktb_mlp_bf16: null argument");
-  KTB_REQUIRE(M % kMlpBlockM == 0, KTB_ERR_ARG, "ktb_mlp_bf16: M=%zu must be a multiple of %d", M, kMlpBlockM);
   KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0, KTB_ERR_ARG, "ktb_mlp_bf16: d_in=%d must be a multiple of 64", d_in);
   KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "ktb_mlp_bf16: d_hidden=%d must be a multiple of 256",
               d_hidden);

@@ -16,8 +16,17 @@ _weight_cache = {}
 _pool = None
 
 
-def _scratch_for(dev: int, M: int, d_hidden: int) -> torch.Tensor:
-    nbytes = L.load().ktb_mlp_scratch_bytes(M, d_hidden)
+def pushed_scratch_bytes(M: int, d_hidden: int, chunk_rows: int) -> int:
+    """Scratch of ktb_mlp_bf16_pushed: two hidden activations of min(chunk_rows, M) rows.  It follows the pushed form's
+    own chunk_rows, not the tuning chunk that ktb_mlp_scratch_bytes uses for the pull forms."""
+    return 2 * min(int(chunk_rows), int(M)) * int(d_hidden) * 2
+
+
+def _scratch_for(dev: int, M: int, d_hidden: int, chunk_rows: Optional[int] = None) -> torch.Tensor:
+    if chunk_rows is None:
+        nbytes = L.load().ktb_mlp_scratch_bytes(M, d_hidden)
+    else:
+        nbytes = pushed_scratch_bytes(M, d_hidden, chunk_rows)
     buf = _scratch.get(dev)
     if buf is None or buf.numel() < nbytes:
         buf = torch.empty(nbytes, dtype=torch.uint8, device=f"cuda:{dev}")
@@ -160,7 +169,7 @@ def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, wei
                    L.arr(ctypes.c_int, list(devs)), ce_ptrs, st.stride, st.ctrl_ptrs, st.ctrl[0].data_ptr(),
                    PUSH_CHUNK_ROWS * d_in, seq, int(root_stream.cuda_stream))
     streams = {d: torch.cuda.current_stream(d) for d in devs[1:]}
-    scratch = {d: _scratch_for(d, max(e - b for b, e in bounds), d_hidden) for d in devs[1:]}
+    scratch = {d: _scratch_for(d, max(e - b for b, e in bounds), d_hidden, PUSH_CHUNK_ROWS) for d in devs[1:]}
 
     def issue(r):
         dev = devs[r]

@@ -199,8 +199,9 @@ def test_two_gpu_peer_path_matches_oracle():
     views = mlp.mlp_scatter_gather(big, *w, devices=[0, 1], transfer="push")
     torch.cuda.synchronize(0)
     torch.cuda.synchronize(1)
-    diff = (torch.cat(views).float() - ref_big.float()).abs().max().item()
-    assert diff <= 2e-2, diff        # chunking differs (fused vs unfused tail): within one bf16 ulp of the logits
+    # the pushed chunks and the single-GPU chunks split the rows differently, and every tile is computed the same way
+    # whatever the chunking: identical bits
+    assert torch.equal(torch.cat(views).cpu(), ref_big.cpu())
     dst = torch.empty(1 << 20, dtype=torch.uint8, device="cuda:1")
     src = torch.randint(0, 255, (1 << 20,), dtype=torch.uint8, device="cuda:0")
     ops.broadcast(src, [dst])

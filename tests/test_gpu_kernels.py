@@ -297,46 +297,6 @@ def test_full_size_properties(K):
     assert torch.equal(z, x)
 
 
-def _mlp_ref(obs, w1, w2, w3):
-    """fp32 evaluation of the bf16 module with bf16 rounding between layers (what ATen does)."""
-    h = torch.relu(obs.float() @ w1.float().t()).bfloat16()
-    h = torch.relu(h.float() @ w2.float().t()).bfloat16()
-    return (h.float() @ w3.float().t()).bfloat16()
-
-
-def test_mlp_wgmma_matches_recorded_reference_and_fp32(K, golden):
-    """bf16 MLP policy (config C4): tolerance rtol=2^-7, atol=1e-2 vs the reference runtime's CPU bf16
-    result and vs an fp32 evaluation (BASELINE.md §3)."""
-    from kubetorch_b200.device import mlp
-
-    inp = golden["all_inputs"]
-    obs, w1, w2, w3 = (inp[k].cuda() for k in ("mlp_obs", "mlp_w1", "mlp_w2", "mlp_w3"))
-    got = mlp.mlp_forward(obs, w1, w2, w3).cpu().float()
-    want_ref = torch.cat(golden["cases"]["mlp_bf16_256_x2"]["result"]).float()
-    want_f32 = _mlp_ref(inp["mlp_obs"], inp["mlp_w1"], inp["mlp_w2"], inp["mlp_w3"]).float()
-    torch.testing.assert_close(got, want_f32, rtol=2**-7, atol=1e-2)
-    torch.testing.assert_close(got, want_ref, rtol=2**-7, atol=1e-2)
-    # larger M (several row chunks, many tiles), random weights at the config's scale
-    g = torch.Generator().manual_seed(7)
-    M = 128 * 300
-    obs2 = torch.randn(M, 256, generator=g).bfloat16()
-    want2 = _mlp_ref(obs2, inp["mlp_w1"], inp["mlp_w2"], inp["mlp_w3"]).float()
-    got2 = mlp.mlp_forward(obs2.cuda(), w1, w2, w3).cpu().float()
-    torch.testing.assert_close(got2, want2, rtol=2**-7, atol=1e-2)
-    try:
-        # several chunks, and the staged form (row chunks pulled through a double-buffered staging area on a side
-        # stream): identical bits, every tile is computed the same way whatever the chunking
-        K.set_tuning(8, 4096)
-        assert torch.equal(mlp.mlp_forward(obs2.cuda(), w1, w2, w3).cpu().float(), got2)
-        assert torch.equal(mlp.mlp_forward(obs2.cuda(), w1, w2, w3, staged=True).cpu().float(), got2)
-    finally:
-        K.set_tuning(8, 16896)   # the shipped chunk size
-    # top-1 action agrees wherever the fp32 top-2 logit gap exceeds 2^-6 (SURVEY.md §8(d) C4)
-    top2 = want2.topk(2, dim=1).values
-    clear = (top2[:, 0] - top2[:, 1]) > 2**-6
-    assert torch.equal(got2.argmax(1)[clear], want2.argmax(1)[clear])
-
-
 def test_push_pipeline_emulated_on_one_gpu(K):
     """push/push flag pipeline with all ranks time-sliced on cuda:0 (same stream → root first): same results
     as the oracle, across consecutive calls (staging parity + ack back-pressure) and ragged shards."""
