@@ -295,6 +295,36 @@ int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, s
                         void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
                         uintptr_t stream);
 
+/* Policy form: the nn.Linear policy  Linear(d_in, d_hidden) → ReLU → Linear(d_hidden, d_hidden) → ReLU →
+ * Linear(d_hidden, d_out)  with biases, a head of any width 1 <= d_out <= 256, and greedy actions.
+ *   - Layer l is act(fp32 sum of the exact bf16 products + b_l) rounded ONCE to nearest-even bf16: the bias
+ *     joins the fp32 accumulator before the ReLU (F.linear / nn.Linear, one rounding).  This differs from
+ *     `x @ w.t() + b` written as two eager ops, which rounds twice.  ReLU is fmaxf, as in ktb_mlp_bf16.
+ *   - b1 [d_hidden], b2 [d_hidden], b3 [d_out] bf16; each may be NULL (no bias on that layer).
+ *   - logits [M, d_out] bf16 and/or actions [M] int64; either may be NULL, not both.  actions[i] =
+ *     torch.argmax(logits[i]) over the ROUNDED logits: ties go to the lowest index, NaN is greater than any
+ *     number (the first NaN wins), -0.0 == +0.0.  With logits NULL no logits are written anywhere.  Both may be
+ *     peer pointers (fused gather).
+ *   - d_out <= 0 is KTB_ERR_ARG, d_out > 256 KTB_ERR_UNSUPPORTED; d_in and d_hidden as ktb_mlp_bf16.
+ *   - logits and the biases need 2-byte alignment (a rank's rows of a root result start at b*d_out*2 bytes),
+ *     actions 8-byte; obs, weights, scratch and stage 16-byte (KTB_ERR_ARG).  scratch and stage are sized as
+ *     for ktb_mlp_bf16 / _staged (ktb_mlp_scratch_bytes, ktb_mlp_stage_bytes).
+ *   - stage == NULL is the plain form (obs local); otherwise the staged form of ktb_mlp_bf16_staged.
+ *   - Writes stay inside logits[M*d_out], actions[M], scratch and stage.  Every chunking and form gives identical
+ *     bits, and with no biases, d_out == 64 and logits only the logits equal ktb_mlp_bf16's bit for bit. */
+int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                        const void* W1, const void* b1, const void* W2, const void* b2,
+                        const void* W3, const void* b3, void* logits, int64_t* actions,
+                        void* scratch, void* stage, uintptr_t stream);
+/* Push-fed policy form: ktb_mlp_bf16_pushed's contract (M % 128 == 0, chunk_rows, stage_stride, control blocks,
+ * scratch of 2*min(chunk_rows, M)*d_hidden bf16) with the biases and outputs of ktb_mlp_bf16_policy.  An empty
+ * shard (M == 0) may pass NULL outputs. */
+int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                               int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                               const void* b2, const void* W3, const void* b3, void* logits, int64_t* actions,
+                               void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                               unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,11 +14,16 @@
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one lane).
 // Activations are rounded to bf16 between layers (like the eager torch module); rows are processed
 // in chunks whose hidden activations stay resident in the 50 MB L2.
+// The policy entries (ktb_mlp_bf16_policy*) run nn.Linear layers: the same main loop, with an epilogue that adds
+// an optional bias to the fp32 accumulator before the activation, masks a head of any width up to 256, and can
+// store the greedy action of every row (mlp_policy_wgmma_kernel).
 #include "ktb_common.cuh"
 
 #include <cuda.h>
 #include <algorithm>
 #include <atomic>
+#include <climits>
+#include <cmath>
 #include <mutex>
 
 namespace ktb {
@@ -85,6 +90,22 @@ struct Wgmma<256> {
 };
 
 template <>
+struct Wgmma<128> {
+  __device__ __forceinline__ static void mma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(scale_d));
+  }
+};
+
+template <>
 struct Wgmma<64> {
   __device__ __forceinline__ static void mma(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t scale_d) {
     asm volatile(
@@ -108,14 +129,14 @@ struct MlpSmem {
   static constexpr int kTotal = kBarrierOff + 2 * STAGES * 8 + 1024 /* alignment slack */;
 };
 
-// C[m0:m0+128, n0:n0+BLOCK_N] = act(A[m0:.., :K] · B[n0:.., :K]ᵀ), one output tile per CTA.  blockIdx.x walks N, so
-// the CTAs of one 128-row block run side by side and read their A tile from L2 once.  A has `rows` rows (the outer
-// dimension of map_a): TMA zero-fills the rows of the last row block past the end (and still counts the whole box
-// toward complete_tx), and the epilogue stores only rows < rows.
-template <int BLOCK_N, int STAGES, bool RELU>
-__global__ void __launch_bounds__(kMlpThreads, 1)
-    gemm_bf16_tn_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                              __nv_bfloat16* __restrict__ C, int ldc, int K, int rows) {
+// The main loop every MLP GEMM kernel shares: the fp32 tile A[m0:m0+128, :K] · B[n0:n0+BLOCK_N, :K]ᵀ.  The TMA
+// producer (warp 8, one lane) fills the STAGES-deep ring and then returns false; each consumer thread returns true
+// with its warpgroup's 64 x BLOCK_N accumulators in acc.  A has `rows` rows (the outer dimension of map_a) and B has
+// N rows: TMA zero-fills the rows of a box past either end (and still counts the whole box toward complete_tx), so
+// the accumulators of those rows and columns are 0 and the epilogue decides what to store.
+template <int BLOCK_N, int STAGES>
+__device__ __forceinline__ bool mlp_tile_mainloop(const CUtensorMap* map_a, const CUtensorMap* map_b, int K, int m0,
+                                                  int n0, float (&acc)[BLOCK_N / 2]) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must be 1024-byte aligned
@@ -125,8 +146,6 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int n0 = blockIdx.x * BLOCK_N;
-  const int m0 = blockIdx.y * kMlpBlockM;
   const int num_kb = K / kMlpBlockK;
 
   if (threadIdx.x == 0) {
@@ -142,23 +161,22 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   if (warp == kMlpConsumers / 32) {
     // ===== TMA producer =====
     if (lane == 0) {
-      prefetch_tensormap(&map_a);
-      prefetch_tensormap(&map_b);
+      prefetch_tensormap(map_a);
+      prefetch_tensormap(map_b);
       for (int kb = 0; kb < num_kb; ++kb) {
         const int s = kb % STAGES;
         mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
         uint8_t* a_dst = smem + (size_t)s * S::kStageBytes;
         mbar_expect_tx(&full[s], S::kStageBytes);
-        tma_load_2d(a_dst, &map_a, kb * kMlpBlockK, m0, &full[s]);
-        tma_load_2d(a_dst + S::kABytes, &map_b, kb * kMlpBlockK, n0, &full[s]);
+        tma_load_2d(a_dst, map_a, kb * kMlpBlockK, m0, &full[s]);
+        tma_load_2d(a_dst + S::kABytes, map_b, kb * kMlpBlockK, n0, &full[s]);
       }
     }
-    return;
+    return false;
   }
 
   // ===== consumer warpgroup wg: rows 64*wg .. 64*wg+63 of the tile =====
   const int wg = warp >> 2;
-  float acc[BLOCK_N / 2];
 #pragma unroll
   for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
   for (int kb = 0; kb < num_kb; ++kb) {
@@ -177,6 +195,23 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     wgmma_wait_all();
     mbar_arrive(&empty[s]);   // this thread no longer reads stage s
   }
+  return true;
+}
+
+// C[m0:m0+128, n0:n0+BLOCK_N] = act(A[m0:.., :K] · B[n0:.., :K]ᵀ), one output tile per CTA.  blockIdx.x walks N, so
+// the CTAs of one 128-row block run side by side and read their A tile from L2 once.  The epilogue stores only
+// rows < rows (A's row count).
+template <int BLOCK_N, int STAGES, bool RELU>
+__global__ void __launch_bounds__(kMlpThreads, 1)
+    gemm_bf16_tn_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                              __nv_bfloat16* __restrict__ C, int ldc, int K, int rows) {
+  const int n0 = blockIdx.x * BLOCK_N;
+  const int m0 = blockIdx.y * kMlpBlockM;
+  float acc[BLOCK_N / 2];
+  if (!mlp_tile_mainloop<BLOCK_N, STAGES>(&map_a, &map_b, K, m0, n0, acc)) return;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
 
   // ===== epilogue: registers → (ReLU) → bf16 → global =====
   // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
@@ -193,6 +228,111 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     }
     if (st0) *reinterpret_cast<__nv_bfloat162*>(c0 + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
     if (st1) *reinterpret_cast<__nv_bfloat162*>(c1 + 8 * j) = __floats2bfloat162_rn(v[2], v[3]);
+  }
+}
+
+// The order of torch.argmax: NaN above every number (the first NaN wins), otherwise the larger value, and between
+// equal values (-0.0 == +0.0) the lower column.  A strict total order on (value, column), so any combination order
+// gives the same winner.
+__device__ __forceinline__ bool argmax_before(float v, int col, float best, int best_col) {
+  const bool v_nan = v != v, best_nan = best != best;
+  if (v_nan || best_nan) return v_nan && (!best_nan || col < best_col);
+  return v > best || (v == best && col < best_col);
+}
+
+// The policy layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid, with the bias added to the fp32
+// accumulator and the sum rounded once to bf16 (nn.Linear / F.linear), and actions[row] = the argmax of the row's
+// ROUNDED values.  Bias, ReLU and both outputs are runtime choices (bias, C and actions may each be null), so one
+// instantiation per tile width serves every layer: 256 for biased hidden layers, and for the head the smallest of
+// 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows (gridDim.x == 1, required with actions)
+// and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and never an action.
+template <int BLOCK_N, int STAGES>
+__global__ void __launch_bounds__(kMlpThreads, 1)
+    mlp_policy_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                            const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ C,
+                            int64_t* __restrict__ actions, int ldc, int n_valid, int K, int rows, int relu) {
+  const int n0 = blockIdx.x * BLOCK_N;
+  const int m0 = blockIdx.y * kMlpBlockM;
+  const int lane = threadIdx.x & 31;
+  const int col0 = n0 + 2 * (lane & 3);
+  float acc[BLOCK_N / 2];
+  if (!mlp_tile_mainloop<BLOCK_N, STAGES>(&map_a, &map_b, K, m0, n0, acc)) return;
+  const int warp = threadIdx.x >> 5;
+  const int wg = warp >> 2;
+
+  // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
+  const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const bool st0 = row < rows, st1 = row + 8 < rows;
+  // a column pair is one 4-byte store where the base and an even row stride allow it; rows of an odd d_out are
+  // only 2-byte aligned and take scalar stores
+  const bool pairs = C != nullptr && (ldc & 1) == 0 && ((uintptr_t)C & 3) == 0;
+  float best[2] = {-INFINITY, -INFINITY};
+  int best_col[2] = {INT_MAX, INT_MAX};
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
+    // no add at all without a bias: -0.0 accumulators stay -0.0, as in the original kernel.  (The bias is read here
+    // rather than before the main loop: 64 more live registers would make the 256-wide instantiation spill.)
+    if (bias != nullptr) {
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        if (col + c < n_valid) {
+          const float b = __bfloat162float(bias[col + c]);
+          v[c] += b;
+          v[2 + c] += b;
+        }
+      }
+    }
+    if (relu) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
+    }
+    const __nv_bfloat162 y0 = __floats2bfloat162_rn(v[0], v[1]);
+    const __nv_bfloat162 y1 = __floats2bfloat162_rn(v[2], v[3]);
+    if (C != nullptr) {
+      __nv_bfloat16* p0 = C + (size_t)row * ldc + col;
+      __nv_bfloat16* p1 = p0 + (size_t)8 * ldc;
+      if (pairs && col + 1 < n_valid) {
+        if (st0) *reinterpret_cast<__nv_bfloat162*>(p0) = y0;
+        if (st1) *reinterpret_cast<__nv_bfloat162*>(p1) = y1;
+      } else {
+        if (st0 && col < n_valid) p0[0] = y0.x;
+        if (st1 && col < n_valid) p1[0] = y1.x;
+        if (st0 && col + 1 < n_valid) p0[1] = y0.y;
+        if (st1 && col + 1 < n_valid) p1[1] = y1.y;
+      }
+    }
+    if (actions != nullptr) {
+      const float r[4] = {__low2float(y0), __high2float(y0), __low2float(y1), __high2float(y1)};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int h = q >> 1, c = col + (q & 1);
+        if (c < n_valid && argmax_before(r[q], c, best[h], best_col[h])) {
+          best[h] = r[q];
+          best_col[h] = c;
+        }
+      }
+    }
+  }
+  if (actions != nullptr) {
+    // the 4 lanes of a quad hold the columns of the same two rows
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
+        const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
+        if (argmax_before(ov, oc, best[h], best_col[h])) {
+          best[h] = ov;
+          best_col[h] = oc;
+        }
+      }
+    }
+    if ((lane & 3) == 0) {
+      if (st0) actions[row] = best_col[0];
+      if (st1) actions[row + 8] = best_col[1];
+    }
   }
 }
 
@@ -294,6 +434,66 @@ static int launch_gemm(int dev, const void* A, const void* B, void* C, size_t M,
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
+
+template <int BLOCK_N>
+static int launch_policy(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions, size_t M,
+                         int N, int K, int ldc, bool relu, cudaStream_t stream) {
+  using S = MlpSmem<BLOCK_N, kMlpStages>;
+  static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
+  CUtensorMap ma, mb;
+  int rc = make_map(&ma, A, M, (uint64_t)K, kMlpBlockM);
+  if (rc) return rc;
+  rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, BLOCK_N);
+  if (rc) return rc;
+  auto kfn = mlp_policy_wgmma_kernel<BLOCK_N, kMlpStages>;
+  static std::atomic<unsigned> attr_done{0};
+  rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
+  if (rc) return rc;
+  dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
+  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias),
+                                                static_cast<__nv_bfloat16*>(C), actions, ldc, N, K, (int)M, relu);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
+}
+
+// Weights, biases and outputs of one MLP call.  `policy` selects the policy entries' kernels for the head (any
+// d_out <= 256, bias, actions) and for biased hidden layers; without it (the original entries, which accept no bias
+// and no actions) every layer runs gemm_bf16_tn_wgmma_kernel as before.
+struct MlpParams {
+  const void *W1, *b1, *W2, *b2, *W3, *b3;
+  void* logits;
+  int64_t* actions;
+  bool policy;
+};
+
+// One hidden layer H[rows, d_hidden] = relu(A · Wᵀ (+ b)).
+static int mlp_hidden(int dev, const void* A, const void* W, const void* b, void* H, size_t rows, int d_hidden, int K,
+                      cudaStream_t st) {
+  if (b != nullptr) return launch_policy<256>(dev, A, W, b, H, nullptr, rows, d_hidden, K, d_hidden, true, st);
+  return launch_gemm<256, true>(dev, A, W, H, rows, d_hidden, K, d_hidden, st);
+}
+
+// The head of rows [r0, r0 + rows): logits and/or actions of those rows from h2.
+static int mlp_head(int dev, const MlpParams& p, const void* h2, size_t r0, size_t rows, int d_hidden, int d_out,
+                    cudaStream_t st) {
+  void* y = p.logits ? static_cast<__nv_bfloat16*>(p.logits) + r0 * d_out : nullptr;
+  if (!p.policy) return launch_gemm<64, false>(dev, h2, p.W3, y, rows, d_out, d_hidden, d_out, st);
+  int64_t* act = p.actions ? p.actions + r0 : nullptr;
+  if (d_out <= 64) return launch_policy<64>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+  if (d_out <= 128) return launch_policy<128>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+  return launch_policy<256>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+}
+
+// The policy entries' checks of the outputs, the head width and the element-aligned pointers.
+static int mlp_check_policy_head(const char* fn, const MlpParams& p, int d_out) {
+  KTB_REQUIRE(p.logits || p.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
+  KTB_REQUIRE(d_out >= 1, KTB_ERR_ARG, "%s: d_out=%d must be positive", fn, d_out);
+  KTB_REQUIRE(d_out <= 256, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (heads up to 256 wide)", fn, d_out);
+  KTB_REQUIRE((((uintptr_t)p.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
+              "%s: logits and biases must be 2-byte aligned", fn);
+  KTB_REQUIRE(((uintptr_t)p.actions & 7) == 0, KTB_ERR_ARG, "%s: actions must be 8-byte aligned", fn);
+  return KTB_OK;
+}
 }  // namespace ktb
 
 using namespace ktb;
@@ -313,19 +513,26 @@ size_t ktb_mlp_stage_bytes(size_t M, int d_in) {
 // ktb_set_tuning(22, v): staged pulls by a pull kernel (0, default) or by copy engine (1)
 int g_mlp_stage_ce = 0;
 
-static int mlp_run(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
-                   const void* W2, const void* W3, void* logits, void* scratch, void* stage, uintptr_t stream) {
+static int mlp_run(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
+                   void* scratch, void* stage, uintptr_t stream) {
+  const char* fn = p.policy ? "ktb_mlp_bf16_policy" : "ktb_mlp_bf16";
   int rc = require_device(dev);
   if (rc) return rc;
   if (M == 0) return KTB_OK;
-  KTB_REQUIRE(obs && W1 && W2 && W3 && logits && scratch, KTB_ERR_ARG, "ktb_mlp_bf16: null argument");
-  KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0, KTB_ERR_ARG, "ktb_mlp_bf16: d_in=%d must be a multiple of 64", d_in);
-  KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "ktb_mlp_bf16: d_hidden=%d must be a multiple of 256",
+  KTB_REQUIRE(obs && p.W1 && p.W2 && p.W3 && (p.logits || p.policy) && scratch, KTB_ERR_ARG, "%s: null argument", fn);
+  KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0, KTB_ERR_ARG, "%s: d_in=%d must be a multiple of 64", fn, d_in);
+  KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "%s: d_hidden=%d must be a multiple of 256", fn,
               d_hidden);
-  KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "ktb_mlp_bf16: d_out=%d (this build carries the 64-wide head)", d_out);
-  KTB_REQUIRE((((uintptr_t)obs | (uintptr_t)W1 | (uintptr_t)W2 | (uintptr_t)W3 | (uintptr_t)logits |
-                (uintptr_t)scratch | (uintptr_t)stage) & 15) == 0,
-              KTB_ERR_ARG, "ktb_mlp_bf16: all pointers must be 16-byte aligned");
+  if (p.policy) {
+    rc = mlp_check_policy_head(fn, p, d_out);
+    if (rc) return rc;
+  } else {
+    KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (this build carries the 64-wide head)", fn, d_out);
+  }
+  const uintptr_t logits16 = p.policy ? 0 : (uintptr_t)p.logits;   // the policy head stores element by element
+  KTB_REQUIRE((((uintptr_t)obs | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | logits16 | (uintptr_t)scratch |
+                (uintptr_t)stage) & 15) == 0,
+              KTB_ERR_ARG, "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
   KTB_REQUIRE(g_mlp_chunk_rows % kMlpBlockM == 0 && g_mlp_chunk_rows > 0, KTB_ERR_ARG, "ktb_mlp_bf16: bad chunk rows");
   rc = get_encoder();
   if (rc) return rc;
@@ -337,7 +544,6 @@ static int mlp_run(int dev, const void* obs, size_t M, int d_in, int d_hidden, i
   __nv_bfloat16* h1 = static_cast<__nv_bfloat16*>(scratch);
   __nv_bfloat16* h2 = h1 + chunk * (size_t)d_hidden;
   const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(obs);
-  __nv_bfloat16* y = static_cast<__nv_bfloat16*>(logits);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(stage);
   const MapParams ident = make_params(1, 0);
   // per-call events: [0] start, [1..2] staged chunk landed (by buffer), [3..4] staging buffer consumed
@@ -378,12 +584,12 @@ static int mlp_run(int dev, const void* obs, size_t M, int d_in, int d_hidden, i
       KTB_CK(cudaStreamWaitEvent(st, evs[1 + b], 0));
       a1 = dstb;
     }
-    rc = launch_gemm<256, true>(dev, a1, W1, h1, rows, d_hidden, d_in, d_hidden, st);
+    rc = mlp_hidden(dev, a1, p.W1, p.b1, h1, rows, d_hidden, d_in, st);
     if (rc) return rc;
     if (stg) KTB_CK(cudaEventRecord(evs[3 + (int)(c & 1)], st));
-    rc = launch_gemm<256, true>(dev, h1, W2, h2, rows, d_hidden, d_hidden, d_hidden, st);
+    rc = mlp_hidden(dev, h1, p.W2, p.b2, h2, rows, d_hidden, d_hidden, st);
     if (rc) return rc;
-    rc = launch_gemm<64, false>(dev, h2, W3, y + r0 * d_out, rows, d_out, d_hidden, d_out, st);
+    rc = mlp_head(dev, p, h2, r0, rows, d_hidden, d_out, st);
     if (rc) return rc;
   }
   return KTB_OK;
@@ -405,24 +611,36 @@ __global__ void mlp_ack_kernel(unsigned long long* ack, unsigned long long seq) 
 }
 }  // namespace ktb
 
-int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_out,
-                        const void* W1, const void* W2, const void* W3, void* logits, void* scratch, void* ctrl_local,
-                        void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+static int mlp_pushed_run(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
+                          int d_out, const MlpParams& p, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                          size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const char* fn = p.policy ? "ktb_mlp_bf16_policy_pushed" : "ktb_mlp_bf16_pushed";
   int rc = require_device(dev);
   if (rc) return rc;
-  KTB_REQUIRE(stage_local && ctrl_local && ctrl_root_peer && W1 && W2 && W3 && scratch && (logits || M == 0), KTB_ERR_ARG,
-              "ktb_mlp_bf16_pushed: null argument");
-  KTB_REQUIRE(rank >= 0 && rank < 16 && seq > 0, KTB_ERR_ARG, "ktb_mlp_bf16_pushed: bad rank/seq");
-  KTB_REQUIRE(M % kMlpBlockM == 0, KTB_ERR_ARG, "ktb_mlp_bf16_pushed: M=%zu must be a multiple of %d", M, kMlpBlockM);
+  KTB_REQUIRE(stage_local && ctrl_local && ctrl_root_peer && p.W1 && p.W2 && p.W3 && scratch &&
+                  (p.logits || p.policy || M == 0),
+              KTB_ERR_ARG, "%s: null argument", fn);
+  KTB_REQUIRE(rank >= 0 && rank < 16 && seq > 0, KTB_ERR_ARG, "%s: bad rank/seq", fn);
+  KTB_REQUIRE(M % kMlpBlockM == 0, KTB_ERR_ARG, "%s: M=%zu must be a multiple of %d", fn, M, kMlpBlockM);
   KTB_REQUIRE(chunk_rows > 0 && chunk_rows % kMlpBlockM == 0, KTB_ERR_ARG,
-              "ktb_mlp_bf16_pushed: chunk_rows=%zu must be a positive multiple of %d", chunk_rows, kMlpBlockM);
+              "%s: chunk_rows=%zu must be a positive multiple of %d", fn, chunk_rows, kMlpBlockM);
   KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0 && d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG,
-              "ktb_mlp_bf16_pushed: d_in %% 64 and d_hidden %% 256 must be 0");
-  KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "ktb_mlp_bf16_pushed: d_out=%d (this build carries the 64-wide head)", d_out);
+              "%s: d_in %% 64 and d_hidden %% 256 must be 0", fn);
+  if (p.policy) {
+    if (M > 0) {   // an empty shard stores nothing: its outputs may be null
+      rc = mlp_check_policy_head(fn, p, d_out);
+      if (rc) return rc;
+    }
+    KTB_REQUIRE((((uintptr_t)stage_local | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | (uintptr_t)scratch) &
+                 15) == 0,
+                KTB_ERR_ARG, "%s: stage, weights and scratch must be 16-byte aligned", fn);
+  } else {
+    KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (this build carries the 64-wide head)", fn, d_out);
+  }
   const size_t n_chunks = (M + chunk_rows - 1) / chunk_rows;
-  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "ktb_mlp_bf16_pushed: %zu chunks exceed %d", n_chunks,
+  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: %zu chunks exceed %d", fn, n_chunks,
               KTB_PUSH_MAX_CHUNKS);
-  KTB_REQUIRE(M * (size_t)d_in * 2 <= stage_stride, KTB_ERR_ARG, "ktb_mlp_bf16_pushed: shard exceeds stage_stride");
+  KTB_REQUIRE(M * (size_t)d_in * 2 <= stage_stride, KTB_ERR_ARG, "%s: shard exceeds stage_stride", fn);
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
@@ -436,18 +654,17 @@ int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, s
       reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(stage_local) + (size_t)(seq & 1) * stage_stride);
   __nv_bfloat16* h1 = static_cast<__nv_bfloat16*>(scratch);
   __nv_bfloat16* h2 = h1 + std::min(chunk_rows, M) * (size_t)d_hidden;
-  __nv_bfloat16* y = static_cast<__nv_bfloat16*>(logits);
   size_t c = 0;
   for (size_t r0 = 0; r0 < M; r0 += chunk_rows, ++c) {
     const size_t rows = std::min(chunk_rows, M - r0);
     mlp_wait_ready_kernel<<<1, 32, 0, st>>>(ready + c, seq, status);
     KTB_CK(cudaGetLastError());
     const __nv_bfloat16* a1 = x + r0 * d_in;
-    rc = launch_gemm<256, true>(dev, a1, W1, h1, rows, d_hidden, d_in, d_hidden, st);
+    rc = mlp_hidden(dev, a1, p.W1, p.b1, h1, rows, d_hidden, d_in, st);
     if (rc) return rc;
-    rc = launch_gemm<256, true>(dev, h1, W2, h2, rows, d_hidden, d_hidden, d_hidden, st);
+    rc = mlp_hidden(dev, h1, p.W2, p.b2, h2, rows, d_hidden, d_hidden, st);
     if (rc) return rc;
-    rc = launch_gemm<64, false>(dev, h2, W3, y + r0 * d_out, rows, d_out, d_hidden, d_out, st);
+    rc = mlp_head(dev, p, h2, r0, rows, d_hidden, d_out, st);
     if (rc) return rc;
   }
   mlp_ack_kernel<<<1, 32, 0, st>>>(ack, seq);
@@ -455,15 +672,42 @@ int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, s
   return KTB_OK;
 }
 
+int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_out,
+                        const void* W1, const void* W2, const void* W3, void* logits, void* scratch, void* ctrl_local,
+                        void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr, false};
+  return mlp_pushed_run(dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
+                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+}
+
+int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
+                               int d_out, const void* W1, const void* b1, const void* W2, const void* b2,
+                               const void* W3, const void* b3, void* logits, int64_t* actions, void* scratch,
+                               void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                               unsigned long long seq, uintptr_t stream) {
+  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions, true};
+  return mlp_pushed_run(dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
+                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+}
+
 int ktb_mlp_bf16(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                  const void* W2, const void* W3, void* logits, void* scratch, uintptr_t stream) {
-  return mlp_run(dev, obs, M, d_in, d_hidden, d_out, W1, W2, W3, logits, scratch, nullptr, stream);
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr, false};
+  return mlp_run(dev, obs, M, d_in, d_hidden, d_out, p, scratch, nullptr, stream);
 }
 
 int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                         const void* W2, const void* W3, void* logits, void* scratch, void* stage, uintptr_t stream) {
   KTB_REQUIRE(stage, KTB_ERR_ARG, "ktb_mlp_bf16_staged: null stage buffer");
-  return mlp_run(dev, obs_peer, M, d_in, d_hidden, d_out, W1, W2, W3, logits, scratch, stage, stream);
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr, false};
+  return mlp_run(dev, obs_peer, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+}
+
+int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                        const void* b1, const void* W2, const void* b2, const void* W3, const void* b3, void* logits,
+                        int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions, true};
+  return mlp_run(dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
 }  // extern "C"

@@ -1,5 +1,6 @@
 """bf16 MLP policy (BASELINE config C4) on wgmma tensor cores — tensor-facing wrapper of
-ktb_mlp_bf16 and its scatter→exec→gather form."""
+ktb_mlp_bf16 / ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions) and their
+scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -43,11 +44,39 @@ def _stage_for(dev: int, M: int, d_in: int) -> torch.Tensor:
     return buf
 
 
+OUTPUTS = ("logits", "actions", "both")
+MAX_D_OUT = 256
+
+
+def _check_policy(w1, w3, biases, output) -> bool:
+    """Validate the policy arguments; True if the call needs the policy entries (a bias, a head other than 64 wide,
+    or actions), False if it is the original bias-free 64-wide logits MLP."""
+    if output not in OUTPUTS:
+        raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
+    if len(biases) != 3:
+        raise ValueError("biases must be (b1, b2, b3), each a tensor or None")
+    d_hidden, d_out = w1.shape[0], w3.shape[0]
+    if not 1 <= d_out <= MAX_D_OUT:
+        raise ValueError(f"d_out={d_out}: the policy head is 1 to {MAX_D_OUT} wide")
+    for name, b, n in zip(("b1", "b2", "b3"), biases, (d_hidden, d_hidden, d_out)):
+        if b is None:
+            continue
+        if not isinstance(b, torch.Tensor) or b.dtype != torch.bfloat16 or not b.is_cuda or not b.is_contiguous() \
+                or b.dim() != 1 or b.shape[0] != n:
+            raise ValueError(f"{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
+    return any(b is not None for b in biases) or d_out != 64 or output != "logits"
+
+
 def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor,
                 out: Optional[torch.Tensor] = None, device: Optional[int] = None,
-                stream: Optional[torch.cuda.Stream] = None, staged: Optional[bool] = None) -> torch.Tensor:
-    """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ)); bf16 storage, fp32 accumulation in registers.
-    `obs` / `out` may be peer-mapped (pull the observations / push the logits over NVLink)."""
+                stream: Optional[torch.cuda.Stream] = None, staged: Optional[bool] = None,
+                biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
+                actions: Optional[torch.Tensor] = None):
+    """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
+    each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
+    "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written) or "both"
+    (returns (logits, actions)).  `obs` / `out` / `actions` may be peer-mapped (pull the observations / push the
+    results over NVLink).  Without biases, at d_out == 64 and with logits only this is ktb_mlp_bf16."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -57,13 +86,28 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
-    if out is None:
-        out = torch.empty(M, d_out, dtype=torch.bfloat16, device=f"cuda:{dev}")
-    else:
-        ops.ensure_init({out.device.index})
+    policy = _check_policy(w1, w3, biases, output)
+    want_logits, want_actions = output != "actions", output != "logits"
+    if want_logits:
+        if out is None:
+            out = torch.empty(M, d_out, dtype=torch.bfloat16, device=f"cuda:{dev}")
+        else:
+            ops.ensure_init({out.device.index})
+    if want_actions:
+        if actions is None:
+            actions = torch.empty(M, dtype=torch.int64, device=f"cuda:{dev}")
+        else:
+            ops.ensure_init({actions.device.index})
     s = stream if stream is not None else torch.cuda.current_stream(dev)
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
+    if policy:
+        ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+        L.call("ktb_mlp_bf16_policy", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]),
+               w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), ptr(out) if want_logits else 0,
+               ptr(actions) if want_actions else 0, _scratch_for(dev, M, d_hidden).data_ptr(),
+               _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
+        return (out, actions) if output == "both" else actions if output == "actions" else out
     if staged:
         L.call("ktb_mlp_bf16_staged", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), w2.data_ptr(),
                w3.data_ptr(), out.data_ptr(), _scratch_for(dev, M, d_hidden).data_ptr(),
@@ -79,7 +123,7 @@ def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     (excluded from per-call bytes, SURVEY.md §8(d) C4)."""
     out = []
     for w in ws:
-        if w.device.index == dev:
+        if w is None or w.device.index == dev:
             out.append(w)
             continue
         key = (w.data_ptr(), w._version, dev)
@@ -131,11 +175,12 @@ def _mlp_push_state(devs: Sequence[int], shard_bytes: int) -> _MlpPushState:
     return st
 
 
-def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights) -> None:
+def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, policy=False, output="logits",
+                               actions_root=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (posted NVLink writes, flags in device memory);
-    every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits straight into the root's
-    result; the root's own shard runs on a side stream beside the scatter.  No host synchronisation, no events between
-    devices."""
+    every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or actions) straight
+    into the root's result; the root's own shard runs on a side stream beside the scatter.  No host synchronisation, no
+    events between devices.  weights[dev] = (w1, w2, w3, b1, b2, b3) on that device (biases may be None)."""
     root, n = devs[0], len(devs)
     d_in, d_hidden, d_out = obs_root.shape[1], w1.shape[0], w3.shape[0]
     st = _mlp_push_state(devs, max(e - b for b, e in bounds) * d_in * 2)
@@ -151,7 +196,9 @@ def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, wei
         st.side.wait_event(st.ev_fork)
         if e0 > b0:
             ws = weights[root]
-            mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=out_root[b0:e0], device=root, stream=st.side, staged=False)
+            mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b0:e0],
+                        device=root, stream=st.side, staged=False, biases=ws[3:], output=output,
+                        actions=None if actions_root is None else actions_root[b0:e0])
         st.ev_join.record(st.side)
         engine = SCATTER_ENGINE if n > 2 or SCATTER_ENGINE != "hybrid" else "ce"
         ptrs = [0 if t is None else t.data_ptr() for t in st.stage]
@@ -175,6 +222,14 @@ def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, wei
         dev = devs[r]
         b, e = bounds[r]
         ws = weights[dev]
+        if policy:
+            ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
+            L.call("ktb_mlp_bf16_policy_pushed", dev, st.stage[r].data_ptr(), st.stride, e - b, d_in, d_hidden, d_out,
+                   ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]),
+                   ptr(None if out_root is None else out_root[b:e]),
+                   ptr(None if actions_root is None else actions_root[b:e]), scratch[dev].data_ptr(),
+                   st.ctrl[r].data_ptr(), st.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, int(streams[dev].cuda_stream))
+            return
         L.call("ktb_mlp_bf16_pushed", dev, st.stage[r].data_ptr(), st.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ws[1].data_ptr(), ws[2].data_ptr(), out_root[b:e].data_ptr() if e > b else 0, scratch[dev].data_ptr(),
                st.ctrl[r].data_ptr(), st.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, int(streams[dev].cuda_stream))
@@ -196,25 +251,41 @@ def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, wei
 
 
 def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int],
-                       out_root: Optional[torch.Tensor] = None, transfer: str = "auto") -> List[torch.Tensor]:
+                       out_root: Optional[torch.Tensor] = None, transfer: str = "auto",
+                       biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
+                       actions_root: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
-    result buffer (gather). Returns rank-ordered views of the root result."""
+    result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
+    int64 actions views for "actions", (logits, actions) pairs for "both".  `biases` as in mlp_forward."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
+    policy = _check_policy(w1, w3, biases, output)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     d_out = w3.shape[0]
-    if out_root is None:
+    if output != "actions" and out_root is None:
         out_root = torch.empty(M, d_out, dtype=torch.bfloat16, device=obs_root.device)
+    if output == "logits":
+        actions_root = None
+    else:
+        if actions_root is None:
+            actions_root = torch.empty(M, dtype=torch.int64, device=obs_root.device)
+        if output == "actions":
+            out_root = None
     root_stream = torch.cuda.current_stream(root)
     ready = torch.cuda.Event()
     ready.record(root_stream)
     bounds = [ops.shard_bounds(M, len(devs), r) for r in range(len(devs))]
-    views = [out_root[b:e] for b, e in bounds]
-    weights = {dev: _weights_on(dev, (w1, w2, w3)) for dev in set(devs)}
+    if output == "logits":
+        views = [out_root[b:e] for b, e in bounds]
+    elif output == "actions":
+        views = [actions_root[b:e] for b, e in bounds]
+    else:
+        views = [(out_root[b:e], actions_root[b:e]) for b, e in bounds]
+    weights = {dev: _weights_on(dev, (w1, w2, w3)) + _weights_on(dev, biases) for dev in set(devs)}
     distinct = len(set(devs)) == len(devs) and len(devs) > 1
     pushable = distinct and all((e - b) % 128 == 0 for b, e in bounds) and \
         -(-max(e - b for b, e in bounds) // PUSH_CHUNK_ROWS) <= 64
@@ -223,7 +294,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights)
+        _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, policy, output, actions_root)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -242,7 +313,9 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         with torch.cuda.device(dev):
             if dev != root:
                 st.wait_event(ready)
-            mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=out_root[b:e], device=dev, stream=st)
+            mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b:e],
+                        device=dev, stream=st, biases=ws[3:], output=output,
+                        actions=None if actions_root is None else actions_root[b:e])
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

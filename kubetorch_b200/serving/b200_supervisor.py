@@ -403,8 +403,11 @@ class B200Supervisor:
             try:
                 import torch
 
+                # a shard view would drag the whole result buffer's storage along
                 if isinstance(result, torch.Tensor):
-                    result = result.clone()  # a shard view would drag the whole result buffer's storage along
+                    result = result.clone()
+                elif isinstance(result, tuple):   # the (logits, actions) of an mlp op with output="both"
+                    result = tuple(t.clone() if isinstance(t, torch.Tensor) else t for t in result)
                 return {"data": base64.b64encode(pickle.dumps(result)).decode("utf-8")}
             except Exception as e:  # noqa: BLE001
                 raise SerializationError(f"Result could not be serialized with pickle: {e}")
@@ -581,9 +584,16 @@ class B200Supervisor:
         from ..device import mlp
 
         names = list(bound)
-        obs, w1, w2, w3 = (bound[n] for n in names[:4])
+        output = spec.extra.get("output", "logits")
+        if spec.extra.get("bias", False):   # (obs, w1, b1, w2, b2, w3, b3): an nn.Linear policy
+            obs, w1, b1, w2, b2, w3, b3 = (bound[n] for n in names[:7])
+            biases = (b1, b2, b3)
+        else:
+            obs, w1, w2, w3 = (bound[n] for n in names[:4])
+            biases = (None, None, None)
         try:
-            out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer)
+            out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
+                                         biases=biases, output=output)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]
