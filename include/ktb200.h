@@ -260,6 +260,8 @@ int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, 
 
 /* logits[M,d_out] = W3·relu(W2·relu(W1·obs^T)) with bf16 storage, fp32 accumulation on wgmma
  * tensor cores (TMA-fed warp-specialised CTAs), activations rounded to bf16 between layers.
+ * ktb_mlp_bf16, _staged and _pushed are the bias-free, 64-wide, logits-only case of the policy form
+ * below (ktb_mlp_bf16_policy, _policy_pushed), run by the same kernel.
  * W_l is [d_l, d_{l-1}] row-major (nn.Linear layout).  This build: any M, d_in % 64 == 0,
  * d_hidden % 256 == 0 (KTB_ERR_ARG otherwise), d_out == 64 (KTB_ERR_UNSUPPORTED otherwise); every
  * pointer 16-byte aligned (KTB_ERR_ARG).  Rows are processed in chunks (16 896 rows by default), each
@@ -287,7 +289,8 @@ int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d
  * straight into `logits` (a peer pointer into the root's result: fused gather) and ack[rank] = seq is published in
  * the root's control block behind the last chunk.  Root NVLink egress carries posted writes only.
  * Requires M % 128 == 0 (a root routes other shards to the staged form), chunk_rows a positive multiple
- * of 128, ceil(M / chunk_rows) <= 64 and M*d_in*2 <= stage_stride (KTB_ERR_ARG otherwise).  `scratch`
+ * of 128, ceil(M / chunk_rows) <= 64, M*d_in*2 <= stage_stride and stage_local, weights and scratch
+ * 16-byte aligned (KTB_ERR_ARG otherwise); d_out == 64 (KTB_ERR_UNSUPPORTED otherwise).  `scratch`
  * holds 2*min(chunk_rows, M)*d_hidden bf16: it follows this call's chunk_rows, not the chunk of
  * ktb_mlp_scratch_bytes. */
 int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,

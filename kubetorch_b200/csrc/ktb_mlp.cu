@@ -8,15 +8,14 @@
 //     into a STAGES-deep ring guarded by mbarriers (full: TMA bytes landed, empty: consumers done),
 //   * wgmma.mma_async m64nNk16 (bf16 x bf16 → fp32) issued by two consumer warpgroups, each owning
 //     64 rows of the 128-row tile, both operands read straight from shared memory by descriptor,
-//   * an epilogue from the fp32 register accumulators: fused ReLU + bf16 rounding, global stores —
-//     the last layer's C may be a peer pointer into the root GPU's result arena, which fuses the
-//     gather into the epilogue.
+//   * an epilogue from the fp32 register accumulators: optional bias (nn.Linear), fused ReLU + bf16
+//     rounding, global stores masked to the head's width, and optionally the greedy action of every
+//     row — the last layer's outputs may be peer pointers into the root GPU's result arena, which
+//     fuses the gather into the epilogue.
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one lane).
 // Activations are rounded to bf16 between layers (like the eager torch module); rows are processed
-// in chunks whose hidden activations stay resident in the 50 MB L2.
-// The policy entries (ktb_mlp_bf16_policy*) run nn.Linear layers: the same main loop, with an epilogue that adds
-// an optional bias to the fp32 accumulator before the activation, masks a head of any width up to 256, and can
-// store the greedy action of every row (mlp_policy_wgmma_kernel).
+// in chunks whose hidden activations stay resident in the 50 MB L2.  One kernel
+// (mlp_layer_wgmma_kernel) runs every layer of every entry point.
 #include "ktb_common.cuh"
 
 #include <cuda.h>
@@ -129,7 +128,7 @@ struct MlpSmem {
   static constexpr int kTotal = kBarrierOff + 2 * STAGES * 8 + 1024 /* alignment slack */;
 };
 
-// The main loop every MLP GEMM kernel shares: the fp32 tile A[m0:m0+128, :K] · B[n0:n0+BLOCK_N, :K]ᵀ.  The TMA
+// The main loop of an MLP layer: the fp32 tile A[m0:m0+128, :K] · B[n0:n0+BLOCK_N, :K]ᵀ.  The TMA
 // producer (warp 8, one lane) fills the STAGES-deep ring and then returns false; each consumer thread returns true
 // with its warpgroup's 64 x BLOCK_N accumulators in acc.  A has `rows` rows (the outer dimension of map_a) and B has
 // N rows: TMA zero-fills the rows of a box past either end (and still counts the whole box toward complete_tx), so
@@ -198,39 +197,6 @@ __device__ __forceinline__ bool mlp_tile_mainloop(const CUtensorMap* map_a, cons
   return true;
 }
 
-// C[m0:m0+128, n0:n0+BLOCK_N] = act(A[m0:.., :K] · B[n0:.., :K]ᵀ), one output tile per CTA.  blockIdx.x walks N, so
-// the CTAs of one 128-row block run side by side and read their A tile from L2 once.  The epilogue stores only
-// rows < rows (A's row count).
-template <int BLOCK_N, int STAGES, bool RELU>
-__global__ void __launch_bounds__(kMlpThreads, 1)
-    gemm_bf16_tn_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                              __nv_bfloat16* __restrict__ C, int ldc, int K, int rows) {
-  const int n0 = blockIdx.x * BLOCK_N;
-  const int m0 = blockIdx.y * kMlpBlockM;
-  float acc[BLOCK_N / 2];
-  if (!mlp_tile_mainloop<BLOCK_N, STAGES>(&map_a, &map_b, K, m0, n0, acc)) return;
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int wg = warp >> 2;
-
-  // ===== epilogue: registers → (ReLU) → bf16 → global =====
-  // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
-  const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  const bool st0 = row < rows, st1 = row + 8 < rows;
-  __nv_bfloat16* c0 = C + (size_t)row * ldc + n0 + 2 * (lane & 3);
-  __nv_bfloat16* c1 = c0 + (size_t)8 * ldc;
-#pragma unroll
-  for (int j = 0; j < BLOCK_N / 8; ++j) {
-    float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
-    if (RELU) {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
-    }
-    if (st0) *reinterpret_cast<__nv_bfloat162*>(c0 + 8 * j) = __floats2bfloat162_rn(v[0], v[1]);
-    if (st1) *reinterpret_cast<__nv_bfloat162*>(c1 + 8 * j) = __floats2bfloat162_rn(v[2], v[3]);
-  }
-}
-
 // The order of torch.argmax: NaN above every number (the first NaN wins), otherwise the larger value, and between
 // equal values (-0.0 == +0.0) the lower column.  A strict total order on (value, column), so any combination order
 // gives the same winner.
@@ -240,17 +206,44 @@ __device__ __forceinline__ bool argmax_before(float v, int col, float best, int 
   return v > best || (v == best && col < best_col);
 }
 
-// The policy layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid, with the bias added to the fp32
+// One column pair (col, col + 1) of a layer in rows r and r + 8: y0 = act(a0 + bias, a1 + bias) of row r, y1 of row
+// r + 8, each rounded once to bf16.  A column >= n_valid gets no bias.
+__device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a3, const __nv_bfloat16* bias, int col,
+                                           int n_valid, int relu, __nv_bfloat162& y0, __nv_bfloat162& y1) {
+  float v[4] = {a0, a1, a2, a3};
+  // no add at all without a bias: -0.0 accumulators stay -0.0 (adding 0 would make them +0.0).  (The bias is read
+  // here rather than before the main loop: 64 more live registers would make the 256-wide instantiation spill.)
+  if (bias != nullptr) {
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      if (col + c < n_valid) {
+        const float b = __bfloat162float(bias[col + c]);
+        v[c] += b;
+        v[2 + c] += b;
+      }
+    }
+  }
+  if (relu) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
+  }
+  y0 = __floats2bfloat162_rn(v[0], v[1]);
+  y1 = __floats2bfloat162_rn(v[2], v[3]);
+}
+
+// One MLP layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid, with the bias added to the fp32
 // accumulator and the sum rounded once to bf16 (nn.Linear / F.linear), and actions[row] = the argmax of the row's
-// ROUNDED values.  Bias, ReLU and both outputs are runtime choices (bias, C and actions may each be null), so one
-// instantiation per tile width serves every layer: 256 for biased hidden layers, and for the head the smallest of
-// 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows (gridDim.x == 1, required with actions)
-// and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and never an action.
+// ROUNDED values.  One output tile per CTA; blockIdx.x walks N, so the CTAs of one 128-row block run side by side and
+// read their A tile from L2 once.  Only rows < rows (A's row count) are stored.  Bias, ReLU and both outputs are
+// runtime choices (bias, C and actions may each be null), so one instantiation per tile width serves every layer:
+// 256 for the hidden layers, and for the head the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one
+// CTA owns whole rows (gridDim.x == 1, required with actions) and the argmax never leaves it.  Columns >= n_valid
+// hold TMA zero fill: they are never stored and never an action.
 template <int BLOCK_N, int STAGES>
 __global__ void __launch_bounds__(kMlpThreads, 1)
-    mlp_policy_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                            const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ C,
-                            int64_t* __restrict__ actions, int ldc, int n_valid, int K, int rows, int relu) {
+    mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+                           const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ C,
+                           int64_t* __restrict__ actions, int ldc, int n_valid, int K, int rows, int relu) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -266,30 +259,27 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   // a column pair is one 4-byte store where the base and an even row stride allow it; rows of an odd d_out are
   // only 2-byte aligned and take scalar stores
   const bool pairs = C != nullptr && (ldc & 1) == 0 && ((uintptr_t)C & 3) == 0;
+  if (pairs && actions == nullptr && n0 + BLOCK_N <= n_valid) {
+    // every column of the tile is stored, in pairs, and no action is taken (every hidden-layer tile): the loop below
+    // without its per-column masks and branches
+    __nv_bfloat16* p0 = C + (size_t)row * ldc + col0;
+    __nv_bfloat16* p1 = p0 + (size_t)8 * ldc;
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      __nv_bfloat162 y0, y1;
+      layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col0 + 8 * j, n_valid, relu, y0, y1);
+      if (st0) *reinterpret_cast<__nv_bfloat162*>(p0 + 8 * j) = y0;
+      if (st1) *reinterpret_cast<__nv_bfloat162*>(p1 + 8 * j) = y1;
+    }
+    return;
+  }
   float best[2] = {-INFINITY, -INFINITY};
   int best_col[2] = {INT_MAX, INT_MAX};
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
-    float v[4] = {acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3]};
-    // no add at all without a bias: -0.0 accumulators stay -0.0, as in the original kernel.  (The bias is read here
-    // rather than before the main loop: 64 more live registers would make the 256-wide instantiation spill.)
-    if (bias != nullptr) {
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        if (col + c < n_valid) {
-          const float b = __bfloat162float(bias[col + c]);
-          v[c] += b;
-          v[2 + c] += b;
-        }
-      }
-    }
-    if (relu) {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
-    }
-    const __nv_bfloat162 y0 = __floats2bfloat162_rn(v[0], v[1]);
-    const __nv_bfloat162 y1 = __floats2bfloat162_rn(v[2], v[3]);
+    __nv_bfloat162 y0, y1;
+    layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, relu, y0, y1);
     if (C != nullptr) {
       __nv_bfloat16* p0 = C + (size_t)row * ldc + col;
       __nv_bfloat16* p1 = p0 + (size_t)8 * ldc;
@@ -415,29 +405,9 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
   return KTB_OK;
 }
 
-template <int BLOCK_N, bool RELU>
-static int launch_gemm(int dev, const void* A, const void* B, void* C, size_t M, int N, int K, int ldc,
-                       cudaStream_t stream) {
-  using S = MlpSmem<BLOCK_N, kMlpStages>;
-  static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
-  CUtensorMap ma, mb;
-  int rc = make_map(&ma, A, M, (uint64_t)K, kMlpBlockM);
-  if (rc) return rc;
-  rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, BLOCK_N);
-  if (rc) return rc;
-  auto kfn = gemm_bf16_tn_wgmma_kernel<BLOCK_N, kMlpStages, RELU>;
-  static std::atomic<unsigned> attr_done{0};
-  rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
-  if (rc) return rc;
-  dim3 grid((unsigned)(N / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
-  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<__nv_bfloat16*>(C), ldc, K, (int)M);
-  KTB_CK(cudaGetLastError());
-  return KTB_OK;
-}
-
 template <int BLOCK_N>
-static int launch_policy(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions, size_t M,
-                         int N, int K, int ldc, bool relu, cudaStream_t stream) {
+static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions, size_t M,
+                        int N, int K, int ldc, bool relu, cudaStream_t stream) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -445,7 +415,7 @@ static int launch_policy(int dev, const void* A, const void* B, const void* bias
   if (rc) return rc;
   rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, BLOCK_N);
   if (rc) return rc;
-  auto kfn = mlp_policy_wgmma_kernel<BLOCK_N, kMlpStages>;
+  auto kfn = mlp_layer_wgmma_kernel<BLOCK_N, kMlpStages>;
   static std::atomic<unsigned> attr_done{0};
   rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
   if (rc) return rc;
@@ -456,42 +426,48 @@ static int launch_policy(int dev, const void* A, const void* B, const void* bias
   return KTB_OK;
 }
 
-// Weights, biases and outputs of one MLP call.  `policy` selects the policy entries' kernels for the head (any
-// d_out <= 256, bias, actions) and for biased hidden layers; without it (the original entries, which accept no bias
-// and no actions) every layer runs gemm_bf16_tn_wgmma_kernel as before.
+// Weights, biases (each may be null) and outputs (either may be null) of one MLP call.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   void* logits;
   int64_t* actions;
-  bool policy;
 };
 
 // One hidden layer H[rows, d_hidden] = relu(A · Wᵀ (+ b)).
 static int mlp_hidden(int dev, const void* A, const void* W, const void* b, void* H, size_t rows, int d_hidden, int K,
                       cudaStream_t st) {
-  if (b != nullptr) return launch_policy<256>(dev, A, W, b, H, nullptr, rows, d_hidden, K, d_hidden, true, st);
-  return launch_gemm<256, true>(dev, A, W, H, rows, d_hidden, K, d_hidden, st);
+  return launch_layer<256>(dev, A, W, b, H, nullptr, rows, d_hidden, K, d_hidden, true, st);
 }
 
 // The head of rows [r0, r0 + rows): logits and/or actions of those rows from h2.
 static int mlp_head(int dev, const MlpParams& p, const void* h2, size_t r0, size_t rows, int d_hidden, int d_out,
                     cudaStream_t st) {
   void* y = p.logits ? static_cast<__nv_bfloat16*>(p.logits) + r0 * d_out : nullptr;
-  if (!p.policy) return launch_gemm<64, false>(dev, h2, p.W3, y, rows, d_out, d_hidden, d_out, st);
   int64_t* act = p.actions ? p.actions + r0 : nullptr;
-  if (d_out <= 64) return launch_policy<64>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
-  if (d_out <= 128) return launch_policy<128>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
-  return launch_policy<256>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+  if (d_out <= 64) return launch_layer<64>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+  if (d_out <= 128) return launch_layer<128>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+  return launch_layer<256>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
 }
 
-// The policy entries' checks of the outputs, the head width and the element-aligned pointers.
-static int mlp_check_policy_head(const char* fn, const MlpParams& p, int d_out) {
-  KTB_REQUIRE(p.logits || p.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
-  KTB_REQUIRE(d_out >= 1, KTB_ERR_ARG, "%s: d_out=%d must be positive", fn, d_out);
-  KTB_REQUIRE(d_out <= 256, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (heads up to 256 wide)", fn, d_out);
-  KTB_REQUIRE((((uintptr_t)p.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
-              "%s: logits and biases must be 2-byte aligned", fn);
-  KTB_REQUIRE(((uintptr_t)p.actions & 7) == 0, KTB_ERR_ARG, "%s: actions must be 8-byte aligned", fn);
+// The checks every MLP entry shares: the layer widths the tiles divide, the head (outputs, width, element-aligned
+// pointers; skipped for an empty call, which stores nothing and may pass null outputs) and the 16-byte alignment TMA
+// needs of every matrix it loads (`obs` is the first layer's input).
+static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p, const void* obs,
+                     const void* scratch, const void* stage) {
+  KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0, KTB_ERR_ARG, "%s: d_in=%d must be a multiple of 64", fn, d_in);
+  KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "%s: d_hidden=%d must be a multiple of 256", fn,
+              d_hidden);
+  if (M > 0) {
+    KTB_REQUIRE(p.logits || p.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
+    KTB_REQUIRE(d_out >= 1, KTB_ERR_ARG, "%s: d_out=%d must be positive", fn, d_out);
+    KTB_REQUIRE(d_out <= 256, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (heads up to 256 wide)", fn, d_out);
+    KTB_REQUIRE((((uintptr_t)p.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
+                "%s: logits and biases must be 2-byte aligned", fn);
+    KTB_REQUIRE(((uintptr_t)p.actions & 7) == 0, KTB_ERR_ARG, "%s: actions must be 8-byte aligned", fn);
+  }
+  KTB_REQUIRE((((uintptr_t)obs | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | (uintptr_t)scratch |
+                (uintptr_t)stage) & 15) == 0,
+              KTB_ERR_ARG, "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
   return KTB_OK;
 }
 }  // namespace ktb
@@ -513,27 +489,15 @@ size_t ktb_mlp_stage_bytes(size_t M, int d_in) {
 // ktb_set_tuning(22, v): staged pulls by a pull kernel (0, default) or by copy engine (1)
 int g_mlp_stage_ce = 0;
 
-static int mlp_run(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
-                   void* scratch, void* stage, uintptr_t stream) {
-  const char* fn = p.policy ? "ktb_mlp_bf16_policy" : "ktb_mlp_bf16";
+static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                   const MlpParams& p, void* scratch, void* stage, uintptr_t stream) {
   int rc = require_device(dev);
   if (rc) return rc;
   if (M == 0) return KTB_OK;
-  KTB_REQUIRE(obs && p.W1 && p.W2 && p.W3 && (p.logits || p.policy) && scratch, KTB_ERR_ARG, "%s: null argument", fn);
-  KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0, KTB_ERR_ARG, "%s: d_in=%d must be a multiple of 64", fn, d_in);
-  KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "%s: d_hidden=%d must be a multiple of 256", fn,
-              d_hidden);
-  if (p.policy) {
-    rc = mlp_check_policy_head(fn, p, d_out);
-    if (rc) return rc;
-  } else {
-    KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (this build carries the 64-wide head)", fn, d_out);
-  }
-  const uintptr_t logits16 = p.policy ? 0 : (uintptr_t)p.logits;   // the policy head stores element by element
-  KTB_REQUIRE((((uintptr_t)obs | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | logits16 | (uintptr_t)scratch |
-                (uintptr_t)stage) & 15) == 0,
-              KTB_ERR_ARG, "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
-  KTB_REQUIRE(g_mlp_chunk_rows % kMlpBlockM == 0 && g_mlp_chunk_rows > 0, KTB_ERR_ARG, "ktb_mlp_bf16: bad chunk rows");
+  KTB_REQUIRE(obs && p.W1 && p.W2 && p.W3 && scratch, KTB_ERR_ARG, "%s: null argument", fn);
+  rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, obs, scratch, stage);
+  if (rc) return rc;
+  KTB_REQUIRE(g_mlp_chunk_rows % kMlpBlockM == 0 && g_mlp_chunk_rows > 0, KTB_ERR_ARG, "%s: bad chunk rows", fn);
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
@@ -611,32 +575,19 @@ __global__ void mlp_ack_kernel(unsigned long long* ack, unsigned long long seq) 
 }
 }  // namespace ktb
 
-static int mlp_pushed_run(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
-                          int d_out, const MlpParams& p, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
-                          size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
-  const char* fn = p.policy ? "ktb_mlp_bf16_policy_pushed" : "ktb_mlp_bf16_pushed";
+static int mlp_pushed_run(const char* fn, int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                          int d_hidden, int d_out, const MlpParams& p, void* scratch, void* ctrl_local,
+                          void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
   int rc = require_device(dev);
   if (rc) return rc;
-  KTB_REQUIRE(stage_local && ctrl_local && ctrl_root_peer && p.W1 && p.W2 && p.W3 && scratch &&
-                  (p.logits || p.policy || M == 0),
-              KTB_ERR_ARG, "%s: null argument", fn);
+  KTB_REQUIRE(stage_local && ctrl_local && ctrl_root_peer && p.W1 && p.W2 && p.W3 && scratch, KTB_ERR_ARG,
+              "%s: null argument", fn);
   KTB_REQUIRE(rank >= 0 && rank < 16 && seq > 0, KTB_ERR_ARG, "%s: bad rank/seq", fn);
   KTB_REQUIRE(M % kMlpBlockM == 0, KTB_ERR_ARG, "%s: M=%zu must be a multiple of %d", fn, M, kMlpBlockM);
   KTB_REQUIRE(chunk_rows > 0 && chunk_rows % kMlpBlockM == 0, KTB_ERR_ARG,
               "%s: chunk_rows=%zu must be a positive multiple of %d", fn, chunk_rows, kMlpBlockM);
-  KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0 && d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG,
-              "%s: d_in %% 64 and d_hidden %% 256 must be 0", fn);
-  if (p.policy) {
-    if (M > 0) {   // an empty shard stores nothing: its outputs may be null
-      rc = mlp_check_policy_head(fn, p, d_out);
-      if (rc) return rc;
-    }
-    KTB_REQUIRE((((uintptr_t)stage_local | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | (uintptr_t)scratch) &
-                 15) == 0,
-                KTB_ERR_ARG, "%s: stage, weights and scratch must be 16-byte aligned", fn);
-  } else {
-    KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (this build carries the 64-wide head)", fn, d_out);
-  }
+  rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, stage_local, scratch, nullptr);
+  if (rc) return rc;
   const size_t n_chunks = (M + chunk_rows - 1) / chunk_rows;
   KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: %zu chunks exceed %d", fn, n_chunks,
               KTB_PUSH_MAX_CHUNKS);
@@ -672,11 +623,19 @@ static int mlp_pushed_run(int dev, const void* stage_local, size_t stage_stride,
   return KTB_OK;
 }
 
+// ktb_mlp_bf16, _staged and _pushed are the policy form without biases, with a 64-wide head and logits only.  Each
+// checks that narrower contract (after the device, and for the pull forms after an empty call, which returns first)
+// and then runs the policy form.
 int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_out,
                         const void* W1, const void* W2, const void* W3, void* logits, void* scratch, void* ctrl_local,
                         void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr, false};
-  return mlp_pushed_run(dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
+  const char* fn = "ktb_mlp_bf16_pushed";
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(logits || M == 0, KTB_ERR_ARG, "%s: null argument", fn);
+  KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr};
+  return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
                         ctrl_root_peer, rank, chunk_rows, seq, stream);
 }
 
@@ -685,29 +644,40 @@ int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_st
                                const void* W3, const void* b3, void* logits, int64_t* actions, void* scratch,
                                void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
                                unsigned long long seq, uintptr_t stream) {
-  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions, true};
-  return mlp_pushed_run(dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
-                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions};
+  return mlp_pushed_run("ktb_mlp_bf16_policy_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p,
+                        scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
+}
+
+static int mlp_run_64(const char* fn, int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                      const void* W1, const void* W2, const void* W3, void* logits, void* scratch, void* stage,
+                      uintptr_t stream) {
+  int rc = require_device(dev);
+  if (rc || M == 0) return rc;
+  KTB_REQUIRE(logits, KTB_ERR_ARG, "%s: null argument", fn);
+  KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
+  KTB_REQUIRE(((uintptr_t)logits & 15) == 0, KTB_ERR_ARG, "%s: logits must be 16-byte aligned", fn);
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr};
+  return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
 int ktb_mlp_bf16(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                  const void* W2, const void* W3, void* logits, void* scratch, uintptr_t stream) {
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr, false};
-  return mlp_run(dev, obs, M, d_in, d_hidden, d_out, p, scratch, nullptr, stream);
+  return mlp_run_64("ktb_mlp_bf16", dev, obs, M, d_in, d_hidden, d_out, W1, W2, W3, logits, scratch, nullptr, stream);
 }
 
 int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                         const void* W2, const void* W3, void* logits, void* scratch, void* stage, uintptr_t stream) {
   KTB_REQUIRE(stage, KTB_ERR_ARG, "ktb_mlp_bf16_staged: null stage buffer");
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr, false};
-  return mlp_run(dev, obs_peer, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  return mlp_run_64("ktb_mlp_bf16_staged", dev, obs_peer, M, d_in, d_hidden, d_out, W1, W2, W3, logits, scratch, stage,
+                    stream);
 }
 
 int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                         const void* b1, const void* W2, const void* b2, const void* W3, const void* b3, void* logits,
                         int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
-  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions, true};
-  return mlp_run(dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions};
+  return mlp_run("ktb_mlp_bf16_policy", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
 }  // extern "C"

@@ -1,6 +1,5 @@
 """bf16 MLP policy (BASELINE config C4) on wgmma tensor cores — tensor-facing wrapper of
-ktb_mlp_bf16 / ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions) and their
-scatter→exec→gather form."""
+ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions) and its scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -18,7 +17,7 @@ _pool = None
 
 
 def pushed_scratch_bytes(M: int, d_hidden: int, chunk_rows: int) -> int:
-    """Scratch of ktb_mlp_bf16_pushed: two hidden activations of min(chunk_rows, M) rows.  It follows the pushed form's
+    """Scratch of ktb_mlp_bf16_policy_pushed: two hidden activations of min(chunk_rows, M) rows.  It follows the pushed form's
     own chunk_rows, not the tuning chunk that ktb_mlp_scratch_bytes uses for the pull forms."""
     return 2 * min(int(chunk_rows), int(M)) * int(d_hidden) * 2
 
@@ -48,9 +47,8 @@ OUTPUTS = ("logits", "actions", "both")
 MAX_D_OUT = 256
 
 
-def _check_policy(w1, w3, biases, output) -> bool:
-    """Validate the policy arguments; True if the call needs the policy entries (a bias, a head other than 64 wide,
-    or actions), False if it is the original bias-free 64-wide logits MLP."""
+def _check_policy(w1, w3, biases, output) -> None:
+    """Raise ValueError for an output mode, a head width or a bias the kernels do not take."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
     if len(biases) != 3:
@@ -64,7 +62,6 @@ def _check_policy(w1, w3, biases, output) -> bool:
         if not isinstance(b, torch.Tensor) or b.dtype != torch.bfloat16 or not b.is_cuda or not b.is_contiguous() \
                 or b.dim() != 1 or b.shape[0] != n:
             raise ValueError(f"{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
-    return any(b is not None for b in biases) or d_out != 64 or output != "logits"
 
 
 def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor,
@@ -76,7 +73,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written) or "both"
     (returns (logits, actions)).  `obs` / `out` / `actions` may be peer-mapped (pull the observations / push the
-    results over NVLink).  Without biases, at d_out == 64 and with logits only this is ktb_mlp_bf16."""
+    results over NVLink).  Without biases, at d_out == 64 and with logits only the logits equal ktb_mlp_bf16's."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -86,7 +83,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
-    policy = _check_policy(w1, w3, biases, output)
+    _check_policy(w1, w3, biases, output)
     want_logits, want_actions = output != "actions", output != "logits"
     if want_logits:
         if out is None:
@@ -101,21 +98,12 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     s = stream if stream is not None else torch.cuda.current_stream(dev)
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
-    if policy:
-        ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
-        L.call("ktb_mlp_bf16_policy", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]),
-               w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), ptr(out) if want_logits else 0,
-               ptr(actions) if want_actions else 0, _scratch_for(dev, M, d_hidden).data_ptr(),
-               _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
-        return (out, actions) if output == "both" else actions if output == "actions" else out
-    if staged:
-        L.call("ktb_mlp_bf16_staged", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), w2.data_ptr(),
-               w3.data_ptr(), out.data_ptr(), _scratch_for(dev, M, d_hidden).data_ptr(),
-               _stage_for(dev, M, d_in).data_ptr(), int(s.cuda_stream))
-    else:
-        L.call("ktb_mlp_bf16", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), w2.data_ptr(),
-               w3.data_ptr(), out.data_ptr(), _scratch_for(dev, M, d_hidden).data_ptr(), int(s.cuda_stream))
-    return out
+    ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+    L.call("ktb_mlp_bf16_policy", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]),
+           w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), ptr(out) if want_logits else 0,
+           ptr(actions) if want_actions else 0, _scratch_for(dev, M, d_hidden).data_ptr(),
+           _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
+    return (out, actions) if output == "both" else actions if output == "actions" else out
 
 
 def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
@@ -175,7 +163,7 @@ def _mlp_push_state(devs: Sequence[int], shard_bytes: int) -> _MlpPushState:
     return st
 
 
-def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, policy=False, output="logits",
+def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, output="logits",
                                actions_root=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (posted NVLink writes, flags in device memory);
     every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or actions) straight
@@ -222,16 +210,11 @@ def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, wei
         dev = devs[r]
         b, e = bounds[r]
         ws = weights[dev]
-        if policy:
-            ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
-            L.call("ktb_mlp_bf16_policy_pushed", dev, st.stage[r].data_ptr(), st.stride, e - b, d_in, d_hidden, d_out,
-                   ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]),
-                   ptr(None if out_root is None else out_root[b:e]),
-                   ptr(None if actions_root is None else actions_root[b:e]), scratch[dev].data_ptr(),
-                   st.ctrl[r].data_ptr(), st.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, int(streams[dev].cuda_stream))
-            return
-        L.call("ktb_mlp_bf16_pushed", dev, st.stage[r].data_ptr(), st.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
-               ws[1].data_ptr(), ws[2].data_ptr(), out_root[b:e].data_ptr() if e > b else 0, scratch[dev].data_ptr(),
+        ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
+        L.call("ktb_mlp_bf16_policy_pushed", dev, st.stage[r].data_ptr(), st.stride, e - b, d_in, d_hidden, d_out,
+               ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]),
+               ptr(None if out_root is None else out_root[b:e]),
+               ptr(None if actions_root is None else actions_root[b:e]), scratch[dev].data_ptr(),
                st.ctrl[r].data_ptr(), st.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, int(streams[dev].cuda_stream))
 
     global _pool
@@ -262,7 +245,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    policy = _check_policy(w1, w3, biases, output)
+    _check_policy(w1, w3, biases, output)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     d_out = w3.shape[0]
@@ -294,7 +277,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, policy, output, actions_root)
+        _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, output, actions_root)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])

@@ -35,9 +35,11 @@ def test_library_is_sm90a_only():
     assert archs == {"90a"}, archs
 
 
-def test_mlp_kernels_issue_wgmma_and_tma():
-    """The shipped MLP GEMM kernels (256-wide hidden layers with ReLU, 64-wide head) feed Hopper tensor cores from
-    TMA-loaded shared memory: asynchronous warpgroup MMAs (HGMMA) of the layer's full tile width and 2-D TMA loads."""
+def test_mlp_layer_kernel_issues_wgmma_and_tma_without_spills():
+    """One MLP layer kernel per tile width 64 / 128 / 256 (the 256-wide one runs every hidden layer, the head the
+    smallest that holds d_out), each feeding Hopper tensor cores from TMA-loaded shared memory: asynchronous warpgroup
+    MMAs (HGMMA) of its full tile width and 2-D TMA loads, with no local-memory traffic (a spill in the 256-wide
+    instantiation would slow every hidden layer).  No other kernel issues wgmma."""
     import subprocess
 
     sass = subprocess.run(["cuobjdump", "-sass", L.lib_path()], capture_output=True, text=True).stdout
@@ -45,11 +47,13 @@ def test_mlp_kernels_issue_wgmma_and_tma():
     found = {}
     for f in funcs:
         name = f.split("\n", 1)[0]
-        if "gemm_bf16_tn_wgmma_kernel" in name:
-            n = 256 if "ILi256E" in name else 64
+        assert "HGMMA" not in f or "mlp_layer_wgmma_kernel" in name, name
+        if "mlp_layer_wgmma_kernel" in name:
+            n = int(re.search(r"mlp_layer_wgmma_kernelILi(\d+)E", name).group(1))
             assert f"HGMMA.64x{n}x16.F32.BF16" in f and "UTMALDG.2D" in f, name
+            assert not re.search(r"\b(STL|LDL)\b", f), name
             found[n] = found.get(n, 0) + 1
-    assert found == {256: 1, 64: 1}, found
+    assert found == {64: 1, 128: 1, 256: 1}, found
 
 
 @pytest.mark.parametrize("n,world", [(0, 1), (1, 4), (3, 4), (5, 4), (1003, 4), (1000, 3), (64, 8), (2**26, 8), (7, 7)])

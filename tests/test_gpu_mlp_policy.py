@@ -1,6 +1,6 @@
-"""-m gpu: the nn.Linear policy form of the bf16 MLP (ktb_mlp_bf16_policy*, mlp_policy_wgmma_kernel) against an fp64
+"""-m gpu: the nn.Linear policy form of the bf16 MLP (ktb_mlp_bf16_policy*, mlp_layer_wgmma_kernel) against an fp64
 reference layer by layer with biases, at every head width class from 1 to 256; its greedy actions against torch.argmax
-of its own logits, with planted ties, NaN and infinities; bit identity with the original entries and across every
+of its own logits, with planted ties, NaN and infinities; bit identity with the 64-wide entries and across every
 form; guard bands around every buffer it writes; the mapped op through the public API; and its status codes."""
 import ctypes
 
@@ -234,9 +234,11 @@ def test_bias_free_64_wide_logits_equal_the_original_entry(K, M):
     L, mlp = _L(), _mlp()
     (w1, w2, w3), _ = _config(71, 64, bias=False)
     obs = _randn((M, 256), 73)
-    want = mlp.mlp_forward(obs, w1, w2, w3)
+    want = torch.empty(M, 64, dtype=torch.bfloat16, device="cuda")
     got = torch.empty_like(want)
     scratch = mlp._scratch_for(0, M, 1024)
+    L.call("ktb_mlp_bf16", 0, obs.data_ptr(), M, 256, 1024, 64, w1.data_ptr(), w2.data_ptr(), w3.data_ptr(),
+           want.data_ptr(), scratch.data_ptr(), _stream())
     L.call("ktb_mlp_bf16_policy", 0, obs.data_ptr(), M, 256, 1024, 64, w1.data_ptr(), 0, w2.data_ptr(), 0,
            w3.data_ptr(), 0, got.data_ptr(), 0, scratch.data_ptr(), 0, _stream())
     assert torch.equal(got, want)

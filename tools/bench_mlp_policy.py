@@ -4,9 +4,9 @@ rows through 256 -> 1024 -> 1024 -> d_out, device-resident on cuda:0.
 
 Variants, timed alternately (one sample = the mean of --calls back-to-back calls between CUDA events; the median of
 --samples samples is reported):
-  a  today's path: ktb_mlp_bf16, no bias, d_out 64, logits
-  b  ktb_mlp_bf16_policy, no bias, d_out 64, logits (its logits must equal a's bit for bit)
-  c  policy with biases, d_out 64, logits
+  a  the C entry ktb_mlp_bf16 (no bias, d_out 64, logits), called directly
+  b  the C entry ktb_mlp_bf16_policy, no bias, d_out 64, logits (its logits must equal a's bit for bit)
+  c  mlp_forward (ktb_mlp_bf16_policy) with biases, d_out 64, logits
   d  policy with biases, d_out 64, actions only
   e  policy with biases, d_out 64, logits and actions
   f  policy with biases, d_out 18 and d_out 256, logits and actions
@@ -64,14 +64,20 @@ def main():
     scratch = mlp._scratch_for(0, M, d_hidden)
     stream = int(torch.cuda.current_stream(0).cuda_stream)
 
+    def original_a(out):
+        L.call("ktb_mlp_bf16", 0, obs.data_ptr(), M, d_in, d_hidden, 64, w1.data_ptr(), w2.data_ptr(),
+               heads[64][0].data_ptr(), out.data_ptr(), scratch.data_ptr(), stream)
+        return out
+
     def policy_b(out):
         L.call("ktb_mlp_bf16_policy", 0, obs.data_ptr(), M, d_in, d_hidden, 64, w1.data_ptr(), 0, w2.data_ptr(), 0,
                heads[64][0].data_ptr(), 0, out.data_ptr(), 0, scratch.data_ptr(), 0, stream)
         return out
 
+    out_a = torch.empty(M, 64, dtype=torch.bfloat16, device="cuda:0")
     out_b = torch.empty(M, 64, dtype=torch.bfloat16, device="cuda:0")
     variants = {
-        "a_original_d64": (64, lambda: mlp.mlp_forward(obs, w1, w2, heads[64][0])),
+        "a_original_d64": (64, lambda: original_a(out_a)),
         "b_policy_nobias_d64": (64, lambda: policy_b(out_b)),
         "c_bias_logits_d64": (64, lambda: mlp.mlp_forward(obs, w1, w2, heads[64][0], biases=(b1, b2, heads[64][1]))),
         "d_bias_actions_d64": (64, lambda: mlp.mlp_forward(obs, w1, w2, heads[64][0], biases=(b1, b2, heads[64][1]),
