@@ -217,12 +217,17 @@ def batch_map(device: int, op: str, alpha: float, beta: float):
 _ws_cache = {}
 
 
-def _workspace(dev: int) -> torch.Tensor:
-    key = (dev, int(torch.cuda.current_stream(dev).cuda_stream))
+def _workspace(dev: int, stream: Optional[int] = None) -> torch.Tensor:
+    """Reduce workspace (ticket counter + per-CTA partials) of one stream on `dev`, default torch's current one.
+    Reductions on one stream run in order and may share it; two streams must never share one."""
+    current = current_stream_handle(dev)
+    key = (dev, current if stream is None else int(stream))
     ws = _ws_cache.get(key)
     if ws is None:
         nbytes = L.load().ktb_reduce_workspace_bytes()
         ws = torch.zeros(nbytes, dtype=torch.uint8, device=f"cuda:{dev}")
+        if key[1] != current:  # the zero fill runs on the current stream: finish it before another stream uses ws
+            torch.cuda.current_stream(dev).synchronize()
         _ws_cache[key] = ws
     return ws
 
@@ -248,9 +253,10 @@ def map_reduce_sum(
         raise TypeError("uint8 is not reducible")
     if out is None:
         out = torch.empty(1, dtype=acc_dtype(x.dtype), device=f"cuda:{dev}")
+    st = _stream(dev, stream)
     L.call(
         "ktb_map_reduce_sum", dev, OPS[op], dtype_code(x.dtype), x.data_ptr(), x.numel(), float(alpha),
-        float(beta), out.data_ptr(), _workspace(dev).data_ptr(), _stream(dev, stream),
+        float(beta), out.data_ptr(), _workspace(dev, st).data_ptr(), st,
     )
     return out
 

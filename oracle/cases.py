@@ -86,11 +86,14 @@ def affine(x, alpha, beta):
 
 
 def shard_sum(x, alpha=1, beta=0):
-    """Gather-reduce variant: each rank returns the sum of its mapped shard."""
+    """Gather-reduce variant: each rank returns the sum of its mapped shard.
+
+    Floating-point shards are summed in fp32 after the op has rounded each element to the tensor dtype, so a
+    bf16 or fp16 sum does not round or overflow in the 2-byte dtype; integer shards are summed in int64."""
     import torch
 
     y = _shard(x) * alpha + beta if (alpha != 1 or beta != 0) else _shard(x)
-    if y.dtype in (torch.float32, torch.bfloat16):
+    if y.dtype in (torch.float32, torch.bfloat16, torch.float16):
         return float(y.float().sum())
     return int(y.sum())
 

@@ -72,6 +72,16 @@ def test_gather_reduce_through_public_api(golden):
         got = remote(x.cuda(), serialization="pickle")
         tol = 8 * torch.finfo(torch.float32).eps * float(x.abs().sum())  # fp32 sum, order differs from torch
         assert all(abs(g - w) <= tol for g, w in zip(got, rec["result"]))
+        # 2-byte floats and i32 products that wrap: integer-valued inputs keep every float sum exact in any order, so
+        # the ranks' sums must equal the oracle's exactly
+        g = torch.Generator().manual_seed(13)
+        for dtype, bound, a, b in ((torch.bfloat16, 127, 0.5, 0.25), (torch.float16, 1023, 0.5, 0.25),
+                                   (torch.float16, 1023, -1, 1), (torch.int32, 2**31, 65537, -7)):
+            x = torch.randint(-bound, bound, (10_003,), generator=g).to(dtype)   # |partial sums| < 2^22 per shard
+            want = ref_dispatch.spmd_call(cases.shard_sum, x, a, b, num_proc=4, serialization="pickle")
+            got = remote(x.cuda(), a, b, serialization="pickle")
+            assert got == want, (dtype, a, b)
+            assert all(isinstance(v, float if dtype.is_floating_point else int) for v in got), dtype
     finally:
         remote.teardown()
 

@@ -1,5 +1,5 @@
 """-m gpu: the CUDA kernels, called through the C-ABI, against the oracle (the reference's SPMD
-semantics evaluated on CPU) — bit-exact for every dtype/op (fp tolerance only for float sums)."""
+semantics evaluated on CPU) — bit-exact for every dtype/op. The sum reduction has its own file, test_gpu_reduce.py."""
 import ctypes
 import os
 
@@ -139,42 +139,6 @@ def test_golden_reference_runtime_cases(K, golden):
             assert e0 - b0 == w.numel(), (name, r)
         checked += 1
     assert checked >= 10
-
-
-def test_golden_sums(K, golden):
-    for name in ("sum_i64_130_x4", "sum_i32_515_x4", "sum_f32_1001_x4"):
-        rec = golden["cases"][name]
-        args = resolve_args(golden, rec["args"])
-        x = args[0]
-        a, b = (args[1], args[2]) if len(args) == 3 else (1, 0)
-        op = "affine" if len(args) == 3 else "identity"
-        total, partials = K.scatter_map_reduce(x.cuda(), op, a, b, devices=[0] * 4)
-        if x.dtype.is_floating_point:
-            # fp32 sums: order differs from torch's pairwise sum; tolerance = 8 ulp of sum(|x|)
-            tol = 8 * torch.finfo(torch.float32).eps * float(x.abs().sum())
-            for g, w in zip(partials.tolist(), rec["result"]):
-                assert abs(g - w) <= tol, name
-        else:
-            assert partials.tolist() == rec["result"], name
-            assert int(total.item()) == sum(rec["result"])
-
-
-@pytest.mark.parametrize("dtype", [torch.float32, torch.bfloat16, torch.float16, torch.int32, torch.int64])
-def test_reduce_sizes(K, dtype):
-    for n in [0, 1, 33, 1000, 70_001, (1 << 21) + 5]:
-        x = _rand(dtype, n, seed=n + 1)
-        if dtype == torch.int64:
-            x = x >> 24  # keep the true sum inside int64
-        got = K.map_reduce_sum(x.cuda(), "identity").cpu()
-        if dtype.is_floating_point:
-            ref = float(x.double().sum())
-            tol = 8 * torch.finfo(torch.float32).eps * float(x.double().abs().sum()) + 1e-30
-            assert abs(float(got) - ref) <= tol, (dtype, n)
-        else:
-            assert int(got) == int(x.sum()), (dtype, n)
-    # workspace is left clean: a second call gives the same answer
-    x = _rand(torch.int32, 5000).cuda()
-    assert int(K.map_reduce_sum(x, "affine", 3, 1)) == int(K.map_reduce_sum(x, "affine", 3, 1))
 
 
 def test_pack_unpack_roundtrip(K):

@@ -142,6 +142,26 @@ def test_exception_rehydration_shape():
     assert _base_name(dyn) == "WeirdError"
 
 
+def test_shard_sum_defines_fp16_like_bf16(golden):
+    """An fp16 shard sums in fp32 after the op rounds each element to fp16, as bf16 does: a float per rank, exact
+    here (integers and quarters far below 2^24), and no fp16 overflow at 65504 or truncation to int."""
+    g = torch.Generator().manual_seed(7)
+    x = (torch.randint(1, 1024, (1001, 3), generator=g) * (1 - 2 * torch.randint(0, 2, (1001, 3), generator=g)))
+    x = x.half()
+    x[:40] = 1000.0                                    # rank 0's shard sums past the fp16 range
+    for world, a, b in ((1, 1, 0), (3, 1, 0), (4, 0.5, 0.25), (16, 2, 0)):
+        got = R.spmd_call(cases.shard_sum, x, a, b, num_proc=world, serialization="pickle")
+        y = x.double() * a + b                         # exact in fp16 for these inputs and ops
+        want = [float(c.sum()) for c in y.chunk(world)] + [0.0] * (world - len(y.chunk(world)))
+        assert all(isinstance(v, float) for v in got), world
+        assert got == want, world
+    assert got[0] > 65504
+    # the recorded gather-reduce cases (i64, i32, f32) replay unchanged
+    for name in ("sum_i64_130_x4", "sum_i32_515_x4", "sum_f32_1001_x4"):
+        rec = golden["cases"][name]
+        assert _same(_run_oracle(rec, resolve_args(golden, rec["args"])), rec["result"]), name
+
+
 def test_oracle_runtime_with_real_processes():
     x = torch.arange(1003, dtype=torch.float32)
     with R.OracleRuntime("oracle.cases", "double", 3, "spmd", extra_path=REPO) as rt:
