@@ -109,6 +109,8 @@ int ktb_broadcast(int root, const void* src, void* const* dsts, int n_dst, size_
   return KTB_OK;
 }
 
+}  // extern "C"
+
 // Per-THREAD event pool: each host thread owns its events (per device: slot 0 "args ready", slot 1+r "rank r done"), created
 // once and reused by every call the thread makes — a call used to pay N+1 cudaEventCreate/Destroy pairs (≈25 µs at
 // N = 8).  Reuse is safe: cudaStreamWaitEvent captures the record that is current WHEN THE WAIT IS ENQUEUED, so
@@ -148,6 +150,59 @@ static int check_ranks(const char* who, int n_ranks, const int* devs, int root_r
   return KTB_OK;
 }
 
+// streams == NULL → library streams; otherwise streams[r] verbatim (0 is the legacy default stream)
+static cudaStream_t rank_stream(const uintptr_t* streams, const int* devs, int r) {
+  return streams ? reinterpret_cast<cudaStream_t>(streams[r]) : device_info(devs[r])->stream_rank;
+}
+
+// The fork/join of the scatter forms: record "args ready" on the root stream; per rank, order the rank's stream
+// after it, run launch(r, dev, b, e, stream) on elements [b, e) of its shard and record "rank r done"; then join
+// every rank on the root stream.  A rank on the root stream itself needs no events.  With skip_empty, a rank whose
+// shard is empty is skipped outright (no launch, no events).
+template <class Launch>
+static int fork_join(const char* who, size_t n_elems, size_t granule, int n_ranks, const int* devs, int root_rank,
+                     const uintptr_t* streams, bool skip_empty, Launch&& launch) {
+  const int root_dev = devs[root_rank];
+  cudaStream_t root_stream = rank_stream(streams, devs, root_rank);
+  CallEvents events;
+  cudaEvent_t done[kMaxDevices] = {nullptr};
+  cudaEvent_t args_ready = events.make(root_dev, 0);
+  KTB_REQUIRE(args_ready, KTB_ERR_CUDA, "%s: cudaEventCreate failed", who);
+  {
+    KTB_GUARD(root_dev);
+    KTB_CK(cudaEventRecord(args_ready, root_stream));  // args are ready on the root
+  }
+  for (int r = 0; r < n_ranks; ++r) {
+    size_t b = 0, e = 0;
+    ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
+    b *= granule;
+    e *= granule;
+    if (skip_empty && e == b) continue;
+    const int dev = devs[r];
+    KTB_GUARD(dev);
+    cudaStream_t st = rank_stream(streams, devs, r);
+    // same ordering domain as the root only if it is the same stream ON the same device (handle 0 is
+    // "the default stream of whichever device is current", so handles alone do not identify a stream)
+    const bool is_root = (r == root_rank) || (dev == root_dev && st == root_stream);
+    if (!is_root) KTB_CK(cudaStreamWaitEvent(st, args_ready, 0));
+    int rc = launch(r, dev, b, e, st);
+    if (rc) return rc;
+    if (!is_root) {
+      done[r] = events.make(dev, 1 + r);
+      KTB_REQUIRE(done[r], KTB_ERR_CUDA, "%s: cudaEventCreate failed", who);
+      KTB_CK(cudaEventRecord(done[r], st));
+    }
+  }
+  // Join on the root stream with the ROOT device current: stream handle 0 names the default stream of
+  // whichever device is current, so the wait must be issued under the root's guard.
+  KTB_GUARD(root_dev);
+  for (int r = 0; r < n_ranks; ++r)
+    if (done[r]) KTB_CK(cudaStreamWaitEvent(root_stream, done[r], 0));
+  return KTB_OK;
+}
+
+extern "C" {
+
 int ktb_scatter_map_gather(int op, int dtype, const void* src_root, void* dst_root, size_t n_elems,
                            size_t granule, double alpha, double beta, int n_ranks, const int* devs,
                            int root_rank, int variant, const uintptr_t* streams) {
@@ -160,52 +215,11 @@ int ktb_scatter_map_gather(int op, int dtype, const void* src_root, void* dst_ro
   KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG,
               "ktb_scatter_map_gather: n_elems %zu is not a multiple of granule %zu", n_elems, granule);
   const MapParams p = make_params(alpha, beta, dtype);
-  const int root_dev = devs[root_rank];
-  DeviceInfo* root = device_info(root_dev);
-  // streams == NULL → library streams; otherwise streams[r] verbatim (0 is the legacy default stream)
-  auto stream_of = [&](int r) {
-    return streams ? reinterpret_cast<cudaStream_t>(streams[r]) : device_info(devs[r])->stream_rank;
-  };
-  cudaStream_t root_stream = stream_of(root_rank);
-  CallEvents events;
-  cudaEvent_t done[kMaxDevices] = {nullptr};
-  cudaEvent_t args_ready = events.make(root_dev, 0);
-  KTB_REQUIRE(args_ready, KTB_ERR_CUDA, "ktb_scatter_map_gather: cudaEventCreate failed");
-  (void)root;
-  {
-    KTB_GUARD(root_dev);
-    KTB_CK(cudaEventRecord(args_ready, root_stream));  // args are ready on the root
-  }
-  for (int r = 0; r < n_ranks; ++r) {
-    size_t b = 0, e = 0;
-    ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
-    b *= granule;
-    e *= granule;
-    if (e == b) continue;
-    const int dev = devs[r];
-    KTB_GUARD(dev);
-    cudaStream_t st = stream_of(r);
-    // same ordering domain as the root only if it is the same stream ON the same device (handle 0 is
-    // "the default stream of whichever device is current", so handles alone do not identify a stream)
-    const bool is_root = (r == root_rank) || (dev == root_dev && st == root_stream);
-    if (!is_root) KTB_CK(cudaStreamWaitEvent(st, args_ready, 0));
-    rc = launch_map(dev, op, dtype, static_cast<const uint8_t*>(src_root) + b * es,
-                    static_cast<uint8_t*>(dst_root) + b * es, e - b, p, variant, st);
-    if (rc) return rc;
-    if (!is_root) {
-      done[r] = events.make(dev, 1 + r);
-      KTB_REQUIRE(done[r], KTB_ERR_CUDA, "ktb_scatter_map_gather: cudaEventCreate failed");
-      KTB_CK(cudaEventRecord(done[r], st));
-    }
-  }
-  // Join on the root stream with the ROOT device current: stream handle 0 names the default stream of
-  // whichever device is current, so the wait must be issued under the root's guard.
-  {
-    KTB_GUARD(root_dev);
-    for (int r = 0; r < n_ranks; ++r)
-      if (done[r]) KTB_CK(cudaStreamWaitEvent(root_stream, done[r], 0));
-  }
-  return KTB_OK;
+  return fork_join("ktb_scatter_map_gather", n_elems, granule, n_ranks, devs, root_rank, streams, true,
+                   [&](int, int dev, size_t b, size_t e, cudaStream_t st) {
+                     return launch_map(dev, op, dtype, static_cast<const uint8_t*>(src_root) + b * es,
+                                       static_cast<uint8_t*>(dst_root) + b * es, e - b, p, variant, st);
+                   });
 }
 
 int ktb_scatter_map_reduce(int op, int dtype, const void* src_root, size_t n_elems, size_t granule,
@@ -217,54 +231,24 @@ int ktb_scatter_map_reduce(int op, int dtype, const void* src_root, size_t n_ele
   const size_t es = dtype_size(dtype);
   KTB_REQUIRE(es != 0 && dtype != KTB_U8, KTB_ERR_ARG, "ktb_scatter_map_reduce: dtype %d not reducible", dtype);
   KTB_REQUIRE(partials_root && out_root && workspaces, KTB_ERR_ARG, "ktb_scatter_map_reduce: null argument");
+  for (int r = 0; r < n_ranks; ++r)
+    KTB_REQUIRE(workspaces[r], KTB_ERR_ARG, "ktb_scatter_map_reduce: workspaces[%d] is null", r);
   KTB_REQUIRE(src_root || n_elems == 0, KTB_ERR_ARG, "ktb_scatter_map_reduce: null src");
   KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG,
               "ktb_scatter_map_reduce: n_elems %zu is not a multiple of granule %zu", n_elems, granule);
   const MapParams p = make_params(alpha, beta, dtype);
   const size_t acc_size = (dtype == KTB_F32 || dtype == KTB_BF16 || dtype == KTB_F16) ? 4 : 8;
-  const int root_dev = devs[root_rank];
-  DeviceInfo* root = device_info(root_dev);
-  // streams == NULL → library streams; otherwise streams[r] verbatim (0 is the legacy default stream)
-  auto stream_of = [&](int r) {
-    return streams ? reinterpret_cast<cudaStream_t>(streams[r]) : device_info(devs[r])->stream_rank;
-  };
-  cudaStream_t root_stream = stream_of(root_rank);
-  CallEvents events;
-  cudaEvent_t done[kMaxDevices] = {nullptr};
-  cudaEvent_t args_ready = events.make(root_dev, 0);
-  KTB_REQUIRE(args_ready, KTB_ERR_CUDA, "ktb_scatter_map_reduce: cudaEventCreate failed");
-  (void)root;
-  {
-    KTB_GUARD(root_dev);
-    KTB_CK(cudaEventRecord(args_ready, root_stream));
-  }
-  for (int r = 0; r < n_ranks; ++r) {
-    size_t b = 0, e = 0;
-    ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
-    b *= granule;
-    e *= granule;
-    const int dev = devs[r];
-    KTB_GUARD(dev);
-    cudaStream_t st = stream_of(r);
-    // same ordering domain as the root only if it is the same stream ON the same device (handle 0 is
-    // "the default stream of whichever device is current", so handles alone do not identify a stream)
-    const bool is_root = (r == root_rank) || (dev == root_dev && st == root_stream);
-    if (!is_root) KTB_CK(cudaStreamWaitEvent(st, args_ready, 0));
-    KTB_REQUIRE(workspaces[r], KTB_ERR_ARG, "ktb_scatter_map_reduce: workspaces[%d] is null", r);
-    // empty shards still write a zero partial (n_elems = 0 → kernel stores 0)
-    rc = launch_map_reduce(dev, op, dtype, static_cast<const uint8_t*>(src_root) + b * es, e - b, p,
-                           static_cast<uint8_t*>(partials_root) + (size_t)r * acc_size, workspaces[r], st);
-    if (rc) return rc;
-    if (!is_root) {
-      done[r] = events.make(dev, 1 + r);
-      KTB_REQUIRE(done[r], KTB_ERR_CUDA, "ktb_scatter_map_reduce: cudaEventCreate failed");
-      KTB_CK(cudaEventRecord(done[r], st));
-    }
-  }
-  KTB_GUARD(root_dev);
-  for (int r = 0; r < n_ranks; ++r)
-    if (done[r]) KTB_CK(cudaStreamWaitEvent(root_stream, done[r], 0));
-  return launch_reduce_partials(root_dev, dtype, partials_root, n_ranks, out_root, root_stream);
+  // empty shards still launch: they write a zero partial (n_elems = 0 → kernel stores 0)
+  rc = fork_join("ktb_scatter_map_reduce", n_elems, granule, n_ranks, devs, root_rank, streams, false,
+                 [&](int r, int dev, size_t b, size_t e, cudaStream_t st) {
+                   return launch_map_reduce(dev, op, dtype, static_cast<const uint8_t*>(src_root) + b * es, e - b, p,
+                                            static_cast<uint8_t*>(partials_root) + (size_t)r * acc_size,
+                                            workspaces[r], st);
+                 });
+  if (rc) return rc;
+  KTB_GUARD(devs[root_rank]);
+  return launch_reduce_partials(devs[root_rank], dtype, partials_root, n_ranks, out_root,
+                                rank_stream(streams, devs, root_rank));
 }
 
 // ktb_map_host / ktb_map_host_multi (host-resident args over PCIe) live in ktb_host.cu.

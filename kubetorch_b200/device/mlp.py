@@ -22,25 +22,30 @@ def pushed_scratch_bytes(M: int, d_hidden: int, chunk_rows: int) -> int:
     return 2 * min(int(chunk_rows), int(M)) * int(d_hidden) * 2
 
 
-def _scratch_for(dev: int, M: int, d_hidden: int, chunk_rows: Optional[int] = None) -> torch.Tensor:
-    if chunk_rows is None:
-        nbytes = L.load().ktb_mlp_scratch_bytes(M, d_hidden)
-    else:
-        nbytes = pushed_scratch_bytes(M, d_hidden, chunk_rows)
-    buf = _scratch.get(dev)
+def _cached_buffer(cache: dict, key, dev: int, nbytes: int) -> torch.Tensor:
+    """cache[key]: a uint8 buffer on `dev` of at least `nbytes`, replaced by a larger one when a call needs more."""
+    buf = cache.get(key)
     if buf is None or buf.numel() < nbytes:
-        buf = torch.empty(nbytes, dtype=torch.uint8, device=f"cuda:{dev}")
-        _scratch[dev] = buf
+        buf = cache[key] = torch.empty(nbytes, dtype=torch.uint8, device=f"cuda:{dev}")
     return buf
+
+
+def _scratch_for(dev: int, M: int, d_hidden: int) -> torch.Tensor:
+    return _cached_buffer(_scratch, dev, dev, L.load().ktb_mlp_scratch_bytes(M, d_hidden))
 
 
 def _stage_for(dev: int, M: int, d_in: int) -> torch.Tensor:
-    nbytes = L.load().ktb_mlp_stage_bytes(M, d_in)
-    buf = _stage.get(dev)
-    if buf is None or buf.numel() < nbytes:
-        buf = torch.empty(nbytes, dtype=torch.uint8, device=f"cuda:{dev}")
-        _stage[dev] = buf
-    return buf
+    return _cached_buffer(_stage, dev, dev, L.load().ktb_mlp_stage_bytes(M, d_in))
+
+
+def _thread_pool():
+    """Threads that issue the ranks' launches in parallel (ctypes releases the GIL)."""
+    global _pool
+    if _pool is None:
+        from concurrent.futures import ThreadPoolExecutor
+
+        _pool = ThreadPoolExecutor(max_workers=16, thread_name_prefix="ktb-mlp")
+    return _pool
 
 
 OUTPUTS = ("logits", "actions", "both")
@@ -125,112 +130,56 @@ def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     return out
 
 
-SCATTER_ENGINE = "ce"        # "ce": copy engines push the observation chunks; "sm": the capped scatter kernel;
-                             # "hybrid": copy engines serve the first CE_RANKS ranks, the capped scatter kernel the rest
-CE_RANKS = 3
-SCATTER_CTAS_PER_SM = 2
 PUSH_CHUNK_ROWS = 16896      # 132 SMs x 128 rows: each 256-wide layer of a chunk is whole waves of 128 x 256 tiles
-_push_states = {}
+_push_sessions = {}          # device tuple -> ops.PushSession
+_push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pushed GEMMs
 
 
-class _MlpPushState:
-    """Per device set: control blocks, per-rank staging (2 call-parity halves), the root's side stream."""
-
-    def __init__(self, devs: Sequence[int], stride: int):
-        self.devs, self.stride, self.seq = list(devs), int(stride), 0
-        cb = L.load().ktb_push_control_bytes()
-        self.ctrl = [torch.zeros(cb, dtype=torch.uint8, device=f"cuda:{d}") for d in devs]
-        self.stage = [None if r == 0 else torch.empty(2 * self.stride, dtype=torch.uint8, device=f"cuda:{d}")
-                      for r, d in enumerate(devs)]
-        for d in set(devs):
-            torch.cuda.synchronize(d)
-        self.stage_ptrs = L.arr(ctypes.c_void_p, [0 if t is None else t.data_ptr() for t in self.stage])
-        self.ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
-        self.side = torch.cuda.Stream(devs[0])
-        self.scatter = torch.cuda.Stream(devs[0])      # the SM scatter kernel of a hybrid scatter
-        self.ev_fork, self.ev_join = torch.cuda.Event(), torch.cuda.Event()
-        self.ev_scatter = torch.cuda.Event()
-        self.status_host = torch.zeros(len(devs), dtype=torch.int32).pin_memory()
-        self.status_dev = [c[1032:1036].view(torch.int32) for c in self.ctrl]
-
-
-def _mlp_push_state(devs: Sequence[int], shard_bytes: int) -> _MlpPushState:
-    key = tuple(devs)
-    st = _push_states.get(key)
-    stride = (int(shard_bytes) + 255) // 256 * 256
-    if st is None or st.stride < stride:
-        st = _push_states[key] = _MlpPushState(devs, stride)
-    return st
-
-
-def _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, output="logits",
-                               actions_root=None) -> None:
-    """The root PUSHES each rank's observation rows in GEMM-sized chunks (posted NVLink writes, flags in device memory);
-    every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or actions) straight
-    into the root's result; the root's own shard runs on a side stream beside the scatter.  No host synchronisation, no
-    events between devices.  weights[dev] = (w1, w2, w3, b1, b2, b3) on that device (biases may be None)."""
-    root, n = devs[0], len(devs)
-    d_in, d_hidden, d_out = obs_root.shape[1], w1.shape[0], w3.shape[0]
-    st = _mlp_push_state(devs, max(e - b for b, e in bounds) * d_in * 2)
-    if bool(st.status_host.any()):
-        _push_states.pop(tuple(devs), None)
-        raise ops.PushTimeout("MLP push pipeline: an in-kernel wait timed out during an earlier call")
-    st.seq += 1
-    seq = st.seq
-    root_stream = torch.cuda.current_stream(root)
-    with torch.cuda.device(root):
-        b0, e0 = bounds[0]
-        st.ev_fork.record(root_stream)          # forked BEFORE the scatter launch: the side stream must not queue behind it
-        st.side.wait_event(st.ev_fork)
-        if e0 > b0:
-            ws = weights[root]
-            mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b0:e0],
-                        device=root, stream=st.side, staged=False, biases=ws[3:], output=output,
-                        actions=None if actions_root is None else actions_root[b0:e0])
-        st.ev_join.record(st.side)
-        engine = SCATTER_ENGINE if n > 2 or SCATTER_ENGINE != "hybrid" else "ce"
-        ptrs = [0 if t is None else t.data_ptr() for t in st.stage]
-        n_ce = n - 1 if engine == "ce" else (0 if engine == "sm" else min(CE_RANKS, n - 2))
-        ce_ptrs = L.arr(ctypes.c_void_p, [p if 1 <= r <= n_ce else 0 for r, p in enumerate(ptrs)])
-        sm_ptrs = L.arr(ctypes.c_void_p, [p if r > n_ce else 0 for r, p in enumerate(ptrs)])
-        if n_ce < n - 1:             # the capped scatter kernel first: its few CTAs per SM leave room for the root's GEMMs
-            st.scatter.wait_event(st.ev_fork)
-            L.call("ktb_push_scatter_chunked", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, sm_ptrs,
-                   st.stride, st.ctrl_ptrs, st.ctrl[0].data_ptr(), PUSH_CHUNK_ROWS * d_in, SCATTER_CTAS_PER_SM, seq,
-                   int(st.scatter.cuda_stream))
-            st.ev_scatter.record(st.scatter)
-        if n_ce > 0:                 # copy engines move the rows of the other ranks: no SM of the root involved
-            L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
-                   L.arr(ctypes.c_int, list(devs)), ce_ptrs, st.stride, st.ctrl_ptrs, st.ctrl[0].data_ptr(),
-                   PUSH_CHUNK_ROWS * d_in, seq, int(root_stream.cuda_stream))
-    streams = {d: torch.cuda.current_stream(d) for d in devs[1:]}
-    scratch = {d: _scratch_for(d, max(e - b for b, e in bounds), d_hidden, PUSH_CHUNK_ROWS) for d in devs[1:]}
+def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root) -> None:
+    """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
+    device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
+    actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
+    scatter.  No host synchronisation, no events between devices.  weights[dev] = (w1, w2, w3, b1, b2, b3) on that
+    device (biases may be None); out_root / actions_root are None when `output` does not want them."""
+    root, n, key = devs[0], len(devs), tuple(devs)
+    d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0]
+    rows = max(e - b for b, e in bounds)
+    sess = _push_sessions.get(key)
+    if sess is None or sess.stride < rows * d_in * 2:
+        sess = _push_sessions[key] = ops.PushSession(devs, rows * d_in * 2)
+    try:
+        seq = sess.begin()
+    except ops.PushTimeout:
+        del _push_sessions[key]
+        raise
+    # scratch per rank, not per device: ranks sharing a device must not share one, nor the root's own shard on the
+    # side stream
+    scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS)
+    scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], scratch_bytes) for r in range(1, n)]
+    streams = [ops.current_stream_handle(d) for d in devs]
+    b0, e0 = bounds[0]
+    own = e0 > b0
+    if own:
+        ws = weights[root]
+        mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b0:e0],
+                    device=root, stream=sess.fork(), staged=False, biases=ws[3:], output=output,
+                    actions=None if actions_root is None else actions_root[b0:e0])
+    L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
+           L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
+           PUSH_CHUNK_ROWS * d_in, seq, streams[0])
 
     def issue(r):
-        dev = devs[r]
         b, e = bounds[r]
-        ws = weights[dev]
+        ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
-        L.call("ktb_mlp_bf16_policy_pushed", dev, st.stage[r].data_ptr(), st.stride, e - b, d_in, d_hidden, d_out,
-               ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]),
+        L.call("ktb_mlp_bf16_policy_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden,
+               d_out, ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]),
                ptr(None if out_root is None else out_root[b:e]),
-               ptr(None if actions_root is None else actions_root[b:e]), scratch[dev].data_ptr(),
-               st.ctrl[r].data_ptr(), st.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, int(streams[dev].cuda_stream))
+               ptr(None if actions_root is None else actions_root[b:e]), scratch[r].data_ptr(),
+               sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
 
-    global _pool
-    if _pool is None:
-        from concurrent.futures import ThreadPoolExecutor
-
-        _pool = ThreadPoolExecutor(max_workers=16, thread_name_prefix="ktb-mlp")
-    list(_pool.map(issue, range(1, n)))
-    with torch.cuda.device(root):
-        L.call("ktb_push_wait", root, st.ctrl[0].data_ptr(), n, 0, seq, int(root_stream.cuda_stream))
-        root_stream.wait_event(st.ev_join)
-        if n_ce < n - 1:
-            root_stream.wait_event(st.ev_scatter)
-    for r, d in enumerate(devs):   # stream-ordered mirror of the sticky status words (seen at the next call)
-        with torch.cuda.device(d):
-            st.status_host[r:r + 1].copy_(st.status_dev[r], non_blocking=True)
+    list(_thread_pool().map(issue, range(1, n)))
+    sess.finish(seq, joined=own)
 
 
 def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int],
@@ -277,7 +226,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, w1, w2, w3, devs, out_root, bounds, weights, output, actions_root)
+        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -305,13 +254,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                 return ev
         return None
 
-    global _pool
     if len(set(devs)) > 1:
-        if _pool is None:
-            from concurrent.futures import ThreadPoolExecutor
-
-            _pool = ThreadPoolExecutor(max_workers=16, thread_name_prefix="ktb-mlp")
-        done = list(_pool.map(issue, range(len(devs))))
+        done = list(_thread_pool().map(issue, range(len(devs))))
     else:
         done = [issue(r) for r in range(len(devs))]
     for ev in done:

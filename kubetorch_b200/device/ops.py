@@ -429,6 +429,16 @@ def broadcast(src: torch.Tensor, dsts: Sequence[torch.Tensor], stream: Optional[
     return dsts
 
 
+def _scatter_devices(x_root: torch.Tensor, devices: Sequence[int], root_rank: int) -> List[int]:
+    """The ranks' devices of a scatter form, registered, with devices[root_rank] checked to hold x_root."""
+    root = _check_dev_tensor(x_root, "x_root")
+    devs = [int(d) for d in devices]
+    if devs[root_rank] != root:
+        raise ValueError(f"x_root lives on cuda:{root} but devices[{root_rank}] is {devs[root_rank]}")
+    ensure_init(set(devs))
+    return devs
+
+
 def scatter_map_gather(
     x_root: torch.Tensor,
     op: str,
@@ -443,11 +453,7 @@ def scatter_map_gather(
     """Fused scatter → map → gather: rank r's kernel pulls shard r of x_root (`x.chunk(world)` along
     dim 0; `granule` = elements per row, default from x_root's shape) from the root GPU over NVLink,
     applies op, and pushes it into out_root."""
-    root = _check_dev_tensor(x_root, "x_root")
-    devs = [int(d) for d in devices]
-    if devs[root_rank] != root:
-        raise ValueError(f"x_root lives on cuda:{root} but devices[{root_rank}] is {devs[root_rank]}")
-    ensure_init(devs)
+    devs = _scatter_devices(x_root, devices, root_rank)
     if out_root is None:
         out_root = torch.empty_like(x_root)
     streams = [current_stream_handle(d) for d in devs]
@@ -469,11 +475,7 @@ def scatter_map_reduce(
     granule: Optional[int] = None,
 ) -> Tuple[torch.Tensor, torch.Tensor]:
     """Gather-reduce variant. Returns (total[1], partials[n_ranks]) on the root GPU."""
-    root = _check_dev_tensor(x_root, "x_root")
-    devs = [int(d) for d in devices]
-    if devs[root_rank] != root:
-        raise ValueError(f"x_root lives on cuda:{root} but devices[{root_rank}] is {devs[root_rank]}")
-    ensure_init(set(devs))
+    devs = _scatter_devices(x_root, devices, root_rank)
     adt = acc_dtype(x_root.dtype)
     partials = torch.zeros(len(devs), dtype=adt, device=x_root.device)
     total = torch.empty(1, dtype=adt, device=x_root.device)
@@ -542,11 +544,19 @@ class PushTimeout(RuntimeError):
     """An in-kernel flag wait of the push/push pipeline timed out (a rank's GPU stalled or died)."""
 
 
+# Control-block fields the host reads or writes (KTB_CTRL_STATUS / KTB_CTRL_TIMEOUT_NS in csrc/ktb_common.cuh).
+_CTRL_STATUS = 1032       # u32 sticky status word: nonzero once an in-kernel wait timed out
+_CTRL_TIMEOUT_NS = 1040   # u64 spin limit of the in-kernel waits in ns, 0 = the 10 s default
+
+
 class PushSession:
     """Push/push scatter → exec → gather driven by ONE controller process over distinct GPUs
     (ktb_push_*): the root's kernel pushes shard pieces into each rank's staging buffer, each rank's
     kernel waits in-kernel for its piece, maps it and pushes the result into the root's result
-    buffer. No events between devices: flags in device memory order everything."""
+    buffer. No events between devices: flags in device memory order everything.
+
+    `call()` is the element-wise form.  Other forms (the MLP's) put their own launches between the same steps:
+    `begin()`, the root's own shard on the stream `fork()` returns, the scatter and the ranks' consumers, `finish()`."""
 
     def __init__(self, devices: Sequence[int], max_shard_bytes: int, n_chunks: int = 32):
         self.devices = [int(d) for d in devices]
@@ -561,41 +571,62 @@ class PushSession:
         for d in set(self.devices):
             torch.cuda.synchronize(d)
         self.seq = 0
-        n = len(self.devices)
         # host mirror of every control block's sticky status word, refreshed by an async D2H copy behind each call:
         # a timed-out in-kernel wait is seen at the NEXT call without a host sync on the data path
-        self._side = torch.cuda.Stream(self.root)       # the root's own shard maps beside the scatter, not behind it
+        self._side = torch.cuda.Stream(self.root)       # the root's own shard runs beside the scatter, not behind it
         self._ev_fork, self._ev_join = torch.cuda.Event(), torch.cuda.Event()
-        self._status_host = torch.zeros(n, dtype=torch.int32).pin_memory()
-        self._status_dev = [c[1032:1036].view(torch.int32) for c in self.ctrl]
-        self._stage_ptrs = L.arr(ctypes.c_void_p, [0 if s is None else s.data_ptr() for s in self.stage])
-        self._ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
-        self._n = n
+        self._status_host = torch.zeros(len(self.devices), dtype=torch.int32).pin_memory()
+        self._status_dev = [c[_CTRL_STATUS:_CTRL_STATUS + 4].view(torch.int32) for c in self.ctrl]
+        self.stage_ptrs = L.arr(ctypes.c_void_p, [0 if s is None else s.data_ptr() for s in self.stage])
+        self.ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
 
-    def call(self, x_root: torch.Tensor, out_root: torch.Tensor, op: str, alpha: float = 1.0, beta: float = 0.0):
+    def begin(self) -> int:
+        """Start a call: raise PushTimeout if an in-kernel wait of an earlier call timed out, else return the new seq."""
         if bool(self._status_host.any()):
             bad = [self.devices[i] for i in self._status_host.nonzero().flatten().tolist()]
             raise PushTimeout(f"push pipeline: an in-kernel wait timed out on cuda:{bad} during an earlier call")
         self.seq += 1
-        seq, n, es = self.seq, self._n, x_root.element_size()
+        return self.seq
+
+    def fork(self) -> torch.cuda.Stream:
+        """The side stream, ordered after the root's current stream, for the root's own shard; finish(joined=True)
+        joins it.  Fork BEFORE the scatter launch and launch the shard before it: the other order lets the two grids
+        interleave on the SMs and costs 0.3 ms at 1 GiB; shard-first costs the shard's own time (41 us for the map at
+        N = 2, 256 MiB)."""
+        with torch.cuda.device(self.root):
+            self._ev_fork.record(torch.cuda.current_stream(self.root))
+            self._side.wait_event(self._ev_fork)
+        return self._side
+
+    def finish(self, seq: int, joined: bool) -> None:
+        """End call `seq` on the root's current stream: wait for every rank's results (ktb_push_wait), join the side
+        stream if the call forked it, and queue each control block's status mirror behind the call on its device."""
+        L.call("ktb_push_wait", self.root, self.ctrl[0].data_ptr(), len(self.devices), 0, seq,
+               current_stream_handle(self.root))
+        if joined:
+            with torch.cuda.device(self.root):
+                self._ev_join.record(self._side)
+                torch.cuda.current_stream(self.root).wait_event(self._ev_join)
+        for r, d in enumerate(self.devices):
+            with torch.cuda.device(d):
+                self._status_host[r:r + 1].copy_(self._status_dev[r], non_blocking=True)
+
+    def call(self, x_root: torch.Tensor, out_root: torch.Tensor, op: str, alpha: float = 1.0, beta: float = 0.0):
+        seq = self.begin()
+        n, es = len(self.devices), x_root.element_size()
         gran = row_elems(x_root)
         rows = x_root.numel() // gran
         dt = dtype_code(x_root.dtype)
-        root_stream = _stream(self.root, None)
-        b, e = shard_bounds(rows, n, 0)  # the root's own shard maps on the root's HBM, on a side stream forked BEFORE the
-        # scatter launch and launched before it: the other order lets the two grids
-        # interleave on the SMs and costs 0.3 ms at 1 GiB; map-first costs the map's own time (41 us at N = 2, 256 MiB)
+        b, e = shard_bounds(rows, n, 0)   # the root's own shard maps on the root's HBM
         own = e > b
         if own:
-            with torch.cuda.device(self.root):
-                self._ev_fork.record(torch.cuda.current_stream(self.root))
-                self._side.wait_event(self._ev_fork)
-                L.call("ktb_map", self.root, OPS[op], dt, x_root.data_ptr() + b * gran * es,
-                       out_root.data_ptr() + b * gran * es, (e - b) * gran, float(alpha), float(beta), L.VARIANT_AUTO,
-                       int(self._side.cuda_stream))
-                self._ev_join.record(self._side)
-        L.call("ktb_push_scatter", self.root, x_root.data_ptr(), x_root.numel(), gran, dt, n, 0, self._stage_ptrs,
-               self.stride, self._ctrl_ptrs, self.ctrl[0].data_ptr(), self.n_chunks, seq, root_stream)
+            side = self.fork()
+            L.call("ktb_map", self.root, OPS[op], dt, x_root.data_ptr() + b * gran * es,
+                   out_root.data_ptr() + b * gran * es, (e - b) * gran, float(alpha), float(beta), L.VARIANT_AUTO,
+                   int(side.cuda_stream))
+        L.call("ktb_push_scatter", self.root, x_root.data_ptr(), x_root.numel(), gran, dt, n, 0, self.stage_ptrs,
+               self.stride, self.ctrl_ptrs, self.ctrl[0].data_ptr(), self.n_chunks, seq,
+               current_stream_handle(self.root))
         for r in range(1, n):
             b, e = shard_bounds(rows, n, r)
             if (e - b) * gran * es > self.stride:
@@ -603,21 +634,15 @@ class PushSession:
             L.call("ktb_push_consume", self.devices[r], OPS[op], dt, self.stage[r].data_ptr(), self.stride,
                    out_root.data_ptr() + b * gran * es, (e - b) * gran, float(alpha), float(beta),
                    self.ctrl[r].data_ptr(), self.ctrl[0].data_ptr(), r, self.n_chunks, seq,
-                   _stream(self.devices[r], None))
-        L.call("ktb_push_wait", self.root, self.ctrl[0].data_ptr(), n, 0, seq, root_stream)
-        if own:
-            with torch.cuda.device(self.root):
-                torch.cuda.current_stream(self.root).wait_event(self._ev_join)
-        for r, d in enumerate(self.devices):   # stream-ordered behind this call's kernels on each device
-            with torch.cuda.device(d):
-                self._status_host[r:r + 1].copy_(self._status_dev[r], non_blocking=True)
+                   current_stream_handle(self.devices[r]))
+        self.finish(seq, joined=own)
         return out_root
 
     def set_spin_timeout(self, seconds: float) -> None:
         """In-kernel flag waits give up after `seconds` (default 10 s) and raise the sticky status word."""
         ns = torch.tensor([int(seconds * 1e9)], dtype=torch.int64)
         for d, c in zip(self.devices, self.ctrl):
-            c[1040:1048].view(torch.int64).copy_(ns.to(f"cuda:{d}"))
+            c[_CTRL_TIMEOUT_NS:_CTRL_TIMEOUT_NS + 8].view(torch.int64).copy_(ns.to(f"cuda:{d}"))
             torch.cuda.synchronize(d)
 
     def check(self):

@@ -341,6 +341,35 @@ def test_pushed_form_on_one_gpu_matches_plain_bits(K, engine, chunk_rows):
     assert rig.statuses() == [0] * rig.n
 
 
+@pytest.mark.parametrize("output", ["logits", "actions", "both"])
+def test_package_push_path_on_one_gpu_matches_plain_bits(K, output):
+    """The package's pushed form (what mlp_scatter_gather(transfer="push") runs: a cached PushSession, copy-engine
+    scatter, the root's shard on the session's side stream) with ranks [0, 0, 0] on cuda:0.  35 072 rows per rank = two
+    full 16 896-row push chunks and a 1 280-row tail; biases; three consecutive calls (both staging halves, ack
+    back-pressure).  Ranks 1 and 2 run beside the root's shard on one device, so each needs its own scratch.  The
+    results equal mlp_forward over all rows bit for bit, and the session's status stays clean."""
+    mlp = _mlp()
+    devs, rows, d_out = [0, 0, 0], 35072, 18
+    M = 3 * rows
+    bounds = [K.shard_bounds(M, 3, r) for r in range(3)]
+    assert [e - b for b, e in bounds] == [rows] * 3 and rows == 2 * mlp.PUSH_CHUNK_ROWS + 1280
+    w, b = _config(131, d_out)
+    weights = {0: (*w, *b)}
+    for it in range(3):
+        obs = _randn((M, 256), 133 + it)
+        want_l, want_a = mlp.mlp_forward(obs, *w, biases=b, output="both")
+        logits = None if output == "actions" else \
+            torch.full((M, d_out), float("nan"), dtype=torch.bfloat16, device="cuda")
+        actions = None if output == "logits" else torch.full((M,), -1, dtype=torch.int64, device="cuda")
+        mlp._mlp_scatter_gather_pushed(obs, devs, bounds, weights, output, logits, actions)
+        torch.cuda.synchronize()
+        if logits is not None:
+            assert torch.equal(logits, want_l), (output, it)
+        if actions is not None:
+            assert torch.equal(actions, want_a), (output, it)
+    mlp._push_sessions[tuple(devs)].check()
+
+
 # ---- 5. guard bands -------------------------------------------------------------------------------------------------
 def _guarded(nbytes, misalign=0):
     """A _Guarded buffer whose start is moved `misalign` bytes past a 256-byte boundary."""

@@ -25,12 +25,6 @@ from oracle import cases  # noqa: E402
 def main():
     n_gpus = int(sys.argv[1]) if len(sys.argv) > 1 else torch.cuda.device_count()
     transfer = sys.argv[2] if len(sys.argv) > 2 else "auto"          # auto | pull | push
-    if len(sys.argv) > 3:                                              # ce | sm | hybrid (engine of the pushed scatter)
-        from kubetorch_b200.device import mlp as _mlp
-
-        _mlp.SCATTER_ENGINE = sys.argv[3]
-        if len(sys.argv) > 4:
-            _mlp.CE_RANKS = int(sys.argv[4])
     shards, rows = 4096, 512
     M = shards * rows
     g = torch.Generator(device="cuda:0").manual_seed(0)
@@ -64,7 +58,7 @@ def main():
     torch.testing.assert_close(logits[idx].float(), ref.float(), rtol=2**-7, atol=1e-2)
     flop = 2 * (256 * 1024 + 1024 * 1024 + 1024 * 64) * M
     nbytes = M * 256 * 2 + M * 64 * 2
-    print(json.dumps({"what": "c4_rl_rollout", "n_gpus": n_gpus, "transfer": transfer, "engine": sys.argv[3] if len(sys.argv) > 3 else "default", "ms_per_call": ms, "calls_per_sec": 1e3 / ms,
+    print(json.dumps({"what": "c4_rl_rollout", "n_gpus": n_gpus, "transfer": transfer, "ms_per_call": ms, "calls_per_sec": 1e3 / ms,
                       "arg_plus_result_gbps": nbytes / ms / 1e6, "tflops": flop / ms / 1e9, "parity": "ok (2048 rows)", "host_issue_ms_per_call": host_issue_ms,
                       "root_nvlink_gbps_each_way": (n_gpus - 1) / n_gpus * (M * 256 * 2) / ms / 1e6 if n_gpus > 1 else 0}),
           flush=True)
