@@ -328,6 +328,36 @@ int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_st
                                void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
                                unsigned long long seq, uintptr_t stream);
 
+/* Sampling form: the policy above with actions SAMPLED from softmax(logits) by Gumbel-max, and the log-probability
+ * of each sampled action.  For the call's global row i (row_base + the row's index in this call) and head column j:
+ *   - x = Philox4x32-10(counter = (i mod 2^32, i >> 32, j >> 1, 0), key = (seed mod 2^32, seed >> 32)), output word
+ *     j & 1.  The round is Random123's (multipliers 0xD2511F53, 0xCD9E8D57; key increments 0x9E3779B9, 0xBB67AE85),
+ *     the round of curand_philox4x32_x.h.
+ *   - u = (2*(x >> 9) + 1) * 2^-24, exact in fp32 and strictly inside (0, 1); g = -log(-log(u)) in fp32 (logf, no
+ *     fast-math), finite, within about [-2.81, 16.6].
+ *   - actions[i] = argmax_j fp32(float(logit_j) + g_j) over j < d_out, where logit_j is the bf16-rounded head output
+ *     (the value ktb_mlp_bf16_policy stores), under the torch.argmax rules of the greedy actions.
+ *   - log_probs[i] = logit_a - m - log(sum_j exp(logit_j - m)) in fp32, m the row's largest logit: torch.log_softmax
+ *     (logits.float(), -1)[a].  NaN on rows with a NaN or +inf logit and on rows whose logits are all -inf, as in
+ *     torch; -inf logits (action masking through b3) are never sampled while the row has a finite logit.
+ *   - The noise depends on (seed, i, j) only: every chunk size, form (plain, staged, pushed), rank count and device
+ *     gives the same bits when each shard passes its first global row as row_base.  A new seed draws new samples.
+ * No logits are written.  actions [M] int64 (8-byte aligned) and log_probs [M] fp32 (4-byte aligned) may be peer
+ * pointers; either one NULL with M > 0 is KTB_ERR_ARG.  Every other argument is checked as in ktb_mlp_bf16_policy
+ * (d_out > 256 is KTB_ERR_UNSUPPORTED).  Writes stay inside actions[M], log_probs[M], scratch and stage. */
+int ktb_mlp_bf16_policy_sample(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                               const void* W1, const void* b1, const void* W2, const void* b2,
+                               const void* W3, const void* b3, uint64_t seed, uint64_t row_base,
+                               int64_t* actions, float* log_probs, void* scratch, void* stage, uintptr_t stream);
+/* Push-fed sampling form: ktb_mlp_bf16_policy_pushed's arguments with (seed, row_base, actions, log_probs) in place
+ * of (logits, actions).  An empty shard (M == 0) may pass NULL outputs. */
+int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                      int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                      const void* b2, const void* W3, const void* b3, uint64_t seed,
+                                      uint64_t row_base, int64_t* actions, float* log_probs, void* scratch,
+                                      void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                      unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -10,8 +10,9 @@
 //     64 rows of the 128-row tile, both operands read straight from shared memory by descriptor,
 //   * an epilogue from the fp32 register accumulators: optional bias (nn.Linear), fused ReLU + bf16
 //     rounding, global stores masked to the head's width, and optionally the greedy action of every
-//     row — the last layer's outputs may be peer pointers into the root GPU's result arena, which
-//     fuses the gather into the epilogue.
+//     row, or instead an action sampled by seeded Gumbel-max with its log-probability — the last
+//     layer's outputs may be peer pointers into the root GPU's result arena, which fuses the gather
+//     into the epilogue.
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one lane).
 // Activations are rounded to bf16 between layers (like the eager torch module); rows are processed
 // in chunks whose hidden activations stay resident in the 50 MB L2.  One kernel
@@ -206,6 +207,25 @@ __device__ __forceinline__ bool argmax_before(float v, int col, float best, int 
   return v > best || (v == best && col < best_col);
 }
 
+// Philox4x32-10 (Random123; the round of curand_philox4x32_x.h): the four words of counter c under key k.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
+}
+
+// Gumbel noise of one random word: u = (2·(x >> 9) + 1)·2^-24 is exact and strictly inside (0, 1), g = -log(-log u).
+__device__ __forceinline__ float gumbel_of(uint32_t x) {
+  const float u = (float)(2u * (x >> 9) + 1u) * 5.9604644775390625e-8f;
+  return -logf(-logf(u));
+}
+
 // One column pair (col, col + 1) of a layer in rows r and r + 8: y0 = act(a0 + bias, a1 + bias) of row r, y1 of row
 // r + 8, each rounded once to bf16.  A column >= n_valid gets no bias.
 __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a3, const __nv_bfloat16* bias, int col,
@@ -231,6 +251,91 @@ __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a
   y1 = __floats2bfloat162_rn(v[2], v[3]);
 }
 
+// The sampling epilogue of a head tile (mlp_layer_wgmma_kernel with log_probs): rows r = row and row + 8 of the
+// thread, global rows row_base + r.  A loop of its own, so that the greedy loop keeps its compact code.  Pass 1 rounds
+// the logits once and keeps them as bf16 pairs (half the registers of the fp32 accumulators it frees: the 256-wide
+// instantiation would spill holding the accumulators, or the bias, through pass 2) and takes each row's largest logit
+// m across the quad (NaN skipped: it reaches the sum instead); pass 2 draws one Philox call per column pair < n_valid
+// and row, ranks fp32(logit + noise) in torch.argmax order and sums exp(logit - m) without a running rescale.  A logit equal to m adds 1 without an exp, so an all -inf (or a +inf) maximum never forms
+// exp(inf - inf): such rows end with a NaN log-probability, as in torch, and -inf logits beside a finite m add 0.
+template <int BLOCK_N>
+__device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
+                                                int n_valid, int relu, int row, bool st0, bool st1, int64_t* actions,
+                                                float* log_probs, uint64_t seed, uint64_t row_base) {
+  float mx[2] = {-INFINITY, -INFINITY};
+  __nv_bfloat162 y[BLOCK_N / 4];   // y[2j + h]: columns (col, col + 1) of row + 8h
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= n_valid) continue;
+    layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, relu, y[2 * j],
+               y[2 * j + 1]);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float v = q & 1 ? __high2float(y[2 * j + (q >> 1)]) : __low2float(y[2 * j + (q >> 1)]);
+      if (col + (q & 1) < n_valid && v > mx[q >> 1]) mx[q >> 1] = v;
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      const float o = __shfl_xor_sync(0xffffffffu, mx[h], m);
+      if (o > mx[h]) mx[h] = o;
+    }
+  }
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  float best[2] = {-INFINITY, -INFINITY}, best_y[2] = {0.f, 0.f}, sum[2] = {0.f, 0.f};
+  int best_col[2] = {INT_MAX, INT_MAX};
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= n_valid) continue;   // a pair wholly past the head draws no noise
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint64_t i = row_base + (uint64_t)(row + 8 * h);
+      const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 0u), key);
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        if (col + c >= n_valid) continue;
+        const float v = c ? __high2float(y[2 * j + h]) : __low2float(y[2 * j + h]);
+        const float s = v + gumbel_of(c ? x.y : x.x);
+        if (argmax_before(s, col + c, best[h], best_col[h])) {
+          best[h] = s;
+          best_col[h] = col + c;
+          best_y[h] = v;
+        }
+        sum[h] += v == mx[h] ? 1.f : expf(v - mx[h]);
+      }
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
+      const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
+      const float oy = __shfl_xor_sync(0xffffffffu, best_y[h], m);
+      sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
+      if (argmax_before(ov, oc, best[h], best_col[h])) {
+        best[h] = ov;
+        best_col[h] = oc;
+        best_y[h] = oy;
+      }
+    }
+  }
+  if ((threadIdx.x & 3) == 0) {
+    if (st0) {
+      actions[row] = best_col[0];
+      log_probs[row] = best_y[0] - mx[0] - logf(sum[0]);
+    }
+    if (st1) {
+      actions[row + 8] = best_col[1];
+      log_probs[row + 8] = best_y[1] - mx[1] - logf(sum[1]);
+    }
+  }
+}
+
 // One MLP layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid, with the bias added to the fp32
 // accumulator and the sum rounded once to bf16 (nn.Linear / F.linear), and actions[row] = the argmax of the row's
 // ROUNDED values.  One output tile per CTA; blockIdx.x walks N, so the CTAs of one 128-row block run side by side and
@@ -239,11 +344,15 @@ __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a
 // 256 for the hidden layers, and for the head the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one
 // CTA owns whole rows (gridDim.x == 1, required with actions) and the argmax never leaves it.  Columns >= n_valid
 // hold TMA zero fill: they are never stored and never an action.
+// With log_probs (and actions; C is then null) the head SAMPLES instead (Gumbel-max): the action of global row
+// i = row_base + row is the argmax of fp32(logit_j + g_j) with g_j the Gumbel noise of Philox word j & 1 of counter
+// (i, j >> 1) under `seed` (include/ktb200.h), and log_probs[row] = log_softmax(logits)[action] in fp32.
 template <int BLOCK_N, int STAGES>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                            const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ C,
-                           int64_t* __restrict__ actions, int ldc, int n_valid, int K, int rows, int relu) {
+                           int64_t* __restrict__ actions, float* __restrict__ log_probs, uint64_t seed,
+                           uint64_t row_base, int ldc, int n_valid, int K, int rows, int relu) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -256,6 +365,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
   const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const bool st0 = row < rows, st1 = row + 8 < rows;
+  if (log_probs != nullptr) {
+    sample_epilogue<BLOCK_N>(acc, bias, col0, n_valid, relu, row, st0, st1, actions, log_probs, seed, row_base);
+    return;
+  }
   // a column pair is one 4-byte store where the base and an even row stride allow it; rows of an odd d_out are
   // only 2-byte aligned and take scalar stores
   const bool pairs = C != nullptr && (ldc & 1) == 0 && ((uintptr_t)C & 3) == 0;
@@ -406,8 +519,9 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
 }
 
 template <int BLOCK_N>
-static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions, size_t M,
-                        int N, int K, int ldc, bool relu, cudaStream_t stream) {
+static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions,
+                        float* log_probs, uint64_t seed, uint64_t row_base, size_t M, int N, int K, int ldc, bool relu,
+                        cudaStream_t stream) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -421,32 +535,41 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
   kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias),
-                                                static_cast<__nv_bfloat16*>(C), actions, ldc, N, K, (int)M, relu);
+                                                static_cast<__nv_bfloat16*>(C), actions, log_probs, seed, row_base,
+                                                ldc, N, K, (int)M, relu);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
 
-// Weights, biases (each may be null) and outputs (either may be null) of one MLP call.
+// Weights, biases (each may be null) and outputs (either may be null) of one MLP call.  With log_probs the head
+// samples (actions required, logits null): row r of the call is global row row_base + r of the noise.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   void* logits;
   int64_t* actions;
+  float* log_probs = nullptr;
+  uint64_t seed = 0, row_base = 0;
 };
 
 // One hidden layer H[rows, d_hidden] = relu(A · Wᵀ (+ b)).
 static int mlp_hidden(int dev, const void* A, const void* W, const void* b, void* H, size_t rows, int d_hidden, int K,
                       cudaStream_t st) {
-  return launch_layer<256>(dev, A, W, b, H, nullptr, rows, d_hidden, K, d_hidden, true, st);
+  return launch_layer<256>(dev, A, W, b, H, nullptr, nullptr, 0, 0, rows, d_hidden, K, d_hidden, true, st);
 }
 
-// The head of rows [r0, r0 + rows): logits and/or actions of those rows from h2.
+// The head of rows [r0, r0 + rows): logits and/or actions (or sampled actions and log-probabilities) of those rows
+// from h2.
 static int mlp_head(int dev, const MlpParams& p, const void* h2, size_t r0, size_t rows, int d_hidden, int d_out,
                     cudaStream_t st) {
   void* y = p.logits ? static_cast<__nv_bfloat16*>(p.logits) + r0 * d_out : nullptr;
   int64_t* act = p.actions ? p.actions + r0 : nullptr;
-  if (d_out <= 64) return launch_layer<64>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
-  if (d_out <= 128) return launch_layer<128>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
-  return launch_layer<256>(dev, h2, p.W3, p.b3, y, act, rows, d_out, d_hidden, d_out, false, st);
+  float* lp = p.log_probs ? p.log_probs + r0 : nullptr;
+  const uint64_t rb = p.row_base + r0;
+  if (d_out <= 64)
+    return launch_layer<64>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, rows, d_out, d_hidden, d_out, false, st);
+  if (d_out <= 128)
+    return launch_layer<128>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, rows, d_out, d_hidden, d_out, false, st);
+  return launch_layer<256>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, rows, d_out, d_hidden, d_out, false, st);
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (outputs, width, element-aligned
@@ -464,6 +587,7 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
     KTB_REQUIRE((((uintptr_t)p.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
                 "%s: logits and biases must be 2-byte aligned", fn);
     KTB_REQUIRE(((uintptr_t)p.actions & 7) == 0, KTB_ERR_ARG, "%s: actions must be 8-byte aligned", fn);
+    KTB_REQUIRE(((uintptr_t)p.log_probs & 3) == 0, KTB_ERR_ARG, "%s: log_probs must be 4-byte aligned", fn);
   }
   KTB_REQUIRE((((uintptr_t)obs | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | (uintptr_t)scratch |
                 (uintptr_t)stage) & 15) == 0,
@@ -678,6 +802,35 @@ int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidd
                         int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
   const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions};
   return mlp_run("ktb_mlp_bf16_policy", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+}
+
+// The sampling entries: the policy forms with (seed, row_base, actions, log_probs) as their outputs, both required
+// for a non-empty call; everything else is checked by the policy form they run.
+int ktb_mlp_bf16_policy_sample(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                               const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                               uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs, void* scratch,
+                               void* stage, uintptr_t stream) {
+  const char* fn = "ktb_mlp_bf16_policy_sample";
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(M == 0 || (actions && log_probs), KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, actions, log_probs, seed, row_base};
+  return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                      int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                      const void* b2, const void* W3, const void* b3, uint64_t seed, uint64_t row_base,
+                                      int64_t* actions, float* log_probs, void* scratch, void* ctrl_local,
+                                      void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
+                                      uintptr_t stream) {
+  const char* fn = "ktb_mlp_bf16_policy_sample_pushed";
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(M == 0 || (actions && log_probs), KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, actions, log_probs, seed, row_base};
+  return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
+                        ctrl_root_peer, rank, chunk_rows, seq, stream);
 }
 
 }  // extern "C"

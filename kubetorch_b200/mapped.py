@@ -23,7 +23,7 @@ from typing import Any, Callable, Dict, Optional
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
-MLP_OUTPUTS = ("logits", "actions", "both")
+MLP_OUTPUTS = ("logits", "actions", "both", "sample")
 
 
 @dataclass
@@ -67,20 +67,31 @@ class MappedSpec:
 def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = None, arg: str = None, **extra):
     """Declare that the decorated function is computed by device op `op` (see module docstring).
 
-    The "mlp" op takes two more options.  ``bias=True``: the callable is ``(obs, w1, b1, w2, b2, w3, b3)``, an
-    nn.Linear policy with biases (default False: ``(obs, w1, w2, w3)``).  ``output``: ``"logits"`` (default),
-    ``"actions"`` (int64 greedy actions, argmax of the bf16 logits) or ``"both"`` (``(logits, actions)`` per rank)."""
+    The "mlp" op takes more options.  ``bias=True``: the callable is ``(obs, w1, b1, w2, b2, w3, b3, ...)``, an
+    nn.Linear policy with biases (default False: ``(obs, w1, w2, w3, ...)``).  ``output``: ``"logits"`` (default),
+    ``"actions"`` (int64 greedy actions, argmax of the bf16 logits), ``"both"`` (``(logits, actions)`` per rank) or
+    ``"sample"`` (``(actions, log_probs)`` per rank: int64 actions drawn from softmax(logits) by Gumbel-max with the
+    noise of kubetorch_b200.sampling.gumbel_noise over the rows' global indices, and the fp32 log-probability of
+    each).  ``seed``, required with ``output="sample"`` and refused otherwise: an int in [0, 2**64) or the name of a
+    call argument that holds one."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if "bias" in extra or "output" in extra:
+    if "bias" in extra or "output" in extra or "seed" in extra:
         if op != "mlp":
-            raise ValueError(f"bias= and output= are options of the 'mlp' op, not of '{op}'")
+            raise ValueError(f"bias=, output= and seed= are options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
+        sample = extra.get("output") == "sample"
+        if sample != ("seed" in extra):
+            raise ValueError('seed= is required with output="sample" and is an option of that output only')
+        if sample and not isinstance(extra["seed"], str):
+            from .sampling import _check_seed
+
+            _check_seed(extra["seed"])
 
     def deco(fn):
         setattr(fn, MAPPED_ATTR, MappedSpec(op=op, alpha=alpha, beta=beta, reduce=reduce, arg=arg, extra=extra))

@@ -406,7 +406,7 @@ class B200Supervisor:
                 # a shard view would drag the whole result buffer's storage along
                 if isinstance(result, torch.Tensor):
                     result = result.clone()
-                elif isinstance(result, tuple):   # the (logits, actions) of an mlp op with output="both"
+                elif isinstance(result, tuple):   # (logits, actions) or (actions, log_probs) of an mlp op
                     result = tuple(t.clone() if isinstance(t, torch.Tensor) else t for t in result)
                 return {"data": base64.b64encode(pickle.dumps(result)).decode("utf-8")}
             except Exception as e:  # noqa: BLE001
@@ -591,9 +591,14 @@ class B200Supervisor:
         else:
             obs, w1, w2, w3 = (bound[n] for n in names[:4])
             biases = (None, None, None)
+        seed = spec.extra.get("seed")
+        if isinstance(seed, str):   # the name of a call argument, resolved per call
+            if seed not in bound:
+                raise TypeError(f"mapped mlp callable: seed argument '{seed}' not found in the call")
+            seed = bound[seed]
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
-                                         biases=biases, output=output)
+                                         biases=biases, output=output, seed=seed)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -10,9 +10,13 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
   d  policy with biases, d_out 64, actions only
   e  policy with biases, d_out 64, logits and actions
   f  policy with biases, d_out 18 and d_out 256, logits and actions
+  g  policy with biases, d_out 18, 64 and 256, sampled actions and log-probabilities (output="sample"), timed in the
+     same alternation as d (actions only), which has the same GEMMs and no noise
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
-exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  The card name and its power
-limit are read in the same run.  Prints one JSON line."""
+exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
+consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
+exceeds 2^-18·(1 + max|s|), and the log-probability is within (d_out + 8)·2^-22·(1 + |ref|) of the fp64 log_softmax.
+The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
 import json
 import os
@@ -27,6 +31,9 @@ import torch  # noqa: E402
 from kubetorch_b200.device import lib as L  # noqa: E402
 from kubetorch_b200.device import mlp  # noqa: E402
 from kubetorch_b200.device import ops  # noqa: E402
+from kubetorch_b200.sampling import gumbel_uniform  # noqa: E402
+
+SEED = 0x5EED
 
 
 def _power_limit_w():
@@ -89,6 +96,9 @@ def main():
         "f_bias_both_d256": (256, lambda: mlp.mlp_forward(obs, w1, w2, heads[256][0], biases=(b1, b2, heads[256][1]),
                                                           output="both")),
     }
+    for d in (18, 64, 256):
+        variants[f"g_bias_sample_d{d}"] = (d, lambda d=d: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]), output="sample", seed=SEED))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -130,6 +140,21 @@ def main():
                           "actions_only_eq_both": "ok"})
         parity[name] = entry
     assert parity["b_equals_a_bitwise"]
+    r0 = M - 2048 - 77
+    for d in (18, 64, 256):
+        actions, log_probs = variants[f"g_bias_sample_d{d}"][1]()
+        w, bs = (w1, w2, heads[d][0]), (b1, b2, heads[d][1])
+        y = mlp.mlp_forward(obs[r0:r0 + 2048], *w, biases=bs).double()
+        s64 = y - torch.log(-torch.log(gumbel_uniform(SEED, r0, 2048, d, device="cuda:0").double()))
+        a = actions[r0:r0 + 2048]
+        eps = 2.0 ** -18 * (1 + s64.abs().amax(1))
+        top2 = s64.topk(2, dim=1).values
+        clear = (top2[:, 0] - top2[:, 1]) > eps
+        assert bool((s64.gather(1, a[:, None]).squeeze(1) >= top2[:, 0] - eps).all())
+        assert torch.equal(a[clear], s64.argmax(1)[clear])
+        ref = y.gather(1, a[:, None]).squeeze(1) - torch.logsumexp(y, -1)
+        assert bool(((log_probs[r0:r0 + 2048].double() - ref).abs() <= (d + 8) * 2.0 ** -22 * (1 + ref.abs())).all())
+        parity[f"g_bias_sample_d{d}"] = {"sample_bars_2048_rows": "ok", "clear_rows": int(clear.sum())}
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
