@@ -358,6 +358,42 @@ int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t s
                                       void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
                                       unsigned long long seq, uintptr_t stream);
 
+/* Gaussian form: the policy above as the mean of a diagonal Gaussian with a state-independent log standard deviation
+ * log_std [d_out] (fp32), as in PPO's continuous policies.  For the call's global row i (row_base + the row's index
+ * in this call) and head column j:
+ *   - x = Philox4x32-10(counter = (i mod 2^32, i >> 32, j >> 1, 1), key = (seed mod 2^32, seed >> 32)), output word
+ *     j & 1: the Philox of the sampling form, with counter word 3 = 1, so that one seed never gives the Gaussian and
+ *     the Gumbel heads the same uniforms.
+ *   - u = (2*(x >> 9) + 1) * 2^-24, exact in fp32, strictly inside (0, 1) and never 0.5; z = normcdfinvf(u) in fp32
+ *     (no fast-math), never 0 and within +-5.29471 (= Phi^-1(1 - 2^-24)): the tails beyond (probability mass about
+ *     1.2e-7) are never drawn.
+ *   - sigma_j = expf(log_std[j]); actions[i, j] = __fadd_rn(mu_ij, __fmul_rn(sigma_j, z_ij)) (no FMA contraction),
+ *     where mu_ij is the bf16-rounded head output (the value ktb_mlp_bf16_policy stores).
+ *   - log_probs[i] = -sum_j (0.5*z_ij^2 + log_std[j]) - d_out*0.5*log(2*pi) in fp32: Normal(mu, sigma).log_prob(a)
+ *     .sum(-1), computed from z, so it does not depend on mu.
+ *   - IEEE cases: log_std[j] = -inf gives sigma = 0, actions[i, j] == mu_ij as a value and log_probs = +inf;
+ *     log_std[j] = +inf gives +-inf actions (z != 0) and log_probs = -inf; a NaN log_std[j] gives a NaN column and
+ *     NaN log-probabilities.  A NaN or +-inf logit affects its own action only; the row's log-probability is unchanged.
+ *   - The noise depends on (seed, i, j) only: every chunk size, form (plain, staged, pushed), rank count and device
+ *     gives the same bits when each shard passes its first global row as row_base.
+ * No logits are written.  actions [M, d_out] fp32 (4-byte aligned; may be a peer pointer), log_probs [M] fp32 (4-byte
+ * aligned) and log_std [d_out] fp32 (4-byte aligned): any one NULL with M > 0 is KTB_ERR_ARG.  Every other argument is
+ * checked as in ktb_mlp_bf16_policy (d_out > 256 is KTB_ERR_UNSUPPORTED).  Writes stay inside actions[M, d_out],
+ * log_probs[M], scratch and stage. */
+int ktb_mlp_bf16_policy_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                 const void* W1, const void* b1, const void* W2, const void* b2,
+                                 const void* W3, const void* b3, const float* log_std, uint64_t seed,
+                                 uint64_t row_base, float* actions, float* log_probs, void* scratch, void* stage,
+                                 uintptr_t stream);
+/* Push-fed Gaussian form: ktb_mlp_bf16_policy_sample_pushed's arguments with log_std before the seed and fp32
+ * actions [M, d_out].  An empty shard (M == 0) may pass NULL outputs. */
+int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                        int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                        const void* b2, const void* W3, const void* b3, const float* log_std,
+                                        uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
+                                        void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                        size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

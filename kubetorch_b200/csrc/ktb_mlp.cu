@@ -336,6 +336,85 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   }
 }
 
+// The Gaussian epilogue of a head tile (mlp_layer_wgmma_kernel with log_std): rows r = row and row + 8 of the thread,
+// global rows row_base + r.  A compact loop of its own, apart from the greedy loop and sample_epilogue: fully unrolled
+// here (as those are) it made the kernel half as large again, and ptxas then scheduled sample_epilogue differently and
+// 3-9 % slower.  So the unrolled part only rounds the logits once (layer_pair: μ, the value ktb_mlp_bf16_policy
+// stores) and parks them as bf16 pairs in the TMA ring, each warp in the 16 A rows of every stage that only its own
+// accumulator rows are made of: once the warp's wgmmas are waited for nothing reads or writes them again (every load
+// has landed, and no other warp's wgmma reads those rows).  A rolled loop then makes one pass over the column pairs
+// < n_valid: one Philox call per pair and row (counter word 3 = 1: never the Gumbel stream's uniforms),
+// z = Φ⁻¹(u) (normcdfinvf, no fast-math; u is never 0.5, so z != 0), the action μ + σ·z rounded twice (no FMA
+// contraction), stored as float2 where the row stride and the base allow and as scalars otherwise, and
+// Σ (0.5·z² + log_std) per row for the log-probability, which does not read μ.
+template <int BLOCK_N, int STAGES>
+__device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
+                                                  int n_valid, int relu, int row, bool st0, bool st1,
+                                                  const float* log_std, float* actions, float* log_probs,
+                                                  uint64_t seed, uint64_t row_base) {
+  // opaque copies of the inputs this epilogue shares with the others: without them the compiler hoists the common
+  // index and address arithmetic above the mode branch, and ptxas schedules sample_epilogue 2-3 % slower
+  asm volatile("" : "+l"(seed), "+l"(row_base), "+l"(bias), "+r"(col0), "+r"(n_valid), "+r"(row));
+  using S = MlpSmem<BLOCK_N, STAGES>;
+  static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  // pair w (= 2j + h) of a lane: stage w / 16, A rows 16·warp .. 16·warp + 15 (2 KiB), word (w % 16)·32 + lane
+  uint8_t* mine = smem + (threadIdx.x >> 5) * 16 * 128 + (threadIdx.x & 31) * 4;
+  auto slot = [&](int w) { return reinterpret_cast<__nv_bfloat162*>(mine + (w >> 4) * S::kStageBytes + (w & 15) * 128); };
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= n_valid) continue;
+    layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, relu, *slot(2 * j),
+               *slot(2 * j + 1));
+  }
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const bool pairs = (n_valid & 1) == 0 && ((uintptr_t)actions & 7) == 0;
+  float sum[2] = {0.f, 0.f};
+#pragma unroll 1
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= n_valid) break;   // a pair wholly past the head draws no noise
+    const __nv_bfloat162 y[2] = {*slot(2 * j), *slot(2 * j + 1)};
+    const bool has1 = col + 1 < n_valid;
+    const float ls[2] = {log_std[col], has1 ? log_std[col + 1] : 0.f};
+    const float sg[2] = {expf(ls[0]), expf(ls[1])};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint64_t i = row_base + (uint64_t)(row + 8 * h);
+      const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 1u), key);
+      float a[2];
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const float u = (float)(2u * ((c ? x.y : x.x) >> 9) + 1u) * 5.9604644775390625e-8f;
+        const float z = normcdfinvf(u);
+        a[c] = __fadd_rn(c ? __high2float(y[h]) : __low2float(y[h]), __fmul_rn(sg[c], z));
+        if (c == 0 || has1) sum[h] += 0.5f * z * z + ls[c];
+      }
+      if (!(h ? st1 : st0)) continue;
+      float* p = actions + (size_t)(row + 8 * h) * n_valid + col;
+      if (pairs) {
+        *reinterpret_cast<float2*>(p) = make_float2(a[0], a[1]);
+      } else {
+        p[0] = a[0];
+        if (has1) p[1] = a[1];
+      }
+    }
+  }
+  // the 4 lanes of a quad hold the columns of the same two rows
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
+  }
+  if ((threadIdx.x & 3) == 0) {
+    const float c = (float)n_valid * 0.918938533204672742f;   // d_out·0.5·log(2π)
+    if (st0) log_probs[row] = -sum[0] - c;
+    if (st1) log_probs[row + 8] = -sum[1] - c;
+  }
+}
+
 // One MLP layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid, with the bias added to the fp32
 // accumulator and the sum rounded once to bf16 (nn.Linear / F.linear), and actions[row] = the argmax of the row's
 // ROUNDED values.  One output tile per CTA; blockIdx.x walks N, so the CTAs of one 128-row block run side by side and
@@ -347,12 +426,16 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
 // With log_probs (and actions; C is then null) the head SAMPLES instead (Gumbel-max): the action of global row
 // i = row_base + row is the argmax of fp32(logit_j + g_j) with g_j the Gumbel noise of Philox word j & 1 of counter
 // (i, j >> 1) under `seed` (include/ktb200.h), and log_probs[row] = log_softmax(logits)[action] in fp32.
+// With log_std (and gauss_actions and log_probs; C and actions are then null) the head draws Gaussian actions
+// instead: gauss_actions[row, j] = logit_j + exp(log_std_j)·z_j with z_j = Φ⁻¹(u) of Philox word j & 1 of counter
+// (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (include/ktb200.h).
 template <int BLOCK_N, int STAGES>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                            const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ C,
                            int64_t* __restrict__ actions, float* __restrict__ log_probs, uint64_t seed,
-                           uint64_t row_base, int ldc, int n_valid, int K, int rows, int relu) {
+                           uint64_t row_base, const float* __restrict__ log_std, float* __restrict__ gauss_actions,
+                           int ldc, int n_valid, int K, int rows, int relu) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -365,6 +448,11 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
   const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const bool st0 = row < rows, st1 = row + 8 < rows;
+  if (log_std != nullptr) {
+    gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, relu, row, st0, st1, log_std, gauss_actions,
+                                       log_probs, seed, row_base);
+    return;
+  }
   if (log_probs != nullptr) {
     sample_epilogue<BLOCK_N>(acc, bias, col0, n_valid, relu, row, st0, st1, actions, log_probs, seed, row_base);
     return;
@@ -520,8 +608,8 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
 
 template <int BLOCK_N>
 static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions,
-                        float* log_probs, uint64_t seed, uint64_t row_base, size_t M, int N, int K, int ldc, bool relu,
-                        cudaStream_t stream) {
+                        float* log_probs, uint64_t seed, uint64_t row_base, const float* log_std, float* gauss_actions,
+                        size_t M, int N, int K, int ldc, bool relu, cudaStream_t stream) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -536,25 +624,29 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
   kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias),
                                                 static_cast<__nv_bfloat16*>(C), actions, log_probs, seed, row_base,
-                                                ldc, N, K, (int)M, relu);
+                                                log_std, gauss_actions, ldc, N, K, (int)M, relu);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
 
 // Weights, biases (each may be null) and outputs (either may be null) of one MLP call.  With log_probs the head
-// samples (actions required, logits null): row r of the call is global row row_base + r of the noise.
+// samples (actions required, logits null): row r of the call is global row row_base + r of the noise.  With log_std
+// as well it draws Gaussian actions into gauss_actions instead (actions and logits null).
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   void* logits;
   int64_t* actions;
   float* log_probs = nullptr;
   uint64_t seed = 0, row_base = 0;
+  const float* log_std = nullptr;
+  float* gauss_actions = nullptr;
 };
 
 // One hidden layer H[rows, d_hidden] = relu(A · Wᵀ (+ b)).
 static int mlp_hidden(int dev, const void* A, const void* W, const void* b, void* H, size_t rows, int d_hidden, int K,
                       cudaStream_t st) {
-  return launch_layer<256>(dev, A, W, b, H, nullptr, nullptr, 0, 0, rows, d_hidden, K, d_hidden, true, st);
+  return launch_layer<256>(dev, A, W, b, H, nullptr, nullptr, 0, 0, nullptr, nullptr, rows, d_hidden, K, d_hidden,
+                           true, st);
 }
 
 // The head of rows [r0, r0 + rows): logits and/or actions (or sampled actions and log-probabilities) of those rows
@@ -564,12 +656,16 @@ static int mlp_head(int dev, const MlpParams& p, const void* h2, size_t r0, size
   void* y = p.logits ? static_cast<__nv_bfloat16*>(p.logits) + r0 * d_out : nullptr;
   int64_t* act = p.actions ? p.actions + r0 : nullptr;
   float* lp = p.log_probs ? p.log_probs + r0 : nullptr;
+  float* ga = p.gauss_actions ? p.gauss_actions + r0 * d_out : nullptr;
   const uint64_t rb = p.row_base + r0;
   if (d_out <= 64)
-    return launch_layer<64>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, rows, d_out, d_hidden, d_out, false, st);
+    return launch_layer<64>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, p.log_std, ga, rows, d_out, d_hidden, d_out,
+                            false, st);
   if (d_out <= 128)
-    return launch_layer<128>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, rows, d_out, d_hidden, d_out, false, st);
-  return launch_layer<256>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, rows, d_out, d_hidden, d_out, false, st);
+    return launch_layer<128>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, p.log_std, ga, rows, d_out, d_hidden, d_out,
+                             false, st);
+  return launch_layer<256>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, p.log_std, ga, rows, d_out, d_hidden, d_out,
+                           false, st);
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (outputs, width, element-aligned
@@ -581,7 +677,13 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
   KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "%s: d_hidden=%d must be a multiple of 256", fn,
               d_hidden);
   if (M > 0) {
-    KTB_REQUIRE(p.logits || p.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
+    KTB_REQUIRE(p.logits || p.actions || p.log_std, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
+    if (p.log_std) {
+      KTB_REQUIRE(p.gauss_actions && p.log_probs && !p.logits && !p.actions, KTB_ERR_ARG,
+                  "%s: the Gaussian head needs fp32 actions and log_probs, and stores nothing else", fn);
+      KTB_REQUIRE((((uintptr_t)p.log_std | (uintptr_t)p.gauss_actions) & 3) == 0, KTB_ERR_ARG,
+                  "%s: log_std and actions must be 4-byte aligned", fn);
+    }
     KTB_REQUIRE(d_out >= 1, KTB_ERR_ARG, "%s: d_out=%d must be positive", fn, d_out);
     KTB_REQUIRE(d_out <= 256, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (heads up to 256 wide)", fn, d_out);
     KTB_REQUIRE((((uintptr_t)p.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
@@ -829,6 +931,37 @@ int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t s
   if (rc) return rc;
   KTB_REQUIRE(M == 0 || (actions && log_probs), KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
   const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, actions, log_probs, seed, row_base};
+  return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
+                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+}
+
+// The Gaussian entries: the policy forms with (log_std, seed, row_base, fp32 actions, log_probs), all three pointers
+// required for a non-empty call; everything else is checked by the policy form they run.
+int ktb_mlp_bf16_policy_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                 const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                                 const float* log_std, uint64_t seed, uint64_t row_base, float* actions,
+                                 float* log_probs, void* scratch, void* stage, uintptr_t stream) {
+  const char* fn = "ktb_mlp_bf16_policy_gaussian";
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(M == 0 || (log_std && actions && log_probs), KTB_ERR_ARG,
+              "%s: log_std, actions and log_probs are required", fn);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, nullptr, log_probs, seed, row_base, log_std, actions};
+  return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                        int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                        const void* b2, const void* W3, const void* b3, const float* log_std,
+                                        uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
+                                        void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                        size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const char* fn = "ktb_mlp_bf16_policy_gaussian_pushed";
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(M == 0 || (log_std && actions && log_probs), KTB_ERR_ARG,
+              "%s: log_std, actions and log_probs are required", fn);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, nullptr, log_probs, seed, row_base, log_std, actions};
   return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
                         ctrl_root_peer, rank, chunk_rows, seq, stream);
 }

@@ -1,6 +1,7 @@
 """bf16 MLP policy (BASELINE config C4) on wgmma tensor cores — tensor-facing wrapper of
 ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions), ktb_mlp_bf16_policy_sample (seeded
-Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling) and their scatter→exec→gather form."""
+Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_mlp_bf16_policy_gaussian (seeded
+diagonal-Gaussian actions with their log-probabilities) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -50,22 +51,29 @@ def _thread_pool():
     return _pool
 
 
-OUTPUTS = ("logits", "actions", "both", "sample")
+OUTPUTS = ("logits", "actions", "both", "sample", "gaussian")
 MAX_D_OUT = 256
 
 
-def _check_policy(w1, w3, biases, output, seed=None) -> None:
-    """Raise ValueError for an output mode, a head width, a bias or (output="sample") a seed the kernels do not
-    take.  A seed is an int (not a bool) in [0, 2**64)."""
+def _check_policy(w1, w3, biases, output, seed=None, log_std=None) -> None:
+    """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed or
+    (output="gaussian") a log_std the kernels do not take.  A seed is an int (not a bool) in [0, 2**64); log_std is
+    a 1-D contiguous CUDA float32 tensor of length d_out, given with output="gaussian" only."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
-    if output == "sample":
+    if output in ("sample", "gaussian"):
         _check_seed(seed)
     if len(biases) != 3:
         raise ValueError("biases must be (b1, b2, b3), each a tensor or None")
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if not 1 <= d_out <= MAX_D_OUT:
         raise ValueError(f"d_out={d_out}: the policy head is 1 to {MAX_D_OUT} wide")
+    if output != "gaussian":
+        if log_std is not None:
+            raise ValueError('log_std is an argument of output="gaussian" only')
+    elif not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32 or not log_std.is_cuda \
+            or not log_std.is_contiguous() or log_std.dim() != 1 or log_std.shape[0] != d_out:
+        raise ValueError(f"log_std must be a 1-D contiguous CUDA float32 tensor of length {d_out}")
     for name, b, n in zip(("b1", "b2", "b3"), biases, (d_hidden, d_hidden, d_out)):
         if b is None:
             continue
@@ -79,15 +87,17 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 stream: Optional[torch.cuda.Stream] = None, staged: Optional[bool] = None,
                 biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
                 actions: Optional[torch.Tensor] = None, seed: Optional[int] = None, row_offset: int = 0,
-                log_probs: Optional[torch.Tensor] = None):
+                log_probs: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
-    (returns (logits, actions)) or "sample" (returns (actions, log_probs): int64 actions drawn from
+    (returns (logits, actions)), "sample" (returns (actions, log_probs): int64 actions drawn from
     softmax(logits) by Gumbel-max with the noise of kubetorch_b200.sampling.gumbel_noise(seed, row_offset, M, d_out),
-    and the fp32 log_softmax(logits)[action] of each row; no logits are written).  `obs` / `out` / `actions` /
-    `log_probs` may be peer-mapped (pull the observations / push the results over NVLink).  Without biases, at
-    d_out == 64 and with logits only the logits equal ktb_mlp_bf16's."""
+    and the fp32 log_softmax(logits)[action] of each row; no logits are written) or "gaussian" (returns (actions,
+    log_probs): fp32 actions[M, d_out] = logits + exp(log_std)·normal_noise(seed, row_offset, M, d_out) and the fp32
+    log-density of each row's action under Normal(logits, exp(log_std)); no logits are written).  `obs` / `out` /
+    `actions` / `log_probs` may be peer-mapped (pull the observations / push the results over NVLink).  Without
+    biases, at d_out == 64 and with logits only the logits equal ktb_mlp_bf16's."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -97,10 +107,11 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
-    _check_policy(w1, w3, biases, output, seed)
-    if output == "sample" and (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
+    _check_policy(w1, w3, biases, output, seed, log_std)
+    if output in ("sample", "gaussian") and \
+            (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
-    want_logits, want_actions = output in ("logits", "both"), output != "logits"
+    want_logits, want_actions = output in ("logits", "both"), output not in ("logits", "gaussian")
     if want_logits:
         if out is None:
             out = torch.empty(M, d_out, dtype=torch.bfloat16, device=f"cuda:{dev}")
@@ -115,6 +126,20 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+    if output == "gaussian":
+        if actions is None:
+            actions = torch.empty(M, d_out, dtype=torch.float32, device=f"cuda:{dev}")
+        else:
+            ops.ensure_init({actions.device.index})
+        if log_probs is None:
+            log_probs = torch.empty(M, dtype=torch.float32, device=f"cuda:{dev}")
+        else:
+            ops.ensure_init({log_probs.device.index})
+        L.call("ktb_mlp_bf16_policy_gaussian", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(),
+               ptr(biases[0]), w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), log_std.data_ptr(), seed,
+               row_offset, ptr(actions), ptr(log_probs), _scratch_for(dev, M, d_hidden).data_ptr(),
+               _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
+        return actions, log_probs
     if output == "sample":
         if log_probs is None:
             log_probs = torch.empty(M, dtype=torch.float32, device=f"cuda:{dev}")
@@ -157,13 +182,15 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
-                               seed=None) -> None:
+                               seed=None, log_std=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
     scatter.  No host synchronisation, no events between devices.  weights[dev] = (w1, w2, w3, b1, b2, b3) on that
-    device (biases may be None); out_root / actions_root / log_probs_root are None when `output` does not want them.
-    With output="sample" rank r draws the noise of global rows b_r .. e_r - 1 (its shard's place in obs_root)."""
+    device (biases may be None); out_root / actions_root / log_probs_root are None when `output` does not want them
+    (with "gaussian", actions_root holds the fp32 actions [M, d_out]).  log_std[dev] is the Gaussian head's log_std on
+    that device.  With output="sample" or "gaussian" rank r draws the noise of global rows b_r .. e_r - 1 (its shard's
+    place in obs_root)."""
     root, n, key = devs[0], len(devs), tuple(devs)
     d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0]
     rows = max(e - b for b, e in bounds)
@@ -187,7 +214,8 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b0:e0],
                     device=root, stream=sess.fork(), staged=False, biases=ws[3:], output=output,
                     actions=None if actions_root is None else actions_root[b0:e0], seed=seed, row_offset=b0,
-                    log_probs=None if log_probs_root is None else log_probs_root[b0:e0])
+                    log_probs=None if log_probs_root is None else log_probs_root[b0:e0],
+                    log_std=None if log_std is None else log_std[root])
     L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
            L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
            PUSH_CHUNK_ROWS * d_in, seq, streams[0])
@@ -196,6 +224,13 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         b, e = bounds[r]
         ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
+        if output == "gaussian":
+            L.call("ktb_mlp_bf16_policy_gaussian_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in,
+                   d_hidden, d_out, ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(),
+                   ptr(ws[5]), ptr(log_std[devs[r]]), seed, b, ptr(actions_root[b:e]), ptr(log_probs_root[b:e]),
+                   scratch[r].data_ptr(), sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq,
+                   streams[r])
+            return
         if output == "sample":
             L.call("ktb_mlp_bf16_policy_sample_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in,
                    d_hidden, d_out, ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(),
@@ -216,18 +251,19 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        out_root: Optional[torch.Tensor] = None, transfer: str = "auto",
                        biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
                        actions_root: Optional[torch.Tensor] = None, seed: Optional[int] = None,
-                       log_probs_root: Optional[torch.Tensor] = None) -> list:
+                       log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
-    int64 actions views for "actions", (logits, actions) pairs for "both", (actions, log_probs) pairs for "sample".
-    With "sample" rank r draws the noise of the global rows of its shard (row_offset = its shard's begin), so the
-    result does not depend on the number of ranks or their devices.  `biases` as in mlp_forward."""
+    int64 actions views for "actions", (logits, actions) pairs for "both", (actions, log_probs) pairs for "sample"
+    and "gaussian" (fp32 actions [rows, d_out] with the latter).  With "sample" or "gaussian" rank r draws the noise of
+    the global rows of its shard (row_offset = its shard's begin), so the result does not depend on the number of
+    ranks or their devices.  `biases`, `seed` and `log_std` as in mlp_forward."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed)
+    _check_policy(w1, w3, biases, output, seed, log_std)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     d_out = w3.shape[0]
@@ -239,8 +275,9 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if output == "logits":
         actions_root = None
     elif actions_root is None:
-        actions_root = torch.empty(M, dtype=torch.int64, device=obs_root.device)
-    if output != "sample":
+        shape, dtype = ((M, d_out), torch.float32) if output == "gaussian" else ((M,), torch.int64)
+        actions_root = torch.empty(shape, dtype=dtype, device=obs_root.device)
+    if output not in ("sample", "gaussian"):
         log_probs_root = None
     elif log_probs_root is None:
         log_probs_root = torch.empty(M, dtype=torch.float32, device=obs_root.device)
@@ -252,11 +289,12 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         views = [out_root[b:e] for b, e in bounds]
     elif output == "actions":
         views = [actions_root[b:e] for b, e in bounds]
-    elif output == "sample":
+    elif output in ("sample", "gaussian"):
         views = [(actions_root[b:e], log_probs_root[b:e]) for b, e in bounds]
     else:
         views = [(out_root[b:e], actions_root[b:e]) for b, e in bounds]
     weights = {dev: _weights_on(dev, (w1, w2, w3)) + _weights_on(dev, biases) for dev in set(devs)}
+    log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
     distinct = len(set(devs)) == len(devs) and len(devs) > 1
     pushable = distinct and all((e - b) % 128 == 0 for b, e in bounds) and \
         -(-max(e - b for b, e in bounds) // PUSH_CHUNK_ROWS) <= 64
@@ -266,7 +304,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root,
-                                   seed)
+                                   seed, log_stds)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -288,7 +326,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
             mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b:e],
                         device=dev, stream=st, biases=ws[3:], output=output,
                         actions=None if actions_root is None else actions_root[b:e], seed=seed, row_offset=b,
-                        log_probs=None if log_probs_root is None else log_probs_root[b:e])
+                        log_probs=None if log_probs_root is None else log_probs_root[b:e],
+                        log_std=None if log_stds is None else log_stds[dev])
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

@@ -23,7 +23,7 @@ from typing import Any, Callable, Dict, Optional
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
-MLP_OUTPUTS = ("logits", "actions", "both", "sample")
+MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian")
 
 
 @dataclass
@@ -72,28 +72,40 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     ``"actions"`` (int64 greedy actions, argmax of the bf16 logits), ``"both"`` (``(logits, actions)`` per rank) or
     ``"sample"`` (``(actions, log_probs)`` per rank: int64 actions drawn from softmax(logits) by Gumbel-max with the
     noise of kubetorch_b200.sampling.gumbel_noise over the rows' global indices, and the fp32 log-probability of
-    each).  ``seed``, required with ``output="sample"`` and refused otherwise: an int in [0, 2**64) or the name of a
-    call argument that holds one."""
+    each) or ``"gaussian"`` (``(actions, log_probs)`` per rank: fp32 actions ``logits + exp(log_std)·z`` with ``z``
+    the noise of kubetorch_b200.sampling.normal_noise over the rows' global indices, and the fp32 log-density of each
+    row's action; the callable is ``(obs, w1, b1, w2, b2, w3, b3, log_std, seed)``).  ``seed``, required with
+    ``output="sample"`` or ``"gaussian"`` and refused otherwise: an int in [0, 2**64) or the name of a call argument
+    that holds one.  ``log_std``, required with ``output="gaussian"`` and refused otherwise: the name of the call
+    argument that holds the fp32 [d_out] log standard deviation."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if "bias" in extra or "output" in extra or "seed" in extra:
+    if "bias" in extra or "output" in extra or "seed" in extra or "log_std" in extra:
         if op != "mlp":
-            raise ValueError(f"bias=, output= and seed= are options of the 'mlp' op, not of '{op}'")
+            raise ValueError(f"bias=, output=, seed= and log_std= are options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
-        sample = extra.get("output") == "sample"
+        sample = extra.get("output") in ("sample", "gaussian")
         if sample != ("seed" in extra):
-            raise ValueError('seed= is required with output="sample" and is an option of that output only')
+            raise ValueError('seed= is required with output="sample" or "gaussian" and is an option of those only')
         if sample and not isinstance(extra["seed"], str):
             from .sampling import _check_seed
 
             _check_seed(extra["seed"])
+        gaussian = extra.get("output") == "gaussian"
+        if gaussian != ("log_std" in extra):
+            raise ValueError('log_std= is required with output="gaussian" and is an option of that output only')
+        if gaussian and not isinstance(extra["log_std"], str):
+            raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
 
     def deco(fn):
+        name = extra.get("log_std")
+        if name is not None and name not in inspect.signature(fn).parameters:
+            raise ValueError(f"log_std={name!r} is not an argument of {getattr(fn, '__name__', fn)!r}")
         setattr(fn, MAPPED_ATTR, MappedSpec(op=op, alpha=alpha, beta=beta, reduce=reduce, arg=arg, extra=extra))
         return fn
 

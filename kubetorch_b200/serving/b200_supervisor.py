@@ -596,9 +596,14 @@ class B200Supervisor:
             if seed not in bound:
                 raise TypeError(f"mapped mlp callable: seed argument '{seed}' not found in the call")
             seed = bound[seed]
+        log_std = spec.extra.get("log_std")
+        if log_std is not None:   # always the name of a call argument, resolved per call
+            if log_std not in bound:
+                raise TypeError(f"mapped mlp callable: log_std argument '{log_std}' not found in the call")
+            log_std = bound[log_std]
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
-                                         biases=biases, output=output, seed=seed)
+                                         biases=biases, output=output, seed=seed, log_std=log_std)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -12,10 +12,14 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
   f  policy with biases, d_out 18 and d_out 256, logits and actions
   g  policy with biases, d_out 18, 64 and 256, sampled actions and log-probabilities (output="sample"), timed in the
      same alternation as d (actions only), which has the same GEMMs and no noise
+  h  policy with biases, d_out 6, 18 and 64, Gaussian actions and log-probabilities (output="gaussian", log_std over
+     [-2, 0.5]), timed in the same alternation beside the logits-only call and output="sample" at the same d_out
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
 exceeds 2^-18·(1 + max|s|), and the log-probability is within (d_out + 8)·2^-22·(1 + |ref|) of the fp64 log_softmax.
+Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
 import json
@@ -32,6 +36,8 @@ from kubetorch_b200.device import lib as L  # noqa: E402
 from kubetorch_b200.device import mlp  # noqa: E402
 from kubetorch_b200.device import ops  # noqa: E402
 from kubetorch_b200.sampling import gumbel_uniform  # noqa: E402
+
+HALF_LOG_2PI = 0.9189385332046727
 
 SEED = 0x5EED
 
@@ -99,6 +105,19 @@ def main():
     for d in (18, 64, 256):
         variants[f"g_bias_sample_d{d}"] = (d, lambda d=d: mlp.mlp_forward(
             obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]), output="sample", seed=SEED))
+    g6 = torch.Generator(device="cuda:0").manual_seed(6)   # its own generator: the other heads and rows stay as they were
+    heads[6] = ((torch.randn(6, d_hidden, device="cuda:0", generator=g6) * 0.02).bfloat16(),
+                (torch.randn(6, device="cuda:0", generator=g6) * 0.1).bfloat16())
+    log_stds = {d: torch.linspace(-2.0, 0.5, d, device="cuda:0") for d in (6, 18, 64)}
+    for d in (6, 18):
+        variants[f"h_bias_logits_d{d}"] = (d, lambda d=d: mlp.mlp_forward(obs, w1, w2, heads[d][0],
+                                                                          biases=(b1, b2, heads[d][1])))
+    variants["h_bias_sample_d6"] = (6, lambda: mlp.mlp_forward(obs, w1, w2, heads[6][0], biases=(b1, b2, heads[6][1]),
+                                                               output="sample", seed=SEED))
+    for d in (6, 18, 64):
+        variants[f"h_bias_gaussian_d{d}"] = (d, lambda d=d: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]), output="gaussian", seed=SEED,
+            log_std=log_stds[d]))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -155,6 +174,20 @@ def main():
         ref = y.gather(1, a[:, None]).squeeze(1) - torch.logsumexp(y, -1)
         assert bool(((log_probs[r0:r0 + 2048].double() - ref).abs() <= (d + 8) * 2.0 ** -22 * (1 + ref.abs())).all())
         parity[f"g_bias_sample_d{d}"] = {"sample_bars_2048_rows": "ok", "clear_rows": int(clear.sum())}
+    for d in (6, 18, 64):
+        actions, log_probs = variants[f"h_bias_gaussian_d{d}"][1]()
+        w, bs = (w1, w2, heads[d][0]), (b1, b2, heads[d][1])
+        y = mlp.mlp_forward(obs[r0:r0 + 2048], *w, biases=bs).double()
+        z = torch.special.ndtri(gumbel_uniform(SEED, r0, 2048, d, device="cuda:0", word3=1).double())
+        ls = log_stds[d].double()
+        sigma = ls.exp()
+        err = (actions[r0:r0 + 2048].double() - (y + sigma * z)).abs()
+        assert bool((err <= 2.0 ** -19 * sigma * (1 + z.abs()) + 2.0 ** -23 * y.abs()).all())
+        t = 0.5 * z * z + ls
+        ref = -t.sum(-1) - d * HALF_LOG_2PI
+        tol = 2.0 ** -20 * ((1 + z.abs()) ** 2).sum(-1) + (d + 8) * 2.0 ** -23 * (t.abs().sum(-1) + d * 0.92)
+        assert bool(((log_probs[r0:r0 + 2048].double() - ref).abs() <= tol).all())
+        parity[f"h_bias_gaussian_d{d}"] = {"gaussian_bars_2048_rows": "ok"}
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
