@@ -606,9 +606,37 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
   return KTB_OK;
 }
 
+// What a policy head computes; each entry point names its own.
+enum class HeadKind {
+  kGreedy,     // bf16 logits and/or int64 argmax actions
+  kSample,     // Gumbel-max int64 actions and fp32 log_probs
+  kGaussian,   // fp32 actions [rows, d_out] (gauss_actions) drawn with log_std, and fp32 log_probs
+};
+
+// The outputs of a head launch; a hidden layer's launch passes an empty one.  Pointers the head kind does not store
+// are null.  Row r of the launch draws the noise of global row row_base + r.
+struct HeadOut {
+  void* logits = nullptr;
+  int64_t* actions = nullptr;
+  float* log_probs = nullptr;
+  uint64_t seed = 0, row_base = 0;
+  const float* log_std = nullptr;
+  float* gauss_actions = nullptr;
+
+  // The same outputs from row r0 of the call on.
+  HeadOut from_row(size_t r0, int d_out) const {
+    HeadOut h = *this;
+    if (logits) h.logits = static_cast<__nv_bfloat16*>(logits) + r0 * d_out;
+    if (actions) h.actions += r0;
+    if (log_probs) h.log_probs += r0;
+    if (gauss_actions) h.gauss_actions += r0 * d_out;
+    h.row_base += r0;
+    return h;
+  }
+};
+
 template <int BLOCK_N>
-static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, int64_t* actions,
-                        float* log_probs, uint64_t seed, uint64_t row_base, const float* log_std, float* gauss_actions,
+static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, const HeadOut& head,
                         size_t M, int N, int K, int ldc, bool relu, cudaStream_t stream) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
@@ -623,73 +651,66 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
   kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias),
-                                                static_cast<__nv_bfloat16*>(C), actions, log_probs, seed, row_base,
-                                                log_std, gauss_actions, ldc, N, K, (int)M, relu);
+                                                static_cast<__nv_bfloat16*>(C), head.actions, head.log_probs,
+                                                head.seed, head.row_base, head.log_std, head.gauss_actions, ldc, N, K,
+                                                (int)M, relu);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
 
-// Weights, biases (each may be null) and outputs (either may be null) of one MLP call.  With log_probs the head
-// samples (actions required, logits null): row r of the call is global row row_base + r of the noise.  With log_std
-// as well it draws Gaussian actions into gauss_actions instead (actions and logits null).
+// Weights and biases (each bias may be null) of one MLP call, and its head.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
-  void* logits;
-  int64_t* actions;
-  float* log_probs = nullptr;
-  uint64_t seed = 0, row_base = 0;
-  const float* log_std = nullptr;
-  float* gauss_actions = nullptr;
+  HeadKind kind;
+  HeadOut out;
 };
 
-// One hidden layer H[rows, d_hidden] = relu(A · Wᵀ (+ b)).
-static int mlp_hidden(int dev, const void* A, const void* W, const void* b, void* H, size_t rows, int d_hidden, int K,
-                      cudaStream_t st) {
-  return launch_layer<256>(dev, A, W, b, H, nullptr, nullptr, 0, 0, nullptr, nullptr, rows, d_hidden, K, d_hidden,
-                           true, st);
+// Rows [r0, r0 + rows) of a call: the hidden layers h1 = relu(a1 · W1ᵀ (+ b1)) and h2 = relu(h1 · W2ᵀ (+ b2)), then
+// the head from h2 in the smallest tile that holds d_out.  `consumed`, unless null, is recorded once layer 1 has read
+// a1.
+static int mlp_chunk(int dev, const MlpParams& p, const void* a1, void* h1, void* h2, size_t r0, size_t rows, int d_in,
+                     int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
+  int rc = launch_layer<256>(dev, a1, p.W1, p.b1, h1, HeadOut{}, rows, d_hidden, d_in, d_hidden, true, st);
+  if (rc) return rc;
+  if (consumed) KTB_CK(cudaEventRecord(consumed, st));
+  rc = launch_layer<256>(dev, h1, p.W2, p.b2, h2, HeadOut{}, rows, d_hidden, d_hidden, d_hidden, true, st);
+  if (rc) return rc;
+  const HeadOut h = p.out.from_row(r0, d_out);
+  const auto head = d_out <= 64 ? launch_layer<64> : d_out <= 128 ? launch_layer<128> : launch_layer<256>;
+  return head(dev, h2, p.W3, p.b3, h.logits, h, rows, d_out, d_hidden, d_out, false, st);
 }
 
-// The head of rows [r0, r0 + rows): logits and/or actions (or sampled actions and log-probabilities) of those rows
-// from h2.
-static int mlp_head(int dev, const MlpParams& p, const void* h2, size_t r0, size_t rows, int d_hidden, int d_out,
-                    cudaStream_t st) {
-  void* y = p.logits ? static_cast<__nv_bfloat16*>(p.logits) + r0 * d_out : nullptr;
-  int64_t* act = p.actions ? p.actions + r0 : nullptr;
-  float* lp = p.log_probs ? p.log_probs + r0 : nullptr;
-  float* ga = p.gauss_actions ? p.gauss_actions + r0 * d_out : nullptr;
-  const uint64_t rb = p.row_base + r0;
-  if (d_out <= 64)
-    return launch_layer<64>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, p.log_std, ga, rows, d_out, d_hidden, d_out,
-                            false, st);
-  if (d_out <= 128)
-    return launch_layer<128>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, p.log_std, ga, rows, d_out, d_hidden, d_out,
-                             false, st);
-  return launch_layer<256>(dev, h2, p.W3, p.b3, y, act, lp, p.seed, rb, p.log_std, ga, rows, d_out, d_hidden, d_out,
-                           false, st);
-}
-
-// The checks every MLP entry shares: the layer widths the tiles divide, the head (outputs, width, element-aligned
-// pointers; skipped for an empty call, which stores nothing and may pass null outputs) and the 16-byte alignment TMA
-// needs of every matrix it loads (`obs` is the first layer's input).
+// The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
+// element-aligned pointers; skipped for an empty call, which stores nothing and may pass null outputs) and the
+// 16-byte alignment TMA needs of every matrix it loads (`obs` is the first layer's input).
 static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p, const void* obs,
                      const void* scratch, const void* stage) {
   KTB_REQUIRE(d_in > 0 && d_in % kMlpBlockK == 0, KTB_ERR_ARG, "%s: d_in=%d must be a multiple of 64", fn, d_in);
   KTB_REQUIRE(d_hidden > 0 && d_hidden % 256 == 0, KTB_ERR_ARG, "%s: d_hidden=%d must be a multiple of 256", fn,
               d_hidden);
   if (M > 0) {
-    KTB_REQUIRE(p.logits || p.actions || p.log_std, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
-    if (p.log_std) {
-      KTB_REQUIRE(p.gauss_actions && p.log_probs && !p.logits && !p.actions, KTB_ERR_ARG,
-                  "%s: the Gaussian head needs fp32 actions and log_probs, and stores nothing else", fn);
-      KTB_REQUIRE((((uintptr_t)p.log_std | (uintptr_t)p.gauss_actions) & 3) == 0, KTB_ERR_ARG,
-                  "%s: log_std and actions must be 4-byte aligned", fn);
+    const HeadOut& o = p.out;
+    switch (p.kind) {
+      case HeadKind::kGreedy:
+        KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
+        break;
+      case HeadKind::kSample:
+        KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
+        break;
+      case HeadKind::kGaussian:
+        KTB_REQUIRE(o.log_std && o.gauss_actions && o.log_probs, KTB_ERR_ARG,
+                    "%s: log_std, actions and log_probs are required", fn);
+        KTB_REQUIRE((((uintptr_t)o.log_std | (uintptr_t)o.gauss_actions) & 3) == 0, KTB_ERR_ARG,
+                    "%s: log_std and actions must be 4-byte aligned", fn);
+        break;
     }
     KTB_REQUIRE(d_out >= 1, KTB_ERR_ARG, "%s: d_out=%d must be positive", fn, d_out);
     KTB_REQUIRE(d_out <= 256, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (heads up to 256 wide)", fn, d_out);
-    KTB_REQUIRE((((uintptr_t)p.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
+    // outputs the kind does not store are null and pass
+    KTB_REQUIRE((((uintptr_t)o.logits | (uintptr_t)p.b1 | (uintptr_t)p.b2 | (uintptr_t)p.b3) & 1) == 0, KTB_ERR_ARG,
                 "%s: logits and biases must be 2-byte aligned", fn);
-    KTB_REQUIRE(((uintptr_t)p.actions & 7) == 0, KTB_ERR_ARG, "%s: actions must be 8-byte aligned", fn);
-    KTB_REQUIRE(((uintptr_t)p.log_probs & 3) == 0, KTB_ERR_ARG, "%s: log_probs must be 4-byte aligned", fn);
+    KTB_REQUIRE(((uintptr_t)o.actions & 7) == 0, KTB_ERR_ARG, "%s: actions must be 8-byte aligned", fn);
+    KTB_REQUIRE(((uintptr_t)o.log_probs & 3) == 0, KTB_ERR_ARG, "%s: log_probs must be 4-byte aligned", fn);
   }
   KTB_REQUIRE((((uintptr_t)obs | (uintptr_t)p.W1 | (uintptr_t)p.W2 | (uintptr_t)p.W3 | (uintptr_t)scratch |
                 (uintptr_t)stage) & 15) == 0,
@@ -774,12 +795,8 @@ static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in,
       KTB_CK(cudaStreamWaitEvent(st, evs[1 + b], 0));
       a1 = dstb;
     }
-    rc = mlp_hidden(dev, a1, p.W1, p.b1, h1, rows, d_hidden, d_in, st);
-    if (rc) return rc;
-    if (stg) KTB_CK(cudaEventRecord(evs[3 + (int)(c & 1)], st));
-    rc = mlp_hidden(dev, h1, p.W2, p.b2, h2, rows, d_hidden, d_hidden, st);
-    if (rc) return rc;
-    rc = mlp_head(dev, p, h2, r0, rows, d_hidden, d_out, st);
+    // evs[3..4] are null unless staged
+    rc = mlp_chunk(dev, p, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
     if (rc) return rc;
   }
   return KTB_OK;
@@ -836,12 +853,7 @@ static int mlp_pushed_run(const char* fn, int dev, const void* stage_local, size
     const size_t rows = std::min(chunk_rows, M - r0);
     mlp_wait_ready_kernel<<<1, 32, 0, st>>>(ready + c, seq, status);
     KTB_CK(cudaGetLastError());
-    const __nv_bfloat16* a1 = x + r0 * d_in;
-    rc = mlp_hidden(dev, a1, p.W1, p.b1, h1, rows, d_hidden, d_in, st);
-    if (rc) return rc;
-    rc = mlp_hidden(dev, h1, p.W2, p.b2, h2, rows, d_hidden, d_hidden, st);
-    if (rc) return rc;
-    rc = mlp_head(dev, p, h2, r0, rows, d_hidden, d_out, st);
+    rc = mlp_chunk(dev, p, x + r0 * d_in, h1, h2, r0, rows, d_in, d_hidden, d_out, nullptr, st);
     if (rc) return rc;
   }
   mlp_ack_kernel<<<1, 32, 0, st>>>(ack, seq);
@@ -860,7 +872,7 @@ int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, s
   if (rc) return rc;
   KTB_REQUIRE(logits || M == 0, KTB_ERR_ARG, "%s: null argument", fn);
   KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr};
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}};
   return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
                         ctrl_root_peer, rank, chunk_rows, seq, stream);
 }
@@ -870,7 +882,7 @@ int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_st
                                const void* W3, const void* b3, void* logits, int64_t* actions, void* scratch,
                                void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
                                unsigned long long seq, uintptr_t stream) {
-  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions};
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}};
   return mlp_pushed_run("ktb_mlp_bf16_policy_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p,
                         scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
 }
@@ -883,7 +895,7 @@ static int mlp_run_64(const char* fn, int dev, const void* obs, size_t M, int d_
   KTB_REQUIRE(logits, KTB_ERR_ARG, "%s: null argument", fn);
   KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
   KTB_REQUIRE(((uintptr_t)logits & 15) == 0, KTB_ERR_ARG, "%s: logits must be 16-byte aligned", fn);
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, logits, nullptr};
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}};
   return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
@@ -902,22 +914,16 @@ int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d
 int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                         const void* b1, const void* W2, const void* b2, const void* W3, const void* b3, void* logits,
                         int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
-  const MlpParams p{W1, b1, W2, b2, W3, b3, logits, actions};
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}};
   return mlp_run("ktb_mlp_bf16_policy", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
-// The sampling entries: the policy forms with (seed, row_base, actions, log_probs) as their outputs, both required
-// for a non-empty call; everything else is checked by the policy form they run.
 int ktb_mlp_bf16_policy_sample(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                                const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
                                uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs, void* scratch,
                                void* stage, uintptr_t stream) {
-  const char* fn = "ktb_mlp_bf16_policy_sample";
-  int rc = require_device(dev);
-  if (rc) return rc;
-  KTB_REQUIRE(M == 0 || (actions && log_probs), KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
-  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, actions, log_probs, seed, row_base};
-  return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}};
+  return mlp_run("ktb_mlp_bf16_policy_sample", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
 int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
@@ -926,28 +932,18 @@ int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t s
                                       int64_t* actions, float* log_probs, void* scratch, void* ctrl_local,
                                       void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
                                       uintptr_t stream) {
-  const char* fn = "ktb_mlp_bf16_policy_sample_pushed";
-  int rc = require_device(dev);
-  if (rc) return rc;
-  KTB_REQUIRE(M == 0 || (actions && log_probs), KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
-  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, actions, log_probs, seed, row_base};
-  return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
-                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}};
+  return mlp_pushed_run("ktb_mlp_bf16_policy_sample_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden, d_out,
+                        p, scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
 }
 
-// The Gaussian entries: the policy forms with (log_std, seed, row_base, fp32 actions, log_probs), all three pointers
-// required for a non-empty call; everything else is checked by the policy form they run.
 int ktb_mlp_bf16_policy_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                                  const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
                                  const float* log_std, uint64_t seed, uint64_t row_base, float* actions,
                                  float* log_probs, void* scratch, void* stage, uintptr_t stream) {
-  const char* fn = "ktb_mlp_bf16_policy_gaussian";
-  int rc = require_device(dev);
-  if (rc) return rc;
-  KTB_REQUIRE(M == 0 || (log_std && actions && log_probs), KTB_ERR_ARG,
-              "%s: log_std, actions and log_probs are required", fn);
-  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, nullptr, log_probs, seed, row_base, log_std, actions};
-  return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian,
+                    {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}};
+  return mlp_run("ktb_mlp_bf16_policy_gaussian", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
 }
 
 int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
@@ -956,14 +952,10 @@ int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t
                                         uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
                                         void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
                                         size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
-  const char* fn = "ktb_mlp_bf16_policy_gaussian_pushed";
-  int rc = require_device(dev);
-  if (rc) return rc;
-  KTB_REQUIRE(M == 0 || (log_std && actions && log_probs), KTB_ERR_ARG,
-              "%s: log_std, actions and log_probs are required", fn);
-  const MlpParams p{W1, b1, W2, b2, W3, b3, nullptr, nullptr, log_probs, seed, row_base, log_std, actions};
-  return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
-                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian,
+                    {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}};
+  return mlp_pushed_run("ktb_mlp_bf16_policy_gaussian_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden,
+                        d_out, p, scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
 }
 
 }  // extern "C"

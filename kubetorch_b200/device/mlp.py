@@ -11,6 +11,7 @@ import torch
 
 from . import lib as L
 from . import ops
+from ..mapped import MLP_OUTPUTS as OUTPUTS
 from ..sampling import _check_seed
 
 _scratch = {}
@@ -51,7 +52,6 @@ def _thread_pool():
     return _pool
 
 
-OUTPUTS = ("logits", "actions", "both", "sample", "gaussian")
 MAX_D_OUT = 256
 
 
@@ -80,6 +80,50 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None) -> None:
         if not isinstance(b, torch.Tensor) or b.dtype != torch.bfloat16 or not b.is_cuda or not b.is_contiguous() \
                 or b.dim() != 1 or b.shape[0] != n:
             raise ValueError(f"{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
+
+
+def _outputs(output, M, d_out, device, logits, actions, log_probs):
+    """(logits, actions, log_probs) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions [M], or
+    fp32 [M, d_out] with "gaussian"; fp32 log_probs [M].  A buffer the mode does not write is None, a missing one is
+    allocated on `device` and a given one is registered with the library (ops.ensure_init)."""
+    def buf(t, shape, dtype):
+        if t is None:
+            return torch.empty(shape, dtype=dtype, device=device)
+        ops.ensure_init({t.device.index})
+        return t
+
+    gaussian = output == "gaussian"
+    return (buf(logits, (M, d_out), torch.bfloat16) if output in ("logits", "both") else None,
+            None if output == "logits" else
+            buf(actions, (M, d_out), torch.float32) if gaussian else buf(actions, (M,), torch.int64),
+            buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian") else None)
+
+
+def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False):
+    """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
+    pointers as ptr(tensor) gives them."""
+    suffix = "_pushed" if pushed else ""
+    if output == "gaussian":
+        return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs))
+    if output == "sample":
+        return "ktb_mlp_bf16_policy_sample" + suffix, (seed, row_base, ptr(actions), ptr(log_probs))
+    return "ktb_mlp_bf16_policy" + suffix, (ptr(logits), ptr(actions))
+
+
+def _rows(bufs, b, e):
+    """Rows b .. e - 1 of each buffer; None stays None."""
+    return [None if t is None else t[b:e] for t in bufs]
+
+
+def _result(output, logits, actions, log_probs):
+    """What a call with `output` returns, from its buffers."""
+    if output == "logits":
+        return logits
+    if output == "actions":
+        return actions
+    if output == "both":
+        return logits, actions
+    return actions, log_probs
 
 
 def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor,
@@ -111,50 +155,16 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     if output in ("sample", "gaussian") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
-    want_logits, want_actions = output in ("logits", "both"), output not in ("logits", "gaussian")
-    if want_logits:
-        if out is None:
-            out = torch.empty(M, d_out, dtype=torch.bfloat16, device=f"cuda:{dev}")
-        else:
-            ops.ensure_init({out.device.index})
-    if want_actions:
-        if actions is None:
-            actions = torch.empty(M, dtype=torch.int64, device=f"cuda:{dev}")
-        else:
-            ops.ensure_init({actions.device.index})
+    out, actions, log_probs = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
-    if output == "gaussian":
-        if actions is None:
-            actions = torch.empty(M, d_out, dtype=torch.float32, device=f"cuda:{dev}")
-        else:
-            ops.ensure_init({actions.device.index})
-        if log_probs is None:
-            log_probs = torch.empty(M, dtype=torch.float32, device=f"cuda:{dev}")
-        else:
-            ops.ensure_init({log_probs.device.index})
-        L.call("ktb_mlp_bf16_policy_gaussian", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(),
-               ptr(biases[0]), w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), log_std.data_ptr(), seed,
-               row_offset, ptr(actions), ptr(log_probs), _scratch_for(dev, M, d_hidden).data_ptr(),
-               _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
-        return actions, log_probs
-    if output == "sample":
-        if log_probs is None:
-            log_probs = torch.empty(M, dtype=torch.float32, device=f"cuda:{dev}")
-        else:
-            ops.ensure_init({log_probs.device.index})
-        L.call("ktb_mlp_bf16_policy_sample", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(),
-               ptr(biases[0]), w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), seed, row_offset,
-               ptr(actions), ptr(log_probs), _scratch_for(dev, M, d_hidden).data_ptr(),
-               _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
-        return actions, log_probs
-    L.call("ktb_mlp_bf16_policy", dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]),
-           w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), ptr(out) if want_logits else 0,
-           ptr(actions) if want_actions else 0, _scratch_for(dev, M, d_hidden).data_ptr(),
+    entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr)
+    L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
+           ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
-    return (out, actions) if output == "both" else actions if output == "actions" else out
+    return _result(output, out, actions, log_probs)
 
 
 def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
@@ -207,14 +217,14 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS)
     scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], scratch_bytes) for r in range(1, n)]
     streams = [ops.current_stream_handle(d) for d in devs]
+    bufs = (out_root, actions_root, log_probs_root)
     b0, e0 = bounds[0]
     own = e0 > b0
     if own:
         ws = weights[root]
-        mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b0:e0],
-                    device=root, stream=sess.fork(), staged=False, biases=ws[3:], output=output,
-                    actions=None if actions_root is None else actions_root[b0:e0], seed=seed, row_offset=b0,
-                    log_probs=None if log_probs_root is None else log_probs_root[b0:e0],
+        logits, actions, log_probs = _rows(bufs, b0, e0)
+        mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=logits, device=root, stream=sess.fork(), staged=False,
+                    biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
                     log_std=None if log_std is None else log_std[root])
     L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
            L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
@@ -224,23 +234,10 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         b, e = bounds[r]
         ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
-        if output == "gaussian":
-            L.call("ktb_mlp_bf16_policy_gaussian_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in,
-                   d_hidden, d_out, ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(),
-                   ptr(ws[5]), ptr(log_std[devs[r]]), seed, b, ptr(actions_root[b:e]), ptr(log_probs_root[b:e]),
-                   scratch[r].data_ptr(), sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq,
-                   streams[r])
-            return
-        if output == "sample":
-            L.call("ktb_mlp_bf16_policy_sample_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in,
-                   d_hidden, d_out, ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(),
-                   ptr(ws[5]), seed, b, ptr(actions_root[b:e]), ptr(log_probs_root[b:e]), scratch[r].data_ptr(),
-                   sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
-            return
-        L.call("ktb_mlp_bf16_policy_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden,
-               d_out, ws[0].data_ptr(), ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]),
-               ptr(None if out_root is None else out_root[b:e]),
-               ptr(None if actions_root is None else actions_root[b:e]), scratch[r].data_ptr(),
+        entry, head = _head(output, *_rows(bufs, b, e), seed, b, None if log_std is None else log_std[devs[r]], ptr,
+                            pushed=True)
+        L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
+               ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
 
     list(_thread_pool().map(issue, range(1, n)))
@@ -266,33 +263,12 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     _check_policy(w1, w3, biases, output, seed, log_std)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
-    d_out = w3.shape[0]
-    if output in ("logits", "both"):
-        if out_root is None:
-            out_root = torch.empty(M, d_out, dtype=torch.bfloat16, device=obs_root.device)
-    else:
-        out_root = None
-    if output == "logits":
-        actions_root = None
-    elif actions_root is None:
-        shape, dtype = ((M, d_out), torch.float32) if output == "gaussian" else ((M,), torch.int64)
-        actions_root = torch.empty(shape, dtype=dtype, device=obs_root.device)
-    if output not in ("sample", "gaussian"):
-        log_probs_root = None
-    elif log_probs_root is None:
-        log_probs_root = torch.empty(M, dtype=torch.float32, device=obs_root.device)
+    bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root)
     root_stream = torch.cuda.current_stream(root)
     ready = torch.cuda.Event()
     ready.record(root_stream)
     bounds = [ops.shard_bounds(M, len(devs), r) for r in range(len(devs))]
-    if output == "logits":
-        views = [out_root[b:e] for b, e in bounds]
-    elif output == "actions":
-        views = [actions_root[b:e] for b, e in bounds]
-    elif output in ("sample", "gaussian"):
-        views = [(actions_root[b:e], log_probs_root[b:e]) for b, e in bounds]
-    else:
-        views = [(out_root[b:e], actions_root[b:e]) for b, e in bounds]
+    views = [_result(output, *_rows(bufs, b, e)) for b, e in bounds]
     weights = {dev: _weights_on(dev, (w1, w2, w3)) + _weights_on(dev, biases) for dev in set(devs)}
     log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
     distinct = len(set(devs)) == len(devs) and len(devs) > 1
@@ -303,8 +279,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root,
-                                   seed, log_stds)
+        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs, seed, log_stds)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -323,10 +298,9 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         with torch.cuda.device(dev):
             if dev != root:
                 st.wait_event(ready)
-            mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=None if out_root is None else out_root[b:e],
-                        device=dev, stream=st, biases=ws[3:], output=output,
-                        actions=None if actions_root is None else actions_root[b:e], seed=seed, row_offset=b,
-                        log_probs=None if log_probs_root is None else log_probs_root[b:e],
+            logits, actions, log_probs = _rows(bufs, b, e)
+            mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=st, biases=ws[3:],
+                        output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
                         log_std=None if log_stds is None else log_stds[dev])
             if dev != root:
                 ev = torch.cuda.Event()

@@ -23,7 +23,7 @@ from typing import Any, Callable, Dict, Optional
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
-MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian")
+MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian")   # also device.mlp.OUTPUTS
 
 
 @dataclass
