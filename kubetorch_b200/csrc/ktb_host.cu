@@ -227,22 +227,6 @@ static int run_host_pipeline(int dev, int op, int dtype, const uint8_t* src_host
   return status;
 }
 
-// Zero-copy variant: ONE kernel per device reads the pinned host shard over PCIe and writes the result straight
-// back into pinned host memory (no staging, no copy engines, one launch).  Selected by ktb_set_tuning(20, 1).
-std::atomic<int> g_host_zero_copy{0};
-
-static int run_host_zero_copy(int dev, int op, int dtype, const uint8_t* src_host, uint8_t* dst_host, size_t n_bytes,
-                              const MapParams& p) {
-  if (n_bytes == 0) return KTB_OK;
-  KTB_GUARD(dev);
-  DeviceInfo* di = device_info(dev);
-  int rc = launch_map(dev, op, dtype, src_host, dst_host, n_bytes / dtype_size(dtype), p, KTB_VARIANT_AUTO,
-                      di->stream_exec);
-  if (rc) return rc;
-  KTB_CK(cudaStreamSynchronize(di->stream_exec));
-  return KTB_OK;
-}
-
 static std::mutex g_host_call_mu;   // the per-device copy/exec streams and events carry one call at a time
 
 struct HostBlockInfo {
@@ -386,7 +370,6 @@ int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, 
   }
   std::lock_guard<std::mutex> lk(g_host_call_mu);
   const MapParams p = make_params(alpha, beta, dtype);
-  const bool zero_copy = g_host_zero_copy.load() != 0;
   const uint8_t* src = static_cast<const uint8_t*>(src_host);
   uint8_t* dst = static_cast<uint8_t*>(dst_host);
   HostWorker* posted[kMaxDevices] = {nullptr};
@@ -408,17 +391,15 @@ int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, 
     void* sout = stage_out[r];
     HostWorker* w = worker_for(dev);
     worker_post(w, [=]() {
-      return zero_copy ? run_host_zero_copy(dev, op, dtype, src + off, dst + off, len, p)
-                       : run_host_pipeline(dev, op, dtype, src + off, dst + off, len, p, chunk_bytes, sin, sout);
+      return run_host_pipeline(dev, op, dtype, src + off, dst + off, len, p, chunk_bytes, sin, sout);
     });
     posted[r] = w;
   }
   int status = KTB_OK;
   char first_err[512] = "";
   if (first >= 0) {
-    status = zero_copy ? run_host_zero_copy(devs[first], op, dtype, src + first_off, dst + first_off, first_len, p)
-                       : run_host_pipeline(devs[first], op, dtype, src + first_off, dst + first_off, first_len, p,
-                                           chunk_bytes, stage_in[first], stage_out[first]);
+    status = run_host_pipeline(devs[first], op, dtype, src + first_off, dst + first_off, first_len, p, chunk_bytes,
+                               stage_in[first], stage_out[first]);
     if (status != KTB_OK) snprintf(first_err, sizeof(first_err), "%s", last_error_cstr());
   }
   for (int r = 0; r < n_ranks; ++r) {

@@ -8,78 +8,38 @@
 // HBM-bound: algorithmic bytes = n*(sizeof in + sizeof out); no data reuse, so the only
 // levers are coalesced wide accesses, enough bytes in flight, and a grid that is a multiple
 // of the SM count.  Three bit-identical variants:
-//   VEC    — 128-bit LDG/STG, UNROLL loads in flight per thread, persistent grid
+//   VEC    — 128-bit LDG/STG, 4 loads in flight per thread, one tile per CTA
 //   TMA    — cp.async.bulk global→shared ring (mbarrier complete_tx), compute in shared,
 //            cp.async.bulk shared→global; one elected thread drives the TMA engine
 //   SCALAR — any alignment
 #include "ktb_common.cuh"
 
 #include <algorithm>
-#include <atomic>
 
 namespace ktb {
 
+// test hooks of ktb_set_tuning, each defined beside the code it steers
 extern int g_red_ctas_per_sm;  // ktb_reduce.cu
 extern int g_red_loads;        // ktb_reduce.cu
-extern int g_red_fold;         // ktb_reduce.cu
 extern int g_seg_large;        // ktb_pack.cu
 extern int g_mlp_chunk_rows;   // ktb_mlp.cu
-}  // namespace ktb
-extern int g_mlp_stage_ce;     // ktb_mlp.cu (file scope there)
-namespace ktb {
-extern std::atomic<int> g_host_zero_copy;   // ktb_host.cu
-}  // namespace ktb
-extern std::atomic<int> g_push_scatter_ctas_per_sm;   // ktb_push.cu (file scope there)
-extern std::atomic<int> g_push_slice;
-namespace ktb {
-
-// ---- tunables (ktb_set_tuning) ---------------------------------------------------------------
-static std::atomic<int> g_vec_ctas_per_sm{0};  // 0 = one tile per CTA
-static std::atomic<int> g_tma_ctas_per_sm{1};
-static std::atomic<int> g_tma_cfg{0};       // 0: 4 x 32 KiB stages, 1: 6 x 32 KiB, 2: 8 x 16 KiB (2 CTA/SM)
-static std::atomic<int> g_auto_variant{KTB_VARIANT_VEC};
-static std::atomic<int> g_vec_flavor{2};    // cache flavor (tunable for F32-scale and identity only)
-static std::atomic<int> g_vec_unroll{4};    // 2 | 4 | 8 (tunable for the same kernels)
+extern int g_mlp_stage_ce;     // ktb_mlp.cu
 
 constexpr int kVecThreads = 256;
-constexpr int kVecUnroll = 4;   // defaults: 4 x 128-bit loads in flight per thread,
-constexpr int kVecFlavor = 2;   // L2::evict_first streaming hints, one 16 KiB tile per CTA
+constexpr int kVecBytes = 16;   // 128 bits: sm_90 has no wider per-thread global access
+constexpr int kVecUnroll = 4;   // 4 x 128-bit loads in flight per thread = one 16 KiB tile per CTA
+
+constexpr int kTmaStages = 4;         // 4 x 32 KiB ring per CTA, one CTA per SM
+constexpr int kTmaStageBytes = 32768;
+constexpr int kTmaThreads = 256;
 
 // ---- VEC -----------------------------------------------------------------------------------------
-// 128-bit accesses, the widest a Hopper thread can issue.  FL (cache flavor): 0 = L1::no_allocate,
-// 1 = default caching, 2 = L1::no_allocate + L2::evict_first on loads and stores, 3 = evict_first loads only.
-template <int VB, int FL>
-__device__ __forceinline__ void ld_vec(const uint8_t* p, uint32_t (&w)[VB / 4]) {
-  static_assert(VB == 16, "sm_90 has no wider per-thread global access than 128 bits");
-  if constexpr (FL == 1) {
-    asm volatile("ld.global.v4.b32 {%0,%1,%2,%3}, [%4];"
-                 : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3])
-                 : "l"(p)
-                 : "memory");
-  } else if constexpr (FL == 2 || FL == 3) {
-    ldg128_stream(p, w);
-  } else {
-    ldg128(p, w);
-  }
-}
-template <int VB, int FL>
-__device__ __forceinline__ void st_vec(uint8_t* p, const uint32_t (&w)[VB / 4]) {
-  static_assert(VB == 16, "sm_90 has no wider per-thread global access than 128 bits");
-  if constexpr (FL == 1) {
-    asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3])
-                 : "memory");
-  } else if constexpr (FL == 2) {
-    stg128_stream(p, w);
-  } else {
-    stg128(p, w);
-  }
-}
-
-template <int DT, int OP, int VB, int FL = kVecFlavor, int UNROLL = kVecUnroll>
+// L1::no_allocate + L2::evict_first loads and stores (the data is touched once).
+template <int DT, int OP>
 __global__ void __launch_bounds__(kVecThreads)
     map_vec_kernel(const uint8_t* src, uint8_t* dst, size_t n_bytes, MapParams p) {
+  constexpr int VB = kVecBytes;
   constexpr int NW = VB / 4;
-  constexpr int kVecUnroll = UNROLL;
   constexpr size_t TILE = (size_t)kVecThreads * kVecUnroll * VB;  // bytes per CTA iteration
   constexpr size_t ROW = (size_t)kVecThreads * VB;                // bytes per unrolled step
   const size_t n_full = n_bytes / TILE;
@@ -88,11 +48,11 @@ __global__ void __launch_bounds__(kVecThreads)
     const size_t off = t * TILE + (size_t)threadIdx.x * VB;
     uint32_t w[kVecUnroll][NW];
 #pragma unroll
-    for (int j = 0; j < kVecUnroll; ++j) ld_vec<VB, FL>(src + off + j * ROW, w[j]);
+    for (int j = 0; j < kVecUnroll; ++j) ldg128_stream(src + off + j * ROW, w[j]);
 #pragma unroll
     for (int j = 0; j < kVecUnroll; ++j) {
       apply_words<DT, OP, NW>(w[j], p);
-      st_vec<VB, FL>(dst + off + j * ROW, w[j]);
+      stg128_stream(dst + off + j * ROW, w[j]);
     }
   }
 
@@ -102,9 +62,9 @@ __global__ void __launch_bounds__(kVecThreads)
     const size_t n_vec = (n_bytes - base) / VB;
     for (size_t v = threadIdx.x; v < n_vec; v += kVecThreads) {
       uint32_t w[NW];
-      ld_vec<VB, FL>(src + base + v * VB, w);
+      ldg128_stream(src + base + v * VB, w);
       apply_words<DT, OP, NW>(w, p);
-      st_vec<VB, FL>(dst + base + v * VB, w);
+      stg128_stream(dst + base + v * VB, w);
     }
     constexpr size_t ES = (DT == KTB_U8) ? 1 : ((DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4));
     const size_t tail = base + n_vec * VB;
@@ -131,9 +91,10 @@ __global__ void __launch_bounds__(256)
 // proxy, and thread 0 issues the bulk store.  A stage is re-armed once the bulk store that
 // read it has finished reading (cp.async.bulk.wait_group.read), one iteration later, so
 // STAGES-1 loads stay in flight per CTA.
-template <int DT, int OP, int STAGES, int STAGE_BYTES, int NT>
-__global__ void __launch_bounds__(NT)
+template <int DT, int OP>
+__global__ void __launch_bounds__(kTmaThreads)
     map_tma_kernel(const uint8_t* src, uint8_t* dst, size_t n_bytes, MapParams p) {
+  constexpr int STAGES = kTmaStages, STAGE_BYTES = kTmaStageBytes, NT = kTmaThreads;
   extern __shared__ __align__(128) uint8_t smem[];
   uint8_t* buf = smem;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE_BYTES);
@@ -218,62 +179,23 @@ static int launch_typed(int dev, const uint8_t* src, uint8_t* dst, size_t n_elem
   const size_t n_bytes = n_elems * es;
   const uintptr_t both = (uintptr_t)src | (uintptr_t)dst;
 
-  if (variant == KTB_VARIANT_AUTO) variant = g_auto_variant.load();
+  if (variant == KTB_VARIANT_AUTO) variant = KTB_VARIANT_VEC;
   // bulk (TMA) and vector paths need 16-byte aligned pointers; ragged shard boundaries fall back
   if (variant == KTB_VARIANT_TMA && (both & 15)) variant = KTB_VARIANT_VEC;
   if (variant == KTB_VARIANT_VEC && (both & 15)) variant = KTB_VARIANT_SCALAR;
 
   if (variant == KTB_VARIANT_VEC) {
-    // ctas_per_sm == 0 → one tile per CTA (the hardware scheduler balances the tail);
-    // otherwise a persistent grid of sm_count * ctas_per_sm CTAs striding over tiles.
-    const int per_sm = g_vec_ctas_per_sm.load();
-    auto grid_for = [&](size_t tile_bytes) {
-      size_t tiles = std::max<size_t>(n_bytes / tile_bytes, 1);
-      if (per_sm <= 0) return (int)std::min<size_t>(tiles, 0x7fffffffULL);
-      return (int)std::min<size_t>(tiles, (size_t)di->sm_count * per_sm);
-    };
-    constexpr bool kTunable = (DT == KTB_U8) || (DT == KTB_F32 && OP == KTB_OP_SCALE);
-    const int fl = kTunable ? g_vec_flavor.load() : kVecFlavor;
-    const int un = kTunable ? g_vec_unroll.load() : kVecUnroll;
-#define KTB_VEC16(FL, UN)                                                                          \
-  map_vec_kernel<DT, OP, 16, FL, UN>                                                               \
-      <<<grid_for((size_t)kVecThreads * (UN)*16), kVecThreads, 0, stream>>>(src, dst, n_bytes, p)
-    if constexpr (kTunable) {
-      if (un == 2) {
-        if (fl == 1) KTB_VEC16(1, 2); else if (fl == 2) KTB_VEC16(2, 2); else if (fl == 3) KTB_VEC16(3, 2); else KTB_VEC16(0, 2);
-      } else if (un == 8) {
-        if (fl == 1) KTB_VEC16(1, 8); else if (fl == 2) KTB_VEC16(2, 8); else if (fl == 3) KTB_VEC16(3, 8); else KTB_VEC16(0, 8);
-      } else {
-        if (fl == 1) KTB_VEC16(1, 4); else if (fl == 2) KTB_VEC16(2, 4); else if (fl == 3) KTB_VEC16(3, 4); else KTB_VEC16(0, 4);
-      }
-    } else {
-      (void)fl; (void)un;
-      KTB_VEC16(kVecFlavor, kVecUnroll);
-    }
-#undef KTB_VEC16
+    // one tile per CTA: the hardware scheduler balances the tail
+    const size_t tiles = std::max<size_t>(n_bytes / ((size_t)kVecThreads * kVecUnroll * kVecBytes), 1);
+    const int grid = (int)std::min<size_t>(tiles, 0x7fffffffULL);
+    map_vec_kernel<DT, OP><<<grid, kVecThreads, 0, stream>>>(src, dst, n_bytes, p);
   } else if (variant == KTB_VARIANT_TMA) {
-    const int cfg = g_tma_cfg.load();
-    const int per_sm = std::max(1, g_tma_ctas_per_sm.load());
-#define KTB_LAUNCH_TMA(ST, SB, NT)                                                              \
-  do {                                                                                          \
-    constexpr size_t smem_bytes = (size_t)(ST) * (SB) + (ST) * sizeof(uint64_t);                \
-    auto kfn = map_tma_kernel<DT, OP, ST, SB, NT>;                                              \
-    KTB_CK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize,               \
-                                (int)smem_bytes));                                              \
-    size_t tiles = ((n_bytes & ~(size_t)15) + (SB)-1) / (SB);                                   \
-    int grid = (int)std::min<size_t>(std::max<size_t>(tiles, 1), (size_t)di->sm_count * per_sm); \
-    kfn<<<grid, NT, smem_bytes, stream>>>(src, dst, n_bytes, p);                                \
-  } while (0)
-    if (cfg == 1) {
-      KTB_LAUNCH_TMA(6, 32768, 256);
-    } else if (cfg == 2) {
-      KTB_LAUNCH_TMA(6, 16384, 256);
-    } else if (cfg == 3) {
-      KTB_LAUNCH_TMA(3, 65536, 512);
-    } else {
-      KTB_LAUNCH_TMA(4, 32768, 256);
-    }
-#undef KTB_LAUNCH_TMA
+    constexpr size_t smem_bytes = (size_t)kTmaStages * kTmaStageBytes + kTmaStages * sizeof(uint64_t);
+    auto kfn = map_tma_kernel<DT, OP>;
+    KTB_CK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    const size_t tiles = ((n_bytes & ~(size_t)15) + kTmaStageBytes - 1) / kTmaStageBytes;
+    const int grid = (int)std::min<size_t>(std::max<size_t>(tiles, 1), (size_t)di->sm_count);
+    kfn<<<grid, kTmaThreads, smem_bytes, stream>>>(src, dst, n_bytes, p);
   } else if (variant == KTB_VARIANT_SCALAR) {
     size_t blocks = (n_elems + 255) / 256;
     int grid = (int)std::min<size_t>(std::max<size_t>(blocks, 1), (size_t)di->sm_count * 8);
@@ -333,32 +255,22 @@ using namespace ktb;
 
 extern "C" {
 
-// Experiment knobs (not part of the stable ABI; used by the bench sweep).
-//   key 0: VEC CTAs per SM (0 = one tile per CTA)   key 1: TMA CTAs per SM   key 2: TMA stage config
-//   key 3: AUTO variant   key 4: VEC cache flavor   key 5: VEC unroll
+// Test hooks (not part of the stable ABI, not in ktb200.h): each key steers a launch geometry or path
+// that the tests compare against the shipped default.
+//   key 6:  map_reduce_sum grid cap in units of 1024 CTAs (<= 0: the default, 4)
+//   key 8:  MLP rows per chunk (a positive multiple of 128)
+//   key 12: 0 = segment maps use only the 96 descriptors of the classic parameter space
+//   key 13: map_reduce_sum 256-bit loads per thread and tile (4, otherwise 8)
+//   key 22: 1 = staged MLP pulls by copy engine instead of a pull kernel
 int ktb_set_tuning(int key, int value) {
   switch (key) {
-    case 0: g_vec_ctas_per_sm = value; return KTB_OK;
-    case 1: g_tma_ctas_per_sm = value; return KTB_OK;
-    case 2: g_tma_cfg = value; return KTB_OK;
-    case 4: g_vec_flavor = value; return KTB_OK;
-    case 5: g_vec_unroll = value; return KTB_OK;
     case 6: g_red_ctas_per_sm = value > 0 ? value : 4; return KTB_OK;
     case 12: g_seg_large = value ? 1 : 0; return KTB_OK;
     case 13: g_red_loads = value == 4 ? 4 : 8; return KTB_OK;
-    case 14: g_red_fold = value ? 1 : 0; return KTB_OK;
-    case 20: g_host_zero_copy = value ? 1 : 0; return KTB_OK;
-    case 23: g_push_slice = value > 0 ? value : 1; return KTB_OK;
     case 22: g_mlp_stage_ce = value ? 1 : 0; return KTB_OK;
-    case 21: g_push_scatter_ctas_per_sm = value > 0 ? value : 0; return KTB_OK;
     case 8:
       KTB_REQUIRE(value > 0 && value % 128 == 0, KTB_ERR_ARG, "ktb_set_tuning: MLP chunk rows must be a multiple of 128");
       g_mlp_chunk_rows = value;
-      return KTB_OK;
-    case 3:
-      KTB_REQUIRE(value >= KTB_VARIANT_VEC && value <= KTB_VARIANT_SCALAR, KTB_ERR_ARG,
-                  "ktb_set_tuning: bad auto variant %d", value);
-      g_auto_variant = value;
       return KTB_OK;
     default: set_error("ktb_set_tuning: unknown key %d", key); return KTB_ERR_ARG;
   }

@@ -37,6 +37,7 @@ constexpr int kMlpThreads = kMlpConsumers + 32;
 int g_mlp_chunk_rows = 16896;  // ktb_set_tuning key 8: rows per chunk = 132 SMs x 128 rows, so each 256-wide layer of a
                                // chunk is four whole waves of 128 x 256 tiles, and one chunk's hidden activation
                                // (34.6 MB at d_hidden = 1024) stays in the 50 MB L2 between the layers
+int g_mlp_stage_ce = 0;        // ktb_set_tuning key 22: staged pulls by a pull kernel (0, default) or by copy engine (1)
 
 // ---- PTX wrappers -----------------------------------------------------------------------------------
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
@@ -732,9 +733,6 @@ size_t ktb_mlp_stage_bytes(size_t M, int d_in) {
   const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
   return 2 * rows * (size_t)d_in * 2;
 }
-
-// ktb_set_tuning(22, v): staged pulls by a pull kernel (0, default) or by copy engine (1)
-int g_mlp_stage_ce = 0;
 
 static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
                    const MlpParams& p, void* scratch, void* stage, uintptr_t stream) {

@@ -17,7 +17,6 @@ constexpr int kRedThreads = 256;
 constexpr int kRedMaxGrid = 4096;  // per-CTA partials: the last CTA folds them in ONE round of 8 x 16-byte loads per thread
 constexpr size_t kRedHeader = 64;  // counter lives in the first 64 bytes of the workspace
 int g_red_ctas_per_sm = 4;         // ktb_set_tuning key 6: grid cap in units of 1024 CTAs (<= kRedMaxGrid)
-int g_red_fold = 1;                // ktb_set_tuning key 14: 0 = skip the cross-CTA fold (measurement only; result invalid)
 int g_red_loads = 8;               // ktb_set_tuning key 13: 256-bit loads in flight per thread (8 = 64 KiB tile per CTA, default; 4 = 32 KiB)
 
 template <int DT>
@@ -113,7 +112,7 @@ __device__ __forceinline__ T block_sum(T v, T* smem /* >= 32 entries */) {
 
 template <int DT, int OP, int LOADS>
 __global__ void __launch_bounds__(kRedThreads)
-    map_reduce_kernel(const uint8_t* src, size_t n_elems, MapParams mp, void* out, uint8_t* ws, int fold) {
+    map_reduce_kernel(const uint8_t* src, size_t n_elems, MapParams mp, void* out, uint8_t* ws) {
   using A = typename Acc<DT>::type;
   // cross-CTA partials are kept in fp64 for float sums, int64 for integer sums
   using P = typename std::conditional<std::is_same<A, float>::value, double, long long>::type;
@@ -160,10 +159,6 @@ __global__ void __launch_bounds__(kRedThreads)
 
   unsigned int* counter = reinterpret_cast<unsigned int*>(ws);
   P* partials = reinterpret_cast<P*>(ws + kRedHeader);
-  if (!fold) {  // measurement aid (ktb_set_tuning key 14): stream + per-CTA partial only
-    if (threadIdx.x == 0) partials[blockIdx.x] = part;
-    return;
-  }
   if (threadIdx.x == 0) {
     partials[blockIdx.x] = part;
     // one acq_rel RMW instead of fence + atomic + fence: releases this CTA's partial, and for the CTA that draws
@@ -225,9 +220,9 @@ static int launch_reduce_typed(int dev, const uint8_t* src, size_t n_elems, cons
   const size_t cap = g_red_ctas_per_sm > 0 ? std::min<size_t>((size_t)kRedMaxGrid, (size_t)g_red_ctas_per_sm * 1024) : kRedMaxGrid;
   int grid = (int)std::min<size_t>(std::max<size_t>(tiles, 1), cap);
   if (loads == 8)
-    map_reduce_kernel<DT, OP, 8><<<grid, kRedThreads, 0, stream>>>(src, n_elems, p, out, (uint8_t*)ws, g_red_fold);
+    map_reduce_kernel<DT, OP, 8><<<grid, kRedThreads, 0, stream>>>(src, n_elems, p, out, (uint8_t*)ws);
   else
-    map_reduce_kernel<DT, OP, 4><<<grid, kRedThreads, 0, stream>>>(src, n_elems, p, out, (uint8_t*)ws, g_red_fold);
+    map_reduce_kernel<DT, OP, 4><<<grid, kRedThreads, 0, stream>>>(src, n_elems, p, out, (uint8_t*)ws);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }

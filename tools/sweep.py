@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Kernel-level sweep on one H100: GB/s of each map variant / tuning, pack, reduce, host paths, and
+"""Kernel-level sweep on one H100: GB/s of each map variant, pack, reduce, host paths, and
 calls/s for small payloads.  Writes JSON lines to gpurun_out/sweep.jsonl (copy summaries to profiles/)."""
 import json
 import os
@@ -51,29 +51,9 @@ def main():
     emit(what="torch_mul_256MiB", ms=ms, gbps=2 * nbytes / ms / 1e6)
 
     for op in ("scale", "identity"):
-        for un in (2, 4, 8):
-            for fl in (0, 1, 2, 3):
-                for cps in (0, 4, 6, 8, 12, 16, 32):
-                    ops.set_tuning(0, cps)
-                    ops.set_tuning(4, fl)
-                    ops.set_tuning(5, un)
-                    ms = timeit(lambda: ops.map_tensor(x, op, 2.0, out=y, variant=L.VARIANT_VEC))
-                    emit(what="map_vec", op=op, unroll=un, flavor=fl, ctas_per_sm=cps, ms=ms,
-                         gbps=2 * nbytes / ms / 1e6)
-        ops.set_tuning(0, 0)   # back to the defaults: one tile per CTA, evict_first, unroll 2
-        ops.set_tuning(4, 2)
-        ops.set_tuning(5, 2)
-        for cfg, per_sm_opts in ((0, (1,)), (1, (1,)), (2, (1, 2)), (3, (1,))):
-            for per_sm in per_sm_opts:
-                ops.set_tuning(2, cfg)
-                ops.set_tuning(1, per_sm)
-                try:
-                    ms = timeit(lambda: ops.map_tensor(x, op, 2.0, out=y, variant=L.VARIANT_TMA))
-                    emit(what="map_tma", op=op, cfg=cfg, ctas_per_sm=per_sm, ms=ms, gbps=2 * nbytes / ms / 1e6)
-                except Exception as e:  # noqa: BLE001
-                    emit(what="map_tma", op=op, cfg=cfg, ctas_per_sm=per_sm, error=str(e)[:200])
-    ops.set_tuning(2, 0)
-    ops.set_tuning(1, 1)
+        for variant, name in ((L.VARIANT_VEC, "map_vec"), (L.VARIANT_TMA, "map_tma")):
+            ms = timeit(lambda: ops.map_tensor(x, op, 2.0, out=y, variant=variant))
+            emit(what=name, op=op, ms=ms, gbps=2 * nbytes / ms / 1e6)
 
     # size sweep (identity over bytes, config C5) with the default variant
     for k in range(10, 31, 2):
@@ -98,7 +78,7 @@ def main():
         ops.set_tuning(6, cap)
         ms = timeit(lambda: ops.map_reduce_sum(x, "scale", 2.0))
         emit(what="reduce_sum_f32_256MiB", grid_cap=cap * 1024, ms=ms, gbps=nbytes / ms / 1e6)
-    ops.set_tuning(6, 8)
+    ops.set_tuning(6, 4)   # back to the library default
 
     # pack: 1024 tensors of 256 KiB, and 4096 of 4 KiB
     for cnt, sz in ((1024, 1 << 18), (4096, 1 << 12), (8, 1 << 25)):

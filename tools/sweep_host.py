@@ -5,7 +5,7 @@
                buffer (wherever torch put it) and from a NUMA-sharded one (ktb_host_alloc_sharded).  Shows what the
                box can deliver whatever our pipeline does.
   e2e_host     kt.fn(mapped).to(kt.Compute(gpus=N)) -> remote(host tensor), by input buffer kind and host mode
-  raw          ops.map_host_multi without the API layer, by chunk size and zero-copy on/off
+  raw          ops.map_host_multi without the API layer, by chunk size
 """
 import json
 import os
@@ -128,21 +128,16 @@ def main():
         remote = kt.fn(double, name=f"host-sweep-{host_mode}").to(
             kt.Compute(gpus=n_gpus).distribute("b200", workers=1, num_proc=n_gpus, host_mode=host_mode))
         for kind, (xh, _) in kinds.items():
-            for zc in (0, 1):
-                if zc and host_mode != "multi":
-                    continue
-                ops.set_tuning(20, zc)
-                for _ in range(3):
-                    out = remote(xh, serialization="pickle")
-                reps = 10
-                t0 = time.perf_counter()
-                for _ in range(reps):
-                    out = remote(xh, serialization="pickle")
-                dt = (time.perf_counter() - t0) / reps
-                ok = bool(torch.equal(torch.cat(out)[-4096:], xh[-4096:] * 2)) and bool(torch.equal(out[0][:4096], xh[:4096] * 2))
-                emit(what="e2e_host", host_mode=host_mode, kind=kind, zero_copy=zc, n_gpus=n_gpus, ms=dt * 1e3,
-                     gbps=2 * n * 4 / dt / 1e9, ok=ok)
-        ops.set_tuning(20, 0)
+            for _ in range(3):
+                out = remote(xh, serialization="pickle")
+            reps = 10
+            t0 = time.perf_counter()
+            for _ in range(reps):
+                out = remote(xh, serialization="pickle")
+            dt = (time.perf_counter() - t0) / reps
+            ok = bool(torch.equal(torch.cat(out)[-4096:], xh[-4096:] * 2)) and bool(torch.equal(out[0][:4096], xh[:4096] * 2))
+            emit(what="e2e_host", host_mode=host_mode, kind=kind, n_gpus=n_gpus, ms=dt * 1e3,
+                 gbps=2 * n * 4 / dt / 1e9, ok=ok)
         remote.teardown()
     # raw pipeline without the API layer, by chunk size
     for kind, (xh, yh) in kinds.items():

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """2-GPU NVLink sweep: a kernel on GPU 1 pulling from / pushing to GPU 0's memory (the per-rank
-kernel of the fused scatter->exec->gather), by variant and tuning; plus the root-push broadcast.
+kernel of the fused scatter->exec->gather), by variant; plus the root-push broadcast.
 Writes JSON lines to gpurun_out/sweep_peer.jsonl."""
 import json
 import os
@@ -75,23 +75,11 @@ def main():
     modes = {"pull(0->1)": (x0, y1), "push(1->0)": (x1, y0), "pull+push(0->1->0)": (x0, y0), "local(1)": (x1, y1)}
     for mode, (src, dst) in modes.items():
         for variant, name in ((L.VARIANT_VEC, "vec"), (L.VARIANT_TMA, "tma")):
-            if variant == L.VARIANT_VEC:
-                grid = [(un, fl, cps) for un in (2, 8) for fl in (2,) for cps in (0, 16)]
-            else:
-                grid = [(cfg, 0, per) for cfg, per in ((0, 1), (1, 1), (2, 2), (3, 1))]
-            for a, b, c in grid:
-                if variant == L.VARIANT_VEC:
-                    ops.set_tuning(5, a); ops.set_tuning(4, b); ops.set_tuning(0, c)
-                    tag = dict(unroll=a, flavor=b, ctas_per_sm=c)
-                else:
-                    ops.set_tuning(2, a); ops.set_tuning(1, c)
-                    tag = dict(cfg=a, ctas_per_sm=c)
-                try:
-                    ms = timeit(lambda: ops.map_tensor(src, "scale", 2.0, out=dst, variant=variant, device=1), 1)
-                    emit(what="peer_map", mode=mode, variant=name, ms=ms, gbps_each_way=nbytes / ms / 1e6, **tag)
-                except Exception as e:  # noqa: BLE001
-                    emit(what="peer_map", mode=mode, variant=name, error=str(e)[:200], **tag)
-    ops.set_tuning(5, 2); ops.set_tuning(4, 2); ops.set_tuning(0, 0); ops.set_tuning(2, 0); ops.set_tuning(1, 1)
+            try:
+                ms = timeit(lambda: ops.map_tensor(src, "scale", 2.0, out=dst, variant=variant, device=1), 1)
+                emit(what="peer_map", mode=mode, variant=name, ms=ms, gbps_each_way=nbytes / ms / 1e6)
+            except Exception as e:  # noqa: BLE001
+                emit(what="peer_map", mode=mode, variant=name, error=str(e)[:200])
     ok = torch.equal(y0.cpu(), x0.cpu() * 2)
     emit(what="peer_parity_last", ok=bool(ok))
 

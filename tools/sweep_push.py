@@ -69,20 +69,6 @@ def main():
             emit(what="c2_device", n_gpus=n, mib=mib, mode="push_push_pipeline", chunks=chunks, ms=ms,
                  gbps=2 * elems * 4 / ms / 1e6, link_gbps_per_dir=(n - 1) / n * elems * 4 / ms / 1e6, ok=ok)
             del sess
-        if mib in (256, 1024):
-            for slice_ in (1, 2, 4, 8, 16):
-                for cps in (0, 4):
-                    ops.set_tuning(23, slice_)
-                    ops.set_tuning(21, cps)
-                    sess = ops.PushSession(devs, ops.shard_bounds(elems, n, 0)[1] * 4, n_chunks=32)
-                    ms = timeit(lambda: sess.call(x, y, "scale", 2.0), devs, iters)
-                    ok = bool(torch.equal(y[-4096:], x[-4096:] * 2))
-                    emit(what="c2_device", n_gpus=n, mib=mib, mode="push_push_pipeline", chunks=32, slice=slice_,
-                         scatter_ctas_per_sm=cps, ms=ms, gbps=2 * elems * 4 / ms / 1e6,
-                         link_gbps_per_dir=(n - 1) / n * elems * 4 / ms / 1e6, ok=ok)
-                    del sess
-            ops.set_tuning(23, 1)
-            ops.set_tuning(21, 0)
         del x, y
 
 
