@@ -80,7 +80,8 @@ constexpr int kMaxDevices = 16;
 DeviceInfo* device_info(int dev);   // nullptr when unregistered
 int require_device(int dev);        // KTB_OK or error (sets message)
 
-inline size_t dtype_size(int dtype) {
+// Bytes per element; 0 = unknown dtype.  constexpr so that kernels can write `constexpr size_t ES = dtype_size(DT)`.
+constexpr size_t dtype_size(int dtype) {
   switch (dtype) {
     case KTB_U8: return 1;
     case KTB_F32: return 4;
@@ -90,6 +91,57 @@ inline size_t dtype_size(int dtype) {
     case KTB_F16: return 2;
     default: return 0;
   }
+}
+
+// Bytes of a sum of the dtype's elements: fp32 for the float types, int64 for the integers; 0 = not reducible.
+constexpr size_t acc_size(int dtype) {
+  return (dtype == KTB_F32 || dtype == KTB_BF16 || dtype == KTB_F16) ? 4
+         : (dtype == KTB_I32 || dtype == KTB_I64)                    ? 8
+                                                                     : 0;
+}
+
+// ---- argument checks of the element-wise entry points (KTB_ERR_ARG with a message naming `who`) ----------------
+inline int check_dtype(const char* who, int dtype) {
+  KTB_REQUIRE(dtype_size(dtype) != 0, KTB_ERR_ARG, "%s: unknown dtype %d", who, dtype);
+  return KTB_OK;
+}
+inline int check_elementwise(const char* who, int op, int dtype) {
+  int rc = check_dtype(who, dtype);
+  if (rc) return rc;
+  KTB_REQUIRE(op >= KTB_OP_IDENTITY && op <= KTB_OP_AFFINE, KTB_ERR_ARG, "%s: unknown op %d", who, op);
+  KTB_REQUIRE(dtype != KTB_U8 || op == KTB_OP_IDENTITY, KTB_ERR_ARG, "%s: KTB_U8 supports KTB_OP_IDENTITY only", who);
+  return KTB_OK;
+}
+inline int check_reducible(const char* who, int op, int dtype) {
+  KTB_REQUIRE(acc_size(dtype) != 0, KTB_ERR_ARG, "%s: dtype %d not reducible", who, dtype);
+  return check_elementwise(who, op, dtype);
+}
+
+// ---- runtime (op, dtype) -> kernel instantiation ----------------------------------------------------------------
+// Calls f(DT, OP), both as IntC, for an (op, dtype) that check_elementwise (kReduce = false) or check_reducible
+// (kReduce = true) accepted, and returns its status.  The map form runs identity of any dtype as a byte copy,
+// <KTB_U8, KTB_OP_IDENTITY>, and {F32, BF16, I32, I64, F16} x {SCALE, AFFINE}; the reduce form runs
+// {F32, BF16, I32, I64, F16} x {IDENTITY, SCALE, AFFINE}, since a sum reads typed elements even for identity.
+template <int V>
+using IntC = std::integral_constant<int, V>;
+template <bool kReduce = false, class F>
+int dispatch_elementwise(int op, int dtype, F&& f) {
+  if constexpr (!kReduce)
+    if (op == KTB_OP_IDENTITY) return f(IntC<KTB_U8>{}, IntC<KTB_OP_IDENTITY>{});
+  auto with_op = [&](auto dt) {
+    if constexpr (kReduce)
+      if (op == KTB_OP_IDENTITY) return f(dt, IntC<KTB_OP_IDENTITY>{});
+    return op == KTB_OP_SCALE ? f(dt, IntC<KTB_OP_SCALE>{}) : f(dt, IntC<KTB_OP_AFFINE>{});
+  };
+  switch (dtype) {
+    case KTB_F32: return with_op(IntC<KTB_F32>{});
+    case KTB_BF16: return with_op(IntC<KTB_BF16>{});
+    case KTB_I32: return with_op(IntC<KTB_I32>{});
+    case KTB_I64: return with_op(IntC<KTB_I64>{});
+    case KTB_F16: return with_op(IntC<KTB_F16>{});
+  }
+  set_error("unsupported dtype/op %d/%d", dtype, op);
+  return KTB_ERR_UNSUPPORTED;
 }
 
 // Op-math parameters of a mapped callable, passed by value to kernels.

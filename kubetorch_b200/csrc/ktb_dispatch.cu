@@ -208,9 +208,10 @@ int ktb_scatter_map_gather(int op, int dtype, const void* src_root, void* dst_ro
                            int root_rank, int variant, const uintptr_t* streams) {
   int rc = check_ranks("ktb_scatter_map_gather", n_ranks, devs, root_rank);
   if (rc) return rc;
+  if (n_elems == 0) return check_dtype("ktb_scatter_map_gather", dtype);   // an empty call checks the dtype only
+  rc = check_elementwise("ktb_scatter_map_gather", op, dtype);   // before the fork: nothing is queued for a bad op
+  if (rc) return rc;
   const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_scatter_map_gather: unknown dtype %d", dtype);
-  if (n_elems == 0) return KTB_OK;
   KTB_REQUIRE(src_root && dst_root, KTB_ERR_ARG, "ktb_scatter_map_gather: null src/dst");
   KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG,
               "ktb_scatter_map_gather: n_elems %zu is not a multiple of granule %zu", n_elems, granule);
@@ -228,8 +229,9 @@ int ktb_scatter_map_reduce(int op, int dtype, const void* src_root, size_t n_ele
                            const uintptr_t* streams) {
   int rc = check_ranks("ktb_scatter_map_reduce", n_ranks, devs, root_rank);
   if (rc) return rc;
+  rc = check_reducible("ktb_scatter_map_reduce", op, dtype);
+  if (rc) return rc;
   const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0 && dtype != KTB_U8, KTB_ERR_ARG, "ktb_scatter_map_reduce: dtype %d not reducible", dtype);
   KTB_REQUIRE(partials_root && out_root && workspaces, KTB_ERR_ARG, "ktb_scatter_map_reduce: null argument");
   for (int r = 0; r < n_ranks; ++r)
     KTB_REQUIRE(workspaces[r], KTB_ERR_ARG, "ktb_scatter_map_reduce: workspaces[%d] is null", r);
@@ -237,12 +239,11 @@ int ktb_scatter_map_reduce(int op, int dtype, const void* src_root, size_t n_ele
   KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG,
               "ktb_scatter_map_reduce: n_elems %zu is not a multiple of granule %zu", n_elems, granule);
   const MapParams p = make_params(alpha, beta, dtype);
-  const size_t acc_size = (dtype == KTB_F32 || dtype == KTB_BF16 || dtype == KTB_F16) ? 4 : 8;
   // empty shards still launch: they write a zero partial (n_elems = 0 → kernel stores 0)
   rc = fork_join("ktb_scatter_map_reduce", n_elems, granule, n_ranks, devs, root_rank, streams, false,
                  [&](int r, int dev, size_t b, size_t e, cudaStream_t st) {
                    return launch_map_reduce(dev, op, dtype, static_cast<const uint8_t*>(src_root) + b * es, e - b, p,
-                                            static_cast<uint8_t*>(partials_root) + (size_t)r * acc_size,
+                                            static_cast<uint8_t*>(partials_root) + (size_t)r * acc_size(dtype),
                                             workspaces[r], st);
                  });
   if (rc) return rc;

@@ -336,9 +336,10 @@ int ktb_map_host(int dev, int op, int dtype, const void* src_host, void* dst_hos
                  double alpha, double beta, size_t chunk_bytes, void* stage_in, void* stage_out) {
   int rc = require_device(dev);
   if (rc) return rc;
+  if (n_elems == 0) return check_dtype("ktb_map_host", dtype);   // an empty call checks the dtype only
+  rc = check_elementwise("ktb_map_host", op, dtype);   // before the pipeline queues its first copy
+  if (rc) return rc;
   const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_map_host: unknown dtype %d", dtype);
-  if (n_elems == 0) return KTB_OK;
   KTB_REQUIRE(src_host && dst_host && stage_in && stage_out, KTB_ERR_ARG, "ktb_map_host: null argument");
   KTB_REQUIRE(chunk_bytes >= 4096 && chunk_bytes % 256 == 0, KTB_ERR_ARG,
               "ktb_map_host: chunk_bytes must be a multiple of 256 and >= 4096 (got %zu)", chunk_bytes);
@@ -352,8 +353,8 @@ int ktb_map_host(int dev, int op, int dtype, const void* src_host, void* dst_hos
 int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, size_t n_elems, size_t granule,
                        double alpha, double beta, int n_ranks, const int* devs, size_t chunk_bytes,
                        void* const* stage_in, void* const* stage_out) {
-  const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_map_host_multi: unknown dtype %d", dtype);
+  int rc = check_dtype("ktb_map_host_multi", dtype);
+  if (rc) return rc;
   KTB_REQUIRE(n_ranks > 0 && n_ranks <= kMaxDevices && devs && stage_in && stage_out, KTB_ERR_ARG,
               "ktb_map_host_multi: bad rank arguments");
   if (n_elems == 0) return KTB_OK;
@@ -362,12 +363,15 @@ int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, 
   KTB_REQUIRE(chunk_bytes >= 4096 && chunk_bytes % 256 == 0, KTB_ERR_ARG,
               "ktb_map_host_multi: chunk_bytes must be a multiple of 256 and >= 4096 (got %zu)", chunk_bytes);
   for (int r = 0; r < n_ranks; ++r) {
-    int rc = require_device(devs[r]);
+    rc = require_device(devs[r]);
     if (rc) return rc;
     for (int q = 0; q < r; ++q)
       KTB_REQUIRE(devs[q] != devs[r], KTB_ERR_ARG, "ktb_map_host_multi: devices must be distinct (use ktb_map_host per rank)");
     KTB_REQUIRE(stage_in[r] && stage_out[r], KTB_ERR_ARG, "ktb_map_host_multi: rank %d has no staging buffers", r);
   }
+  rc = check_elementwise("ktb_map_host_multi", op, dtype);   // before any rank's pipeline starts
+  if (rc) return rc;
+  const size_t es = dtype_size(dtype);
   std::lock_guard<std::mutex> lk(g_host_call_mu);
   const MapParams p = make_params(alpha, beta, dtype);
   const uint8_t* src = static_cast<const uint8_t*>(src_host);

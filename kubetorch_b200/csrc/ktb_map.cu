@@ -66,7 +66,7 @@ __global__ void __launch_bounds__(kVecThreads)
       apply_words<DT, OP, NW>(w, p);
       stg128_stream(dst + base + v * VB, w);
     }
-    constexpr size_t ES = (DT == KTB_U8) ? 1 : ((DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4));
+    constexpr size_t ES = dtype_size(DT);
     const size_t tail = base + n_vec * VB;
     const size_t n_tail = (n_bytes - tail) / ES;
     for (size_t e = threadIdx.x; e < n_tail; e += kVecThreads)
@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(kVecThreads)
 template <int DT, int OP>
 __global__ void __launch_bounds__(256)
     map_scalar_kernel(const uint8_t* src, uint8_t* dst, size_t n_elems, MapParams p) {
-  constexpr size_t ES = (DT == KTB_U8) ? 1 : ((DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4));
+  constexpr size_t ES = dtype_size(DT);
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_elems; i += stride)
     apply_elem<DT, OP>(src + i * ES, dst + i * ES, p);
@@ -164,7 +164,7 @@ __global__ void __launch_bounds__(kTmaThreads)
 
   // < 16 trailing bytes: element tail by CTA 0.
   if (blockIdx.x == 0) {
-    constexpr size_t ES = (DT == KTB_U8) ? 1 : ((DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4));
+    constexpr size_t ES = dtype_size(DT);
     const size_t n_tail = (n_bytes - n16) / ES;
     for (size_t e = threadIdx.x; e < n_tail; e += NT)
       apply_elem<DT, OP>(src + n16 + e * ES, dst + n16 + e * ES, p);
@@ -173,10 +173,10 @@ __global__ void __launch_bounds__(kTmaThreads)
 
 // ---- launch plumbing --------------------------------------------------------------------------
 template <int DT, int OP>
-static int launch_typed(int dev, const uint8_t* src, uint8_t* dst, size_t n_elems, size_t es,
-                        const MapParams& p, int variant, cudaStream_t stream) {
+static int launch_typed(int dev, const uint8_t* src, uint8_t* dst, size_t n_bytes, const MapParams& p, int variant,
+                        cudaStream_t stream) {
   const DeviceInfo* di = device_info(dev);
-  const size_t n_bytes = n_elems * es;
+  const size_t n_elems = n_bytes / dtype_size(DT);
   const uintptr_t both = (uintptr_t)src | (uintptr_t)dst;
 
   if (variant == KTB_VARIANT_AUTO) variant = KTB_VARIANT_VEC;
@@ -212,12 +212,10 @@ int launch_map(int dev, int op, int dtype, const void* src_, void* dst_, size_t 
                const MapParams& p, int variant, cudaStream_t stream) {
   const uint8_t* src = static_cast<const uint8_t*>(src_);
   uint8_t* dst = static_cast<uint8_t*>(dst_);
-  const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_map: unknown dtype %d", dtype);
-  KTB_REQUIRE(op >= KTB_OP_IDENTITY && op <= KTB_OP_AFFINE, KTB_ERR_ARG, "ktb_map: unknown op %d", op);
-  KTB_REQUIRE(!(dtype == KTB_U8 && op != KTB_OP_IDENTITY), KTB_ERR_ARG,
-              "ktb_map: KTB_U8 supports KTB_OP_IDENTITY only");
+  int rc = check_elementwise("ktb_map", op, dtype);
+  if (rc) return rc;
   if (n_elems == 0) return KTB_OK;
+  const size_t es = dtype_size(dtype);
   KTB_REQUIRE(src && dst, KTB_ERR_ARG, "ktb_map: null src/dst with n_elems=%zu", n_elems);
   KTB_REQUIRE((((uintptr_t)src | (uintptr_t)dst) & (es - 1)) == 0, KTB_ERR_ARG,
               "ktb_map: src/dst not aligned to the element size %zu", es);
@@ -228,25 +226,9 @@ int launch_map(int dev, int op, int dtype, const void* src_, void* dst_, size_t 
     KTB_REQUIRE(se <= dst || de <= src, KTB_ERR_ARG, "ktb_map: src and dst partially overlap");
   }
 
-  // identity is a byte copy whatever the dtype
-  if (op == KTB_OP_IDENTITY)
-    return launch_typed<KTB_U8, KTB_OP_IDENTITY>(dev, src, dst, n_elems * es, 1, p, variant, stream);
-
-#define KTB_CASE(DT)                                                                              \
-  case DT:                                                                                        \
-    return (op == KTB_OP_SCALE)                                                                   \
-               ? launch_typed<DT, KTB_OP_SCALE>(dev, src, dst, n_elems, es, p, variant, stream)   \
-               : launch_typed<DT, KTB_OP_AFFINE>(dev, src, dst, n_elems, es, p, variant, stream);
-  switch (dtype) {
-    KTB_CASE(KTB_F32)
-    KTB_CASE(KTB_BF16)
-    KTB_CASE(KTB_I32)
-    KTB_CASE(KTB_I64)
-    KTB_CASE(KTB_F16)
-  }
-#undef KTB_CASE
-  set_error("ktb_map: unsupported dtype/op %d/%d", dtype, op);
-  return KTB_ERR_UNSUPPORTED;
+  return dispatch_elementwise(op, dtype, [&](auto dt, auto o) {
+    return launch_typed<dt, o>(dev, src, dst, n_elems * es, p, variant, stream);
+  });
 }
 
 }  // namespace ktb

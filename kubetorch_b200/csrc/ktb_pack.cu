@@ -42,7 +42,7 @@ static_assert(sizeof(SegBatch<kSegLarge>) + sizeof(MapParams) <= 32764, "large b
 template <int DT, int OP, int CAP>
 __global__ void __launch_bounds__(kSegThreads)
     seg_map_kernel(const __grid_constant__ SegBatch<CAP> b, const __grid_constant__ MapParams p) {
-  constexpr size_t ES = (DT == KTB_U8) ? 1 : ((DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4));
+  constexpr size_t ES = dtype_size(DT);
   const uint32_t n_tiles = b.tile_prefix[b.n];
   for (uint32_t t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     // binary search: largest i with tile_prefix[i] <= t
@@ -109,33 +109,16 @@ __global__ void __launch_bounds__(kSegThreads)
   }
 }
 
-template <int DT, int OP, int CAP>
-static int launch_seg_typed(const SegBatch<CAP>& b, const MapParams& p, cudaStream_t stream) {
+template <int CAP>
+static int launch_seg(int op, int dtype, const SegBatch<CAP>& b, const MapParams& p, cudaStream_t stream) {
   const uint32_t n_tiles = b.tile_prefix[b.n];
   if (n_tiles == 0) return KTB_OK;
   int grid = (int)n_tiles;  // one 32 KiB tile per CTA: the hardware scheduler balances ragged segments
-  seg_map_kernel<DT, OP, CAP><<<grid, kSegThreads, 0, stream>>>(b, p);
-  KTB_CK(cudaGetLastError());
-  return KTB_OK;
-}
-
-template <int CAP>
-static int launch_seg(int op, int dtype, const SegBatch<CAP>& b, const MapParams& p, cudaStream_t stream) {
-  if (op == KTB_OP_IDENTITY) return launch_seg_typed<KTB_U8, KTB_OP_IDENTITY, CAP>(b, p, stream);
-#define KTB_SCASE(DT)                                                                    \
-  case DT:                                                                               \
-    return (op == KTB_OP_SCALE) ? launch_seg_typed<DT, KTB_OP_SCALE, CAP>(b, p, stream)  \
-                                : launch_seg_typed<DT, KTB_OP_AFFINE, CAP>(b, p, stream);
-  switch (dtype) {
-    KTB_SCASE(KTB_F32)
-    KTB_SCASE(KTB_BF16)
-    KTB_SCASE(KTB_I32)
-    KTB_SCASE(KTB_I64)
-    KTB_SCASE(KTB_F16)
-  }
-#undef KTB_SCASE
-  set_error("ktb_map_batch: unsupported dtype/op %d/%d", dtype, op);
-  return KTB_ERR_UNSUPPORTED;
+  return dispatch_elementwise(op, dtype, [&](auto dt, auto o) {
+    seg_map_kernel<dt, o, CAP><<<grid, kSegThreads, 0, stream>>>(b, p);
+    KTB_CK(cudaGetLastError());
+    return KTB_OK;
+  });
 }
 
 // Splits n segments into launches of <= CAP descriptors (and < 2^31 tiles).
@@ -244,11 +227,9 @@ int ktb_map_batch(int dev, int op, int dtype, const void* const* srcs, void* con
   KTB_REQUIRE(n >= 0, KTB_ERR_ARG, "ktb_map_batch: negative n");
   if (n == 0) return KTB_OK;
   KTB_REQUIRE(srcs && dsts && n_elems, KTB_ERR_ARG, "ktb_map_batch: null argument");
+  rc = check_elementwise("ktb_map_batch", op, dtype);
+  if (rc) return rc;
   const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_map_batch: unknown dtype %d", dtype);
-  KTB_REQUIRE(op >= KTB_OP_IDENTITY && op <= KTB_OP_AFFINE, KTB_ERR_ARG, "ktb_map_batch: unknown op %d", op);
-  KTB_REQUIRE(!(dtype == KTB_U8 && op != KTB_OP_IDENTITY), KTB_ERR_ARG,
-              "ktb_map_batch: KTB_U8 supports KTB_OP_IDENTITY only");
   std::vector<size_t> nb((size_t)n);
   for (int i = 0; i < n; ++i) nb[(size_t)i] = n_elems[i] * es;
   KTB_GUARD(dev);

@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(kPushThreads)
                         uint32_t tiles_per_chunk, MapParams p,
                         const unsigned long long* ready, unsigned long long seq, unsigned long long* ack,
                         unsigned int* ticket, unsigned int* status) {
-  constexpr size_t ES = (DT == KTB_U8) ? 1 : ((DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4));
+  constexpr size_t ES = dtype_size(DT);
   __shared__ bool flag;
   // One CTA per tile, tiles in increasing order = chunk order, and no tile loop: the kernel then keeps few registers
   // and many CTAs per SM (with a grid-stride loop it took 40 registers and 11 % longer on an H100 80GB HBM3 at 700 W).
@@ -188,14 +188,44 @@ __global__ void push_wait_kernel(const unsigned long long* ack, int n_ranks, int
   if (r < n_ranks && r != root_rank) spin_until(&ack[r], seq, status);
 }
 
-// Chunk c of a shard of `shard_elems` elements: element range [b, e), chunk size rounded to 64 elements.
-static inline void chunk_bounds(size_t shard_elems, int n_chunks, int c, size_t* b, size_t* e) {
-  size_t per = (shard_elems + (size_t)n_chunks - 1) / (size_t)n_chunks;
-  per = (per + 63) / 64 * 64;
-  size_t lo = std::min(shard_elems, per * (size_t)c);
-  size_t hi = std::min(shard_elems, lo + per);
-  *b = lo;
-  *e = hi;
+// Elements per chunk when a shard of shard_elems elements is cut into n_chunks pieces: ceil(shard / n_chunks) rounded
+// up to 64 elements, at most the whole shard.  The root and the rank (possibly in different processes) both use it,
+// so they agree on every chunk's bounds.
+static size_t push_chunk_elems(size_t shard_elems, int n_chunks) {
+  const size_t per = (shard_elems + (size_t)n_chunks - 1) / (size_t)n_chunks;
+  return std::min(shard_elems, (per + 63) / 64 * 64);
+}
+
+// n_chunks of the chunk_elems form: as many pieces of exactly chunk_elems elements as the largest shard (rank 0's)
+// needs, at least 1; any count past KTB_PUSH_MAX_CHUNKS comes back as KTB_PUSH_MAX_CHUNKS + 1 for the caller to reject.
+static int push_chunk_count(size_t n_elems, size_t granule, int n_ranks, size_t chunk_elems) {
+  size_t b0 = 0, e0 = 0;
+  ktb_shard_bounds(n_elems / granule, n_ranks, 0, &b0, &e0);
+  const size_t n = std::max<size_t>(1, ((e0 - b0) * granule + chunk_elems - 1) / chunk_elems);
+  return (int)std::min<size_t>(n, KTB_PUSH_MAX_CHUNKS + 1);
+}
+
+// The argument checks of the root side that the SM form (push_scatter_impl) and the copy-engine form share.
+static int check_push_scatter(const char* who, int root_dev, const void* src_root, size_t n_elems, size_t granule,
+                              int dtype, int n_ranks, int root_rank, void* const* stage_peer, size_t stage_stride,
+                              void* const* ctrl_peer, const void* ctrl_root, unsigned long long seq) {
+  int rc = require_device(root_dev);
+  if (rc) return rc;
+  rc = check_dtype(who, dtype);
+  if (rc) return rc;
+  KTB_REQUIRE(n_ranks > 0 && n_ranks <= kPushMaxRanks && root_rank >= 0 && root_rank < n_ranks, KTB_ERR_ARG,
+              "%s: bad ranks %d/%d", who, root_rank, n_ranks);
+  KTB_REQUIRE(src_root && stage_peer && ctrl_peer && ctrl_root && seq > 0, KTB_ERR_ARG, "%s: null argument", who);
+  KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG, "%s: n_elems not a multiple of granule", who);
+  for (int r = 0; r < n_ranks; ++r) {
+    if (r == root_rank || !stage_peer[r]) continue;   // null staging = rank served by another scatter call
+    size_t b = 0, e = 0;
+    ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
+    KTB_REQUIRE(ctrl_peer[r], KTB_ERR_ARG, "%s: rank %d has no control block", who, r);
+    KTB_REQUIRE((e - b) * granule * dtype_size(dtype) <= stage_stride, KTB_ERR_ARG,
+                "%s: shard of rank %d exceeds stage_stride", who, r);
+  }
+  return KTB_OK;
 }
 
 }  // namespace ktb
@@ -208,26 +238,18 @@ size_t ktb_push_control_bytes(void) { return 4096; }
 
 // (control-block layout: KTB_CTRL_* in ktb_common.cuh)
 
-// chunk_elems == 0: n_chunks pieces per shard (chunk_bounds); otherwise pieces of exactly chunk_elems elements
+// chunk_elems == 0: n_chunks pieces per shard (push_chunk_elems); otherwise pieces of exactly chunk_elems elements
 // (the consumer of ktb_mlp_bf16_pushed wants whole GEMM row chunks), n_chunks = ceil(largest shard / chunk_elems).
 static int push_scatter_impl(const char* who, int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
                              int n_ranks, int root_rank, void* const* stage_peer, size_t stage_stride,
                              void* const* ctrl_peer, void* ctrl_root, int n_chunks, size_t chunk_elems,
                              unsigned long long seq, int ctas_per_sm, uintptr_t stream) {
-  int rc = require_device(root_dev);
+  int rc = check_push_scatter(who, root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank, stage_peer,
+                              stage_stride, ctrl_peer, ctrl_root, seq);
   if (rc) return rc;
-  const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "%s: unknown dtype %d", who, dtype);
-  KTB_REQUIRE(n_ranks > 0 && n_ranks <= kPushMaxRanks && root_rank >= 0 && root_rank < n_ranks, KTB_ERR_ARG,
-              "%s: bad ranks %d/%d", who, root_rank, n_ranks);
-  KTB_REQUIRE(src_root && stage_peer && ctrl_peer && ctrl_root && seq > 0, KTB_ERR_ARG, "%s: null argument", who);
-  KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG, "%s: n_elems not a multiple of granule", who);
-  if (chunk_elems) {
-    size_t b0 = 0, e0 = 0;
-    ktb_shard_bounds(n_elems / granule, n_ranks, 0, &b0, &e0);   // rank 0 holds the largest shard
-    n_chunks = (int)std::max<size_t>(1, ((e0 - b0) * granule + chunk_elems - 1) / chunk_elems);
-  }
+  if (chunk_elems) n_chunks = push_chunk_count(n_elems, granule, n_ranks, chunk_elems);
   KTB_REQUIRE(n_chunks > 0 && n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: n_chunks %d out of range", who, n_chunks);
+  const size_t es = dtype_size(dtype);
   KTB_GUARD(root_dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   uint8_t* croot = static_cast<uint8_t*>(ctrl_root);
@@ -242,19 +264,13 @@ static int push_scatter_impl(const char* who, int root_dev, const void* src_root
   a.seq = seq;
   a.tile_prefix[0] = 0;
   for (int r = 0; r < n_ranks; ++r) {
-    if (r == root_rank) continue;
-    size_t sb = 0, se = 0, c0b = 0, c0e = 0, per = chunk_elems, dummy = 0;
+    // a null stage_peer[r]: not served by this call (a hybrid scatter splits the ranks between two engines)
+    if (r == root_rank || !stage_peer[r]) continue;
+    size_t sb = 0, se = 0;
     ktb_shard_bounds(n_elems / granule, n_ranks, r, &sb, &se);
     sb *= granule;
     se *= granule;
-    if (!chunk_elems) {
-      chunk_bounds(se - sb, n_chunks, 0, &c0b, &c0e);
-      chunk_bounds(se - sb, n_chunks, 1, &per, &dummy);   // start of chunk 1 = elements per chunk
-      if (per == 0) per = c0e - c0b;                      // single-chunk (or empty) shard
-    }
-    if (!stage_peer[r]) continue;   // not served by this call (a hybrid scatter splits the ranks between two engines)
-    KTB_REQUIRE(ctrl_peer[r], KTB_ERR_ARG, "%s: rank %d has no control block", who, r);
-    KTB_REQUIRE((se - sb) * es <= stage_stride, KTB_ERR_ARG, "%s: shard of rank %d exceeds stage_stride", who, r);
+    const size_t per = chunk_elems ? chunk_elems : push_chunk_elems(se - sb, n_chunks);
     const int i = a.n++;
     a.src[i] = static_cast<const uint8_t*>(src_root) + sb * es;
     a.dst[i] = static_cast<uint8_t*>(stage_peer[r]) + buf_off;
@@ -312,20 +328,13 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
                         int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
                         void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, unsigned long long seq,
                         uintptr_t stream) {
-  int rc = require_device(root_dev);
+  int rc = check_push_scatter("ktb_push_scatter_ce", root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank,
+                              stage_peer, stage_stride, ctrl_peer, ctrl_root, seq);
   if (rc) return rc;
+  KTB_REQUIRE(devs && chunk_elems > 0, KTB_ERR_ARG, "ktb_push_scatter_ce: null devs or zero chunk_elems");
+  const int n_chunks = push_chunk_count(n_elems, granule, n_ranks, chunk_elems);
+  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "ktb_push_scatter_ce: more than %d chunks", KTB_PUSH_MAX_CHUNKS);
   const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_push_scatter_ce: unknown dtype %d", dtype);
-  KTB_REQUIRE(n_ranks > 0 && n_ranks <= kPushMaxRanks && root_rank >= 0 && root_rank < n_ranks && devs, KTB_ERR_ARG,
-              "ktb_push_scatter_ce: bad ranks %d/%d", root_rank, n_ranks);
-  KTB_REQUIRE(src_root && stage_peer && ctrl_peer && ctrl_root && seq > 0 && chunk_elems > 0, KTB_ERR_ARG,
-              "ktb_push_scatter_ce: null/zero argument");
-  KTB_REQUIRE(granule > 0 && n_elems % granule == 0, KTB_ERR_ARG, "ktb_push_scatter_ce: n_elems not a multiple of granule");
-  size_t b0 = 0, e0 = 0;
-  ktb_shard_bounds(n_elems / granule, n_ranks, 0, &b0, &e0);
-  const size_t n_chunks = std::max<size_t>(1, ((e0 - b0) * granule + chunk_elems - 1) / chunk_elems);
-  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "ktb_push_scatter_ce: %zu chunks exceed %d", n_chunks,
-              KTB_PUSH_MAX_CHUNKS);
   KTB_GUARD(root_dev);
   // one library stream (and fork/join event pair) per destination rank on the root device, created on first use:
   // every peer's copies ride their own copy-engine queue, chunk-major issue order
@@ -347,8 +356,6 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
     sb[r] = b * granule;
     sl[r] = (e - b) * granule;
     if (r == root_rank || !stage_peer[r]) continue;   // null staging = rank served by another scatter call
-    KTB_REQUIRE(ctrl_peer[r], KTB_ERR_ARG, "ktb_push_scatter_ce: rank %d has no control block", r);
-    KTB_REQUIRE(sl[r] * es <= stage_stride, KTB_ERR_ARG, "ktb_push_scatter_ce: shard of rank %d exceeds stage_stride", r);
     if (!ce_stream[root_dev][r]) {
       KTB_CK(cudaStreamCreateWithFlags(&ce_stream[root_dev][r], cudaStreamNonBlocking));
       KTB_CK(cudaEventCreateWithFlags(&ce_done[root_dev][r], cudaEventDisableTiming));
@@ -360,7 +367,7 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
       KTB_CK(cudaGetLastError());
     }
   }
-  for (size_t c = 0; c < n_chunks; ++c) {
+  for (size_t c = 0; c < (size_t)n_chunks; ++c) {
     for (int r = 0; r < n_ranks; ++r) {
       if (r == root_rank || !stage_peer[r]) continue;
       cudaStream_t cs = ce_stream[root_dev][r];
@@ -387,10 +394,8 @@ int ktb_push_consume(int dev, int op, int dtype, const void* stage_local, size_t
                      int n_chunks, unsigned long long seq, uintptr_t stream) {
   int rc = require_device(dev);
   if (rc) return rc;
-  const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(es != 0, KTB_ERR_ARG, "ktb_push_consume: unknown dtype %d", dtype);
-  KTB_REQUIRE(op >= KTB_OP_IDENTITY && op <= KTB_OP_AFFINE && !(dtype == KTB_U8 && op != KTB_OP_IDENTITY), KTB_ERR_ARG,
-              "ktb_push_consume: bad op/dtype %d/%d", op, dtype);
+  rc = check_elementwise("ktb_push_consume", op, dtype);
+  if (rc) return rc;
   KTB_REQUIRE(n_chunks > 0 && n_chunks <= KTB_PUSH_MAX_CHUNKS && rank >= 0 && rank < kPushMaxRanks && seq > 0, KTB_ERR_ARG,
               "ktb_push_consume: bad chunk/rank arguments");
   KTB_REQUIRE(stage_local && ctrl_local && ctrl_root_peer && (dst_root_shard || shard_elems == 0), KTB_ERR_ARG,
@@ -405,31 +410,17 @@ int ktb_push_consume(int dev, int op, int dtype, const void* stage_local, size_t
   unsigned long long* ack =
       reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctrl_root_peer) + KTB_CTRL_ACK) + rank;
   const uint8_t* stage = static_cast<const uint8_t*>(stage_local) + (size_t)(seq & 1) * stage_stride;
-  size_t per = 0, dummy = 0, c0b = 0, c0e = 0;
-  chunk_bounds(shard_elems, n_chunks, 0, &c0b, &c0e);
-  chunk_bounds(shard_elems, n_chunks, 1, &per, &dummy);
-  if (per == 0) per = c0e - c0b;
-  const size_t chunk_bytes = per * es, shard_bytes = shard_elems * es;
+  const size_t es = dtype_size(dtype);
+  const size_t chunk_bytes = push_chunk_elems(shard_elems, n_chunks) * es, shard_bytes = shard_elems * es;
   const uint32_t tpc = (uint32_t)std::max<size_t>(1, (chunk_bytes + kPushTile - 1) / kPushTile);
   const unsigned grid = (unsigned)((size_t)tpc * (size_t)n_chunks);   // one CTA per tile
   uint8_t* d = static_cast<uint8_t*>(dst_root_shard);
-#define KTB_PC(DT, OPC)                                                                                       \
-  push_consume_kernel<DT, OPC><<<grid, kPushThreads, 0, st>>>(stage, d, shard_bytes, chunk_bytes, tpc, p, ready, seq, \
-                                                              ack, ticket, status)
-  if (op == KTB_OP_IDENTITY) {
-    KTB_PC(KTB_U8, KTB_OP_IDENTITY);
-  } else {
-    switch (dtype) {
-      case KTB_F32: if (op == KTB_OP_SCALE) KTB_PC(KTB_F32, KTB_OP_SCALE); else KTB_PC(KTB_F32, KTB_OP_AFFINE); break;
-      case KTB_BF16: if (op == KTB_OP_SCALE) KTB_PC(KTB_BF16, KTB_OP_SCALE); else KTB_PC(KTB_BF16, KTB_OP_AFFINE); break;
-      case KTB_I32: if (op == KTB_OP_SCALE) KTB_PC(KTB_I32, KTB_OP_SCALE); else KTB_PC(KTB_I32, KTB_OP_AFFINE); break;
-      case KTB_F16: if (op == KTB_OP_SCALE) KTB_PC(KTB_F16, KTB_OP_SCALE); else KTB_PC(KTB_F16, KTB_OP_AFFINE); break;
-      default: if (op == KTB_OP_SCALE) KTB_PC(KTB_I64, KTB_OP_SCALE); else KTB_PC(KTB_I64, KTB_OP_AFFINE); break;
-    }
-  }
-#undef KTB_PC
-  KTB_CK(cudaGetLastError());
-  return KTB_OK;
+  return dispatch_elementwise(op, dtype, [&](auto dt, auto o) {
+    push_consume_kernel<dt, o><<<grid, kPushThreads, 0, st>>>(stage, d, shard_bytes, chunk_bytes, tpc, p, ready, seq,
+                                                              ack, ticket, status);
+    KTB_CK(cudaGetLastError());
+    return KTB_OK;
+  });
 }
 
 int ktb_push_wait(int root_dev, void* ctrl_root, int n_ranks, int root_rank, unsigned long long seq, uintptr_t stream) {

@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(kRedThreads)
   using A = typename Acc<DT>::type;
   // cross-CTA partials are kept in fp64 for float sums, int64 for integer sums
   using P = typename std::conditional<std::is_same<A, float>::value, double, long long>::type;
-  constexpr size_t ES = (DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4);
+  constexpr size_t ES = dtype_size(DT);
   __shared__ P red[32];
   __shared__ bool is_last;
 
@@ -213,7 +213,7 @@ template <int DT, int OP>
 static int launch_reduce_typed(int dev, const uint8_t* src, size_t n_elems, const MapParams& p,
                                void* out, void* ws, cudaStream_t stream) {
   (void)dev;
-  constexpr size_t ES = (DT == KTB_BF16 || DT == KTB_F16) ? 2 : (DT == KTB_I64 ? 8 : 4);
+  constexpr size_t ES = dtype_size(DT);
   const int loads = g_red_loads == 4 ? 4 : 8;
   const size_t tile = (size_t)loads * kRedThreads * 32;  // one tile per CTA
   const size_t tiles = (n_elems * ES + tile - 1) / tile;
@@ -229,47 +229,25 @@ static int launch_reduce_typed(int dev, const uint8_t* src, size_t n_elems, cons
 
 int launch_map_reduce(int dev, int op, int dtype, const void* src, size_t n_elems, const MapParams& p,
                       void* out, void* workspace, cudaStream_t stream) {
-  KTB_REQUIRE(dtype == KTB_F32 || dtype == KTB_BF16 || dtype == KTB_F16 || dtype == KTB_I32 || dtype == KTB_I64, KTB_ERR_ARG,
-              "ktb_map_reduce_sum: dtype %d not reducible", dtype);
-  KTB_REQUIRE(op >= KTB_OP_IDENTITY && op <= KTB_OP_AFFINE, KTB_ERR_ARG, "ktb_map_reduce_sum: unknown op %d", op);
+  int rc = check_reducible("ktb_map_reduce_sum", op, dtype);
+  if (rc) return rc;
   KTB_REQUIRE(out && workspace, KTB_ERR_ARG, "ktb_map_reduce_sum: null out/workspace");
   KTB_REQUIRE(src || n_elems == 0, KTB_ERR_ARG, "ktb_map_reduce_sum: null src");
-  const size_t es = dtype_size(dtype);
-  KTB_REQUIRE((((uintptr_t)src) & (es - 1)) == 0, KTB_ERR_ARG, "ktb_map_reduce_sum: src misaligned");
-  const uint8_t* s = static_cast<const uint8_t*>(src);
-#define KTB_RCASE(DT)                                                                         \
-  case DT:                                                                                    \
-    switch (op) {                                                                             \
-      case KTB_OP_IDENTITY:                                                                   \
-        return launch_reduce_typed<DT, KTB_OP_IDENTITY>(dev, s, n_elems, p, out, workspace, stream); \
-      case KTB_OP_SCALE:                                                                      \
-        return launch_reduce_typed<DT, KTB_OP_SCALE>(dev, s, n_elems, p, out, workspace, stream);    \
-      default:                                                                                \
-        return launch_reduce_typed<DT, KTB_OP_AFFINE>(dev, s, n_elems, p, out, workspace, stream);   \
-    }
-  switch (dtype) {
-    KTB_RCASE(KTB_F32)
-    KTB_RCASE(KTB_BF16)
-    KTB_RCASE(KTB_I32)
-    KTB_RCASE(KTB_I64)
-    KTB_RCASE(KTB_F16)
-  }
-#undef KTB_RCASE
-  return KTB_ERR_UNSUPPORTED;
+  KTB_REQUIRE((((uintptr_t)src) & (dtype_size(dtype) - 1)) == 0, KTB_ERR_ARG, "ktb_map_reduce_sum: src misaligned");
+  return dispatch_elementwise<true>(op, dtype, [&](auto dt, auto o) {
+    return launch_reduce_typed<dt, o>(dev, static_cast<const uint8_t*>(src), n_elems, p, out, workspace, stream);
+  });
 }
 
 int launch_reduce_partials(int dev, int dtype, const void* partials, int n, void* out, cudaStream_t stream) {
   (void)dev;
   KTB_REQUIRE(partials && out && n > 0, KTB_ERR_ARG, "ktb_reduce_partials: bad arguments");
-  if (dtype == KTB_F32 || dtype == KTB_BF16 || dtype == KTB_F16)
+  KTB_REQUIRE(acc_size(dtype) != 0, KTB_ERR_ARG, "ktb_reduce_partials: dtype %d not reducible", dtype);
+  if (acc_size(dtype) == 4)
     reduce_partials_kernel<float, double><<<1, kRedThreads, 0, stream>>>((const float*)partials, n, (float*)out);
-  else if (dtype == KTB_I32 || dtype == KTB_I64)
+  else
     reduce_partials_kernel<long long, long long>
         <<<1, kRedThreads, 0, stream>>>((const long long*)partials, n, (long long*)out);
-  else {
-    set_error("ktb_reduce_partials: dtype %d not reducible", dtype);
-    return KTB_ERR_ARG;
-  }
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
