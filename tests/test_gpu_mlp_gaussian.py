@@ -2,7 +2,6 @@
 and log-probabilities against fp64 restatements built from the kernel's own logits, its noise against fp64 ndtri and
 N(0, 1), deterministic columns, bit identity across chunkings, forms, row offsets and repeat calls, seeds, planted NaN
 and infinite logits and log_std, guard bands, status codes, and the mapped op through the public API."""
-import ctypes
 import math
 import os
 from unittest import mock
@@ -11,43 +10,18 @@ import pytest
 import torch
 
 from conftest import mapped_copy
-from test_gpu_mlp import SHIPPED_CHUNK, _Guarded
-from test_gpu_mlp_policy import _PolicyPushRig, _config, _policy_weights, _randn, _stream
+from kubetorch_b200.device import lib as L
+from kubetorch_b200.device import mlp
+from mlp_rig import (GAUSSIAN, SHIPPED_CHUNK, Guarded, K, PushRig, config, deployed, expect_status,  # noqa: F401
+                     identity, plain, policy_weights, pushed, randn, run_guarded, tuning)
 
 pytestmark = pytest.mark.gpu
 
 import policy_gaussian_cases  # noqa: E402
 from oracle import ref_dispatch  # noqa: E402
+from policy_cases import mlp_policy_biased  # noqa: E402
 
 from kubetorch_b200.sampling import gumbel_uniform  # noqa: E402
-
-
-@pytest.fixture(scope="module")
-def K():
-    assert torch.cuda.is_available()
-    from kubetorch_b200.device import lib as L
-    from kubetorch_b200.device import ops
-
-    L.load()
-    ops.ensure_init([0])
-    return ops
-
-
-def _L():
-    from kubetorch_b200.device import lib as L
-
-    return L
-
-
-def _mlp():
-    from kubetorch_b200.device import mlp
-
-    return mlp
-
-
-def _ptr(t):
-    return 0 if t is None else t.data_ptr()
-
 
 HALF_LOG_2PI = 0.5 * math.log(2 * math.pi)
 
@@ -92,11 +66,11 @@ def _check_gaussian(y, log_std, seed, row0, actions, log_probs, what):
 
 
 def _gauss(obs, w, b, log_std, seed, **kw):
-    return _mlp().mlp_forward(obs, *w, biases=b, output="gaussian", log_std=log_std, seed=seed, **kw)
+    return mlp.mlp_forward(obs, *w, biases=b, output="gaussian", log_std=log_std, seed=seed, **kw)
 
 
 def _logits(obs, w, b):
-    return _mlp().mlp_forward(obs, *w, biases=b, output="logits")
+    return mlp.mlp_forward(obs, *w, biases=b, output="logits")
 
 
 def _log_std(d_out, lo=-3.0, hi=1.0):
@@ -110,22 +84,19 @@ def test_gaussian_bars_at_every_head_width(K, d_out, chunk):
     """17 901 rows: more than one chunk at either chunk size, and a partial last tile; a seed past 2^32; log_std spread
     over [-3, 1]; logits of a few units."""
     M, seed = SHIPPED_CHUNK + 1005, 2**33 + 7 * d_out
-    w, b = _config(200 + d_out, d_out)
+    w, b = config(200 + d_out, d_out)
     w = (w[0], w[1], w[2] * 50)
-    obs = _randn((M, 256), 210 + d_out)
+    obs = randn((M, 256), 210 + d_out)
     log_std = _log_std(d_out)
-    K.set_tuning(8, chunk)
-    try:
+    with tuning(chunk):
         y = _logits(obs, w, b)
         actions, log_probs = _gauss(obs, w, b, log_std, seed)
-    finally:
-        K.set_tuning(8, SHIPPED_CHUNK)
     _check_gaussian(y, log_std, seed, 0, actions, log_probs, f"d_out={d_out} chunk={chunk}")
 
 
 # ---- 2. the noise and its distribution ---------------------------------------------------------------------------------
 def _zero_head(seed_cfg, d_out):
-    (w1, w2, _), (b1, b2, _) = _config(seed_cfg, d_out)
+    (w1, w2, _), (b1, b2, _) = config(seed_cfg, d_out)
     w3 = torch.zeros(d_out, 1024, dtype=torch.bfloat16, device="cuda")
     b3 = torch.zeros(d_out, dtype=torch.bfloat16, device="cuda")
     return (w1, w2, w3), (b1, b2, b3)
@@ -140,7 +111,7 @@ def test_noise_meets_its_bar_and_follows_the_standard_normal(K):
 
     d_out, M, seed = 8, 1 << 20, 20240611
     w, b = _zero_head(300, d_out)
-    obs = _randn((M, 256), 301)
+    obs = randn((M, 256), 301)
     z, log_probs = _gauss(obs, w, b, torch.zeros(d_out, device="cuda"), seed)
     z64 = _z64(seed, 0, M, d_out)
     err = (z.double() - z64).abs()
@@ -174,8 +145,8 @@ def test_noise_meets_its_bar_and_follows_the_standard_normal(K):
 def test_minus_inf_log_std_gives_the_logits(K, d_out):
     """log_std = -inf on some columns: σ = 0, so those actions equal the logits of output="logits" (==), and every
     row's log-probability is +inf; the other columns still meet the bar."""
-    w, b = _config(350 + d_out, d_out)
-    obs = _randn((3000, 256), 351)
+    w, b = config(350 + d_out, d_out)
+    obs = randn((3000, 256), 351)
     log_std = _log_std(d_out).clone()
     det = list(range(0, d_out, 3))
     log_std[det] = float("-inf")
@@ -197,25 +168,18 @@ def test_minus_inf_log_std_gives_the_logits(K, d_out):
 def test_every_chunking_form_and_row_split_gives_identical_bits(K, d_out):
     """Repeat calls, chunk sizes 256 / 512 / shipped, plain and staged (kernel or copy-engine pull), and one call over
     M rows against two calls over [0, b) and [b, M) with row_offset = b."""
-    w, b = _config(400 + d_out, d_out)
+    w, b = config(400 + d_out, d_out)
     M, seed = SHIPPED_CHUNK + 1000, 77
-    obs = _randn((M, 256), 401)
+    obs = randn((M, 256), 401)
     log_std = _log_std(d_out)
     want_a, want_lp = _gauss(obs, w, b, log_std, seed)
     again = _gauss(obs, w, b, log_std, seed)
     assert torch.equal(again[0], want_a) and torch.equal(again[1], want_lp)
-    try:
-        for chunk in (256, 512, SHIPPED_CHUNK):
-            K.set_tuning(8, chunk)
-            a, lp = _gauss(obs, w, b, log_std, seed)
-            assert torch.equal(a, want_a) and torch.equal(lp, want_lp), ("plain", chunk)
-            for ce in (0, 1):
-                K.set_tuning(22, ce)
-                a, lp = _gauss(obs, w, b, log_std, seed, staged=True)
-                assert torch.equal(a, want_a) and torch.equal(lp, want_lp), ("staged", chunk, ce)
-    finally:
-        K.set_tuning(8, SHIPPED_CHUNK)
-        K.set_tuning(22, 0)
+    for chunk in (256, 512, SHIPPED_CHUNK):
+        for ce in (None, 0, 1):      # plain, then staged pulled by kernel and by copy engine
+            with tuning(chunk, ce):
+                a, lp = _gauss(obs, w, b, log_std, seed, staged=ce is not None)
+            assert torch.equal(a, want_a) and torch.equal(lp, want_lp), (chunk, ce)
     for split in (1, 1000, 16896, 16900):
         a0, lp0 = _gauss(obs[:split], w, b, log_std, seed)
         a1, lp1 = _gauss(obs[split:], w, b, log_std, seed, row_offset=split)
@@ -224,52 +188,21 @@ def test_every_chunking_form_and_row_split_gives_identical_bits(K, d_out):
     assert not torch.equal(shifted[0], want_a)
 
 
-class _GaussianPushRig(_PolicyPushRig):
-    """_PolicyPushRig driving ktb_mlp_bf16_policy_gaussian_pushed; rank r's row_base is its shard's begin."""
-
-    def call(self, obs, w, b, d_out, log_std, seed, actions_ptr, log_probs_ptr):
-        L = _L()
-        self.seq += 1
-        seq, n, d_in, st = self.seq, self.n, self.d_in, _stream()
-        stage_ptrs = L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in self.stage[1:]])
-        ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
-        if self.engine == "sm":
-            L.call("ktb_push_scatter_chunked", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0, stage_ptrs,
-                   self.stride, ctrl_ptrs, self.ctrl[0].data_ptr(), self.chunk_rows * d_in, 0, seq, st)
-        else:
-            L.call("ktb_push_scatter_ce", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
-                   L.arr(ctypes.c_int, [0] * n), stage_ptrs, self.stride, ctrl_ptrs, self.ctrl[0].data_ptr(),
-                   self.chunk_rows * d_in, seq, st)
-        for r in range(1, n):
-            lo, hi = self.bounds[r]
-            L.call("ktb_mlp_bf16_policy_gaussian_pushed", 0, self.stage[r].ptr(), self.stride, hi - lo, d_in,
-                   self.d_hidden, d_out, w[0].data_ptr(), _ptr(b[0]), w[1].data_ptr(), _ptr(b[1]), w[2].data_ptr(),
-                   _ptr(b[2]), log_std.data_ptr(), seed, lo, actions_ptr + lo * d_out * 4, log_probs_ptr + lo * 4,
-                   self.scratch[r].ptr(), self.ctrl[r].data_ptr(), self.ctrl[0].data_ptr(), r, self.chunk_rows, seq, st)
-        lo, hi = self.bounds[0]
-        scratch = _mlp()._scratch_for(0, hi - lo, self.d_hidden)
-        L.call("ktb_mlp_bf16_policy_gaussian", 0, obs.data_ptr() + lo * d_in * 2, hi - lo, d_in, self.d_hidden, d_out,
-               w[0].data_ptr(), _ptr(b[0]), w[1].data_ptr(), _ptr(b[1]), w[2].data_ptr(), _ptr(b[2]),
-               log_std.data_ptr(), seed, lo, actions_ptr + lo * d_out * 4, log_probs_ptr + lo * 4, scratch.data_ptr(),
-               0, st)
-        L.call("ktb_push_wait", 0, self.ctrl[0].data_ptr(), n, 0, seq, st)
-
-
 @pytest.mark.parametrize("engine", ["sm", "ce"])
 def test_pushed_form_on_one_gpu_matches_plain_bits(K, engine):
     """ktb_mlp_bf16_policy_gaussian_pushed fed by either scatter engine with ranks [0, 0, 0] on cuda:0, three
     consecutive calls with fresh observations: the actions and log-probabilities equal one plain call over all rows,
     bit for bit."""
     M, d_out, seed = 3 * 1408, 17, 2**40 + 3
-    w, b = _config(500, d_out)
+    w, b = config(500, d_out)
     log_std = _log_std(d_out)
-    rig = _GaussianPushRig(K, M, 256, 1024, 512, engine)
+    rig = PushRig(K, M, 256, 1024, 512, engine, GAUSSIAN)
     for it in range(3):
-        obs = _randn((M, 256), 501 + it)
+        obs = randn((M, 256), 501 + it)
         want_a, want_lp = _gauss(obs, w, b, log_std, seed)
         actions = torch.full((M, d_out), float("nan"), dtype=torch.float32, device="cuda")
         log_probs = torch.full((M,), float("nan"), dtype=torch.float32, device="cuda")
-        rig.call(obs, w, b, d_out, log_std, seed, actions.data_ptr(), log_probs.data_ptr())
+        rig.call(obs, w, b, {"actions": actions.data_ptr(), "log_probs": log_probs.data_ptr()}, seed, log_std)
         torch.cuda.synchronize()
         assert torch.equal(actions, want_a) and torch.equal(log_probs, want_lp), (engine, it)
     assert rig.statuses() == [0] * rig.n
@@ -278,15 +211,14 @@ def test_pushed_form_on_one_gpu_matches_plain_bits(K, engine):
 def test_package_push_path_on_one_gpu_matches_plain_bits(K):
     """mlp_scatter_gather's pushed form (a cached PushSession, copy-engine scatter, the root's shard on the side
     stream) with ranks [0, 0, 0] on cuda:0 and output="gaussian": equal to one plain call over all rows."""
-    mlp = _mlp()
     devs, rows, d_out, seed = [0, 0, 0], 35072, 6, 9
     M = 3 * rows
     bounds = [K.shard_bounds(M, 3, r) for r in range(3)]
-    w, b = _config(510, d_out)
+    w, b = config(510, d_out)
     log_std = _log_std(d_out)
     weights = {0: (*w, *b)}
     for it in range(2):
-        obs = _randn((M, 256), 511 + it)
+        obs = randn((M, 256), 511 + it)
         want_a, want_lp = _gauss(obs, w, b, log_std, seed)
         actions = torch.full((M, d_out), float("nan"), dtype=torch.float32, device="cuda")
         log_probs = torch.full((M,), float("nan"), dtype=torch.float32, device="cuda")
@@ -303,7 +235,7 @@ def test_nearby_seeds_draw_different_noise_and_not_the_gumbel_stream(K):
     seed are not the Gaussian transform of the Gumbel stream's uniforms at the same seed."""
     d_out = 6
     w, b = _zero_head(600, d_out)
-    obs = _randn((8192, 256), 601)
+    obs = randn((8192, 256), 601)
     zeros = torch.zeros(d_out, device="cuda")
     s = 123456789
     draws = [_gauss(obs, w, b, zeros, seed)[0] for seed in (s, s + 1, s + 2**32)]
@@ -319,8 +251,8 @@ def test_planted_nan_and_infinite_logits_touch_their_column_only(K):
     """NaN, +inf and -inf logits from b3 (columns 3, 5, 6): those action columns are NaN, +inf and -inf, every other
     column and every log-probability equal a call with a finite b3 bit for bit."""
     d_out = 9
-    w, b = _config(650, d_out)
-    obs = _randn((2000, 256), 651)
+    w, b = config(650, d_out)
+    obs = randn((2000, 256), 651)
     log_std = _log_std(d_out)
     want_a, want_lp = _gauss(obs, w, b, log_std, 44)
     b3 = b[2].clone()
@@ -336,8 +268,6 @@ def test_planted_nan_and_infinite_logits_touch_their_column_only(K):
 def test_overflowing_logits_touch_their_column_only(K):
     """Identity hidden layers pass non-negative observations through exactly; trigger units of 2^100 times W3 entries
     of ±2^100 overflow the head's accumulator to ±inf in columns 1 and 4 on every other row."""
-    from test_gpu_mlp import _identity
-
     d, d_out, M, big = 256, 6, 2048, 2.0 ** 100
     obs = torch.rand(M, d, generator=torch.Generator(device="cuda").manual_seed(7), device="cuda") * 0.5
     obs[:, 200:] = 0
@@ -347,7 +277,7 @@ def test_overflowing_logits_touch_their_column_only(K):
     rows = torch.arange(0, M, 2, device="cuda")
     obs[rows, 255] = big
     obs, w3 = obs.bfloat16(), w3.bfloat16()
-    w, b = (_identity(d), _identity(d), w3), (None, None, None)
+    w, b = (identity(d), identity(d), w3), (None, None, None)
     log_std = _log_std(d_out)
     y = _logits(obs, w, b)
     a, lp = _gauss(obs, w, b, log_std, 3)
@@ -370,8 +300,8 @@ def test_planted_nan_and_infinite_log_std(K):
     -inf; NaN at column 2: a NaN column and NaN log-probabilities; -inf at column 0 with +inf elsewhere: NaN
     log-probabilities (inf - inf), and the column equals the logits."""
     d_out, M, seed = 5, 3000, 81
-    w, b = _config(660, d_out)
-    obs = _randn((M, 256), 661)
+    w, b = config(660, d_out)
+    obs = randn((M, 256), 661)
     y = _logits(obs, w, b).float()
     z64 = _z64(seed, 0, M, d_out)
     base = _log_std(d_out)
@@ -397,15 +327,6 @@ def test_planted_nan_and_infinite_log_std(K):
 
 
 # ---- 7. guard bands --------------------------------------------------------------------------------------------------
-class _Offset4(_Guarded):
-    """A _Guarded buffer whose base is 4 bytes past an 8-byte boundary: float2 stores would be misaligned."""
-
-    def __init__(self, nbytes):
-        super().__init__(nbytes)
-        self.band += 4
-        self.raw = torch.full((self.nbytes + 2 * self.band,), self.FILL, dtype=torch.uint8, device="cuda")
-
-
 @pytest.mark.parametrize("form,M,chunk,d_out,offset", [
     ("plain", 1000, SHIPPED_CHUNK, 7, False), ("plain", 1000, 256, 18, True), ("plain", 1000, 256, 130, False),
     ("staged", 1408, 256, 17, False), ("staged", 1408, 256, 18, True), ("pushed", 3 * 1408, 256, 7, False),
@@ -415,118 +336,62 @@ def test_writes_stay_inside_actions_and_log_probs(K, form, M, chunk, d_out, offs
     """actions (M·d_out·4 bytes), log_probs (M·4), scratch and stage between guard bands; an odd d_out (scalar
     stores) and an even d_out with the actions base 4 bytes past an 8-byte boundary (the scalar fallback); a logits
     buffer passed to no one stays untouched; the results equal mlp_forward's bit for bit."""
-    L = _L()
-    d_in, d_hidden, seed = 256, 1024, 5
-    w, b = _config(700, d_out)
-    obs = _randn((M, d_in), 701)
+    seed = 5
+    w, b = config(700, d_out)
+    obs = randn((M, 256), 701)
     log_std = _log_std(d_out)
     want_a, want_lp = _gauss(obs, w, b, log_std, seed)
-    K.set_tuning(8, chunk)
-    try:
-        actions = (_Offset4 if offset else _Guarded)(M * d_out * 4)
-        assert (actions.ptr() % 8 == 4) == offset
-        log_probs, logits = _Guarded(M * 4), _Guarded(M * d_out * 2)
-        buffers = {"actions": actions, "log_probs": log_probs}
-        if form == "pushed":
-            rig = _GaussianPushRig(K, M, d_in, d_hidden, 512, "sm")
-            for _ in range(3):
-                rig.call(obs, w, b, d_out, log_std, seed, actions.ptr(), log_probs.ptr())
-            torch.cuda.synchronize()
-            assert rig.statuses() == [0] * rig.n
-            buffers.update({f"stage[{r}]": rig.stage[r] for r in range(1, rig.n)})
-            buffers.update({f"scratch[{r}]": rig.scratch[r] for r in range(1, rig.n)})
-        else:
-            scratch = _Guarded(L.load().ktb_mlp_scratch_bytes(M, d_hidden))
-            buffers["scratch"] = scratch
-            stage = 0
-            if form == "staged":
-                buffers["stage"] = _Guarded(L.load().ktb_mlp_stage_bytes(M, d_in))
-                stage = buffers["stage"].ptr()
-            L.call("ktb_mlp_bf16_policy_gaussian", 0, obs.data_ptr(), M, d_in, d_hidden, d_out, w[0].data_ptr(),
-                   b[0].data_ptr(), w[1].data_ptr(), b[1].data_ptr(), w[2].data_ptr(), b[2].data_ptr(),
-                   log_std.data_ptr(), seed, 0, actions.ptr(), log_probs.ptr(), scratch.ptr(), stage, _stream())
-        for name, buf in buffers.items():
-            buf.check(f"{form} M={M} chunk={chunk} d_out={d_out} offset={offset}: {name}")
-        assert bool((logits.view() == _Guarded.FILL).all()), "a logits buffer nobody was given changed"
-        assert torch.equal(actions.view(torch.float32).view(M, d_out), want_a)
-        assert torch.equal(log_probs.view(torch.float32), want_lp)
-    finally:
-        K.set_tuning(8, SHIPPED_CHUNK)
+    logits = Guarded(M * d_out * 2)
+    bufs = run_guarded(form, GAUSSIAN, K, chunk, obs, w, b, seed, log_std, offsets={"actions": 4 * offset})
+    assert (bufs["actions"].ptr() % 8 == 4) == offset
+    for name, buf in bufs.items():
+        buf.check(f"{form} M={M} chunk={chunk} d_out={d_out} offset={offset}: {name}")
+    assert bool((logits.view() == Guarded.FILL).all()), "a logits buffer nobody was given changed"
+    assert torch.equal(bufs["actions"].view(torch.float32).view(M, d_out), want_a)
+    assert torch.equal(bufs["log_probs"].view(torch.float32), want_lp)
 
 
 # ---- 8. status codes -------------------------------------------------------------------------------------------------
-def _arg_case(name):
-    L = _L()
-    w1, w2, w3 = (torch.zeros(s, dtype=torch.bfloat16, device="cuda") for s in ((1024, 256), (1024, 1024), (512, 1024)))
-    bias = torch.zeros(1024, dtype=torch.bfloat16, device="cuda")
-    obs = torch.zeros(2048, 256, dtype=torch.bfloat16, device="cuda")
-    act = torch.zeros(2048 * 512, dtype=torch.float32, device="cuda")
-    lp = torch.zeros(2048, dtype=torch.float32, device="cuda")
-    ls = torch.zeros(512, dtype=torch.float32, device="cuda")
-    scratch = torch.zeros(1 << 24, dtype=torch.uint8, device="cuda")
-    ctrl = torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda")
-    p = lambda t, off=0: t.data_ptr() + off   # noqa: E731
-
-    def plain(d_out=18, actions=None, log_probs=None, log_std=None):
-        return ("ktb_mlp_bf16_policy_gaussian", 0, p(obs), 256, 256, 1024, d_out, p(w1), p(bias), p(w2), p(bias),
-                p(w3), p(bias), p(ls) if log_std is None else log_std, 1, 0, p(act) if actions is None else actions,
-                p(lp) if log_probs is None else log_probs, p(scratch), 0, _stream())
-
-    def pushed(d_out=18, actions=None, log_probs=None, log_std=None):
-        return ("ktb_mlp_bf16_policy_gaussian_pushed", 0, p(scratch), 1 << 20, 256, 256, 1024, d_out, p(w1), p(bias),
-                p(w2), p(bias), p(w3), p(bias), p(ls) if log_std is None else log_std, 1, 0,
-                p(act) if actions is None else actions, p(lp) if log_probs is None else log_probs, p(scratch),
-                p(ctrl), p(ctrl), 1, 256, 1, _stream())
-
-    table = {
-        "null_actions": (plain(actions=0), L.ERR_ARG),
-        "null_log_probs": (plain(log_probs=0), L.ERR_ARG),
-        "null_log_std": (plain(log_std=0), L.ERR_ARG),
-        "misaligned_actions": (plain(actions=p(act, 2)), L.ERR_ARG),
-        "misaligned_log_probs": (plain(log_probs=p(lp, 2)), L.ERR_ARG),
-        "misaligned_log_std": (plain(log_std=p(ls, 1)), L.ERR_ARG),
-        "d_out_257": (plain(d_out=257), L.ERR_UNSUPPORTED),
-        "pushed_null_actions": (pushed(actions=0), L.ERR_ARG),
-        "pushed_null_log_probs": (pushed(log_probs=0), L.ERR_ARG),
-        "pushed_null_log_std": (pushed(log_std=0), L.ERR_ARG),
-        "pushed_misaligned_actions": (pushed(actions=p(act, 1)), L.ERR_ARG),
-        "pushed_misaligned_log_probs": (pushed(log_probs=p(lp, 1)), L.ERR_ARG),
-        "pushed_misaligned_log_std": (pushed(log_std=p(ls, 2)), L.ERR_ARG),
-        "pushed_d_out_257": (pushed(d_out=257), L.ERR_UNSUPPORTED),
-    }
-    return table[name]
+STATUS_CASES = {
+    "null_actions": (plain, dict(actions=0), L.ERR_ARG),
+    "null_log_probs": (plain, dict(log_probs=0), L.ERR_ARG),
+    "null_log_std": (plain, dict(log_std=0), L.ERR_ARG),
+    "misaligned_actions": (plain, dict(actions_off=2), L.ERR_ARG),
+    "misaligned_log_probs": (plain, dict(log_probs_off=2), L.ERR_ARG),
+    "misaligned_log_std": (plain, dict(log_std_off=1), L.ERR_ARG),
+    "d_out_257": (plain, dict(d_out=257), L.ERR_UNSUPPORTED),
+    "pushed_null_actions": (pushed, dict(actions=0), L.ERR_ARG),
+    "pushed_null_log_probs": (pushed, dict(log_probs=0), L.ERR_ARG),
+    "pushed_null_log_std": (pushed, dict(log_std=0), L.ERR_ARG),
+    "pushed_misaligned_actions": (pushed, dict(actions_off=1), L.ERR_ARG),
+    "pushed_misaligned_log_probs": (pushed, dict(log_probs_off=1), L.ERR_ARG),
+    "pushed_misaligned_log_std": (pushed, dict(log_std_off=2), L.ERR_ARG),
+    "pushed_d_out_257": (pushed, dict(d_out=257), L.ERR_UNSUPPORTED),
+}
 
 
-@pytest.mark.parametrize("name", [
-    "null_actions", "null_log_probs", "null_log_std", "misaligned_actions", "misaligned_log_probs",
-    "misaligned_log_std", "d_out_257", "pushed_null_actions", "pushed_null_log_probs", "pushed_null_log_std",
-    "pushed_misaligned_actions", "pushed_misaligned_log_probs", "pushed_misaligned_log_std", "pushed_d_out_257",
-])
+@pytest.mark.parametrize("name", list(STATUS_CASES))
 def test_bad_arguments_get_the_documented_status(K, name):
-    L = _L()
-    args, status = _arg_case(name)
-    with pytest.raises(L.KtbError) as ei:
-        L.call(*args)
-    assert ei.value.status == status, (name, str(ei.value))
-    torch.cuda.synchronize()    # nothing was launched; the device stays healthy
+    form, overrides, status = STATUS_CASES[name]
+    expect_status(form(GAUSSIAN, **overrides), status)
 
 
 def test_python_checks_reach_mlp_forward(K):
-    (w1, w2, w3), b = _config(800, 18)
-    obs = _randn((256, 256), 801)
+    (w1, w2, w3), b = config(800, 18)
+    obs = randn((256, 256), 801)
     ls = torch.zeros(18, device="cuda")
     for bad in (None, -1, 2**64, True, 1.0):
         with pytest.raises(ValueError):
-            _mlp().mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=bad, log_std=ls)
+            mlp.mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=bad, log_std=ls)
     for bad in (None, torch.zeros(18), torch.zeros(17, device="cuda"), torch.zeros(18, device="cuda").double(),
                 torch.zeros(36, device="cuda")[::2]):
         with pytest.raises(ValueError):
-            _mlp().mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=1, log_std=bad)
+            mlp.mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=1, log_std=bad)
     with pytest.raises(ValueError):
-        _mlp().mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=1, log_std=ls, row_offset=-1)
+        mlp.mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=1, log_std=ls, row_offset=-1)
     with pytest.raises(ValueError):
-        _mlp().mlp_forward(obs, w1, w2, w3, biases=b, output="sample", seed=1, log_std=ls)
-    a, lp = _mlp().mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=1, log_std=ls)
+        mlp.mlp_forward(obs, w1, w2, w3, biases=b, output="sample", seed=1, log_std=ls)
+    a, lp = mlp.mlp_forward(obs, w1, w2, w3, biases=b, output="gaussian", seed=1, log_std=ls)
     assert a.shape == (256, 18) and lp.shape == (256,)
 
 
@@ -537,32 +402,25 @@ def test_mapped_gaussian_through_public_api(K, golden, case):
     ranks on cuda:0, against the oracle's run of the body: each rank's draws satisfy the bars over its rows' global
     indices, and agree with the body's actions within the action bar wherever the body's bf16 logits equal the
     kernel's."""
-    import kubetorch_b200 as kt
-
     if case == "recorded":
         obs, d_out = golden["all_inputs"]["mlp_obs"], 64
     else:
         rows = 1000 if case.startswith("ragged") else 2
         obs, d_out = torch.randn(rows, 256, generator=torch.Generator().manual_seed(rows)).bfloat16(), 6
-    p = _policy_weights(golden, d_out)
+    p = policy_weights(golden, d_out)
     log_std = torch.linspace(-3, 1, d_out)
     n_ranks, seed = 3, 2**35 + 17
     want = ref_dispatch.spmd_call(policy_gaussian_cases.mlp_policy_gaussian, obs, *p, log_std, seed,
                                   num_proc=n_ranks, serialization="pickle")
     policy = mapped_copy(policy_gaussian_cases.mlp_policy_gaussian, "mlp", bias=True, output="gaussian", seed="seed",
                          log_std="log_std")
-    remote = kt.fn(policy, name=f"t-gaussian-{case}").to(
-        kt.Compute(gpus=1, allowed_serialization=["json", "pickle"]).distribute(
-            "b200", workers=1, num_proc=n_ranks, devices=[0] * n_ranks))
-    try:
+    with deployed(policy, f"t-gaussian-{case}", [0] * n_ranks) as remote:
         pc = [t.cuda() for t in p]
         lsc = log_std.cuda()
         got = remote(obs.cuda(), *pc, lsc, seed, serialization="pickle")
         torch.cuda.synchronize()
         assert len(got) == len(want) == n_ranks
-        y = _mlp().mlp_forward(obs.cuda(), pc[0], pc[2], pc[4], biases=(pc[1], pc[3], pc[5]))
-        from policy_cases import mlp_policy_biased
-
+        y = mlp.mlp_forward(obs.cuda(), pc[0], pc[2], pc[4], biases=(pc[1], pc[3], pc[5]))
         same, total = 0, 0
         for r, (g, h) in enumerate(zip(got, want)):
             lo, hi = K.shard_bounds(obs.shape[0], n_ranks, r)
@@ -582,34 +440,25 @@ def test_mapped_gaussian_through_public_api(K, golden, case):
             same += int(eq.sum())
             total += eq.numel()
         print(f"{case}: the body's logits equal the kernel's on {same} of {total} elements")
-    finally:
-        remote.teardown()
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")
 @pytest.mark.parametrize("transfer", ["pull", "push"])
 def test_mapped_gaussian_on_two_gpus(K, golden, transfer):
     """Two ranks on two GPUs, staged pull and pushed form: the same bits as one plain call over all rows."""
-    import kubetorch_b200 as kt
-
     obs = torch.randn(2 * 1408, 256, generator=torch.Generator().manual_seed(5)).bfloat16()
-    p = _policy_weights(golden, 18)
+    p = policy_weights(golden, 18)
     log_std = torch.linspace(-2, 0.5, 18)
     seed = 4242
     policy = mapped_copy(policy_gaussian_cases.mlp_policy_gaussian, "mlp", bias=True, output="gaussian", seed="seed",
                          log_std="log_std")
-    remote = kt.fn(policy, name=f"t-gaussian-2gpu-{transfer}").to(
-        kt.Compute(gpus=2, allowed_serialization=["json", "pickle"]).distribute(
-            "b200", workers=1, num_proc=2, devices=[0, 1], transfer=transfer))
-    try:
+    with deployed(policy, f"t-gaussian-2gpu-{transfer}", [0, 1], transfer=transfer) as remote:
         pc = [t.cuda(0) for t in p]
         lsc = log_std.cuda(0)
         got = remote(obs.cuda(0), *pc, lsc, seed, serialization="pickle")
         torch.cuda.synchronize(0)
         torch.cuda.synchronize(1)
-        want_a, want_lp = _mlp().mlp_forward(obs.cuda(0), pc[0], pc[2], pc[4], biases=(pc[1], pc[3], pc[5]),
-                                             output="gaussian", seed=seed, log_std=lsc)
+        want_a, want_lp = mlp.mlp_forward(obs.cuda(0), pc[0], pc[2], pc[4], biases=(pc[1], pc[3], pc[5]),
+                                          output="gaussian", seed=seed, log_std=lsc)
         assert torch.equal(torch.cat([g[0].cpu() for g in got]), want_a.cpu())
         assert torch.equal(torch.cat([g[1].cpu() for g in got]), want_lp.cpu())
-    finally:
-        remote.teardown()
