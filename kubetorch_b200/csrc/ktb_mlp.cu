@@ -8,15 +8,16 @@
 //     into a STAGES-deep ring guarded by mbarriers (full: TMA bytes landed, empty: consumers done),
 //   * wgmma.mma_async m64nNk16 (bf16 x bf16 → fp32) issued by two consumer warpgroups, each owning
 //     64 rows of the 128-row tile, both operands read straight from shared memory by descriptor,
-//   * an epilogue from the fp32 register accumulators: optional bias (nn.Linear), fused ReLU + bf16
-//     rounding, global stores masked to the head's width, and optionally the greedy action of every
-//     row, or instead an action sampled by seeded Gumbel-max with its log-probability — the last
-//     layer's outputs may be peer pointers into the root GPU's result arena, which fuses the gather
-//     into the epilogue.
+//   * an epilogue from the fp32 register accumulators, chosen at compile time by HeadKind: optional
+//     bias (nn.Linear) and bf16 rounding, then for the hidden layers ReLU and full-tile stores, and
+//     for the head one of: logits masked to its width and/or the greedy action of every row; an
+//     action sampled by seeded Gumbel-max with its log-probability; or Gaussian actions with their
+//     log-probability — the head's outputs may be peer pointers into the root GPU's result arena,
+//     which fuses the gather into the epilogue.
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one lane).
 // Activations are rounded to bf16 between layers (like the eager torch module); rows are processed
-// in chunks whose hidden activations stay resident in the 50 MB L2.  One kernel
-// (mlp_layer_wgmma_kernel) runs every layer of every entry point.
+// in chunks whose hidden activations stay resident in the 50 MB L2.  One kernel template
+// (mlp_layer_wgmma_kernel<BLOCK_N, STAGES, HeadKind>) runs every layer of every entry point.
 #include "ktb_common.cuh"
 
 #include <cuda.h>
@@ -228,9 +229,11 @@ __device__ __forceinline__ float gumbel_of(uint32_t x) {
 }
 
 // One column pair (col, col + 1) of a layer in rows r and r + 8: y0 = act(a0 + bias, a1 + bias) of row r, y1 of row
-// r + 8, each rounded once to bf16.  A column >= n_valid gets no bias.
+// r + 8, each rounded once to bf16; act is ReLU in the hidden layers and the identity in the head.  A column >= n_valid
+// gets no bias.
+template <bool RELU>
 __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a3, const __nv_bfloat16* bias, int col,
-                                           int n_valid, int relu, __nv_bfloat162& y0, __nv_bfloat162& y1) {
+                                           int n_valid, __nv_bfloat162& y0, __nv_bfloat162& y1) {
   float v[4] = {a0, a1, a2, a3};
   // no add at all without a bias: -0.0 accumulators stay -0.0 (adding 0 would make them +0.0).  (The bias is read
   // here rather than before the main loop: 64 more live registers would make the 256-wide instantiation spill.)
@@ -244,7 +247,7 @@ __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a
       }
     }
   }
-  if (relu) {
+  if constexpr (RELU) {
 #pragma unroll
     for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
   }
@@ -252,16 +255,101 @@ __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a
   y1 = __floats2bfloat162_rn(v[2], v[3]);
 }
 
-// The sampling epilogue of a head tile (mlp_layer_wgmma_kernel with log_probs): rows r = row and row + 8 of the
-// thread, global rows row_base + r.  A loop of its own, so that the greedy loop keeps its compact code.  Pass 1 rounds
-// the logits once and keeps them as bf16 pairs (half the registers of the fp32 accumulators it frees: the 256-wide
-// instantiation would spill holding the accumulators, or the bias, through pass 2) and takes each row's largest logit
-// m across the quad (NaN skipped: it reaches the sum instead); pass 2 draws one Philox call per column pair < n_valid
-// and row, ranks fp32(logit + noise) in torch.argmax order and sums exp(logit - m) without a running rescale.  A logit equal to m adds 1 without an exp, so an all -inf (or a +inf) maximum never forms
-// exp(inf - inf): such rows end with a NaN log-probability, as in torch, and -inf logits beside a finite m add 0.
+// Every column of a tile stored in pairs, with no per-column masks or branches: the hidden layers (RELU; d_hidden is
+// a multiple of 256 and the scratch is 16-byte aligned, so every hidden tile is full and pair-aligned) and a greedy
+// head whose one tile is full and pair-aligned and that takes no actions.  C has n_valid columns.
+template <int BLOCK_N, bool RELU>
+__device__ __forceinline__ void store_tile(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias,
+                                           __nv_bfloat16* C, int col0, int n_valid, int row, bool st0, bool st1) {
+  __nv_bfloat16* p0 = C + (size_t)row * n_valid + col0;
+  __nv_bfloat16* p1 = p0 + (size_t)8 * n_valid;
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    __nv_bfloat162 y0, y1;
+    layer_pair<RELU>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col0 + 8 * j, n_valid, y0, y1);
+    if (st0) *reinterpret_cast<__nv_bfloat162*>(p0 + 8 * j) = y0;
+    if (st1) *reinterpret_cast<__nv_bfloat162*>(p1 + 8 * j) = y1;
+  }
+}
+
+// The greedy epilogue of a head tile: logits (C, unless null) masked to the head's n_valid columns over the TMA zero
+// fill, and actions[row] (unless null) the argmax of the row's ROUNDED logits.  The head's one tile holds whole rows
+// (n_valid <= BLOCK_N), so the argmax never leaves the CTA.
+template <int BLOCK_N>
+__device__ __forceinline__ void greedy_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias,
+                                                __nv_bfloat16* C, int64_t* actions, int col0, int n_valid, int row,
+                                                bool st0, bool st1) {
+  // a column pair is one 4-byte store where the base and an even row stride allow it; rows of an odd d_out are
+  // only 2-byte aligned and take scalar stores
+  const bool pairs = C != nullptr && (n_valid & 1) == 0 && ((uintptr_t)C & 3) == 0;
+  if (pairs && actions == nullptr && n_valid == BLOCK_N) {
+    store_tile<BLOCK_N, false>(acc, bias, C, col0, n_valid, row, st0, st1);
+    return;
+  }
+  float best[2] = {-INFINITY, -INFINITY};
+  int best_col[2] = {INT_MAX, INT_MAX};
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    __nv_bfloat162 y0, y1;
+    layer_pair<false>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, y0, y1);
+    if (C != nullptr) {
+      __nv_bfloat16* p0 = C + (size_t)row * n_valid + col;
+      __nv_bfloat16* p1 = p0 + (size_t)8 * n_valid;
+      if (pairs && col + 1 < n_valid) {
+        if (st0) *reinterpret_cast<__nv_bfloat162*>(p0) = y0;
+        if (st1) *reinterpret_cast<__nv_bfloat162*>(p1) = y1;
+      } else {
+        if (st0 && col < n_valid) p0[0] = y0.x;
+        if (st1 && col < n_valid) p1[0] = y1.x;
+        if (st0 && col + 1 < n_valid) p0[1] = y0.y;
+        if (st1 && col + 1 < n_valid) p1[1] = y1.y;
+      }
+    }
+    if (actions != nullptr) {
+      const float r[4] = {__low2float(y0), __high2float(y0), __low2float(y1), __high2float(y1)};
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int h = q >> 1, c = col + (q & 1);
+        if (c < n_valid && argmax_before(r[q], c, best[h], best_col[h])) {
+          best[h] = r[q];
+          best_col[h] = c;
+        }
+      }
+    }
+  }
+  if (actions != nullptr) {
+    // the 4 lanes of a quad hold the columns of the same two rows
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
+        const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
+        if (argmax_before(ov, oc, best[h], best_col[h])) {
+          best[h] = ov;
+          best_col[h] = oc;
+        }
+      }
+    }
+    if ((threadIdx.x & 3) == 0) {
+      if (st0) actions[row] = best_col[0];
+      if (st1) actions[row + 8] = best_col[1];
+    }
+  }
+}
+
+// The sampling epilogue of a head tile (HeadKind::kSample): rows r = row and row + 8 of the thread, global rows
+// row_base + r.  Pass 1 rounds the logits once and keeps them as bf16 pairs (half the registers of the fp32
+// accumulators it frees: the 256-wide instantiation would spill holding the accumulators, or the bias, through pass 2)
+// and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum instead); pass 2 draws one
+// Philox call per column pair < n_valid and row, ranks fp32(logit + noise) in torch.argmax order and sums
+// exp(logit - m) without a running rescale.  A logit equal to m adds 1 without an exp, so an all -inf (or a +inf)
+// maximum never forms exp(inf - inf): such rows end with a NaN log-probability, as in torch, and -inf logits beside a
+// finite m add 0.
 template <int BLOCK_N>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
-                                                int n_valid, int relu, int row, bool st0, bool st1, int64_t* actions,
+                                                int n_valid, int row, bool st0, bool st1, int64_t* actions,
                                                 float* log_probs, uint64_t seed, uint64_t row_base) {
   float mx[2] = {-INFINITY, -INFINITY};
   __nv_bfloat162 y[BLOCK_N / 4];   // y[2j + h]: columns (col, col + 1) of row + 8h
@@ -269,8 +357,8 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
     if (col >= n_valid) continue;
-    layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, relu, y[2 * j],
-               y[2 * j + 1]);
+    layer_pair<false>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, y[2 * j],
+                      y[2 * j + 1]);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       const float v = q & 1 ? __high2float(y[2 * j + (q >> 1)]) : __low2float(y[2 * j + (q >> 1)]);
@@ -337,25 +425,19 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   }
 }
 
-// The Gaussian epilogue of a head tile (mlp_layer_wgmma_kernel with log_std): rows r = row and row + 8 of the thread,
-// global rows row_base + r.  A compact loop of its own, apart from the greedy loop and sample_epilogue: fully unrolled
-// here (as those are) it made the kernel half as large again, and ptxas then scheduled sample_epilogue differently and
-// 3-9 % slower.  So the unrolled part only rounds the logits once (layer_pair: μ, the value ktb_mlp_bf16_policy
-// stores) and parks them as bf16 pairs in the TMA ring, each warp in the 16 A rows of every stage that only its own
-// accumulator rows are made of: once the warp's wgmmas are waited for nothing reads or writes them again (every load
-// has landed, and no other warp's wgmma reads those rows).  A rolled loop then makes one pass over the column pairs
-// < n_valid: one Philox call per pair and row (counter word 3 = 1: never the Gumbel stream's uniforms),
-// z = Φ⁻¹(u) (normcdfinvf, no fast-math; u is never 0.5, so z != 0), the action μ + σ·z rounded twice (no FMA
-// contraction), stored as float2 where the row stride and the base allow and as scalars otherwise, and
-// Σ (0.5·z² + log_std) per row for the log-probability, which does not read μ.
+// The Gaussian epilogue of a head tile (HeadKind::kGaussian): rows r = row and row + 8 of the thread, global rows
+// row_base + r.  Only its first part is unrolled over the accumulators, so that the Philox and Φ⁻¹ code is not repeated
+// BLOCK_N / 8 times: it rounds the logits once (layer_pair: μ, the value ktb_mlp_bf16_policy stores) and parks them as
+// bf16 pairs in the TMA ring, each warp in the 16 A rows of every stage that only its own accumulator rows are made of:
+// once the warp's wgmmas are waited for nothing reads or writes them again (every load has landed, and no other warp's
+// wgmma reads those rows).  A rolled loop then makes one pass over the column pairs < n_valid: one Philox call per pair
+// and row (counter word 3 = 1: never the Gumbel stream's uniforms), z = Φ⁻¹(u) (normcdfinvf, no fast-math; u is never
+// 0.5, so z != 0), the action μ + σ·z rounded twice (no FMA contraction), stored as float2 where the row stride and the
+// base allow and as scalars otherwise, and Σ (0.5·z² + log_std) per row for the log-probability, which does not read μ.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
-                                                  int n_valid, int relu, int row, bool st0, bool st1,
-                                                  const float* log_std, float* actions, float* log_probs,
-                                                  uint64_t seed, uint64_t row_base) {
-  // opaque copies of the inputs this epilogue shares with the others: without them the compiler hoists the common
-  // index and address arithmetic above the mode branch, and ptxas schedules sample_epilogue 2-3 % slower
-  asm volatile("" : "+l"(seed), "+l"(row_base), "+l"(bias), "+r"(col0), "+r"(n_valid), "+r"(row));
+                                                  int n_valid, int row, bool st0, bool st1, const float* log_std,
+                                                  float* actions, float* log_probs, uint64_t seed, uint64_t row_base) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -367,8 +449,8 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
     if (col >= n_valid) continue;
-    layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, relu, *slot(2 * j),
-               *slot(2 * j + 1));
+    layer_pair<false>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, *slot(2 * j),
+                      *slot(2 * j + 1));
   }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const bool pairs = (n_valid & 1) == 0 && ((uintptr_t)actions & 7) == 0;
@@ -416,27 +498,56 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
   }
 }
 
-// One MLP layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid, with the bias added to the fp32
-// accumulator and the sum rounded once to bf16 (nn.Linear / F.linear), and actions[row] = the argmax of the row's
-// ROUNDED values.  One output tile per CTA; blockIdx.x walks N, so the CTAs of one 128-row block run side by side and
-// read their A tile from L2 once.  Only rows < rows (A's row count) are stored.  Bias, ReLU and both outputs are
-// runtime choices (bias, C and actions may each be null), so one instantiation per tile width serves every layer:
-// 256 for the hidden layers, and for the head the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one
-// CTA owns whole rows (gridDim.x == 1, required with actions) and the argmax never leaves it.  Columns >= n_valid
-// hold TMA zero fill: they are never stored and never an action.
-// With log_probs (and actions; C is then null) the head SAMPLES instead (Gumbel-max): the action of global row
-// i = row_base + row is the argmax of fp32(logit_j + g_j) with g_j the Gumbel noise of Philox word j & 1 of counter
-// (i, j >> 1) under `seed` (include/ktb200.h), and log_probs[row] = log_softmax(logits)[action] in fp32.
-// With log_std (and gauss_actions and log_probs; C and actions are then null) the head draws Gaussian actions
-// instead: gauss_actions[row, j] = logit_j + exp(log_std_j)·z_j with z_j = Φ⁻¹(u) of Philox word j & 1 of counter
-// (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (include/ktb200.h).
-template <int BLOCK_N, int STAGES>
+// What a layer's epilogue computes: the hidden layers' activation, or the head each entry point names.
+enum class HeadKind {
+  kHidden,     // bf16 relu(A · Bᵀ + bias) of full tiles (layers 1 and 2)
+  kGreedy,     // bf16 logits and/or int64 argmax actions
+  kSample,     // Gumbel-max int64 actions and fp32 log_probs
+  kGaussian,   // fp32 actions [rows, d_out] (gauss_actions) drawn with log_std, and fp32 log_probs
+};
+
+// The outputs of a layer launch.  A hidden layer stores only its bf16 activation, in `logits`.  Pointers the head
+// kind does not store are null.  Row r of the launch draws the noise of global row row_base + r.
+struct HeadOut {
+  void* logits = nullptr;
+  int64_t* actions = nullptr;
+  float* log_probs = nullptr;
+  uint64_t seed = 0, row_base = 0;
+  const float* log_std = nullptr;
+  float* gauss_actions = nullptr;
+
+  // The same outputs from row r0 of the call on.
+  HeadOut from_row(size_t r0, int d_out) const {
+    HeadOut h = *this;
+    if (logits) h.logits = static_cast<__nv_bfloat16*>(logits) + r0 * d_out;
+    if (actions) h.actions += r0;
+    if (log_probs) h.log_probs += r0;
+    if (gauss_actions) h.gauss_actions += r0 * d_out;
+    h.row_base += r0;
+    return h;
+  }
+};
+
+// One MLP layer: C[:, col] = act(A · Bᵀ + bias[col]) for col < n_valid (C = out.logits, n_valid columns), with the
+// bias (unless null) added to the fp32 accumulator and the sum rounded once to bf16 (nn.Linear / F.linear).  One
+// output tile per CTA; blockIdx.x walks N, so the CTAs of one 128-row block run side by side and read their A tile from
+// L2 once.  Only rows < rows (A's row count) are stored.  KIND picks the epilogue at compile time:
+//   kHidden (BLOCK_N = 256): C = relu(...), every tile full (store_tile);
+//   kGreedy: logits and/or actions[row] = the argmax of the row's ROUNDED logits (greedy_epilogue);
+//   kSample: the action of global row i = row_base + row is the argmax of fp32(logit_j + g_j) with g_j the Gumbel
+//     noise of Philox word j & 1 of counter (i, j >> 1) under `seed` (include/ktb200.h), and log_probs[row] =
+//     log_softmax(logits)[action] in fp32 (sample_epilogue);
+//   kGaussian: gauss_actions[row, j] = logit_j + exp(log_std_j)·z_j with z_j = Φ⁻¹(u) of Philox word j & 1 of counter
+//     (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (gaussian_epilogue).
+// A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
+// (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
+// never an action.
+// `bias` is deliberately not __restrict__: with it the compiler reads the bias through the non-coherent cache in
+// batches ahead of the stores, and a biased hidden layer takes 3 % longer (H100 80GB HBM3, 700 W).
+template <int BLOCK_N, int STAGES, HeadKind KIND>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                           const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ C,
-                           int64_t* __restrict__ actions, float* __restrict__ log_probs, uint64_t seed,
-                           uint64_t row_base, const float* __restrict__ log_std, float* __restrict__ gauss_actions,
-                           int ldc, int n_valid, int K, int rows, int relu) {
+                           const __nv_bfloat16* bias, const HeadOut out, int n_valid, int K, int rows) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -449,82 +560,17 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   // accumulator layout of m64nNk16: acc[4j + 2h + c] is row 16*(warp%4) + lane/4 + 8h, column 8j + 2*(lane%4) + c
   const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const bool st0 = row < rows, st1 = row + 8 < rows;
-  if (log_std != nullptr) {
-    gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, relu, row, st0, st1, log_std, gauss_actions,
-                                       log_probs, seed, row_base);
-    return;
-  }
-  if (log_probs != nullptr) {
-    sample_epilogue<BLOCK_N>(acc, bias, col0, n_valid, relu, row, st0, st1, actions, log_probs, seed, row_base);
-    return;
-  }
-  // a column pair is one 4-byte store where the base and an even row stride allow it; rows of an odd d_out are
-  // only 2-byte aligned and take scalar stores
-  const bool pairs = C != nullptr && (ldc & 1) == 0 && ((uintptr_t)C & 3) == 0;
-  if (pairs && actions == nullptr && n0 + BLOCK_N <= n_valid) {
-    // every column of the tile is stored, in pairs, and no action is taken (every hidden-layer tile): the loop below
-    // without its per-column masks and branches
-    __nv_bfloat16* p0 = C + (size_t)row * ldc + col0;
-    __nv_bfloat16* p1 = p0 + (size_t)8 * ldc;
-#pragma unroll
-    for (int j = 0; j < BLOCK_N / 8; ++j) {
-      __nv_bfloat162 y0, y1;
-      layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col0 + 8 * j, n_valid, relu, y0, y1);
-      if (st0) *reinterpret_cast<__nv_bfloat162*>(p0 + 8 * j) = y0;
-      if (st1) *reinterpret_cast<__nv_bfloat162*>(p1 + 8 * j) = y1;
-    }
-    return;
-  }
-  float best[2] = {-INFINITY, -INFINITY};
-  int best_col[2] = {INT_MAX, INT_MAX};
-#pragma unroll
-  for (int j = 0; j < BLOCK_N / 8; ++j) {
-    const int col = col0 + 8 * j;
-    __nv_bfloat162 y0, y1;
-    layer_pair(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, relu, y0, y1);
-    if (C != nullptr) {
-      __nv_bfloat16* p0 = C + (size_t)row * ldc + col;
-      __nv_bfloat16* p1 = p0 + (size_t)8 * ldc;
-      if (pairs && col + 1 < n_valid) {
-        if (st0) *reinterpret_cast<__nv_bfloat162*>(p0) = y0;
-        if (st1) *reinterpret_cast<__nv_bfloat162*>(p1) = y1;
-      } else {
-        if (st0 && col < n_valid) p0[0] = y0.x;
-        if (st1 && col < n_valid) p1[0] = y1.x;
-        if (st0 && col + 1 < n_valid) p0[1] = y0.y;
-        if (st1 && col + 1 < n_valid) p1[1] = y1.y;
-      }
-    }
-    if (actions != nullptr) {
-      const float r[4] = {__low2float(y0), __high2float(y0), __low2float(y1), __high2float(y1)};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int h = q >> 1, c = col + (q & 1);
-        if (c < n_valid && argmax_before(r[q], c, best[h], best_col[h])) {
-          best[h] = r[q];
-          best_col[h] = c;
-        }
-      }
-    }
-  }
-  if (actions != nullptr) {
-    // the 4 lanes of a quad hold the columns of the same two rows
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-#pragma unroll
-      for (int m = 1; m <= 2; m <<= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
-        const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
-        if (argmax_before(ov, oc, best[h], best_col[h])) {
-          best[h] = ov;
-          best_col[h] = oc;
-        }
-      }
-    }
-    if ((lane & 3) == 0) {
-      if (st0) actions[row] = best_col[0];
-      if (st1) actions[row + 8] = best_col[1];
-    }
+  __nv_bfloat16* C = static_cast<__nv_bfloat16*>(out.logits);
+  if constexpr (KIND == HeadKind::kHidden) {
+    store_tile<BLOCK_N, true>(acc, bias, C, col0, n_valid, row, st0, st1);
+  } else if constexpr (KIND == HeadKind::kGreedy) {
+    greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, col0, n_valid, row, st0, st1);
+  } else if constexpr (KIND == HeadKind::kSample) {
+    sample_epilogue<BLOCK_N>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.seed,
+                             out.row_base);
+  } else {
+    gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
+                                       out.log_probs, out.seed, out.row_base);
   }
 }
 
@@ -607,38 +653,10 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
   return KTB_OK;
 }
 
-// What a policy head computes; each entry point names its own.
-enum class HeadKind {
-  kGreedy,     // bf16 logits and/or int64 argmax actions
-  kSample,     // Gumbel-max int64 actions and fp32 log_probs
-  kGaussian,   // fp32 actions [rows, d_out] (gauss_actions) drawn with log_std, and fp32 log_probs
-};
-
-// The outputs of a head launch; a hidden layer's launch passes an empty one.  Pointers the head kind does not store
-// are null.  Row r of the launch draws the noise of global row row_base + r.
-struct HeadOut {
-  void* logits = nullptr;
-  int64_t* actions = nullptr;
-  float* log_probs = nullptr;
-  uint64_t seed = 0, row_base = 0;
-  const float* log_std = nullptr;
-  float* gauss_actions = nullptr;
-
-  // The same outputs from row r0 of the call on.
-  HeadOut from_row(size_t r0, int d_out) const {
-    HeadOut h = *this;
-    if (logits) h.logits = static_cast<__nv_bfloat16*>(logits) + r0 * d_out;
-    if (actions) h.actions += r0;
-    if (log_probs) h.log_probs += r0;
-    if (gauss_actions) h.gauss_actions += r0 * d_out;
-    h.row_base += r0;
-    return h;
-  }
-};
-
-template <int BLOCK_N>
-static int launch_layer(int dev, const void* A, const void* B, const void* bias, void* C, const HeadOut& head,
-                        size_t M, int N, int K, int ldc, bool relu, cudaStream_t stream) {
+// One layer through the epilogue of KIND in BLOCK_N-wide tiles: out = A[M, K] · B[N, K]ᵀ (+ bias), N columns.
+template <int BLOCK_N, HeadKind KIND>
+static int launch_layer(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
+                        int K, cudaStream_t stream) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -646,17 +664,22 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   if (rc) return rc;
   rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, BLOCK_N);
   if (rc) return rc;
-  auto kfn = mlp_layer_wgmma_kernel<BLOCK_N, kMlpStages>;
+  auto kfn = mlp_layer_wgmma_kernel<BLOCK_N, kMlpStages, KIND>;
   static std::atomic<unsigned> attr_done{0};
   rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
-  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias),
-                                                static_cast<__nv_bfloat16*>(C), head.actions, head.log_probs,
-                                                head.seed, head.row_base, head.log_std, head.gauss_actions, ldc, N, K,
-                                                (int)M, relu);
+  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
+}
+
+// The head of KIND, in the smallest tile that holds its N = d_out columns.
+template <HeadKind KIND>
+static int launch_head(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
+                       int K, cudaStream_t stream) {
+  const auto launch = N <= 64 ? launch_layer<64, KIND> : N <= 128 ? launch_layer<128, KIND> : launch_layer<256, KIND>;
+  return launch(dev, A, B, bias, out, M, N, K, stream);
 }
 
 // Weights and biases (each bias may be null) of one MLP call, and its head.
@@ -671,14 +694,15 @@ struct MlpParams {
 // a1.
 static int mlp_chunk(int dev, const MlpParams& p, const void* a1, void* h1, void* h2, size_t r0, size_t rows, int d_in,
                      int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
-  int rc = launch_layer<256>(dev, a1, p.W1, p.b1, h1, HeadOut{}, rows, d_hidden, d_in, d_hidden, true, st);
+  int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
   if (rc) return rc;
   if (consumed) KTB_CK(cudaEventRecord(consumed, st));
-  rc = launch_layer<256>(dev, h1, p.W2, p.b2, h2, HeadOut{}, rows, d_hidden, d_hidden, d_hidden, true, st);
+  rc = launch_layer<256, HeadKind::kHidden>(dev, h1, p.W2, p.b2, HeadOut{h2}, rows, d_hidden, d_hidden, st);
   if (rc) return rc;
-  const HeadOut h = p.out.from_row(r0, d_out);
-  const auto head = d_out <= 64 ? launch_layer<64> : d_out <= 128 ? launch_layer<128> : launch_layer<256>;
-  return head(dev, h2, p.W3, p.b3, h.logits, h, rows, d_out, d_hidden, d_out, false, st);
+  const auto head = p.kind == HeadKind::kGreedy   ? launch_head<HeadKind::kGreedy>
+                    : p.kind == HeadKind::kSample ? launch_head<HeadKind::kSample>
+                                                  : launch_head<HeadKind::kGaussian>;
+  return head(dev, h2, p.W3, p.b3, p.out.from_row(r0, d_out), rows, d_out, d_hidden, st);
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -692,6 +716,8 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
   if (M > 0) {
     const HeadOut& o = p.out;
     switch (p.kind) {
+      case HeadKind::kHidden:   // the hidden layers' epilogue, never an entry point's head
+        break;
       case HeadKind::kGreedy:
         KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
         break;

@@ -35,25 +35,27 @@ def test_library_is_sm90a_only():
     assert archs == {"90a"}, archs
 
 
-def test_mlp_layer_kernel_issues_wgmma_and_tma_without_spills():
-    """One MLP layer kernel per tile width 64 / 128 / 256 (the 256-wide one runs every hidden layer, the head the
-    smallest that holds d_out), each feeding Hopper tensor cores from TMA-loaded shared memory: asynchronous warpgroup
-    MMAs (HGMMA) of its full tile width and 2-D TMA loads, with no local-memory traffic (a spill in the 256-wide
-    instantiation would slow every hidden layer).  No other kernel issues wgmma."""
+def test_mlp_layer_kernel_per_epilogue_issues_wgmma_and_tma_without_spills():
+    """One MLP layer kernel per (tile width, epilogue): the hidden layers' at 256, and each head kind (greedy, sample,
+    Gaussian) at 64 / 128 / 256, the smallest that holds d_out.  Each feeds Hopper tensor cores from TMA-loaded shared
+    memory: asynchronous warpgroup MMAs (HGMMA) of its full tile width and 2-D TMA loads, with no local-memory traffic
+    (a spill in the hidden instantiation would slow every hidden layer).  No other kernel issues wgmma."""
     import subprocess
 
+    kinds = {0: "hidden", 1: "greedy", 2: "sample", 3: "gaussian"}   # HeadKind in ktb_mlp.cu
     sass = subprocess.run(["cuobjdump", "-sass", L.lib_path()], capture_output=True, text=True).stdout
     funcs = sass.split("Function : ")[1:]
-    found = {}
+    found = []
     for f in funcs:
         name = f.split("\n", 1)[0]
         assert "HGMMA" not in f or "mlp_layer_wgmma_kernel" in name, name
         if "mlp_layer_wgmma_kernel" in name:
-            n = int(re.search(r"mlp_layer_wgmma_kernelILi(\d+)E", name).group(1))
+            n, kind = re.search(r"mlp_layer_wgmma_kernelILi(\d+)ELi\d+ELNS_8HeadKindE(\d)E", name).groups()
             assert f"HGMMA.64x{n}x16.F32.BF16" in f and "UTMALDG.2D" in f, name
             assert not re.search(r"\b(STL|LDL)\b", f), name
-            found[n] = found.get(n, 0) + 1
-    assert found == {64: 1, 128: 1, 256: 1}, found
+            found.append((kinds[int(kind)], int(n)))
+    want = [("hidden", 256)] + [(k, n) for k in ("greedy", "sample", "gaussian") for n in (64, 128, 256)]
+    assert sorted(found) == sorted(want), found
 
 
 @pytest.mark.parametrize("n,world", [(0, 1), (1, 4), (3, 4), (5, 4), (1003, 4), (1000, 3), (64, 8), (2**26, 8), (7, 7)])
