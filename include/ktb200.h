@@ -127,7 +127,10 @@ int ktb_shard_bounds(size_t n, int world, int rank, size_t* begin, size_t* end);
 /* dst[i] = op(src[i]) for i in [0, n_elems).  src/dst may be local, peer or mapped-host
  * pointers valid on `dev`; they must be element-aligned and must not partially overlap
  * (src == dst is allowed).  alpha/beta are converted to the dtype's op-math type
- * (float for F32/BF16, int64 for I32/I64).  KTB_U8 supports KTB_OP_IDENTITY only.
+ * (float for F32/BF16/F16, int64 for I32/I64).  For I32/I64 they must hold integers: the kernels take
+ * (long long)alpha and compute modulo 2^32 / 2^64, so pass the scalar reduced to that width's signed range,
+ * where it is exact in a double for I32 and, for I64, exact only when |value| <= 2^53 or otherwise representable.
+ * KTB_U8 supports KTB_OP_IDENTITY only.
  * KTB_VARIANT_TMA / _VEC need 16-byte aligned src and dst and silently use the next narrower
  * path otherwise (all variants are bit-identical). */
 int ktb_map(int dev, int op, int dtype, const void* src, void* dst, size_t n_elems,

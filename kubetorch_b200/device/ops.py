@@ -83,6 +83,38 @@ def dtype_code(dtype: torch.dtype) -> int:
         raise TypeError(f"kubetorch_b200 mapped ops support {sorted(str(k) for k in _DTYPE_CODES)}, got {dtype}")
 
 
+_INT_BITS = {torch.int32: 32, torch.int64: 64}
+
+
+def _int_scalar(name: str, v, dtype: torch.dtype) -> float:
+    """An integer alpha/beta of a `dtype` tensor as the double the C-ABI takes, exact or refused.  The kernels compute
+    modulo 2^32 (i32) or 2^64 (i64), so the scalar is first reduced to signed two's complement of that width, like
+    torch's own wrap; every i32 scalar is then exact in a double, an i64 one only when it is representable (every
+    |v| <= 2^53 is) — a rounded scalar would give wrong bits, so it is refused."""
+    if isinstance(v, float):
+        if not v.is_integer():
+            raise TypeError(f"{name}={v!r} on a {dtype} tensor is not an integer: torch would promote the result to "
+                            "floating point, which the integer kernels do not do")
+        v = int(v)
+    bits = _INT_BITS[dtype]
+    half = 1 << (bits - 1)
+    r = (int(v) + half) % (1 << bits) - half
+    f = float(r)
+    if int(f) != r:
+        raise TypeError(f"{name}={v!r} on a {dtype} tensor wraps to {r}, which a double does not hold exactly: int64 "
+                        "scalars must be exactly representable as a double (every |v| <= 2**53 is)")
+    return f
+
+
+def scalar_args(dtype: torch.dtype, alpha, beta) -> Tuple[float, float]:
+    """(alpha, beta) as the doubles every element-wise entry of the C-ABI takes for a `dtype` tensor: plain float()
+    for the float dtypes, _int_scalar() for int32/int64 (raises TypeError for a scalar the kernels cannot apply
+    exactly)."""
+    if dtype in _INT_BITS:
+        return _int_scalar("alpha", alpha, dtype), _int_scalar("beta", beta, dtype)
+    return float(alpha), float(beta)
+
+
 _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
 
 
@@ -150,49 +182,64 @@ def map_tensor(
         ensure_init({od})
         if out.dtype != x.dtype or out.numel() != x.numel():
             raise ValueError("out must match x in dtype and numel")
+    a, b = scalar_args(x.dtype, alpha, beta)
     L.call(
         "ktb_map", dev, OPS[op], dtype_code(x.dtype), x.data_ptr(), out.data_ptr(), x.numel(),
-        float(alpha), float(beta), int(variant), _stream(dev, stream),
+        a, b, int(variant), _stream(dev, stream),
     )
     return out
 
 
-def fast_dtype_codes(integral_params: bool) -> dict:
-    """dtype -> code for the small-call lane; integer dtypes only when alpha/beta are integral (torch would promote)."""
-    codes = dict(_DTYPE_CODES)
-    if not integral_params:
-        codes.pop(torch.int32, None)
-        codes.pop(torch.int64, None)
-    return codes
+def _scalars_by_code(alpha, beta) -> list:
+    """scalar_args(dtype, alpha, beta) of every dtype, indexed by dtype code; None where scalar_args refuses."""
+    by_code = [None] * (max(_DTYPE_CODES.values()) + 1)
+    for dtype, code in _DTYPE_CODES.items():
+        try:
+            by_code[code] = scalar_args(dtype, alpha, beta)
+        except TypeError:
+            pass
+    return by_code
 
 
-def fast_map(device: int, op: str, alpha: float, beta: float):
+def fast_dtype_codes(alpha, beta) -> dict:
+    """dtype -> code for the small-call lanes with these constant alpha/beta: the integer dtypes only when the scalars
+    apply to them exactly (scalar_args accepts them), so a refused scalar takes the general path and its TypeError."""
+    by_code = _scalars_by_code(alpha, beta)
+    return {dtype: code for dtype, code in _DTYPE_CODES.items() if by_code[code] is not None}
+
+
+def fast_map(device: int, op: str, alpha, beta):
     """launch(dtype_code, src_ptr, dst_ptr, n_elems): ONE ctypes hop into ktb_map on torch's current stream of
-    `device`, everything else pre-bound (no per-call marshalling of constants, no Python-level checks)."""
+    `device`, everything else pre-bound (no per-call marshalling of constants, no Python-level checks): the scalars of
+    every dtype are converted here, once.  Codes outside fast_dtype_codes(alpha, beta) are not launchable."""
     ensure_init({device})
     fn = L.load().ktb_map
     op_code, dev = OPS[op], int(device)
     raw = _raw_stream if _raw_stream is not None else (lambda d: torch.cuda.current_stream(d).cuda_stream)
     check = L.check
+    by_code = _scalars_by_code(alpha, beta)
 
     def launch(code, src, dst, n):
-        rc = fn(dev, op_code, code, src, dst, n, alpha, beta, 0, raw(dev))
+        a, b = by_code[code]
+        rc = fn(dev, op_code, code, src, dst, n, a, b, 0, raw(dev))
         if rc:
             check(rc)
 
     return launch
 
 
-def batch_map(device: int, op: str, alpha: float, beta: float):
+def batch_map(device: int, op: str, alpha, beta):
     """run(dtype_code, dtype, xs, sizes) -> tuple of outputs: n small calls out_i = op(x_i) in ONE segmented launch
     (ktb_map_batch), the outputs carved out of one fresh arena (256-byte aligned, so every output is a valid vector
-    target)."""
+    target).  The scalars are converted once per dtype, as in fast_map()."""
     ensure_init({device})
     fn = L.load().ktb_map_batch
     op_code, dev = OPS[op], int(device)
     raw = _raw_stream if _raw_stream is not None else (lambda d: torch.cuda.current_stream(d).cuda_stream)
+    by_code = _scalars_by_code(alpha, beta)
 
     def run(code, dtype, xs, sizes):
+        alpha, beta = by_code[code]
         n = len(xs)
         es = xs[0].element_size()
         align = 256 // es
@@ -254,9 +301,10 @@ def map_reduce_sum(
     if out is None:
         out = torch.empty(1, dtype=acc_dtype(x.dtype), device=f"cuda:{dev}")
     st = _stream(dev, stream)
+    a, b = scalar_args(x.dtype, alpha, beta)
     L.call(
-        "ktb_map_reduce_sum", dev, OPS[op], dtype_code(x.dtype), x.data_ptr(), x.numel(), float(alpha),
-        float(beta), out.data_ptr(), _workspace(dev, st).data_ptr(), st,
+        "ktb_map_reduce_sum", dev, OPS[op], dtype_code(x.dtype), x.data_ptr(), x.numel(), a, b, out.data_ptr(),
+        _workspace(dev, st).data_ptr(), st,
     )
     return out
 
@@ -338,7 +386,7 @@ class BatchPlan:
         self._src = L.arr(ctypes.c_void_p, [t.data_ptr() for t in xs])
         self._dst = L.arr(ctypes.c_void_p, [t.data_ptr() for t in outs])
         self._n_elems = L.arr(ctypes.c_size_t, [t.numel() for t in xs])
-        self._args = (OPS[op], dtype_code(xs[0].dtype), float(alpha), float(beta))
+        self._args = (OPS[op], dtype_code(xs[0].dtype), *scalar_args(xs[0].dtype, alpha, beta))
 
     def run(self, stream: Optional[torch.cuda.Stream] = None):
         op, dt, a, b = self._args
@@ -401,12 +449,13 @@ def map_batch(
         _check_dev_tensor(t, f"xs[{i}]")
         if t.dtype != dt:
             raise ValueError("map_batch needs one dtype per batch")
+    a, b = scalar_args(dt, alpha, beta)
     if outs is None:
         outs = [torch.empty_like(t) for t in xs]
     L.call(
         "ktb_map_batch", dev, OPS[op], dtype_code(dt), L.arr(ctypes.c_void_p, [t.data_ptr() for t in xs]),
         L.arr(ctypes.c_void_p, [t.data_ptr() for t in outs]), L.arr(ctypes.c_size_t, [t.numel() for t in xs]),
-        len(xs), float(alpha), float(beta), _stream(dev, stream),
+        len(xs), a, b, _stream(dev, stream),
     )
     return outs
 
@@ -454,12 +503,13 @@ def scatter_map_gather(
     dim 0; `granule` = elements per row, default from x_root's shape) from the root GPU over NVLink,
     applies op, and pushes it into out_root."""
     devs = _scatter_devices(x_root, devices, root_rank)
+    a, b = scalar_args(x_root.dtype, alpha, beta)
     if out_root is None:
         out_root = torch.empty_like(x_root)
     streams = [current_stream_handle(d) for d in devs]
     L.call(
         "ktb_scatter_map_gather", OPS[op], dtype_code(x_root.dtype), x_root.data_ptr(), out_root.data_ptr(),
-        x_root.numel(), int(granule or row_elems(x_root)), float(alpha), float(beta), len(devs), L.arr(ctypes.c_int, devs), root_rank, int(variant),
+        x_root.numel(), int(granule or row_elems(x_root)), a, b, len(devs), L.arr(ctypes.c_int, devs), root_rank, int(variant),
         L.arr(L.c_uintptr, streams),
     )
     return out_root
@@ -476,6 +526,7 @@ def scatter_map_reduce(
 ) -> Tuple[torch.Tensor, torch.Tensor]:
     """Gather-reduce variant. Returns (total[1], partials[n_ranks]) on the root GPU."""
     devs = _scatter_devices(x_root, devices, root_rank)
+    a, b = scalar_args(x_root.dtype, alpha, beta)
     adt = acc_dtype(x_root.dtype)
     partials = torch.zeros(len(devs), dtype=adt, device=x_root.device)
     total = torch.empty(1, dtype=adt, device=x_root.device)
@@ -483,8 +534,7 @@ def scatter_map_reduce(
     streams = [int(torch.cuda.current_stream(d).cuda_stream) for d in devs]
     L.call(
         "ktb_scatter_map_reduce", OPS[op], dtype_code(x_root.dtype), x_root.data_ptr(), x_root.numel(),
-        int(granule or row_elems(x_root)), float(alpha),
-        float(beta), len(devs), L.arr(ctypes.c_int, devs), root_rank, partials.data_ptr(), total.data_ptr(),
+        int(granule or row_elems(x_root)), a, b, len(devs), L.arr(ctypes.c_int, devs), root_rank, partials.data_ptr(), total.data_ptr(),
         L.arr(ctypes.c_void_p, [w.data_ptr() for w in wss]), L.arr(L.c_uintptr, streams),
     )
     return total, partials
@@ -612,6 +662,7 @@ class PushSession:
                 self._status_host[r:r + 1].copy_(self._status_dev[r], non_blocking=True)
 
     def call(self, x_root: torch.Tensor, out_root: torch.Tensor, op: str, alpha: float = 1.0, beta: float = 0.0):
+        alpha, beta = scalar_args(x_root.dtype, alpha, beta)   # before begin(): a refused scalar leaves no call open
         seq = self.begin()
         n, es = len(self.devices), x_root.element_size()
         gran = row_elems(x_root)
@@ -622,7 +673,7 @@ class PushSession:
         if own:
             side = self.fork()
             L.call("ktb_map", self.root, OPS[op], dt, x_root.data_ptr() + b * gran * es,
-                   out_root.data_ptr() + b * gran * es, (e - b) * gran, float(alpha), float(beta), L.VARIANT_AUTO,
+                   out_root.data_ptr() + b * gran * es, (e - b) * gran, alpha, beta, L.VARIANT_AUTO,
                    int(side.cuda_stream))
         L.call("ktb_push_scatter", self.root, x_root.data_ptr(), x_root.numel(), gran, dt, n, 0, self.stage_ptrs,
                self.stride, self.ctrl_ptrs, self.ctrl[0].data_ptr(), self.n_chunks, seq,
@@ -632,7 +683,7 @@ class PushSession:
             if (e - b) * gran * es > self.stride:
                 raise ValueError("shard larger than the session's staging buffers")
             L.call("ktb_push_consume", self.devices[r], OPS[op], dt, self.stage[r].data_ptr(), self.stride,
-                   out_root.data_ptr() + b * gran * es, (e - b) * gran, float(alpha), float(beta),
+                   out_root.data_ptr() + b * gran * es, (e - b) * gran, alpha, beta,
                    self.ctrl[r].data_ptr(), self.ctrl[0].data_ptr(), r, self.n_chunks, seq,
                    current_stream_handle(self.devices[r]))
         self.finish(seq, joined=own)
@@ -751,6 +802,7 @@ def map_host(
     elif out_host.is_cuda or not out_host.is_pinned():
         raise ValueError("out_host must be a pinned host tensor")
     ensure_init({device})
+    a, b = scalar_args(x_host.dtype, alpha, beta)
     key = (device, chunk_bytes)
     # one host-path call at a time per device: the staging buffers and the library's three copy/exec
     # streams are per-device (the PCIe link serialises them anyway)
@@ -766,7 +818,7 @@ def map_host(
             _stage_cache[key] = st
         L.call(
             "ktb_map_host", device, OPS[op], dtype_code(x_host.dtype), x_host.data_ptr(), out_host.data_ptr(),
-            x_host.numel(), float(alpha), float(beta), chunk_bytes, st[0].data_ptr(), st[1].data_ptr(),
+            x_host.numel(), a, b, chunk_bytes, st[0].data_ptr(), st[1].data_ptr(),
         )
     return out_host
 
@@ -797,6 +849,7 @@ def map_host_multi(
         out_host = torch.empty_like(x_host).pin_memory()
     devs = [int(d) for d in devices]
     ensure_init(set(devs))
+    a, b = scalar_args(x_host.dtype, alpha, beta)
     gran = row_elems(x_host)
     rows = x_host.numel() // gran
     shard_bytes = shard_bounds(rows, len(devs), 0)[1] * gran * x_host.element_size()
@@ -814,7 +867,7 @@ def map_host_multi(
             stages.append(st)
         L.call(
             "ktb_map_host_multi", OPS[op], dtype_code(x_host.dtype), x_host.data_ptr(), out_host.data_ptr(),
-            x_host.numel(), gran, float(alpha), float(beta), len(devs), L.arr(ctypes.c_int, devs), cb,
+            x_host.numel(), gran, a, b, len(devs), L.arr(ctypes.c_int, devs), cb,
             L.arr(ctypes.c_void_p, [s[0].data_ptr() for s in stages]),
             L.arr(ctypes.c_void_p, [s[1].data_ptr() for s in stages]),
         )

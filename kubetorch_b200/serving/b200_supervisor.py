@@ -281,14 +281,13 @@ class B200Supervisor:
             return None
         if len(inspect.signature(method).parameters) != 1 or self.ops is None or not hasattr(self.ops, "fast_map"):
             return None
-        integral = float(spec.alpha).is_integer() and float(spec.beta).is_integer()
         world, root, distributed = self.world_size, self.devices[0], self.distributed
         if self.placement == "ranks" and world > 1:
             return None                      # explicit spread placement: every call fans out, whatever its size
         spread_ok = self.placement == "auto" and world > 1 and len(set(self.devices)) == world
         small = self.SMALL_CALL_BYTES
-        launch = self.ops.fast_map(root, spec.op, float(spec.alpha), float(spec.beta))
-        codes = self.ops.fast_dtype_codes(integral)
+        launch = self.ops.fast_map(root, spec.op, spec.alpha, spec.beta)
+        codes = self.ops.fast_dtype_codes(spec.alpha, spec.beta)
         Tensor, empty_like = torch.Tensor, torch.empty_like
 
         def fast(x):
@@ -329,10 +328,9 @@ class B200Supervisor:
             return None
         if len(inspect.signature(method).parameters) != 1 or (self.placement == "ranks" and self.world_size > 1):
             return None
-        integral = float(spec.alpha).is_integer() and float(spec.beta).is_integer()
         world, root, distributed = self.world_size, self.devices[0], self.distributed
-        codes = self.ops.fast_dtype_codes(integral)
-        run = self.ops.batch_map(root, spec.op, float(spec.alpha), float(spec.beta))
+        codes = self.ops.fast_dtype_codes(spec.alpha, spec.beta)
+        run = self.ops.batch_map(root, spec.op, spec.alpha, spec.beta)
         small = self.SMALL_CALL_BYTES
         Tensor = torch.Tensor
 
@@ -430,9 +428,13 @@ class B200Supervisor:
         if not isinstance(x, torch.Tensor):
             raise TypeError(f"mapped callable '{name}' expects a torch.Tensor argument, got {type(x).__name__}")
         if str(x.dtype) in _INT_DTYPES and spec.op != "identity":
-            # the Python body (`x * 0.5`) would promote to float; the integer kernels do wrapping integer math only
-            for label, v in (("alpha", alpha), ("beta", beta if spec.op == "affine" else 0)):
-                if isinstance(v, float) and not v.is_integer() or not isinstance(v, (int, float)):
+            # the Python body (`x * 0.5`) would promote to float; the integer kernels do wrapping integer math only.  A
+            # float passed as a call argument is refused even when integral (`x * 2.0` is float32 in torch); a declared
+            # constant such as alpha=2.0 is checked against the body at deploy instead (_self_check)
+            for label, v, declared in (("alpha", alpha, spec.alpha),
+                                       ("beta", beta if spec.op == "affine" else 0, spec.beta)):
+                if isinstance(v, float) and (not v.is_integer() or isinstance(declared, str)) \
+                        or not isinstance(v, (int, float)):
                     raise TypeError(
                         f"mapped op '{spec.op}' on {x.dtype}: {label}={v!r} is not an integer — torch would promote "
                         "the result to floating point, which the integer kernels do not do")
