@@ -292,8 +292,9 @@ int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d
  * straight into `logits` (a peer pointer into the root's result: fused gather) and ack[rank] = seq is published in
  * the root's control block behind the last chunk.  Root NVLink egress carries posted writes only.
  * Requires M % 128 == 0 (a root routes other shards to the staged form), chunk_rows a positive multiple
- * of 128, ceil(M / chunk_rows) <= 64, M*d_in*2 <= stage_stride and stage_local, weights and scratch
- * 16-byte aligned (KTB_ERR_ARG otherwise); d_out == 64 (KTB_ERR_UNSUPPORTED otherwise).  `scratch`
+ * of 128, ceil(M / chunk_rows) <= 64, M*d_in*2 <= stage_stride, stage_stride % 16 == 0 (each call's half is
+ * 16-byte aligned) and stage_local, weights and scratch 16-byte aligned (KTB_ERR_ARG otherwise, before anything
+ * is enqueued); d_out == 64 (KTB_ERR_UNSUPPORTED otherwise).  `scratch`
  * holds 2*min(chunk_rows, M)*d_hidden bf16: it follows this call's chunk_rows, not the chunk of
  * ktb_mlp_scratch_bytes. */
 int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,

@@ -73,7 +73,7 @@ struct DeviceInfo {
   int sm_count = 0;
   cudaStream_t stream_h2d = nullptr, stream_exec = nullptr, stream_d2h = nullptr;  // ktb_map_host
   cudaStream_t stream_rank = nullptr;                                              // multi-GPU default
-  cudaEvent_t ev_a = nullptr, ev_b = nullptr;
+  cudaStream_t stream_stage = nullptr;                                             // staged MLP pulls
   cudaEvent_t host_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // ktb_map_host_multi
 };
 constexpr int kMaxDevices = 16;
@@ -386,7 +386,7 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_all() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
-// ---- in-kernel flag synchronisation of the push pipeline (ktb_push.cu, ktb_mlp.cu) ------------------------------
+// ---- in-kernel flag synchronisation of the push pipeline (ktb_push.cu) ------------------------------------------
 constexpr unsigned long long kSpinTimeoutNs = 10ull * 1000 * 1000 * 1000;  // 10 s
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -442,6 +442,11 @@ __device__ __forceinline__ bool spin_until(const unsigned long long* flag, unsig
 // (ktb_map.cu) enqueue dst = op(src) on the current device.
 int launch_map(int dev, int op, int dtype, const void* src, void* dst, size_t n_elems,
                const MapParams& p, int variant, cudaStream_t stream);
+// (ktb_push.cu) one warp that holds `stream` until *flag >= want (a timeout raises *status), and one that publishes
+// *flag = seq once everything before it on `stream` is visible system-wide.
+int launch_flag_wait(const unsigned long long* flag, unsigned long long want, unsigned int* status,
+                     cudaStream_t stream);
+int launch_flag_publish(unsigned long long* flag, unsigned long long seq, cudaStream_t stream);
 // (ktb_reduce.cu)
 int launch_map_reduce(int dev, int op, int dtype, const void* src, size_t n_elems, const MapParams& p,
                       void* out, void* workspace, cudaStream_t stream);

@@ -18,6 +18,10 @@
 // Activations are rounded to bf16 between layers (like the eager torch module); rows are processed
 // in chunks whose hidden activations stay resident in the 50 MB L2.  One kernel template
 // (mlp_layer_wgmma_kernel<BLOCK_N, STAGES, HeadKind>) runs every layer of every entry point.
+// On the host every entry point sits on two axes: its head (MlpParams: weights, biases, HeadKind and outputs) and its
+// form (MlpFeed: how each row chunk reaches layer 1 — read in place, pulled from a peer into `stage`, or pushed by the
+// root and waited for in-stream).  Each entry only builds the two and calls mlp_run, which checks them, then runs one
+// chunk loop over mlp_chunk (layer 1, layer 2, head).
 #include "ktb_common.cuh"
 
 #include <cuda.h>
@@ -682,11 +686,13 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
   return launch(dev, A, B, bias, out, M, N, K, stream);
 }
 
-// Weights and biases (each bias may be null) of one MLP call, and its head.
+// Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
+// and _pushed: no biases and a 64-wide greedy head that stores logits only.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
   HeadOut out;
+  bool logits64 = false;
 };
 
 // Rows [r0, r0 + rows) of a call: the hidden layers h1 = relu(a1 · W1ᵀ (+ b1)) and h2 = relu(h1 · W2ᵀ (+ b2)), then
@@ -744,42 +750,76 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
               KTB_ERR_ARG, "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
   return KTB_OK;
 }
-}  // namespace ktb
 
-using namespace ktb;
+// How the rows of each chunk of a call reach layer 1: the form of an entry point.
+//   plain : layer 1 reads the chunk in `in` (obs).
+//   staged: (stage != null) the chunk is pulled from `in` (obs on a peer) into half c & 1 of `stage` on the device's
+//           stage stream while the previous chunk computes, and layer 1 reads it there.
+//   pushed: the root pushes the rows into half seq & 1 of `in` (stage_local, halves `stride` bytes apart) and publishes
+//           ready[c] = seq in this rank's control block `ctrl`; layer 1 of chunk c waits in-stream for it, and the
+//           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.
+struct MlpFeed {
+  const void* in;
+  size_t chunk_rows;
+  void* stage = nullptr;
+  bool pushed = false;
+  size_t stride = 0;
+  void *ctrl = nullptr, *ctrl_root = nullptr;
+  int rank = 0;
+  unsigned long long seq = 0;
 
-extern "C" {
+  static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
+  static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
+                      unsigned long long seq) {
+    return {stage_local, chunk_rows, nullptr, true, stride, ctrl, ctrl_root, rank, seq};
+  }
+};
 
-size_t ktb_mlp_scratch_bytes(size_t M, int d_hidden) {
-  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
-  return 2 * rows * (size_t)d_hidden * 2;
-}
-
-size_t ktb_mlp_stage_bytes(size_t M, int d_in) {
-  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
-  return 2 * rows * (size_t)d_in * 2;
-}
-
-static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
-                   const MlpParams& p, void* scratch, void* stage, uintptr_t stream) {
+// One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
+// right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
+// ktb_push_wait waits for.
+static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
+                   const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
   if (rc) return rc;
-  if (M == 0) return KTB_OK;
-  KTB_REQUIRE(obs && p.W1 && p.W2 && p.W3 && scratch, KTB_ERR_ARG, "%s: null argument", fn);
-  rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, obs, scratch, stage);
+  if (M == 0 && !f.pushed) return KTB_OK;
+  if (p.logits64) {
+    KTB_REQUIRE(p.out.logits || M == 0, KTB_ERR_ARG, "%s: null argument", fn);
+    KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
+    KTB_REQUIRE(f.pushed || ((uintptr_t)p.out.logits & 15) == 0, KTB_ERR_ARG, "%s: logits must be 16-byte aligned",
+                fn);
+  }
+  KTB_REQUIRE(f.in && p.W1 && p.W2 && p.W3 && scratch && (!f.pushed || (f.ctrl && f.ctrl_root)), KTB_ERR_ARG,
+              "%s: null argument", fn);
+  if (f.pushed) {
+    KTB_REQUIRE(f.rank >= 0 && f.rank < 16 && f.seq > 0, KTB_ERR_ARG, "%s: bad rank/seq", fn);
+    KTB_REQUIRE(M % kMlpBlockM == 0, KTB_ERR_ARG, "%s: M=%zu must be a multiple of %d", fn, M, kMlpBlockM);
+  }
+  KTB_REQUIRE(f.chunk_rows > 0 && f.chunk_rows % kMlpBlockM == 0, KTB_ERR_ARG,
+              "%s: chunk_rows=%zu must be a positive multiple of %d", fn, f.chunk_rows, kMlpBlockM);
+  rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, f.in, scratch, f.stage);
   if (rc) return rc;
-  KTB_REQUIRE(g_mlp_chunk_rows % kMlpBlockM == 0 && g_mlp_chunk_rows > 0, KTB_ERR_ARG, "%s: bad chunk rows", fn);
+  if (f.pushed) {
+    const size_t n_chunks = (M + f.chunk_rows - 1) / f.chunk_rows;
+    KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: %zu chunks exceed %d", fn, n_chunks,
+                KTB_PUSH_MAX_CHUNKS);
+    KTB_REQUIRE(M * (size_t)d_in * 2 <= f.stride, KTB_ERR_ARG, "%s: shard exceeds stage_stride", fn);
+    // layer 1 reads half seq & 1 through a tensor map, whose base TMA needs 16-byte aligned
+    KTB_REQUIRE(f.stride % 16 == 0, KTB_ERR_ARG, "%s: stage_stride=%zu must be a multiple of 16", fn, f.stride);
+  }
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
-  DeviceInfo* di = device_info(dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  cudaStream_t side = di->stream_exec;   // pulls the next chunk while this one computes
-  const size_t chunk = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
+  const size_t chunk = std::min(f.chunk_rows, M);
   __nv_bfloat16* h1 = static_cast<__nv_bfloat16*>(scratch);
   __nv_bfloat16* h2 = h1 + chunk * (size_t)d_hidden;
-  const __nv_bfloat16* x = static_cast<const __nv_bfloat16*>(obs);
-  __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(stage);
+  // the call's rows: obs, or this call's staging half (the pull forms have seq = stride = 0)
+  const __nv_bfloat16* x =
+      reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride);
+  uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
+  __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
+  cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
   const MapParams ident = make_params(1, 0);
   // per-call events: [0] start, [1..2] staged chunk landed (by buffer), [3..4] staging buffer consumed
   cudaEvent_t evs[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -790,7 +830,7 @@ static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in,
         if (e[i]) cudaEventDestroy(e[i]);
     }
   } ev_guard{evs};
-  static std::mutex side_mu[kMaxDevices];   // the side stream of a device carries one staged call at a time
+  static std::mutex side_mu[kMaxDevices];   // the stage stream of a device carries one staged call at a time
   std::unique_lock<std::mutex> side_lock;
   if (stg) {
     side_lock = std::unique_lock<std::mutex>(side_mu[dev]);
@@ -802,7 +842,12 @@ static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in,
   for (size_t r0 = 0; r0 < M; r0 += chunk, ++c) {
     const size_t rows = std::min(chunk, M - r0);
     const __nv_bfloat16* a1 = x + r0 * d_in;
-    if (stg) {
+    if (f.pushed) {
+      // one warp spins until the root's ready[c] = seq (a timeout raises the sticky status)
+      rc = launch_flag_wait(reinterpret_cast<const unsigned long long*>(ctrl + KTB_CTRL_READY) + c, f.seq,
+                            reinterpret_cast<unsigned int*>(ctrl + KTB_CTRL_STATUS), st);
+      if (rc) return rc;
+    } else if (stg) {
       // staged pull: rows of this chunk travel peer → local ONCE (the layer-1 GEMM would otherwise fetch every
       // A tile d_hidden/256 times over NVLink, peer reads being uncached in the local L2)
       const int b = (int)(c & 1);
@@ -823,82 +868,56 @@ static int mlp_run(const char* fn, int dev, const void* obs, size_t M, int d_in,
     rc = mlp_chunk(dev, p, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
     if (rc) return rc;
   }
-  return KTB_OK;
-}
-
-// ---- pushed form: the root PUSHES this rank's observation rows chunk by chunk (ktb_push_scatter_chunked) ------------
-namespace ktb {
-// Stream-ordered "chunk c has landed": one warp spins on the local ready flag (a timeout raises the sticky status).
-__global__ void mlp_wait_ready_kernel(const unsigned long long* ready, unsigned long long seq, unsigned int* status) {
-  if (threadIdx.x == 0) (void)spin_until(ready, seq, status);
-}
-// Stream-ordered completion of the rank's call: everything before it on the stream (incl. the peer-stored logits)
-// is visible system-wide before the root sees ack[rank] = seq.
-__global__ void mlp_ack_kernel(unsigned long long* ack, unsigned long long seq) {
-  if (threadIdx.x == 0) {
-    __threadfence_system();
-    st_release_sys(ack, seq);
-  }
+  if (!f.pushed) return KTB_OK;
+  // everything before it on `st`, the peer-stored outputs included, is visible system-wide before the root sees
+  // ack[rank] = seq
+  return launch_flag_publish(
+      reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(f.ctrl_root) + KTB_CTRL_ACK) + f.rank, f.seq, st);
 }
 }  // namespace ktb
 
-static int mlp_pushed_run(const char* fn, int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
-                          int d_hidden, int d_out, const MlpParams& p, void* scratch, void* ctrl_local,
-                          void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
-  int rc = require_device(dev);
-  if (rc) return rc;
-  KTB_REQUIRE(stage_local && ctrl_local && ctrl_root_peer && p.W1 && p.W2 && p.W3 && scratch, KTB_ERR_ARG,
-              "%s: null argument", fn);
-  KTB_REQUIRE(rank >= 0 && rank < 16 && seq > 0, KTB_ERR_ARG, "%s: bad rank/seq", fn);
-  KTB_REQUIRE(M % kMlpBlockM == 0, KTB_ERR_ARG, "%s: M=%zu must be a multiple of %d", fn, M, kMlpBlockM);
-  KTB_REQUIRE(chunk_rows > 0 && chunk_rows % kMlpBlockM == 0, KTB_ERR_ARG,
-              "%s: chunk_rows=%zu must be a positive multiple of %d", fn, chunk_rows, kMlpBlockM);
-  rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, stage_local, scratch, nullptr);
-  if (rc) return rc;
-  const size_t n_chunks = (M + chunk_rows - 1) / chunk_rows;
-  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: %zu chunks exceed %d", fn, n_chunks,
-              KTB_PUSH_MAX_CHUNKS);
-  KTB_REQUIRE(M * (size_t)d_in * 2 <= stage_stride, KTB_ERR_ARG, "%s: shard exceeds stage_stride", fn);
-  rc = get_encoder();
-  if (rc) return rc;
-  KTB_GUARD(dev);
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  uint8_t* cl = static_cast<uint8_t*>(ctrl_local);
-  const unsigned long long* ready = reinterpret_cast<const unsigned long long*>(cl + KTB_CTRL_READY);
-  unsigned int* status = reinterpret_cast<unsigned int*>(cl + KTB_CTRL_STATUS);
-  unsigned long long* ack =
-      reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctrl_root_peer) + KTB_CTRL_ACK) + rank;
-  const __nv_bfloat16* x =
-      reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(stage_local) + (size_t)(seq & 1) * stage_stride);
-  __nv_bfloat16* h1 = static_cast<__nv_bfloat16*>(scratch);
-  __nv_bfloat16* h2 = h1 + std::min(chunk_rows, M) * (size_t)d_hidden;
-  size_t c = 0;
-  for (size_t r0 = 0; r0 < M; r0 += chunk_rows, ++c) {
-    const size_t rows = std::min(chunk_rows, M - r0);
-    mlp_wait_ready_kernel<<<1, 32, 0, st>>>(ready + c, seq, status);
-    KTB_CK(cudaGetLastError());
-    rc = mlp_chunk(dev, p, x + r0 * d_in, h1, h2, r0, rows, d_in, d_hidden, d_out, nullptr, st);
-    if (rc) return rc;
-  }
-  mlp_ack_kernel<<<1, 32, 0, st>>>(ack, seq);
-  KTB_CK(cudaGetLastError());
-  return KTB_OK;
+using namespace ktb;
+
+extern "C" {
+
+size_t ktb_mlp_scratch_bytes(size_t M, int d_hidden) {
+  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
+  return 2 * rows * (size_t)d_hidden * 2;
 }
 
-// ktb_mlp_bf16, _staged and _pushed are the policy form without biases, with a 64-wide head and logits only.  Each
-// checks that narrower contract (after the device, and for the pull forms after an empty call, which returns first)
-// and then runs the policy form.
+size_t ktb_mlp_stage_bytes(size_t M, int d_in) {
+  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
+  return 2 * rows * (size_t)d_in * 2;
+}
+
+int ktb_mlp_bf16(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                 const void* W2, const void* W3, void* logits, void* scratch, uintptr_t stream) {
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}, true};
+  return mlp_run("ktb_mlp_bf16", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, nullptr), scratch, stream);
+}
+
+int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                        const void* W2, const void* W3, void* logits, void* scratch, void* stage, uintptr_t stream) {
+  KTB_REQUIRE(stage, KTB_ERR_ARG, "ktb_mlp_bf16_staged: null stage buffer");
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}, true};
+  return mlp_run("ktb_mlp_bf16_staged", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs_peer, stage), scratch,
+                 stream);
+}
+
 int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_out,
                         const void* W1, const void* W2, const void* W3, void* logits, void* scratch, void* ctrl_local,
                         void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
-  const char* fn = "ktb_mlp_bf16_pushed";
-  int rc = require_device(dev);
-  if (rc) return rc;
-  KTB_REQUIRE(logits || M == 0, KTB_ERR_ARG, "%s: null argument", fn);
-  KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}};
-  return mlp_pushed_run(fn, dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p, scratch, ctrl_local,
-                        ctrl_root_peer, rank, chunk_rows, seq, stream);
+  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}, true};
+  return mlp_run("ktb_mlp_bf16_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                        const void* b1, const void* W2, const void* b2, const void* W3, const void* b3, void* logits,
+                        int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}};
+  return mlp_run("ktb_mlp_bf16_policy", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage), scratch, stream);
 }
 
 int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
@@ -907,39 +926,9 @@ int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_st
                                void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
                                unsigned long long seq, uintptr_t stream) {
   const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}};
-  return mlp_pushed_run("ktb_mlp_bf16_policy_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden, d_out, p,
-                        scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
-}
-
-static int mlp_run_64(const char* fn, int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
-                      const void* W1, const void* W2, const void* W3, void* logits, void* scratch, void* stage,
-                      uintptr_t stream) {
-  int rc = require_device(dev);
-  if (rc || M == 0) return rc;
-  KTB_REQUIRE(logits, KTB_ERR_ARG, "%s: null argument", fn);
-  KTB_REQUIRE(d_out == 64, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the 64-wide head)", fn, d_out);
-  KTB_REQUIRE(((uintptr_t)logits & 15) == 0, KTB_ERR_ARG, "%s: logits must be 16-byte aligned", fn);
-  const MlpParams p{W1, nullptr, W2, nullptr, W3, nullptr, HeadKind::kGreedy, {logits}};
-  return mlp_run(fn, dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
-}
-
-int ktb_mlp_bf16(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
-                 const void* W2, const void* W3, void* logits, void* scratch, uintptr_t stream) {
-  return mlp_run_64("ktb_mlp_bf16", dev, obs, M, d_in, d_hidden, d_out, W1, W2, W3, logits, scratch, nullptr, stream);
-}
-
-int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
-                        const void* W2, const void* W3, void* logits, void* scratch, void* stage, uintptr_t stream) {
-  KTB_REQUIRE(stage, KTB_ERR_ARG, "ktb_mlp_bf16_staged: null stage buffer");
-  return mlp_run_64("ktb_mlp_bf16_staged", dev, obs_peer, M, d_in, d_hidden, d_out, W1, W2, W3, logits, scratch, stage,
-                    stream);
-}
-
-int ktb_mlp_bf16_policy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
-                        const void* b1, const void* W2, const void* b2, const void* W3, const void* b3, void* logits,
-                        int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
-  const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}};
-  return mlp_run("ktb_mlp_bf16_policy", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  return mlp_run("ktb_mlp_bf16_policy_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
 }
 
 int ktb_mlp_bf16_policy_sample(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
@@ -947,7 +936,8 @@ int ktb_mlp_bf16_policy_sample(int dev, const void* obs, size_t M, int d_in, int
                                uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs, void* scratch,
                                void* stage, uintptr_t stream) {
   const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}};
-  return mlp_run("ktb_mlp_bf16_policy_sample", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  return mlp_run("ktb_mlp_bf16_policy_sample", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage), scratch,
+                 stream);
 }
 
 int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
@@ -957,8 +947,9 @@ int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t s
                                       void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
                                       uintptr_t stream) {
   const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}};
-  return mlp_pushed_run("ktb_mlp_bf16_policy_sample_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden, d_out,
-                        p, scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
+  return mlp_run("ktb_mlp_bf16_policy_sample_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
 }
 
 int ktb_mlp_bf16_policy_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
@@ -967,7 +958,8 @@ int ktb_mlp_bf16_policy_gaussian(int dev, const void* obs, size_t M, int d_in, i
                                  float* log_probs, void* scratch, void* stage, uintptr_t stream) {
   const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian,
                     {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}};
-  return mlp_run("ktb_mlp_bf16_policy_gaussian", dev, obs, M, d_in, d_hidden, d_out, p, scratch, stage, stream);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage), scratch,
+                 stream);
 }
 
 int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
@@ -978,9 +970,9 @@ int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t
                                         size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
   const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian,
                     {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}};
-  return mlp_pushed_run("ktb_mlp_bf16_policy_gaussian_pushed", dev, stage_local, stage_stride, M, d_in, d_hidden,
-                        d_out, p, scratch, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq, stream);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
 }
 
 }  // extern "C"
-

@@ -188,6 +188,31 @@ __global__ void push_wait_kernel(const unsigned long long* ack, int n_ranks, int
   if (r < n_ranks && r != root_rank) spin_until(&ack[r], seq, status);
 }
 
+// One flag per launch, stream-ordered: the copy-engine scatter's "rank consumed call seq-2" and "chunk landed", and the
+// pushed MLP's "chunk c landed" and "this rank's call is done" (ktb_mlp.cu).
+__global__ void flag_wait_kernel(const unsigned long long* flag, unsigned long long want, unsigned int* status) {
+  if (threadIdx.x == 0) (void)spin_until(flag, want, status);
+}
+__global__ void flag_publish_kernel(unsigned long long* flag, unsigned long long seq) {
+  if (threadIdx.x == 0) {
+    __threadfence_system();
+    st_release_sys(flag, seq);
+  }
+}
+
+int launch_flag_wait(const unsigned long long* flag, unsigned long long want, unsigned int* status,
+                     cudaStream_t stream) {
+  flag_wait_kernel<<<1, 32, 0, stream>>>(flag, want, status);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
+}
+
+int launch_flag_publish(unsigned long long* flag, unsigned long long seq, cudaStream_t stream) {
+  flag_publish_kernel<<<1, 32, 0, stream>>>(flag, seq);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
+}
+
 // Elements per chunk when a shard of shard_elems elements is cut into n_chunks pieces: ceil(shard / n_chunks) rounded
 // up to 64 elements, at most the whole shard.  The root and the rank (possibly in different processes) both use it,
 // so they agree on every chunk's bounds.
@@ -312,18 +337,6 @@ int ktb_push_scatter_chunked(int root_dev, const void* src_root, size_t n_elems,
 }
 
 // ---- copy-engine form of the root side: no SM of the root is used ------------------------------------------------
-namespace ktb {
-__global__ void push_publish_one_kernel(unsigned long long* ready, unsigned long long seq) {
-  if (threadIdx.x == 0) {
-    __threadfence_system();
-    st_release_sys(ready, seq);
-  }
-}
-__global__ void push_wait_ack_kernel(const unsigned long long* ack, unsigned long long want, unsigned int* status) {
-  if (threadIdx.x == 0) (void)spin_until(ack, want, status);
-}
-}  // namespace ktb
-
 int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype, int n_ranks,
                         int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
                         void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, unsigned long long seq,
@@ -362,9 +375,9 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
     }
     KTB_CK(cudaStreamWaitEvent(ce_stream[root_dev][r], ce_start[root_dev], 0));
     if (seq > 2) {   // do not overwrite staging half (seq & 1) before the rank consumed call seq-2
-      push_wait_ack_kernel<<<1, 32, 0, ce_stream[root_dev][r]>>>(
-          reinterpret_cast<const unsigned long long*>(croot + KTB_CTRL_ACK) + r, seq - 2, status);
-      KTB_CK(cudaGetLastError());
+      rc = launch_flag_wait(reinterpret_cast<const unsigned long long*>(croot + KTB_CTRL_ACK) + r, seq - 2, status,
+                            ce_stream[root_dev][r]);
+      if (rc) return rc;
     }
   }
   for (size_t c = 0; c < (size_t)n_chunks; ++c) {
@@ -377,8 +390,8 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
                                    static_cast<const uint8_t*>(src_root) + (sb[r] + lo) * es, root_dev, (hi - lo) * es, cs));
       unsigned long long* ready =
           reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctrl_peer[r]) + KTB_CTRL_READY) + c;
-      push_publish_one_kernel<<<1, 32, 0, cs>>>(ready, seq);   // stream-ordered behind the copy
-      KTB_CK(cudaGetLastError());
+      rc = launch_flag_publish(ready, seq, cs);   // stream-ordered behind the copy
+      if (rc) return rc;
     }
   }
   for (int r = 0; r < n_ranks; ++r) {   // the caller's stream "contains" the scatter (src may be reused after it)

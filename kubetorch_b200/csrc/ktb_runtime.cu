@@ -60,8 +60,7 @@ static int register_device(int dev) {
   KTB_CK(cudaStreamCreateWithFlags(&d.stream_exec, cudaStreamNonBlocking));
   KTB_CK(cudaStreamCreateWithFlags(&d.stream_d2h, cudaStreamNonBlocking));
   KTB_CK(cudaStreamCreateWithFlags(&d.stream_rank, cudaStreamNonBlocking));
-  KTB_CK(cudaEventCreateWithFlags(&d.ev_a, cudaEventDisableTiming));
-  KTB_CK(cudaEventCreateWithFlags(&d.ev_b, cudaEventDisableTiming));
+  KTB_CK(cudaStreamCreateWithFlags(&d.stream_stage, cudaStreamNonBlocking));
   for (int i = 0; i < 6; ++i) KTB_CK(cudaEventCreateWithFlags(&d.host_ev[i], cudaEventDisableTiming));
   d.registered = true;
   g_peer[dev][dev] = true;
@@ -140,8 +139,7 @@ int ktb_shutdown(void) {
     cudaStreamDestroy(g_dev[d].stream_exec);
     cudaStreamDestroy(g_dev[d].stream_d2h);
     cudaStreamDestroy(g_dev[d].stream_rank);
-    cudaEventDestroy(g_dev[d].ev_a);
-    cudaEventDestroy(g_dev[d].ev_b);
+    cudaStreamDestroy(g_dev[d].stream_stage);
     for (int i = 0; i < 6; ++i) cudaEventDestroy(g_dev[d].host_ev[i]);
     g_dev[d] = DeviceInfo();
   }

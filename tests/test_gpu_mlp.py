@@ -172,6 +172,8 @@ STATUS_CASES = {
     "pushed_shard_exceeds_stage_stride": (pushed, dict(M=256, stride=256 * 256 * 2 - 256), L.ERR_ARG),
     "pushed_rows_not_multiple_of_128": (pushed, dict(M=200), L.ERR_ARG),
     "pushed_d_out_not_64": (pushed, dict(d_out=128), L.ERR_UNSUPPORTED),
+    "pushed_stride_not_multiple_of_16": (pushed, dict(stride=(1 << 20) + 8), L.ERR_ARG),
+    "pushed_stride_not_multiple_of_16_even_seq": (pushed, dict(stride=(1 << 20) + 8, seq=2), L.ERR_ARG),
 }
 
 

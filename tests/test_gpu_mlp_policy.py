@@ -317,6 +317,8 @@ STATUS_CASES = {
     "pushed_both_outputs_null": (pushed, dict(logits=0, actions=0), L.ERR_ARG),
     "pushed_misaligned_actions": (pushed, dict(actions_off=4), L.ERR_ARG),
     "pushed_misaligned_w2": (pushed, dict(w2_off=2), L.ERR_ARG),
+    "pushed_stride_not_multiple_of_16": (pushed, dict(stride=(1 << 20) + 8), L.ERR_ARG),
+    "pushed_stride_not_multiple_of_16_even_seq": (pushed, dict(stride=(1 << 20) + 8, seq=2), L.ERR_ARG),
 }
 
 

@@ -274,6 +274,8 @@ STATUS_CASES = {
     "pushed_null_log_probs": (pushed, dict(log_probs=0), L.ERR_ARG),
     "pushed_misaligned_log_probs": (pushed, dict(log_probs_off=1), L.ERR_ARG),
     "pushed_d_out_257": (pushed, dict(d_out=257), L.ERR_UNSUPPORTED),
+    "pushed_stride_not_multiple_of_16": (pushed, dict(stride=(1 << 20) + 8), L.ERR_ARG),
+    "pushed_stride_not_multiple_of_16_even_seq": (pushed, dict(stride=(1 << 20) + 8, seq=2), L.ERR_ARG),
 }
 
 
