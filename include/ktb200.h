@@ -244,17 +244,17 @@ int ktb_push_status(int dev, const void* ctrl, unsigned int* out);
 
 /* ---- host-resident args/results (the reference's client lives outside the GPU) -------------------- */
 
-/* dst_host = op(src_host) with both buffers in pinned host memory, chunked through
- * device staging buffers (each >= 2*chunk_bytes) on three library streams so that H2D copy,
- * kernel and D2H copy of successive chunks overlap (PCIe is full duplex).  Synchronous:
- * returns when dst_host is complete. */
-int ktb_map_host(int dev, int op, int dtype, const void* src_host, void* dst_host, size_t n_elems,
-                 double alpha, double beta, size_t chunk_bytes, void* stage_in, void* stage_out);
-
-/* The same for a sharded call on n_ranks DISTINCT devices: rank r's `x.chunk(n_ranks)[r]` (granule as in
- * ktb_scatter_map_gather) moves host → devs[r] → host over that GPU's own PCIe link, each pipeline enqueued by a
- * persistent library issue thread bound to the CPUs of that GPU's NUMA node (all links run concurrently).
- * stage_in[r] / stage_out[r] are device buffers of >= 2*chunk_bytes on devs[r].  Synchronous. */
+/* dst_host = op(src_host) with both buffers in pinned host memory, sharded over n_ranks: rank r's
+ * `x.chunk(n_ranks)[r]` (granule as in ktb_scatter_map_gather) moves host → devs[r] → host over that GPU's own
+ * PCIe link, chunked through device staging buffers stage_in[r] / stage_out[r] (each >= 2*chunk_bytes, on
+ * devs[r]) on three library streams so that H2D copy, kernel and D2H copy of successive chunks overlap (PCIe is
+ * full duplex).  Each device's pipeline is enqueued by a persistent library issue thread bound to the CPUs of
+ * that GPU's NUMA node (all links run concurrently); the first device's runs on the calling thread.  A one-GPU
+ * call is n_ranks = 1, devs = {dev}, granule = 1.  Synchronous: returns when dst_host is complete.
+ *   - Rank subsets: a rank whose stage_in[r] and stage_out[r] are both NULL is not part of the call and its shard of
+ *     dst_host is left alone; exactly one of the two NULL is KTB_ERR_ARG; every rank NULL moves nothing (KTB_OK).
+ *   - devs may repeat: the selected ranks of one device run one after another in rank order (they share its
+ *     streams, events and staging, so they may share staging buffers too). */
 int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, size_t n_elems,
                        size_t granule, double alpha, double beta, int n_ranks, const int* devs,
                        size_t chunk_bytes, void* const* stage_in, void* const* stage_out);

@@ -71,10 +71,10 @@ struct DeviceGuard {
 struct DeviceInfo {
   bool registered = false;
   int sm_count = 0;
-  cudaStream_t stream_h2d = nullptr, stream_exec = nullptr, stream_d2h = nullptr;  // ktb_map_host
+  cudaStream_t stream_h2d = nullptr, stream_exec = nullptr, stream_d2h = nullptr;  // host pipeline
   cudaStream_t stream_rank = nullptr;                                              // multi-GPU default
   cudaStream_t stream_stage = nullptr;                                             // staged MLP pulls
-  cudaEvent_t host_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // ktb_map_host_multi
+  cudaEvent_t host_ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};  // host pipeline
 };
 constexpr int kMaxDevices = 16;
 DeviceInfo* device_info(int dev);   // nullptr when unregistered

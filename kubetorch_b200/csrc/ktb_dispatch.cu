@@ -252,6 +252,6 @@ int ktb_scatter_map_reduce(int op, int dtype, const void* src_root, size_t n_ele
                                 rank_stream(streams, devs, root_rank));
 }
 
-// ktb_map_host / ktb_map_host_multi (host-resident args over PCIe) live in ktb_host.cu.
+// ktb_map_host_multi (host-resident args over PCIe) lives in ktb_host.cu.
 
 }  // extern "C"

@@ -9,6 +9,8 @@
 //   * NUMA-SHARDED pinned buffers (ktb_host_alloc_sharded): the pages of shard r are first-touched by GPU r's
 //     issue thread, i.e. on GPU r's NUMA node, before the block is page-locked (cudaHostRegister), so no DMA
 //     crosses the socket interconnect.
+// One entry, ktb_map_host_multi, serves every host-path call: one GPU, all ranks, a subset of the ranks (NULL
+// staging), and ranks that share a GPU (they run one after another in that GPU's job).
 // Replaces, for host-resident tensors, the whole client→pod→client round trip of the reference
 // (serving/utils.py:730-749 pack, process_pool.py:125-234 queues, http_server.py:1768-1842 decode/encode,
 // serving/utils.py:787-813 unpack).
@@ -332,24 +334,6 @@ int ktb_host_free_sharded(void* ptr) {
   return KTB_OK;
 }
 
-int ktb_map_host(int dev, int op, int dtype, const void* src_host, void* dst_host, size_t n_elems,
-                 double alpha, double beta, size_t chunk_bytes, void* stage_in, void* stage_out) {
-  int rc = require_device(dev);
-  if (rc) return rc;
-  if (n_elems == 0) return check_dtype("ktb_map_host", dtype);   // an empty call checks the dtype only
-  rc = check_elementwise("ktb_map_host", op, dtype);   // before the pipeline queues its first copy
-  if (rc) return rc;
-  const size_t es = dtype_size(dtype);
-  KTB_REQUIRE(src_host && dst_host && stage_in && stage_out, KTB_ERR_ARG, "ktb_map_host: null argument");
-  KTB_REQUIRE(chunk_bytes >= 4096 && chunk_bytes % 256 == 0, KTB_ERR_ARG,
-              "ktb_map_host: chunk_bytes must be a multiple of 256 and >= 4096 (got %zu)", chunk_bytes);
-  const MapParams p = make_params(alpha, beta, dtype);
-  // one host-path call at a time per process: the per-device streams/events carry a single pipeline
-  std::lock_guard<std::mutex> lk(g_host_call_mu);
-  return run_host_pipeline(dev, op, dtype, static_cast<const uint8_t*>(src_host), static_cast<uint8_t*>(dst_host),
-                           n_elems * es, p, chunk_bytes, stage_in, stage_out);
-}
-
 int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, size_t n_elems, size_t granule,
                        double alpha, double beta, int n_ranks, const int* devs, size_t chunk_bytes,
                        void* const* stage_in, void* const* stage_out) {
@@ -365,50 +349,52 @@ int ktb_map_host_multi(int op, int dtype, const void* src_host, void* dst_host, 
   for (int r = 0; r < n_ranks; ++r) {
     rc = require_device(devs[r]);
     if (rc) return rc;
-    for (int q = 0; q < r; ++q)
-      KTB_REQUIRE(devs[q] != devs[r], KTB_ERR_ARG, "ktb_map_host_multi: devices must be distinct (use ktb_map_host per rank)");
-    KTB_REQUIRE(stage_in[r] && stage_out[r], KTB_ERR_ARG, "ktb_map_host_multi: rank %d has no staging buffers", r);
+    KTB_REQUIRE((stage_in[r] == nullptr) == (stage_out[r] == nullptr), KTB_ERR_ARG,
+                "ktb_map_host_multi: rank %d has one staging buffer (both, or neither to skip the rank)", r);
   }
   rc = check_elementwise("ktb_map_host_multi", op, dtype);   // before any rank's pipeline starts
   if (rc) return rc;
   const size_t es = dtype_size(dtype);
+  const size_t rows = n_elems / granule;
   std::lock_guard<std::mutex> lk(g_host_call_mu);
   const MapParams p = make_params(alpha, beta, dtype);
   const uint8_t* src = static_cast<const uint8_t*>(src_host);
   uint8_t* dst = static_cast<uint8_t*>(dst_host);
-  HostWorker* posted[kMaxDevices] = {nullptr};
-  int first = -1;             // the first non-empty rank runs on the calling thread (saves one wake-up)
-  size_t first_off = 0, first_len = 0;
+  // one job per device: its selected ranks in rank order, one after another, since they share the device's
+  // streams, events and staging buffers
+  auto run_device = [=](int dev) {
+    int status = KTB_OK;
+    for (int r = 0; r < n_ranks && status == KTB_OK; ++r) {
+      if (devs[r] != dev || !stage_in[r]) continue;
+      size_t b = 0, e = 0;
+      ktb_shard_bounds(rows, n_ranks, r, &b, &e);
+      const size_t off = b * granule * es;
+      status = run_host_pipeline(dev, op, dtype, src + off, dst + off, (e - b) * granule * es, p, chunk_bytes,
+                                 stage_in[r], stage_out[r]);
+    }
+    return status;
+  };
+  int jobs[kMaxDevices];   // devices with at least one selected, non-empty rank, in order of first appearance
+  int n_jobs = 0;
   for (int r = 0; r < n_ranks; ++r) {
     size_t b = 0, e = 0;
-    ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
-    const size_t off = b * granule * es, len = (e - b) * granule * es;
-    if (len == 0) continue;
-    if (first < 0) {
-      first = r;
-      first_off = off;
-      first_len = len;
-      continue;
-    }
-    const int dev = devs[r];
-    void* sin = stage_in[r];
-    void* sout = stage_out[r];
-    HostWorker* w = worker_for(dev);
-    worker_post(w, [=]() {
-      return run_host_pipeline(dev, op, dtype, src + off, dst + off, len, p, chunk_bytes, sin, sout);
-    });
-    posted[r] = w;
+    ktb_shard_bounds(rows, n_ranks, r, &b, &e);
+    if (stage_in[r] && e > b && std::find(jobs, jobs + n_jobs, devs[r]) == jobs + n_jobs) jobs[n_jobs++] = devs[r];
+  }
+  HostWorker* posted[kMaxDevices] = {nullptr};
+  for (int j = 1; j < n_jobs; ++j) {
+    const int dev = jobs[j];
+    posted[j] = worker_for(dev);
+    worker_post(posted[j], [=]() { return run_device(dev); });
   }
   int status = KTB_OK;
   char first_err[512] = "";
-  if (first >= 0) {
-    status = run_host_pipeline(devs[first], op, dtype, src + first_off, dst + first_off, first_len, p, chunk_bytes,
-                               stage_in[first], stage_out[first]);
+  if (n_jobs > 0) {   // the first device's job runs on the calling thread (saves one wake-up)
+    status = run_device(jobs[0]);
     if (status != KTB_OK) snprintf(first_err, sizeof(first_err), "%s", last_error_cstr());
   }
-  for (int r = 0; r < n_ranks; ++r) {
-    if (!posted[r]) continue;
-    int rc = worker_wait(posted[r]);   // always wait for every rank: the buffers are borrowed until then
+  for (int j = 1; j < n_jobs; ++j) {
+    int rc = worker_wait(posted[j]);   // always wait for every job: the buffers are borrowed until then
     if (rc != KTB_OK && status == KTB_OK) status = rc;
   }
   if (first_err[0]) set_error("%s", first_err);

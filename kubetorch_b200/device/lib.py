@@ -82,7 +82,6 @@ _SIGNATURES = {
                                  c_void_p, c_void_p, c_int, c_int, ctypes.c_ulonglong, c_uintptr]),
     "ktb_push_wait": (c_int, [c_int, c_void_p, c_int, c_int, ctypes.c_ulonglong, c_uintptr]),
     "ktb_push_status": (c_int, [c_int, c_void_p, POINTER(ctypes.c_uint)]),
-    "ktb_map_host": (c_int, [c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_double, c_double, c_size_t, c_void_p, c_void_p]),
     "ktb_map_host_multi": (c_int, [c_int, c_int, c_void_p, c_void_p, c_size_t, c_size_t, c_double, c_double, c_int,
                                    POINTER(c_int), c_size_t, POINTER(c_void_p), POINTER(c_void_p)]),
     "ktb_mlp_scratch_bytes": (c_size_t, [c_size_t, c_int]),

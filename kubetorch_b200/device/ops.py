@@ -781,49 +781,7 @@ def device_numa_node(device: int) -> int:
 
 # ---- host-resident args ------------------------------------------------------------------------------
 _stage_cache = {}
-_host_locks = {}
-
-
-def map_host(
-    x_host: torch.Tensor,
-    op: str = "identity",
-    alpha: float = 1.0,
-    beta: float = 0.0,
-    out_host: Optional[torch.Tensor] = None,
-    device: int = 0,
-    chunk_bytes: int = 16 << 20,
-) -> torch.Tensor:
-    """out_host = op(x_host), both pinned host tensors; H2D, kernel and D2H of successive chunks overlap."""
-    require_cuda()
-    if x_host.is_cuda or not x_host.is_pinned():
-        raise ValueError("x_host must be a pinned host tensor")
-    if out_host is None:
-        out_host = torch.empty_like(x_host).pin_memory()
-    elif out_host.is_cuda or not out_host.is_pinned():
-        raise ValueError("out_host must be a pinned host tensor")
-    ensure_init({device})
-    a, b = scalar_args(x_host.dtype, alpha, beta)
-    key = (device, chunk_bytes)
-    # one host-path call at a time per device: the staging buffers and the library's three copy/exec
-    # streams are per-device (the PCIe link serialises them anyway)
-    with _init_lock:
-        lock = _host_locks.setdefault(device, threading.Lock())
-    with lock:
-        st = _stage_cache.get(key)
-        if st is None:
-            st = (
-                torch.empty(2 * chunk_bytes, dtype=torch.uint8, device=f"cuda:{device}"),
-                torch.empty(2 * chunk_bytes, dtype=torch.uint8, device=f"cuda:{device}"),
-            )
-            _stage_cache[key] = st
-        L.call(
-            "ktb_map_host", device, OPS[op], dtype_code(x_host.dtype), x_host.data_ptr(), out_host.data_ptr(),
-            x_host.numel(), a, b, chunk_bytes, st[0].data_ptr(), st[1].data_ptr(),
-        )
-    return out_host
-
-
-_multi_lock = threading.Lock()
+_stage_lock = threading.Lock()
 
 
 def host_chunk_bytes(shard_bytes: int) -> int:
@@ -832,21 +790,26 @@ def host_chunk_bytes(shard_bytes: int) -> int:
     return (c + 255) // 256 * 256
 
 
-def map_host_multi(
+def map_host(
     x_host: torch.Tensor,
-    op: str,
+    op: str = "identity",
     alpha: float = 1.0,
     beta: float = 0.0,
     out_host: Optional[torch.Tensor] = None,
     devices: Sequence[int] = (0,),
+    ranks: Optional[Sequence[int]] = None,
     chunk_bytes: Optional[int] = None,
 ) -> torch.Tensor:
-    """Sharded host-resident call on distinct GPUs from ONE host thread (ktb_map_host_multi)."""
+    """out_host = op(x_host), both pinned host tensors, sharded `x.chunk(len(devices))` on dim 0: rank r's shard goes
+    host → devices[r] → host, H2D, kernel and D2H of successive chunks overlapping (ktb_map_host_multi).  Devices may
+    repeat.  With `ranks`, only those ranks' shards are computed; the rest of out_host is left as it was."""
     require_cuda()
     if x_host.is_cuda or not x_host.is_pinned():
         raise ValueError("x_host must be a pinned host tensor")
     if out_host is None:
         out_host = torch.empty_like(x_host).pin_memory()
+    elif out_host.is_cuda or not out_host.is_pinned():
+        raise ValueError("out_host must be a pinned host tensor")
     devs = [int(d) for d in devices]
     ensure_init(set(devs))
     a, b = scalar_args(x_host.dtype, alpha, beta)
@@ -854,22 +817,30 @@ def map_host_multi(
     rows = x_host.numel() // gran
     shard_bytes = shard_bounds(rows, len(devs), 0)[1] * gran * x_host.element_size()
     cb = int(chunk_bytes or host_chunk_bytes(shard_bytes))
-    with _multi_lock:
-        stages = []
-        for d in devs:
-            key = (d, cb)
-            st = _stage_cache.get(key)
+    sel = set(range(len(devs)) if ranks is None else ranks)
+    if not sel <= set(range(len(devs))):
+        raise ValueError(f"ranks {sorted(sel)} out of range for {len(devs)} devices")
+    # one host-path call at a time: the staging buffers are per (device, chunk size), and the library's copy/exec
+    # streams and events are per device
+    with _stage_lock:
+        stage_in, stage_out = [], []   # NULL for a rank outside `ranks`: the library skips it
+        for r, d in enumerate(devs):
+            if r not in sel:
+                stage_in.append(None)
+                stage_out.append(None)
+                continue
+            st = _stage_cache.get((d, cb))
             if st is None:
                 st = (torch.empty(2 * cb, dtype=torch.uint8, device=f"cuda:{d}"),
                       torch.empty(2 * cb, dtype=torch.uint8, device=f"cuda:{d}"))
                 torch.cuda.synchronize(d)
-                _stage_cache[key] = st
-            stages.append(st)
+                _stage_cache[(d, cb)] = st
+            stage_in.append(st[0].data_ptr())
+            stage_out.append(st[1].data_ptr())
         L.call(
             "ktb_map_host_multi", OPS[op], dtype_code(x_host.dtype), x_host.data_ptr(), out_host.data_ptr(),
             x_host.numel(), gran, a, b, len(devs), L.arr(ctypes.c_int, devs), cb,
-            L.arr(ctypes.c_void_p, [s[0].data_ptr() for s in stages]),
-            L.arr(ctypes.c_void_p, [s[1].data_ptr() for s in stages]),
+            L.arr(ctypes.c_void_p, stage_in), L.arr(ctypes.c_void_p, stage_out),
         )
     return out_host
 

@@ -193,7 +193,7 @@ class Module:
         if use_b200:
             per_worker = None if num_proc in ("auto", None) and not compute.gpus else \
                 (None if num_proc == "auto" else int(num_proc or compute.gpus or 1))
-            extra = {k: dist[k] for k in ("devices", "transfer", "host_mode", "placement", "self_check") if dist and k in dist}
+            extra = {k: dist[k] for k in ("devices", "transfer", "placement", "self_check") if dist and k in dist}
             return dict(distribution_type="b200", callable_obj=target, num_proc=per_worker, workers=workers,
                         distributed=bool(dist), **extra, **common)
         if dtype in SPMD_TYPES:

@@ -33,7 +33,7 @@ One controller process drives N local H100s.  For a @kt.mapped callable a remote
         scatter, exec and gather are ONE kernel per rank; the caller gets N views, rank-ordered.
     host-resident arg (CPU tensor; the reference's client lives outside the GPU)
         each rank's shard goes host → its own GPU → host over that GPU's own PCIe link
-        (ktb_map_host*: chunked H2D / kernel / D2H), ranks in parallel.
+        (ktb_map_host_multi: chunked H2D / kernel / D2H), ranks in parallel.
     reduce="sum"
         ktb_scatter_map_reduce: per-rank warp-shuffle reduction, scalar peer-stored to the root.
 
@@ -46,7 +46,6 @@ import json
 import os
 import pickle
 import threading
-from concurrent.futures import ThreadPoolExecutor
 from typing import List, Optional
 
 from ..distributed import local_pod_ips
@@ -62,8 +61,8 @@ _INT_DTYPES = ("torch.int32", "torch.int64")
 class B200Supervisor:
     def __init__(self, pointers=None, init_args=None, name: str = None, devices: Optional[List[int]] = None,
                  num_proc=None, workers: int = None, quorum_workers: int = None, distributed: bool = True,
-                 allowed_serialization: Optional[str] = None, host_chunk_bytes: int = 16 << 20, variant: int = 0,
-                 callable_obj=None, transfer: str = "auto", host_mode: str = "multi", placement: str = "auto",
+                 allowed_serialization: Optional[str] = None, variant: int = 0,
+                 callable_obj=None, transfer: str = "auto", placement: str = "auto",
                  quorum_timeout=None, monitor_members=None, port=None, restart_procs: bool = True,
                  max_threads_per_proc: int = 10, self_check: bool = True, **extra):
         # (pointers, init_args, name, callable_obj) are the in-package deploy path; the reference's server passes
@@ -75,11 +74,9 @@ class B200Supervisor:
         self.workers = int(workers or quorum_workers or 1)
         self.distributed = distributed
         self.allowed_serialization = allowed_serialization  # None → KT_ALLOWED_SERIALIZATION at call time
-        self.host_chunk_bytes = host_chunk_bytes
         self.variant = variant
         self.self_check = bool(self_check)
         self._callable = None
-        self._host_pool: Optional[ThreadPoolExecutor] = None
         self._pin_cache = {}
         self._lock = threading.Lock()
         self._host_lock = threading.Lock()
@@ -89,7 +86,6 @@ class B200Supervisor:
         if transfer not in ("auto", "pull", "push"):
             raise ValueError("transfer must be 'auto', 'pull' or 'push'")
         self.transfer = transfer
-        self.host_mode = host_mode  # "multi": one C call drives all GPUs; "threads": one host thread per rank
         # where device-resident element-wise shards execute: "ranks" = rank r on GPU r whatever the size (the sharded
         # path the benchmarks measure); "root" = every rank's shard on the root GPU (same results; for HBM-bound ops a
         # root-resident arg is served faster by the root's own HBM than through its NVLink port, profiles §2);
@@ -135,7 +131,6 @@ class B200Supervisor:
             self._callable = load_callable(self.pointers, self.init_args)
         else:
             self._callable = load_callable_from_env()  # the reference server's path
-        self._host_pool = ThreadPoolExecutor(max_workers=len(self.devices), thread_name_prefix="ktb-host")
         if self.self_check:
             self._self_check()
 
@@ -167,9 +162,6 @@ class B200Supervisor:
 
     def cleanup(self):
         self._callable = None
-        if self._host_pool is not None:
-            self._host_pool.shutdown(wait=False)
-            self._host_pool = None
         self._pin_cache.clear()
         self._push = None
         self._small = None
@@ -548,25 +540,12 @@ class B200Supervisor:
         # results are FRESH tensors every call (the reference returns new objects); the pinned allocations are
         # cached per size and laid out so that shard r's pages sit on the NUMA node of GPU r (ops.pinned_empty)
         out = ops.pinned_empty(tuple(x.shape), x.dtype, devices=self.devices)
-        x_shards = self._shard_views(x, x)
+        # one C call drives every selected rank's copy/exec/copy pipeline (persistent per-GPU issue threads in the
+        # library); ranks outside a `workers=` subset are skipped
+        all_ranks = self._all_ranks(ranks)
+        ops.map_host(x, op, alpha, beta, out_host=out, devices=self.devices, ranks=None if all_ranks else ranks)
         o_shards = self._shard_views(out, x)
-        distinct = len(set(self.devices)) == len(self.devices)
-        if self._all_ranks(ranks) and self.host_mode == "multi" and distinct:
-            # one C call drives every GPU's copy/exec/copy pipeline (persistent per-GPU issue threads in the library)
-            ops.map_host_multi(x, op, alpha, beta, out_host=out, devices=self.devices)
-            return o_shards
-        sel = list(range(self.world_size)) if ranks is None else list(ranks)
-
-        def run(rank):
-            if x_shards[rank].numel():
-                ops.map_host(x_shards[rank], op, alpha, beta, out_host=o_shards[rank], device=self.devices[rank],
-                             chunk_bytes=self.host_chunk_bytes)
-
-        if len(sel) == 1:
-            run(sel[0])
-        else:
-            list(self._host_pool.map(run, sel))
-        return [o_shards[r] for r in sel]
+        return o_shards if all_ranks else [o_shards[r] for r in ranks]
 
     def _reduce(self, x, op, alpha, beta, ranks=None):
         ops = self.ops

@@ -59,14 +59,8 @@ def _stub_device():
             return x * alpha if op == "scale" else x * alpha + beta
 
         @classmethod
-        def map_host_multi(cls, x, op, alpha=1.0, beta=0.0, out_host=None, devices=(0,), chunk_bytes=None):
-            cls.calls.append(["map_host_multi", len(devices)])
-            out_host.copy_(cls._apply(x, op, alpha, beta))
-            return out_host
-
-        @classmethod
-        def map_host(cls, x, op, alpha=1.0, beta=0.0, out_host=None, device=0, chunk_bytes=None):
-            cls.calls.append(["map_host", device])
+        def map_host(cls, x, op, alpha=1.0, beta=0.0, out_host=None, devices=(0,), ranks=None, chunk_bytes=None):
+            cls.calls.append(["map_host", len(devices)] + ([list(ranks)] if ranks is not None else []))
             out_host.copy_(cls._apply(x, op, alpha, beta))
             return out_host
 

@@ -182,7 +182,7 @@ def test_two_gpu_peer_path_matches_oracle():
     total, partials = ops.scatter_map_reduce(xi.cuda(0), "identity", devices=[0, 1])
     assert partials.tolist() == ref_dispatch.spmd_call(cases.shard_sum, xi, num_proc=2, serialization="pickle")
     xh = torch.randn((1 << 21) + 3).pin_memory()   # host-resident, both GPUs from one host thread
-    assert torch.equal(ops.map_host_multi(xh, "scale", 2.0, devices=[0, 1]), xh * 2.0)
+    assert torch.equal(ops.map_host(xh, "scale", 2.0, devices=[0, 1]), xh * 2.0)
     from kubetorch_b200.device import mlp
 
     g = torch.Generator().manual_seed(3)

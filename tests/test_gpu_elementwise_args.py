@@ -15,7 +15,9 @@ ES_MAX = 8               # the widest element (I64): buffers hold N of them
 CHUNK = 1 << 16          # chunk_bytes of the host-resident entries
 BAD_OPS = (-1, 3, 7)
 BAD_DTYPES = (-1, 6, 99)
-MAP = ("ktb_map", "ktb_map_batch", "ktb_push_consume", "ktb_scatter_map_gather", "ktb_map_host", "ktb_map_host_multi")
+# ktb_map_host_multi_subset: ktb_map_host_multi with two ranks on device 0, rank 1 left out (NULL staging)
+MAP = ("ktb_map", "ktb_map_batch", "ktb_push_consume", "ktb_scatter_map_gather", "ktb_map_host_multi",
+       "ktb_map_host_multi_subset")
 REDUCE = ("ktb_map_reduce_sum", "ktb_scatter_map_reduce")
 SCATTER = ("ktb_push_scatter", "ktb_push_scatter_chunked", "ktb_push_scatter_ce")   # take no op
 
@@ -55,10 +57,10 @@ def call():
                                                                    ptr(ctrl_rank), ptr(ctrl_root), 1, 4, 1, 0),
         "ktb_scatter_map_gather": lambda op, dt, n: lib.ktb_scatter_map_gather(op, dt, ptr(src), ptr(dst), n, 1, 2.0,
                                                                                1.0, 1, one, 0, L.VARIANT_AUTO, None),
-        "ktb_map_host": lambda op, dt, n: lib.ktb_map_host(0, op, dt, ptr(src_h), ptr(dst_h), n, 2.0, 1.0, CHUNK,
-                                                           ptr(stage_in), ptr(stage_out)),
         "ktb_map_host_multi": lambda op, dt, n: lib.ktb_map_host_multi(op, dt, ptr(src_h), ptr(dst_h), n, 1, 2.0, 1.0,
                                                                        1, one, CHUNK, vp(stage_in), vp(stage_out)),
+        "ktb_map_host_multi_subset": lambda op, dt, n: lib.ktb_map_host_multi(
+            op, dt, ptr(src_h), ptr(dst_h), n, 1, 2.0, 1.0, 2, two, CHUNK, vp(stage_in, None), vp(stage_out, None)),
         "ktb_map_reduce_sum": lambda op, dt, n: lib.ktb_map_reduce_sum(0, op, dt, ptr(src), n, 2.0, 1.0, ptr(out),
                                                                        ptr(ws), 0),
         "ktb_scatter_map_reduce": lambda op, dt, n: lib.ktb_scatter_map_reduce(op, dt, ptr(src), n, 1, 2.0, 1.0, 1, one,
@@ -98,7 +100,7 @@ def test_bad_op_or_dtype_is_rejected(call, entry, op, dtype):
 # even empty ones); the entries whose empty call returns before any work return KTB_OK.
 EMPTY = [("ktb_map", L.ERR_ARG), ("ktb_map_batch", L.ERR_ARG), ("ktb_map_reduce_sum", L.ERR_ARG),
          ("ktb_scatter_map_reduce", L.ERR_ARG), ("ktb_push_consume", L.ERR_ARG),
-         ("ktb_map_host", L.OK), ("ktb_map_host_multi", L.OK), ("ktb_scatter_map_gather", L.OK)]
+         ("ktb_map_host_multi", L.OK), ("ktb_map_host_multi_subset", L.OK), ("ktb_scatter_map_gather", L.OK)]
 
 
 @pytest.mark.parametrize("op", BAD_OPS)
@@ -112,3 +114,36 @@ def test_map_batch_without_segments_is_ok_whatever_the_op(call, op):
     lib = L.load()
     assert lib.ktb_map_batch(0, op, L.F32, None, None, None, 0, 2.0, 1.0, 0) == L.OK
     torch.cuda.synchronize()
+
+
+# ktb_map_host_multi's rank rules, two ranks on device 0: a rank whose two staging buffers are NULL is not part of the
+# call, one NULL of a pair is an error, and a device may carry several ranks (a bad op or dtype on a rank subset: the
+# ktb_map_host_multi_subset rows above).  case: (op, stage_in, stage_out, status)
+HOST_RANKS = {
+    "one_null_stage": (L.OP_SCALE, ("in", "in"), ("out", None), L.ERR_ARG),
+    "all_ranks_null": (L.OP_SCALE, (None, None), (None, None), L.OK),
+    "shared_device": (L.OP_SCALE, ("in", "in"), ("out", "out"), L.OK),
+}
+
+
+@pytest.mark.parametrize("case", list(HOST_RANKS))
+def test_map_host_multi_rank_rules(case):
+    from kubetorch_b200.device import ops
+
+    lib = L.load()
+    ops.ensure_init([0])
+    op, ins, outs, want = HOST_RANKS[case]
+    stage = {"in": torch.zeros(2 * CHUNK, dtype=torch.uint8, device="cuda"),
+             "out": torch.zeros(2 * CHUNK, dtype=torch.uint8, device="cuda")}
+    src = torch.arange(N, dtype=torch.float32).pin_memory()
+    dst = torch.full((N,), -1.0).pin_memory()
+
+    def stages(keys):
+        return L.arr(c_void_p, [stage[k].data_ptr() if k else None for k in keys])
+
+    status = lib.ktb_map_host_multi(op, L.F32, src.data_ptr(), dst.data_ptr(), N, 1, 2.0, 1.0, 2, L.arr(c_int, [0, 0]),
+                                    CHUNK, stages(ins), stages(outs))
+    torch.cuda.synchronize()
+    assert status == want
+    # a rejected call and a call without ranks leave dst untouched; two ranks sharing the device compute all of it
+    assert torch.equal(dst, src * 2.0 if case == "shared_device" else torch.full((N,), -1.0))

@@ -358,27 +358,37 @@ class HostGuarded:
 
 @pytest.mark.parametrize("dtype,op", CASES, ids=CASE_IDS)
 def test_map_host_exact(K, dtype, op):
-    """map_host and map_host_multi with 4096-byte chunks (the smallest the entries take; a shard spans several and the
-    last is a few bytes), pinned src and dst views at element offsets."""
+    """map_host with 4096-byte chunks (the smallest the entry takes; a shard spans several and the last is a few
+    bytes), pinned src and dst views at element offsets: one rank on [0]; three ranks of 3-element rows on [0, 0, 0];
+    and ranks 0 and 2 of those three, which leave rank 1's shard of dst as it was."""
     es = R.ES[dtype]
     n = 5 * 4096 // es + 3
     x = patterns(dtype, n, phase=7)
+    rows = n // 3
+    lo, hi = (3 * i for i in K.shard_bounds(rows, 3, 1))   # rank 1's elements
+    skipped = np.zeros(rows * 3, dtype=bool)
+    skipped[lo:hi] = True
     for a, b in {ROW[dtype], SECOND_ROW[dtype]}:
         for src_off, dst_off in ((es, 3 * es), (0, es)):
             src = HostGuarded(n * es, src_off)
             src.view(torch.uint8).copy_(torch.from_numpy(np.ascontiguousarray(x).view(np.uint8)))
             dst = HostGuarded(n * es, dst_off)
-            K.map_host(src.view(dtype), op, a, b, out_host=dst.view(dtype), device=0, chunk_bytes=4096)
-            dst.check("map_host")
+            K.map_host(src.view(dtype), op, a, b, out_host=dst.view(dtype), devices=[0], chunk_bytes=4096)
+            dst.check("one rank")
             vec = run_map(K, dtype, op, x, a, b, VEC)
-            expect(dtype, op, got_bits(dst.view(dtype), dtype), x, a, b, f"map_host {dtype} {op}", same_as=vec)
-            rows = n // 3
-            dst2 = HostGuarded(rows * 3 * es, dst_off)
-            K.map_host_multi(src.view(dtype)[:rows * 3].view(rows, 3), op, a, b,
-                             out_host=dst2.view(dtype).view(rows, 3), devices=[0], chunk_bytes=4096)
-            dst2.check("map_host_multi")
-            expect(dtype, op, got_bits(dst2.view(dtype), dtype), x[:rows * 3], a, b, f"map_host_multi {dtype} {op}",
-                   same_as=vec[:rows * 3])
+            expect(dtype, op, got_bits(dst.view(dtype), dtype), x, a, b, f"one rank {dtype} {op}", same_as=vec)
+            for ranks in (None, [0, 2]):
+                what = f"ranks {ranks} of [0, 0, 0] {dtype} {op}"
+                dst = HostGuarded(rows * 3 * es, dst_off)
+                K.map_host(src.view(dtype)[:rows * 3].view(rows, 3), op, a, b,
+                           out_host=dst.view(dtype).view(rows, 3), devices=[0, 0, 0], ranks=ranks, chunk_bytes=4096)
+                dst.check(what)
+                done = ~skipped if ranks else np.ones(rows * 3, dtype=bool)
+                expect(dtype, op, got_bits(dst.view(dtype), dtype)[done], x[:rows * 3][done], a, b, what,
+                       same_as=vec[:rows * 3][done])
+                if ranks:
+                    assert bool((dst.view(torch.uint8)[lo * es:hi * es] == Guarded.FILL).all()), \
+                        f"{what}: rank 1's shard was written"
 
 
 # ---- the public API ---------------------------------------------------------------------------------------------------

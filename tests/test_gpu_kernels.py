@@ -226,10 +226,10 @@ def test_map_host_pipeline(K):
 def test_map_host_multi_single_thread_pipeline(K):
     for n in [3, 70_001, (1 << 22) + 5]:
         x = _rand(torch.float32, n, seed=9).pin_memory()
-        out = K.map_host_multi(x, "affine", 1.5, 0.5, devices=[0], chunk_bytes=1 << 20)
+        out = K.map_host(x, "affine", 1.5, 0.5, devices=[0], chunk_bytes=1 << 20)
         assert torch.equal(out, x * 1.5 + 0.5)
     x2 = _rand(torch.int32, 40_000).reshape(100, 400).pin_memory()
-    assert torch.equal(K.map_host_multi(x2, "scale", 3, devices=[0]), x2 * 3)
+    assert torch.equal(K.map_host(x2, "scale", 3, devices=[0]), x2 * 3)
 
 
 def test_zero_copy_host_pointers(K):
@@ -293,7 +293,7 @@ def test_numa_sharded_pinned_buffers_are_pinned_pooled_and_correct(K):
     x = kt.pinned_empty((n,), torch.float32, gpus=1)
     assert x.is_pinned() and not x.is_cuda and x.numel() == n
     x.copy_(torch.arange(n, dtype=torch.float32))
-    y = K.map_host(x, "scale", 2.0, device=0)
+    y = K.map_host(x, "scale", 2.0, devices=[0])
     assert torch.equal(y, x * 2)
     ptr = x.data_ptr()
     view = x[10:20]

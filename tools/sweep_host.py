@@ -4,8 +4,8 @@
   pcie_probe   raw copy-engine bandwidth, all selected GPUs at once: H2D only, D2H only, both — from a plain pinned
                buffer (wherever torch put it) and from a NUMA-sharded one (ktb_host_alloc_sharded).  Shows what the
                box can deliver whatever our pipeline does.
-  e2e_host     kt.fn(mapped).to(kt.Compute(gpus=N)) -> remote(host tensor), by input buffer kind and host mode
-  raw          ops.map_host_multi without the API layer, by chunk size
+  e2e_host     kt.fn(mapped).to(kt.Compute(gpus=N)) -> remote(host tensor), by input buffer kind
+  raw          ops.map_host without the API layer, by chunk size
 """
 import json
 import os
@@ -124,31 +124,29 @@ def main():
         pcie_probe(sub, n, k2)
 
     double = kt.mapped("scale", alpha=2.0)(_clone(cases.double))
-    for host_mode in ("multi", "threads"):
-        remote = kt.fn(double, name=f"host-sweep-{host_mode}").to(
-            kt.Compute(gpus=n_gpus).distribute("b200", workers=1, num_proc=n_gpus, host_mode=host_mode))
-        for kind, (xh, _) in kinds.items():
-            for _ in range(3):
-                out = remote(xh, serialization="pickle")
-            reps = 10
-            t0 = time.perf_counter()
-            for _ in range(reps):
-                out = remote(xh, serialization="pickle")
-            dt = (time.perf_counter() - t0) / reps
-            ok = bool(torch.equal(torch.cat(out)[-4096:], xh[-4096:] * 2)) and bool(torch.equal(out[0][:4096], xh[:4096] * 2))
-            emit(what="e2e_host", host_mode=host_mode, kind=kind, n_gpus=n_gpus, ms=dt * 1e3,
-                 gbps=2 * n * 4 / dt / 1e9, ok=ok)
-        remote.teardown()
+    remote = kt.fn(double, name="host-sweep").to(
+        kt.Compute(gpus=n_gpus).distribute("b200", workers=1, num_proc=n_gpus))
+    for kind, (xh, _) in kinds.items():
+        for _ in range(3):
+            out = remote(xh, serialization="pickle")
+        reps = 10
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            out = remote(xh, serialization="pickle")
+        dt = (time.perf_counter() - t0) / reps
+        ok = bool(torch.equal(torch.cat(out)[-4096:], xh[-4096:] * 2)) and bool(torch.equal(out[0][:4096], xh[:4096] * 2))
+        emit(what="e2e_host", kind=kind, n_gpus=n_gpus, ms=dt * 1e3, gbps=2 * n * 4 / dt / 1e9, ok=ok)
+    remote.teardown()
     # raw pipeline without the API layer, by chunk size
     for kind, (xh, yh) in kinds.items():
         for cb in (1 << 20, 2 << 20, 4 << 20, 8 << 20, 16 << 20):
             for _ in range(2):
-                ops.map_host_multi(xh, "scale", 2.0, out_host=yh, devices=devs, chunk_bytes=cb)
+                ops.map_host(xh, "scale", 2.0, out_host=yh, devices=devs, chunk_bytes=cb)
             t0 = time.perf_counter()
             for _ in range(8):
-                ops.map_host_multi(xh, "scale", 2.0, out_host=yh, devices=devs, chunk_bytes=cb)
+                ops.map_host(xh, "scale", 2.0, out_host=yh, devices=devs, chunk_bytes=cb)
             dt = (time.perf_counter() - t0) / 8
-            emit(what="map_host_multi_raw", kind=kind, n_gpus=n_gpus, chunk_bytes=cb, ms=dt * 1e3, gbps=2 * n * 4 / dt / 1e9,
+            emit(what="map_host_raw", kind=kind, n_gpus=n_gpus, chunk_bytes=cb, ms=dt * 1e3, gbps=2 * n * 4 / dt / 1e9,
                  ok=bool(torch.equal(yh[-4096:], xh[-4096:] * 2)))
 
 
