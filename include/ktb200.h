@@ -229,6 +229,18 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
                         int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
                         void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, unsigned long long seq,
                         uintptr_t stream);
+/* ktb_push_scatter_ce with a second source per row for the masked MLP heads: row i of obs (granule elements) has
+ * row_bytes bytes at mask_root + i*row_bytes (the legal-action mask, row_bytes = d_out).  On each rank's copy-engine
+ * stream, after the same wait for ack[r] >= seq-2, chunk c's mask rows are copied to stage_peer[r] + (seq&1)*stage_stride
+ * + mask_offset + (the chunk's first row in the shard)*row_bytes, and ready[c] is published behind both copies.  After
+ * every check of ktb_push_scatter_ce, in its order: a NULL mask_root with n_elems > 0, row_bytes == 0, chunk_elems not
+ * a multiple of granule, and for a served rank mask_offset < its shard's bytes or mask_offset + rows*row_bytes >
+ * stage_stride are KTB_ERR_ARG. */
+int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
+                               int n_ranks, int root_rank, const int* devs, void* const* stage_peer,
+                               size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
+                               const void* mask_root, size_t row_bytes, size_t mask_offset, unsigned long long seq,
+                               uintptr_t stream);
 /* RANK side: for each piece, spin in-kernel until ready[chunk] >= seq, then
  * dst_root_shard[piece] = op(stage_local[piece]) (peer stores into the root's result arena); after the
  * last piece publish ack[rank] = seq in the root's control block (ctrl_root_peer). */
@@ -343,7 +355,8 @@ int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_st
  *     (the value ktb_mlp_bf16_policy stores), under the torch.argmax rules of the greedy actions.
  *   - log_probs[i] = logit_a - m - log(sum_j exp(logit_j - m)) in fp32, m the row's largest logit: torch.log_softmax
  *     (logits.float(), -1)[a].  NaN on rows with a NaN or +inf logit and on rows whose logits are all -inf, as in
- *     torch; -inf logits (action masking through b3) are never sampled while the row has a finite logit.
+ *     torch; -inf logits (one mask for every row through b3; per-row masks: the _masked forms below) are never
+ *     sampled while the row has a finite logit.
  *   - The noise depends on (seed, i, j) only: every chunk size, form (plain, staged, pushed), rank count and device
  *     gives the same bits when each shard passes its first global row as row_base.  A new seed draws new samples.
  * No logits are written.  actions [M] int64 (8-byte aligned) and log_probs [M] fp32 (4-byte aligned) may be peer
@@ -397,6 +410,42 @@ int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t
                                         uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
                                         void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
                                         size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
+/* Masked forms: ktb_mlp_bf16_policy and ktb_mlp_bf16_policy_sample with a per-row legal-action mask.
+ *   - mask [M, d_out] bytes, row-major (torch.bool): any nonzero byte means legal.  It may be a peer pointer (the
+ *     rank's rows of the root's mask); it is read once per row, only at rows < M and columns < d_out.
+ *   - The head computes exactly y.masked_fill(~legal, -inf) on its bf16-rounded output y (the value
+ *     ktb_mlp_bf16_policy stores), and every rule of the unmasked entry then applies to those masked logits: logits
+ *     hold bf16 -inf in illegal columns; actions are torch.argmax of the masked logits; the sampling form draws
+ *     Gumbel-max over them with the same Philox counters, and log_probs = log_softmax(masked.float())[a].
+ *   - A row with no legal action gets action 0 (and a NaN log-probability when sampled); a row with exactly one legal
+ *     action, whose logit is finite, gets that action with log-probability exactly 0.0.  A NaN or +inf logit in an
+ *     illegal column has no effect.  An all-legal mask gives the bits of the unmasked entry.
+ *   - A NULL mask with M > 0 is KTB_ERR_ARG, checked after every check of the unmasked entry, in the same order. */
+int ktb_mlp_bf16_policy_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                               const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                               const void* b3, const uint8_t* mask, void* logits, int64_t* actions, void* scratch,
+                               void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                      const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                      const void* b3, const uint8_t* mask, uint64_t seed, uint64_t row_base,
+                                      int64_t* actions, float* log_probs, void* scratch, void* stage,
+                                      uintptr_t stream);
+/* Push-fed masked forms: the _pushed entries' arguments with mask_offset after b3.  The rank's mask rows are read
+ * from its own staging half, at stage_local + (seq & 1)*stage_stride + mask_offset (ktb_push_scatter_ce_masked puts
+ * them there), never from a peer.  mask_offset < M*d_in*2 (overlapping the rows) or mask_offset + M*d_out >
+ * stage_stride is KTB_ERR_ARG, checked after every check of the unmasked pushed entry. */
+int ktb_mlp_bf16_policy_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                      int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                      const void* b2, const void* W3, const void* b3, size_t mask_offset, void* logits,
+                                      int64_t* actions, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                      size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                             int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                             const void* b2, const void* W3, const void* b3, size_t mask_offset,
+                                             uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs,
+                                             void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                             size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
 #ifdef __cplusplus
 }

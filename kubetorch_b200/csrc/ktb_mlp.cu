@@ -11,7 +11,8 @@
 //   * an epilogue from the fp32 register accumulators, chosen at compile time by HeadKind: optional
 //     bias (nn.Linear) and bf16 rounding, then for the hidden layers ReLU and full-tile stores, and
 //     for the head one of: logits masked to its width and/or the greedy action of every row; an
-//     action sampled by seeded Gumbel-max with its log-probability; or Gaussian actions with their
+//     action sampled by seeded Gumbel-max with its log-probability (either of these two optionally under a per-row
+//     legal-action mask, a runtime input); or Gaussian actions with their
 //     log-probability — the head's outputs may be peer pointers into the root GPU's result arena,
 //     which fuses the gather into the epilogue.
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one lane).
@@ -30,6 +31,7 @@
 #include <climits>
 #include <cmath>
 #include <mutex>
+#include <type_traits>
 
 namespace ktb {
 
@@ -259,6 +261,40 @@ __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a
   y1 = __floats2bfloat162_rn(v[2], v[3]);
 }
 
+// The columns a head epilogue ranks, one bit per column of the thread: bit 2j + c of live[h] is column col0 + 8j + c of
+// row + 8h.  Without a mask a column is live when it is < n_valid (a closed form, no loop); with a legal-action mask
+// [rows, n_valid] (row-major, nonzero byte: legal) it must also be legal, and the bytes are read in a rolled loop only
+// for stored rows (st0, st1) and columns < n_valid, so nothing past legal[rows, n_valid] is touched.  The epilogues skip
+// dead columns in the tests they already make for columns past n_valid, which is what ranking and summing
+// logits.masked_fill(~legal, -inf) comes to; the masked code stays out of the unrolled loops of the unmasked heads.
+template <int BLOCK_N>
+using ColBits = typename std::conditional<(BLOCK_N > 128), unsigned long long, unsigned>::type;
+
+template <int BLOCK_N>
+__device__ __forceinline__ void live_columns(const uint8_t* mask, int row, int col0, int n_valid, bool st0, bool st1,
+                                             ColBits<BLOCK_N> (&live)[2]) {
+  using B = ColBits<BLOCK_N>;
+  constexpr int kBits = BLOCK_N / 4;
+  const int r = n_valid - col0;   // columns col0 + 8j + c < n_valid: 8j < r (even bits), 8j + 1 < r (odd bits)
+  const int ne = r <= 0 ? 0 : min((r + 7) / 8, BLOCK_N / 8);
+  const int no = r <= 1 ? 0 : min((r + 6) / 8, BLOCK_N / 8);
+  const auto low = [](int n) { return n >= kBits ? ~B(0) : (B(1) << n) - B(1); };
+  live[0] = live[1] = (B(0x5555555555555555ull) & low(2 * ne)) | (B(0xAAAAAAAAAAAAAAAAull) & low(2 * no));
+  if (mask == nullptr) return;
+  const uint8_t* m0 = mask + (size_t)row * n_valid + col0;
+  const uint8_t* m1 = m0 + (size_t)8 * n_valid;
+  B l0 = 0, l1 = 0;
+#pragma unroll 1
+  for (int k = 0; k < kBits; ++k) {
+    if (!((live[0] >> k) & 1)) break;   // columns grow with k: the first column past n_valid ends the row
+    const int off = 8 * (k >> 1) + (k & 1);
+    if (st0 && m0[off] != 0) l0 |= B(1) << k;
+    if (st1 && m1[off] != 0) l1 |= B(1) << k;
+  }
+  live[0] = l0;
+  live[1] = l1;
+}
+
 // Every column of a tile stored in pairs, with no per-column masks or branches: the hidden layers (RELU; d_hidden is
 // a multiple of 256 and the scratch is 16-byte aligned, so every hidden tile is full and pair-aligned) and a greedy
 // head whose one tile is full and pair-aligned and that takes no actions.  C has n_valid columns.
@@ -277,19 +313,23 @@ __device__ __forceinline__ void store_tile(const float (&acc)[BLOCK_N / 2], cons
 }
 
 // The greedy epilogue of a head tile: logits (C, unless null) masked to the head's n_valid columns over the TMA zero
-// fill, and actions[row] (unless null) the argmax of the row's ROUNDED logits.  The head's one tile holds whole rows
-// (n_valid <= BLOCK_N), so the argmax never leaves the CTA.
+// fill, and actions[row] (unless null) the argmax of the row's ROUNDED logits.  With a legal-action mask only legal
+// columns are ranked (live_columns), a row whose ranked logits are all -inf or that has none takes action 0 as
+// torch.argmax does, and a rolled pass overwrites the stored logits of illegal columns with -inf.  The head's one tile
+// holds whole rows (n_valid <= BLOCK_N), so the argmax never leaves the CTA.
 template <int BLOCK_N>
 __device__ __forceinline__ void greedy_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias,
-                                                __nv_bfloat16* C, int64_t* actions, int col0, int n_valid, int row,
-                                                bool st0, bool st1) {
+                                                __nv_bfloat16* C, int64_t* actions, const uint8_t* mask, int col0,
+                                                int n_valid, int row, bool st0, bool st1) {
   // a column pair is one 4-byte store where the base and an even row stride allow it; rows of an odd d_out are
   // only 2-byte aligned and take scalar stores
   const bool pairs = C != nullptr && (n_valid & 1) == 0 && ((uintptr_t)C & 3) == 0;
-  if (pairs && actions == nullptr && n_valid == BLOCK_N) {
+  if (pairs && actions == nullptr && mask == nullptr && n_valid == BLOCK_N) {
     store_tile<BLOCK_N, false>(acc, bias, C, col0, n_valid, row, st0, st1);
     return;
   }
+  ColBits<BLOCK_N> live[2];
+  live_columns<BLOCK_N>(mask, row, col0, n_valid, st0, st1, live);
   float best[2] = {-INFINITY, -INFINITY};
   int best_col[2] = {INT_MAX, INT_MAX};
 #pragma unroll
@@ -315,7 +355,7 @@ __device__ __forceinline__ void greedy_epilogue(const float (&acc)[BLOCK_N / 2],
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         const int h = q >> 1, c = col + (q & 1);
-        if (c < n_valid && argmax_before(r[q], c, best[h], best_col[h])) {
+        if (((live[h] >> (2 * j + (q & 1))) & 1) && argmax_before(r[q], c, best[h], best_col[h])) {
           best[h] = r[q];
           best_col[h] = c;
         }
@@ -337,36 +377,63 @@ __device__ __forceinline__ void greedy_epilogue(const float (&acc)[BLOCK_N / 2],
       }
     }
     if ((threadIdx.x & 3) == 0) {
-      if (st0) actions[row] = best_col[0];
-      if (st1) actions[row + 8] = best_col[1];
+      if (st0) actions[row] = best[0] == -INFINITY ? 0 : best_col[0];
+      if (st1) actions[row + 8] = best[1] == -INFINITY ? 0 : best_col[1];
+    }
+  }
+  if (mask != nullptr && C != nullptr) {
+    const __nv_bfloat16 ninf = __ushort_as_bfloat16((unsigned short)0xFF80u);
+#pragma unroll 1
+    for (int k = 0; k < BLOCK_N / 4; ++k) {
+      const int col = col0 + 8 * (k >> 1) + (k & 1);
+      if (col >= n_valid) break;
+      if (st0 && !((live[0] >> k) & 1)) C[(size_t)row * n_valid + col] = ninf;
+      if (st1 && !((live[1] >> k) & 1)) C[(size_t)(row + 8) * n_valid + col] = ninf;
     }
   }
 }
 
 // The sampling epilogue of a head tile (HeadKind::kSample): rows r = row and row + 8 of the thread, global rows
-// row_base + r.  Pass 1 rounds the logits once and keeps them as bf16 pairs (half the registers of the fp32
-// accumulators it frees: the 256-wide instantiation would spill holding the accumulators, or the bias, through pass 2)
-// and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum instead); pass 2 draws one
+// row_base + r.  Pass 1 (unrolled over the accumulators) rounds the logits once, parks them as bf16 pairs in the TMA
+// ring as gaussian_epilogue does, and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum
+// instead); pass 2 is a rolled loop, so the Philox code is not repeated BLOCK_N / 8 times (the 256-wide head had
+// 17 576 instructions with it unrolled, and any code added to it, even code the unmasked call skips, made that call
+// 3 % slower, H100 80GB HBM3, 700 W).  It draws one
 // Philox call per column pair < n_valid and row, ranks fp32(logit + noise) in torch.argmax order and sums
 // exp(logit - m) without a running rescale.  A logit equal to m adds 1 without an exp, so an all -inf (or a +inf)
 // maximum never forms exp(inf - inf): such rows end with a NaN log-probability, as in torch, and -inf logits beside a
-// finite m add 0.
-template <int BLOCK_N>
+// finite m add 0.  With a legal-action mask both passes skip illegal columns (live_columns): a -inf logit adds 0 beside
+// a finite or +inf m and never wins the Gumbel-max while a legal logit is finite, so this is the sample of
+// logits.masked_fill(~legal, -inf).  A row whose ranked values are all -inf (every legal logit -inf, or no legal
+// column) takes action 0 with a NaN log-probability, as torch does.
+template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                 int n_valid, int row, bool st0, bool st1, int64_t* actions,
-                                                float* log_probs, uint64_t seed, uint64_t row_base) {
+                                                float* log_probs, const uint8_t* mask, uint64_t seed,
+                                                uint64_t row_base) {
+  using S = MlpSmem<BLOCK_N, STAGES>;
+  static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  // pair w (= 2j + h) of a lane parked as in gaussian_epilogue: stage w / 16, the warp's own 16 A rows, word
+  // (w % 16)·32 + lane
+  uint8_t* mine = smem + (threadIdx.x >> 5) * 16 * 128 + (threadIdx.x & 31) * 4;
+  auto slot = [&](int w) { return reinterpret_cast<__nv_bfloat162*>(mine + (w >> 4) * S::kStageBytes + (w & 15) * 128); };
+  ColBits<BLOCK_N> live[2];
+  live_columns<BLOCK_N>(mask, row, col0, n_valid, st0, st1, live);
   float mx[2] = {-INFINITY, -INFINITY};
-  __nv_bfloat162 y[BLOCK_N / 4];   // y[2j + h]: columns (col, col + 1) of row + 8h
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
     if (col >= n_valid) continue;
-    layer_pair<false>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, y[2 * j],
-                      y[2 * j + 1]);
+    __nv_bfloat162 y[2];   // y[h]: columns (col, col + 1) of row + 8h
+    layer_pair<false>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, y[0], y[1]);
+    *slot(2 * j) = y[0];
+    *slot(2 * j + 1) = y[1];
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
-      const float v = q & 1 ? __high2float(y[2 * j + (q >> 1)]) : __low2float(y[2 * j + (q >> 1)]);
-      if (col + (q & 1) < n_valid && v > mx[q >> 1]) mx[q >> 1] = v;
+      const float v = q & 1 ? __high2float(y[q >> 1]) : __low2float(y[q >> 1]);
+      if (((live[q >> 1] >> (2 * j + (q & 1))) & 1) && v > mx[q >> 1]) mx[q >> 1] = v;
     }
   }
 #pragma unroll
@@ -378,20 +445,21 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
     }
   }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-  float best[2] = {-INFINITY, -INFINITY}, best_y[2] = {0.f, 0.f}, sum[2] = {0.f, 0.f};
+  float best[2] = {-INFINITY, -INFINITY}, best_y[2] = {NAN, NAN}, sum[2] = {0.f, 0.f};
   int best_col[2] = {INT_MAX, INT_MAX};
-#pragma unroll
+#pragma unroll 1
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
-    if (col >= n_valid) continue;   // a pair wholly past the head draws no noise
+    if (col >= n_valid) break;   // a pair wholly past the head draws no noise
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint64_t i = row_base + (uint64_t)(row + 8 * h);
       const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 0u), key);
+      const __nv_bfloat162 y = *slot(2 * j + h);
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
-        if (col + c >= n_valid) continue;
-        const float v = c ? __high2float(y[2 * j + h]) : __low2float(y[2 * j + h]);
+        if (!((live[h] >> (2 * j + c)) & 1)) continue;
+        const float v = c ? __high2float(y) : __low2float(y);
         const float s = v + gumbel_of(c ? x.y : x.x);
         if (argmax_before(s, col + c, best[h], best_col[h])) {
           best[h] = s;
@@ -419,11 +487,11 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   }
   if ((threadIdx.x & 3) == 0) {
     if (st0) {
-      actions[row] = best_col[0];
+      actions[row] = best[0] == -INFINITY ? 0 : best_col[0];
       log_probs[row] = best_y[0] - mx[0] - logf(sum[0]);
     }
     if (st1) {
-      actions[row + 8] = best_col[1];
+      actions[row + 8] = best[1] == -INFINITY ? 0 : best_col[1];
       log_probs[row + 8] = best_y[1] - mx[1] - logf(sum[1]);
     }
   }
@@ -511,7 +579,9 @@ enum class HeadKind {
 };
 
 // The outputs of a layer launch.  A hidden layer stores only its bf16 activation, in `logits`.  Pointers the head
-// kind does not store are null.  Row r of the launch draws the noise of global row row_base + r.
+// kind does not store are null.  Row r of the launch draws the noise of global row row_base + r.  `mask`, unless null,
+// is the greedy or sampling head's legal-action mask [rows, d_out] (nonzero byte: legal), a runtime input of the same
+// instantiations.
 struct HeadOut {
   void* logits = nullptr;
   int64_t* actions = nullptr;
@@ -519,6 +589,7 @@ struct HeadOut {
   uint64_t seed = 0, row_base = 0;
   const float* log_std = nullptr;
   float* gauss_actions = nullptr;
+  const uint8_t* mask = nullptr;
 
   // The same outputs from row r0 of the call on.
   HeadOut from_row(size_t r0, int d_out) const {
@@ -527,6 +598,7 @@ struct HeadOut {
     if (actions) h.actions += r0;
     if (log_probs) h.log_probs += r0;
     if (gauss_actions) h.gauss_actions += r0 * d_out;
+    if (mask) h.mask += r0 * d_out;
     h.row_base += r0;
     return h;
   }
@@ -538,6 +610,7 @@ struct HeadOut {
 // L2 once.  Only rows < rows (A's row count) are stored.  KIND picks the epilogue at compile time:
 //   kHidden (BLOCK_N = 256): C = relu(...), every tile full (store_tile);
 //   kGreedy: logits and/or actions[row] = the argmax of the row's ROUNDED logits (greedy_epilogue);
+//   kGreedy and kSample with out.mask: what the head computes from logits.masked_fill(~legal, -inf);
 //   kSample: the action of global row i = row_base + row is the argmax of fp32(logit_j + g_j) with g_j the Gumbel
 //     noise of Philox word j & 1 of counter (i, j >> 1) under `seed` (include/ktb200.h), and log_probs[row] =
 //     log_softmax(logits)[action] in fp32 (sample_epilogue);
@@ -568,9 +641,9 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   if constexpr (KIND == HeadKind::kHidden) {
     store_tile<BLOCK_N, true>(acc, bias, C, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kGreedy) {
-    greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, col0, n_valid, row, st0, st1);
+    greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, out.mask, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kSample) {
-    sample_epilogue<BLOCK_N>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.seed,
+    sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
                              out.row_base);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
@@ -687,19 +760,29 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 }
 
 // Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
-// and _pushed: no biases and a 64-wide greedy head that stores logits only.
+// and _pushed: no biases and a 64-wide greedy head that stores logits only.  `masked` marks the _masked entries: the
+// head applies a legal-action mask, out.mask in the pull forms and the bytes at MlpFeed::mask_offset of the call's
+// staging half in the pushed forms.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
   HeadOut out;
   bool logits64 = false;
+  bool masked = false;
+
+  MlpParams with_mask(const uint8_t* mask) const {
+    MlpParams p = *this;
+    p.out.mask = mask;
+    p.masked = true;
+    return p;
+  }
 };
 
 // Rows [r0, r0 + rows) of a call: the hidden layers h1 = relu(a1 · W1ᵀ (+ b1)) and h2 = relu(h1 · W2ᵀ (+ b2)), then
-// the head from h2 in the smallest tile that holds d_out.  `consumed`, unless null, is recorded once layer 1 has read
-// a1.
-static int mlp_chunk(int dev, const MlpParams& p, const void* a1, void* h1, void* h2, size_t r0, size_t rows, int d_in,
-                     int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
+// the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds d_out.
+// `consumed`, unless null, is recorded once layer 1 has read a1.
+static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void* a1, void* h1, void* h2, size_t r0,
+                     size_t rows, int d_in, int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
   int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
   if (rc) return rc;
   if (consumed) KTB_CK(cudaEventRecord(consumed, st));
@@ -708,7 +791,7 @@ static int mlp_chunk(int dev, const MlpParams& p, const void* a1, void* h1, void
   const auto head = p.kind == HeadKind::kGreedy   ? launch_head<HeadKind::kGreedy>
                     : p.kind == HeadKind::kSample ? launch_head<HeadKind::kSample>
                                                   : launch_head<HeadKind::kGaussian>;
-  return head(dev, h2, p.W3, p.b3, p.out.from_row(r0, d_out), rows, d_out, d_hidden, st);
+  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, d_out, d_hidden, st);
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -757,7 +840,9 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //           stage stream while the previous chunk computes, and layer 1 reads it there.
 //   pushed: the root pushes the rows into half seq & 1 of `in` (stage_local, halves `stride` bytes apart) and publishes
 //           ready[c] = seq in this rank's control block `ctrl`; layer 1 of chunk c waits in-stream for it, and the
-//           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.
+//           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A masked head reads
+//           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows).
+// The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
   size_t chunk_rows;
@@ -767,17 +852,24 @@ struct MlpFeed {
   void *ctrl = nullptr, *ctrl_root = nullptr;
   int rank = 0;
   unsigned long long seq = 0;
+  size_t mask_offset = 0;
 
   static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
   static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
                       unsigned long long seq) {
     return {stage_local, chunk_rows, nullptr, true, stride, ctrl, ctrl_root, rank, seq};
   }
+  MlpFeed with_mask_offset(size_t off) const {
+    MlpFeed f = *this;
+    f.mask_offset = off;
+    return f;
+  }
 };
 
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
 // right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
-// ktb_push_wait waits for.
+// ktb_push_wait waits for.  A masked entry's own checks (a mask in the pull forms, mask_offset inside the staging half
+// and past the rows in the pushed forms) come after every check of the unmasked entry.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -807,6 +899,14 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     // layer 1 reads half seq & 1 through a tensor map, whose base TMA needs 16-byte aligned
     KTB_REQUIRE(f.stride % 16 == 0, KTB_ERR_ARG, "%s: stage_stride=%zu must be a multiple of 16", fn, f.stride);
   }
+  if (p.masked && f.pushed) {
+    KTB_REQUIRE(f.mask_offset >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: mask_offset=%zu overlaps the rows", fn,
+                f.mask_offset);
+    KTB_REQUIRE(f.mask_offset <= f.stride && M * (size_t)d_out <= f.stride - f.mask_offset, KTB_ERR_ARG,
+                "%s: mask_offset=%zu + M*d_out exceeds stage_stride", fn, f.mask_offset);
+  } else if (p.masked) {
+    KTB_REQUIRE(p.out.mask, KTB_ERR_ARG, "%s: null mask", fn);   // M > 0 here: an empty pull call has returned
+  }
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
@@ -817,6 +917,8 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   // the call's rows: obs, or this call's staging half (the pull forms have seq = stride = 0)
   const __nv_bfloat16* x =
       reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride);
+  HeadOut out = p.out;
+  if (p.masked && f.pushed) out.mask = reinterpret_cast<const uint8_t*>(x) + f.mask_offset;
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
   cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
@@ -865,7 +967,7 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       a1 = dstb;
     }
     // evs[3..4] are null unless staged
-    rc = mlp_chunk(dev, p, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
+    rc = mlp_chunk(dev, p, out, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
     if (rc) return rc;
   }
   if (!f.pushed) return KTB_OK;
@@ -931,6 +1033,27 @@ int ktb_mlp_bf16_policy_pushed(int dev, const void* stage_local, size_t stage_st
                  stream);
 }
 
+int ktb_mlp_bf16_policy_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                               const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                               const uint8_t* mask, void* logits, int64_t* actions, void* scratch, void* stage,
+                               uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}}.with_mask(mask);
+  return mlp_run("ktb_mlp_bf16_policy_masked", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                      int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                      const void* b2, const void* W3, const void* b3, size_t mask_offset, void* logits,
+                                      int64_t* actions, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                      size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}}.with_mask(nullptr);
+  return mlp_run("ktb_mlp_bf16_policy_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset),
+                 scratch, stream);
+}
+
 int ktb_mlp_bf16_policy_sample(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
                                const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
                                uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs, void* scratch,
@@ -950,6 +1073,31 @@ int ktb_mlp_bf16_policy_sample_pushed(int dev, const void* stage_local, size_t s
   return mlp_run("ktb_mlp_bf16_policy_sample_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
                  stream);
+}
+
+int ktb_mlp_bf16_policy_sample_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                      const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                      const void* b3, const uint8_t* mask, uint64_t seed, uint64_t row_base,
+                                      int64_t* actions, float* log_probs, void* scratch, void* stage,
+                                      uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}}
+                          .with_mask(mask);
+  return mlp_run("ktb_mlp_bf16_policy_sample_masked", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                             int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                             const void* b2, const void* W3, const void* b3, size_t mask_offset,
+                                             uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs,
+                                             void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                             size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}}
+                          .with_mask(nullptr);
+  return mlp_run("ktb_mlp_bf16_policy_sample_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset),
+                 scratch, stream);
 }
 
 int ktb_mlp_bf16_policy_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,

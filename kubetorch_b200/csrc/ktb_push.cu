@@ -337,17 +337,36 @@ int ktb_push_scatter_chunked(int root_dev, const void* src_root, size_t n_elems,
 }
 
 // ---- copy-engine form of the root side: no SM of the root is used ------------------------------------------------
-int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype, int n_ranks,
-                        int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
-                        void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, unsigned long long seq,
-                        uintptr_t stream) {
-  int rc = check_push_scatter("ktb_push_scatter_ce", root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank,
-                              stage_peer, stage_stride, ctrl_peer, ctrl_root, seq);
+// With `with_side`, a second source rides along: row i of the shard (granule elements) has row_bytes bytes at
+// side + i·row_bytes, and they land side_offset bytes into the rank's staging half, chunk by chunk beside the rows and
+// behind the same ack wait, with ready[c] published after both copies of chunk c.  Its checks come after every check
+// of the plain form.
+static int push_scatter_ce_impl(const char* who, int root_dev, const void* src_root, size_t n_elems, size_t granule,
+                                int dtype, int n_ranks, int root_rank, const int* devs, void* const* stage_peer,
+                                size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
+                                bool with_side, const void* side, size_t row_bytes, size_t side_offset,
+                                unsigned long long seq, uintptr_t stream) {
+  int rc = check_push_scatter(who, root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank, stage_peer,
+                              stage_stride, ctrl_peer, ctrl_root, seq);
   if (rc) return rc;
-  KTB_REQUIRE(devs && chunk_elems > 0, KTB_ERR_ARG, "ktb_push_scatter_ce: null devs or zero chunk_elems");
+  KTB_REQUIRE(devs && chunk_elems > 0, KTB_ERR_ARG, "%s: null devs or zero chunk_elems", who);
   const int n_chunks = push_chunk_count(n_elems, granule, n_ranks, chunk_elems);
-  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "ktb_push_scatter_ce: more than %d chunks", KTB_PUSH_MAX_CHUNKS);
+  KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: more than %d chunks", who, KTB_PUSH_MAX_CHUNKS);
   const size_t es = dtype_size(dtype);
+  if (with_side) {
+    KTB_REQUIRE(side || n_elems == 0, KTB_ERR_ARG, "%s: null mask", who);
+    KTB_REQUIRE(row_bytes > 0 && chunk_elems % granule == 0, KTB_ERR_ARG,
+                "%s: row_bytes must be positive and chunk_elems whole rows", who);
+    for (int r = 0; r < n_ranks; ++r) {
+      if (r == root_rank || !stage_peer[r]) continue;
+      size_t b = 0, e = 0;
+      ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
+      KTB_REQUIRE(side_offset >= (e - b) * granule * es, KTB_ERR_ARG, "%s: mask_offset overlaps the rows of rank %d",
+                  who, r);
+      KTB_REQUIRE(side_offset <= stage_stride && (e - b) * row_bytes <= stage_stride - side_offset, KTB_ERR_ARG,
+                  "%s: mask of rank %d exceeds stage_stride", who, r);
+    }
+  }
   KTB_GUARD(root_dev);
   // one library stream (and fork/join event pair) per destination rank on the root device, created on first use:
   // every peer's copies ride their own copy-engine queue, chunk-major issue order
@@ -388,6 +407,11 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
       if (hi > lo)
         KTB_CK(cudaMemcpyPeerAsync(static_cast<uint8_t*>(stage_peer[r]) + buf_off + lo * es, devs[r],
                                    static_cast<const uint8_t*>(src_root) + (sb[r] + lo) * es, root_dev, (hi - lo) * es, cs));
+      if (hi > lo && side != nullptr)   // the same rows' second source, beside them
+        KTB_CK(cudaMemcpyPeerAsync(
+            static_cast<uint8_t*>(stage_peer[r]) + buf_off + side_offset + lo / granule * row_bytes, devs[r],
+            static_cast<const uint8_t*>(side) + (sb[r] + lo) / granule * row_bytes, root_dev,
+            (hi - lo) / granule * row_bytes, cs));
       unsigned long long* ready =
           reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctrl_peer[r]) + KTB_CTRL_READY) + c;
       rc = launch_flag_publish(ready, seq, cs);   // stream-ordered behind the copy
@@ -400,6 +424,25 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
     KTB_CK(cudaStreamWaitEvent(st, ce_done[root_dev][r], 0));
   }
   return KTB_OK;
+}
+
+int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype, int n_ranks,
+                        int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
+                        void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, unsigned long long seq,
+                        uintptr_t stream) {
+  return push_scatter_ce_impl("ktb_push_scatter_ce", root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank,
+                              devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, false, nullptr, 0, 0,
+                              seq, stream);
+}
+
+int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
+                               int n_ranks, int root_rank, const int* devs, void* const* stage_peer,
+                               size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
+                               const void* mask_root, size_t row_bytes, size_t mask_offset, unsigned long long seq,
+                               uintptr_t stream) {
+  return push_scatter_ce_impl("ktb_push_scatter_ce_masked", root_dev, src_root, n_elems, granule, dtype, n_ranks,
+                              root_rank, devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, true,
+                              mask_root, row_bytes, mask_offset, seq, stream);
 }
 
 int ktb_push_consume(int dev, int op, int dtype, const void* stage_local, size_t stage_stride, void* dst_root_shard,

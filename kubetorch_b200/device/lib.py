@@ -78,6 +78,9 @@ _SIGNATURES = {
                                          c_uintptr]),
     "ktb_push_scatter_ce": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int, c_int, POINTER(c_int), POINTER(c_void_p),
                                     c_size_t, POINTER(c_void_p), c_void_p, c_size_t, ctypes.c_ulonglong, c_uintptr]),
+    "ktb_push_scatter_ce_masked": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int, c_int, POINTER(c_int),
+                                           POINTER(c_void_p), c_size_t, POINTER(c_void_p), c_void_p, c_size_t,
+                                           c_void_p, c_size_t, c_size_t, ctypes.c_ulonglong, c_uintptr]),
     "ktb_push_consume": (c_int, [c_int, c_int, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_double, c_double,
                                  c_void_p, c_void_p, c_int, c_int, ctypes.c_ulonglong, c_uintptr]),
     "ktb_push_wait": (c_int, [c_int, c_void_p, c_int, c_int, ctypes.c_ulonglong, c_uintptr]),
@@ -112,6 +115,22 @@ _SIGNATURES = {
                                                     c_void_p, ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_void_p,
                                                     c_void_p, c_void_p, c_void_p, c_int, c_size_t, ctypes.c_ulonglong,
                                                     c_uintptr]),
+    "ktb_mlp_bf16_policy_masked": (c_int, [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_uintptr]),
+    "ktb_mlp_bf16_policy_masked_pushed": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int, c_int,
+                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                  c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                                  c_size_t, ctypes.c_ulonglong, c_uintptr]),
+    "ktb_mlp_bf16_policy_sample_masked": (c_int, [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p,
+                                                  c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                  ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_void_p, c_void_p,
+                                                  c_void_p, c_uintptr]),
+    "ktb_mlp_bf16_policy_sample_masked_pushed": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int, c_int,
+                                                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                         c_size_t, ctypes.c_uint64, ctypes.c_uint64, c_void_p,
+                                                         c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_size_t,
+                                                         ctypes.c_ulonglong, c_uintptr]),
     # experiment knob, not in the stable header
     "ktb_set_tuning": (c_int, [c_int, c_int]),
 }

@@ -1,7 +1,8 @@
 """bf16 MLP policy (BASELINE config C4) on wgmma tensor cores — tensor-facing wrapper of
 ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions), ktb_mlp_bf16_policy_sample (seeded
 Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_mlp_bf16_policy_gaussian (seeded
-diagonal-Gaussian actions with their log-probabilities) and their scatter→exec→gather form."""
+diagonal-Gaussian actions with their log-probabilities), the _masked forms of the first two (a per-row legal-action
+mask) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -55,14 +56,18 @@ def _thread_pool():
 MAX_D_OUT = 256
 
 
-def _check_policy(w1, w3, biases, output, seed=None, log_std=None) -> None:
-    """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed or
-    (output="gaussian") a log_std the kernels do not take.  A seed is an int (not a bool) in [0, 2**64); log_std is
-    a 1-D contiguous CUDA float32 tensor of length d_out, given with output="gaussian" only."""
+def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None) -> None:
+    """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
+    (output="gaussian") a log_std or a legal-action mask the kernels do not take.  A seed is an int (not a bool) in
+    [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with output="gaussian" only; a
+    mask is a contiguous CUDA torch.bool tensor [M, d_out] on the device of obs [M, d_in], given with any output but
+    "gaussian"."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
     if output in ("sample", "gaussian"):
         _check_seed(seed)
+    if mask is not None and output == "gaussian":
+        raise ValueError('mask is an argument of the categorical outputs, not of output="gaussian"')
     if len(biases) != 3:
         raise ValueError("biases must be (b1, b2, b3), each a tensor or None")
     d_hidden, d_out = w1.shape[0], w3.shape[0]
@@ -74,6 +79,17 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None) -> None:
     elif not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32 or not log_std.is_cuda \
             or not log_std.is_contiguous() or log_std.dim() != 1 or log_std.shape[0] != d_out:
         raise ValueError(f"log_std must be a 1-D contiguous CUDA float32 tensor of length {d_out}")
+    if mask is not None:
+        if not isinstance(obs, torch.Tensor):
+            raise ValueError("a mask is checked against obs: pass the obs [M, d_in] it goes with")
+        if not isinstance(mask, torch.Tensor) or mask.dtype != torch.bool:
+            raise ValueError("mask must be a torch.bool tensor")
+        if tuple(mask.shape) != (obs.shape[0], d_out):
+            raise ValueError(f"mask must have shape ({obs.shape[0]}, {d_out}), got {tuple(mask.shape)}")
+        if not mask.is_contiguous():
+            raise ValueError("mask must be contiguous")
+        if not mask.is_cuda or mask.device != obs.device:
+            raise ValueError(f"mask must be a CUDA tensor on the device of obs ({obs.device}), got {mask.device}")
     for name, b, n in zip(("b1", "b2", "b3"), biases, (d_hidden, d_hidden, d_out)):
         if b is None:
             continue
@@ -99,15 +115,17 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs):
             buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian") else None)
 
 
-def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False):
+def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
-    pointers as ptr(tensor) gives them."""
-    suffix = "_pushed" if pushed else ""
+    pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
+    mask's address in the pull forms, its offset in the staging half in the pushed forms."""
+    suffix = ("" if mask is None else "_masked") + ("_pushed" if pushed else "")
+    masked = () if mask is None else (mask,)
     if output == "gaussian":
         return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs))
     if output == "sample":
-        return "ktb_mlp_bf16_policy_sample" + suffix, (seed, row_base, ptr(actions), ptr(log_probs))
-    return "ktb_mlp_bf16_policy" + suffix, (ptr(logits), ptr(actions))
+        return "ktb_mlp_bf16_policy_sample" + suffix, (*masked, seed, row_base, ptr(actions), ptr(log_probs))
+    return "ktb_mlp_bf16_policy" + suffix, (*masked, ptr(logits), ptr(actions))
 
 
 def _rows(bufs, b, e):
@@ -131,7 +149,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 stream: Optional[torch.cuda.Stream] = None, staged: Optional[bool] = None,
                 biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
                 actions: Optional[torch.Tensor] = None, seed: Optional[int] = None, row_offset: int = 0,
-                log_probs: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None):
+                log_probs: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
+                mask: Optional[torch.Tensor] = None):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -141,7 +160,10 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     log_probs): fp32 actions[M, d_out] = logits + exp(log_std)·normal_noise(seed, row_offset, M, d_out) and the fp32
     log-density of each row's action under Normal(logits, exp(log_std)); no logits are written).  `obs` / `out` /
     `actions` / `log_probs` may be peer-mapped (pull the observations / push the results over NVLink).  Without
-    biases, at d_out == 64 and with logits only the logits equal ktb_mlp_bf16's."""
+    biases, at d_out == 64 and with logits only the logits equal ktb_mlp_bf16's.  `mask`, a bool [M, d_out] tensor on
+    the device of obs (True: legal), applies a per-row legal-action mask to every output but "gaussian": the head
+    computes logits.masked_fill(~mask, -inf) and stores, ranks and samples those masked logits; an all-True mask gives
+    the unmasked bits."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -151,7 +173,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
-    _check_policy(w1, w3, biases, output, seed, log_std)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs)
     if output in ("sample", "gaussian") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
@@ -160,7 +182,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
-    entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr)
+    entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
+                        mask=None if mask is None else ptr(mask))
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
@@ -192,7 +215,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
-                               seed=None, log_std=None) -> None:
+                               seed=None, log_std=None, mask=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -200,13 +223,17 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     device (biases may be None); out_root / actions_root / log_probs_root are None when `output` does not want them
     (with "gaussian", actions_root holds the fp32 actions [M, d_out]).  log_std[dev] is the Gaussian head's log_std on
     that device.  With output="sample" or "gaussian" rank r draws the noise of global rows b_r .. e_r - 1 (its shard's
-    place in obs_root)."""
+    place in obs_root).  A legal-action `mask` [M, d_out] on the root travels with its rows: the copy engines push each
+    rank's mask rows into the same staging half, 256-byte aligned after the largest shard's observation rows, so no
+    rank reads the root's memory."""
     root, n, key = devs[0], len(devs), tuple(devs)
     d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0]
     rows = max(e - b for b, e in bounds)
+    mask_offset = (rows * d_in * 2 + 255) // 256 * 256
+    stage_bytes = rows * d_in * 2 if mask is None else mask_offset + rows * d_out
     sess = _push_sessions.get(key)
-    if sess is None or sess.stride < rows * d_in * 2:
-        sess = _push_sessions[key] = ops.PushSession(devs, rows * d_in * 2)
+    if sess is None or sess.stride < stage_bytes:
+        sess = _push_sessions[key] = ops.PushSession(devs, stage_bytes)
     try:
         seq = sess.begin()
     except ops.PushTimeout:
@@ -225,17 +252,22 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         logits, actions, log_probs = _rows(bufs, b0, e0)
         mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=logits, device=root, stream=sess.fork(), staged=False,
                     biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
-                    log_std=None if log_std is None else log_std[root])
-    L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
-           L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
-           PUSH_CHUNK_ROWS * d_in, seq, streams[0])
+                    log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0])
+    scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
+               PUSH_CHUNK_ROWS * d_in)
+    if mask is None:
+        L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, *scatter, seq,
+               streams[0])
+    else:
+        L.call("ktb_push_scatter_ce_masked", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
+               *scatter, mask.data_ptr(), d_out, mask_offset, seq, streams[0])
 
     def issue(r):
         b, e = bounds[r]
         ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
         entry, head = _head(output, *_rows(bufs, b, e), seed, b, None if log_std is None else log_std[devs[r]], ptr,
-                            pushed=True)
+                            pushed=True, mask=None if mask is None else mask_offset)
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -248,19 +280,21 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        out_root: Optional[torch.Tensor] = None, transfer: str = "auto",
                        biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
                        actions_root: Optional[torch.Tensor] = None, seed: Optional[int] = None,
-                       log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None) -> list:
+                       log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
+                       mask: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
     int64 actions views for "actions", (logits, actions) pairs for "both", (actions, log_probs) pairs for "sample"
     and "gaussian" (fp32 actions [rows, d_out] with the latter).  With "sample" or "gaussian" rank r draws the noise of
     the global rows of its shard (row_offset = its shard's begin), so the result does not depend on the number of
-    ranks or their devices.  `biases`, `seed` and `log_std` as in mlp_forward."""
+    ranks or their devices.  `biases`, `seed`, `log_std` and `mask` as in mlp_forward; the mask lives on the root GPU
+    and each rank applies its rows of it (read in place by the pull form, pushed with the rows by the push form)."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed, log_std)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root)
@@ -279,7 +313,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs, seed, log_stds)
+        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs, seed, log_stds, mask)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -301,7 +335,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
             logits, actions, log_probs = _rows(bufs, b, e)
             mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=st, biases=ws[3:],
                         output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
-                        log_std=None if log_stds is None else log_stds[dev])
+                        log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e])
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

@@ -77,14 +77,17 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     row's action; the callable is ``(obs, w1, b1, w2, b2, w3, b3, log_std, seed)``).  ``seed``, required with
     ``output="sample"`` or ``"gaussian"`` and refused otherwise: an int in [0, 2**64) or the name of a call argument
     that holds one.  ``log_std``, required with ``output="gaussian"`` and refused otherwise: the name of the call
-    argument that holds the fp32 [d_out] log standard deviation."""
+    argument that holds the fp32 [d_out] log standard deviation.  ``mask``, an option of every output but
+    ``"gaussian"``: the name of the call argument that holds a per-row legal-action mask, a bool [M, d_out] tensor on
+    the device of obs (True: legal); the head then computes ``logits.masked_fill(~mask, -inf)`` and every output is
+    taken from those masked logits (the body applies ``legal.chunk(WORLD_SIZE)[RANK]`` to its rows)."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if "bias" in extra or "output" in extra or "seed" in extra or "log_std" in extra:
+    if "bias" in extra or "output" in extra or "seed" in extra or "log_std" in extra or "mask" in extra:
         if op != "mlp":
-            raise ValueError(f"bias=, output=, seed= and log_std= are options of the 'mlp' op, not of '{op}'")
+            raise ValueError(f"bias=, output=, seed=, log_std= and mask= are options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
@@ -101,11 +104,17 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
             raise ValueError('log_std= is required with output="gaussian" and is an option of that output only')
         if gaussian and not isinstance(extra["log_std"], str):
             raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
+        if "mask" in extra:
+            if gaussian:
+                raise ValueError('mask= is an option of the categorical outputs, not of output="gaussian"')
+            if not isinstance(extra["mask"], str):
+                raise ValueError(f"mask must be the name of a call argument, got {extra['mask']!r}")
 
     def deco(fn):
-        name = extra.get("log_std")
-        if name is not None and name not in inspect.signature(fn).parameters:
-            raise ValueError(f"log_std={name!r} is not an argument of {getattr(fn, '__name__', fn)!r}")
+        for option in ("log_std", "mask"):
+            name = extra.get(option)
+            if name is not None and name not in inspect.signature(fn).parameters:
+                raise ValueError(f"{option}={name!r} is not an argument of {getattr(fn, '__name__', fn)!r}")
         setattr(fn, MAPPED_ATTR, MappedSpec(op=op, alpha=alpha, beta=beta, reduce=reduce, arg=arg, extra=extra))
         return fn
 

@@ -582,9 +582,14 @@ class B200Supervisor:
             if log_std not in bound:
                 raise TypeError(f"mapped mlp callable: log_std argument '{log_std}' not found in the call")
             log_std = bound[log_std]
+        mask = spec.extra.get("mask")
+        if mask is not None:   # always the name of a call argument, resolved per call
+            if mask not in bound:
+                raise TypeError(f"mapped mlp callable: mask argument '{mask}' not found in the call")
+            mask = bound[mask]
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
-                                         biases=biases, output=output, seed=seed, log_std=log_std)
+                                         biases=biases, output=output, seed=seed, log_std=log_std, mask=mask)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -14,11 +14,14 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      same alternation as d (actions only), which has the same GEMMs and no noise
   h  policy with biases, d_out 6, 18 and 64, Gaussian actions and log-probabilities (output="gaussian", log_std over
      [-2, 0.5]), timed in the same alternation beside the logits-only call and output="sample" at the same d_out
+  i  policy with biases, d_out 18, 64 and 256, a random legal-action mask (about 50 % legal): masked actions right
+     after the same unmasked call, and masked sampled actions right after the unmasked output="sample" call
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
 exceeds 2^-18·(1 + max|s|), and the log-probability is within (d_out + 8)·2^-22·(1 + |ref|) of the fp64 log_softmax.
-Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+Masked rows: the masked actions equal torch.argmax of the kernel's logits filled with -inf on every row, and every
+sampled action on a row with a legal action is legal.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -118,6 +121,18 @@ def main():
         variants[f"h_bias_gaussian_d{d}"] = (d, lambda d=d: mlp.mlp_forward(
             obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]), output="gaussian", seed=SEED,
             log_std=log_stds[d]))
+    gm = torch.Generator(device="cuda:0").manual_seed(7)
+    legal = {d: torch.rand(M, d, device="cuda:0", generator=gm) < 0.5 for d in (18, 64, 256)}
+    for d in (18, 64, 256):
+        bs = (b1, b2, heads[d][1])
+        variants[f"i_bias_actions_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, output="actions"))
+        variants[f"i_bias_masked_actions_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, output="actions", mask=legal[d]))
+        variants[f"i_bias_sample_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED))
+        variants[f"i_bias_masked_sample_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED, mask=legal[d]))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -188,6 +203,17 @@ def main():
         tol = 2.0 ** -20 * ((1 + z.abs()) ** 2).sum(-1) + (d + 8) * 2.0 ** -23 * (t.abs().sum(-1) + d * 0.92)
         assert bool(((log_probs[r0:r0 + 2048].double() - ref).abs() <= tol).all())
         parity[f"h_bias_gaussian_d{d}"] = {"gaussian_bars_2048_rows": "ok"}
+
+    for d in (18, 64, 256):
+        logits = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]))
+        actions = variants[f"i_bias_masked_actions_d{d}"][1]()
+        assert torch.equal(actions, logits.masked_fill(~legal[d], float("-inf")).argmax(-1))
+        del logits
+        sampled, _ = variants[f"i_bias_masked_sample_d{d}"][1]()
+        has = legal[d].any(-1)
+        assert bool(legal[d][has].gather(1, sampled[has][:, None]).all())
+        parity[f"i_bias_masked_d{d}"] = {"masked_actions_eq_masked_argmax_all_rows": "ok",
+                                         "sampled_actions_legal_all_rows": "ok"}
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
