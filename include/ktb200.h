@@ -447,6 +447,56 @@ int ktb_mlp_bf16_policy_sample_masked_pushed(int dev, const void* stage_local, s
                                              void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
                                              size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* Value forms: the sampling, masked sampling and Gaussian entries with a value head V(s) on the same trunk, the critic
+ * nn.Linear(d_hidden, 1) of a shared-trunk actor-critic.
+ *   - W3v [d_out + 1, d_hidden] bf16 is the policy's W3 with the critic's weight wv [1, d_hidden] stacked under it, and
+ *     b3v [d_out + 1] is b3 with the critic's bias bv after it, or NULL when neither has a bias.  d_out stays the
+ *     policy's width.
+ *   - values[i] = fp32(bf16(h2_i . wv + bv)): column d_out of the head, rounded once to bf16 with the bias in the fp32
+ *     accumulator (F.linear), then widened exactly to fp32.  It is the value column d_out of ktb_mlp_bf16_policy's
+ *     logits for the same W3v and b3v.
+ *   - Actions and log-probabilities have the bits of the entry without a value head over W3 and b3: the value column
+ *     is never ranked, sampled, summed into the softmax or given a log_std, and it draws no Philox noise.  A
+ *     legal-action mask [M, d_out] never touches the values.
+ *   - values [M] fp32 follows log_probs and may be a peer pointer.  With M > 0, a NULL or not 4-byte aligned values is
+ *     KTB_ERR_ARG and d_out = 256 is KTB_ERR_UNSUPPORTED (the d_out + 1 columns must fit one 256-wide tile); these are
+ *     checked after every check of the entry without a value head.  An empty pushed shard (M == 0) may pass NULL
+ *     outputs and still publishes its ack.  Writes stay inside the outputs of that entry, values[M], scratch and
+ *     stage. */
+int ktb_mlp_bf16_policy_sample_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                     const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v,
+                                     const void* b3v, uint64_t seed, uint64_t row_base, int64_t* actions,
+                                     float* log_probs, float* values, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                            int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                            const void* b2, const void* W3v, const void* b3v, uint64_t seed,
+                                            uint64_t row_base, int64_t* actions, float* log_probs, float* values,
+                                            void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                            size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_masked_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                            const void* W1, const void* b1, const void* W2, const void* b2,
+                                            const void* W3v, const void* b3v, const uint8_t* mask, uint64_t seed,
+                                            uint64_t row_base, int64_t* actions, float* log_probs, float* values,
+                                            void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_masked_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                   int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                   const void* W2, const void* b2, const void* W3v, const void* b3v,
+                                                   size_t mask_offset, uint64_t seed, uint64_t row_base,
+                                                   int64_t* actions, float* log_probs, float* values, void* scratch,
+                                                   void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                   unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v,
+                                       const void* b3v, const float* log_std, uint64_t seed, uint64_t row_base,
+                                       float* actions, float* log_probs, float* values, void* scratch, void* stage,
+                                       uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                              int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                              const void* b2, const void* W3v, const void* b3v, const float* log_std,
+                                              uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
+                                              float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                              int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

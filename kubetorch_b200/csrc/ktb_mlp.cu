@@ -13,7 +13,8 @@
 //     for the head one of: logits masked to its width and/or the greedy action of every row; an
 //     action sampled by seeded Gumbel-max with its log-probability (either of these two optionally under a per-row
 //     legal-action mask, a runtime input); or Gaussian actions with their
-//     log-probability — the head's outputs may be peer pointers into the root GPU's result arena,
+//     log-probability (the sampled and Gaussian heads optionally with a critic's state value, one more head column,
+//     also a runtime input) — the head's outputs may be peer pointers into the root GPU's result arena,
 //     which fuses the gather into the epilogue.
 // Warp roles (288 threads): warps 0-7 = two consumer warpgroups, warp 8 = TMA producer (one lane).
 // Activations are rounded to bf16 between layers (like the eager torch module); rows are processed
@@ -393,6 +394,20 @@ __device__ __forceinline__ void greedy_epilogue(const float (&acc)[BLOCK_N / 2],
   }
 }
 
+// The value column d of a head tile with a value head, which pass 1 of the sampling and Gaussian epilogues parked
+// with the policy's columns: bf16 pair 2·(d >> 3) + h of the lane whose columns include d (col0 = 2·(lane % 4) in the
+// head's one tile), element d & 1.  That lane widens it to fp32 into values[row + 8h] of the stored rows.  It reads
+// the ring rather than acc[]: a run-time index into the accumulators would put them in local memory.
+template <typename Slot>
+__device__ __forceinline__ void store_values(Slot slot, int d, int row, bool st0, bool st1, float* values) {
+  if (values == nullptr || (int)(threadIdx.x & 3) != ((d >> 1) & 3)) return;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const __nv_bfloat162 y = *slot(2 * (d >> 3) + h);
+    if (h ? st1 : st0) values[row + 8 * h] = d & 1 ? __high2float(y) : __low2float(y);
+  }
+}
+
 // The sampling epilogue of a head tile (HeadKind::kSample): rows r = row and row + 8 of the thread, global rows
 // row_base + r.  Pass 1 (unrolled over the accumulators) rounds the logits once, parks them as bf16 pairs in the TMA
 // ring as gaussian_epilogue does, and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum
@@ -406,11 +421,13 @@ __device__ __forceinline__ void greedy_epilogue(const float (&acc)[BLOCK_N / 2],
 // a finite or +inf m and never wins the Gumbel-max while a legal logit is finite, so this is the sample of
 // logits.masked_fill(~legal, -inf).  A row whose ranked values are all -inf (every legal logit -inf, or no legal
 // column) takes action 0 with a NaN log-probability, as torch does.
+// With a value head (values != null) the tile holds n_valid = d + 1 columns: the policy's d, then the value column d.
+// Pass 1 parks column d with the rest; everything ranked, drawn, summed or masked stops at d; store_values reads it.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                 int n_valid, int row, bool st0, bool st1, int64_t* actions,
                                                 float* log_probs, const uint8_t* mask, uint64_t seed,
-                                                uint64_t row_base) {
+                                                uint64_t row_base, float* values) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -419,8 +436,9 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   // (w % 16)·32 + lane
   uint8_t* mine = smem + (threadIdx.x >> 5) * 16 * 128 + (threadIdx.x & 31) * 4;
   auto slot = [&](int w) { return reinterpret_cast<__nv_bfloat162*>(mine + (w >> 4) * S::kStageBytes + (w & 15) * 128); };
+  const int d = n_valid - (values != nullptr);   // the policy's columns
   ColBits<BLOCK_N> live[2];
-  live_columns<BLOCK_N>(mask, row, col0, n_valid, st0, st1, live);
+  live_columns<BLOCK_N>(mask, row, col0, d, st0, st1, live);
   float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -450,11 +468,12 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
 #pragma unroll 1
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
-    if (col >= n_valid) break;   // a pair wholly past the head draws no noise
+    if (col >= d) break;   // a pair wholly past the policy draws no noise
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const uint64_t i = row_base + (uint64_t)(row + 8 * h);
       const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 0u), key);
+      // (column d of a value head is never live: live_columns stops at d)
       const __nv_bfloat162 y = *slot(2 * j + h);
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
@@ -470,6 +489,7 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
       }
     }
   }
+  store_values(slot, d, row, st0, st1, values);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -506,10 +526,13 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
 // and row (counter word 3 = 1: never the Gumbel stream's uniforms), z = Φ⁻¹(u) (normcdfinvf, no fast-math; u is never
 // 0.5, so z != 0), the action μ + σ·z rounded twice (no FMA contraction), stored as float2 where the row stride and the
 // base allow and as scalars otherwise, and Σ (0.5·z² + log_std) per row for the log-probability, which does not read μ.
+// With a value head (values != null) the tile holds n_valid = d + 1 columns, as in sample_epilogue: the rolled pass,
+// the actions' row stride and the log-density's constant cover the policy's d columns only.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                   int n_valid, int row, bool st0, bool st1, const float* log_std,
-                                                  float* actions, float* log_probs, uint64_t seed, uint64_t row_base) {
+                                                  float* actions, float* log_probs, uint64_t seed, uint64_t row_base,
+                                                  float* values) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -524,15 +547,16 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
     layer_pair<false>(acc[4 * j], acc[4 * j + 1], acc[4 * j + 2], acc[4 * j + 3], bias, col, n_valid, *slot(2 * j),
                       *slot(2 * j + 1));
   }
+  const int d = n_valid - (values != nullptr);   // the policy's columns
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-  const bool pairs = (n_valid & 1) == 0 && ((uintptr_t)actions & 7) == 0;
+  const bool pairs = (d & 1) == 0 && ((uintptr_t)actions & 7) == 0;
   float sum[2] = {0.f, 0.f};
 #pragma unroll 1
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
-    if (col >= n_valid) break;   // a pair wholly past the head draws no noise
+    if (col >= d) break;   // a pair wholly past the policy draws no noise
     const __nv_bfloat162 y[2] = {*slot(2 * j), *slot(2 * j + 1)};
-    const bool has1 = col + 1 < n_valid;
+    const bool has1 = col + 1 < d;
     const float ls[2] = {log_std[col], has1 ? log_std[col + 1] : 0.f};
     const float sg[2] = {expf(ls[0]), expf(ls[1])};
 #pragma unroll
@@ -548,7 +572,7 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
         if (c == 0 || has1) sum[h] += 0.5f * z * z + ls[c];
       }
       if (!(h ? st1 : st0)) continue;
-      float* p = actions + (size_t)(row + 8 * h) * n_valid + col;
+      float* p = actions + (size_t)(row + 8 * h) * d + col;
       if (pairs) {
         *reinterpret_cast<float2*>(p) = make_float2(a[0], a[1]);
       } else {
@@ -557,6 +581,7 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
       }
     }
   }
+  store_values(slot, d, row, st0, st1, values);
   // the 4 lanes of a quad hold the columns of the same two rows
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -564,7 +589,7 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
     for (int m = 1; m <= 2; m <<= 1) sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
   }
   if ((threadIdx.x & 3) == 0) {
-    const float c = (float)n_valid * 0.918938533204672742f;   // d_out·0.5·log(2π)
+    const float c = (float)d * 0.918938533204672742f;   // d_out·0.5·log(2π)
     if (st0) log_probs[row] = -sum[0] - c;
     if (st1) log_probs[row + 8] = -sum[1] - c;
   }
@@ -581,7 +606,8 @@ enum class HeadKind {
 // The outputs of a layer launch.  A hidden layer stores only its bf16 activation, in `logits`.  Pointers the head
 // kind does not store are null.  Row r of the launch draws the noise of global row row_base + r.  `mask`, unless null,
 // is the greedy or sampling head's legal-action mask [rows, d_out] (nonzero byte: legal), a runtime input of the same
-// instantiations.
+// instantiations.  `values`, unless null, marks a sampling or Gaussian head with a value head: the head's weight has
+// d_out + 1 rows (the policy's, then the critic's), and column d_out of each stored row goes to values[row] in fp32.
 struct HeadOut {
   void* logits = nullptr;
   int64_t* actions = nullptr;
@@ -590,8 +616,9 @@ struct HeadOut {
   const float* log_std = nullptr;
   float* gauss_actions = nullptr;
   const uint8_t* mask = nullptr;
+  float* values = nullptr;
 
-  // The same outputs from row r0 of the call on.
+  // The same outputs from row r0 of the call on (d_out: the policy's width).
   HeadOut from_row(size_t r0, int d_out) const {
     HeadOut h = *this;
     if (logits) h.logits = static_cast<__nv_bfloat16*>(logits) + r0 * d_out;
@@ -599,6 +626,7 @@ struct HeadOut {
     if (log_probs) h.log_probs += r0;
     if (gauss_actions) h.gauss_actions += r0 * d_out;
     if (mask) h.mask += r0 * d_out;
+    if (values) h.values += r0;
     h.row_base += r0;
     return h;
   }
@@ -615,7 +643,8 @@ struct HeadOut {
 //     noise of Philox word j & 1 of counter (i, j >> 1) under `seed` (include/ktb200.h), and log_probs[row] =
 //     log_softmax(logits)[action] in fp32 (sample_epilogue);
 //   kGaussian: gauss_actions[row, j] = logit_j + exp(log_std_j)·z_j with z_j = Φ⁻¹(u) of Philox word j & 1 of counter
-//     (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (gaussian_epilogue).
+//     (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (gaussian_epilogue);
+//   kSample and kGaussian with out.values: n_valid = d_out + 1, and values[row] = fp32(column d_out) (store_values).
 // A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
 // (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
 // never an action.
@@ -644,10 +673,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, out.mask, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
-                             out.row_base);
+                             out.row_base, out.values);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
-                                       out.log_probs, out.seed, out.row_base);
+                                       out.log_probs, out.seed, out.row_base, out.values);
   }
 }
 
@@ -751,7 +780,7 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   return KTB_OK;
 }
 
-// The head of KIND, in the smallest tile that holds its N = d_out columns.
+// The head of KIND, in the smallest tile that holds its N columns (d_out, or d_out + 1 with a value head).
 template <HeadKind KIND>
 static int launch_head(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
                        int K, cudaStream_t stream) {
@@ -762,13 +791,15 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
 // and _pushed: no biases and a 64-wide greedy head that stores logits only.  `masked` marks the _masked entries: the
 // head applies a legal-action mask, out.mask in the pull forms and the bytes at MlpFeed::mask_offset of the call's
-// staging half in the pushed forms.
+// staging half in the pushed forms.  `valued` marks the _value entries: W3 / b3 are the stacked W3v [d_out + 1,
+// d_hidden] / b3v [d_out + 1] of the policy and its value head, and out.values receives the value of each row.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
   HeadOut out;
   bool logits64 = false;
   bool masked = false;
+  bool valued = false;
 
   MlpParams with_mask(const uint8_t* mask) const {
     MlpParams p = *this;
@@ -776,11 +807,17 @@ struct MlpParams {
     p.masked = true;
     return p;
   }
+  MlpParams with_values(float* values) const {
+    MlpParams p = *this;
+    p.out.values = values;
+    p.valued = true;
+    return p;
+  }
 };
 
 // Rows [r0, r0 + rows) of a call: the hidden layers h1 = relu(a1 · W1ᵀ (+ b1)) and h2 = relu(h1 · W2ᵀ (+ b2)), then
-// the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds d_out.
-// `consumed`, unless null, is recorded once layer 1 has read a1.
+// the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds its d_out
+// columns, d_out + 1 with a value head.  `consumed`, unless null, is recorded once layer 1 has read a1.
 static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void* a1, void* h1, void* h2, size_t r0,
                      size_t rows, int d_in, int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
   int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
@@ -791,7 +828,7 @@ static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void
   const auto head = p.kind == HeadKind::kGreedy   ? launch_head<HeadKind::kGreedy>
                     : p.kind == HeadKind::kSample ? launch_head<HeadKind::kSample>
                                                   : launch_head<HeadKind::kGaussian>;
-  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, d_out, d_hidden, st);
+  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, d_out + (int)p.valued, d_hidden, st);
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -869,7 +906,8 @@ struct MlpFeed {
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
 // right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
 // ktb_push_wait waits for.  A masked entry's own checks (a mask in the pull forms, mask_offset inside the staging half
-// and past the rows in the pushed forms) come after every check of the unmasked entry.
+// and past the rows in the pushed forms) come after every check of the unmasked entry, and a value entry's (values,
+// d_out <= 255; skipped for an empty call) after every check of the entry without a value head.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -906,6 +944,12 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
                 "%s: mask_offset=%zu + M*d_out exceeds stage_stride", fn, f.mask_offset);
   } else if (p.masked) {
     KTB_REQUIRE(p.out.mask, KTB_ERR_ARG, "%s: null mask", fn);   // M > 0 here: an empty pull call has returned
+  }
+  if (p.valued && M > 0) {
+    KTB_REQUIRE(p.out.values, KTB_ERR_ARG, "%s: null values", fn);
+    KTB_REQUIRE(((uintptr_t)p.out.values & 3) == 0, KTB_ERR_ARG, "%s: values must be 4-byte aligned", fn);
+    KTB_REQUIRE(d_out <= 255, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the policy and its value column fit one 256-wide tile)",
+                fn, d_out);
   }
   rc = get_encoder();
   if (rc) return rc;
@@ -1119,6 +1163,83 @@ int ktb_mlp_bf16_policy_gaussian_pushed(int dev, const void* stage_local, size_t
   const MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian,
                     {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}};
   return mlp_run("ktb_mlp_bf16_policy_gaussian_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_sample_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                     const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v,
+                                     const void* b3v, uint64_t seed, uint64_t row_base, int64_t* actions,
+                                     float* log_probs, float* values, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3v, b3v, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}}
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_value", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                            int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                            const void* b2, const void* W3v, const void* b3v, uint64_t seed,
+                                            uint64_t row_base, int64_t* actions, float* log_probs, float* values,
+                                            void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                            size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3v, b3v, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}}
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_sample_masked_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                            const void* W1, const void* b1, const void* W2, const void* b2,
+                                            const void* W3v, const void* b3v, const uint8_t* mask, uint64_t seed,
+                                            uint64_t row_base, int64_t* actions, float* log_probs, float* values,
+                                            void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3v, b3v, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}}
+                          .with_mask(mask)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_masked_value", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_masked_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                   int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                   const void* W2, const void* b2, const void* W3v, const void* b3v,
+                                                   size_t mask_offset, uint64_t seed, uint64_t row_base,
+                                                   int64_t* actions, float* log_probs, float* values, void* scratch,
+                                                   void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                   unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3v, b3v, HeadKind::kSample, {nullptr, actions, log_probs, seed, row_base}}
+                          .with_mask(nullptr)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v,
+                                       const void* b3v, const float* log_std, uint64_t seed, uint64_t row_base,
+                                       float* actions, float* log_probs, float* values, void* scratch, void* stage,
+                                       uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3v, b3v, HeadKind::kGaussian,
+                                {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}}
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_value", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                              int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                              const void* b2, const void* W3v, const void* b3v, const float* log_std,
+                                              uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
+                                              float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                              int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams{W1, b1, W2, b2, W3v, b3v, HeadKind::kGaussian,
+                                {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}}
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
                  stream);
 }

@@ -131,6 +131,34 @@ _SIGNATURES = {
                                                          c_size_t, ctypes.c_uint64, ctypes.c_uint64, c_void_p,
                                                          c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_size_t,
                                                          ctypes.c_ulonglong, c_uintptr]),
+    "ktb_mlp_bf16_policy_sample_value": (c_int, [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                 c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_uint64,
+                                                 ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                 c_uintptr]),
+    "ktb_mlp_bf16_policy_sample_value_pushed": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int, c_int,
+                                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                        ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_void_p, c_void_p,
+                                                        c_void_p, c_void_p, c_void_p, c_int, c_size_t,
+                                                        ctypes.c_ulonglong, c_uintptr]),
+    "ktb_mlp_bf16_policy_sample_masked_value": (c_int, [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p,
+                                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                        ctypes.c_uint64, ctypes.c_uint64, c_void_p, c_void_p, c_void_p,
+                                                        c_void_p, c_void_p, c_uintptr]),
+    "ktb_mlp_bf16_policy_sample_masked_value_pushed": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int,
+                                                               c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                               c_void_p, c_size_t, ctypes.c_uint64, ctypes.c_uint64,
+                                                               c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                               c_void_p, c_int, c_size_t, ctypes.c_ulonglong,
+                                                               c_uintptr]),
+    "ktb_mlp_bf16_policy_gaussian_value": (c_int, [c_int, c_void_p, c_size_t, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                   c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.c_uint64,
+                                                   ctypes.c_uint64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                   c_uintptr]),
+    "ktb_mlp_bf16_policy_gaussian_value_pushed": (c_int, [c_int, c_void_p, c_size_t, c_size_t, c_int, c_int, c_int,
+                                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                          c_void_p, ctypes.c_uint64, ctypes.c_uint64, c_void_p,
+                                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int,
+                                                          c_size_t, ctypes.c_ulonglong, c_uintptr]),
     # experiment knob, not in the stable header
     "ktb_set_tuning": (c_int, [c_int, c_int]),
 }

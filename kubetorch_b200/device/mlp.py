@@ -2,11 +2,13 @@
 ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions), ktb_mlp_bf16_policy_sample (seeded
 Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_mlp_bf16_policy_gaussian (seeded
 diagonal-Gaussian actions with their log-probabilities), the _masked forms of the first two (a per-row legal-action
-mask) and their scatter→exec→gather form."""
+mask), the _value forms of the sampled heads (a critic's state value on the same trunk) and their scatter→exec→gather
+form."""
 from __future__ import annotations
 
 import ctypes
-from typing import List, Optional, Sequence
+import weakref
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 
@@ -18,6 +20,7 @@ from ..sampling import _check_seed
 _scratch = {}
 _stage = {}
 _weight_cache = {}
+_stacked_heads = {}   # (device, id(w3)) -> [weakref to w3, stamp of w3 / b3 / wv / bv, W3v, b3v]
 _pool = None
 
 
@@ -56,12 +59,40 @@ def _thread_pool():
 MAX_D_OUT = 256
 
 
-def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None) -> None:
+def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
+    """_check_policy's checks of a value head (wv, bv), in this order: the output, the pair, the head width, bv given
+    exactly when b3 is, then wv's dtype and shape, layout and device, then bv."""
+    if output not in ("sample", "gaussian"):
+        raise ValueError(f'value is an argument of output="sample" and "gaussian", not of output={output!r}')
+    if not isinstance(value, (tuple, list)) or len(value) != 2:
+        raise ValueError("value must be (wv, bv): the critic's weight [1, d_hidden] and its bias [1] or None")
+    wv, bv = value
+    if d_out == MAX_D_OUT:
+        raise ValueError(f"d_out={d_out}: with a value head the policy is 1 to {MAX_D_OUT - 1} wide (its "
+                         f"columns and the value's must fit one {MAX_D_OUT}-wide tile)")
+    if (bv is None) != (b3 is None):
+        raise ValueError("value: bv is given exactly when b3 is (a zero bias in the policy's columns would turn -0.0 "
+                         "logits into +0.0)")
+    if not isinstance(wv, torch.Tensor) or wv.dtype != torch.bfloat16 or tuple(wv.shape) != (1, d_hidden):
+        raise ValueError(f"value: wv must be a bfloat16 tensor of shape (1, {d_hidden})")
+    if not wv.is_contiguous():
+        raise ValueError("value: wv must be contiguous")
+    if not wv.is_cuda or wv.device != w3.device:
+        raise ValueError(f"value: wv must be a CUDA tensor on the device of w3 ({w3.device}), got {wv.device}")
+    if bv is not None and (not isinstance(bv, torch.Tensor) or bv.dtype != torch.bfloat16 or tuple(bv.shape) != (1,)
+                           or not bv.is_contiguous() or bv.device != w3.device):
+        raise ValueError(f"value: bv must be a contiguous bfloat16 tensor of shape (1,) on the device of w3 "
+                         f"({w3.device})")
+
+
+def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
-    (output="gaussian") a log_std or a legal-action mask the kernels do not take.  A seed is an int (not a bool) in
-    [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with output="gaussian" only; a
-    mask is a contiguous CUDA torch.bool tensor [M, d_out] on the device of obs [M, d_in], given with any output but
-    "gaussian"."""
+    (output="gaussian") a log_std, a legal-action mask or a value head the kernels do not take.  A seed is an int (not
+    a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
+    output="gaussian" only; a mask is a contiguous CUDA torch.bool tensor [M, d_out] on the device of obs [M, d_in],
+    given with any output but "gaussian"; a value head (wv, bv), given with output="sample" or "gaussian" only, is a
+    contiguous bfloat16 wv [1, d_hidden] and a contiguous bfloat16 bv [1] (given exactly when b3 is), both on the
+    device of w3, beside a policy at most 255 wide."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
     if output in ("sample", "gaussian"):
@@ -90,6 +121,8 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
             raise ValueError("mask must be contiguous")
         if not mask.is_cuda or mask.device != obs.device:
             raise ValueError(f"mask must be a CUDA tensor on the device of obs ({obs.device}), got {mask.device}")
+    if value is not None:
+        _check_value(value, output, w3, biases[2], d_hidden, d_out)
     for name, b, n in zip(("b1", "b2", "b3"), biases, (d_hidden, d_hidden, d_out)):
         if b is None:
             continue
@@ -98,10 +131,38 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
             raise ValueError(f"{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
 
 
-def _outputs(output, M, d_out, device, logits, actions, log_probs):
-    """(logits, actions, log_probs) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions [M], or
-    fp32 [M, d_out] with "gaussian"; fp32 log_probs [M].  A buffer the mode does not write is None, a missing one is
-    allocated on `device` and a given one is registered with the library (ops.ensure_init)."""
+def _stacked_head(w3, b3, wv, bv) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """(W3v, b3v): the policy's head with the critic's under it, W3v = [w3; wv] [d_out + 1, d_hidden] and
+    b3v = [b3; bv] (None without biases), on the device of w3.  One entry per (device, head) is kept, and rewritten in
+    place when w3, b3, wv or bv has a new data_ptr or _version: a PPO loop updates its weights in place between
+    rollouts.  Rewriting in place bumps W3v's and b3v's own _version, so _weights_on copies the new head to other
+    devices."""
+    stamp = tuple(None if t is None else (t.data_ptr(), t._version) for t in (w3, b3, wv, bv))
+    key = (w3.device.index, id(w3))
+    entry = _stacked_heads.get(key)
+    if entry is None or entry[0]() is not w3:
+        for k, e in list(_stacked_heads.items()):   # heads whose w3 is gone, or a new w3 that reuses an old id
+            if e[0]() is None or k == key:
+                del _stacked_heads[k]
+        entry = _stacked_heads[key] = [weakref.ref(w3), None, None, None]
+    if entry[1] != stamp:
+        for i, parts in ((2, (w3, wv)), (3, None if b3 is None else (b3, bv))):
+            if parts is None:
+                entry[i] = None
+            elif entry[i] is not None and entry[i].shape[0] == parts[0].shape[0] + 1 \
+                    and entry[i].shape[1:] == parts[0].shape[1:]:
+                torch.cat(parts, out=entry[i])
+            else:
+                entry[i] = torch.cat(parts)
+        entry[1] = stamp
+    return entry[2], entry[3]
+
+
+def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False):
+    """(logits, actions, log_probs, values) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions
+    [M], or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values [M].  A buffer the mode
+    does not write is None, a missing one is allocated on `device` and a given one is registered with the library
+    (ops.ensure_init)."""
     def buf(t, shape, dtype):
         if t is None:
             return torch.empty(shape, dtype=dtype, device=device)
@@ -112,19 +173,23 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs):
     return (buf(logits, (M, d_out), torch.bfloat16) if output in ("logits", "both") else None,
             None if output == "logits" else
             buf(actions, (M, d_out), torch.float32) if gaussian else buf(actions, (M,), torch.int64),
-            buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian") else None)
+            buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian") else None,
+            buf(values, (M,), torch.float32) if valued else None)
 
 
-def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None):
+def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
-    mask's address in the pull forms, its offset in the staging half in the pushed forms."""
-    suffix = ("" if mask is None else "_masked") + ("_pushed" if pushed else "")
+    mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
+    picks the _value entry (whose W3 and b3 are the stacked head) and is its values buffer."""
+    suffix = ("" if mask is None else "_masked") + ("" if values is None else "_value") + ("_pushed" if pushed else "")
     masked = () if mask is None else (mask,)
+    valued = () if values is None else (ptr(values),)
     if output == "gaussian":
-        return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs))
+        return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs),
+                                                         *valued)
     if output == "sample":
-        return "ktb_mlp_bf16_policy_sample" + suffix, (*masked, seed, row_base, ptr(actions), ptr(log_probs))
+        return "ktb_mlp_bf16_policy_sample" + suffix, (*masked, seed, row_base, ptr(actions), ptr(log_probs), *valued)
     return "ktb_mlp_bf16_policy" + suffix, (*masked, ptr(logits), ptr(actions))
 
 
@@ -133,7 +198,7 @@ def _rows(bufs, b, e):
     return [None if t is None else t[b:e] for t in bufs]
 
 
-def _result(output, logits, actions, log_probs):
+def _result(output, logits, actions, log_probs, values=None):
     """What a call with `output` returns, from its buffers."""
     if output == "logits":
         return logits
@@ -141,7 +206,7 @@ def _result(output, logits, actions, log_probs):
         return actions
     if output == "both":
         return logits, actions
-    return actions, log_probs
+    return (actions, log_probs) if values is None else (actions, log_probs, values)
 
 
 def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch.Tensor,
@@ -150,7 +215,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
                 actions: Optional[torch.Tensor] = None, seed: Optional[int] = None, row_offset: int = 0,
                 log_probs: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
-                mask: Optional[torch.Tensor] = None):
+                mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                values: Optional[torch.Tensor] = None, _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -163,7 +229,12 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     biases, at d_out == 64 and with logits only the logits equal ktb_mlp_bf16's.  `mask`, a bool [M, d_out] tensor on
     the device of obs (True: legal), applies a per-row legal-action mask to every output but "gaussian": the head
     computes logits.masked_fill(~mask, -inf) and stores, ranks and samples those masked logits; an all-True mask gives
-    the unmasked bits."""
+    the unmasked bits.  `value` = (wv, bv), with output="sample" or "gaussian" (masked or not), adds the state value of
+    a critic nn.Linear(d_hidden, 1) on the same trunk (wv its bf16 weight [1, d_hidden], bv its bf16 bias [1], given
+    exactly when b3 is): the call returns (actions, log_probs, values) with fp32 values[M] = F.linear(h, wv, bv), the
+    bf16 result widened exactly, into `values` when given; the actions and log-probabilities keep their bits.  The
+    head then runs over W3v = [w3; wv], stacked once per device and head (_stacked_head).  `_stacked` (internal, from
+    mlp_scatter_gather, which checked the call): w3 and biases[2] are already the stacked W3v and b3v."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -173,21 +244,29 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
-    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs)
+    if _stacked:
+        d_out -= 1
+    else:
+        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value)
     if output in ("sample", "gaussian") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
-    out, actions, log_probs = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs)
+    valued = _stacked or value is not None
+    out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
+    if value is not None:
+        with torch.cuda.stream(s):   # a rewrite of the stacked head is ordered after earlier calls on s
+            w3, b3 = _stacked_head(w3, biases[2], *value)
+        biases = (biases[0], biases[1], b3)
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
-                        mask=None if mask is None else ptr(mask))
+                        mask=None if mask is None else ptr(mask), values=values)
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
-    return _result(output, out, actions, log_probs)
+    return _result(output, out, actions, log_probs, values)
 
 
 def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
@@ -215,7 +294,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
-                               seed=None, log_std=None, mask=None) -> None:
+                               seed=None, log_std=None, mask=None, values_root=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -225,9 +304,11 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     that device.  With output="sample" or "gaussian" rank r draws the noise of global rows b_r .. e_r - 1 (its shard's
     place in obs_root).  A legal-action `mask` [M, d_out] on the root travels with its rows: the copy engines push each
     rank's mask rows into the same staging half, 256-byte aligned after the largest shard's observation rows, so no
-    rank reads the root's memory."""
+    rank reads the root's memory.  With `values_root` (fp32 [M]) weights[dev] holds the stacked W3v and b3v in place of
+    w3 and b3, and each rank stores its values there too."""
     root, n, key = devs[0], len(devs), tuple(devs)
-    d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0]
+    valued = values_root is not None
+    d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0] - valued
     rows = max(e - b for b, e in bounds)
     mask_offset = (rows * d_in * 2 + 255) // 256 * 256
     stage_bytes = rows * d_in * 2 if mask is None else mask_offset + rows * d_out
@@ -244,15 +325,16 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS)
     scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], scratch_bytes) for r in range(1, n)]
     streams = [ops.current_stream_handle(d) for d in devs]
-    bufs = (out_root, actions_root, log_probs_root)
+    bufs = (out_root, actions_root, log_probs_root, values_root)
     b0, e0 = bounds[0]
     own = e0 > b0
     if own:
         ws = weights[root]
-        logits, actions, log_probs = _rows(bufs, b0, e0)
+        logits, actions, log_probs, values = _rows(bufs, b0, e0)
         mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=logits, device=root, stream=sess.fork(), staged=False,
                     biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
-                    log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0])
+                    log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0],
+                    values=values, _stacked=valued)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
     if mask is None:
@@ -266,8 +348,10 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         b, e = bounds[r]
         ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
-        entry, head = _head(output, *_rows(bufs, b, e), seed, b, None if log_std is None else log_std[devs[r]], ptr,
-                            pushed=True, mask=None if mask is None else mask_offset)
+        logits, actions, log_probs, values = _rows(bufs, b, e)
+        entry, head = _head(output, logits, actions, log_probs, seed, b,
+                            None if log_std is None else log_std[devs[r]], ptr, pushed=True,
+                            mask=None if mask is None else mask_offset, values=values)
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -281,23 +365,32 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        biases: Sequence[Optional[torch.Tensor]] = (None, None, None), output: str = "logits",
                        actions_root: Optional[torch.Tensor] = None, seed: Optional[int] = None,
                        log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
-                       mask: Optional[torch.Tensor] = None) -> list:
+                       mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                       values_root: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
     int64 actions views for "actions", (logits, actions) pairs for "both", (actions, log_probs) pairs for "sample"
-    and "gaussian" (fp32 actions [rows, d_out] with the latter).  With "sample" or "gaussian" rank r draws the noise of
-    the global rows of its shard (row_offset = its shard's begin), so the result does not depend on the number of
-    ranks or their devices.  `biases`, `seed`, `log_std` and `mask` as in mlp_forward; the mask lives on the root GPU
-    and each rank applies its rows of it (read in place by the pull form, pushed with the rows by the push form)."""
+    and "gaussian" (fp32 actions [rows, d_out] with the latter), (actions, log_probs, values) triples with a value head.
+    With "sample" or "gaussian" rank r draws the noise of the global rows of its shard (row_offset = its shard's begin),
+    so the result does not depend on the number of ranks or their devices.  `biases`, `seed`, `log_std`, `mask` and
+    `value` as in mlp_forward; the mask lives on the root GPU and each rank applies its rows of it (read in place by
+    the pull form, pushed with the rows by the push form); the head with the value head stacked under it is built on
+    the root and copied to the other devices like the other weights, and every rank stores its values into
+    `values_root` (allocated on the root when None)."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
-    bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root)
+    valued = value is not None
+    bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
+                    valued)
+    if valued:
+        w3, b3 = _stacked_head(w3, biases[2], *value)
+        biases = (biases[0], biases[1], b3)
     root_stream = torch.cuda.current_stream(root)
     ready = torch.cuda.Event()
     ready.record(root_stream)
@@ -313,7 +406,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs, seed, log_stds, mask)
+        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3])
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -332,10 +425,11 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         with torch.cuda.device(dev):
             if dev != root:
                 st.wait_event(ready)
-            logits, actions, log_probs = _rows(bufs, b, e)
+            logits, actions, log_probs, values = _rows(bufs, b, e)
             mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=st, biases=ws[3:],
                         output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
-                        log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e])
+                        log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e],
+                        values=values, _stacked=valued)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

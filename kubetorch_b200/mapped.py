@@ -80,14 +80,19 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     argument that holds the fp32 [d_out] log standard deviation.  ``mask``, an option of every output but
     ``"gaussian"``: the name of the call argument that holds a per-row legal-action mask, a bool [M, d_out] tensor on
     the device of obs (True: legal); the head then computes ``logits.masked_fill(~mask, -inf)`` and every output is
-    taken from those masked logits (the body applies ``legal.chunk(WORLD_SIZE)[RANK]`` to its rows)."""
+    taken from those masked logits (the body applies ``legal.chunk(WORLD_SIZE)[RANK]`` to its rows).  ``value``, an
+    option of ``output="sample"`` and ``"gaussian"`` with ``bias=True``: the names ``(wv, bv)`` of the two call
+    arguments that hold a critic ``nn.Linear(d_hidden, 1)`` on the same trunk, its bf16 weight [1, d_hidden] and bias
+    [1]; each rank then returns ``(actions, log_probs, values)`` with fp32 ``values = F.linear(h, wv, bv)`` of its
+    rows, the bf16 result widened exactly."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if "bias" in extra or "output" in extra or "seed" in extra or "log_std" in extra or "mask" in extra:
+    if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value")):
         if op != "mlp":
-            raise ValueError(f"bias=, output=, seed=, log_std= and mask= are options of the 'mlp' op, not of '{op}'")
+            raise ValueError(f"bias=, output=, seed=, log_std=, mask= and value= are options of the 'mlp' op, not of "
+                             f"'{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
@@ -109,12 +114,23 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
                 raise ValueError('mask= is an option of the categorical outputs, not of output="gaussian"')
             if not isinstance(extra["mask"], str):
                 raise ValueError(f"mask must be the name of a call argument, got {extra['mask']!r}")
+        if "value" in extra:
+            if not sample:
+                raise ValueError('value= is an option of output="sample" and "gaussian" only')
+            if not extra.get("bias", False):
+                raise ValueError("value= needs bias=True: the critic's bias is given exactly when b3 is")
+            v = extra["value"]
+            if not isinstance(v, (tuple, list)) or len(v) != 2 or not all(isinstance(n, str) for n in v):
+                raise ValueError(f"value must name two call arguments (wv, bv), got {v!r}")
 
     def deco(fn):
-        for option in ("log_std", "mask"):
-            name = extra.get(option)
-            if name is not None and name not in inspect.signature(fn).parameters:
-                raise ValueError(f"{option}={name!r} is not an argument of {getattr(fn, '__name__', fn)!r}")
+        params = inspect.signature(fn).parameters
+        for option in ("log_std", "mask", "value"):
+            names = extra.get(option)
+            for name in (names,) if isinstance(names, str) or names is None else names:
+                if name is not None and name not in params:
+                    raise ValueError(f"{option}={names!r}: {name!r} is not an argument of "
+                                     f"{getattr(fn, '__name__', fn)!r}")
         setattr(fn, MAPPED_ATTR, MappedSpec(op=op, alpha=alpha, beta=beta, reduce=reduce, arg=arg, extra=extra))
         return fn
 

@@ -587,9 +587,16 @@ class B200Supervisor:
             if mask not in bound:
                 raise TypeError(f"mapped mlp callable: mask argument '{mask}' not found in the call")
             mask = bound[mask]
+        value = spec.extra.get("value")
+        if value is not None:   # always the names (wv, bv) of two call arguments, resolved per call
+            for name in value:
+                if name not in bound:
+                    raise TypeError(f"mapped mlp callable: value argument '{name}' not found in the call")
+            value = tuple(bound[name] for name in value)
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
-                                         biases=biases, output=output, seed=seed, log_std=log_std, mask=mask)
+                                         biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
+                                         value=value)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -16,12 +16,18 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      [-2, 0.5]), timed in the same alternation beside the logits-only call and output="sample" at the same d_out
   i  policy with biases, d_out 18, 64 and 256, a random legal-action mask (about 50 % legal): masked actions right
      after the same unmasked call, and masked sampled actions right after the unmasked output="sample" call
+  j  policy with biases and a value head (a critic nn.Linear(1024, 1) on the same trunk, value=(wv, bv)), d_out 6, 18,
+     63, 64 and 255: output="sample", output="sample" with a random legal-action mask and output="gaussian", each
+     right after the same call without a value head; and the eager critic, what a user pays without the fused value:
+     the unfused output="sample" call plus the trunk and the value head recomputed with F.linear in torch
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
 exceeds 2^-18·(1 + max|s|), and the log-probability is within (d_out + 8)·2^-22·(1 + |ref|) of the fp64 log_softmax.
 Masked rows: the masked actions equal torch.argmax of the kernel's logits filled with -inf on every row, and every
-sampled action on a row with a legal action is legal.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+sampled action on a row with a legal action is legal.  Value rows: every valued call's actions and log-probabilities
+equal those of the same call without a value head on every row, bit for bit, the masked call's values equal the
+unmasked call's, and the values are within rtol 2^-7, atol 1e-2 of the eager critic's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -34,6 +40,7 @@ import sys
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, REPO)
 import torch  # noqa: E402
+import torch.nn.functional as F  # noqa: E402
 
 from kubetorch_b200.device import lib as L  # noqa: E402
 from kubetorch_b200.device import mlp  # noqa: E402
@@ -133,6 +140,32 @@ def main():
             obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED))
         variants[f"i_bias_masked_sample_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
             obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED, mask=legal[d]))
+    gj = torch.Generator(device="cuda:0").manual_seed(8)   # its own generator again
+    for d in (63, 255):
+        heads[d] = ((torch.randn(d, d_hidden, device="cuda:0", generator=gj) * 0.02).bfloat16(),
+                    (torch.randn(d, device="cuda:0", generator=gj) * 0.1).bfloat16())
+    critic = ((torch.randn(1, d_hidden, device="cuda:0", generator=gj) * 0.02).bfloat16(),
+              (torch.randn(1, device="cuda:0", generator=gj) * 0.1).bfloat16())
+    for d in (6, 18, 63, 64, 255):
+        legal.setdefault(d, torch.rand(M, d, device="cuda:0", generator=gj) < 0.5)
+        log_stds.setdefault(d, torch.linspace(-2.0, 0.5, d, device="cuda:0"))
+    value_widths = (6, 18, 63, 64, 255)
+    for d in value_widths:
+        bs = (b1, b2, heads[d][1])
+        for kind, kw in (("sample", dict(output="sample", seed=SEED)),
+                         ("masked_sample", dict(output="sample", seed=SEED, mask=legal[d])),
+                         ("gaussian", dict(output="gaussian", seed=SEED, log_std=log_stds[d]))):
+            variants[f"j_bias_{kind}_d{d}"] = (d, lambda d=d, bs=bs, kw=kw: mlp.mlp_forward(
+                obs, w1, w2, heads[d][0], biases=bs, **kw))
+            variants[f"j_bias_{kind}_value_d{d}"] = (d, lambda d=d, bs=bs, kw=kw: mlp.mlp_forward(
+                obs, w1, w2, heads[d][0], biases=bs, value=critic, **kw))
+
+        def eager_critic(d=d, bs=bs):
+            actions, log_probs = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED)
+            h = torch.relu(F.linear(torch.relu(F.linear(obs, w1, b1)), w2, b2))
+            return actions, log_probs, F.linear(h, *critic).float().squeeze(-1)
+
+        variants[f"j_bias_eager_critic_d{d}"] = (d, eager_critic)
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -214,6 +247,26 @@ def main():
         assert bool(legal[d][has].gather(1, sampled[has][:, None]).all())
         parity[f"i_bias_masked_d{d}"] = {"masked_actions_eq_masked_argmax_all_rows": "ok",
                                          "sampled_actions_legal_all_rows": "ok"}
+
+    for d in value_widths:
+        entry = {}
+        _, _, eager = variants[f"j_bias_eager_critic_d{d}"][1]()
+        values = {}
+        for kind in ("sample", "masked_sample", "gaussian"):
+            want = variants[f"j_bias_{kind}_d{d}"][1]()
+            got = variants[f"j_bias_{kind}_value_d{d}"][1]()
+            for g_, w_ in zip(got[:2], want):
+                assert torch.equal(g_.view(torch.int32) if g_.dtype == torch.float32 else g_,
+                                   w_.view(torch.int32) if w_.dtype == torch.float32 else w_), (kind, d)
+            values[kind] = got[2]
+            torch.testing.assert_close(got[2], eager, rtol=2**-7, atol=1e-2)
+            entry[f"{kind}_draws_eq_unvalued_all_rows"] = "ok"
+            del want, got
+        assert torch.equal(values["masked_sample"].view(torch.int32), values["sample"].view(torch.int32))
+        entry["masked_values_eq_unmasked"] = "ok"
+        entry["values_vs_eager_critic"] = "ok"
+        parity[f"j_bias_value_d{d}"] = entry
+        del eager, values
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
