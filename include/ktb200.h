@@ -497,6 +497,104 @@ int ktb_mlp_bf16_policy_gaussian_value_pushed(int dev, const void* stage_local, 
                                               float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer,
                                               int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* Multi-discrete forms: the greedy and sampling entries above (masked, pushed and with a value head as they come) for
+ * a MultiDiscrete(nvec) action space, one categorical sub-action per group of head columns.  Each takes the
+ * arguments of its categorical counterpart with (nvec, n_groups) inserted after b3 (or b3v).
+ *   - nvec [n_groups] int32 is a host array, read before the call returns.  Group g is the columns [lo_g, lo_g + n_g)
+ *     with lo_g = n_0 + ... + n_{g-1}; the groups tile the policy's d_out columns (a value column lies outside them).
+ *   - actions [M, n_groups] int64 (8-byte aligned; may be a peer pointer) holds group-relative actions in [0, n_g):
+ *     the counterpart's rule applied to each group's columns alone.  Greedy: torch.argmax of the group's (masked)
+ *     logits.  Sampled: Gumbel-max over the group's columns with the counterpart's noise (column j of global row i
+ *     draws Philox word j & 1 of counter (i, j >> 1, 0)), each pair of columns drawn once.
+ *   - log_probs [M] fp32: the sum, in fp32 and in group order starting from group 0's term, of each group's
+ *     log_softmax(group.float())[a_g].  A group whose ranked values are all -inf (no legal column, or only -inf
+ *     logits) takes action 0 and makes the row's log-probability NaN, as torch does.
+ *   - logits (greedy entries only, may be NULL) are those of ktb_mlp_bf16_policy or its _masked form, bit for bit; a
+ *     greedy entry needs logits or actions, as ktb_mlp_bf16_policy does.  values as in the value forms.
+ *   - nvec = {d_out} gives the bits of the counterpart's outputs, and group g of any nvec gives, bit for bit, the
+ *     action (minus lo_g) and log-probability of the counterpart under the mask legal & (column in group g).
+ *   - Checks: every check of the counterpart first, then, with M > 0: a NULL nvec, n_groups outside [1, d_out], any
+ *     nvec[g] < 1 or a sum other than d_out is KTB_ERR_ARG.  An empty pushed shard (M == 0) may pass NULL outputs and
+ *     a NULL nvec and still publishes its ack.  Writes stay inside the counterpart's outputs with actions [M, n_groups],
+ *     scratch and stage. */
+int ktb_mlp_bf16_policy_multidiscrete(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                      const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                      const void* b3, const int32_t* nvec, int n_groups, void* logits,
+                                      int64_t* actions, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_multidiscrete_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                             int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                             const void* b2, const void* W3, const void* b3, const int32_t* nvec,
+                                             int n_groups, void* logits, int64_t* actions, void* scratch,
+                                             void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                             unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_multidiscrete_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                             const void* W1, const void* b1, const void* W2, const void* b2,
+                                             const void* W3, const void* b3, const int32_t* nvec, int n_groups,
+                                             const uint8_t* mask, void* logits, int64_t* actions, void* scratch,
+                                             void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_multidiscrete_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                    int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                    const void* W2, const void* b2, const void* W3, const void* b3,
+                                                    const int32_t* nvec, int n_groups, size_t mask_offset,
+                                                    void* logits, int64_t* actions, void* scratch, void* ctrl_local,
+                                                    void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                    unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                             const void* W1, const void* b1, const void* W2, const void* b2,
+                                             const void* W3, const void* b3, const int32_t* nvec, int n_groups,
+                                             uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs,
+                                             void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                    int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                    const void* W2, const void* b2, const void* W3, const void* b3,
+                                                    const int32_t* nvec, int n_groups, uint64_t seed,
+                                                    uint64_t row_base, int64_t* actions, float* log_probs,
+                                                    void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                                    size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden,
+                                                    int d_out, const void* W1, const void* b1, const void* W2,
+                                                    const void* b2, const void* W3, const void* b3,
+                                                    const int32_t* nvec, int n_groups, const uint8_t* mask,
+                                                    uint64_t seed, uint64_t row_base, int64_t* actions,
+                                                    float* log_probs, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked_pushed(int dev, const void* stage_local, size_t stage_stride,
+                                                           size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                                           const void* b1, const void* W2, const void* b2,
+                                                           const void* W3, const void* b3, const int32_t* nvec,
+                                                           int n_groups, size_t mask_offset, uint64_t seed,
+                                                           uint64_t row_base, int64_t* actions, float* log_probs,
+                                                           void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                                           int rank, size_t chunk_rows, unsigned long long seq,
+                                                           uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_value(int dev, const void* obs, size_t M, int d_in, int d_hidden,
+                                                   int d_out, const void* W1, const void* b1, const void* W2,
+                                                   const void* b2, const void* W3v, const void* b3v,
+                                                   const int32_t* nvec, int n_groups, uint64_t seed,
+                                                   uint64_t row_base, int64_t* actions, float* log_probs,
+                                                   float* values, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_value_pushed(int dev, const void* stage_local, size_t stage_stride,
+                                                          size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                                          const void* b1, const void* W2, const void* b2,
+                                                          const void* W3v, const void* b3v, const int32_t* nvec,
+                                                          int n_groups, uint64_t seed, uint64_t row_base,
+                                                          int64_t* actions, float* log_probs, float* values,
+                                                          void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                                          int rank, size_t chunk_rows, unsigned long long seq,
+                                                          uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value(int dev, const void* obs, size_t M, int d_in, int d_hidden,
+                                                          int d_out, const void* W1, const void* b1, const void* W2,
+                                                          const void* b2, const void* W3v, const void* b3v,
+                                                          const int32_t* nvec, int n_groups, const uint8_t* mask,
+                                                          uint64_t seed, uint64_t row_base, int64_t* actions,
+                                                          float* log_probs, float* values, void* scratch, void* stage,
+                                                          uintptr_t stream);
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed(
+    int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_out,
+    const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v, const void* b3v,
+    const int32_t* nvec, int n_groups, size_t mask_offset, uint64_t seed, uint64_t row_base, int64_t* actions,
+    float* log_probs, float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+    size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -12,7 +12,8 @@
 //     bias (nn.Linear) and bf16 rounding, then for the hidden layers ReLU and full-tile stores, and
 //     for the head one of: logits masked to its width and/or the greedy action of every row; an
 //     action sampled by seeded Gumbel-max with its log-probability (either of these two optionally under a per-row
-//     legal-action mask, a runtime input); or Gaussian actions with their
+//     legal-action mask, a runtime input, and either optionally split into groups of columns with one greedy or
+//     sampled action per group, a multi-discrete action space); or Gaussian actions with their
 //     log-probability (the sampled and Gaussian heads optionally with a critic's state value, one more head column,
 //     also a runtime input) — the head's outputs may be peer pointers into the root GPU's result arena,
 //     which fuses the gather into the epilogue.
@@ -408,6 +409,158 @@ __device__ __forceinline__ void store_values(Slot slot, int d, int row, bool st0
   }
 }
 
+// The column groups of a multi-discrete head (HeadOut::groups), passed by value with the launch: group g is the
+// policy's columns [lo_g, lo_{g+1}), bit j of `starts` is set when column j begins a group (bit 0 included), and the
+// last group ends at the policy's width.  n == 0 is the one categorical over every column of the existing entries.
+struct HeadGroups {
+  uint32_t starts[8] = {};
+  int n = 0;
+  bool greedy = false;   // rank the logits alone: no noise and no log-probabilities (outputs "actions" and "both")
+};
+
+// The end of the group that begins at column lo: the next set bit of `starts` past lo, or d.  The words are indexed
+// at compile time, so the bitmap stays in the kernel's parameters.
+__device__ __forceinline__ int group_end(const uint32_t (&starts)[8], int lo, int d) {
+  int hi = d;
+#pragma unroll
+  for (int w = 7; w >= 0; --w) {
+    const int s = lo + 1 - 32 * w;   // bits >= s of word w are the columns past lo
+    const uint32_t b = s <= 0 ? starts[w] : s >= 32 ? 0u : starts[w] & (~0u << s);
+    if (b) hi = 32 * w + __ffs(b) - 1;
+  }
+  return hi;
+}
+
+// The grouped pass of sample_epilogue (groups.n > 0) over the bf16 pairs that its pass 1 parked in the ring.  Each
+// group is the rolled pass of the single categorical over the group's columns alone: a per-thread max of the live
+// columns in [lo, hi) and a quad max, then one pass that ranks y + Gumbel noise (y alone when greedy) in
+// torch.argmax order and sums exp(y - m), each in the single categorical's per-thread and quad order, so a group is
+// bit for bit that head under the mask legal ∧ (column in the group).  The loop over groups is uniform across the warp,
+// so every shuffle is converged.  A pair that straddles a group boundary draws its Philox words once: x[] keeps the
+// last pair's.  actions[row·n + g] is the group-relative action (0 when the group's ranked values are all -inf), and
+// log_probs[row] the fp32 sum of the groups' log-probabilities in group order, starting from group 0's.  With C, the
+// bf16 logits of "both" are stored from the ring, -inf in illegal columns, as greedy_epilogue stores them.
+template <int BLOCK_N, typename Slot>
+__device__ __forceinline__ void group_pass(Slot slot, const ColBits<BLOCK_N> (&live)[2], const HeadGroups& groups,
+                                           int d, int col0, int row, bool st0, bool st1, __nv_bfloat16* C,
+                                           int64_t* actions, float* log_probs, uint64_t seed, uint64_t row_base) {
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const bool draw = !groups.greedy;
+  const int G = groups.n;
+  float lp[2] = {0.f, 0.f};
+  uint2 x[2] = {make_uint2(0u, 0u), make_uint2(0u, 0u)};
+  int drawn = -1;   // the pair whose Philox words x[] hold
+  int lo = 0;
+#pragma unroll 1
+  for (int g = 0; g < G; ++g) {
+    const int hi = group_end(groups.starts, lo, d);
+    const int j0 = max(0, (lo - col0 + 6) >> 3);   // the first pair of the thread with col0 + 8j + 1 >= lo
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll 1
+    for (int j = j0; j < BLOCK_N / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= hi) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const float v = c ? __high2float(y) : __low2float(y);
+          if (col + c >= lo && col + c < hi && ((live[h] >> (2 * j + c)) & 1) && v > mx[h]) mx[h] = v;
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        const float o = __shfl_xor_sync(0xffffffffu, mx[h], m);
+        if (o > mx[h]) mx[h] = o;
+      }
+    }
+    float best[2] = {-INFINITY, -INFINITY}, best_y[2] = {NAN, NAN}, sum[2] = {0.f, 0.f};
+    int best_col[2] = {INT_MAX, INT_MAX};
+#pragma unroll 1
+    for (int j = j0; j < BLOCK_N / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= hi) break;
+      if (draw && j != drawn) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t i = row_base + (uint64_t)(row + 8 * h);
+          const uint4 w = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 0u), key);
+          x[h] = make_uint2(w.x, w.y);
+        }
+        drawn = j;
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          if (col + c < lo || col + c >= hi || !((live[h] >> (2 * j + c)) & 1)) continue;
+          const float v = c ? __high2float(y) : __low2float(y);
+          const float s = draw ? v + gumbel_of(c ? x[h].y : x[h].x) : v;
+          if (argmax_before(s, col + c, best[h], best_col[h])) {
+            best[h] = s;
+            best_col[h] = col + c;
+            best_y[h] = v;
+          }
+          if (draw) sum[h] += v == mx[h] ? 1.f : expf(v - mx[h]);
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
+        const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
+        const float oy = __shfl_xor_sync(0xffffffffu, best_y[h], m);
+        sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
+        if (argmax_before(ov, oc, best[h], best_col[h])) {
+          best[h] = ov;
+          best_col[h] = oc;
+          best_y[h] = oy;
+        }
+      }
+      const float t = best_y[h] - mx[h] - logf(sum[h]);
+      lp[h] = g == 0 ? t : lp[h] + t;
+    }
+    if ((threadIdx.x & 3) == 0 && actions != nullptr) {
+      if (st0) actions[(size_t)row * G + g] = best[0] == -INFINITY ? 0 : best_col[0] - lo;
+      if (st1) actions[(size_t)(row + 8) * G + g] = best[1] == -INFINITY ? 0 : best_col[1] - lo;
+    }
+    lo = hi;
+  }
+  if (draw && (threadIdx.x & 3) == 0) {
+    if (st0) log_probs[row] = lp[0];
+    if (st1) log_probs[row + 8] = lp[1];
+  }
+  if (C == nullptr) return;
+  const __nv_bfloat16 ninf = __ushort_as_bfloat16((unsigned short)0xFF80u);
+  const bool pairs = (d & 1) == 0 && ((uintptr_t)C & 3) == 0;
+#pragma unroll 1
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= d) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!(h ? st1 : st0)) continue;
+      __nv_bfloat162 y = *slot(2 * j + h);
+      if (!((live[h] >> (2 * j)) & 1)) y.x = ninf;
+      if (!((live[h] >> (2 * j + 1)) & 1)) y.y = ninf;
+      __nv_bfloat16* p = C + (size_t)(row + 8 * h) * d + col;
+      if (pairs) {
+        *reinterpret_cast<__nv_bfloat162*>(p) = y;
+      } else {
+        p[0] = y.x;
+        if (col + 1 < d) p[1] = y.y;
+      }
+    }
+  }
+}
+
 // The sampling epilogue of a head tile (HeadKind::kSample): rows r = row and row + 8 of the thread, global rows
 // row_base + r.  Pass 1 (unrolled over the accumulators) rounds the logits once, parks them as bf16 pairs in the TMA
 // ring as gaussian_epilogue does, and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum
@@ -423,11 +576,14 @@ __device__ __forceinline__ void store_values(Slot slot, int d, int row, bool st0
 // column) takes action 0 with a NaN log-probability, as torch does.
 // With a value head (values != null) the tile holds n_valid = d + 1 columns: the policy's d, then the value column d.
 // Pass 1 parks column d with the rest; everything ranked, drawn, summed or masked stops at d; store_values reads it.
+// A multi-discrete head (groups.n > 0) takes group_pass in place of the rolled pass: the greedy one as well, whose
+// logits (C, unless null) it also stores.  The single categorical's rolled pass stays as it is.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                 int n_valid, int row, bool st0, bool st1, int64_t* actions,
                                                 float* log_probs, const uint8_t* mask, uint64_t seed,
-                                                uint64_t row_base, float* values) {
+                                                uint64_t row_base, float* values, const HeadGroups& groups,
+                                                __nv_bfloat16* C) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -461,6 +617,11 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
       const float o = __shfl_xor_sync(0xffffffffu, mx[h], m);
       if (o > mx[h]) mx[h] = o;
     }
+  }
+  if (groups.n > 0) {
+    group_pass<BLOCK_N>(slot, live, groups, d, col0, row, st0, st1, C, actions, log_probs, seed, row_base);
+    store_values(slot, d, row, st0, st1, values);
+    return;
   }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   float best[2] = {-INFINITY, -INFINITY}, best_y[2] = {NAN, NAN}, sum[2] = {0.f, 0.f};
@@ -598,8 +759,9 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
 // What a layer's epilogue computes: the hidden layers' activation, or the head each entry point names.
 enum class HeadKind {
   kHidden,     // bf16 relu(A · Bᵀ + bias) of full tiles (layers 1 and 2)
-  kGreedy,     // bf16 logits and/or int64 argmax actions
-  kSample,     // Gumbel-max int64 actions and fp32 log_probs
+  kGreedy,     // bf16 logits and/or int64 argmax actions (unrolled; the single categorical)
+  kSample,     // the rolled categorical head: Gumbel-max int64 actions and fp32 log_probs, or with groups (HeadGroups)
+               // greedy or Gumbel-max actions per group, with the logits of "both" or the summed log_probs
   kGaussian,   // fp32 actions [rows, d_out] (gauss_actions) drawn with log_std, and fp32 log_probs
 };
 
@@ -608,6 +770,7 @@ enum class HeadKind {
 // is the greedy or sampling head's legal-action mask [rows, d_out] (nonzero byte: legal), a runtime input of the same
 // instantiations.  `values`, unless null, marks a sampling or Gaussian head with a value head: the head's weight has
 // d_out + 1 rows (the policy's, then the critic's), and column d_out of each stored row goes to values[row] in fp32.
+// `groups`, with groups.n > 0, marks a multi-discrete kSample head: actions is [rows, groups.n].
 struct HeadOut {
   void* logits = nullptr;
   int64_t* actions = nullptr;
@@ -617,12 +780,13 @@ struct HeadOut {
   float* gauss_actions = nullptr;
   const uint8_t* mask = nullptr;
   float* values = nullptr;
+  HeadGroups groups;
 
   // The same outputs from row r0 of the call on (d_out: the policy's width).
   HeadOut from_row(size_t r0, int d_out) const {
     HeadOut h = *this;
     if (logits) h.logits = static_cast<__nv_bfloat16*>(logits) + r0 * d_out;
-    if (actions) h.actions += r0;
+    if (actions) h.actions += r0 * (groups.n > 0 ? groups.n : 1);
     if (log_probs) h.log_probs += r0;
     if (gauss_actions) h.gauss_actions += r0 * d_out;
     if (mask) h.mask += r0 * d_out;
@@ -644,7 +808,9 @@ struct HeadOut {
 //     log_softmax(logits)[action] in fp32 (sample_epilogue);
 //   kGaussian: gauss_actions[row, j] = logit_j + exp(log_std_j)·z_j with z_j = Φ⁻¹(u) of Philox word j & 1 of counter
 //     (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (gaussian_epilogue);
-//   kSample and kGaussian with out.values: n_valid = d_out + 1, and values[row] = fp32(column d_out) (store_values).
+//   kSample and kGaussian with out.values: n_valid = d_out + 1, and values[row] = fp32(column d_out) (store_values);
+//   kSample with out.groups: one greedy or sampled action per group of columns into actions[row, g], the summed
+//     log-probability of the sampled ones, and the logits of a greedy head that stores them (group_pass).
 // A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
 // (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
 // never an action.
@@ -673,7 +839,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, out.mask, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
-                             out.row_base, out.values);
+                             out.row_base, out.values, out.groups, C);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
                                        out.log_probs, out.seed, out.row_base, out.values);
@@ -793,6 +959,7 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // head applies a legal-action mask, out.mask in the pull forms and the bytes at MlpFeed::mask_offset of the call's
 // staging half in the pushed forms.  `valued` marks the _value entries: W3 / b3 are the stacked W3v [d_out + 1,
 // d_hidden] / b3v [d_out + 1] of the policy and its value head, and out.values receives the value of each row.
+// `nvec` (n_groups entries, a host array) marks the _multidiscrete entries: mlp_run checks it and builds out.groups.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -800,6 +967,21 @@ struct MlpParams {
   bool logits64 = false;
   bool masked = false;
   bool valued = false;
+  const int32_t* nvec = nullptr;
+  int n_groups = 0;
+  bool grouped = false;
+
+  // A multi-discrete head: the greedy one (logits and/or actions, ranked without noise) or the sampled one, both in
+  // the kSample instantiations.
+  static MlpParams multidiscrete(const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                 const void* b3, const int32_t* nvec, int n_groups, const HeadOut& out, bool greedy) {
+    MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, out};
+    p.out.groups.greedy = greedy;
+    p.nvec = nvec;
+    p.n_groups = n_groups;
+    p.grouped = true;
+    return p;
+  }
 
   MlpParams with_mask(const uint8_t* mask) const {
     MlpParams p = *this;
@@ -848,7 +1030,10 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
         KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
         break;
       case HeadKind::kSample:
-        KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
+        if (o.groups.greedy)   // a greedy multi-discrete head takes what the greedy entries take
+          KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
+        else
+          KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
         KTB_REQUIRE(o.log_std && o.gauss_actions && o.log_probs, KTB_ERR_ARG,
@@ -907,7 +1092,9 @@ struct MlpFeed {
 // right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
 // ktb_push_wait waits for.  A masked entry's own checks (a mask in the pull forms, mask_offset inside the staging half
 // and past the rows in the pushed forms) come after every check of the unmasked entry, and a value entry's (values,
-// d_out <= 255; skipped for an empty call) after every check of the entry without a value head.
+// d_out <= 255; skipped for an empty call) after every check of the entry without a value head.  A multi-discrete
+// entry's nvec (skipped for an empty call) is checked last, and read into the launch's HeadGroups before the call
+// returns.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -951,6 +1138,20 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     KTB_REQUIRE(d_out <= 255, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the policy and its value column fit one 256-wide tile)",
                 fn, d_out);
   }
+  HeadGroups groups = p.out.groups;
+  if (p.grouped && M > 0) {
+    KTB_REQUIRE(p.nvec, KTB_ERR_ARG, "%s: null nvec", fn);
+    KTB_REQUIRE(p.n_groups >= 1 && p.n_groups <= d_out, KTB_ERR_ARG, "%s: n_groups=%d must be in [1, d_out=%d]", fn,
+                p.n_groups, d_out);
+    long long lo = 0;
+    for (int g = 0; g < p.n_groups; ++g) {
+      KTB_REQUIRE(p.nvec[g] >= 1, KTB_ERR_ARG, "%s: nvec[%d]=%d must be positive", fn, g, (int)p.nvec[g]);
+      if (lo < d_out) groups.starts[lo >> 5] |= 1u << (lo & 31);
+      lo += p.nvec[g];
+    }
+    KTB_REQUIRE(lo == d_out, KTB_ERR_ARG, "%s: nvec sums to %lld, not d_out=%d", fn, lo, d_out);
+    groups.n = p.n_groups;
+  }
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
@@ -962,6 +1163,7 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   const __nv_bfloat16* x =
       reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride);
   HeadOut out = p.out;
+  out.groups = groups;
   if (p.masked && f.pushed) out.mask = reinterpret_cast<const uint8_t*>(x) + f.mask_offset;
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
@@ -1242,6 +1444,170 @@ int ktb_mlp_bf16_policy_gaussian_value_pushed(int dev, const void* stage_local, 
   return mlp_run("ktb_mlp_bf16_policy_gaussian_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
                  stream);
+}
+
+int ktb_mlp_bf16_policy_multidiscrete(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                      const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                      const void* b3, const int32_t* nvec, int n_groups, void* logits,
+                                      int64_t* actions, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups, {logits, actions}, true);
+  return mlp_run("ktb_mlp_bf16_policy_multidiscrete", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_multidiscrete_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                             int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                             const void* b2, const void* W3, const void* b3, const int32_t* nvec,
+                                             int n_groups, void* logits, int64_t* actions, void* scratch,
+                                             void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                             unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups, {logits, actions}, true);
+  return mlp_run("ktb_mlp_bf16_policy_multidiscrete_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_multidiscrete_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                             const void* W1, const void* b1, const void* W2, const void* b2,
+                                             const void* W3, const void* b3, const int32_t* nvec, int n_groups,
+                                             const uint8_t* mask, void* logits, int64_t* actions, void* scratch,
+                                             void* stage, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups, {logits, actions}, true).with_mask(mask);
+  return mlp_run("ktb_mlp_bf16_policy_multidiscrete_masked", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_multidiscrete_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                    int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                    const void* W2, const void* b2, const void* W3, const void* b3,
+                                                    const int32_t* nvec, int n_groups, size_t mask_offset,
+                                                    void* logits, int64_t* actions, void* scratch, void* ctrl_local,
+                                                    void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                    unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups, {logits, actions}, true).with_mask(nullptr);
+  return mlp_run("ktb_mlp_bf16_policy_multidiscrete_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                             const void* W1, const void* b1, const void* W2, const void* b2,
+                                             const void* W3, const void* b3, const int32_t* nvec, int n_groups,
+                                             uint64_t seed, uint64_t row_base, int64_t* actions, float* log_probs,
+                                             void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                    int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                    const void* W2, const void* b2, const void* W3, const void* b3,
+                                                    const int32_t* nvec, int n_groups, uint64_t seed,
+                                                    uint64_t row_base, int64_t* actions, float* log_probs,
+                                                    void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                                    size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden,
+                                                    int d_out, const void* W1, const void* b1, const void* W2,
+                                                    const void* b2, const void* W3, const void* b3,
+                                                    const int32_t* nvec, int n_groups, const uint8_t* mask,
+                                                    uint64_t seed, uint64_t row_base, int64_t* actions,
+                                                    float* log_probs, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false)
+                          .with_mask(mask);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked_pushed(int dev, const void* stage_local, size_t stage_stride,
+                                                           size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                                           const void* b1, const void* W2, const void* b2,
+                                                           const void* W3, const void* b3, const int32_t* nvec,
+                                                           int n_groups, size_t mask_offset, uint64_t seed,
+                                                           uint64_t row_base, int64_t* actions, float* log_probs,
+                                                           void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                                           int rank, size_t chunk_rows, unsigned long long seq,
+                                                           uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false)
+                          .with_mask(nullptr);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_value(int dev, const void* obs, size_t M, int d_in, int d_hidden,
+                                                   int d_out, const void* W1, const void* b1, const void* W2,
+                                                   const void* b2, const void* W3v, const void* b3v,
+                                                   const int32_t* nvec, int n_groups, uint64_t seed,
+                                                   uint64_t row_base, int64_t* actions, float* log_probs,
+                                                   float* values, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3v, b3v, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_value", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_value_pushed(int dev, const void* stage_local, size_t stage_stride,
+                                                          size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                                          const void* b1, const void* W2, const void* b2,
+                                                          const void* W3v, const void* b3v, const int32_t* nvec,
+                                                          int n_groups, uint64_t seed, uint64_t row_base,
+                                                          int64_t* actions, float* log_probs, float* values,
+                                                          void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                                          int rank, size_t chunk_rows, unsigned long long seq,
+                                                          uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3v, b3v, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value(int dev, const void* obs, size_t M, int d_in, int d_hidden,
+                                                          int d_out, const void* W1, const void* b1, const void* W2,
+                                                          const void* b2, const void* W3v, const void* b3v,
+                                                          const int32_t* nvec, int n_groups, const uint8_t* mask,
+                                                          uint64_t seed, uint64_t row_base, int64_t* actions,
+                                                          float* log_probs, float* values, void* scratch, void* stage,
+                                                          uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3v, b3v, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false)
+                          .with_mask(mask)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked_value", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed(
+    int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_out,
+    const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v, const void* b3v,
+    const int32_t* nvec, int n_groups, size_t mask_offset, uint64_t seed, uint64_t row_base, int64_t* actions,
+    float* log_probs, float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+    size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::multidiscrete(W1, b1, W2, b2, W3v, b3v, nvec, n_groups,
+                                               {nullptr, actions, log_probs, seed, row_base}, false)
+                          .with_mask(nullptr)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset),
+                 scratch, stream);
 }
 
 }  // extern "C"

@@ -162,6 +162,15 @@ _SIGNATURES = {
     # experiment knob, not in the stable header
     "ktb_set_tuning": (c_int, [c_int, c_int]),
 }
+# The _multidiscrete entries: each takes its categorical counterpart's arguments with (nvec, n_groups) after b3 (or
+# b3v), the 12th argument of the plain and staged forms and the 13th of the pushed ones.
+for _head, _suffixes in (("ktb_mlp_bf16_policy", ("", "_masked")),
+                         ("ktb_mlp_bf16_policy_sample", ("", "_masked", "_value", "_masked_value"))):
+    for _suffix in _suffixes:
+        for _form, _at in (("", 12), ("_pushed", 13)):
+            _restype, _args = _SIGNATURES[_head + _suffix + _form]
+            _SIGNATURES[_head + "_multidiscrete" + _suffix + _form] = (
+                _restype, _args[:_at] + [POINTER(ctypes.c_int32), c_int] + _args[_at:])
 
 _lib = None
 _lock = threading.Lock()

@@ -2,8 +2,8 @@
 ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions), ktb_mlp_bf16_policy_sample (seeded
 Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_mlp_bf16_policy_gaussian (seeded
 diagonal-Gaussian actions with their log-probabilities), the _masked forms of the first two (a per-row legal-action
-mask), the _value forms of the sampled heads (a critic's state value on the same trunk) and their scatter→exec→gather
-form."""
+mask), the _value forms of the sampled heads (a critic's state value on the same trunk), the _multidiscrete forms of
+the greedy and sampled heads (one categorical per group of columns) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -15,6 +15,7 @@ import torch
 from . import lib as L
 from . import ops
 from ..mapped import MLP_OUTPUTS as OUTPUTS
+from ..mapped import check_nvec
 from ..sampling import _check_seed
 
 _scratch = {}
@@ -85,14 +86,16 @@ def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
                          f"({w3.device})")
 
 
-def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None) -> None:
+def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
+                  nvec=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
-    (output="gaussian") a log_std, a legal-action mask or a value head the kernels do not take.  A seed is an int (not
+    (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
     output="gaussian" only; a mask is a contiguous CUDA torch.bool tensor [M, d_out] on the device of obs [M, d_in],
     given with any output but "gaussian"; a value head (wv, bv), given with output="sample" or "gaussian" only, is a
     contiguous bfloat16 wv [1, d_hidden] and a contiguous bfloat16 bv [1] (given exactly when b3 is), both on the
-    device of w3, beside a policy at most 255 wide."""
+    device of w3, beside a policy at most 255 wide; nvec (output="actions", "both" or "sample" only) is a non-empty
+    tuple or list of ints >= 1 that sums to d_out (mapped.check_nvec)."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
     if output in ("sample", "gaussian"):
@@ -104,6 +107,8 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if not 1 <= d_out <= MAX_D_OUT:
         raise ValueError(f"d_out={d_out}: the policy head is 1 to {MAX_D_OUT} wide")
+    if nvec is not None:
+        check_nvec(nvec, output, d_out)
     if output != "gaussian":
         if log_std is not None:
             raise ValueError('log_std is an argument of output="gaussian" only')
@@ -158,11 +163,11 @@ def _stacked_head(w3, b3, wv, bv) -> Tuple[torch.Tensor, Optional[torch.Tensor]]
     return entry[2], entry[3]
 
 
-def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False):
+def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False, nvec=None):
     """(logits, actions, log_probs, values) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions
-    [M], or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values [M].  A buffer the mode
-    does not write is None, a missing one is allocated on `device` and a given one is registered with the library
-    (ops.ensure_init)."""
+    [M], [M, len(nvec)] with nvec, or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values
+    [M].  A buffer the mode does not write is None, a missing one is allocated on `device` and a given one is
+    registered with the library (ops.ensure_init); given multi-discrete actions must be [M, len(nvec)]."""
     def buf(t, shape, dtype):
         if t is None:
             return torch.empty(shape, dtype=dtype, device=device)
@@ -170,27 +175,36 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
         return t
 
     gaussian = output == "gaussian"
+    if nvec is not None and actions is not None and tuple(actions.shape) != (M, len(nvec)):
+        raise ValueError(f"actions must have shape ({M}, {len(nvec)}) with nvec of {len(nvec)} groups, got "
+                         f"{tuple(actions.shape)}")
     return (buf(logits, (M, d_out), torch.bfloat16) if output in ("logits", "both") else None,
             None if output == "logits" else
-            buf(actions, (M, d_out), torch.float32) if gaussian else buf(actions, (M,), torch.int64),
+            buf(actions, (M, d_out), torch.float32) if gaussian else
+            buf(actions, (M,) if nvec is None else (M, len(nvec)), torch.int64),
             buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian") else None,
             buf(values, (M,), torch.float32) if valued else None)
 
 
-def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None):
+def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None,
+          nvec=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
     mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
-    picks the _value entry (whose W3 and b3 are the stacked head) and is its values buffer."""
-    suffix = ("" if mask is None else "_masked") + ("" if values is None else "_value") + ("_pushed" if pushed else "")
+    picks the _value entry (whose W3 and b3 are the stacked head) and is its values buffer.  `nvec`, unless None,
+    picks the _multidiscrete entry and is its group sizes."""
+    suffix = ("" if nvec is None else "_multidiscrete") + ("" if mask is None else "_masked") + \
+        ("" if values is None else "_value") + ("_pushed" if pushed else "")
+    grouped = () if nvec is None else (L.arr(ctypes.c_int32, nvec), len(nvec))
     masked = () if mask is None else (mask,)
     valued = () if values is None else (ptr(values),)
     if output == "gaussian":
         return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs),
                                                          *valued)
     if output == "sample":
-        return "ktb_mlp_bf16_policy_sample" + suffix, (*masked, seed, row_base, ptr(actions), ptr(log_probs), *valued)
-    return "ktb_mlp_bf16_policy" + suffix, (*masked, ptr(logits), ptr(actions))
+        return "ktb_mlp_bf16_policy_sample" + suffix, (*grouped, *masked, seed, row_base, ptr(actions), ptr(log_probs),
+                                                       *valued)
+    return "ktb_mlp_bf16_policy" + suffix, (*grouped, *masked, ptr(logits), ptr(actions))
 
 
 def _rows(bufs, b, e):
@@ -216,7 +230,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 actions: Optional[torch.Tensor] = None, seed: Optional[int] = None, row_offset: int = 0,
                 log_probs: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
                 mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
-                values: Optional[torch.Tensor] = None, _stacked: bool = False):
+                values: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None, _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -233,7 +247,13 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     a critic nn.Linear(d_hidden, 1) on the same trunk (wv its bf16 weight [1, d_hidden], bv its bf16 bias [1], given
     exactly when b3 is): the call returns (actions, log_probs, values) with fp32 values[M] = F.linear(h, wv, bv), the
     bf16 result widened exactly, into `values` when given; the actions and log-probabilities keep their bits.  The
-    head then runs over W3v = [w3; wv], stacked once per device and head (_stacked_head).  `_stacked` (internal, from
+    head then runs over W3v = [w3; wv], stacked once per device and head (_stacked_head).  `nvec` = (n_0, ...,
+    n_{G-1}), ints >= 1 summing to d_out, with output="actions", "both" or "sample" (masked or not, and with a value
+    head where "sample" takes one), makes the head multi-discrete: group g is the columns [lo_g, lo_g + n_g) with lo_g
+    = n_0 + ... + n_{g-1}, actions are int64 [M, G] of group-relative indices (the greedy or sampled action of each
+    group's logits alone, with the noise of "sample"), and log_probs[i] is the fp32 sum of the groups'
+    log_softmax(group)[a_g] in group order; a group with no legal action takes action 0 with a NaN log-probability.
+    The logits of "both" and nvec = (d_out,) keep the bits of the call without nvec.  `_stacked` (internal, from
     mlp_scatter_gather, which checked the call): w3 and biases[2] are already the stacked W3v and b3v."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
@@ -247,12 +267,13 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     if _stacked:
         d_out -= 1
     else:
-        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value)
+        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec)
     if output in ("sample", "gaussian") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
     valued = _stacked or value is not None
-    out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued)
+    out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued,
+                                               nvec)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
     if value is not None:
         with torch.cuda.stream(s):   # a rewrite of the stacked head is ordered after earlier calls on s
@@ -262,7 +283,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
-                        mask=None if mask is None else ptr(mask), values=values)
+                        mask=None if mask is None else ptr(mask), values=values, nvec=nvec)
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
@@ -294,7 +315,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
-                               seed=None, log_std=None, mask=None, values_root=None) -> None:
+                               seed=None, log_std=None, mask=None, values_root=None, nvec=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -305,7 +326,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     place in obs_root).  A legal-action `mask` [M, d_out] on the root travels with its rows: the copy engines push each
     rank's mask rows into the same staging half, 256-byte aligned after the largest shard's observation rows, so no
     rank reads the root's memory.  With `values_root` (fp32 [M]) weights[dev] holds the stacked W3v and b3v in place of
-    w3 and b3, and each rank stores its values there too."""
+    w3 and b3, and each rank stores its values there too.  `nvec` picks every rank's multi-discrete entry."""
     root, n, key = devs[0], len(devs), tuple(devs)
     valued = values_root is not None
     d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0] - valued
@@ -334,7 +355,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=logits, device=root, stream=sess.fork(), staged=False,
                     biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
                     log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0],
-                    values=values, _stacked=valued)
+                    values=values, nvec=nvec, _stacked=valued)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
     if mask is None:
@@ -351,7 +372,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         logits, actions, log_probs, values = _rows(bufs, b, e)
         entry, head = _head(output, logits, actions, log_probs, seed, b,
                             None if log_std is None else log_std[devs[r]], ptr, pushed=True,
-                            mask=None if mask is None else mask_offset, values=values)
+                            mask=None if mask is None else mask_offset, values=values, nvec=nvec)
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -366,7 +387,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        actions_root: Optional[torch.Tensor] = None, seed: Optional[int] = None,
                        log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
                        mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
-                       values_root: Optional[torch.Tensor] = None) -> list:
+                       values_root: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -377,17 +398,17 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     `value` as in mlp_forward; the mask lives on the root GPU and each rank applies its rows of it (read in place by
     the pull form, pushed with the rows by the push form); the head with the value head stacked under it is built on
     the root and copied to the other devices like the other weights, and every rank stores its values into
-    `values_root` (allocated on the root when None)."""
+    `values_root` (allocated on the root when None).  `nvec` as in mlp_forward: actions are [rows, G] views."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     valued = value is not None
     bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
-                    valued)
+                    valued, nvec)
     if valued:
         w3, b3 = _stacked_head(w3, biases[2], *value)
         biases = (biases[0], biases[1], b3)
@@ -406,7 +427,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if transfer == "push" and not pushable:
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
-        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3])
+        _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
+                                   nvec)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -429,7 +451,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
             mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=st, biases=ws[3:],
                         output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
                         log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e],
-                        values=values, _stacked=valued)
+                        values=values, nvec=nvec, _stacked=valued)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

@@ -84,15 +84,19 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     option of ``output="sample"`` and ``"gaussian"`` with ``bias=True``: the names ``(wv, bv)`` of the two call
     arguments that hold a critic ``nn.Linear(d_hidden, 1)`` on the same trunk, its bf16 weight [1, d_hidden] and bias
     [1]; each rank then returns ``(actions, log_probs, values)`` with fp32 ``values = F.linear(h, wv, bv)`` of its
-    rows, the bf16 result widened exactly."""
+    rows, the bf16 result widened exactly.  ``nvec``, an option of ``output="actions"``, ``"both"`` and ``"sample"``
+    (with ``mask=`` and ``value=`` as those allow): a tuple of ints ``(n_0, ..., n_{G-1})`` summing to d_out, a
+    constant of the deployment, for a ``MultiDiscrete(nvec)`` action space.  The logits split into G groups of
+    columns, one categorical each: actions become int64 ``[rows, G]`` of group-relative indices (greedy, or sampled
+    per group with the same noise), and log_probs the fp32 sum of the groups' log-probabilities in group order."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value")):
+    if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec")):
         if op != "mlp":
-            raise ValueError(f"bias=, output=, seed=, log_std=, mask= and value= are options of the 'mlp' op, not of "
-                             f"'{op}'")
+            raise ValueError(f"bias=, output=, seed=, log_std=, mask=, value= and nvec= are options of the 'mlp' op, "
+                             f"not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
@@ -122,6 +126,8 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
             v = extra["value"]
             if not isinstance(v, (tuple, list)) or len(v) != 2 or not all(isinstance(n, str) for n in v):
                 raise ValueError(f"value must name two call arguments (wv, bv), got {v!r}")
+        if "nvec" in extra:
+            extra["nvec"] = check_nvec(extra["nvec"], extra.get("output", "logits"))
 
     def deco(fn):
         params = inspect.signature(fn).parameters
@@ -135,6 +141,23 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
         return fn
 
     return deco
+
+
+def check_nvec(nvec, output: str, d_out: Optional[int] = None) -> tuple:
+    """nvec as a tuple, or ValueError naming what is wrong with it: given with an output other than "actions", "both"
+    and "sample"; not a tuple or list of ints (bools refused); empty; an entry below 1; (with d_out) a sum other than
+    d_out."""
+    if output not in ("actions", "both", "sample"):
+        raise ValueError(f'nvec is an option of output="actions", "both" and "sample", not of output={output!r}')
+    if not isinstance(nvec, (tuple, list)) or not all(isinstance(n, int) and not isinstance(n, bool) for n in nvec):
+        raise ValueError(f"nvec must be a tuple of ints, got {nvec!r}")
+    if len(nvec) == 0:
+        raise ValueError("nvec is empty: a multi-discrete action space has at least one group")
+    if any(n < 1 for n in nvec):
+        raise ValueError(f"every entry of nvec must be >= 1 (a group of at least one action), got {tuple(nvec)}")
+    if d_out is not None and sum(nvec) != d_out:
+        raise ValueError(f"nvec sums to {sum(nvec)}, not d_out={d_out}: its groups tile the head's columns")
+    return tuple(nvec)
 
 
 def mapped_spec(fn) -> Optional[MappedSpec]:

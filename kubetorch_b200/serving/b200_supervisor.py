@@ -596,7 +596,7 @@ class B200Supervisor:
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
-                                         value=value)
+                                         value=value, nvec=spec.extra.get("nvec"))
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

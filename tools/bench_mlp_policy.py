@@ -20,6 +20,11 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      63, 64 and 255: output="sample", output="sample" with a random legal-action mask and output="gaussian", each
      right after the same call without a value head; and the eager critic, what a user pays without the fused value:
      the unfused output="sample" call plus the trunk and the value head recomputed with F.linear in torch
+  k  multi-discrete heads (nvec=), nvec (3,)*6, (2,)*32, (6, 4, 4, 4, 4, 7, 49) and (2,)*128 (d_out 18, 64, 78 and
+     256): greedy actions and output="sample", each unmasked and under a random legal-action mask, each beside the
+     single-categorical call of the same d_out and output; and the eager arm, what a user pays without the grouped
+     head: the logits entry (masked in torch under a mask), then split, Gumbel noise, argmax and log_softmax in torch.
+     (2,)*128 shows the cost of 128 per-group quad reductions.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -27,7 +32,11 @@ exceeds 2^-18·(1 + max|s|), and the log-probability is within (d_out + 8)·2^-2
 Masked rows: the masked actions equal torch.argmax of the kernel's logits filled with -inf on every row, and every
 sampled action on a row with a legal action is legal.  Value rows: every valued call's actions and log-probabilities
 equal those of the same call without a value head on every row, bit for bit, the masked call's values equal the
-unmasked call's, and the values are within rtol 2^-7, atol 1e-2 of the eager critic's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+unmasked call's, and the values are within rtol 2^-7, atol 1e-2 of the eager critic's.  Multi-discrete rows: the
+greedy actions equal the per-group argmax of the kernel's (masked) logits on every row; the sampled actions equal the
+eager arm's on at least 99.9 % of the rows (its noise comes from torch's log, not the kernel's logf), its
+log-probabilities within 2^-16·(1 + |ref|) on those rows, and every masked sample in a group with a legal action is
+legal.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -45,7 +54,7 @@ import torch.nn.functional as F  # noqa: E402
 from kubetorch_b200.device import lib as L  # noqa: E402
 from kubetorch_b200.device import mlp  # noqa: E402
 from kubetorch_b200.device import ops  # noqa: E402
-from kubetorch_b200.sampling import gumbel_uniform  # noqa: E402
+from kubetorch_b200.sampling import gumbel_noise, gumbel_uniform  # noqa: E402
 
 HALF_LOG_2PI = 0.9189385332046727
 
@@ -166,6 +175,40 @@ def main():
             return actions, log_probs, F.linear(h, *critic).float().squeeze(-1)
 
         variants[f"j_bias_eager_critic_d{d}"] = (d, eager_critic)
+    gk = torch.Generator(device="cuda:0").manual_seed(9)   # its own generator again
+    heads[78] = ((torch.randn(78, d_hidden, device="cuda:0", generator=gk) * 0.02).bfloat16(),
+                 (torch.randn(78, device="cuda:0", generator=gk) * 0.1).bfloat16())
+    legal[78] = torch.rand(M, 78, device="cuda:0", generator=gk) < 0.5
+    nvecs = {18: (3,) * 6, 64: (2,) * 32, 78: (6, 4, 4, 4, 4, 7, 49), 256: (2,) * 128}
+
+    def eager_groups(d, mask, sample):
+        """The logits entry, then the grouped head in torch: what a user pays without nvec=."""
+        y = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]))
+        if mask:
+            y = y.masked_fill(~legal[d], float("-inf"))
+        y = y.float()
+        z = y + gumbel_noise(SEED, 0, M, d, device="cuda:0") if sample else y
+        acts = torch.stack([p.argmax(-1) for p in z.split(nvecs[d], -1)], -1)
+        if not sample:
+            return acts
+        lp = None
+        for i, p in enumerate(y.split(nvecs[d], -1)):
+            t = torch.log_softmax(p, -1).gather(-1, acts[:, i:i + 1]).squeeze(-1)
+            lp = t if lp is None else lp + t
+        return acts, lp
+
+    for d, nvec in nvecs.items():
+        bs = (b1, b2, heads[d][1])
+        for mask in (False, True):
+            m = dict(mask=legal[d]) if mask else {}
+            tag = "masked_" if mask else ""
+            for out, kw in (("actions", dict(output="actions")), ("sample", dict(output="sample", seed=SEED))):
+                variants[f"k_bias_{tag}{out}_d{d}"] = (d, lambda d=d, bs=bs, kw=kw, m=m: mlp.mlp_forward(
+                    obs, w1, w2, heads[d][0], biases=bs, **kw, **m))
+                variants[f"k_bias_{tag}{out}_nvec_d{d}"] = (d, lambda d=d, bs=bs, kw=kw, m=m, nvec=nvec: mlp.mlp_forward(
+                    obs, w1, w2, heads[d][0], biases=bs, nvec=nvec, **kw, **m))
+                variants[f"k_bias_{tag}{out}_eager_d{d}"] = (d, lambda d=d, mask=mask, out=out: eager_groups(
+                    d, mask, out == "sample"))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -267,6 +310,37 @@ def main():
         entry["values_vs_eager_critic"] = "ok"
         parity[f"j_bias_value_d{d}"] = entry
         del eager, values
+
+    for d, nvec in nvecs.items():
+        entry = {}
+        for tag in ("", "masked_"):
+            logits = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]))
+            if tag:
+                logits = logits.masked_fill(~legal[d], float("-inf"))
+            greedy = variants[f"k_bias_{tag}actions_nvec_d{d}"][1]()
+            assert torch.equal(greedy, torch.stack([p.argmax(-1) for p in logits.split(nvec, -1)], -1)), (tag, d)
+            assert torch.equal(greedy, variants[f"k_bias_{tag}actions_eager_d{d}"][1]()), (tag, d)
+            del logits, greedy
+            acts, lp = variants[f"k_bias_{tag}sample_nvec_d{d}"][1]()
+            want_a, want_lp = variants[f"k_bias_{tag}sample_eager_d{d}"][1]()
+            rows = (acts == want_a).all(-1)
+            assert float(rows.double().mean()) >= 0.999, (tag, d, float(rows.double().mean()))
+            a_lp, b_lp = lp[rows], want_lp[rows]
+            fin = b_lp.isfinite()
+            assert torch.equal(fin, a_lp.isfinite()), (tag, d)
+            assert bool(((a_lp[fin] - b_lp[fin]).abs() <= 2.0 ** -16 * (1 + b_lp[fin].abs())).all()), (tag, d)
+            entry[f"{tag}greedy_eq_group_argmax_all_rows"] = "ok"
+            entry[f"{tag}sample_rows_eq_eager"] = round(float(rows.double().mean()), 6)
+            if tag:
+                lo = 0
+                for i, n in enumerate(nvec):
+                    part = legal[d][:, lo:lo + n]
+                    has = part.any(-1)
+                    assert bool(part[has].gather(1, acts[has][:, i:i + 1]).all()), (d, i)
+                    lo += n
+                entry["masked_samples_legal_all_rows"] = "ok"
+            del acts, lp, want_a, want_lp
+        parity[f"k_bias_nvec_d{d}"] = entry
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
