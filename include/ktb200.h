@@ -497,6 +497,59 @@ int ktb_mlp_bf16_policy_gaussian_value_pushed(int dev, const void* stage_local, 
                                               float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer,
                                               int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* State-dependent Gaussian forms: the Gaussian entries with a per-row log standard deviation from a second linear head
+ * on the same trunk, clamped, and optionally tanh-squashed actions (SAC's actor).  Each takes the arguments of its
+ * _gaussian counterpart with W3s / b3s (W3sv / b3sv) in place of W3 / b3 (W3v / b3v) and (log_std_min, log_std_max,
+ * squash) in place of log_std.  d_out stays the action width.
+ *   - W3s [2*d_out, d_hidden] bf16 interleaves the mean's and the log-std's weights: row 2j is w3[j], row 2j + 1 is
+ *     w_ls[j]; b3s [2*d_out] likewise interleaves b3 and b_ls, or is NULL when neither has a bias.  With a value head,
+ *     W3sv / b3sv have the critic's row 2*d_out after them, and values are as in the value forms.
+ *   - mu_ij and l_ij are the bf16-rounded head outputs of rows 2j and 2j + 1 (ktb_mlp_bf16_policy's logits over W3s);
+ *     lc = l clamped to [log_std_min, log_std_max] by comparisons, so a NaN l stays NaN; infinite bounds clamp nothing.
+ *   - z_ij is the noise of the Gaussian form for action column j (Philox word j & 1 of counter (i, j >> 1, 1)), and
+ *     u = __fadd_rn(mu_ij, __fmul_rn(expf(lc), z_ij)), the Gaussian form's rounding.  actions[i, j] = tanhf(u) when
+ *     squash != 0, u otherwise.  Squashed actions may be exactly +-1.0 in fp32.
+ *   - log_probs[i] = -sum_j (0.5*z^2 + lc) - d_out*0.5*log(2*pi), and with squash also -sum_j c(u) with
+ *     c(u) = 2*(log 2 - |u| - log1pf(expf(-2|u|))) = log(1 - tanh(u)^2) exactly (not SB3's log(1 - tanh^2 + 1e-6),
+ *     which differs where 1 - tanh^2 nears 1e-6, |u| > about 7).  It is computed from u, so it stays finite where the
+ *     action rounds to +-1.0.  Terms are summed per thread and then across 4 lanes, so the order differs from the
+ *     Gaussian form's.
+ *   - IEEE cases: a NaN l gives a NaN action in its column and a NaN log-probability.  An infinite log_std_max lets
+ *     expf(lc) overflow to +inf: then u = +-inf, the action is +-1.0 (squashed) or +-inf, and c(u) = -inf makes
+ *     the squashed log-probability +inf (NaN when lc is itself +inf: -inf + inf); unsquashed it is -inf only when lc
+ *     is +inf.  lc = -inf gives sigma = 0, u == mu and an unsquashed log-probability of +inf.
+ *   - With w_ls = 0 and b_ls = c, the unsquashed actions are those of the Gaussian form with log_std = c, bit for bit.
+ *   - Checks: every check of the _gaussian counterpart first (log_std excepted), then, with M > 0: 2*d_out (+1 with
+ *     a value head) > 256, that is d_out > 128 (> 127), is KTB_ERR_UNSUPPORTED; a NaN bound or log_std_min >
+ *     log_std_max is KTB_ERR_ARG.  An empty pushed shard (M == 0) may pass NULL outputs and still publishes its ack.
+ *     Writes stay inside actions[M, d_out], log_probs[M], values[M] (value forms), scratch and stage. */
+int ktb_mlp_bf16_policy_gaussian_state(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3s,
+                                       const void* b3s, float log_std_min, float log_std_max, int squash,
+                                       uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
+                                       void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_state_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                              int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                              const void* b2, const void* W3s, const void* b3s, float log_std_min,
+                                              float log_std_max, int squash, uint64_t seed, uint64_t row_base,
+                                              float* actions, float* log_probs, void* scratch, void* ctrl_local,
+                                              void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                              unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_state_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                             const void* W1, const void* b1, const void* W2, const void* b2,
+                                             const void* W3sv, const void* b3sv, float log_std_min, float log_std_max,
+                                             int squash, uint64_t seed, uint64_t row_base, float* actions,
+                                             float* log_probs, float* values, void* scratch, void* stage,
+                                             uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_state_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                    int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                    const void* W2, const void* b2, const void* W3sv,
+                                                    const void* b3sv, float log_std_min, float log_std_max, int squash,
+                                                    uint64_t seed, uint64_t row_base, float* actions,
+                                                    float* log_probs, float* values, void* scratch, void* ctrl_local,
+                                                    void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                    unsigned long long seq, uintptr_t stream);
+
 /* Multi-discrete forms: the greedy and sampling entries above (masked, pushed and with a value head as they come) for
  * a MultiDiscrete(nvec) action space, one categorical sub-action per group of head columns.  Each takes the
  * arguments of its categorical counterpart with (nvec, n_groups) inserted after b3 (or b3v).

@@ -418,6 +418,17 @@ struct HeadGroups {
   bool greedy = false;   // rank the logits alone: no noise and no log-probabilities (outputs "actions" and "both")
 };
 
+// The log-std of a state-dependent Gaussian head, the layer kernel's last parameter (by value: no upload per call):
+// with `state` the head's weight interleaves the mean's and the log-std's rows, and the log-std is clamped to
+// [lo, hi]; `squash` passes the actions through tanh.  state == false is the state-independent log_std of the other
+// entries.  It is a parameter of its own rather than a member of HeadOut: a larger HeadOut re-schedules the kSample
+// instantiations, which never read it.
+struct HeadStd {
+  float lo = 0.f, hi = 0.f;
+  bool state = false;
+  bool squash = false;
+};
+
 // The end of the group that begins at column lo: the next set bit of `starts` past lo, or d.  The words are indexed
 // at compile time, so the bitmap stays in the kernel's parameters.
 __device__ __forceinline__ int group_end(const uint32_t (&starts)[8], int lo, int d) {
@@ -689,11 +700,17 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
 // base allow and as scalars otherwise, and Σ (0.5·z² + log_std) per row for the log-probability, which does not read μ.
 // With a value head (values != null) the tile holds n_valid = d + 1 columns, as in sample_epilogue: the rolled pass,
 // the actions' row stride and the log-density's constant cover the policy's d columns only.
+// A state-dependent head (sd.state) takes a rolled pass of its own after the same pass 1: its d = 2·d_out policy
+// columns interleave the mean and the log-std, so pair (2a, 2a + 1) of a thread is (μ_a, ℓ_a) of action a, one parked
+// bf16x2 slot.  ℓ is clamped to [sd.lo, sd.hi] by compares (a NaN stays NaN), σ = expf(ℓc), z is Philox word a & 1
+// of counter (i, a >> 1, 1) (the noise of action a in the head above), u = μ + σ·z rounded as above, and the action is
+// tanhf(u) with sd.squash, u without; the row sums 0.5·z² + ℓc, plus 2·(log 2 − |u| − log1p(e^−2|u|)) =
+// −log(1 − tanh²u) with sd.squash, over its d_out actions.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                   int n_valid, int row, bool st0, bool st1, const float* log_std,
                                                   float* actions, float* log_probs, uint64_t seed, uint64_t row_base,
-                                                  float* values) {
+                                                  float* values, const HeadStd& sd) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -711,9 +728,33 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
   const int d = n_valid - (values != nullptr);   // the policy's columns
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const bool pairs = (d & 1) == 0 && ((uintptr_t)actions & 7) == 0;
+  const int d_act = sd.state ? d >> 1 : d;   // the actions per row
   float sum[2] = {0.f, 0.f};
 #pragma unroll 1
-  for (int j = 0; j < BLOCK_N / 8; ++j) {
+  for (int j = 0; sd.state && j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= d) break;   // d is even: col + 1 < d
+    const int a = col >> 1;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const __nv_bfloat162 y = *slot(2 * j + h);
+      const float l = __high2float(y);
+      const float lc = l < sd.lo ? sd.lo : l > sd.hi ? sd.hi : l;   // not fminf / fmaxf: they drop a NaN
+      const uint64_t i = row_base + (uint64_t)(row + 8 * h);
+      const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)a >> 1, 1u), key);
+      const float z = normcdfinvf((float)(2u * ((a & 1 ? x.y : x.x) >> 9) + 1u) * 5.9604644775390625e-8f);
+      const float u = __fadd_rn(__low2float(y), __fmul_rn(expf(lc), z));
+      float t = 0.5f * z * z + lc;
+      if (sd.squash) {
+        const float au = fabsf(u);
+        t += 2.f * (0.693147180559945309f - au - log1pf(expf(-2.f * au)));
+      }
+      sum[h] += t;
+      if (h ? st1 : st0) actions[(size_t)(row + 8 * h) * d_act + a] = sd.squash ? tanhf(u) : u;
+    }
+  }
+#pragma unroll 1
+  for (int j = 0; !sd.state && j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
     if (col >= d) break;   // a pair wholly past the policy draws no noise
     const __nv_bfloat162 y[2] = {*slot(2 * j), *slot(2 * j + 1)};
@@ -750,7 +791,7 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
     for (int m = 1; m <= 2; m <<= 1) sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
   }
   if ((threadIdx.x & 3) == 0) {
-    const float c = (float)d * 0.918938533204672742f;   // d_out·0.5·log(2π)
+    const float c = (float)d_act * 0.918938533204672742f;   // d_out·0.5·log(2π)
     if (st0) log_probs[row] = -sum[0] - c;
     if (st1) log_probs[row + 8] = -sum[1] - c;
   }
@@ -808,6 +849,9 @@ struct HeadOut {
 //     log_softmax(logits)[action] in fp32 (sample_epilogue);
 //   kGaussian: gauss_actions[row, j] = logit_j + exp(log_std_j)·z_j with z_j = Φ⁻¹(u) of Philox word j & 1 of counter
 //     (i, j >> 1, 1), and log_probs[row] the diagonal Normal's log-density of that action (gaussian_epilogue);
+//   kGaussian with sd.state: μ and the clamped log-std from the interleaved columns (2a, 2a + 1), optionally
+//     tanh-squashed actions, and the log-density with its tanh correction (gaussian_epilogue); n_valid = 2·d_out, and
+//     a value head's column is 2·d_out;
 //   kSample and kGaussian with out.values: n_valid = d_out + 1, and values[row] = fp32(column d_out) (store_values);
 //   kSample with out.groups: one greedy or sampled action per group of columns into actions[row, g], the summed
 //     log-probability of the sampled ones, and the logits of a greedy head that stores them (group_pass).
@@ -819,7 +863,8 @@ struct HeadOut {
 template <int BLOCK_N, int STAGES, HeadKind KIND>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                           const __nv_bfloat16* bias, const HeadOut out, int n_valid, int K, int rows) {
+                           const __nv_bfloat16* bias, const HeadOut out, int n_valid, int K, int rows,
+                           const HeadStd sd) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -842,7 +887,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
                              out.row_base, out.values, out.groups, C);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
-                                       out.log_probs, out.seed, out.row_base, out.values);
+                                       out.log_probs, out.seed, out.row_base, out.values, sd);
   }
 }
 
@@ -928,7 +973,7 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
 // One layer through the epilogue of KIND in BLOCK_N-wide tiles: out = A[M, K] · B[N, K]ᵀ (+ bias), N columns.
 template <int BLOCK_N, HeadKind KIND>
 static int launch_layer(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                        int K, cudaStream_t stream) {
+                        int K, cudaStream_t stream, const HeadStd& sd = HeadStd{}) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -941,17 +986,18 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
-  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M);
+  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M, sd);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
 
-// The head of KIND, in the smallest tile that holds its N columns (d_out, or d_out + 1 with a value head).
+// The head of KIND, in the smallest tile that holds its N columns (d_out, 2·d_out for a state-dependent Gaussian
+// head, one more with a value head).
 template <HeadKind KIND>
 static int launch_head(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                       int K, cudaStream_t stream) {
+                       int K, cudaStream_t stream, const HeadStd& sd) {
   const auto launch = N <= 64 ? launch_layer<64, KIND> : N <= 128 ? launch_layer<128, KIND> : launch_layer<256, KIND>;
-  return launch(dev, A, B, bias, out, M, N, K, stream);
+  return launch(dev, A, B, bias, out, M, N, K, stream, sd);
 }
 
 // Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
@@ -960,6 +1006,8 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // staging half in the pushed forms.  `valued` marks the _value entries: W3 / b3 are the stacked W3v [d_out + 1,
 // d_hidden] / b3v [d_out + 1] of the policy and its value head, and out.values receives the value of each row.
 // `nvec` (n_groups entries, a host array) marks the _multidiscrete entries: mlp_run checks it and builds out.groups.
+// std.state marks the _gaussian_state entries: W3 / b3 are the interleaved W3s [2·d_out, d_hidden] / b3s (with a
+// value head W3sv / b3sv, one more row), log_std is null, and mlp_run checks the bounds.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -970,6 +1018,7 @@ struct MlpParams {
   const int32_t* nvec = nullptr;
   int n_groups = 0;
   bool grouped = false;
+  HeadStd std;
 
   // A multi-discrete head: the greedy one (logits and/or actions, ranked without noise) or the sampled one, both in
   // the kSample instantiations.
@@ -980,6 +1029,14 @@ struct MlpParams {
     p.nvec = nvec;
     p.n_groups = n_groups;
     p.grouped = true;
+    return p;
+  }
+
+  // A state-dependent Gaussian head, in the kGaussian instantiations: log-std bounds [lo, hi], tanh with squash != 0.
+  static MlpParams gaussian_state(const void* W1, const void* b1, const void* W2, const void* b2, const void* W3s,
+                                  const void* b3s, float lo, float hi, int squash, const HeadOut& out) {
+    MlpParams p{W1, b1, W2, b2, W3s, b3s, HeadKind::kGaussian, out};
+    p.std = HeadStd{lo, hi, true, squash != 0};
     return p;
   }
 
@@ -999,7 +1056,8 @@ struct MlpParams {
 
 // Rows [r0, r0 + rows) of a call: the hidden layers h1 = relu(a1 · W1ᵀ (+ b1)) and h2 = relu(h1 · W2ᵀ (+ b2)), then
 // the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds its d_out
-// columns, d_out + 1 with a value head.  `consumed`, unless null, is recorded once layer 1 has read a1.
+// columns (2·d_out for a state-dependent Gaussian head), one more with a value head.  `consumed`, unless null, is
+// recorded once layer 1 has read a1.
 static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void* a1, void* h1, void* h2, size_t r0,
                      size_t rows, int d_in, int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
   int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
@@ -1010,7 +1068,8 @@ static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void
   const auto head = p.kind == HeadKind::kGreedy   ? launch_head<HeadKind::kGreedy>
                     : p.kind == HeadKind::kSample ? launch_head<HeadKind::kSample>
                                                   : launch_head<HeadKind::kGaussian>;
-  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, d_out + (int)p.valued, d_hidden, st);
+  const int n = (p.std.state ? 2 * d_out : d_out) + (int)p.valued;
+  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std);
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -1036,8 +1095,11 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
           KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
-        KTB_REQUIRE(o.log_std && o.gauss_actions && o.log_probs, KTB_ERR_ARG,
-                    "%s: log_std, actions and log_probs are required", fn);
+        if (p.std.state)   // a state-dependent head reads its log-std from the head's own columns
+          KTB_REQUIRE(o.gauss_actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
+        else
+          KTB_REQUIRE(o.log_std && o.gauss_actions && o.log_probs, KTB_ERR_ARG,
+                      "%s: log_std, actions and log_probs are required", fn);
         KTB_REQUIRE((((uintptr_t)o.log_std | (uintptr_t)o.gauss_actions) & 3) == 0, KTB_ERR_ARG,
                     "%s: log_std and actions must be 4-byte aligned", fn);
         break;
@@ -1094,7 +1156,8 @@ struct MlpFeed {
 // and past the rows in the pushed forms) come after every check of the unmasked entry, and a value entry's (values,
 // d_out <= 255; skipped for an empty call) after every check of the entry without a value head.  A multi-discrete
 // entry's nvec (skipped for an empty call) is checked last, and read into the launch's HeadGroups before the call
-// returns.
+// returns.  A state-dependent Gaussian entry's head width (2·d_out, one more with a value head, <= 256) and log-std
+// bounds (skipped for an empty call) come after every check of its state-independent counterpart.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1137,6 +1200,14 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     KTB_REQUIRE(((uintptr_t)p.out.values & 3) == 0, KTB_ERR_ARG, "%s: values must be 4-byte aligned", fn);
     KTB_REQUIRE(d_out <= 255, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the policy and its value column fit one 256-wide tile)",
                 fn, d_out);
+  }
+  if (p.std.state && M > 0) {
+    KTB_REQUIRE(2 * d_out + (int)p.valued <= 256, KTB_ERR_UNSUPPORTED,
+                "%s: d_out=%d (the interleaved mean and log-std%s fit one 256-wide tile)", fn, d_out,
+                p.valued ? " and the value column" : "");
+    const float lo = p.std.lo, hi = p.std.hi;
+    KTB_REQUIRE(lo == lo && hi == hi && lo <= hi, KTB_ERR_ARG, "%s: log_std bounds [%g, %g] must be ordered, not NaN",
+                fn, (double)lo, (double)hi);
   }
   HeadGroups groups = p.out.groups;
   if (p.grouped && M > 0) {
@@ -1442,6 +1513,60 @@ int ktb_mlp_bf16_policy_gaussian_value_pushed(int dev, const void* stage_local, 
                                 {nullptr, nullptr, log_probs, seed, row_base, log_std, actions}}
                           .with_values(values);
   return mlp_run("ktb_mlp_bf16_policy_gaussian_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_state(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3s,
+                                       const void* b3s, float log_std_min, float log_std_max, int squash,
+                                       uint64_t seed, uint64_t row_base, float* actions, float* log_probs,
+                                       void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::gaussian_state(W1, b1, W2, b2, W3s, b3s, log_std_min, log_std_max, squash,
+                                                {nullptr, nullptr, log_probs, seed, row_base, nullptr, actions});
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_state", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_state_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                              int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                              const void* b2, const void* W3s, const void* b3s, float log_std_min,
+                                              float log_std_max, int squash, uint64_t seed, uint64_t row_base,
+                                              float* actions, float* log_probs, void* scratch, void* ctrl_local,
+                                              void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                              unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::gaussian_state(W1, b1, W2, b2, W3s, b3s, log_std_min, log_std_max, squash,
+                                                {nullptr, nullptr, log_probs, seed, row_base, nullptr, actions});
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_state_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_state_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                             const void* W1, const void* b1, const void* W2, const void* b2,
+                                             const void* W3sv, const void* b3sv, float log_std_min, float log_std_max,
+                                             int squash, uint64_t seed, uint64_t row_base, float* actions,
+                                             float* log_probs, float* values, void* scratch, void* stage,
+                                             uintptr_t stream) {
+  const MlpParams p = MlpParams::gaussian_state(W1, b1, W2, b2, W3sv, b3sv, log_std_min, log_std_max, squash,
+                                                {nullptr, nullptr, log_probs, seed, row_base, nullptr, actions})
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_state_value", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_state_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                    int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                    const void* W2, const void* b2, const void* W3sv,
+                                                    const void* b3sv, float log_std_min, float log_std_max, int squash,
+                                                    uint64_t seed, uint64_t row_base, float* actions,
+                                                    float* log_probs, float* values, void* scratch, void* ctrl_local,
+                                                    void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                    unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::gaussian_state(W1, b1, W2, b2, W3sv, b3sv, log_std_min, log_std_max, squash,
+                                                {nullptr, nullptr, log_probs, seed, row_base, nullptr, actions})
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_state_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
                  stream);
 }

@@ -171,6 +171,13 @@ for _head, _suffixes in (("ktb_mlp_bf16_policy", ("", "_masked")),
             _restype, _args = _SIGNATURES[_head + _suffix + _form]
             _SIGNATURES[_head + "_multidiscrete" + _suffix + _form] = (
                 _restype, _args[:_at] + [POINTER(ctypes.c_int32), c_int] + _args[_at:])
+# The _gaussian_state entries: each takes its _gaussian counterpart's arguments with (log_std_min, log_std_max, squash)
+# in place of log_std, the 13th argument of the plain and staged forms and the 14th of the pushed ones.
+for _suffix in ("", "_value"):
+    for _form, _at in (("", 12), ("_pushed", 13)):
+        _restype, _args = _SIGNATURES["ktb_mlp_bf16_policy_gaussian" + _suffix + _form]
+        _SIGNATURES["ktb_mlp_bf16_policy_gaussian_state" + _suffix + _form] = (
+            _restype, _args[:_at] + [ctypes.c_float, ctypes.c_float, c_int] + _args[_at + 1:])
 
 _lib = None
 _lock = threading.Lock()

@@ -3,7 +3,8 @@ ktb_mlp_bf16_policy (biases, heads of 1 to 256 outputs, greedy actions), ktb_mlp
 Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_mlp_bf16_policy_gaussian (seeded
 diagonal-Gaussian actions with their log-probabilities), the _masked forms of the first two (a per-row legal-action
 mask), the _value forms of the sampled heads (a critic's state value on the same trunk), the _multidiscrete forms of
-the greedy and sampled heads (one categorical per group of columns) and their scatter→exec→gather form."""
+the greedy and sampled heads (one categorical per group of columns), the _gaussian_state forms (a per-row log-std
+head, optionally tanh-squashed actions) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -21,7 +22,7 @@ from ..sampling import _check_seed
 _scratch = {}
 _stage = {}
 _weight_cache = {}
-_stacked_heads = {}   # (device, id(w3)) -> [weakref to w3, stamp of w3 / b3 / wv / bv, W3v, b3v]
+_stacked_heads = {}   # (device, id(w3)) -> [weakref to w3, stamp of w3 / b3 / wv / bv / w_ls / b_ls, W3, b3]
 _pool = None
 
 
@@ -58,6 +59,7 @@ def _thread_pool():
 
 
 MAX_D_OUT = 256
+LOG_STD_BOUNDS = (-20.0, 2.0)   # SB3's and Spinning Up's clamp of a SAC actor's log-std
 
 
 def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
@@ -86,8 +88,46 @@ def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
                          f"({w3.device})")
 
 
+def _check_state_std(log_std, log_std_bounds, squash, w3, b3, d_hidden, d_out, valued) -> None:
+    """_check_policy's checks of a state-dependent log-std head log_std = (w_ls, b_ls), in this order: the pair, the
+    head width (2·d_out columns, one more with a value head, in one 256-wide tile), b_ls given exactly when b3 is,
+    w_ls's dtype and shape, layout and device, b_ls, then the bounds and squash."""
+    if len(log_std) != 2:
+        raise ValueError("log_std must be a tensor or (w_ls, b_ls): the log-std head's weight [d_out, d_hidden] and "
+                         "its bias [d_out] or None")
+    w_ls, b_ls = log_std
+    limit = (MAX_D_OUT - valued) // 2
+    if d_out > limit:
+        raise ValueError(f"d_out={d_out}: a log-std head allows 1 to {limit} actions (the interleaved mean and "
+                         f"log-std{' and the value column' if valued else ''} must fit one {MAX_D_OUT}-wide tile)")
+    if (b_ls is None) != (b3 is None):
+        raise ValueError("log_std: b_ls is given exactly when b3 is (a zero bias in the mean's columns would turn -0.0 "
+                         "means into +0.0)")
+    if not isinstance(w_ls, torch.Tensor) or w_ls.dtype != torch.bfloat16 or tuple(w_ls.shape) != (d_out, d_hidden):
+        raise ValueError(f"log_std: w_ls must be a bfloat16 tensor of shape ({d_out}, {d_hidden})")
+    if not w_ls.is_contiguous():
+        raise ValueError("log_std: w_ls must be contiguous")
+    if not w_ls.is_cuda or w_ls.device != w3.device:
+        raise ValueError(f"log_std: w_ls must be a CUDA tensor on the device of w3 ({w3.device}), got {w_ls.device}")
+    if b_ls is not None and (not isinstance(b_ls, torch.Tensor) or b_ls.dtype != torch.bfloat16
+                             or tuple(b_ls.shape) != (d_out,) or not b_ls.is_contiguous() or b_ls.device != w3.device):
+        raise ValueError(f"log_std: b_ls must be a contiguous bfloat16 tensor of shape ({d_out},) on the device of w3 "
+                         f"({w3.device})")
+    if log_std_bounds is not None:
+        if not isinstance(log_std_bounds, (tuple, list)) or len(log_std_bounds) != 2 or \
+                not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in log_std_bounds):
+            raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {log_std_bounds!r}")
+        lo, hi = (float(b) for b in log_std_bounds)
+        if lo != lo or hi != hi:
+            raise ValueError(f"log_std_bounds must not be NaN, got {log_std_bounds!r}")
+        if lo > hi:
+            raise ValueError(f"log_std_bounds must have low <= high, got {log_std_bounds!r}")
+    if squash is not None and not isinstance(squash, bool):
+        raise ValueError(f"squash must be True or False, got {squash!r}")
+
+
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
-                  nvec=None) -> None:
+                  nvec=None, log_std_bounds=None, squash=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
     (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
@@ -95,7 +135,9 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     given with any output but "gaussian"; a value head (wv, bv), given with output="sample" or "gaussian" only, is a
     contiguous bfloat16 wv [1, d_hidden] and a contiguous bfloat16 bv [1] (given exactly when b3 is), both on the
     device of w3, beside a policy at most 255 wide; nvec (output="actions", "both" or "sample" only) is a non-empty
-    tuple or list of ints >= 1 that sums to d_out (mapped.check_nvec)."""
+    tuple or list of ints >= 1 that sums to d_out (mapped.check_nvec).  With output="gaussian", log_std may instead
+    be a state-dependent head (w_ls, b_ls) (_check_state_std), and log_std_bounds and squash are taken with that form
+    only."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
     if output in ("sample", "gaussian"):
@@ -109,11 +151,16 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
         raise ValueError(f"d_out={d_out}: the policy head is 1 to {MAX_D_OUT} wide")
     if nvec is not None:
         check_nvec(nvec, output, d_out)
-    if output != "gaussian":
-        if log_std is not None:
-            raise ValueError('log_std is an argument of output="gaussian" only')
-    elif not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32 or not log_std.is_cuda \
-            or not log_std.is_contiguous() or log_std.dim() != 1 or log_std.shape[0] != d_out:
+    state = isinstance(log_std, (tuple, list))
+    if output != "gaussian" and log_std is not None:
+        raise ValueError('log_std is an argument of output="gaussian" only')
+    if not state and (log_std_bounds is not None or squash is not None):
+        raise ValueError("log_std_bounds and squash are options of a state-dependent log_std=(w_ls, b_ls) only")
+    if output == "gaussian" and state:
+        _check_state_std(log_std, log_std_bounds, squash, w3, biases[2], d_hidden, d_out, value is not None)
+    elif output == "gaussian" and (not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32
+                                   or not log_std.is_cuda or not log_std.is_contiguous() or log_std.dim() != 1
+                                   or log_std.shape[0] != d_out):
         raise ValueError(f"log_std must be a 1-D contiguous CUDA float32 tensor of length {d_out}")
     if mask is not None:
         if not isinstance(obs, torch.Tensor):
@@ -136,13 +183,14 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
             raise ValueError(f"{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
 
 
-def _stacked_head(w3, b3, wv, bv) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
-    """(W3v, b3v): the policy's head with the critic's under it, W3v = [w3; wv] [d_out + 1, d_hidden] and
-    b3v = [b3; bv] (None without biases), on the device of w3.  One entry per (device, head) is kept, and rewritten in
-    place when w3, b3, wv or bv has a new data_ptr or _version: a PPO loop updates its weights in place between
-    rollouts.  Rewriting in place bumps W3v's and b3v's own _version, so _weights_on copies the new head to other
-    devices."""
-    stamp = tuple(None if t is None else (t.data_ptr(), t._version) for t in (w3, b3, wv, bv))
+def _stacked_head(w3, b3, wv=None, bv=None, w_ls=None, b_ls=None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """(W3, b3) of the head a C entry runs, on the device of w3: with a log-std head (w_ls, b_ls) the rows of w3 and
+    w_ls interleaved, W3s = [w3_0; w_ls_0; w3_1; w_ls_1; ...] [2·d_out, d_hidden]; with a value head the critic's wv
+    under them (W3v = [w3; wv] or W3sv = [W3s; wv]); the biases likewise (None without biases).  One entry per
+    (device, head) is kept, and rewritten in place when any part has a new data_ptr or _version: PPO and SAC loops
+    update their weights in place between rollout steps.  Rewriting in place bumps the head's own _version, so
+    _weights_on copies the new head to other devices."""
+    stamp = tuple(None if t is None else (t.data_ptr(), t._version) for t in (w3, b3, wv, bv, w_ls, b_ls))
     key = (w3.device.index, id(w3))
     entry = _stacked_heads.get(key)
     if entry is None or entry[0]() is not w3:
@@ -151,14 +199,21 @@ def _stacked_head(w3, b3, wv, bv) -> Tuple[torch.Tensor, Optional[torch.Tensor]]
                 del _stacked_heads[k]
         entry = _stacked_heads[key] = [weakref.ref(w3), None, None, None]
     if entry[1] != stamp:
-        for i, parts in ((2, (w3, wv)), (3, None if b3 is None else (b3, bv))):
-            if parts is None:
+        for i, (mean, ls, v) in ((2, (w3, w_ls, wv)), (3, (b3, b_ls, bv))):
+            if mean is None:
                 entry[i] = None
-            elif entry[i] is not None and entry[i].shape[0] == parts[0].shape[0] + 1 \
-                    and entry[i].shape[1:] == parts[0].shape[1:]:
-                torch.cat(parts, out=entry[i])
+                continue
+            d = mean.shape[0]
+            shape = ((2 * d if ls is not None else d) + (v is not None),) + tuple(mean.shape[1:])
+            if entry[i] is None or tuple(entry[i].shape) != shape:
+                entry[i] = torch.empty(shape, dtype=mean.dtype, device=mean.device)
+            if ls is None:
+                entry[i][:d].copy_(mean)
             else:
-                entry[i] = torch.cat(parts)
+                entry[i][0:2 * d:2].copy_(mean)
+                entry[i][1:2 * d:2].copy_(ls)
+            if v is not None:
+                entry[i][shape[0] - 1:].copy_(v)
         entry[1] = stamp
     return entry[2], entry[3]
 
@@ -187,17 +242,21 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
 
 
 def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None,
-          nvec=None):
+          nvec=None, std=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
     mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
     picks the _value entry (whose W3 and b3 are the stacked head) and is its values buffer.  `nvec`, unless None,
-    picks the _multidiscrete entry and is its group sizes."""
+    picks the _multidiscrete entry and is its group sizes.  `std` = (log_std_min, log_std_max, squash), unless None,
+    picks the _gaussian_state entry (whose W3 and b3 are the interleaved head) in place of log_std."""
     suffix = ("" if nvec is None else "_multidiscrete") + ("" if mask is None else "_masked") + \
         ("" if values is None else "_value") + ("_pushed" if pushed else "")
     grouped = () if nvec is None else (L.arr(ctypes.c_int32, nvec), len(nvec))
     masked = () if mask is None else (mask,)
     valued = () if values is None else (ptr(values),)
+    if output == "gaussian" and std is not None:
+        return "ktb_mlp_bf16_policy_gaussian_state" + suffix, (*std, seed, row_base, ptr(actions), ptr(log_probs),
+                                                               *valued)
     if output == "gaussian":
         return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs),
                                                          *valued)
@@ -205,6 +264,14 @@ def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, push
         return "ktb_mlp_bf16_policy_sample" + suffix, (*grouped, *masked, seed, row_base, ptr(actions), ptr(log_probs),
                                                        *valued)
     return "ktb_mlp_bf16_policy" + suffix, (*grouped, *masked, ptr(logits), ptr(actions))
+
+
+def _std(log_std, log_std_bounds, squash):
+    """The (log_std_min, log_std_max, squash) arguments of a _gaussian_state entry, or None for any other log_std."""
+    if not isinstance(log_std, (tuple, list)):
+        return None
+    lo, hi = LOG_STD_BOUNDS if log_std_bounds is None else log_std_bounds
+    return float(lo), float(hi), int(bool(squash))
 
 
 def _rows(bufs, b, e):
@@ -230,7 +297,9 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 actions: Optional[torch.Tensor] = None, seed: Optional[int] = None, row_offset: int = 0,
                 log_probs: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
                 mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
-                values: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None, _stacked: bool = False):
+                values: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
+                log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
+                _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -253,8 +322,16 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     = n_0 + ... + n_{g-1}, actions are int64 [M, G] of group-relative indices (the greedy or sampled action of each
     group's logits alone, with the noise of "sample"), and log_probs[i] is the fp32 sum of the groups'
     log_softmax(group)[a_g] in group order; a group with no legal action takes action 0 with a NaN log-probability.
-    The logits of "both" and nvec = (d_out,) keep the bits of the call without nvec.  `_stacked` (internal, from
-    mlp_scatter_gather, which checked the call): w3 and biases[2] are already the stacked W3v and b3v."""
+    The logits of "both" and nvec = (d_out,) keep the bits of the call without nvec.  With output="gaussian",
+    `log_std` = (w_ls, b_ls) makes the log-std state-dependent (SAC's actor): w_ls a bf16 [d_out, d_hidden] and b_ls a
+    bf16 [d_out] (given exactly when b3 is), so ls = F.linear(h, w_ls, b_ls).float() clamped to `log_std_bounds`
+    (default (-20.0, 2.0); a NaN stays NaN), u = logits + exp(ls)·normal_noise(seed, row_offset, M, d_out), actions
+    are tanh(u) with `squash=True` and u otherwise, and log_probs the Normal log-density of u minus, when squashed,
+    sum_j log(1 - tanh(u_j)^2), taken exactly as 2·(log 2 - |u| - softplus(-2|u|)) (not SB3's
+    log(1 - tanh^2 + 1e-6), which differs where |u| > about 7).  The head then runs over the interleaved rows of w3 and
+    w_ls (_stacked_head), at most 128 actions (127 with a value head).  log_std_bounds and squash are refused with a
+    tensor log_std.  `_stacked` (internal, from mlp_scatter_gather, which checked the call): w3 and biases[2] are
+    already the head the C entry takes (stacked with a value head, interleaved with a log-std head)."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -264,26 +341,27 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
+    if not _stacked:
+        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash)
+    std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
+    valued = value is not None or (_stacked and values is not None)
     if _stacked:
-        d_out -= 1
-    else:
-        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec)
+        d_out = (d_out - valued) // (2 if std is not None else 1)
     if output in ("sample", "gaussian") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
-    valued = _stacked or value is not None
     out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued,
                                                nvec)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
-    if value is not None:
+    if not _stacked and (value is not None or std is not None):
         with torch.cuda.stream(s):   # a rewrite of the stacked head is ordered after earlier calls on s
-            w3, b3 = _stacked_head(w3, biases[2], *value)
+            w3, b3 = _stacked_head(w3, biases[2], *(value or (None, None)), *(log_std if std is not None else ()))
         biases = (biases[0], biases[1], b3)
     if staged is None:
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
-                        mask=None if mask is None else ptr(mask), values=values, nvec=nvec)
+                        mask=None if mask is None else ptr(mask), values=values, nvec=nvec, std=std)
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
@@ -315,7 +393,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
-                               seed=None, log_std=None, mask=None, values_root=None, nvec=None) -> None:
+                               seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -326,10 +404,12 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     place in obs_root).  A legal-action `mask` [M, d_out] on the root travels with its rows: the copy engines push each
     rank's mask rows into the same staging half, 256-byte aligned after the largest shard's observation rows, so no
     rank reads the root's memory.  With `values_root` (fp32 [M]) weights[dev] holds the stacked W3v and b3v in place of
-    w3 and b3, and each rank stores its values there too.  `nvec` picks every rank's multi-discrete entry."""
+    w3 and b3, and each rank stores its values there too.  `nvec` picks every rank's multi-discrete entry.  `std`
+    (_std) picks every rank's _gaussian_state entry, weights[dev] then holding the interleaved head."""
     root, n, key = devs[0], len(devs), tuple(devs)
     valued = values_root is not None
-    d_in, d_hidden, d_out = obs_root.shape[1], weights[root][0].shape[0], weights[root][2].shape[0] - valued
+    d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
+    d_out = (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
     rows = max(e - b for b, e in bounds)
     mask_offset = (rows * d_in * 2 + 255) // 256 * 256
     stage_bytes = rows * d_in * 2 if mask is None else mask_offset + rows * d_out
@@ -355,7 +435,8 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=logits, device=root, stream=sess.fork(), staged=False,
                     biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
                     log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0],
-                    values=values, nvec=nvec, _stacked=valued)
+                    values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
+                    squash=None if std is None else bool(std[2]), _stacked=valued or std is not None)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
     if mask is None:
@@ -372,7 +453,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         logits, actions, log_probs, values = _rows(bufs, b, e)
         entry, head = _head(output, logits, actions, log_probs, seed, b,
                             None if log_std is None else log_std[devs[r]], ptr, pushed=True,
-                            mask=None if mask is None else mask_offset, values=values, nvec=nvec)
+                            mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std)
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -387,7 +468,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        actions_root: Optional[torch.Tensor] = None, seed: Optional[int] = None,
                        log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
                        mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
-                       values_root: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None) -> list:
+                       values_root: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
+                       log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -398,19 +480,22 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     `value` as in mlp_forward; the mask lives on the root GPU and each rank applies its rows of it (read in place by
     the pull form, pushed with the rows by the push form); the head with the value head stacked under it is built on
     the root and copied to the other devices like the other weights, and every rank stores its values into
-    `values_root` (allocated on the root when None).  `nvec` as in mlp_forward: actions are [rows, G] views."""
+    `values_root` (allocated on the root when None).  `nvec` as in mlp_forward: actions are [rows, G] views.
+    A state-dependent log_std = (w_ls, b_ls), with `log_std_bounds` and `squash`, as in mlp_forward: the interleaved
+    head is built on the root and copied to the other devices like the other weights."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     valued = value is not None
     bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
                     valued, nvec)
-    if valued:
-        w3, b3 = _stacked_head(w3, biases[2], *value)
+    std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
+    if valued or std is not None:
+        w3, b3 = _stacked_head(w3, biases[2], *(value or (None, None)), *(log_std if std is not None else ()))
         biases = (biases[0], biases[1], b3)
     root_stream = torch.cuda.current_stream(root)
     ready = torch.cuda.Event()
@@ -418,7 +503,10 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     bounds = [ops.shard_bounds(M, len(devs), r) for r in range(len(devs))]
     views = [_result(output, *_rows(bufs, b, e)) for b, e in bounds]
     weights = {dev: _weights_on(dev, (w1, w2, w3)) + _weights_on(dev, biases) for dev in set(devs)}
-    log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
+    if std is not None:   # the pair only marks the form on each rank: its rows are in the interleaved head
+        log_stds = {dev: log_std for dev in set(devs)}
+    else:
+        log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
     distinct = len(set(devs)) == len(devs) and len(devs) > 1
     pushable = distinct and all((e - b) % 128 == 0 for b, e in bounds) and \
         -(-max(e - b for b, e in bounds) // PUSH_CHUNK_ROWS) <= 64
@@ -428,7 +516,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec)
+                                   nvec, std)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -451,7 +539,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
             mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=st, biases=ws[3:],
                         output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
                         log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e],
-                        values=values, nvec=nvec, _stacked=valued)
+                        values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
+                        squash=None if std is None else bool(std[2]), _stacked=valued or std is not None)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

@@ -88,15 +88,20 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     (with ``mask=`` and ``value=`` as those allow): a tuple of ints ``(n_0, ..., n_{G-1})`` summing to d_out, a
     constant of the deployment, for a ``MultiDiscrete(nvec)`` action space.  The logits split into G groups of
     columns, one categorical each: actions become int64 ``[rows, G]`` of group-relative indices (greedy, or sampled
-    per group with the same noise), and log_probs the fp32 sum of the groups' log-probabilities in group order."""
+    per group with the same noise), and log_probs the fp32 sum of the groups' log-probabilities in group order.
+    ``log_std`` may instead name two call arguments ``(w_ls, b_ls)`` (with ``bias=True``): a state-dependent log-std
+    head ``nn.Linear(d_hidden, d_out)`` on the same trunk, clamped to ``log_std_bounds`` (two numbers, default
+    ``(-20.0, 2.0)``), with ``squash=True`` for tanh-squashed actions and the log-probability's tanh correction (SAC's
+    actor); ``value=`` may go beside it.  ``log_std_bounds`` and ``squash`` are options of that form only."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec")):
+    if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
+                                "squash")):
         if op != "mlp":
-            raise ValueError(f"bias=, output=, seed=, log_std=, mask=, value= and nvec= are options of the 'mlp' op, "
-                             f"not of '{op}'")
+            raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value= and nvec= are "
+                             f"options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
@@ -111,8 +116,30 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
         gaussian = extra.get("output") == "gaussian"
         if gaussian != ("log_std" in extra):
             raise ValueError('log_std= is required with output="gaussian" and is an option of that output only')
-        if gaussian and not isinstance(extra["log_std"], str):
+        state = gaussian and isinstance(extra["log_std"], (tuple, list))
+        if state:
+            ls = extra["log_std"]
+            if len(ls) != 2 or not all(isinstance(n, str) for n in ls):
+                raise ValueError(f"log_std must name one call argument or two (w_ls, b_ls), got {ls!r}")
+            if not extra.get("bias", False):
+                raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when "
+                                 "b3 is")
+        elif gaussian and not isinstance(extra["log_std"], str):
             raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
+        if not state and ("log_std_bounds" in extra or "squash" in extra):
+            raise ValueError("log_std_bounds= and squash= are options of a state-dependent log_std=(w_ls, b_ls) only")
+        if "log_std_bounds" in extra:
+            lb = extra["log_std_bounds"]
+            if not isinstance(lb, (tuple, list)) or len(lb) != 2 or \
+                    not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in lb):
+                raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {lb!r}")
+            if lb[0] != lb[0] or lb[1] != lb[1]:
+                raise ValueError(f"log_std_bounds must not be NaN, got {lb!r}")
+            if lb[0] > lb[1]:
+                raise ValueError(f"log_std_bounds must have low <= high, got {lb!r}")
+            extra["log_std_bounds"] = (float(lb[0]), float(lb[1]))
+        if "squash" in extra and not isinstance(extra["squash"], bool):
+            raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
         if "mask" in extra:
             if gaussian:
                 raise ValueError('mask= is an option of the categorical outputs, not of output="gaussian"')

@@ -578,10 +578,11 @@ class B200Supervisor:
                 raise TypeError(f"mapped mlp callable: seed argument '{seed}' not found in the call")
             seed = bound[seed]
         log_std = spec.extra.get("log_std")
-        if log_std is not None:   # always the name of a call argument, resolved per call
-            if log_std not in bound:
-                raise TypeError(f"mapped mlp callable: log_std argument '{log_std}' not found in the call")
-            log_std = bound[log_std]
+        if log_std is not None:   # the name of a call argument, or the names (w_ls, b_ls) of two, resolved per call
+            for name in (log_std,) if isinstance(log_std, str) else log_std:
+                if name not in bound:
+                    raise TypeError(f"mapped mlp callable: log_std argument '{name}' not found in the call")
+            log_std = bound[log_std] if isinstance(log_std, str) else tuple(bound[name] for name in log_std)
         mask = spec.extra.get("mask")
         if mask is not None:   # always the name of a call argument, resolved per call
             if mask not in bound:
@@ -596,7 +597,9 @@ class B200Supervisor:
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
-                                         value=value, nvec=spec.extra.get("nvec"))
+                                         value=value, nvec=spec.extra.get("nvec"),
+                                         log_std_bounds=spec.extra.get("log_std_bounds"),
+                                         squash=spec.extra.get("squash"))
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -25,6 +25,11 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      single-categorical call of the same d_out and output; and the eager arm, what a user pays without the grouped
      head: the logits entry (masked in torch under a mask), then split, Gumbel noise, argmax and log_softmax in torch.
      (2,)*128 shows the cost of 128 per-group quad reductions.
+  l  state-dependent Gaussian heads (log_std=(w_ls, b_ls), SAC's actor), d_out 6, 17, 64 and 128, unsquashed and
+     squashed (squash=True), each beside output="gaussian" at the same d_out; and the eager arm, what a user pays
+     without the fused head: the logits entry over the stacked head [w3; w_ls], then clamp, exp, noise, tanh and the
+     log-density in torch.  The interleaved head doubles the head's columns: d_out 64 runs in the 128-wide tile and 128
+     in the 256-wide one.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -36,7 +41,10 @@ unmasked call's, and the values are within rtol 2^-7, atol 1e-2 of the eager cri
 greedy actions equal the per-group argmax of the kernel's (masked) logits on every row; the sampled actions equal the
 eager arm's on at least 99.9 % of the rows (its noise comes from torch's log, not the kernel's logf), its
 log-probabilities within 2^-16·(1 + |ref|) on those rows, and every masked sample in a group with a legal action is
-legal.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+legal.  State-dependent rows: on 2048 consecutive rows, the unsquashed actions are within 2^-19·σ·(1 + |z|) +
+2^-23·|μ| of μ + σ·z (μ and ℓ the kernel's logits over the interleaved head, σ = exp(clamp(ℓ))), the squashed actions
+within 2 ulp of tanh of the unsquashed ones, and on every row both the actions and log-probabilities are within rtol
+1e-4, atol 1e-4 of the eager arm's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -54,9 +62,10 @@ import torch.nn.functional as F  # noqa: E402
 from kubetorch_b200.device import lib as L  # noqa: E402
 from kubetorch_b200.device import mlp  # noqa: E402
 from kubetorch_b200.device import ops  # noqa: E402
-from kubetorch_b200.sampling import gumbel_noise, gumbel_uniform  # noqa: E402
+from kubetorch_b200.sampling import gumbel_noise, gumbel_uniform, normal_noise  # noqa: E402
 
 HALF_LOG_2PI = 0.9189385332046727
+LN2 = 0.6931471805599453
 
 SEED = 0x5EED
 
@@ -209,6 +218,40 @@ def main():
                     obs, w1, w2, heads[d][0], biases=bs, nvec=nvec, **kw, **m))
                 variants[f"k_bias_{tag}{out}_eager_d{d}"] = (d, lambda d=d, mask=mask, out=out: eager_groups(
                     d, mask, out == "sample"))
+    gl = torch.Generator(device="cuda:0").manual_seed(10)   # its own generator again
+    state_widths = (6, 17, 64, 128)
+    for d in state_widths:
+        if d not in heads:
+            heads[d] = ((torch.randn(d, d_hidden, device="cuda:0", generator=gl) * 0.02).bfloat16(),
+                        (torch.randn(d, device="cuda:0", generator=gl) * 0.1).bfloat16())
+        log_stds.setdefault(d, torch.linspace(-2.0, 0.5, d, device="cuda:0"))
+    ls_heads = {d: ((torch.randn(d, d_hidden, device="cuda:0", generator=gl) * 0.02).bfloat16(),
+                    torch.linspace(-2.0, 0.5, d, device="cuda:0").bfloat16()) for d in state_widths}
+    stacked_ls = {d: (torch.cat((heads[d][0], ls_heads[d][0])), torch.cat((heads[d][1], ls_heads[d][1])))
+                  for d in state_widths}
+
+    def eager_state(d, squash):
+        """The logits entry over [w3; w_ls], then the state-dependent head in torch: what a user pays without it."""
+        y = mlp.mlp_forward(obs, w1, w2, stacked_ls[d][0], biases=(b1, b2, stacked_ls[d][1])).float()
+        mu, ls = y[:, :d], y[:, d:].clamp(-20.0, 2.0)
+        z = normal_noise(SEED, 0, M, d, device="cuda:0")
+        u = mu + torch.exp(ls) * z
+        lp = (-0.5 * z * z - ls - HALF_LOG_2PI).sum(-1)
+        if not squash:
+            return u, lp
+        au = u.abs()
+        return torch.tanh(u), lp - (2 * (LN2 - au - torch.log1p(torch.exp(-2 * au)))).sum(-1)
+
+    for d in state_widths:
+        bs = (b1, b2, heads[d][1])
+        variants[f"l_bias_gaussian_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, output="gaussian", seed=SEED, log_std=log_stds[d]))
+        for squash in (False, True):
+            tag = "squashed" if squash else "unsquashed"
+            variants[f"l_bias_state_{tag}_d{d}"] = (d, lambda d=d, bs=bs, squash=squash: mlp.mlp_forward(
+                obs, w1, w2, heads[d][0], biases=bs, output="gaussian", seed=SEED, log_std=ls_heads[d],
+                squash=squash))
+            variants[f"l_bias_state_{tag}_eager_d{d}"] = (d, lambda d=d, squash=squash: eager_state(d, squash))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -341,6 +384,28 @@ def main():
                 entry["masked_samples_legal_all_rows"] = "ok"
             del acts, lp, want_a, want_lp
         parity[f"k_bias_nvec_d{d}"] = entry
+
+    for d in state_widths:
+        entry = {}
+        w3s, b3s = mlp._stacked_head(heads[d][0], heads[d][1], None, None, *ls_heads[d])
+        y = mlp.mlp_forward(obs[r0:r0 + 2048], w1, w2, w3s, biases=(b1, b2, b3s)).double()
+        mu, sigma = y[:, 0::2], y[:, 1::2].clamp(-20.0, 2.0).exp()
+        z = torch.special.ndtri(gumbel_uniform(SEED, r0, 2048, d, device="cuda:0", word3=1).double())
+        u, lp = variants[f"l_bias_state_unsquashed_d{d}"][1]()
+        a, lp_sq = variants[f"l_bias_state_squashed_d{d}"][1]()
+        err = (u[r0:r0 + 2048].double() - (mu + sigma * z)).abs()
+        assert bool((err <= 2.0 ** -19 * sigma * (1 + z.abs()) + 2.0 ** -23 * mu.abs()).all()), d
+        t = torch.tanh(u[r0:r0 + 2048].double())
+        assert bool(((a[r0:r0 + 2048].double() - t).abs() <= 2.0 ** -22 * t.abs() + 2.0 ** -126).all()), d
+        entry["state_bars_2048_rows"] = "ok"
+        for tag, got in (("unsquashed", (u, lp)), ("squashed", (a, lp_sq))):
+            want = variants[f"l_bias_state_{tag}_eager_d{d}"][1]()
+            for g_, w_ in zip(got, want):
+                torch.testing.assert_close(g_, w_, rtol=1e-4, atol=1e-4)
+            entry[f"{tag}_vs_eager_all_rows"] = "ok"
+            del want
+        parity[f"l_bias_state_d{d}"] = entry
+        del u, lp, a, lp_sq
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
