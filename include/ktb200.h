@@ -241,6 +241,19 @@ int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elem
                                size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
                                const void* mask_root, size_t row_bytes, size_t mask_offset, unsigned long long seq,
                                uintptr_t stream);
+/* ktb_push_scatter_ce with n_sides (1 or 2) per-row side sources, for the masked and epsilon-greedy MLP heads (the
+ * legal-action mask and the per-row epsilon): row i of obs has side_row_bytes[k] bytes at side_src[k] +
+ * i*side_row_bytes[k], copied chunk by chunk, after the same wait for ack[r] >= seq-2, to stage_peer[r] +
+ * (seq&1)*stage_stride + side_offset[k] + (the chunk's first row in the shard)*side_row_bytes[k]; ready[c] is
+ * published behind every copy of chunk c.  ktb_push_scatter_ce_masked is its one-side case.  After every check of
+ * ktb_push_scatter_ce, in its order: n_sides outside [1, 2] or a NULL array; then per side in order a NULL source with
+ * n_elems > 0, side_row_bytes == 0 or chunk_elems not a multiple of granule, and for a served rank a side that
+ * overlaps its shard's rows, ends past stage_stride, or overlaps an earlier side, are KTB_ERR_ARG. */
+int ktb_push_scatter_ce_sides(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
+                              int n_ranks, int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
+                              void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, int n_sides,
+                              const void* const* side_src, const size_t* side_row_bytes, const size_t* side_offset,
+                              unsigned long long seq, uintptr_t stream);
 /* RANK side: for each piece, spin in-kernel until ready[chunk] >= seq, then
  * dst_root_shard[piece] = op(stage_local[piece]) (peer stores into the root's result arena); after the
  * last piece publish ack[rank] = seq in the root's control block (ctrl_root_peer). */
@@ -647,6 +660,62 @@ int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed(
     const int32_t* nvec, int n_groups, size_t mask_offset, uint64_t seed, uint64_t row_base, int64_t* actions,
     float* log_probs, float* values, void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
     size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
+/* Epsilon-greedy forms: the actor of a Q-network (DQN, Ape-X, R2D2), whose head outputs one Q-value per action.  Each
+ * takes ktb_mlp_bf16_policy's arguments up to b3, then (masked forms) the legal-action mask, then
+ * (const float* epsilon, uint64_t seed, uint64_t row_base, int64_t* actions, float* q, float* q_max), then scratch,
+ * stage (NULL: the plain form) and stream.  For the call's global row i (row_base + the row's index in this call), head
+ * column j < d_out and key = (seed mod 2^32, seed >> 32):
+ *   - q_ij is the bf16-rounded head output (ktb_mlp_bf16_policy's logits); masked: q.masked_fill(~legal, -inf) as the
+ *     _masked entries compute it.
+ *   - The greedy action g_i is torch.argmax(q_i): ties to the lowest column, the first NaN wins, -0.0 == +0.0, and a
+ *     row whose ranked values are all -inf, or that has no legal column, gets 0.
+ *   - The coin: x = word 0 of Philox4x32-10((i mod 2^32, i >> 32, 0, 3), key), u_i = (2*(x >> 9) + 1)*2^-24; row i
+ *     explores iff u_i < epsilon[i] as an fp32 compare, so epsilon <= 0 and a NaN epsilon never explore, epsilon >= 1
+ *     always does, and P(explore) is the count of the 2^23 grid points below epsilon over 2^23.
+ *   - The exploratory action e_i: w_ij = word j & 1 of counter (i mod 2^32, i >> 32, j >> 1, 2) as a uint32; e_i is
+ *     the legal column with the largest w_ij, ties to the lowest column, 0 when the row has no legal column.  It is
+ *     uniform over the legal columns (ties have probability below d^2*2^-33) and reads no Q-value, so NaN or +-inf
+ *     Q-values do not change it.  Counter word 3 = 2 (exploration) and 3 (coin) never reuse the Gumbel (0) or
+ *     Gaussian (1) uniforms of the same seed.  Only an exploring row draws words: one Philox call per column pair.
+ *   - actions[i] = explore ? e_i : g_i (int64); q[i] = fp32(q_i[actions[i]]), the masked Q-value of the action taken
+ *     widened exactly (-inf for column 0 of a row with no legal column); q_max[i] = fp32(q_i[g_i]), NaN when a legal
+ *     column holds a NaN.  No logits are written: 16 B per row.
+ *   - The draws depend on (seed, i, j) only: every chunk size, form, rank count and row_base split gives the same bits.
+ *   - epsilon, actions, q and q_max may be peer pointers in the plain and staged forms.
+ *   - Checks: every check of the greedy counterpart (ktb_mlp_bf16_policy or _masked) first, in its order (d_out > 256
+ *     is KTB_ERR_UNSUPPORTED), then, with M > 0: a NULL or misaligned (4 bytes; actions 8) epsilon, actions, q or q_max
+ *     is KTB_ERR_ARG.  Writes stay inside actions[M], q[M], q_max[M], scratch and stage. */
+int ktb_mlp_bf16_policy_epsilon_greedy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                       const void* b3, const float* epsilon, uint64_t seed, uint64_t row_base,
+                                       int64_t* actions, float* q, float* q_max, void* scratch, void* stage,
+                                       uintptr_t stream);
+int ktb_mlp_bf16_policy_epsilon_greedy_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                              const void* W1, const void* b1, const void* W2, const void* b2,
+                                              const void* W3, const void* b3, const uint8_t* mask,
+                                              const float* epsilon, uint64_t seed, uint64_t row_base,
+                                              int64_t* actions, float* q, float* q_max, void* scratch, void* stage,
+                                              uintptr_t stream);
+/* Push-fed epsilon-greedy forms: the _pushed entries' arguments with (mask_offset,) epsilon_offset after b3 in place of
+ * the pointers.  The rank reads its rows' epsilon (fp32, M*4 bytes) and mask from its own staging half, at
+ * stage_local + (seq & 1)*stage_stride + the offset (ktb_push_scatter_ce_sides puts them there), never from a peer.
+ * After the counterpart's checks: an epsilon region that overlaps the rows (epsilon_offset < M*d_in*2) or the mask
+ * region, that ends past stage_stride, or whose offset is not a multiple of 4, is KTB_ERR_ARG; then the output checks
+ * above.  An empty shard (M == 0) may pass NULL outputs and still publishes its ack. */
+int ktb_mlp_bf16_policy_epsilon_greedy_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                              int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                              const void* b2, const void* W3, const void* b3, size_t epsilon_offset,
+                                              uint64_t seed, uint64_t row_base, int64_t* actions, float* q,
+                                              float* q_max, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                              int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                     int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                     const void* W2, const void* b2, const void* W3, const void* b3,
+                                                     size_t mask_offset, size_t epsilon_offset, uint64_t seed,
+                                                     uint64_t row_base, int64_t* actions, float* q, float* q_max,
+                                                     void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                                     size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
 #ifdef __cplusplus
 }

@@ -429,6 +429,19 @@ struct HeadStd {
   bool squash = false;
 };
 
+// The per-row inputs and outputs of an ε-greedy kSample head, the layer kernel's last parameter (by value, like
+// HeadStd, and for the same reason: a larger HeadOut re-schedules the other instantiations).  epsilon != null marks
+// the head: ε [rows] in, q [rows] and q_max [rows] out beside HeadOut::actions (epsilon_pass).
+struct HeadEps {
+  const float* epsilon = nullptr;
+  float* q = nullptr;
+  float* q_max = nullptr;
+
+  HeadEps from_row(size_t r0) const {
+    return epsilon ? HeadEps{epsilon + r0, q + r0, q_max + r0} : *this;
+  }
+};
+
 // The end of the group that begins at column lo: the next set bit of `starts` past lo, or d.  The words are indexed
 // at compile time, so the bitmap stays in the kernel's parameters.
 __device__ __forceinline__ int group_end(const uint32_t (&starts)[8], int lo, int d) {
@@ -572,6 +585,107 @@ __device__ __forceinline__ void group_pass(Slot slot, const ColBits<BLOCK_N> (&l
   }
 }
 
+// The ε-greedy pass of sample_epilogue (epsilon != null) over the bf16 pairs that its pass 1 parked in the ring: a
+// Q-network's actor.  For each of the thread's rows r = row + 8h (global row i = row_base + r):
+//   * the greedy action g: torch.argmax of the live columns (argmax_before; 0 when their values are all -inf or there
+//     are none), ranked in the greedy epilogue's per-thread and quad order;
+//   * the coin: u = (2·(x >> 9) + 1)·2^-24 of word 0 of Philox counter (i, 0, 3), drawn once per row by lane h of the
+//     quad's pair (lanes 0, 2 draw row's, lanes 1, 3 row + 8's) and shared by shfl.xor; the row explores iff
+//     u < epsilon[r] in fp32 (so ε <= 0 and a NaN ε never explore);
+//   * an exploring row, and only such a row, draws Philox word c of counter (i, col >> 1, 2) for each pair (col,
+//     col + 1), and takes the live column with the largest word, ties to the lower column (0 when none is live).  The
+//     rank key is (word << 32) | ~col, so 0 means "no live column" and a larger key wins.
+// Lane 0 of the quad stores actions[r], q[r] = the masked Q-value of the action taken and q_max[r] = that of g, both
+// widened exactly from bf16 (an illegal column's is -inf).
+template <int BLOCK_N, typename Slot>
+__device__ __forceinline__ void epsilon_pass(Slot slot, const ColBits<BLOCK_N> (&live)[2], int d, int col0, int row,
+                                             bool st0, bool st1, const float* epsilon, int64_t* actions, float* q,
+                                             float* q_max, uint64_t seed, uint64_t row_base) {
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  float best[2] = {-INFINITY, -INFINITY};
+  int best_col[2] = {INT_MAX, INT_MAX};
+#pragma unroll 1
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= d) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const float v = c ? __high2float(y) : __low2float(y);
+        if (((live[h] >> (2 * j + c)) & 1) && argmax_before(v, col + c, best[h], best_col[h])) {
+          best[h] = v;
+          best_col[h] = col + c;
+        }
+      }
+    }
+  }
+  const int hc = threadIdx.x & 1;   // the row whose coin this lane draws
+  int mine = 0;
+  if (hc ? st1 : st0) {
+    const uint64_t i = row_base + (uint64_t)(row + 8 * hc);
+    const uint32_t x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), 0u, 3u), key).x;
+    mine = (float)(2u * (x >> 9) + 1u) * 5.9604644775390625e-8f < epsilon[row + 8 * hc];
+  }
+  const int other = __shfl_xor_sync(0xffffffffu, mine, 1);
+  const bool explore[2] = {(hc ? other : mine) != 0, (hc ? mine : other) != 0};
+  unsigned long long rank[2] = {0ull, 0ull};
+  float ey[2] = {-INFINITY, -INFINITY};
+  if (explore[0] || explore[1]) {
+#pragma unroll 1
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= d) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!explore[h]) continue;
+        const uint64_t i = row_base + (uint64_t)(row + 8 * h);
+        const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 2u), key);
+        const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const unsigned long long k = (unsigned long long)(c ? x.y : x.x) << 32 | (uint32_t)~(col + c);
+          if (((live[h] >> (2 * j + c)) & 1) && k > rank[h]) {
+            rank[h] = k;
+            ey[h] = c ? __high2float(y) : __low2float(y);
+          }
+        }
+      }
+    }
+  }
+  // the 4 lanes of a quad hold the columns of the same two rows
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
+      const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
+      if (argmax_before(ov, oc, best[h], best_col[h])) {
+        best[h] = ov;
+        best_col[h] = oc;
+      }
+      const unsigned long long ok = __shfl_xor_sync(0xffffffffu, rank[h], m);
+      const float oy = __shfl_xor_sync(0xffffffffu, ey[h], m);
+      if (ok > rank[h]) {
+        rank[h] = ok;
+        ey[h] = oy;
+      }
+    }
+  }
+  if ((threadIdx.x & 3) == 0) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!(h ? st1 : st0)) continue;
+      const int g = best[h] == -INFINITY ? 0 : best_col[h];
+      const int e = rank[h] == 0 ? 0 : (int)~(uint32_t)rank[h];
+      actions[row + 8 * h] = explore[h] ? e : g;
+      q[row + 8 * h] = explore[h] ? ey[h] : best[h];
+      q_max[row + 8 * h] = best[h];
+    }
+  }
+}
+
 // The sampling epilogue of a head tile (HeadKind::kSample): rows r = row and row + 8 of the thread, global rows
 // row_base + r.  Pass 1 (unrolled over the accumulators) rounds the logits once, parks them as bf16 pairs in the TMA
 // ring as gaussian_epilogue does, and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum
@@ -588,13 +702,14 @@ __device__ __forceinline__ void group_pass(Slot slot, const ColBits<BLOCK_N> (&l
 // With a value head (values != null) the tile holds n_valid = d + 1 columns: the policy's d, then the value column d.
 // Pass 1 parks column d with the rest; everything ranked, drawn, summed or masked stops at d; store_values reads it.
 // A multi-discrete head (groups.n > 0) takes group_pass in place of the rolled pass: the greedy one as well, whose
-// logits (C, unless null) it also stores.  The single categorical's rolled pass stays as it is.
+// logits (C, unless null) it also stores.  An ε-greedy head (epsilon != null) takes epsilon_pass in its place.  The
+// single categorical's rolled pass stays as it is.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                 int n_valid, int row, bool st0, bool st1, int64_t* actions,
                                                 float* log_probs, const uint8_t* mask, uint64_t seed,
                                                 uint64_t row_base, float* values, const HeadGroups& groups,
-                                                __nv_bfloat16* C) {
+                                                __nv_bfloat16* C, const float* epsilon, float* q, float* q_max) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -632,6 +747,10 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   if (groups.n > 0) {
     group_pass<BLOCK_N>(slot, live, groups, d, col0, row, st0, st1, C, actions, log_probs, seed, row_base);
     store_values(slot, d, row, st0, st1, values);
+    return;
+  }
+  if (epsilon != nullptr) {
+    epsilon_pass<BLOCK_N>(slot, live, d, col0, row, st0, st1, epsilon, actions, q, q_max, seed, row_base);
     return;
   }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
@@ -802,7 +921,8 @@ enum class HeadKind {
   kHidden,     // bf16 relu(A · Bᵀ + bias) of full tiles (layers 1 and 2)
   kGreedy,     // bf16 logits and/or int64 argmax actions (unrolled; the single categorical)
   kSample,     // the rolled categorical head: Gumbel-max int64 actions and fp32 log_probs, or with groups (HeadGroups)
-               // greedy or Gumbel-max actions per group, with the logits of "both" or the summed log_probs
+               // greedy or Gumbel-max actions per group, with the logits of "both" or the summed log_probs, or with
+               // epsilon ε-greedy actions and their fp32 Q-values
   kGaussian,   // fp32 actions [rows, d_out] (gauss_actions) drawn with log_std, and fp32 log_probs
 };
 
@@ -854,7 +974,9 @@ struct HeadOut {
 //     a value head's column is 2·d_out;
 //   kSample and kGaussian with out.values: n_valid = d_out + 1, and values[row] = fp32(column d_out) (store_values);
 //   kSample with out.groups: one greedy or sampled action per group of columns into actions[row, g], the summed
-//     log-probability of the sampled ones, and the logits of a greedy head that stores them (group_pass).
+//     log-probability of the sampled ones, and the logits of a greedy head that stores them (group_pass);
+//   kSample with eg.epsilon: the ε-greedy action of each row with the Q-values of the taken and the greedy action
+//     (epsilon_pass).
 // A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
 // (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
 // never an action.
@@ -864,7 +986,7 @@ template <int BLOCK_N, int STAGES, HeadKind KIND>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                            const __nv_bfloat16* bias, const HeadOut out, int n_valid, int K, int rows,
-                           const HeadStd sd) {
+                           const HeadStd sd, const HeadEps eg) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -884,7 +1006,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, out.mask, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
-                             out.row_base, out.values, out.groups, C);
+                             out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
                                        out.log_probs, out.seed, out.row_base, out.values, sd);
@@ -973,7 +1095,7 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
 // One layer through the epilogue of KIND in BLOCK_N-wide tiles: out = A[M, K] · B[N, K]ᵀ (+ bias), N columns.
 template <int BLOCK_N, HeadKind KIND>
 static int launch_layer(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                        int K, cudaStream_t stream, const HeadStd& sd = HeadStd{}) {
+                        int K, cudaStream_t stream, const HeadStd& sd = HeadStd{}, const HeadEps& eg = HeadEps{}) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -986,7 +1108,8 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
-  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M, sd);
+  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M, sd,
+                                                eg);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
@@ -995,9 +1118,9 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
 // head, one more with a value head).
 template <HeadKind KIND>
 static int launch_head(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                       int K, cudaStream_t stream, const HeadStd& sd) {
+                       int K, cudaStream_t stream, const HeadStd& sd, const HeadEps& eg) {
   const auto launch = N <= 64 ? launch_layer<64, KIND> : N <= 128 ? launch_layer<128, KIND> : launch_layer<256, KIND>;
-  return launch(dev, A, B, bias, out, M, N, K, stream, sd);
+  return launch(dev, A, B, bias, out, M, N, K, stream, sd, eg);
 }
 
 // Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
@@ -1007,7 +1130,9 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // d_hidden] / b3v [d_out + 1] of the policy and its value head, and out.values receives the value of each row.
 // `nvec` (n_groups entries, a host array) marks the _multidiscrete entries: mlp_run checks it and builds out.groups.
 // std.state marks the _gaussian_state entries: W3 / b3 are the interleaved W3s [2·d_out, d_hidden] / b3s (with a
-// value head W3sv / b3sv, one more row), log_std is null, and mlp_run checks the bounds.
+// value head W3sv / b3sv, one more row), log_std is null, and mlp_run checks the bounds.  `eps` marks the
+// _epsilon_greedy entries: eg.epsilon (the pull forms) or the bytes at MlpFeed::epsilon_offset of the call's staging
+// half (the pushed forms) hold each row's ε, and out.actions, eg.q and eg.q_max receive the outputs.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1019,6 +1144,8 @@ struct MlpParams {
   int n_groups = 0;
   bool grouped = false;
   HeadStd std;
+  bool eps = false;
+  HeadEps eg;
 
   // A multi-discrete head: the greedy one (logits and/or actions, ranked without noise) or the sampled one, both in
   // the kSample instantiations.
@@ -1040,6 +1167,16 @@ struct MlpParams {
     return p;
   }
 
+  // An ε-greedy head, in the kSample instantiations: epsilon [M] in (null in the pushed forms), actions, q, q_max out.
+  static MlpParams epsilon_greedy(const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                  const void* b3, const float* epsilon, uint64_t seed, uint64_t row_base,
+                                  int64_t* actions, float* q, float* q_max) {
+    MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, actions, nullptr, seed, row_base}};
+    p.eg = HeadEps{epsilon, q, q_max};
+    p.eps = true;
+    return p;
+  }
+
   MlpParams with_mask(const uint8_t* mask) const {
     MlpParams p = *this;
     p.out.mask = mask;
@@ -1058,8 +1195,9 @@ struct MlpParams {
 // the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds its d_out
 // columns (2·d_out for a state-dependent Gaussian head), one more with a value head.  `consumed`, unless null, is
 // recorded once layer 1 has read a1.
-static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void* a1, void* h1, void* h2, size_t r0,
-                     size_t rows, int d_in, int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
+static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const HeadEps& eg, const void* a1, void* h1,
+                     void* h2, size_t r0, size_t rows, int d_in, int d_hidden, int d_out, cudaEvent_t consumed,
+                     cudaStream_t st) {
   int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
   if (rc) return rc;
   if (consumed) KTB_CK(cudaEventRecord(consumed, st));
@@ -1069,7 +1207,7 @@ static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const void
                     : p.kind == HeadKind::kSample ? launch_head<HeadKind::kSample>
                                                   : launch_head<HeadKind::kGaussian>;
   const int n = (p.std.state ? 2 * d_out : d_out) + (int)p.valued;
-  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std);
+  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std, eg.from_row(r0));
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -1091,7 +1229,7 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
       case HeadKind::kSample:
         if (o.groups.greedy)   // a greedy multi-discrete head takes what the greedy entries take
           KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
-        else
+        else if (!p.eps)   // an ε-greedy head's outputs are checked by mlp_run after every other check
           KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
@@ -1125,7 +1263,8 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //   pushed: the root pushes the rows into half seq & 1 of `in` (stage_local, halves `stride` bytes apart) and publishes
 //           ready[c] = seq in this rank's control block `ctrl`; layer 1 of chunk c waits in-stream for it, and the
 //           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A masked head reads
-//           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows).
+//           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows), and
+//           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in.
 // The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
@@ -1137,6 +1276,7 @@ struct MlpFeed {
   int rank = 0;
   unsigned long long seq = 0;
   size_t mask_offset = 0;
+  size_t epsilon_offset = 0;
 
   static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
   static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
@@ -1148,6 +1288,11 @@ struct MlpFeed {
     f.mask_offset = off;
     return f;
   }
+  MlpFeed with_epsilon_offset(size_t off) const {
+    MlpFeed f = *this;
+    f.epsilon_offset = off;
+    return f;
+  }
 };
 
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
@@ -1157,7 +1302,9 @@ struct MlpFeed {
 // d_out <= 255; skipped for an empty call) after every check of the entry without a value head.  A multi-discrete
 // entry's nvec (skipped for an empty call) is checked last, and read into the launch's HeadGroups before the call
 // returns.  A state-dependent Gaussian entry's head width (2·d_out, one more with a value head, <= 256) and log-std
-// bounds (skipped for an empty call) come after every check of its state-independent counterpart.
+// bounds (skipped for an empty call) come after every check of its state-independent counterpart.  An ε-greedy entry's
+// own checks come after every check of its greedy counterpart (ktb_mlp_bf16_policy or _masked): its ε region in the
+// pushed forms, then (skipped for an empty call) ε, actions, q and q_max non-null and aligned.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1194,6 +1341,22 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
                 "%s: mask_offset=%zu + M*d_out exceeds stage_stride", fn, f.mask_offset);
   } else if (p.masked) {
     KTB_REQUIRE(p.out.mask, KTB_ERR_ARG, "%s: null mask", fn);   // M > 0 here: an empty pull call has returned
+  }
+  if (p.eps && f.pushed) {
+    const size_t off = f.epsilon_offset, n = M * sizeof(float);
+    KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: epsilon_offset=%zu overlaps the rows", fn, off);
+    KTB_REQUIRE(!p.masked || off >= f.mask_offset + M * (size_t)d_out || off + n <= f.mask_offset, KTB_ERR_ARG,
+                "%s: epsilon_offset=%zu overlaps the mask", fn, off);
+    KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG,
+                "%s: epsilon_offset=%zu + 4*M exceeds stage_stride", fn, off);
+    KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: epsilon_offset=%zu must be a multiple of 4", fn, off);
+  }
+  if (p.eps && M > 0) {
+    const HeadEps& o = p.eg;
+    KTB_REQUIRE((o.epsilon || f.pushed) && p.out.actions && o.q && o.q_max, KTB_ERR_ARG,
+                "%s: epsilon, actions, q and q_max are required", fn);
+    KTB_REQUIRE((((uintptr_t)o.epsilon | (uintptr_t)o.q | (uintptr_t)o.q_max) & 3) == 0, KTB_ERR_ARG,
+                "%s: epsilon, q and q_max must be 4-byte aligned", fn);
   }
   if (p.valued && M > 0) {
     KTB_REQUIRE(p.out.values, KTB_ERR_ARG, "%s: null values", fn);
@@ -1236,6 +1399,9 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   HeadOut out = p.out;
   out.groups = groups;
   if (p.masked && f.pushed) out.mask = reinterpret_cast<const uint8_t*>(x) + f.mask_offset;
+  HeadEps eg = p.eg;
+  if (p.eps && f.pushed)
+    eg.epsilon = reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(x) + f.epsilon_offset);
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
   cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
@@ -1284,7 +1450,7 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       a1 = dstb;
     }
     // evs[3..4] are null unless staged
-    rc = mlp_chunk(dev, p, out, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
+    rc = mlp_chunk(dev, p, out, eg, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
     if (rc) return rc;
   }
   if (!f.pushed) return KTB_OK;
@@ -1732,6 +1898,57 @@ int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed(
   return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
                      .with_mask_offset(mask_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_epsilon_greedy(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                       const void* b3, const float* epsilon, uint64_t seed, uint64_t row_base,
+                                       int64_t* actions, float* q, float* q_max, void* scratch, void* stage,
+                                       uintptr_t stream) {
+  const MlpParams p = MlpParams::epsilon_greedy(W1, b1, W2, b2, W3, b3, epsilon, seed, row_base, actions, q, q_max);
+  return mlp_run("ktb_mlp_bf16_policy_epsilon_greedy", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_epsilon_greedy_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                              int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                              const void* b2, const void* W3, const void* b3, size_t epsilon_offset,
+                                              uint64_t seed, uint64_t row_base, int64_t* actions, float* q,
+                                              float* q_max, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                              int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::epsilon_greedy(W1, b1, W2, b2, W3, b3, nullptr, seed, row_base, actions, q, q_max);
+  return mlp_run("ktb_mlp_bf16_policy_epsilon_greedy_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_epsilon_offset(epsilon_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_epsilon_greedy_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                              const void* W1, const void* b1, const void* W2, const void* b2,
+                                              const void* W3, const void* b3, const uint8_t* mask,
+                                              const float* epsilon, uint64_t seed, uint64_t row_base,
+                                              int64_t* actions, float* q, float* q_max, void* scratch, void* stage,
+                                              uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::epsilon_greedy(W1, b1, W2, b2, W3, b3, epsilon, seed, row_base, actions, q, q_max).with_mask(mask);
+  return mlp_run("ktb_mlp_bf16_policy_epsilon_greedy_masked", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                     int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                     const void* W2, const void* b2, const void* W3, const void* b3,
+                                                     size_t mask_offset, size_t epsilon_offset, uint64_t seed,
+                                                     uint64_t row_base, int64_t* actions, float* q, float* q_max,
+                                                     void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                                     size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::epsilon_greedy(W1, b1, W2, b2, W3, b3, nullptr, seed, row_base, actions, q, q_max).with_mask(nullptr);
+  return mlp_run("ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset)
+                     .with_epsilon_offset(epsilon_offset),
                  scratch, stream);
 }
 

@@ -337,15 +337,23 @@ int ktb_push_scatter_chunked(int root_dev, const void* src_root, size_t n_elems,
 }
 
 // ---- copy-engine form of the root side: no SM of the root is used ------------------------------------------------
-// With `with_side`, a second source rides along: row i of the shard (granule elements) has row_bytes bytes at
-// side + i·row_bytes, and they land side_offset bytes into the rank's staging half, chunk by chunk beside the rows and
-// behind the same ack wait, with ready[c] published after both copies of chunk c.  Its checks come after every check
-// of the plain form.
+// A per-row source that rides along with the rows (the masked and ε-greedy MLP heads): row i of the shard (granule
+// elements) has row_bytes bytes at src + i·row_bytes, and they land `offset` bytes into the rank's staging half.
+// `name` names it in the errors.
+struct PushSide {
+  const void* src;
+  size_t row_bytes, offset;
+  const char* name;
+};
+
+// With n_sides (0 to 2; anything else, or null sides, is KTB_ERR_ARG) side sources, each rides along chunk by chunk
+// beside the rows and behind the same ack wait, with ready[c] published after every copy of chunk c.  Their checks come
+// after every check of the plain form: per side in order a null source, then row_bytes and whole-row chunks, then per
+// served rank the side's overlap with the rows, its end past stage_stride, and its overlap with an earlier side.
 static int push_scatter_ce_impl(const char* who, int root_dev, const void* src_root, size_t n_elems, size_t granule,
                                 int dtype, int n_ranks, int root_rank, const int* devs, void* const* stage_peer,
                                 size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
-                                bool with_side, const void* side, size_t row_bytes, size_t side_offset,
-                                unsigned long long seq, uintptr_t stream) {
+                                int n_sides, const PushSide* sides, unsigned long long seq, uintptr_t stream) {
   int rc = check_push_scatter(who, root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank, stage_peer,
                               stage_stride, ctrl_peer, ctrl_root, seq);
   if (rc) return rc;
@@ -353,18 +361,25 @@ static int push_scatter_ce_impl(const char* who, int root_dev, const void* src_r
   const int n_chunks = push_chunk_count(n_elems, granule, n_ranks, chunk_elems);
   KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: more than %d chunks", who, KTB_PUSH_MAX_CHUNKS);
   const size_t es = dtype_size(dtype);
-  if (with_side) {
-    KTB_REQUIRE(side || n_elems == 0, KTB_ERR_ARG, "%s: null mask", who);
-    KTB_REQUIRE(row_bytes > 0 && chunk_elems % granule == 0, KTB_ERR_ARG,
+  KTB_REQUIRE(n_sides >= 0 && n_sides <= 2 && (n_sides == 0 || sides), KTB_ERR_ARG,
+              "%s: 1 or 2 side sources, with non-null arrays", who);
+  for (int k = 0; k < n_sides; ++k) {
+    const PushSide& sd = sides[k];
+    KTB_REQUIRE(sd.src || n_elems == 0, KTB_ERR_ARG, "%s: null %s", who, sd.name);
+    KTB_REQUIRE(sd.row_bytes > 0 && chunk_elems % granule == 0, KTB_ERR_ARG,
                 "%s: row_bytes must be positive and chunk_elems whole rows", who);
     for (int r = 0; r < n_ranks; ++r) {
       if (r == root_rank || !stage_peer[r]) continue;
       size_t b = 0, e = 0;
       ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
-      KTB_REQUIRE(side_offset >= (e - b) * granule * es, KTB_ERR_ARG, "%s: mask_offset overlaps the rows of rank %d",
-                  who, r);
-      KTB_REQUIRE(side_offset <= stage_stride && (e - b) * row_bytes <= stage_stride - side_offset, KTB_ERR_ARG,
-                  "%s: mask of rank %d exceeds stage_stride", who, r);
+      KTB_REQUIRE(sd.offset >= (e - b) * granule * es, KTB_ERR_ARG, "%s: %s_offset overlaps the rows of rank %d", who,
+                  sd.name, r);
+      KTB_REQUIRE(sd.offset <= stage_stride && (e - b) * sd.row_bytes <= stage_stride - sd.offset, KTB_ERR_ARG,
+                  "%s: %s of rank %d exceeds stage_stride", who, sd.name, r);
+      for (int o = 0; o < k; ++o)
+        KTB_REQUIRE(sd.offset >= sides[o].offset + (e - b) * sides[o].row_bytes ||
+                        sd.offset + (e - b) * sd.row_bytes <= sides[o].offset,
+                    KTB_ERR_ARG, "%s: %s of rank %d overlaps %s", who, sd.name, r, sides[o].name);
     }
   }
   KTB_GUARD(root_dev);
@@ -407,11 +422,11 @@ static int push_scatter_ce_impl(const char* who, int root_dev, const void* src_r
       if (hi > lo)
         KTB_CK(cudaMemcpyPeerAsync(static_cast<uint8_t*>(stage_peer[r]) + buf_off + lo * es, devs[r],
                                    static_cast<const uint8_t*>(src_root) + (sb[r] + lo) * es, root_dev, (hi - lo) * es, cs));
-      if (hi > lo && side != nullptr)   // the same rows' second source, beside them
+      for (int k = 0; k < n_sides && hi > lo; ++k)   // the same rows' side sources, beside them
         KTB_CK(cudaMemcpyPeerAsync(
-            static_cast<uint8_t*>(stage_peer[r]) + buf_off + side_offset + lo / granule * row_bytes, devs[r],
-            static_cast<const uint8_t*>(side) + (sb[r] + lo) / granule * row_bytes, root_dev,
-            (hi - lo) / granule * row_bytes, cs));
+            static_cast<uint8_t*>(stage_peer[r]) + buf_off + sides[k].offset + lo / granule * sides[k].row_bytes,
+            devs[r], static_cast<const uint8_t*>(sides[k].src) + (sb[r] + lo) / granule * sides[k].row_bytes,
+            root_dev, (hi - lo) / granule * sides[k].row_bytes, cs));
       unsigned long long* ready =
           reinterpret_cast<unsigned long long*>(static_cast<uint8_t*>(ctrl_peer[r]) + KTB_CTRL_READY) + c;
       rc = launch_flag_publish(ready, seq, cs);   // stream-ordered behind the copy
@@ -431,8 +446,8 @@ int ktb_push_scatter_ce(int root_dev, const void* src_root, size_t n_elems, size
                         void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, unsigned long long seq,
                         uintptr_t stream) {
   return push_scatter_ce_impl("ktb_push_scatter_ce", root_dev, src_root, n_elems, granule, dtype, n_ranks, root_rank,
-                              devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, false, nullptr, 0, 0,
-                              seq, stream);
+                              devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, 0, nullptr, seq,
+                              stream);
 }
 
 int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
@@ -440,9 +455,25 @@ int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elem
                                size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
                                const void* mask_root, size_t row_bytes, size_t mask_offset, unsigned long long seq,
                                uintptr_t stream) {
+  const PushSide side{mask_root, row_bytes, mask_offset, "mask"};
   return push_scatter_ce_impl("ktb_push_scatter_ce_masked", root_dev, src_root, n_elems, granule, dtype, n_ranks,
-                              root_rank, devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, true,
-                              mask_root, row_bytes, mask_offset, seq, stream);
+                              root_rank, devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, 1, &side,
+                              seq, stream);
+}
+
+int ktb_push_scatter_ce_sides(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
+                              int n_ranks, int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
+                              void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems, int n_sides,
+                              const void* const* side_src, const size_t* side_row_bytes, const size_t* side_offset,
+                              unsigned long long seq, uintptr_t stream) {
+  static const char* const kNames[2] = {"side 0", "side 1"};
+  // a bad count or null arrays reach the impl as no sides at all, which it refuses after the plain form's checks
+  const bool ok = n_sides >= 1 && n_sides <= 2 && side_src && side_row_bytes && side_offset;
+  PushSide sides[2];
+  for (int k = 0; ok && k < n_sides; ++k) sides[k] = {side_src[k], side_row_bytes[k], side_offset[k], kNames[k]};
+  return push_scatter_ce_impl("ktb_push_scatter_ce_sides", root_dev, src_root, n_elems, granule, dtype, n_ranks,
+                              root_rank, devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems,
+                              ok ? n_sides : -1, ok ? sides : nullptr, seq, stream);
 }
 
 int ktb_push_consume(int dev, int op, int dtype, const void* stage_local, size_t stage_stride, void* dst_root_shard,

@@ -178,6 +178,19 @@ for _suffix in ("", "_value"):
         _restype, _args = _SIGNATURES["ktb_mlp_bf16_policy_gaussian" + _suffix + _form]
         _SIGNATURES["ktb_mlp_bf16_policy_gaussian_state" + _suffix + _form] = (
             _restype, _args[:_at] + [ctypes.c_float, ctypes.c_float, c_int] + _args[_at + 1:])
+# The _epsilon_greedy entries: the sample entries' arguments with (epsilon, seed, row_base, actions, q, q_max) in place
+# of (seed, row_base, actions, log_probs); the masked ones with the mask before epsilon, and the pushed ones with
+# (mask_offset and) epsilon_offset in place of the pointers.
+# seed is the 13th argument of the plain and staged forms and the 14th of the pushed ones, one later when masked.
+for _masked in ("", "_masked"):
+    for _form, _eps, _at in (("", c_void_p, 12), ("_pushed", c_size_t, 13)):
+        _restype, _args = _SIGNATURES["ktb_mlp_bf16_policy_sample" + _masked + _form]
+        _at += bool(_masked)
+        _SIGNATURES["ktb_mlp_bf16_policy_epsilon_greedy" + _masked + _form] = (
+            _restype, _args[:_at] + [_eps] + _args[_at:_at + 4] + [c_void_p] + _args[_at + 4:])
+_SIGNATURES["ktb_push_scatter_ce_sides"] = (
+    c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
+                                                         ctypes.c_ulonglong, c_uintptr])
 
 _lib = None
 _lock = threading.Lock()

@@ -4,10 +4,12 @@ Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_m
 diagonal-Gaussian actions with their log-probabilities), the _masked forms of the first two (a per-row legal-action
 mask), the _value forms of the sampled heads (a critic's state value on the same trunk), the _multidiscrete forms of
 the greedy and sampled heads (one categorical per group of columns), the _gaussian_state forms (a per-row log-std
-head, optionally tanh-squashed actions) and their scatter→exec→gather form."""
+head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network's ε-greedy actor) and their
+scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
+import math
 import weakref
 from typing import List, Optional, Sequence, Tuple
 
@@ -126,8 +128,30 @@ def _check_state_std(log_std, log_std_bounds, squash, w3, b3, d_hidden, d_out, v
         raise ValueError(f"squash must be True or False, got {squash!r}")
 
 
+def _check_epsilon(epsilon, obs) -> None:
+    """_check_policy's checks of output="epsilon_greedy"'s epsilon: given; a number (not a bool) that is not NaN, or a
+    contiguous CUDA float32 tensor [M] on the device of obs [M, d_in]."""
+    if epsilon is None:
+        raise ValueError('epsilon is required with output="epsilon_greedy": a float or a float32 tensor [M]')
+    if isinstance(epsilon, torch.Tensor):
+        if not isinstance(obs, torch.Tensor):
+            raise ValueError("an epsilon tensor is checked against obs: pass the obs [M, d_in] it goes with")
+        if epsilon.dtype != torch.float32 or tuple(epsilon.shape) != (obs.shape[0],):
+            raise ValueError(f"epsilon must be a float32 tensor of shape ({obs.shape[0]},), got {epsilon.dtype} "
+                             f"{tuple(epsilon.shape)}")
+        if not epsilon.is_contiguous():
+            raise ValueError("epsilon must be contiguous")
+        if not epsilon.is_cuda or epsilon.device != obs.device:
+            raise ValueError(f"epsilon must be a CUDA tensor on the device of obs ({obs.device}), got {epsilon.device}")
+        return
+    if isinstance(epsilon, bool) or not isinstance(epsilon, (int, float)):
+        raise ValueError(f"epsilon must be a float or a float32 tensor [M], got {epsilon!r}")
+    if math.isnan(epsilon):
+        raise ValueError("epsilon must not be NaN (a NaN float never explores: pass 0.0 for that)")
+
+
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
-                  nvec=None, log_std_bounds=None, squash=None) -> None:
+                  nvec=None, log_std_bounds=None, squash=None, epsilon=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
     (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
@@ -137,11 +161,16 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     device of w3, beside a policy at most 255 wide; nvec (output="actions", "both" or "sample" only) is a non-empty
     tuple or list of ints >= 1 that sums to d_out (mapped.check_nvec).  With output="gaussian", log_std may instead
     be a state-dependent head (w_ls, b_ls) (_check_state_std), and log_std_bounds and squash are taken with that form
-    only."""
+    only.  output="epsilon_greedy" takes a seed and an epsilon (_check_epsilon), and epsilon is refused with any other
+    output; its value=, nvec= and log_std= are refused by the checks of those options."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
-    if output in ("sample", "gaussian"):
+    if output in ("sample", "gaussian", "epsilon_greedy"):
         _check_seed(seed)
+    if output == "epsilon_greedy":
+        _check_epsilon(epsilon, obs)
+    elif epsilon is not None:
+        raise ValueError(f'epsilon is an argument of output="epsilon_greedy", not of output={output!r}')
     if mask is not None and output == "gaussian":
         raise ValueError('mask is an argument of the categorical outputs, not of output="gaussian"')
     if len(biases) != 3:
@@ -221,7 +250,8 @@ def _stacked_head(w3, b3, wv=None, bv=None, w_ls=None, b_ls=None) -> Tuple[torch
 def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False, nvec=None):
     """(logits, actions, log_probs, values) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions
     [M], [M, len(nvec)] with nvec, or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values
-    [M].  A buffer the mode does not write is None, a missing one is allocated on `device` and a given one is
+    [M].  With "epsilon_greedy" the last two slots hold its fp32 q [M] and q_max [M].  A buffer the mode does not
+    write is None, a missing one is allocated on `device` and a given one is
     registered with the library (ops.ensure_init); given multi-discrete actions must be [M, len(nvec)]."""
     def buf(t, shape, dtype):
         if t is None:
@@ -237,20 +267,23 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
             None if output == "logits" else
             buf(actions, (M, d_out), torch.float32) if gaussian else
             buf(actions, (M,) if nvec is None else (M, len(nvec)), torch.int64),
-            buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian") else None,
-            buf(values, (M,), torch.float32) if valued else None)
+            buf(log_probs, (M,), torch.float32) if output in ("sample", "gaussian", "epsilon_greedy") else None,
+            buf(values, (M,), torch.float32) if valued or output == "epsilon_greedy" else None)
 
 
 def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None,
-          nvec=None, std=None):
+          nvec=None, std=None, epsilon=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
     mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
     picks the _value entry (whose W3 and b3 are the stacked head) and is its values buffer.  `nvec`, unless None,
     picks the _multidiscrete entry and is its group sizes.  `std` = (log_std_min, log_std_max, squash), unless None,
-    picks the _gaussian_state entry (whose W3 and b3 are the interleaved head) in place of log_std."""
+    picks the _gaussian_state entry (whose W3 and b3 are the interleaved head) in place of log_std.  With
+    "epsilon_greedy", `epsilon` is ε's address (pull forms) or its offset in the staging half (pushed forms), and
+    log_probs and values are its q and q_max buffers."""
+    eps = output == "epsilon_greedy"
     suffix = ("" if nvec is None else "_multidiscrete") + ("" if mask is None else "_masked") + \
-        ("" if values is None else "_value") + ("_pushed" if pushed else "")
+        ("" if values is None or eps else "_value") + ("_pushed" if pushed else "")
     grouped = () if nvec is None else (L.arr(ctypes.c_int32, nvec), len(nvec))
     masked = () if mask is None else (mask,)
     valued = () if values is None else (ptr(values),)
@@ -260,6 +293,9 @@ def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, push
     if output == "gaussian":
         return "ktb_mlp_bf16_policy_gaussian" + suffix, (ptr(log_std), seed, row_base, ptr(actions), ptr(log_probs),
                                                          *valued)
+    if eps:
+        return "ktb_mlp_bf16_policy_epsilon_greedy" + suffix, (*masked, epsilon, seed, row_base, ptr(actions),
+                                                               ptr(log_probs), ptr(values))
     if output == "sample":
         return "ktb_mlp_bf16_policy_sample" + suffix, (*grouped, *masked, seed, row_base, ptr(actions), ptr(log_probs),
                                                        *valued)
@@ -299,6 +335,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
                 values: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
                 log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
+                epsilon=None, q: Optional[torch.Tensor] = None, q_max: Optional[torch.Tensor] = None,
                 _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
@@ -330,7 +367,13 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     sum_j log(1 - tanh(u_j)^2), taken exactly as 2·(log 2 - |u| - softplus(-2|u|)) (not SB3's
     log(1 - tanh^2 + 1e-6), which differs where |u| > about 7).  The head then runs over the interleaved rows of w3 and
     w_ls (_stacked_head), at most 128 actions (127 with a value head).  log_std_bounds and squash are refused with a
-    tensor log_std.  `_stacked` (internal, from mlp_scatter_gather, which checked the call): w3 and biases[2] are
+    tensor log_std.  output="epsilon_greedy" (a Q-network's actor; masked or not, with `seed`) returns (actions, q,
+    q_max): with u, w = kubetorch_b200.sampling.explore_noise(seed, row_offset, M, d_out), row i explores iff u[i] <
+    epsilon[i] in fp32 and then takes the legal column with the largest w (ties to the lower column), and otherwise
+    the argmax of its (masked) logits; q is the fp32 (masked) logit of the action taken and q_max that of the argmax,
+    into `q` and `q_max` when given; no logits are written.  `epsilon` is a CUDA float32 tensor [M] on the device of
+    obs or a number broadcast to every row (rounded to fp32; NaN refused).  `_stacked` (internal, from
+    mlp_scatter_gather, which checked the call): w3 and biases[2] are
     already the head the C entry takes (stacked with a value head, interleaved with a log-std head)."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
@@ -342,17 +385,23 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
     if not _stacked:
-        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash)
+        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     valued = value is not None or (_stacked and values is not None)
     if _stacked:
         d_out = (d_out - valued) // (2 if std is not None else 1)
-    if output in ("sample", "gaussian") and \
+    if output in ("sample", "gaussian", "epsilon_greedy") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
+    eps = output == "epsilon_greedy"
+    if eps:   # q and q_max ride in the log_probs and values slots
+        log_probs, values = q, q_max
     out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued,
                                                nvec)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
+    if eps and not isinstance(epsilon, torch.Tensor):
+        with torch.cuda.stream(s):   # freed after the call, its memory is reused in s's order, after the kernel
+            epsilon = torch.full((M,), float(epsilon), dtype=torch.float32, device=f"cuda:{dev}")
     if not _stacked and (value is not None or std is not None):
         with torch.cuda.stream(s):   # a rewrite of the stacked head is ordered after earlier calls on s
             w3, b3 = _stacked_head(w3, biases[2], *(value or (None, None)), *(log_std if std is not None else ()))
@@ -361,7 +410,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
         staged = obs.device.index != dev   # observations on another GPU: pull each row chunk over NVLink once
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
-                        mask=None if mask is None else ptr(mask), values=values, nvec=nvec, std=std)
+                        mask=None if mask is None else ptr(mask), values=values, nvec=nvec, std=std,
+                        epsilon=ptr(epsilon) if eps else None)
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
@@ -393,7 +443,8 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
-                               seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None) -> None:
+                               seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None,
+                               epsilon=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -405,14 +456,21 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     rank's mask rows into the same staging half, 256-byte aligned after the largest shard's observation rows, so no
     rank reads the root's memory.  With `values_root` (fp32 [M]) weights[dev] holds the stacked W3v and b3v in place of
     w3 and b3, and each rank stores its values there too.  `nvec` picks every rank's multi-discrete entry.  `std`
-    (_std) picks every rank's _gaussian_state entry, weights[dev] then holding the interleaved head."""
+    (_std) picks every rank's _gaussian_state entry, weights[dev] then holding the interleaved head.  With
+    output="epsilon_greedy", `epsilon` is the fp32 [M] on the root, pushed with the rows like the mask: each staging
+    half is rows | mask | ε, each 256-byte aligned (ktb_push_scatter_ce_sides), and log_probs_root / values_root are
+    its q and q_max."""
     root, n, key = devs[0], len(devs), tuple(devs)
-    valued = values_root is not None
+    valued = values_root is not None and epsilon is None   # an ε-greedy head's values_root is its q_max
     d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
     d_out = (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
     rows = max(e - b for b, e in bounds)
     mask_offset = (rows * d_in * 2 + 255) // 256 * 256
     stage_bytes = rows * d_in * 2 if mask is None else mask_offset + rows * d_out
+    eps_offset = None
+    if epsilon is not None:
+        eps_offset = mask_offset if mask is None else (mask_offset + rows * d_out + 255) // 256 * 256
+        stage_bytes = eps_offset + rows * 4
     sess = _push_sessions.get(key)
     if sess is None or sess.stride < stage_bytes:
         sess = _push_sessions[key] = ops.PushSession(devs, stage_bytes)
@@ -436,10 +494,18 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
                     biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
                     log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0],
                     values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
-                    squash=None if std is None else bool(std[2]), _stacked=valued or std is not None)
+                    squash=None if std is None else bool(std[2]),
+                    **({} if epsilon is None else dict(epsilon=epsilon[b0:e0], q=log_probs, q_max=values)),
+                    _stacked=valued or std is not None)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
-    if mask is None:
+    if epsilon is not None:
+        sides = ([] if mask is None else [(mask.data_ptr(), d_out, mask_offset)]) + [(epsilon.data_ptr(), 4, eps_offset)]
+        src, row_bytes, offsets = zip(*sides)
+        L.call("ktb_push_scatter_ce_sides", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, *scatter,
+               len(sides), L.arr(ctypes.c_void_p, src), L.arr(ctypes.c_size_t, row_bytes),
+               L.arr(ctypes.c_size_t, offsets), seq, streams[0])
+    elif mask is None:
         L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, *scatter, seq,
                streams[0])
     else:
@@ -453,7 +519,8 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         logits, actions, log_probs, values = _rows(bufs, b, e)
         entry, head = _head(output, logits, actions, log_probs, seed, b,
                             None if log_std is None else log_std[devs[r]], ptr, pushed=True,
-                            mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std)
+                            mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std,
+                            epsilon=eps_offset)
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -469,7 +536,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        log_probs_root: Optional[torch.Tensor] = None, log_std: Optional[torch.Tensor] = None,
                        mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
                        values_root: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
-                       log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None) -> list:
+                       log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
+                       epsilon=None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -482,14 +550,18 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     the root and copied to the other devices like the other weights, and every rank stores its values into
     `values_root` (allocated on the root when None).  `nvec` as in mlp_forward: actions are [rows, G] views.
     A state-dependent log_std = (w_ls, b_ls), with `log_std_bounds` and `squash`, as in mlp_forward: the interleaved
-    head is built on the root and copied to the other devices like the other weights."""
+    head is built on the root and copied to the other devices like the other weights.  output="epsilon_greedy" with
+    `epsilon` (a float, or an fp32 [M] on the root) as in mlp_forward returns (actions, q, q_max) triples; each rank
+    reads its rows of ε in place on the pull form, and the push form pushes them with the rows."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
+    if output == "epsilon_greedy" and not isinstance(epsilon, torch.Tensor):   # before `ready`: every rank reads it
+        epsilon = torch.full((M,), float(epsilon), dtype=torch.float32, device=obs_root.device)
     valued = value is not None
     bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
                     valued, nvec)
@@ -516,7 +588,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec, std)
+                                   nvec, std, epsilon)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -540,7 +612,9 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                         output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
                         log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e],
                         values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
-                        squash=None if std is None else bool(std[2]), _stacked=valued or std is not None)
+                        squash=None if std is None else bool(std[2]),
+                        **({} if epsilon is None else dict(epsilon=epsilon[b:e], q=log_probs, q_max=values)),
+                        _stacked=valued or std is not None)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

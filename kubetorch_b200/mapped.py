@@ -23,7 +23,7 @@ from typing import Any, Callable, Dict, Optional
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
-MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian")   # also device.mlp.OUTPUTS
+MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy")   # also device.mlp.OUTPUTS
 
 
 @dataclass
@@ -92,24 +92,32 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     ``log_std`` may instead name two call arguments ``(w_ls, b_ls)`` (with ``bias=True``): a state-dependent log-std
     head ``nn.Linear(d_hidden, d_out)`` on the same trunk, clamped to ``log_std_bounds`` (two numbers, default
     ``(-20.0, 2.0)``), with ``squash=True`` for tanh-squashed actions and the log-probability's tanh correction (SAC's
-    actor); ``value=`` may go beside it.  ``log_std_bounds`` and ``squash`` are options of that form only."""
+    actor); ``value=`` may go beside it.  ``log_std_bounds`` and ``squash`` are options of that form only.
+    ``output="epsilon_greedy"`` (a Q-network's actor: DQN, Ape-X, R2D2) returns ``(actions, q, q_max)`` per rank and
+    takes ``seed=`` and ``epsilon=``, a number or the name of a call argument that holds a float or a per-row fp32
+    tensor [M] on the device of obs (the body takes ``eps.chunk(WORLD_SIZE)[RANK]`` of a tensor): with ``u, w =
+    kubetorch_b200.sampling.explore_noise(seed, row0, rows, d_out)`` a row explores iff ``u < ε`` and takes the legal
+    column with the largest ``w``, and otherwise the argmax of its logits; ``q`` is the fp32 logit of the action taken
+    and ``q_max`` that of the argmax (``mask=`` applies, ``value=`` and ``nvec=`` do not)."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
     if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
-                                "squash")):
+                                "squash", "epsilon")):
         if op != "mlp":
-            raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value= and nvec= are "
-                             f"options of the 'mlp' op, not of '{op}'")
+            raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value=, nvec= and "
+                             f"epsilon= are options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
         sample = extra.get("output") in ("sample", "gaussian")
-        if sample != ("seed" in extra):
-            raise ValueError('seed= is required with output="sample" or "gaussian" and is an option of those only')
-        if sample and not isinstance(extra["seed"], str):
+        eps = extra.get("output") == "epsilon_greedy"
+        if (sample or eps) != ("seed" in extra):
+            raise ValueError('seed= is required with output="sample" or "gaussian" (or "epsilon_greedy") and is an '
+                             'option of those only')
+        if (sample or eps) and not isinstance(extra["seed"], str):
             from .sampling import _check_seed
 
             _check_seed(extra["seed"])
@@ -155,11 +163,21 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
                 raise ValueError(f"value must name two call arguments (wv, bv), got {v!r}")
         if "nvec" in extra:
             extra["nvec"] = check_nvec(extra["nvec"], extra.get("output", "logits"))
+        if eps != ("epsilon" in extra):
+            raise ValueError('epsilon= is required with output="epsilon_greedy" and is an option of that output only')
+        if eps and not isinstance(extra["epsilon"], str):
+            e = extra["epsilon"]
+            if isinstance(e, bool) or not isinstance(e, (int, float)):
+                raise ValueError(f"epsilon must be a number or the name of a call argument, got {e!r}")
+            if e != e:
+                raise ValueError("epsilon must not be NaN (a NaN never explores: pass 0.0 for that)")
 
     def deco(fn):
         params = inspect.signature(fn).parameters
-        for option in ("log_std", "mask", "value"):
+        for option in ("log_std", "mask", "value", "epsilon"):
             names = extra.get(option)
+            if option == "epsilon" and not isinstance(names, str):   # a constant ε names no argument
+                continue
             for name in (names,) if isinstance(names, str) or names is None else names:
                 if name is not None and name not in params:
                     raise ValueError(f"{option}={names!r}: {name!r} is not an argument of "

@@ -1,16 +1,20 @@
-"""The Gumbel noise of @kt.mapped("mlp", output="sample") and the Gaussian noise of output="gaussian", in plain torch
-(no GPU, no library).
+"""The Gumbel noise of @kt.mapped("mlp", output="sample"), the Gaussian noise of output="gaussian" and the exploration
+draws of output="epsilon_greedy", in plain torch (no GPU, no library).
 
 A sampled policy body adds ``gumbel_noise(seed, row0, rows, d_out)`` to its fp32 logits, takes the argmax and gathers
-the log_softmax; a Gaussian policy body adds ``exp(log_std)·normal_noise(seed, row0, rows, d_out)`` to its mean.  The
-device kernel draws the very same noise in its head epilogue (include/ktb200.h).  For global row i (the row's index
-in the whole observation batch) and column j:
+the log_softmax; a Gaussian policy body adds ``exp(log_std)·normal_noise(seed, row0, rows, d_out)`` to its mean; an
+ε-greedy body takes ``u, w = explore_noise(seed, row0, rows, d_out)``, explores where ``u < ε`` and then takes the
+legal column with the largest word ``w``.  The device kernel draws the very same numbers in its head epilogue
+(include/ktb200.h).  For global row i (the row's index in the whole observation batch) and column j:
 
     x = Philox4x32-10(counter = (i mod 2^32, i >> 32, j >> 1, s), key = (seed mod 2^32, seed >> 32)), word j & 1
-        with s = 0 for the Gumbel noise and s = 1 for the Gaussian noise
     u = (2·(x >> 9) + 1)·2^-24          exact in fp32, strictly inside (0, 1), never 0.5
-    g = -log(-log(u))                   in fp32 (Gumbel)
-    z = Φ⁻¹(u)                          in fp32 (Gaussian), within ±5.29471 and never 0
+
+    stream  s   use
+    Gumbel  0   g = -log(-log(u)) in fp32, added to the logits of output="sample"
+    Gaussian 1  z = Φ⁻¹(u) in fp32, within ±5.29471 and never 0, the noise of output="gaussian"
+    explore 2   the word x itself (a uint32): ranks the legal columns of an exploring row of output="epsilon_greedy"
+    coin    3   u of column 0 only (one draw per row): the row explores iff u < ε in fp32
 
 The noise depends on (seed, i, j) only, so every sharding of the rows draws the same noise for the same row.
 """
@@ -53,7 +57,7 @@ def _check_seed(seed) -> int:
 
 def random_words(seed: int, row_offset: int, rows: int, cols: int, device="cpu", word3: int = 0) -> torch.Tensor:
     """int64 [rows, cols]: the 32-bit Philox word of global row row_offset + r and column j.  `word3` is the fourth
-    counter word: 0 for the Gumbel noise, 1 for the Gaussian noise."""
+    counter word: 0 for the Gumbel noise, 1 for the Gaussian noise, 2 for the exploration words, 3 for the coin."""
     seed = _check_seed(seed)
     if row_offset < 0 or rows < 0 or cols < 0:
         raise ValueError("row_offset, rows and cols must be non-negative")
@@ -87,3 +91,12 @@ def gumbel_noise(seed: int, row_offset: int, rows: int, cols: int, device="cpu")
     """float32 [rows, cols]: the Gumbel noise g = -log(-log(u)) of global rows row_offset .. row_offset + rows - 1."""
     u = gumbel_uniform(seed, row_offset, rows, cols, device)
     return -torch.log(-torch.log(u))
+
+
+def explore_noise(seed: int, row_offset: int, rows: int, cols: int, device="cpu"):
+    """(u, words) of output="epsilon_greedy" for global rows row_offset .. row_offset + rows - 1: u float32 [rows], the
+    exact uniform of word 0 of counter (i, 0, 3) (a row explores iff u < ε in fp32), and words int64 [rows, cols], the
+    uint32 Philox word j & 1 of counter (i, j >> 1, 2) (an exploring row takes the legal column with the largest word,
+    ties to the lower column).  Neither stream reuses the Gumbel (0) or Gaussian (1) draws of the same seed."""
+    u = gumbel_uniform(seed, row_offset, rows, 1, device, word3=3)[:, 0]
+    return u, random_words(seed, row_offset, rows, cols, device, word3=2)

@@ -594,12 +594,17 @@ class B200Supervisor:
                 if name not in bound:
                     raise TypeError(f"mapped mlp callable: value argument '{name}' not found in the call")
             value = tuple(bound[name] for name in value)
+        epsilon = spec.extra.get("epsilon")
+        if isinstance(epsilon, str):   # the name of a call argument (a float or a per-row tensor), resolved per call
+            if epsilon not in bound:
+                raise TypeError(f"mapped mlp callable: epsilon argument '{epsilon}' not found in the call")
+            epsilon = bound[epsilon]
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
                                          value=value, nvec=spec.extra.get("nvec"),
                                          log_std_bounds=spec.extra.get("log_std_bounds"),
-                                         squash=spec.extra.get("squash"))
+                                         squash=spec.extra.get("squash"), epsilon=epsilon)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

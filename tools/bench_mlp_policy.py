@@ -30,6 +30,11 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      without the fused head: the logits entry over the stacked head [w3; w_ls], then clamp, exp, noise, tanh and the
      log-density in torch.  The interleaved head doubles the head's columns: d_out 64 runs in the 128-wide tile and 128
      in the 256-wide one.
+  m  ε-greedy Q-network heads (output="epsilon_greedy"), d_out 6, 18 and 64, ε 0.01, 0.05 and 1.0 (the worst case:
+     every row draws a Philox call per column pair), unmasked and under a random legal-action mask, each beside
+     output="actions" and output="sample" at the same d_out and mask; and the eager arm, what a user pays without the
+     fused head: the logits entry (masked in torch under a mask), then argmax, the exploration draws of explore_noise,
+     where and two gathers in torch.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -44,7 +49,8 @@ log-probabilities within 2^-16·(1 + |ref|) on those rows, and every masked samp
 legal.  State-dependent rows: on 2048 consecutive rows, the unsquashed actions are within 2^-19·σ·(1 + |z|) +
 2^-23·|μ| of μ + σ·z (μ and ℓ the kernel's logits over the interleaved head, σ = exp(clamp(ℓ))), the squashed actions
 within 2 ulp of tanh of the unsquashed ones, and on every row both the actions and log-probabilities are within rtol
-1e-4, atol 1e-4 of the eager arm's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+1e-4, atol 1e-4 of the eager arm's.  ε-greedy rows: actions, q and q_max equal the eager arm's on every row, bit for
+bit.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -62,7 +68,7 @@ import torch.nn.functional as F  # noqa: E402
 from kubetorch_b200.device import lib as L  # noqa: E402
 from kubetorch_b200.device import mlp  # noqa: E402
 from kubetorch_b200.device import ops  # noqa: E402
-from kubetorch_b200.sampling import gumbel_noise, gumbel_uniform, normal_noise  # noqa: E402
+from kubetorch_b200.sampling import explore_noise, gumbel_noise, gumbel_uniform, normal_noise  # noqa: E402
 
 HALF_LOG_2PI = 0.9189385332046727
 LN2 = 0.6931471805599453
@@ -252,6 +258,34 @@ def main():
                 obs, w1, w2, heads[d][0], biases=bs, output="gaussian", seed=SEED, log_std=ls_heads[d],
                 squash=squash))
             variants[f"l_bias_state_{tag}_eager_d{d}"] = (d, lambda d=d, squash=squash: eager_state(d, squash))
+    eps_widths, eps_values = (6, 18, 64), (0.01, 0.05, 1.0)
+
+    def eager_epsilon(d, mask, eps):
+        """The logits entry, then the ε-greedy head in torch: what a user pays without output="epsilon_greedy"."""
+        q = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]))
+        if mask:
+            q = q.masked_fill(~legal[d], float("-inf"))
+        u, w = explore_noise(SEED, 0, M, d, device="cuda:0")
+        greedy = q.argmax(-1)
+        explore_a = w.masked_fill(~legal[d], -1).argmax(-1) if mask else w.argmax(-1)
+        actions = torch.where(u < eps, explore_a, greedy)
+        qf = q.float()
+        return actions, qf.gather(1, actions[:, None])[:, 0], qf.gather(1, greedy[:, None])[:, 0]
+
+    for d in eps_widths:
+        bs = (b1, b2, heads[d][1])
+        for mask in (False, True):
+            m = dict(mask=legal[d]) if mask else {}
+            tag = "masked_" if mask else ""
+            variants[f"m_bias_{tag}actions_d{d}"] = (d, lambda d=d, bs=bs, m=m: mlp.mlp_forward(
+                obs, w1, w2, heads[d][0], biases=bs, output="actions", **m))
+            variants[f"m_bias_{tag}sample_d{d}"] = (d, lambda d=d, bs=bs, m=m: mlp.mlp_forward(
+                obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED, **m))
+            for eps in eps_values:
+                variants[f"m_bias_{tag}epsilon{eps}_d{d}"] = (d, lambda d=d, bs=bs, m=m, eps=eps: mlp.mlp_forward(
+                    obs, w1, w2, heads[d][0], biases=bs, output="epsilon_greedy", seed=SEED, epsilon=eps, **m))
+                variants[f"m_bias_{tag}epsilon{eps}_eager_d{d}"] = (
+                    d, lambda d=d, mask=mask, eps=eps: eager_epsilon(d, mask, eps))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -406,6 +440,19 @@ def main():
             del want
         parity[f"l_bias_state_d{d}"] = entry
         del u, lp, a, lp_sq
+
+    for d in eps_widths:
+        entry = {}
+        for tag in ("", "masked_"):
+            for eps in eps_values:
+                got = variants[f"m_bias_{tag}epsilon{eps}_d{d}"][1]()
+                want = variants[f"m_bias_{tag}epsilon{eps}_eager_d{d}"][1]()
+                for g_, w_ in zip(got, want):
+                    assert torch.equal(g_.view(torch.int32) if g_.dtype == torch.float32 else g_,
+                                       w_.view(torch.int32) if w_.dtype == torch.float32 else w_), (tag, eps, d)
+                entry[f"{tag}epsilon{eps}_eq_eager_all_rows"] = "ok"
+                del got, want
+        parity[f"m_bias_epsilon_d{d}"] = entry
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
