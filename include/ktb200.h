@@ -717,6 +717,125 @@ int ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed(int dev, const void* stage_
                                                      void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
                                                      size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* Evaluating forms: the log-probability and the entropy of actions the caller already holds, under the categorical
+ * (single or multi-discrete, masked or not) or the state-independent Gaussian policy, with no noise drawn and no logits
+ * written: SB3's policy.evaluate_actions and RLlib's dist.logp / dist.entropy, forward only.
+ * Categorical (ktb_mlp_bf16_policy_evaluate and its _masked, _value and _masked_value forms): ktb_mlp_bf16_policy's
+ * arguments up to b3 (W3v / b3v in the value forms), then (const int32_t* nvec, int n_groups, [const uint8_t* mask,]
+ * const int64_t* taken, float* log_probs, float* entropy, [float* values,] void* scratch, void* stage, uintptr_t stream).
+ *   - y is the bf16-rounded head output (ktb_mlp_bf16_policy's logits); masked: y.masked_fill(~legal, -inf).
+ *   - Groups as in the multi-discrete forms; nvec == NULL with n_groups == 0 is one group of the d_out columns.  taken
+ *     [M] (no nvec) or [M, n_groups] int64 holds group-relative actions a_g.
+ *   - For group g over columns [lo, hi) and its legal columns: m = their max (NaN skipped), S = sum (y == m ? 1 :
+ *     expf(y - m)), T = sum w*(y - m) with w the term of S (one fused multiply-add; a -inf column adds 0 to both), in
+ *     the sampling forms' per-thread and quad order.  Then, in this order of precedence: a_g outside [0, hi - lo) gives
+ *     lp_g = H_g = NaN; no legal column, or m == -inf, gives lp_g = H_g = NaN (torch's log_softmax of an all -inf row);
+ *     an illegal column lo + a_g gives lp_g = -inf; otherwise lp_g = y[lo + a_g] - m - logf(S), the expression of the
+ *     sampling forms; and H_g = logf(S) - T / S.
+ *   - log_probs[i] and entropy[i] are the fp32 sums over groups in group order, starting from group 0's term.  With a
+ *     value head values[i] is computed as in the value forms.
+ *   - So evaluating the actions a sampling form drew (same weights, mask and nvec) returns its log_probs bit for bit,
+ *     NaN in the same rows.  A row with one legal column gives lp = 0 and H = 0 for that column; n equal logits give
+ *     H = logf(n).  A NaN legal logit makes S, T, the row's lp (but an illegal action's -inf) and H NaN; a +inf logit
+ *     makes T, H and the lp of a +inf column NaN, and the lp of a finite column -inf.
+ *   - An action out of range is a caller error: it is not checked (that would need a host synchronisation) and gives a
+ *     NaN row.
+ * Gaussian (ktb_mlp_bf16_policy_gaussian_evaluate and its _value form): ktb_mlp_bf16_policy_gaussian's arguments up to
+ * log_std, then (const float* taken, float* log_probs, float* entropy, [float* values,] void* scratch, void* stage,
+ * uintptr_t stream).  There is no seed and no row_base.
+ *   - mu is the bf16-rounded head output; taken [M, d_out] fp32.  z_j = __fdiv_rn(__fsub_rn(a_j, mu_j),
+ *     expf(log_std[j])), with no FMA contraction.
+ *   - log_probs[i] = -sum_j (0.5*z_j^2 + log_std[j]) - d_out*0.5*log(2*pi), in the Gaussian form's per-thread and quad
+ *     order: Normal(mu, exp(log_std)).log_prob(taken).sum(-1).
+ *   - entropy[i] = sum_j (log_std[j] + 0.5) + d_out*0.5*log(2*pi), the same value in every row: Normal.entropy().sum(-1).
+ *   - IEEE cases follow the formulas: log_std[j] = -inf gives sigma = 0, z = +-inf (NaN where a_j == mu_j) and an
+ *     lp of -inf (or NaN); a NaN log_std, action or mean makes lp NaN; H is NaN for a NaN log_std.
+ * Checks: every check of the counterpart without evaluation first, in its order (ktb_mlp_bf16_policy or _masked; the
+ * value forms' values and d_out = 256 KTB_ERR_UNSUPPORTED; ktb_mlp_bf16_policy_gaussian's log_std), then the nvec checks
+ * of the multi-discrete forms unless nvec == NULL and n_groups == 0, then, with M > 0, a NULL or misaligned taken (8
+ * bytes categorical, 4 Gaussian), log_probs or entropy (4 bytes) is KTB_ERR_ARG.  Every chunk size, form and row split
+ * gives the same bits.  taken and the outputs may be peer pointers in the plain and staged forms.  Writes stay inside
+ * log_probs[M], entropy[M], values[M] (value forms), scratch and stage. */
+int ktb_mlp_bf16_policy_evaluate(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                 const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                                 const int32_t* nvec, int n_groups, const int64_t* taken, float* log_probs,
+                                 float* entropy, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_evaluate_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                        const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                        const void* b3, const int32_t* nvec, int n_groups, const uint8_t* mask,
+                                        const int64_t* taken, float* log_probs, float* entropy, void* scratch,
+                                        void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_evaluate_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v,
+                                       const void* b3v, const int32_t* nvec, int n_groups, const int64_t* taken,
+                                       float* log_probs, float* entropy, float* values, void* scratch, void* stage,
+                                       uintptr_t stream);
+int ktb_mlp_bf16_policy_evaluate_masked_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                              const void* W1, const void* b1, const void* W2, const void* b2,
+                                              const void* W3v, const void* b3v, const int32_t* nvec, int n_groups,
+                                              const uint8_t* mask, const int64_t* taken, float* log_probs,
+                                              float* entropy, float* values, void* scratch, void* stage,
+                                              uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_evaluate(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                          const void* W1, const void* b1, const void* W2, const void* b2,
+                                          const void* W3, const void* b3, const float* log_std, const float* taken,
+                                          float* log_probs, float* entropy, void* scratch, void* stage,
+                                          uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_evaluate_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                                const void* W1, const void* b1, const void* W2, const void* b2,
+                                                const void* W3v, const void* b3v, const float* log_std,
+                                                const float* taken, float* log_probs, float* entropy, float* values,
+                                                void* scratch, void* stage, uintptr_t stream);
+/* Push-fed evaluating forms: the _pushed entries' arguments with the evaluating arguments above after b3 (b3v), and
+ * (mask_offset,) taken_offset in place of the pointers.  The rank reads its rows' actions (M*8*max(n_groups, 1) bytes
+ * categorical, M*4*d_out Gaussian) and mask from its own staging half, at stage_local + (seq & 1)*stage_stride + the
+ * offset (ktb_push_scatter_ce_sides puts them there), never from a peer.  After the checks above: a taken region that
+ * overlaps the rows (taken_offset < M*d_in*2) or the mask region, that ends past stage_stride, or whose offset is not a
+ * multiple of 8 (categorical) or 4 (Gaussian), is KTB_ERR_ARG.  An empty shard (M == 0) may pass NULL outputs and a
+ * NULL nvec and still publishes its ack. */
+int ktb_mlp_bf16_policy_evaluate_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                        int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                        const void* b2, const void* W3, const void* b3, const int32_t* nvec,
+                                        int n_groups, size_t taken_offset, float* log_probs, float* entropy,
+                                        void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                        size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_evaluate_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                               int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                               const void* W2, const void* b2, const void* W3, const void* b3,
+                                               const int32_t* nvec, int n_groups, size_t mask_offset,
+                                               size_t taken_offset, float* log_probs, float* entropy, void* scratch,
+                                               void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                               unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_evaluate_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                              int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                              const void* W2, const void* b2, const void* W3v, const void* b3v,
+                                              const int32_t* nvec, int n_groups, size_t taken_offset,
+                                              float* log_probs, float* entropy, float* values, void* scratch,
+                                              void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                              unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_evaluate_masked_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                     int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                     const void* W2, const void* b2, const void* W3v, const void* b3v,
+                                                     const int32_t* nvec, int n_groups, size_t mask_offset,
+                                                     size_t taken_offset, float* log_probs, float* entropy,
+                                                     float* values, void* scratch, void* ctrl_local,
+                                                     void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                     unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_evaluate_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                 int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                 const void* W2, const void* b2, const void* W3, const void* b3,
+                                                 const float* log_std, size_t taken_offset, float* log_probs,
+                                                 float* entropy, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                                 int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                       int d_in, int d_hidden, int d_out, const void* W1,
+                                                       const void* b1, const void* W2, const void* b2,
+                                                       const void* W3v, const void* b3v, const float* log_std,
+                                                       size_t taken_offset, float* log_probs, float* entropy,
+                                                       float* values, void* scratch, void* ctrl_local,
+                                                       void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                       unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

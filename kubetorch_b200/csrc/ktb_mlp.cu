@@ -442,6 +442,25 @@ struct HeadEps {
   }
 };
 
+// The given actions and the entropy output of an evaluating head, the layer kernel's last parameter (by value, like
+// HeadEps, and for the same reason).  `actions` != null marks a kSample head that scores int64 group-relative actions
+// [rows, max(groups.n, 1)] (evaluate_pass); `gauss_actions` != null marks a kGaussian head that scores fp32 actions
+// [rows, d_out] (gaussian_epilogue).  Either writes HeadOut::log_probs and entropy [rows] and draws no noise.
+struct HeadEval {
+  const int64_t* actions = nullptr;
+  const float* gauss_actions = nullptr;
+  float* entropy = nullptr;
+
+  // The same inputs and outputs from row r0 on, `per_row` actions per row.
+  HeadEval from_row(size_t r0, size_t per_row) const {
+    HeadEval e = *this;
+    if (actions) e.actions += r0 * per_row;
+    if (gauss_actions) e.gauss_actions += r0 * per_row;
+    if (entropy) e.entropy += r0;
+    return e;
+  }
+};
+
 // The end of the group that begins at column lo: the next set bit of `starts` past lo, or d.  The words are indexed
 // at compile time, so the bitmap stays in the kernel's parameters.
 __device__ __forceinline__ int group_end(const uint32_t (&starts)[8], int lo, int d) {
@@ -585,6 +604,110 @@ __device__ __forceinline__ void group_pass(Slot slot, const ColBits<BLOCK_N> (&l
   }
 }
 
+// The evaluating pass of sample_epilogue (HeadEval::actions != null) over the bf16 pairs that its pass 1 parked in the
+// ring: the log-probability and the entropy of given actions.  The single categorical is one group over the policy's
+// d columns (groups.n == 0: group_end gives d).  Each group is group_pass's with the action read instead of drawn: a
+// per-thread max of the live columns in [lo, hi) and a quad max m, then S = Σ (y == m ? 1 : expf(y − m)) and
+// T = Σ w·(y − m) (w the term of S, one fused multiply-add; a -inf column adds to neither) in group_pass's per-thread
+// and quad order, so S, m and the log-probability of the sampled action are group_pass's (and the single rolled pass's)
+// bits.  Every lane of a quad reads taken[r, g] of its two rows; the lane whose columns include lo + a reads y_a from
+// its slot (-inf when illegal) and shfl.xor shares it across the quad.  lp_g is NaN for a ∉ [0, hi − lo) or m == -inf
+// (no legal column, or only -inf ones), -inf for an illegal column, else y_a − m − logf(S); H_g is NaN in the first two
+// cases, else logf(S) − T / S.  log_probs[r] and entropy[r] are the fp32 sums over groups in group order, starting from
+// group 0's term.
+template <int BLOCK_N, typename Slot>
+__device__ __forceinline__ void evaluate_pass(Slot slot, const ColBits<BLOCK_N> (&live)[2], const HeadGroups& groups,
+                                              int d, int col0, int row, bool st0, bool st1, const int64_t* taken,
+                                              float* log_probs, float* entropy) {
+  const int G = groups.n > 0 ? groups.n : 1;
+  const int lane = threadIdx.x & 31;
+  float lp[2] = {0.f, 0.f}, ent[2] = {0.f, 0.f};
+  int lo = 0;
+#pragma unroll 1
+  for (int g = 0; g < G; ++g) {
+    const int hi = group_end(groups.starts, lo, d);
+    const int j0 = max(0, (lo - col0 + 6) >> 3);   // the first pair of the thread with col0 + 8j + 1 >= lo
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll 1
+    for (int j = j0; j < BLOCK_N / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= hi) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const float v = c ? __high2float(y) : __low2float(y);
+          if (col + c >= lo && col + c < hi && ((live[h] >> (2 * j + c)) & 1) && v > mx[h]) mx[h] = v;
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        const float o = __shfl_xor_sync(0xffffffffu, mx[h], m);
+        if (o > mx[h]) mx[h] = o;
+      }
+    }
+    float sum[2] = {0.f, 0.f}, t[2] = {0.f, 0.f};
+#pragma unroll 1
+    for (int j = j0; j < BLOCK_N / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= hi) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          if (col + c < lo || col + c >= hi || !((live[h] >> (2 * j + c)) & 1)) continue;
+          const float v = c ? __high2float(y) : __low2float(y);
+          const float w = v == mx[h] ? 1.f : expf(v - mx[h]);
+          sum[h] += w;
+          if (v != -INFINITY) t[h] = __fmaf_rn(w, v - mx[h], t[h]);
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      // the action's column (-1: out of range); every lane of the quad reads the same row's
+      const int64_t a = (h ? st1 : st0) ? taken[(size_t)(row + 8 * h) * G + g] : -1;
+      const int col = a >= 0 && a < hi - lo ? lo + (int)a : -1;
+      const int owner = col < 0 ? lane & 3 : (col >> 1) & 3;
+      float ya = -INFINITY;
+      if (col >= 0 && owner == (lane & 3)) {
+        const int j = (col - col0) >> 3, c = col & 1;
+        const __nv_bfloat162 y = *slot(2 * j + h);
+        if ((live[h] >> (2 * j + c)) & 1) ya = c ? __high2float(y) : __low2float(y);
+      }
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
+        t[h] += __shfl_xor_sync(0xffffffffu, t[h], m);
+        const float oy = __shfl_xor_sync(0xffffffffu, ya, m);
+        if ((lane ^ owner) & m) ya = oy;   // the partner is nearer the owner: after m = 1, 2 every lane holds y_a
+      }
+      const bool bad = col < 0 || mx[h] == -INFINITY;
+      const float l = logf(sum[h]);
+      const float lpg = bad ? NAN : ya == -INFINITY ? -INFINITY : ya - mx[h] - l;
+      const float hg = bad ? NAN : l - t[h] / sum[h];
+      lp[h] = g == 0 ? lpg : lp[h] + lpg;
+      ent[h] = g == 0 ? hg : ent[h] + hg;
+    }
+    lo = hi;
+  }
+  if ((threadIdx.x & 3) == 0) {
+    if (st0) {
+      log_probs[row] = lp[0];
+      entropy[row] = ent[0];
+    }
+    if (st1) {
+      log_probs[row + 8] = lp[1];
+      entropy[row + 8] = ent[1];
+    }
+  }
+}
+
 // The ε-greedy pass of sample_epilogue (epsilon != null) over the bf16 pairs that its pass 1 parked in the ring: a
 // Q-network's actor.  For each of the thread's rows r = row + 8h (global row i = row_base + r):
 //   * the greedy action g: torch.argmax of the live columns (argmax_before; 0 when their values are all -inf or there
@@ -702,14 +825,16 @@ __device__ __forceinline__ void epsilon_pass(Slot slot, const ColBits<BLOCK_N> (
 // With a value head (values != null) the tile holds n_valid = d + 1 columns: the policy's d, then the value column d.
 // Pass 1 parks column d with the rest; everything ranked, drawn, summed or masked stops at d; store_values reads it.
 // A multi-discrete head (groups.n > 0) takes group_pass in place of the rolled pass: the greedy one as well, whose
-// logits (C, unless null) it also stores.  An ε-greedy head (epsilon != null) takes epsilon_pass in its place.  The
-// single categorical's rolled pass stays as it is.
+// logits (C, unless null) it also stores.  An ε-greedy head (epsilon != null) takes epsilon_pass in its place, and an
+// evaluating head (ev.actions != null), grouped or not, evaluate_pass.  The single categorical's rolled pass stays as
+// it is.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                 int n_valid, int row, bool st0, bool st1, int64_t* actions,
                                                 float* log_probs, const uint8_t* mask, uint64_t seed,
                                                 uint64_t row_base, float* values, const HeadGroups& groups,
-                                                __nv_bfloat16* C, const float* epsilon, float* q, float* q_max) {
+                                                __nv_bfloat16* C, const float* epsilon, float* q, float* q_max,
+                                                const HeadEval& ev) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -743,6 +868,11 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
       const float o = __shfl_xor_sync(0xffffffffu, mx[h], m);
       if (o > mx[h]) mx[h] = o;
     }
+  }
+  if (ev.actions != nullptr) {
+    evaluate_pass<BLOCK_N>(slot, live, groups, d, col0, row, st0, st1, ev.actions, log_probs, ev.entropy);
+    store_values(slot, d, row, st0, st1, values);
+    return;
   }
   if (groups.n > 0) {
     group_pass<BLOCK_N>(slot, live, groups, d, col0, row, st0, st1, C, actions, log_probs, seed, row_base);
@@ -819,6 +949,10 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
 // base allow and as scalars otherwise, and Σ (0.5·z² + log_std) per row for the log-probability, which does not read μ.
 // With a value head (values != null) the tile holds n_valid = d + 1 columns, as in sample_epilogue: the rolled pass,
 // the actions' row stride and the log-density's constant cover the policy's d columns only.
+// An evaluating head (ev.gauss_actions != null) takes a third rolled pass in place of the sampling one: it draws no
+// noise, reads the given actions a [rows, d] (float2 where the row stride and the base allow, as the action stores),
+// sums 0.5·z² + log_std with z = __fdiv_rn(__fsub_rn(a, μ), expf(log_std)) in the sampling pass's per-thread and quad
+// order, and stores ev.entropy[row] = Σ (log_std + 0.5) + d·0.5·log(2π), summed in the same order for every row.
 // A state-dependent head (sd.state) takes a rolled pass of its own after the same pass 1: its d = 2·d_out policy
 // columns interleave the mean and the log-std, so pair (2a, 2a + 1) of a thread is (μ_a, ℓ_a) of action a, one parked
 // bf16x2 slot.  ℓ is clamped to [sd.lo, sd.hi] by compares (a NaN stays NaN), σ = expf(ℓc), z is Philox word a & 1
@@ -829,7 +963,7 @@ template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                   int n_valid, int row, bool st0, bool st1, const float* log_std,
                                                   float* actions, float* log_probs, uint64_t seed, uint64_t row_base,
-                                                  float* values, const HeadStd& sd) {
+                                                  float* values, const HeadStd& sd, const HeadEval& ev) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -873,7 +1007,7 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
     }
   }
 #pragma unroll 1
-  for (int j = 0; !sd.state && j < BLOCK_N / 8; ++j) {
+  for (int j = 0; !sd.state && ev.gauss_actions == nullptr && j < BLOCK_N / 8; ++j) {
     const int col = col0 + 8 * j;
     if (col >= d) break;   // a pair wholly past the policy draws no noise
     const __nv_bfloat162 y[2] = {*slot(2 * j), *slot(2 * j + 1)};
@@ -902,6 +1036,39 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
       }
     }
   }
+  const float* taken = ev.gauss_actions;
+  const bool taken_pairs = (d & 1) == 0 && ((uintptr_t)taken & 7) == 0;
+  float ent = 0.f;
+#pragma unroll 1
+  for (int j = 0; taken != nullptr && j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= d) break;
+    const __nv_bfloat162 y[2] = {*slot(2 * j), *slot(2 * j + 1)};
+    const bool has1 = col + 1 < d;
+    const float ls[2] = {log_std[col], has1 ? log_std[col + 1] : 0.f};
+    const float sg[2] = {expf(ls[0]), expf(ls[1])};
+    ent += ls[0] + 0.5f;
+    if (has1) ent += ls[1] + 0.5f;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      if (!(h ? st1 : st0)) continue;
+      const float* p = taken + (size_t)(row + 8 * h) * d + col;
+      float a[2];
+      if (taken_pairs) {
+        const float2 t = *reinterpret_cast<const float2*>(p);
+        a[0] = t.x;
+        a[1] = t.y;
+      } else {
+        a[0] = p[0];
+        a[1] = has1 ? p[1] : 0.f;
+      }
+#pragma unroll
+      for (int c = 0; c < 2; ++c) {
+        const float z = __fdiv_rn(__fsub_rn(a[c], c ? __high2float(y[h]) : __low2float(y[h])), sg[c]);
+        if (c == 0 || has1) sum[h] += 0.5f * z * z + ls[c];
+      }
+    }
+  }
   store_values(slot, d, row, st0, st1, values);
   // the 4 lanes of a quad hold the columns of the same two rows
 #pragma unroll
@@ -909,10 +1076,16 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
 #pragma unroll
     for (int m = 1; m <= 2; m <<= 1) sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], m);
   }
+  if (taken != nullptr) {
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) ent += __shfl_xor_sync(0xffffffffu, ent, m);
+  }
   if ((threadIdx.x & 3) == 0) {
     const float c = (float)d_act * 0.918938533204672742f;   // d_out·0.5·log(2π)
     if (st0) log_probs[row] = -sum[0] - c;
     if (st1) log_probs[row + 8] = -sum[1] - c;
+    if (taken != nullptr && st0) ev.entropy[row] = ent + c;
+    if (taken != nullptr && st1) ev.entropy[row + 8] = ent + c;
   }
 }
 
@@ -976,7 +1149,9 @@ struct HeadOut {
 //   kSample with out.groups: one greedy or sampled action per group of columns into actions[row, g], the summed
 //     log-probability of the sampled ones, and the logits of a greedy head that stores them (group_pass);
 //   kSample with eg.epsilon: the ε-greedy action of each row with the Q-values of the taken and the greedy action
-//     (epsilon_pass).
+//     (epsilon_pass);
+//   kSample with ev.actions and kGaussian with ev.gauss_actions: the log-probability and the entropy of given actions
+//     (evaluate_pass, gaussian_epilogue).
 // A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
 // (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
 // never an action.
@@ -986,7 +1161,7 @@ template <int BLOCK_N, int STAGES, HeadKind KIND>
 __global__ void __launch_bounds__(kMlpThreads, 1)
     mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                            const __nv_bfloat16* bias, const HeadOut out, int n_valid, int K, int rows,
-                           const HeadStd sd, const HeadEps eg) {
+                           const HeadStd sd, const HeadEps eg, const HeadEval ev) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
@@ -1006,10 +1181,10 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, out.mask, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
-                             out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max);
+                             out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max, ev);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
-                                       out.log_probs, out.seed, out.row_base, out.values, sd);
+                                       out.log_probs, out.seed, out.row_base, out.values, sd, ev);
   }
 }
 
@@ -1095,7 +1270,8 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
 // One layer through the epilogue of KIND in BLOCK_N-wide tiles: out = A[M, K] · B[N, K]ᵀ (+ bias), N columns.
 template <int BLOCK_N, HeadKind KIND>
 static int launch_layer(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                        int K, cudaStream_t stream, const HeadStd& sd = HeadStd{}, const HeadEps& eg = HeadEps{}) {
+                        int K, cudaStream_t stream, const HeadStd& sd = HeadStd{}, const HeadEps& eg = HeadEps{},
+                        const HeadEval& ev = HeadEval{}) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
   CUtensorMap ma, mb;
@@ -1109,7 +1285,7 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
   kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M, sd,
-                                                eg);
+                                                eg, ev);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
@@ -1118,9 +1294,9 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
 // head, one more with a value head).
 template <HeadKind KIND>
 static int launch_head(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                       int K, cudaStream_t stream, const HeadStd& sd, const HeadEps& eg) {
+                       int K, cudaStream_t stream, const HeadStd& sd, const HeadEps& eg, const HeadEval& ev) {
   const auto launch = N <= 64 ? launch_layer<64, KIND> : N <= 128 ? launch_layer<128, KIND> : launch_layer<256, KIND>;
-  return launch(dev, A, B, bias, out, M, N, K, stream, sd, eg);
+  return launch(dev, A, B, bias, out, M, N, K, stream, sd, eg, ev);
 }
 
 // Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
@@ -1132,7 +1308,10 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // std.state marks the _gaussian_state entries: W3 / b3 are the interleaved W3s [2·d_out, d_hidden] / b3s (with a
 // value head W3sv / b3sv, one more row), log_std is null, and mlp_run checks the bounds.  `eps` marks the
 // _epsilon_greedy entries: eg.epsilon (the pull forms) or the bytes at MlpFeed::epsilon_offset of the call's staging
-// half (the pushed forms) hold each row's ε, and out.actions, eg.q and eg.q_max receive the outputs.
+// half (the pushed forms) hold each row's ε, and out.actions, eg.q and eg.q_max receive the outputs.  `evaluate` marks
+// the _evaluate entries: ev.actions (kSample) or ev.gauss_actions (kGaussian), or in the pushed forms the bytes at
+// MlpFeed::taken_offset of the call's staging half, hold the given actions, and out.log_probs and ev.entropy receive
+// the outputs; a categorical one is grouped unless nvec == null and n_groups == 0.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1146,6 +1325,8 @@ struct MlpParams {
   HeadStd std;
   bool eps = false;
   HeadEps eg;
+  bool evaluate = false;
+  HeadEval ev;
 
   // A multi-discrete head: the greedy one (logits and/or actions, ranked without noise) or the sampled one, both in
   // the kSample instantiations.
@@ -1177,6 +1358,31 @@ struct MlpParams {
     return p;
   }
 
+  // A categorical evaluating head, in the kSample instantiations: taken [M] or [M, n_groups] int64 (null in the pushed
+  // forms) in, log_probs and entropy out.  nvec == null with n_groups == 0 is the single categorical.
+  static MlpParams evaluate_categorical(const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                        const void* b3, const int32_t* nvec, int n_groups, const int64_t* taken,
+                                        float* log_probs, float* entropy) {
+    MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kSample, {nullptr, nullptr, log_probs}};
+    p.grouped = nvec != nullptr || n_groups != 0;
+    p.nvec = nvec;
+    p.n_groups = n_groups;
+    p.evaluate = true;
+    p.ev = HeadEval{taken, nullptr, entropy};
+    return p;
+  }
+
+  // A state-independent Gaussian evaluating head, in the kGaussian instantiations: taken [M, d_out] fp32 (null in the
+  // pushed forms) in, log_probs and entropy out.
+  static MlpParams evaluate_gaussian(const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                     const void* b3, const float* log_std, const float* taken, float* log_probs,
+                                     float* entropy) {
+    MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian, {nullptr, nullptr, log_probs, 0, 0, log_std}};
+    p.evaluate = true;
+    p.ev = HeadEval{nullptr, taken, entropy};
+    return p;
+  }
+
   MlpParams with_mask(const uint8_t* mask) const {
     MlpParams p = *this;
     p.out.mask = mask;
@@ -1195,9 +1401,9 @@ struct MlpParams {
 // the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds its d_out
 // columns (2·d_out for a state-dependent Gaussian head), one more with a value head.  `consumed`, unless null, is
 // recorded once layer 1 has read a1.
-static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const HeadEps& eg, const void* a1, void* h1,
-                     void* h2, size_t r0, size_t rows, int d_in, int d_hidden, int d_out, cudaEvent_t consumed,
-                     cudaStream_t st) {
+static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const HeadEps& eg, const HeadEval& ev,
+                     const void* a1, void* h1, void* h2, size_t r0, size_t rows, int d_in, int d_hidden, int d_out,
+                     cudaEvent_t consumed, cudaStream_t st) {
   int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
   if (rc) return rc;
   if (consumed) KTB_CK(cudaEventRecord(consumed, st));
@@ -1207,7 +1413,9 @@ static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const Head
                     : p.kind == HeadKind::kSample ? launch_head<HeadKind::kSample>
                                                   : launch_head<HeadKind::kGaussian>;
   const int n = (p.std.state ? 2 * d_out : d_out) + (int)p.valued;
-  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std, eg.from_row(r0));
+  const size_t per_row = ev.gauss_actions ? (size_t)d_out : (size_t)std::max(out.groups.n, 1);   // given actions
+  return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std, eg.from_row(r0),
+              ev.from_row(r0, per_row));
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -1229,12 +1437,14 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
       case HeadKind::kSample:
         if (o.groups.greedy)   // a greedy multi-discrete head takes what the greedy entries take
           KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
-        else if (!p.eps)   // an ε-greedy head's outputs are checked by mlp_run after every other check
+        else if (!p.eps && !p.evaluate)   // ε-greedy and evaluating heads: checked by mlp_run after every other check
           KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
         if (p.std.state)   // a state-dependent head reads its log-std from the head's own columns
           KTB_REQUIRE(o.gauss_actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
+        else if (p.evaluate)   // an evaluating head's actions and outputs are checked by mlp_run after every other check
+          KTB_REQUIRE(o.log_std, KTB_ERR_ARG, "%s: log_std is required", fn);
         else
           KTB_REQUIRE(o.log_std && o.gauss_actions && o.log_probs, KTB_ERR_ARG,
                       "%s: log_std, actions and log_probs are required", fn);
@@ -1264,7 +1474,8 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //           ready[c] = seq in this rank's control block `ctrl`; layer 1 of chunk c waits in-stream for it, and the
 //           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A masked head reads
 //           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows), and
-//           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in.
+//           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in, and an evaluating head its rows' given
+//           actions from taken_offset bytes in.
 // The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
@@ -1277,6 +1488,7 @@ struct MlpFeed {
   unsigned long long seq = 0;
   size_t mask_offset = 0;
   size_t epsilon_offset = 0;
+  size_t taken_offset = 0;
 
   static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
   static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
@@ -1293,6 +1505,11 @@ struct MlpFeed {
     f.epsilon_offset = off;
     return f;
   }
+  MlpFeed with_taken_offset(size_t off) const {
+    MlpFeed f = *this;
+    f.taken_offset = off;
+    return f;
+  }
 };
 
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
@@ -1304,7 +1521,9 @@ struct MlpFeed {
 // returns.  A state-dependent Gaussian entry's head width (2·d_out, one more with a value head, <= 256) and log-std
 // bounds (skipped for an empty call) come after every check of its state-independent counterpart.  An ε-greedy entry's
 // own checks come after every check of its greedy counterpart (ktb_mlp_bf16_policy or _masked): its ε region in the
-// pushed forms, then (skipped for an empty call) ε, actions, q and q_max non-null and aligned.
+// pushed forms, then (skipped for an empty call) ε, actions, q and q_max non-null and aligned.  An evaluating entry's
+// own checks come after every check of its counterpart and its nvec: (skipped for an empty call) taken, log_probs,
+// entropy non-null and aligned, then its taken region in the pushed forms.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1386,6 +1605,28 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     KTB_REQUIRE(lo == d_out, KTB_ERR_ARG, "%s: nvec sums to %lld, not d_out=%d", fn, lo, d_out);
     groups.n = p.n_groups;
   }
+  if (p.evaluate) {
+    const bool cat = p.kind == HeadKind::kSample;
+    const void* taken = cat ? (const void*)p.ev.actions : (const void*)p.ev.gauss_actions;
+    const size_t align = cat ? 8 : 4;
+    if (M > 0) {
+      KTB_REQUIRE((taken || f.pushed) && p.out.log_probs && p.ev.entropy, KTB_ERR_ARG,
+                  "%s: taken, log_probs and entropy are required", fn);
+      KTB_REQUIRE((uintptr_t)taken % align == 0, KTB_ERR_ARG, "%s: taken must be %zu-byte aligned", fn, align);
+      KTB_REQUIRE((((uintptr_t)p.out.log_probs | (uintptr_t)p.ev.entropy) & 3) == 0, KTB_ERR_ARG,
+                  "%s: log_probs and entropy must be 4-byte aligned", fn);
+    }
+    if (f.pushed) {
+      const size_t off = f.taken_offset;
+      const size_t n = M * (cat ? 8 * (size_t)std::max(groups.n, 1) : 4 * (size_t)d_out);
+      KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: taken_offset=%zu overlaps the rows", fn, off);
+      KTB_REQUIRE(!p.masked || off >= f.mask_offset + M * (size_t)d_out || off + n <= f.mask_offset, KTB_ERR_ARG,
+                  "%s: taken_offset=%zu overlaps the mask", fn, off);
+      KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG, "%s: taken_offset=%zu + taken exceeds stage_stride",
+                  fn, off);
+      KTB_REQUIRE(off % align == 0, KTB_ERR_ARG, "%s: taken_offset=%zu must be a multiple of %zu", fn, off, align);
+    }
+  }
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
@@ -1402,6 +1643,14 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   HeadEps eg = p.eg;
   if (p.eps && f.pushed)
     eg.epsilon = reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(x) + f.epsilon_offset);
+  HeadEval ev = p.ev;
+  if (p.evaluate && f.pushed) {
+    const uint8_t* t = reinterpret_cast<const uint8_t*>(x) + f.taken_offset;
+    if (p.kind == HeadKind::kSample)
+      ev.actions = reinterpret_cast<const int64_t*>(t);
+    else
+      ev.gauss_actions = reinterpret_cast<const float*>(t);
+  }
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
   cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
@@ -1450,7 +1699,7 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       a1 = dstb;
     }
     // evs[3..4] are null unless staged
-    rc = mlp_chunk(dev, p, out, eg, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
+    rc = mlp_chunk(dev, p, out, eg, ev, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
     if (rc) return rc;
   }
   if (!f.pushed) return KTB_OK;
@@ -1949,6 +2198,169 @@ int ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed(int dev, const void* stage_
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
                      .with_mask_offset(mask_offset)
                      .with_epsilon_offset(epsilon_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                                 const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                                 const int32_t* nvec, int n_groups, const int64_t* taken, float* log_probs,
+                                 float* entropy, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3, b3, nvec, n_groups, taken, log_probs, entropy);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                        int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                        const void* b2, const void* W3, const void* b3, const int32_t* nvec,
+                                        int n_groups, size_t taken_offset, float* log_probs, float* entropy,
+                                        void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                        size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3, b3, nvec, n_groups, nullptr, log_probs, entropy);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_taken_offset(taken_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                       const void* W1, const void* b1, const void* W2, const void* b2, const void* W3v,
+                                       const void* b3v, const int32_t* nvec, int n_groups, const int64_t* taken,
+                                       float* log_probs, float* entropy, float* values, void* scratch, void* stage,
+                                       uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3v, b3v, nvec, n_groups, taken, log_probs, entropy)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_value", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                              int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                              const void* W2, const void* b2, const void* W3v, const void* b3v,
+                                              const int32_t* nvec, int n_groups, size_t taken_offset, float* log_probs,
+                                              float* entropy, float* values, void* scratch, void* ctrl_local,
+                                              void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                              unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3v, b3v, nvec, n_groups, nullptr, log_probs, entropy)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_taken_offset(taken_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                        const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                        const void* b3, const int32_t* nvec, int n_groups, const uint8_t* mask,
+                                        const int64_t* taken, float* log_probs, float* entropy, void* scratch,
+                                        void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::evaluate_categorical(W1, b1, W2, b2, W3, b3, nvec, n_groups, taken, log_probs, entropy)
+                          .with_mask(mask);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_masked", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                               int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                               const void* W2, const void* b2, const void* W3, const void* b3,
+                                               const int32_t* nvec, int n_groups, size_t mask_offset,
+                                               size_t taken_offset, float* log_probs, float* entropy, void* scratch,
+                                               void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                               unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3, b3, nvec, n_groups, nullptr, log_probs, entropy)
+                          .with_mask(nullptr);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset)
+                     .with_taken_offset(taken_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_masked_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                              const void* W1, const void* b1, const void* W2, const void* b2,
+                                              const void* W3v, const void* b3v, const int32_t* nvec, int n_groups,
+                                              const uint8_t* mask, const int64_t* taken, float* log_probs,
+                                              float* entropy, float* values, void* scratch, void* stage,
+                                              uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3v, b3v, nvec, n_groups, taken, log_probs, entropy)
+                          .with_mask(mask)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_masked_value", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_evaluate_masked_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                     int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                     const void* W2, const void* b2, const void* W3v, const void* b3v,
+                                                     const int32_t* nvec, int n_groups, size_t mask_offset,
+                                                     size_t taken_offset, float* log_probs, float* entropy,
+                                                     float* values, void* scratch, void* ctrl_local,
+                                                     void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                                     unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::evaluate_categorical(W1, b1, W2, b2, W3v, b3v, nvec, n_groups, nullptr, log_probs, entropy)
+                          .with_mask(nullptr)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_evaluate_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_mask_offset(mask_offset)
+                     .with_taken_offset(taken_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_evaluate(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                          const void* W1, const void* b1, const void* W2, const void* b2,
+                                          const void* W3, const void* b3, const float* log_std, const float* taken,
+                                          float* log_probs, float* entropy, void* scratch, void* stage,
+                                          uintptr_t stream) {
+  const MlpParams p = MlpParams::evaluate_gaussian(W1, b1, W2, b2, W3, b3, log_std, taken, log_probs, entropy);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_evaluate", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_evaluate_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                 int d_in, int d_hidden, int d_out, const void* W1, const void* b1,
+                                                 const void* W2, const void* b2, const void* W3, const void* b3,
+                                                 const float* log_std, size_t taken_offset, float* log_probs,
+                                                 float* entropy, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                                 int rank, size_t chunk_rows, unsigned long long seq,
+                                                 uintptr_t stream) {
+  const MlpParams p = MlpParams::evaluate_gaussian(W1, b1, W2, b2, W3, b3, log_std, nullptr, log_probs, entropy);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_evaluate_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_taken_offset(taken_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_evaluate_value(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                                const void* W1, const void* b1, const void* W2, const void* b2,
+                                                const void* W3v, const void* b3v, const float* log_std,
+                                                const float* taken, float* log_probs, float* entropy, float* values,
+                                                void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::evaluate_gaussian(W1, b1, W2, b2, W3v, b3v, log_std, taken, log_probs, entropy)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_evaluate_value", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M,
+                                                       int d_in, int d_hidden, int d_out, const void* W1,
+                                                       const void* b1, const void* W2, const void* b2, const void* W3v,
+                                                       const void* b3v, const float* log_std, size_t taken_offset,
+                                                       float* log_probs, float* entropy, float* values, void* scratch,
+                                                       void* ctrl_local, void* ctrl_root_peer, int rank,
+                                                       size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::evaluate_gaussian(W1, b1, W2, b2, W3v, b3v, log_std, nullptr, log_probs, entropy)
+                          .with_values(values);
+  return mlp_run("ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_taken_offset(taken_offset),
                  scratch, stream);
 }
 

@@ -188,6 +188,19 @@ for _masked in ("", "_masked"):
         _at += bool(_masked)
         _SIGNATURES["ktb_mlp_bf16_policy_epsilon_greedy" + _masked + _form] = (
             _restype, _args[:_at] + [_eps] + _args[_at:_at + 4] + [c_void_p] + _args[_at + 4:])
+# The _evaluate entries: ktb_mlp_bf16_policy's arguments up to b3 (the first 12 of the plain and staged forms, 13 of
+# the pushed ones), then (nvec, n_groups, [mask,] taken, log_probs, entropy, [values,]) with (mask_offset,) taken_offset
+# in the pushed forms; the _gaussian_evaluate ones take log_std in place of (nvec, n_groups, [mask,]).
+for _masked in ("", "_masked"):
+    for _valued in ("", "_value"):
+        for _form, _in, _at in (("", c_void_p, 12), ("_pushed", c_size_t, 13)):
+            _args = _SIGNATURES["ktb_mlp_bf16_policy" + _form][1]
+            _head_args = [POINTER(ctypes.c_int32), c_int] + [_in] * (1 + bool(_masked)) + [c_void_p] * (2 + bool(_valued))
+            _SIGNATURES["ktb_mlp_bf16_policy_evaluate" + _masked + _valued + _form] = (
+                c_int, _args[:_at] + _head_args + _args[_at + 2:])
+            if not _masked:
+                _SIGNATURES["ktb_mlp_bf16_policy_gaussian_evaluate" + _valued + _form] = (
+                    c_int, _args[:_at] + [c_void_p, _in] + [c_void_p] * (2 + bool(_valued)) + _args[_at + 2:])
 _SIGNATURES["ktb_push_scatter_ce_sides"] = (
     c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
                                                          ctypes.c_ulonglong, c_uintptr])

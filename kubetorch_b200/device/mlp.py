@@ -4,8 +4,8 @@ Gumbel-max actions with their log-probabilities, kubetorch_b200.sampling), ktb_m
 diagonal-Gaussian actions with their log-probabilities), the _masked forms of the first two (a per-row legal-action
 mask), the _value forms of the sampled heads (a critic's state value on the same trunk), the _multidiscrete forms of
 the greedy and sampled heads (one categorical per group of columns), the _gaussian_state forms (a per-row log-std
-head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network's ε-greedy actor) and their
-scatter→exec→gather form."""
+head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network's ε-greedy actor), the _evaluate
+and _gaussian_evaluate forms (the log-probability and entropy of given actions) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -18,7 +18,7 @@ import torch
 from . import lib as L
 from . import ops
 from ..mapped import MLP_OUTPUTS as OUTPUTS
-from ..mapped import check_nvec
+from ..mapped import EVALUATE_OUTPUTS, check_nvec
 from ..sampling import _check_seed
 
 _scratch = {}
@@ -67,8 +67,9 @@ LOG_STD_BOUNDS = (-20.0, 2.0)   # SB3's and Spinning Up's clamp of a SAC actor's
 def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
     """_check_policy's checks of a value head (wv, bv), in this order: the output, the pair, the head width, bv given
     exactly when b3 is, then wv's dtype and shape, layout and device, then bv."""
-    if output not in ("sample", "gaussian"):
-        raise ValueError(f'value is an argument of output="sample" and "gaussian", not of output={output!r}')
+    if output not in ("sample", "gaussian") + EVALUATE_OUTPUTS:
+        raise ValueError(f'value is an argument of output="sample" and "gaussian" (and "evaluate" and '
+                         f'"gaussian_evaluate"), not of output={output!r}')
     if not isinstance(value, (tuple, list)) or len(value) != 2:
         raise ValueError("value must be (wv, bv): the critic's weight [1, d_hidden] and its bias [1] or None")
     wv, bv = value
@@ -150,8 +151,32 @@ def _check_epsilon(epsilon, obs) -> None:
         raise ValueError("epsilon must not be NaN (a NaN float never explores: pass 0.0 for that)")
 
 
+def _check_taken(taken, output, obs, d_out, nvec) -> None:
+    """_check_policy's checks of an evaluate output's given actions `taken`, in this order: given; the dtype and shape
+    (int64 [M], [M, len(nvec)] with nvec, for "evaluate"; float32 [M, d_out] for "gaussian_evaluate"; obs [M, d_in]);
+    contiguous; a CUDA tensor on the device of obs."""
+    if taken is None:
+        raise ValueError(f"taken is required with output={output!r}: the actions to evaluate")
+    if not isinstance(taken, torch.Tensor):
+        raise ValueError(f"taken must be a tensor, got {type(taken).__name__}")
+    if not isinstance(obs, torch.Tensor):
+        raise ValueError("taken is checked against obs: pass the obs [M, d_in] it goes with")
+    M = obs.shape[0]
+    if output == "gaussian_evaluate":
+        dtype, shape = torch.float32, (M, d_out)
+    else:
+        dtype, shape = torch.int64, (M,) if nvec is None else (M, len(nvec))
+    if taken.dtype != dtype or tuple(taken.shape) != shape:
+        raise ValueError(f"taken must be a {str(dtype).replace('torch.', '')} tensor of shape {shape}, got "
+                         f"{str(taken.dtype).replace('torch.', '')} {tuple(taken.shape)}")
+    if not taken.is_contiguous():
+        raise ValueError("taken must be contiguous")
+    if not taken.is_cuda or taken.device != obs.device:
+        raise ValueError(f"taken must be a CUDA tensor on the device of obs ({obs.device}), got {taken.device}")
+
+
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
-                  nvec=None, log_std_bounds=None, squash=None, epsilon=None) -> None:
+                  nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
     (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
@@ -162,17 +187,30 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     tuple or list of ints >= 1 that sums to d_out (mapped.check_nvec).  With output="gaussian", log_std may instead
     be a state-dependent head (w_ls, b_ls) (_check_state_std), and log_std_bounds and squash are taken with that form
     only.  output="epsilon_greedy" takes a seed and an epsilon (_check_epsilon), and epsilon is refused with any other
-    output; its value=, nvec= and log_std= are refused by the checks of those options."""
+    output; its value=, nvec= and log_std= are refused by the checks of those options.  output="evaluate" and
+    "gaussian_evaluate" take the actions to score, `taken` (_check_taken), refused with any other output; they refuse
+    a seed, epsilon, squash, log_std_bounds and a log_std pair, and "gaussian_evaluate" a mask."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
+    evaluate = output in EVALUATE_OUTPUTS
+    if evaluate:
+        for name, v in (("seed", seed), ("epsilon", epsilon), ("squash", squash), ("log_std_bounds", log_std_bounds)):
+            if v is not None:
+                raise ValueError(f"{name} is not an argument of output={output!r}: evaluating given actions draws no "
+                                 f"noise")
+        if isinstance(log_std, (tuple, list)):
+            raise ValueError('output="gaussian_evaluate" takes a state-independent log_std tensor, not a log_std=(w_ls, '
+                             'b_ls) pair (evaluating a state-dependent or squashed head is not supported)')
+    elif taken is not None:
+        raise ValueError(f'taken is an argument of output="evaluate" and "gaussian_evaluate", not of output={output!r}')
     if output in ("sample", "gaussian", "epsilon_greedy"):
         _check_seed(seed)
     if output == "epsilon_greedy":
         _check_epsilon(epsilon, obs)
     elif epsilon is not None:
         raise ValueError(f'epsilon is an argument of output="epsilon_greedy", not of output={output!r}')
-    if mask is not None and output == "gaussian":
-        raise ValueError('mask is an argument of the categorical outputs, not of output="gaussian"')
+    if mask is not None and output in ("gaussian", "gaussian_evaluate"):
+        raise ValueError(f'mask is an argument of the categorical outputs, not of output={output!r}')
     if len(biases) != 3:
         raise ValueError("biases must be (b1, b2, b3), each a tensor or None")
     d_hidden, d_out = w1.shape[0], w3.shape[0]
@@ -180,14 +218,17 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
         raise ValueError(f"d_out={d_out}: the policy head is 1 to {MAX_D_OUT} wide")
     if nvec is not None:
         check_nvec(nvec, output, d_out)
+    if evaluate:
+        _check_taken(taken, output, obs, d_out, nvec)
     state = isinstance(log_std, (tuple, list))
-    if output != "gaussian" and log_std is not None:
-        raise ValueError('log_std is an argument of output="gaussian" only')
+    gaussian = output in ("gaussian", "gaussian_evaluate")
+    if not gaussian and log_std is not None:
+        raise ValueError('log_std is an argument of output="gaussian" only (and of "gaussian_evaluate")')
     if not state and (log_std_bounds is not None or squash is not None):
         raise ValueError("log_std_bounds and squash are options of a state-dependent log_std=(w_ls, b_ls) only")
     if output == "gaussian" and state:
         _check_state_std(log_std, log_std_bounds, squash, w3, biases[2], d_hidden, d_out, value is not None)
-    elif output == "gaussian" and (not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32
+    elif gaussian and (not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32
                                    or not log_std.is_cuda or not log_std.is_contiguous() or log_std.dim() != 1
                                    or log_std.shape[0] != d_out):
         raise ValueError(f"log_std must be a 1-D contiguous CUDA float32 tensor of length {d_out}")
@@ -250,7 +291,8 @@ def _stacked_head(w3, b3, wv=None, bv=None, w_ls=None, b_ls=None) -> Tuple[torch
 def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False, nvec=None):
     """(logits, actions, log_probs, values) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions
     [M], [M, len(nvec)] with nvec, or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values
-    [M].  With "epsilon_greedy" the last two slots hold its fp32 q [M] and q_max [M].  A buffer the mode does not
+    [M].  With "epsilon_greedy" the last two slots hold its fp32 q [M] and q_max [M]; with "evaluate" and
+    "gaussian_evaluate" the actions slot holds the fp32 entropy [M].  A buffer the mode does not
     write is None, a missing one is allocated on `device` and a given one is
     registered with the library (ops.ensure_init); given multi-discrete actions must be [M, len(nvec)]."""
     def buf(t, shape, dtype):
@@ -260,6 +302,9 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
         return t
 
     gaussian = output == "gaussian"
+    if output in EVALUATE_OUTPUTS:
+        return None, buf(actions, (M,), torch.float32), buf(log_probs, (M,), torch.float32), \
+            buf(values, (M,), torch.float32) if valued else None
     if nvec is not None and actions is not None and tuple(actions.shape) != (M, len(nvec)):
         raise ValueError(f"actions must have shape ({M}, {len(nvec)}) with nvec of {len(nvec)} groups, got "
                          f"{tuple(actions.shape)}")
@@ -272,7 +317,7 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
 
 
 def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None,
-          nvec=None, std=None, epsilon=None):
+          nvec=None, std=None, epsilon=None, taken=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
     mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
@@ -280,7 +325,18 @@ def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, push
     picks the _multidiscrete entry and is its group sizes.  `std` = (log_std_min, log_std_max, squash), unless None,
     picks the _gaussian_state entry (whose W3 and b3 are the interleaved head) in place of log_std.  With
     "epsilon_greedy", `epsilon` is ε's address (pull forms) or its offset in the staging half (pushed forms), and
-    log_probs and values are its q and q_max buffers."""
+    log_probs and values are its q and q_max buffers.  With "evaluate" and "gaussian_evaluate", `taken` is the given
+    actions' address or offset likewise, and `actions` is the entropy buffer."""
+    valued = () if values is None else (ptr(values),)
+    pushed_suffix = "_pushed" if pushed else ""
+    if output == "gaussian_evaluate":
+        return "ktb_mlp_bf16_policy_gaussian_evaluate" + ("" if values is None else "_value") + pushed_suffix, \
+            (ptr(log_std), taken, ptr(log_probs), ptr(actions), *valued)
+    if output == "evaluate":
+        groups = (None, 0) if nvec is None else (L.arr(ctypes.c_int32, nvec), len(nvec))
+        return "ktb_mlp_bf16_policy_evaluate" + ("" if mask is None else "_masked") + \
+            ("" if values is None else "_value") + pushed_suffix, \
+            (*groups, *(() if mask is None else (mask,)), taken, ptr(log_probs), ptr(actions), *valued)
     eps = output == "epsilon_greedy"
     suffix = ("" if nvec is None else "_multidiscrete") + ("" if mask is None else "_masked") + \
         ("" if values is None or eps else "_value") + ("_pushed" if pushed else "")
@@ -323,6 +379,8 @@ def _result(output, logits, actions, log_probs, values=None):
         return actions
     if output == "both":
         return logits, actions
+    if output in EVALUATE_OUTPUTS:   # the entropy rides in the actions slot
+        return (log_probs, actions) if values is None else (log_probs, actions, values)
     return (actions, log_probs) if values is None else (actions, log_probs, values)
 
 
@@ -336,6 +394,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 values: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
                 log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
                 epsilon=None, q: Optional[torch.Tensor] = None, q_max: Optional[torch.Tensor] = None,
+                taken: Optional[torch.Tensor] = None, entropy: Optional[torch.Tensor] = None,
                 _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
@@ -372,7 +431,15 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     epsilon[i] in fp32 and then takes the legal column with the largest w (ties to the lower column), and otherwise
     the argmax of its (masked) logits; q is the fp32 (masked) logit of the action taken and q_max that of the argmax,
     into `q` and `q_max` when given; no logits are written.  `epsilon` is a CUDA float32 tensor [M] on the device of
-    obs or a number broadcast to every row (rounded to fp32; NaN refused).  `_stacked` (internal, from
+    obs or a number broadcast to every row (rounded to fp32; NaN refused).  output="evaluate" (masked, multi-discrete
+    and with a value head as "sample" takes them) and "gaussian_evaluate" (with a tensor log_std, and a value head)
+    score the actions `taken` on the device of obs (int64 [M], [M, len(nvec)] with nvec, of group-relative indices; fp32
+    [M, d_out] for the Gaussian) and return (log_probs, entropy), or (log_probs, entropy, values) with a value head,
+    into `log_probs`, `entropy` and `values` when given: fp32 log_probs[i] = sum_g log_softmax(group_g)[a_g] of the
+    (masked) logits and entropy[i] = sum_g entr(softmax(group_g)).sum(), or Normal(logits, exp(log_std))'s
+    log_prob(taken).sum(-1) and entropy().sum(-1); an action out of range gives a NaN row (it is not checked, which
+    would need a host synchronisation), an illegal one -inf.  No noise is drawn and no logits are written.
+    `_stacked` (internal, from
     mlp_scatter_gather, which checked the call): w3 and biases[2] are
     already the head the C entry takes (stacked with a value head, interleaved with a log-std head)."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
@@ -385,7 +452,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
     if not _stacked:
-        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon)
+        _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon,
+                      taken)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     valued = value is not None or (_stacked and values is not None)
     if _stacked:
@@ -396,6 +464,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     eps = output == "epsilon_greedy"
     if eps:   # q and q_max ride in the log_probs and values slots
         log_probs, values = q, q_max
+    if output in EVALUATE_OUTPUTS:   # the entropy rides in the actions slot
+        actions = entropy
     out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued,
                                                nvec)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
@@ -411,7 +481,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
                         mask=None if mask is None else ptr(mask), values=values, nvec=nvec, std=std,
-                        epsilon=ptr(epsilon) if eps else None)
+                        epsilon=ptr(epsilon) if eps else None, taken=ptr(taken))
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
@@ -444,7 +514,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
                                seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None,
-                               epsilon=None) -> None:
+                               epsilon=None, taken=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -459,7 +529,9 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     (_std) picks every rank's _gaussian_state entry, weights[dev] then holding the interleaved head.  With
     output="epsilon_greedy", `epsilon` is the fp32 [M] on the root, pushed with the rows like the mask: each staging
     half is rows | mask | ε, each 256-byte aligned (ktb_push_scatter_ce_sides), and log_probs_root / values_root are
-    its q and q_max."""
+    its q and q_max.  With output="evaluate" or "gaussian_evaluate", `taken` (on the root) is pushed with the rows the
+    same way, each staging half rows | mask | taken with taken's offset rounded up to 8 bytes, and actions_root is the
+    entropy."""
     root, n, key = devs[0], len(devs), tuple(devs)
     valued = values_root is not None and epsilon is None   # an ε-greedy head's values_root is its q_max
     d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
@@ -471,6 +543,11 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     if epsilon is not None:
         eps_offset = mask_offset if mask is None else (mask_offset + rows * d_out + 255) // 256 * 256
         stage_bytes = eps_offset + rows * 4
+    taken_offset = None
+    if taken is not None:
+        taken_row = taken[0].numel() * taken.element_size() if taken.dim() > 1 else taken.element_size()
+        taken_offset = (stage_bytes + 7) // 8 * 8
+        stage_bytes = taken_offset + rows * taken_row
     sess = _push_sessions.get(key)
     if sess is None or sess.stride < stage_bytes:
         sess = _push_sessions[key] = ops.PushSession(devs, stage_bytes)
@@ -496,11 +573,14 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
                     values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
                     squash=None if std is None else bool(std[2]),
                     **({} if epsilon is None else dict(epsilon=epsilon[b0:e0], q=log_probs, q_max=values)),
+                    **({} if taken is None else dict(taken=taken[b0:e0], entropy=actions)),
                     _stacked=valued or std is not None)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
-    if epsilon is not None:
-        sides = ([] if mask is None else [(mask.data_ptr(), d_out, mask_offset)]) + [(epsilon.data_ptr(), 4, eps_offset)]
+    if epsilon is not None or taken is not None:
+        last = (epsilon.data_ptr(), 4, eps_offset) if epsilon is not None else \
+            (taken.data_ptr(), taken_row, taken_offset)
+        sides = ([] if mask is None else [(mask.data_ptr(), d_out, mask_offset)]) + [last]
         src, row_bytes, offsets = zip(*sides)
         L.call("ktb_push_scatter_ce_sides", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, *scatter,
                len(sides), L.arr(ctypes.c_void_p, src), L.arr(ctypes.c_size_t, row_bytes),
@@ -520,7 +600,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         entry, head = _head(output, logits, actions, log_probs, seed, b,
                             None if log_std is None else log_std[devs[r]], ptr, pushed=True,
                             mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std,
-                            epsilon=eps_offset)
+                            epsilon=eps_offset, taken=taken_offset)
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -537,7 +617,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        mask: Optional[torch.Tensor] = None, value: Optional[Sequence[Optional[torch.Tensor]]] = None,
                        values_root: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
                        log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
-                       epsilon=None) -> list:
+                       epsilon=None, taken: Optional[torch.Tensor] = None,
+                       entropy_root: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -552,17 +633,23 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     A state-dependent log_std = (w_ls, b_ls), with `log_std_bounds` and `squash`, as in mlp_forward: the interleaved
     head is built on the root and copied to the other devices like the other weights.  output="epsilon_greedy" with
     `epsilon` (a float, or an fp32 [M] on the root) as in mlp_forward returns (actions, q, q_max) triples; each rank
-    reads its rows of ε in place on the pull form, and the push form pushes them with the rows."""
+    reads its rows of ε in place on the pull form, and the push form pushes them with the rows.  output="evaluate" and
+    "gaussian_evaluate" with `taken` on the root as in mlp_forward return (log_probs, entropy) pairs, or triples with
+    a value head, into `log_probs_root`, `entropy_root` and `values_root` when given; each rank reads its rows of taken
+    in place on the pull form, and the push form pushes them with the rows."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
-    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon)
+    _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon,
+                  taken)
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     if output == "epsilon_greedy" and not isinstance(epsilon, torch.Tensor):   # before `ready`: every rank reads it
         epsilon = torch.full((M,), float(epsilon), dtype=torch.float32, device=obs_root.device)
     valued = value is not None
+    if taken is not None:   # the entropy rides in the actions slot
+        actions_root = entropy_root
     bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
                     valued, nvec)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
@@ -588,7 +675,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec, std, epsilon)
+                                   nvec, std, epsilon, taken)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -614,6 +701,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                         values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
                         squash=None if std is None else bool(std[2]),
                         **({} if epsilon is None else dict(epsilon=epsilon[b:e], q=log_probs, q_max=values)),
+                        **({} if taken is None else dict(taken=taken[b:e], entropy=actions)),
                         _stacked=valued or std is not None)
             if dev != root:
                 ev = torch.cuda.Event()

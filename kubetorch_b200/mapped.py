@@ -23,7 +23,9 @@ from typing import Any, Callable, Dict, Optional
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
-MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy")   # also device.mlp.OUTPUTS
+MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
+               "gaussian_evaluate")   # also device.mlp.OUTPUTS
+EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
 
 
 @dataclass
@@ -98,22 +100,39 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     tensor [M] on the device of obs (the body takes ``eps.chunk(WORLD_SIZE)[RANK]`` of a tensor): with ``u, w =
     kubetorch_b200.sampling.explore_noise(seed, row0, rows, d_out)`` a row explores iff ``u < ε`` and takes the legal
     column with the largest ``w``, and otherwise the argmax of its logits; ``q`` is the fp32 logit of the action taken
-    and ``q_max`` that of the argmax (``mask=`` applies, ``value=`` and ``nvec=`` do not)."""
+    and ``q_max`` that of the argmax (``mask=`` applies, ``value=`` and ``nvec=`` do not).
+    ``output="evaluate"`` and ``"gaussian_evaluate"`` score actions the caller already holds (SB3's
+    ``evaluate_actions``): ``taken=`` names the call argument that holds them, int64 ``[M]`` (``[M, G]`` with
+    ``nvec=``) group-relative indices, or fp32 ``[M, d_out]`` with ``"gaussian_evaluate"``, on the device of obs (the
+    body takes ``taken.chunk(WORLD_SIZE)[RANK]``).  Each rank returns ``(log_probs, entropy)``, or ``(log_probs,
+    entropy, values)`` with ``value=``: the fp32 log-probability of each row's action and the entropy of its policy,
+    summed over groups, under ``logits.masked_fill(~mask, -inf)`` (``"evaluate"``; ``mask=`` and ``nvec=`` apply) or
+    ``Normal(logits, exp(log_std))`` (``"gaussian_evaluate"``, with ``log_std=`` naming one argument).  They draw no
+    noise, so ``seed=``, ``epsilon=``, ``squash=``, ``log_std_bounds=`` and a ``log_std`` pair are refused."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
     if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
-                                "squash", "epsilon")):
+                                "squash", "epsilon", "taken")):
         if op != "mlp":
-            raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value=, nvec= and "
-                             f"epsilon= are options of the 'mlp' op, not of '{op}'")
+            raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value=, nvec=, "
+                             f"epsilon= and taken= are options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
         sample = extra.get("output") in ("sample", "gaussian")
         eps = extra.get("output") == "epsilon_greedy"
+        evaluate = extra.get("output") in EVALUATE_OUTPUTS
+        if evaluate != ("taken" in extra):
+            raise ValueError('taken= is required with output="evaluate" and "gaussian_evaluate" and is an option of '
+                             'those outputs only')
+        if evaluate and not isinstance(extra["taken"], str):
+            raise ValueError(f"taken must be the name of a call argument, got {extra['taken']!r}")
+        if evaluate and "seed" in extra:
+            raise ValueError(f'seed= is not an option of output={extra["output"]!r}: evaluating given actions draws '
+                             f'no noise')
         if (sample or eps) != ("seed" in extra):
             raise ValueError('seed= is required with output="sample" or "gaussian" (or "epsilon_greedy") and is an '
                              'option of those only')
@@ -121,10 +140,14 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
             from .sampling import _check_seed
 
             _check_seed(extra["seed"])
-        gaussian = extra.get("output") == "gaussian"
+        gaussian = extra.get("output") in ("gaussian", "gaussian_evaluate")
         if gaussian != ("log_std" in extra):
-            raise ValueError('log_std= is required with output="gaussian" and is an option of that output only')
+            raise ValueError('log_std= is required with output="gaussian" (and "gaussian_evaluate") and is an option of '
+                             'those outputs only')
         state = gaussian and isinstance(extra["log_std"], (tuple, list))
+        if state and evaluate:
+            raise ValueError('output="gaussian_evaluate" takes a state-independent log_std (the name of one call '
+                             'argument), not a log_std=(w_ls, b_ls) pair')
         if state:
             ls = extra["log_std"]
             if len(ls) != 2 or not all(isinstance(n, str) for n in ls):
@@ -150,12 +173,13 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
             raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
         if "mask" in extra:
             if gaussian:
-                raise ValueError('mask= is an option of the categorical outputs, not of output="gaussian"')
+                raise ValueError(f'mask= is an option of the categorical outputs, not of output={extra["output"]!r}')
             if not isinstance(extra["mask"], str):
                 raise ValueError(f"mask must be the name of a call argument, got {extra['mask']!r}")
         if "value" in extra:
-            if not sample:
-                raise ValueError('value= is an option of output="sample" and "gaussian" only')
+            if not (sample or evaluate):
+                raise ValueError('value= is an option of output="sample", "gaussian", "evaluate" and '
+                                 '"gaussian_evaluate" only')
             if not extra.get("bias", False):
                 raise ValueError("value= needs bias=True: the critic's bias is given exactly when b3 is")
             v = extra["value"]
@@ -174,7 +198,7 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
 
     def deco(fn):
         params = inspect.signature(fn).parameters
-        for option in ("log_std", "mask", "value", "epsilon"):
+        for option in ("log_std", "mask", "value", "epsilon", "taken"):
             names = extra.get(option)
             if option == "epsilon" and not isinstance(names, str):   # a constant ε names no argument
                 continue
@@ -189,11 +213,12 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
 
 
 def check_nvec(nvec, output: str, d_out: Optional[int] = None) -> tuple:
-    """nvec as a tuple, or ValueError naming what is wrong with it: given with an output other than "actions", "both"
-    and "sample"; not a tuple or list of ints (bools refused); empty; an entry below 1; (with d_out) a sum other than
-    d_out."""
-    if output not in ("actions", "both", "sample"):
-        raise ValueError(f'nvec is an option of output="actions", "both" and "sample", not of output={output!r}')
+    """nvec as a tuple, or ValueError naming what is wrong with it: given with an output other than "actions", "both",
+    "sample" and "evaluate"; not a tuple or list of ints (bools refused); empty; an entry below 1; (with d_out) a sum
+    other than d_out."""
+    if output not in ("actions", "both", "sample", "evaluate"):
+        raise ValueError(f'nvec is an option of output="actions", "both", "sample" and "evaluate", not of '
+                         f'output={output!r}')
     if not isinstance(nvec, (tuple, list)) or not all(isinstance(n, int) and not isinstance(n, bool) for n in nvec):
         raise ValueError(f"nvec must be a tuple of ints, got {nvec!r}")
     if len(nvec) == 0:

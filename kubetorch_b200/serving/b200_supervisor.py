@@ -599,12 +599,17 @@ class B200Supervisor:
             if epsilon not in bound:
                 raise TypeError(f"mapped mlp callable: epsilon argument '{epsilon}' not found in the call")
             epsilon = bound[epsilon]
+        taken = spec.extra.get("taken")
+        if taken is not None:   # always the name of a call argument (the whole batch's actions), resolved per call
+            if taken not in bound:
+                raise TypeError(f"mapped mlp callable: taken argument '{taken}' not found in the call")
+            taken = bound[taken]
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
                                          value=value, nvec=spec.extra.get("nvec"),
                                          log_std_bounds=spec.extra.get("log_std_bounds"),
-                                         squash=spec.extra.get("squash"), epsilon=epsilon)
+                                         squash=spec.extra.get("squash"), epsilon=epsilon, taken=taken)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -35,6 +35,11 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      output="actions" and output="sample" at the same d_out and mask; and the eager arm, what a user pays without the
      fused head: the logits entry (masked in torch under a mask), then argmax, the exploration draws of explore_noise,
      where and two gathers in torch.
+  n  evaluating given actions (output="evaluate" and "gaussian_evaluate"): the categorical head at d_out 18, 64 and
+     256, the masked MicroRTS nvec (6, 4, 4, 4, 4, 7, 49) with a value head, and the Gaussian head at d_out 6 and 17,
+     each scoring the actions of the matching sampling call and timed beside it; and the eager arm, what a user pays
+     without the evaluating head: the logits entry, then mask, split, log_softmax, gather, softmax and entr (or
+     Normal.log_prob and entropy) in torch.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -50,7 +55,10 @@ legal.  State-dependent rows: on 2048 consecutive rows, the unsquashed actions a
 2^-23·|μ| of μ + σ·z (μ and ℓ the kernel's logits over the interleaved head, σ = exp(clamp(ℓ))), the squashed actions
 within 2 ulp of tanh of the unsquashed ones, and on every row both the actions and log-probabilities are within rtol
 1e-4, atol 1e-4 of the eager arm's.  ε-greedy rows: actions, q and q_max equal the eager arm's on every row, bit for
-bit.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+bit.  Evaluating rows: the categorical log-probabilities of the sampled actions equal the sampling call's on every row,
+bit for bit (NaN in the same rows), its values too; log-probabilities and entropies are within rtol 1e-4, atol 1e-4 of
+the eager arm's (the Gaussian's log-probabilities within rtol 1e-4, atol 1e-3 of the sampling call's), and the values
+within rtol 2^-7, atol 1e-2 of the eager critic's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -286,6 +294,53 @@ def main():
                     obs, w1, w2, heads[d][0], biases=bs, output="epsilon_greedy", seed=SEED, epsilon=eps, **m))
                 variants[f"m_bias_{tag}epsilon{eps}_eager_d{d}"] = (
                     d, lambda d=d, mask=mask, eps=eps: eager_epsilon(d, mask, eps))
+    def eager_evaluate(d, taken, mask=None, nvec=None, value=None):
+        """The logits entry, then the evaluation in torch: what a user pays without output="evaluate"."""
+        y = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]))
+        if mask is not None:
+            y = y.masked_fill(~mask, float("-inf"))
+        parts = y.float().split(list(nvec or (d,)), -1)
+        a = taken if nvec else taken[:, None]
+        lp = sum(q.log_softmax(-1).gather(-1, a[:, g:g + 1])[:, 0] for g, q in enumerate(parts))
+        ent = sum(torch.special.entr(q.softmax(-1)).sum(-1) for q in parts)
+        if value is None:
+            return lp, ent
+        h = torch.relu(F.linear(torch.relu(F.linear(obs, w1, b1)), w2, b2))
+        return lp, ent, F.linear(h, *value).float().squeeze(-1)
+
+    def eager_gaussian_evaluate(d, taken):
+        mu = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1])).float()
+        dist = torch.distributions.Normal(mu, log_stds[d].exp())
+        return dist.log_prob(taken).sum(-1), dist.entropy().sum(-1)
+
+    evaluate_cases = {}
+    for d in (18, 64, 256):
+        bs = (b1, b2, heads[d][1])
+        taken = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=bs, output="sample", seed=SEED)[0]
+        evaluate_cases[f"d{d}"] = (d, "sample", dict(output="sample", seed=SEED),
+                                   dict(output="evaluate", taken=taken), lambda d=d, t=taken: eager_evaluate(d, t))
+    nv = nvecs[78]
+    kw78 = dict(mask=legal[78], nvec=nv, value=critic)
+    taken = mlp.mlp_forward(obs, w1, w2, heads[78][0], biases=(b1, b2, heads[78][1]), output="sample", seed=SEED,
+                            **kw78)[0]
+    evaluate_cases["masked_nvec_value_d78"] = (78, "sample", dict(output="sample", seed=SEED, **kw78),
+                                               dict(output="evaluate", taken=taken, **kw78),
+                                               lambda t=taken: eager_evaluate(78, t, legal[78], nv, critic))
+    for d in (6, 17):
+        log_stds.setdefault(d, torch.linspace(-2.0, 0.5, d, device="cuda:0"))
+        bs = (b1, b2, heads[d][1])
+        taken = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=bs, output="gaussian", seed=SEED,
+                                log_std=log_stds[d])[0]
+        evaluate_cases[f"gaussian_d{d}"] = (d, "gaussian", dict(output="gaussian", seed=SEED, log_std=log_stds[d]),
+                                            dict(output="gaussian_evaluate", taken=taken, log_std=log_stds[d]),
+                                            lambda d=d, t=taken: eager_gaussian_evaluate(d, t))
+    for tag, (d, sampled, kw_s, kw_e, eager) in evaluate_cases.items():
+        bs = (b1, b2, heads[d][1])
+        variants[f"n_bias_{sampled}_{tag}"] = (d, lambda d=d, bs=bs, kw=kw_s: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, **kw))
+        variants[f"n_bias_evaluate_{tag}"] = (d, lambda d=d, bs=bs, kw=kw_e: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, **kw))
+        variants[f"n_bias_evaluate_eager_{tag}"] = (d, eager)
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -453,6 +508,26 @@ def main():
                 entry[f"{tag}epsilon{eps}_eq_eager_all_rows"] = "ok"
                 del got, want
         parity[f"m_bias_epsilon_d{d}"] = entry
+
+    for tag, (d, sampled, _, _, _) in evaluate_cases.items():
+        drawn = variants[f"n_bias_{sampled}_{tag}"][1]()
+        got = variants[f"n_bias_evaluate_{tag}"][1]()
+        want = variants[f"n_bias_evaluate_eager_{tag}"][1]()
+        if sampled == "sample":
+            lp, ref = got[0], drawn[1]
+            nan = lp.isnan()
+            assert torch.equal(nan, ref.isnan()) and torch.equal(lp[~nan].view(torch.int32),
+                                                                 ref[~nan].view(torch.int32)), tag
+            if len(got) == 3:
+                assert torch.equal(got[2].view(torch.int32), drawn[2].view(torch.int32)), tag
+        else:
+            assert torch.allclose(got[0], drawn[1], rtol=1e-4, atol=1e-3), tag
+        for g_, w_ in zip(got[:2], want[:2]):
+            assert torch.allclose(g_, w_, rtol=1e-4, atol=1e-4, equal_nan=True), tag
+        if len(got) == 3:   # the eager critic is a different GEMM: the value rows' bar
+            assert torch.allclose(got[2], want[2], rtol=2.0 ** -7, atol=1e-2), tag
+        parity[f"n_bias_evaluate_{tag}"] = "ok"
+        del drawn, got, want
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
