@@ -836,6 +836,40 @@ int ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed(int dev, const void* stag
                                                        void* ctrl_root_peer, int rank, size_t chunk_rows,
                                                        unsigned long long seq, uintptr_t stream);
 
+/* Deterministic actor (TD3, DDPG): tanh(mu) with seeded, clipped Gaussian noise, fused into the head.  ktb_mlp_bf16_policy's
+ * arguments up to b3, then (noise, noise_clip, squash, seed, row_base, actions).  It stores no logits and no
+ * log-probabilities.
+ *   - mu_ij is the bf16-rounded head output (ktb_mlp_bf16_policy's logits), t = tanhf(mu) when squash != 0, mu widened
+ *     to fp32 otherwise.
+ *   - noise (sigma) != 0: z_ij is the noise of ktb_mlp_bf16_policy_gaussian (Philox word j & 1 of counter
+ *     (i, j >> 1, 1), i = row_base + row), n = __fmul_rn(sigma, z) clamped to [-noise_clip, noise_clip] by comparisons,
+ *     and t = __fadd_rn(t, n).  noise == 0 draws no Philox word and adds nothing.
+ *   - actions[i, j] (fp32 [M, d_out], 4 bytes per column; may be a peer pointer) = t clamped to [-1, 1] by comparisons
+ *     when squash != 0, t otherwise.  Exploration is noise = sigma with noise_clip = +inf; TD3's target policy
+ *     smoothing is noise = 0.2, noise_clip = 0.5; noise = 0 is the deterministic mode of a squashed (SAC: W3 / b3 the
+ *     mean rows) or unsquashed (the Gaussian head's mean, widened) policy.
+ *   - IEEE cases: a NaN mu gives a NaN action (comparisons keep it).  mu = +-inf gives t = +-1 when squashed, the
+ *     action without noise.  noise = +inf with noise_clip = +inf gives +-1 (the sign of z) when squashed, and +-inf
+ *     (NaN where mu is the opposite infinity) unsquashed.
+ *     noise_clip = 0 adds a signed zero, so t is unchanged but for the sign of a zero t.
+ *   - With squash == 0: noise = 1, noise_clip = +inf gives ktb_mlp_bf16_policy_gaussian's actions with log_std = 0 bit
+ *     for bit, and noise = 0 gives ktb_mlp_bf16_policy's logits widened to fp32.
+ *   - Checks: every check ktb_mlp_bf16_policy runs first; then, with M > 0, a NULL or not 4-byte aligned actions is
+ *     KTB_ERR_ARG and d_out > 256 is KTB_ERR_UNSUPPORTED; then a NaN or negative noise or noise_clip is KTB_ERR_ARG.
+ *     The pushed form reads only the observation rows from its staging half (ktb_push_scatter_ce feeds it); an empty
+ *     pushed shard (M == 0) may pass NULL actions and still publishes its ack.  Writes stay inside actions[M, d_out],
+ *     scratch and stage. */
+int ktb_mlp_bf16_policy_deterministic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                      const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                      const void* b3, float noise, float noise_clip, int squash, uint64_t seed,
+                                      uint64_t row_base, float* actions, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_policy_deterministic_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                             int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                             const void* b2, const void* W3, const void* b3, float noise,
+                                             float noise_clip, int squash, uint64_t seed, uint64_t row_base,
+                                             float* actions, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                             int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

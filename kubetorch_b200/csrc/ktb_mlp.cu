@@ -422,11 +422,14 @@ struct HeadGroups {
 // with `state` the head's weight interleaves the mean's and the log-std's rows, and the log-std is clamped to
 // [lo, hi]; `squash` passes the actions through tanh.  state == false is the state-independent log_std of the other
 // entries.  It is a parameter of its own rather than a member of HeadOut: a larger HeadOut re-schedules the kSample
-// instantiations, which never read it.
+// instantiations, which never read it.  `det` marks a deterministic actor (TD3 / DDPG) instead: the action is the
+// mean, tanh-squashed with `squash`, plus σ·z clamped to [−clip, clip] when σ = `noise` != 0 (deterministic_pass).
 struct HeadStd {
   float lo = 0.f, hi = 0.f;
   bool state = false;
   bool squash = false;
+  bool det = false;
+  float noise = 0.f, clip = 0.f;
 };
 
 // The per-row inputs and outputs of an ε-greedy kSample head, the layer kernel's last parameter (by value, like
@@ -938,6 +941,57 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   }
 }
 
+// The deterministic actor's pass of gaussian_epilogue (HeadStd::det) over the bf16 pairs its pass 1 parked: one rolled
+// step per column pair < d.  t = tanhf(μ) with sd.squash, μ otherwise; when sd.noise != 0 one Philox call per pair and
+// row draws the Gaussian head's z (word col & 1 of counter (i, col >> 1, 1)), n = σ·z rounded once and clamped to
+// [−clip, clip], and t = t + n rounded once (no FMA contraction: the same rounding as the torch body); with sd.squash t
+// is then clamped to [−1, 1].  The clamps are compares, not fminf / fmaxf, so a NaN μ stays NaN.  σ = 0 draws no
+// Philox word.  Stored as in the sampling branch: float2 where the row stride and the base allow, scalars otherwise.
+template <int BLOCK_N, typename Slot>
+__device__ __forceinline__ void deterministic_pass(Slot slot, int col0, int d, int row, bool st0, bool st1,
+                                                   float* actions, uint2 key, uint64_t row_base, const HeadStd& sd,
+                                                   bool pairs) {
+  const float s = sd.noise, c = sd.clip;
+#pragma unroll 1
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int col = col0 + 8 * j;
+    if (col >= d) break;
+    const bool has1 = col + 1 < d;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const __nv_bfloat162 y = *slot(2 * j + h);
+      float a[2] = {__low2float(y), __high2float(y)};
+      if (sd.squash) {
+        a[0] = tanhf(a[0]);
+        a[1] = tanhf(a[1]);
+      }
+      if (s != 0.f) {
+        const uint64_t i = row_base + (uint64_t)(row + 8 * h);
+        const uint4 x = philox4x32_10(make_uint4((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)col >> 1, 1u), key);
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const float z = normcdfinvf((float)(2u * ((k ? x.y : x.x) >> 9) + 1u) * 5.9604644775390625e-8f);
+          float n = __fmul_rn(s, z);
+          n = n < -c ? -c : n > c ? c : n;
+          a[k] = __fadd_rn(a[k], n);
+        }
+      }
+      if (sd.squash) {
+#pragma unroll
+        for (int k = 0; k < 2; ++k) a[k] = a[k] < -1.f ? -1.f : a[k] > 1.f ? 1.f : a[k];
+      }
+      if (!(h ? st1 : st0)) continue;
+      float* p = actions + (size_t)(row + 8 * h) * d + col;
+      if (pairs) {
+        *reinterpret_cast<float2*>(p) = make_float2(a[0], a[1]);
+      } else {
+        p[0] = a[0];
+        if (has1) p[1] = a[1];
+      }
+    }
+  }
+}
+
 // The Gaussian epilogue of a head tile (HeadKind::kGaussian): rows r = row and row + 8 of the thread, global rows
 // row_base + r.  Only its first part is unrolled over the accumulators, so that the Philox and Φ⁻¹ code is not repeated
 // BLOCK_N / 8 times: it rounds the logits once (layer_pair: μ, the value ktb_mlp_bf16_policy stores) and parks them as
@@ -959,6 +1013,8 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
 // of counter (i, a >> 1, 1) (the noise of action a in the head above), u = μ + σ·z rounded as above, and the action is
 // tanhf(u) with sd.squash, u without; the row sums 0.5·z² + ℓc, plus 2·(log 2 − |u| − log1p(e^−2|u|)) =
 // −log(1 − tanh²u) with sd.squash, over its d_out actions.
+// A deterministic actor (sd.det) takes deterministic_pass after the same pass 1 and returns: it stores no
+// log-probabilities.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                   int n_valid, int row, bool st0, bool st1, const float* log_std,
@@ -981,6 +1037,10 @@ __device__ __forceinline__ void gaussian_epilogue(const float (&acc)[BLOCK_N / 2
   const int d = n_valid - (values != nullptr);   // the policy's columns
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
   const bool pairs = (d & 1) == 0 && ((uintptr_t)actions & 7) == 0;
+  if (sd.det) {   // no log-probabilities and no value head
+    deterministic_pass<BLOCK_N>(slot, col0, d, row, st0, st1, actions, key, row_base, sd, pairs);
+    return;
+  }
   const int d_act = sd.state ? d >> 1 : d;   // the actions per row
   float sum[2] = {0.f, 0.f};
 #pragma unroll 1
@@ -1151,7 +1211,9 @@ struct HeadOut {
 //   kSample with eg.epsilon: the ε-greedy action of each row with the Q-values of the taken and the greedy action
 //     (epsilon_pass);
 //   kSample with ev.actions and kGaussian with ev.gauss_actions: the log-probability and the entropy of given actions
-//     (evaluate_pass, gaussian_epilogue).
+//     (evaluate_pass, gaussian_epilogue);
+//   kGaussian with sd.det: gauss_actions[row, j] = the deterministic actor's action, tanh(logit_j) (or logit_j) plus
+//     clipped noise, and no log_probs (deterministic_pass).
 // A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
 // (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
 // never an action.
@@ -1311,7 +1373,8 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // half (the pushed forms) hold each row's ε, and out.actions, eg.q and eg.q_max receive the outputs.  `evaluate` marks
 // the _evaluate entries: ev.actions (kSample) or ev.gauss_actions (kGaussian), or in the pushed forms the bytes at
 // MlpFeed::taken_offset of the call's staging half, hold the given actions, and out.log_probs and ev.entropy receive
-// the outputs; a categorical one is grouped unless nvec == null and n_groups == 0.
+// the outputs; a categorical one is grouped unless nvec == null and n_groups == 0.  std.det marks the _deterministic
+// entries: out.gauss_actions receives the actions, and mlp_run checks σ and the clip.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1369,6 +1432,19 @@ struct MlpParams {
     p.n_groups = n_groups;
     p.evaluate = true;
     p.ev = HeadEval{taken, nullptr, entropy};
+    return p;
+  }
+
+  // A deterministic actor, in the kGaussian instantiations: actions [M, d_out] fp32 out, σ = noise, clip, tanh with
+  // squash != 0.
+  static MlpParams deterministic(const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                 const void* b3, float noise, float clip, int squash, uint64_t seed, uint64_t row_base,
+                                 float* actions) {
+    MlpParams p{W1, b1, W2, b2, W3, b3, HeadKind::kGaussian, {nullptr, nullptr, nullptr, seed, row_base, nullptr, actions}};
+    p.std.det = true;
+    p.std.squash = squash != 0;
+    p.std.noise = noise;
+    p.std.clip = clip;
     return p;
   }
 
@@ -1441,7 +1517,9 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
           KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
-        if (p.std.state)   // a state-dependent head reads its log-std from the head's own columns
+        if (p.std.det)   // a deterministic actor stores its actions only
+          KTB_REQUIRE(o.gauss_actions, KTB_ERR_ARG, "%s: actions is required", fn);
+        else if (p.std.state)   // a state-dependent head reads its log-std from the head's own columns
           KTB_REQUIRE(o.gauss_actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         else if (p.evaluate)   // an evaluating head's actions and outputs are checked by mlp_run after every other check
           KTB_REQUIRE(o.log_std, KTB_ERR_ARG, "%s: log_std is required", fn);
@@ -1523,7 +1601,8 @@ struct MlpFeed {
 // own checks come after every check of its greedy counterpart (ktb_mlp_bf16_policy or _masked): its ε region in the
 // pushed forms, then (skipped for an empty call) ε, actions, q and q_max non-null and aligned.  An evaluating entry's
 // own checks come after every check of its counterpart and its nvec: (skipped for an empty call) taken, log_probs,
-// entropy non-null and aligned, then its taken region in the pushed forms.
+// entropy non-null and aligned, then its taken region in the pushed forms.  A deterministic entry's actions are checked
+// with the head (mlp_check), its noise and noise_clip (>= 0, not NaN; skipped for an empty call) after every check.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1590,6 +1669,11 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     const float lo = p.std.lo, hi = p.std.hi;
     KTB_REQUIRE(lo == lo && hi == hi && lo <= hi, KTB_ERR_ARG, "%s: log_std bounds [%g, %g] must be ordered, not NaN",
                 fn, (double)lo, (double)hi);
+  }
+  if (p.std.det && M > 0) {
+    const float s = p.std.noise, c = p.std.clip;
+    KTB_REQUIRE(s == s && s >= 0.f, KTB_ERR_ARG, "%s: noise=%g must be >= 0, not NaN", fn, (double)s);
+    KTB_REQUIRE(c == c && c >= 0.f, KTB_ERR_ARG, "%s: noise_clip=%g must be >= 0, not NaN", fn, (double)c);
   }
   HeadGroups groups = p.out.groups;
   if (p.grouped && M > 0) {
@@ -2362,6 +2446,29 @@ int ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed(int dev, const void* stag
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
                      .with_taken_offset(taken_offset),
                  scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_deterministic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                      const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                      const void* b3, float noise, float noise_clip, int squash, uint64_t seed,
+                                      uint64_t row_base, float* actions, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::deterministic(W1, b1, W2, b2, W3, b3, noise, noise_clip, squash, seed, row_base, actions);
+  return mlp_run("ktb_mlp_bf16_policy_deterministic", dev, M, d_in, d_hidden, d_out, p, MlpFeed::pull(obs, stage),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_policy_deterministic_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                             int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                             const void* b2, const void* W3, const void* b3, float noise,
+                                             float noise_clip, int squash, uint64_t seed, uint64_t row_base,
+                                             float* actions, void* scratch, void* ctrl_local, void* ctrl_root_peer,
+                                             int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams p =
+      MlpParams::deterministic(W1, b1, W2, b2, W3, b3, noise, noise_clip, squash, seed, row_base, actions);
+  return mlp_run("ktb_mlp_bf16_policy_deterministic_pushed", dev, M, d_in, d_hidden, d_out, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
+                 stream);
 }
 
 }  // extern "C"

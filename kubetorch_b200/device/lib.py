@@ -201,6 +201,12 @@ for _masked in ("", "_masked"):
             if not _masked:
                 _SIGNATURES["ktb_mlp_bf16_policy_gaussian_evaluate" + _valued + _form] = (
                     c_int, _args[:_at] + [c_void_p, _in] + [c_void_p] * (2 + bool(_valued)) + _args[_at + 2:])
+# The _deterministic entries: the _gaussian_state entries' arguments with (noise, noise_clip, squash) in place of
+# (log_std_min, log_std_max, squash) and without log_probs, the 19th argument of the plain and staged forms and the 20th
+# of the pushed ones.
+for _form, _at in (("", 18), ("_pushed", 19)):
+    _restype, _args = _SIGNATURES["ktb_mlp_bf16_policy_gaussian_state" + _form]
+    _SIGNATURES["ktb_mlp_bf16_policy_deterministic" + _form] = (_restype, _args[:_at] + _args[_at + 1:])
 _SIGNATURES["ktb_push_scatter_ce_sides"] = (
     c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
                                                          ctypes.c_ulonglong, c_uintptr])

@@ -5,7 +5,8 @@ diagonal-Gaussian actions with their log-probabilities), the _masked forms of th
 mask), the _value forms of the sampled heads (a critic's state value on the same trunk), the _multidiscrete forms of
 the greedy and sampled heads (one categorical per group of columns), the _gaussian_state forms (a per-row log-std
 head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network's ε-greedy actor), the _evaluate
-and _gaussian_evaluate forms (the log-probability and entropy of given actions) and their scatter→exec→gather form."""
+and _gaussian_evaluate forms (the log-probability and entropy of given actions), the _deterministic forms (DDPG's and
+TD3's actor: tanh actions with clipped Gaussian noise) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -175,8 +176,31 @@ def _check_taken(taken, output, obs, d_out, nvec) -> None:
         raise ValueError(f"taken must be a CUDA tensor on the device of obs ({obs.device}), got {taken.device}")
 
 
+def _check_deterministic(seed, noise, noise_clip, squash) -> None:
+    """_check_policy's checks of output="deterministic"'s own options, in this order: a seed exactly when noise is
+    given (then _check_seed), noise_clip with noise only, noise and noise_clip numbers (not bools) >= 0 and not NaN,
+    squash True or False."""
+    if (noise is None) != (seed is None):
+        raise ValueError('output="deterministic" takes a seed exactly when it takes noise: the noise-free actor draws '
+                         'nothing')
+    if noise_clip is not None and noise is None:
+        raise ValueError("noise_clip is an option of noise only: it clips the noise")
+    if seed is not None:
+        _check_seed(seed)
+    for name, v in (("noise", noise), ("noise_clip", noise_clip)):
+        if v is None:
+            continue
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            raise ValueError(f"{name} must be a number, got {v!r}")
+        if v != v or v < 0:
+            raise ValueError(f"{name} must be >= 0 and not NaN, got {v!r}")
+    if squash is not None and not isinstance(squash, bool):
+        raise ValueError(f"squash must be True or False, got {squash!r}")
+
+
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
-                  nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None) -> None:
+                  nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None, noise=None,
+                  noise_clip=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
     (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
@@ -189,9 +213,21 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     only.  output="epsilon_greedy" takes a seed and an epsilon (_check_epsilon), and epsilon is refused with any other
     output; its value=, nvec= and log_std= are refused by the checks of those options.  output="evaluate" and
     "gaussian_evaluate" take the actions to score, `taken` (_check_taken), refused with any other output; they refuse
-    a seed, epsilon, squash, log_std_bounds and a log_std pair, and "gaussian_evaluate" a mask."""
+    a seed, epsilon, squash, log_std_bounds and a log_std pair, and "gaussian_evaluate" a mask.  output="deterministic"
+    takes noise, noise_clip, a seed and squash (_check_deterministic) and refuses mask, value, nvec, log_std,
+    log_std_bounds, epsilon and taken; noise and noise_clip are refused with any other output."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
+    det = output == "deterministic"
+    if det:
+        for name, v in (("mask", mask), ("value", value), ("nvec", nvec), ("log_std", log_std),
+                        ("log_std_bounds", log_std_bounds), ("epsilon", epsilon), ("taken", taken)):
+            if v is not None:
+                raise ValueError(f'{name} is not an argument of output="deterministic": the deterministic actor takes '
+                                 f'noise, noise_clip, seed and squash only')
+        _check_deterministic(seed, noise, noise_clip, squash)
+    elif noise is not None or noise_clip is not None:
+        raise ValueError(f'noise and noise_clip are arguments of output="deterministic", not of output={output!r}')
     evaluate = output in EVALUATE_OUTPUTS
     if evaluate:
         for name, v in (("seed", seed), ("epsilon", epsilon), ("squash", squash), ("log_std_bounds", log_std_bounds)):
@@ -224,7 +260,7 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     gaussian = output in ("gaussian", "gaussian_evaluate")
     if not gaussian and log_std is not None:
         raise ValueError('log_std is an argument of output="gaussian" only (and of "gaussian_evaluate")')
-    if not state and (log_std_bounds is not None or squash is not None):
+    if not state and (log_std_bounds is not None or squash is not None and not det):
         raise ValueError("log_std_bounds and squash are options of a state-dependent log_std=(w_ls, b_ls) only")
     if output == "gaussian" and state:
         _check_state_std(log_std, log_std_bounds, squash, w3, biases[2], d_hidden, d_out, value is not None)
@@ -291,7 +327,8 @@ def _stacked_head(w3, b3, wv=None, bv=None, w_ls=None, b_ls=None) -> Tuple[torch
 def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False, nvec=None):
     """(logits, actions, log_probs, values) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions
     [M], [M, len(nvec)] with nvec, or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values
-    [M].  With "epsilon_greedy" the last two slots hold its fp32 q [M] and q_max [M]; with "evaluate" and
+    [M].  "deterministic" writes fp32 actions [M, d_out] only.  With "epsilon_greedy" the last two slots hold its fp32
+    q [M] and q_max [M]; with "evaluate" and
     "gaussian_evaluate" the actions slot holds the fp32 entropy [M].  A buffer the mode does not
     write is None, a missing one is allocated on `device` and a given one is
     registered with the library (ops.ensure_init); given multi-discrete actions must be [M, len(nvec)]."""
@@ -301,7 +338,7 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
         ops.ensure_init({t.device.index})
         return t
 
-    gaussian = output == "gaussian"
+    gaussian = output in ("gaussian", "deterministic")
     if output in EVALUATE_OUTPUTS:
         return None, buf(actions, (M,), torch.float32), buf(log_probs, (M,), torch.float32), \
             buf(values, (M,), torch.float32) if valued else None
@@ -317,7 +354,7 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
 
 
 def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None,
-          nvec=None, std=None, epsilon=None, taken=None):
+          nvec=None, std=None, epsilon=None, taken=None, det=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
     mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
@@ -326,9 +363,12 @@ def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, push
     picks the _gaussian_state entry (whose W3 and b3 are the interleaved head) in place of log_std.  With
     "epsilon_greedy", `epsilon` is ε's address (pull forms) or its offset in the staging half (pushed forms), and
     log_probs and values are its q and q_max buffers.  With "evaluate" and "gaussian_evaluate", `taken` is the given
-    actions' address or offset likewise, and `actions` is the entropy buffer."""
+    actions' address or offset likewise, and `actions` is the entropy buffer.  With "deterministic", `det` is the
+    entry's (noise, noise_clip, squash) (_det); a noise-free call passes seed 0, which draws nothing."""
     valued = () if values is None else (ptr(values),)
     pushed_suffix = "_pushed" if pushed else ""
+    if output == "deterministic":
+        return "ktb_mlp_bf16_policy_deterministic" + pushed_suffix, (*det, seed or 0, row_base, ptr(actions))
     if output == "gaussian_evaluate":
         return "ktb_mlp_bf16_policy_gaussian_evaluate" + ("" if values is None else "_value") + pushed_suffix, \
             (ptr(log_std), taken, ptr(log_probs), ptr(actions), *valued)
@@ -366,6 +406,13 @@ def _std(log_std, log_std_bounds, squash):
     return float(lo), float(hi), int(bool(squash))
 
 
+def _det(noise, noise_clip, squash):
+    """The (noise, noise_clip, squash) arguments of a _deterministic entry: no noise is σ = 0, no clip is +inf and
+    squash defaults to True."""
+    return (0.0 if noise is None else float(noise), math.inf if noise_clip is None else float(noise_clip),
+            int(squash is None or squash))
+
+
 def _rows(bufs, b, e):
     """Rows b .. e - 1 of each buffer; None stays None."""
     return [None if t is None else t[b:e] for t in bufs]
@@ -381,6 +428,8 @@ def _result(output, logits, actions, log_probs, values=None):
         return logits, actions
     if output in EVALUATE_OUTPUTS:   # the entropy rides in the actions slot
         return (log_probs, actions) if values is None else (log_probs, actions, values)
+    if output == "deterministic":
+        return actions
     return (actions, log_probs) if values is None else (actions, log_probs, values)
 
 
@@ -395,7 +444,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
                 epsilon=None, q: Optional[torch.Tensor] = None, q_max: Optional[torch.Tensor] = None,
                 taken: Optional[torch.Tensor] = None, entropy: Optional[torch.Tensor] = None,
-                _stacked: bool = False):
+                noise: Optional[float] = None, noise_clip: Optional[float] = None, _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -439,6 +488,11 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     (masked) logits and entropy[i] = sum_g entr(softmax(group_g)).sum(), or Normal(logits, exp(log_std))'s
     log_prob(taken).sum(-1) and entropy().sum(-1); an action out of range gives a NaN row (it is not checked, which
     would need a host synchronisation), an illegal one -inf.  No noise is drawn and no logits are written.
+    output="deterministic" (DDPG's and TD3's actor) returns fp32 actions[M, d_out], into `actions` when given:
+    t = tanh(logits.float()) with `squash` True or None, logits.float() with squash=False; with `noise` σ >= 0 (and then
+    `seed`) t + (σ·normal_noise(seed, row_offset, M, d_out)).clamp(-noise_clip, noise_clip), noise_clip >= 0 defaulting
+    to +inf; then clamp(-1, 1) when squashed (NaN stays NaN).  σ = 0.1 is exploration, σ = 0.2 with noise_clip = 0.5
+    TD3's target policy smoothing, no noise the deterministic mode of a tanh-squashed or an unsquashed policy.
     `_stacked` (internal, from
     mlp_scatter_gather, which checked the call): w3 and biases[2] are
     already the head the C entry takes (stacked with a value head, interleaved with a log-std head)."""
@@ -453,12 +507,12 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
     if not _stacked:
         _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon,
-                      taken)
+                      taken, noise, noise_clip)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     valued = value is not None or (_stacked and values is not None)
     if _stacked:
         d_out = (d_out - valued) // (2 if std is not None else 1)
-    if output in ("sample", "gaussian", "epsilon_greedy") and \
+    if output in ("sample", "gaussian", "epsilon_greedy", "deterministic") and \
             (isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0):
         raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
     eps = output == "epsilon_greedy"
@@ -481,7 +535,8 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
                         mask=None if mask is None else ptr(mask), values=values, nvec=nvec, std=std,
-                        epsilon=ptr(epsilon) if eps else None, taken=ptr(taken))
+                        epsilon=ptr(epsilon) if eps else None, taken=ptr(taken),
+                        det=_det(noise, noise_clip, squash) if output == "deterministic" else None)
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
            ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
@@ -514,7 +569,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
                                seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None,
-                               epsilon=None, taken=None) -> None:
+                               epsilon=None, taken=None, det=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -531,7 +586,8 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     half is rows | mask | ε, each 256-byte aligned (ktb_push_scatter_ce_sides), and log_probs_root / values_root are
     its q and q_max.  With output="evaluate" or "gaussian_evaluate", `taken` (on the root) is pushed with the rows the
     same way, each staging half rows | mask | taken with taken's offset rounded up to 8 bytes, and actions_root is the
-    entropy."""
+    entropy.  With output="deterministic", `det` is the call's dict(noise=, noise_clip=, squash=), and each staging
+    half holds the rows only."""
     root, n, key = devs[0], len(devs), tuple(devs)
     valued = values_root is not None and epsilon is None   # an ε-greedy head's values_root is its q_max
     d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
@@ -571,7 +627,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
                     biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
                     log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0],
                     values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
-                    squash=None if std is None else bool(std[2]),
+                    **(det or dict(squash=None if std is None else bool(std[2]))),
                     **({} if epsilon is None else dict(epsilon=epsilon[b0:e0], q=log_probs, q_max=values)),
                     **({} if taken is None else dict(taken=taken[b0:e0], entropy=actions)),
                     _stacked=valued or std is not None)
@@ -600,7 +656,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         entry, head = _head(output, logits, actions, log_probs, seed, b,
                             None if log_std is None else log_std[devs[r]], ptr, pushed=True,
                             mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std,
-                            epsilon=eps_offset, taken=taken_offset)
+                            epsilon=eps_offset, taken=taken_offset, det=None if det is None else _det(**det))
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -618,7 +674,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        values_root: Optional[torch.Tensor] = None, nvec: Optional[Sequence[int]] = None,
                        log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
                        epsilon=None, taken: Optional[torch.Tensor] = None,
-                       entropy_root: Optional[torch.Tensor] = None) -> list:
+                       entropy_root: Optional[torch.Tensor] = None, noise: Optional[float] = None,
+                       noise_clip: Optional[float] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -636,13 +693,16 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     reads its rows of ε in place on the pull form, and the push form pushes them with the rows.  output="evaluate" and
     "gaussian_evaluate" with `taken` on the root as in mlp_forward return (log_probs, entropy) pairs, or triples with
     a value head, into `log_probs_root`, `entropy_root` and `values_root` when given; each rank reads its rows of taken
-    in place on the pull form, and the push form pushes them with the rows."""
+    in place on the pull form, and the push form pushes them with the rows.  output="deterministic" with `noise`,
+    `noise_clip`, `seed` and `squash` as in mlp_forward returns fp32 actions [rows, d_out] views of `actions_root`;
+    each rank draws the noise of its shard's global rows."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
     _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon,
-                  taken)
+                  taken, noise, noise_clip)
+    det = dict(noise=noise, noise_clip=noise_clip, squash=squash) if output == "deterministic" else None
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     if output == "epsilon_greedy" and not isinstance(epsilon, torch.Tensor):   # before `ready`: every rank reads it
@@ -675,7 +735,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec, std, epsilon, taken)
+                                   nvec, std, epsilon, taken, det)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
         _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
@@ -699,7 +759,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                         output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
                         log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e],
                         values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
-                        squash=None if std is None else bool(std[2]),
+                        **(det or dict(squash=None if std is None else bool(std[2]))),
                         **({} if epsilon is None else dict(epsilon=epsilon[b:e], q=log_probs, q_max=values)),
                         **({} if taken is None else dict(taken=taken[b:e], entropy=actions)),
                         _stacked=valued or std is not None)

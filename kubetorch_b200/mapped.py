@@ -24,7 +24,7 @@ MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
-               "gaussian_evaluate")   # also device.mlp.OUTPUTS
+               "gaussian_evaluate", "deterministic")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
 
 
@@ -108,22 +108,35 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     entropy, values)`` with ``value=``: the fp32 log-probability of each row's action and the entropy of its policy,
     summed over groups, under ``logits.masked_fill(~mask, -inf)`` (``"evaluate"``; ``mask=`` and ``nvec=`` apply) or
     ``Normal(logits, exp(log_std))`` (``"gaussian_evaluate"``, with ``log_std=`` naming one argument).  They draw no
-    noise, so ``seed=``, ``epsilon=``, ``squash=``, ``log_std_bounds=`` and a ``log_std`` pair are refused."""
+    noise, so ``seed=``, ``epsilon=``, ``squash=``, ``log_std_bounds=`` and a ``log_std`` pair are refused.
+    ``output="deterministic"`` is the actor of DDPG and TD3: each rank returns fp32 actions ``[rows, d_out]``,
+    ``tanh(logits)`` with ``squash=True`` (the default) and the fp32 logits with ``squash=False``, plus, with ``noise=``
+    σ (a number >= 0 or the name of a call argument that holds one), ``(σ·z).clamp(-c, c)`` with ``z`` the noise of
+    ``"gaussian"`` and ``c`` = ``noise_clip=`` (a number >= 0, default +inf), then clamped to [-1, 1] when squashed.
+    ``seed=`` is required exactly when ``noise=`` is given.  Exploration is ``noise=0.1``; TD3's target policy
+    smoothing is ``noise=0.2, noise_clip=0.5``.  ``mask=``, ``value=``, ``nvec=``, ``log_std=``, ``log_std_bounds=``,
+    ``epsilon=`` and ``taken=`` are refused."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
     if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
-                                "squash", "epsilon", "taken")):
+                                "squash", "epsilon", "taken", "noise", "noise_clip")):
         if op != "mlp":
             raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value=, nvec=, "
-                             f"epsilon= and taken= are options of the 'mlp' op, not of '{op}'")
+                             f"epsilon=, taken=, noise= and noise_clip= are options of the 'mlp' op, not of '{op}'")
         if not isinstance(extra.get("bias", False), bool):
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
         sample = extra.get("output") in ("sample", "gaussian")
         eps = extra.get("output") == "epsilon_greedy"
+        det = extra.get("output") == "deterministic"
+        if det:
+            _check_deterministic(extra)
+        elif "noise" in extra or "noise_clip" in extra:
+            raise ValueError(f'noise= and noise_clip= are options of output="deterministic", not of '
+                             f'output={extra.get("output", "logits")!r}')
         evaluate = extra.get("output") in EVALUATE_OUTPUTS
         if evaluate != ("taken" in extra):
             raise ValueError('taken= is required with output="evaluate" and "gaussian_evaluate" and is an option of '
@@ -133,10 +146,10 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
         if evaluate and "seed" in extra:
             raise ValueError(f'seed= is not an option of output={extra["output"]!r}: evaluating given actions draws '
                              f'no noise')
-        if (sample or eps) != ("seed" in extra):
+        if not det and (sample or eps) != ("seed" in extra):
             raise ValueError('seed= is required with output="sample" or "gaussian" (or "epsilon_greedy") and is an '
                              'option of those only')
-        if (sample or eps) and not isinstance(extra["seed"], str):
+        if (sample or eps or det) and "seed" in extra and not isinstance(extra["seed"], str):
             from .sampling import _check_seed
 
             _check_seed(extra["seed"])
@@ -157,7 +170,7 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
                                  "b3 is")
         elif gaussian and not isinstance(extra["log_std"], str):
             raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
-        if not state and ("log_std_bounds" in extra or "squash" in extra):
+        if not state and ("log_std_bounds" in extra or "squash" in extra and not det):
             raise ValueError("log_std_bounds= and squash= are options of a state-dependent log_std=(w_ls, b_ls) only")
         if "log_std_bounds" in extra:
             lb = extra["log_std_bounds"]
@@ -198,9 +211,9 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
 
     def deco(fn):
         params = inspect.signature(fn).parameters
-        for option in ("log_std", "mask", "value", "epsilon", "taken"):
+        for option in ("log_std", "mask", "value", "epsilon", "taken", "noise"):
             names = extra.get(option)
-            if option == "epsilon" and not isinstance(names, str):   # a constant ε names no argument
+            if option in ("epsilon", "noise") and not isinstance(names, str):   # a constant names no argument
                 continue
             for name in (names,) if isinstance(names, str) or names is None else names:
                 if name is not None and name not in params:
@@ -210,6 +223,30 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
         return fn
 
     return deco
+
+
+def _check_deterministic(extra) -> None:
+    """mapped()'s checks of output="deterministic", in this order: the options it refuses, seed= given exactly when
+    noise= is, noise (a number that is not NaN and >= 0, or the name of a call argument), noise_clip (with noise= only;
+    a number that is not NaN and >= 0)."""
+    for name in ("mask", "value", "nvec", "log_std", "log_std_bounds", "epsilon", "taken"):
+        if name in extra:
+            raise ValueError(f'{name}= is not an option of output="deterministic": the deterministic actor takes '
+                             f'noise=, noise_clip=, seed= and squash= only')
+    if ("noise" in extra) != ("seed" in extra):
+        raise ValueError('output="deterministic" takes seed= exactly when it takes noise=: the noise-free actor draws '
+                         'nothing')
+    if "noise_clip" in extra and "noise" not in extra:
+        raise ValueError("noise_clip= is an option of noise= only: it clips the noise")
+    for name in ("noise", "noise_clip"):
+        v = extra.get(name)
+        if v is None or name == "noise" and isinstance(v, str):
+            continue
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            what = "a number or the name of a call argument" if name == "noise" else "a number"
+            raise ValueError(f"{name} must be {what}, got {v!r}")
+        if v != v or v < 0:
+            raise ValueError(f"{name} must be >= 0 and not NaN, got {v!r}")
 
 
 def check_nvec(nvec, output: str, d_out: Optional[int] = None) -> tuple:

@@ -12,7 +12,8 @@ legal column with the largest word ``w``.  The device kernel draws the very same
 
     stream  s   use
     Gumbel  0   g = -log(-log(u)) in fp32, added to the logits of output="sample"
-    Gaussian 1  z = Φ⁻¹(u) in fp32, within ±5.29471 and never 0, the noise of output="gaussian"
+    Gaussian 1  z = Φ⁻¹(u) in fp32, within ±5.29471 and never 0, the noise of output="gaussian" (and of
+                "deterministic", scaled by σ and clipped)
     explore 2   the word x itself (a uint32): ranks the legal columns of an exploring row of output="epsilon_greedy"
     coin    3   u of column 0 only (one draw per row): the row explores iff u < ε in fp32
 

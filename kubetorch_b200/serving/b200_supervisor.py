@@ -604,12 +604,18 @@ class B200Supervisor:
             if taken not in bound:
                 raise TypeError(f"mapped mlp callable: taken argument '{taken}' not found in the call")
             taken = bound[taken]
+        noise = spec.extra.get("noise")
+        if isinstance(noise, str):   # the name of a call argument (a float), resolved per call
+            if noise not in bound:
+                raise TypeError(f"mapped mlp callable: noise argument '{noise}' not found in the call")
+            noise = bound[noise]
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
                                          value=value, nvec=spec.extra.get("nvec"),
                                          log_std_bounds=spec.extra.get("log_std_bounds"),
-                                         squash=spec.extra.get("squash"), epsilon=epsilon, taken=taken)
+                                         squash=spec.extra.get("squash"), epsilon=epsilon, taken=taken, noise=noise,
+                                         noise_clip=spec.extra.get("noise_clip"))
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -40,6 +40,10 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      each scoring the actions of the matching sampling call and timed beside it; and the eager arm, what a user pays
      without the evaluating head: the logits entry, then mask, split, log_softmax, gather, softmax and entr (or
      Normal.log_prob and entropy) in torch.
+  o  deterministic actors (output="deterministic", DDPG's and TD3's), d_out 6, 17 and 64: the noise-free squashed
+     actor beside output="logits", exploration (σ = 0.1) beside output="gaussian", and TD3's target policy smoothing
+     (σ = 0.2, noise_clip = 0.5), at the same d_out; and the eager arm, what a user pays without the fused head: the
+     logits entry, then tanh, normal_noise on the device and the two clamps in torch.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -58,7 +62,10 @@ within 2 ulp of tanh of the unsquashed ones, and on every row both the actions a
 bit.  Evaluating rows: the categorical log-probabilities of the sampled actions equal the sampling call's on every row,
 bit for bit (NaN in the same rows), its values too; log-probabilities and entropies are within rtol 1e-4, atol 1e-4 of
 the eager arm's (the Gaussian's log-probabilities within rtol 1e-4, atol 1e-3 of the sampling call's), and the values
-within rtol 2^-7, atol 1e-2 of the eager critic's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+within rtol 2^-7, atol 1e-2 of the eager critic's.  Deterministic rows: on 2048 consecutive rows, the noise-free
+actions are within tanhf's 2 ulp of fp64 tanh(y) (y the kernel's logits) and the noisy ones within
+σ·2^-19·(1 + |z|) + 2^-22·|t| + 2^-23·(|t| + |n|) of clamp(tanh(y) + clamp(σ·z, ±c), ±1) in fp64; on every row
+the smoothing actions are within rtol 1e-5, atol 1e-5 of the eager arm's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -341,6 +348,25 @@ def main():
         variants[f"n_bias_evaluate_{tag}"] = (d, lambda d=d, bs=bs, kw=kw_e: mlp.mlp_forward(
             obs, w1, w2, heads[d][0], biases=bs, **kw))
         variants[f"n_bias_evaluate_eager_{tag}"] = (d, eager)
+    det_opts = {"deterministic": {}, "explore": dict(noise=0.1, seed=SEED),
+                "smooth": dict(noise=0.2, noise_clip=0.5, seed=SEED)}
+
+    def eager_deterministic(d, noise=0.2, clip=0.5):
+        """The logits entry, then tanh, the noise and the clamps in torch: what a user pays without the fused head."""
+        y = mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=(b1, b2, heads[d][1]))
+        z = normal_noise(SEED, 0, M, d, device="cuda:0")
+        return (y.float().tanh() + (noise * z).clamp(-clip, clip)).clamp(-1.0, 1.0)
+
+    for d in (6, 17, 64):
+        bs = (b1, b2, heads[d][1])
+        log_stds.setdefault(d, torch.linspace(-2.0, 0.5, d, device="cuda:0"))
+        variants[f"o_bias_logits_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(obs, w1, w2, heads[d][0], biases=bs))
+        variants[f"o_bias_gaussian_d{d}"] = (d, lambda d=d, bs=bs: mlp.mlp_forward(
+            obs, w1, w2, heads[d][0], biases=bs, output="gaussian", seed=SEED, log_std=log_stds[d]))
+        for tag, kw in det_opts.items():
+            variants[f"o_bias_{tag}_d{d}"] = (d, lambda d=d, bs=bs, kw=kw: mlp.mlp_forward(
+                obs, w1, w2, heads[d][0], biases=bs, output="deterministic", **kw))
+        variants[f"o_bias_smooth_eager_d{d}"] = (d, lambda d=d: eager_deterministic(d))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -528,6 +554,26 @@ def main():
             assert torch.allclose(got[2], want[2], rtol=2.0 ** -7, atol=1e-2), tag
         parity[f"n_bias_evaluate_{tag}"] = "ok"
         del drawn, got, want
+
+    r0 = int(torch.randint(0, M - 2048, (1,), device="cuda:0", generator=g))
+    for d in (6, 17, 64):
+        y = variants[f"o_bias_logits_d{d}"][1]()[r0:r0 + 2048].double()
+        t64 = y.tanh()
+        z64 = torch.special.ndtri(gumbel_uniform(SEED, r0, 2048, d, device="cuda:0", word3=1).double())
+        for tag, kw in det_opts.items():
+            got = variants[f"o_bias_{tag}_d{d}"][1]()[r0:r0 + 2048].double()
+            sigma, clip = kw.get("noise", 0.0), kw.get("noise_clip", float("inf"))
+            n64 = (sigma * z64).clamp(-clip, clip)
+            ref = (t64 + n64).clamp(-1, 1)
+            tol = 2.0 ** -22 * t64.abs() + 2.0 ** -148
+            if sigma:
+                tol = tol + sigma * 2.0 ** -19 * (1 + z64.abs()) + 2.0 ** -23 * (t64.abs() + n64.abs())
+            assert bool(((got - ref).abs() <= tol).all()), (tag, d)
+        got = variants[f"o_bias_smooth_d{d}"][1]()
+        want = variants[f"o_bias_smooth_eager_d{d}"][1]()
+        assert torch.allclose(got, want, rtol=1e-5, atol=1e-5), d
+        parity[f"o_bias_deterministic_d{d}"] = "ok"
+        del y, got, want
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
