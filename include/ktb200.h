@@ -870,6 +870,57 @@ int ktb_mlp_bf16_policy_deterministic_pushed(int dev, const void* stage_local, s
                                              float* actions, void* scratch, void* ctrl_local, void* ctrl_root_peer,
                                              int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* Q(s, a) critics (SAC, TD3, DDPG; Ape-X DPG and R2D2 priorities), forward only, with the actions fed into layer 1
+ * beside the observations.  One critic on M rows, the user's nn.Linear(d_in + d_act, d_h) -> ReLU -> nn.Linear(d_h,
+ * d_h) -> ReLU -> nn.Linear(d_h, 1) over torch.cat([obs, act.to(torch.bfloat16)], -1):
+ *     x = [obs | bf16(act)]                     obs bf16 [M, d_in], act fp32 [M, d_act]
+ *     h = relu(x W1ᵀ + b1), h = relu(h W2ᵀ + b2), q = fp32(h W3ᵀ + b3)      q fp32 [M]
+ *   - Every layer follows ktb_mlp_bf16_policy's rules: the bias joins the fp32 accumulator, each layer rounds once to
+ *     bf16, ReLU is fmaxf (so a NaN or infinite action need not give a NaN q: a NaN pre-activation becomes 0).
+ *   - The action is rounded to bf16 once, to nearest even, as .to(torch.bfloat16) does.  q is the bf16 head output
+ *     widened exactly.
+ *   - W1p is the user's W1 [d_hidden, d_in + d_act] padded with zero columns to [d_hidden, d_in + 64]; layer 1 runs
+ *     over K = d_in + 64, its last K block an action tile [rows, 64] (bf16(act), zero past d_act) packed into scratch
+ *     per chunk.  So q equals ktb_mlp_bf16_policy's logits at d_out = 1 over x = [obs | bf16(act) | 0] and W1p, widened
+ *     to fp32, bit for bit.  d_in is a multiple of 64, d_hidden of 256, and 1 <= d_act <= 64.
+ *   - Arguments: ktb_mlp_bf16_policy's, with d_act in place of d_out, W1p for W1, W3 [1, d_hidden] and b3 [1], then
+ *     act (act_offset, a byte offset into the rank's staging half, in the pushed forms) and q.  The _twin entries run
+ *     two independent critics on the same (obs, act), the second's (W1p, b1, W2, b2, W3, b3) after the first's, and
+ *     store q1, q2 and q_min = q2 < q1 ? q2 : q1, NaN when either is (payload unspecified); a tie gives q1, signed
+ *     zeros included, as torch.minimum(q1, q2) does on 0-d CPU tensors (its vectorised CPU kernel gives q2 on a tie
+ *     of signed zeros).  A zero q is +0 on H100: the tensor cores sum all-zero products to +0 and a −0 bias
+ *     adds to it as +0, so no signed-zero tie of q1 and q2 arises from the kernel.  The action tile is packed once
+ *     per chunk for both.
+ *   - scratch holds ktb_mlp_critic_scratch_bytes(M, d_hidden): the two hidden activations and the action tile.
+ *   - act and the outputs may be peer pointers.  The pushed forms read the actions from their staging half (pushed
+ *     there beside the rows by ktb_push_scatter_ce_sides), act_offset bytes in.
+ *   - Checks: every check ktb_mlp_bf16_policy runs first, at d_out = 1 (a twin's second weights and biases as the
+ *     first's, right after them); then d_act < 1 is KTB_ERR_ARG and d_act > 64 KTB_ERR_UNSUPPORTED; then, with M > 0, a
+ *     NULL or not 4-byte aligned act, q, q1, q2 or q_min is KTB_ERR_ARG; then, in the pushed forms, an action region
+ *     that overlaps the rows, ends past stage_stride or is not 4-byte aligned is KTB_ERR_ARG.  An empty pushed shard
+ *     (M == 0) may pass NULL outputs and still publishes its ack.  Writes stay inside the outputs, scratch and stage. */
+size_t ktb_mlp_critic_scratch_bytes(size_t M, int d_hidden);
+int ktb_mlp_bf16_critic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act, const void* W1p,
+                        const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                        const float* act, float* q, void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_critic_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
+                               int d_act, const void* W1p, const void* b1, const void* W2, const void* b2,
+                               const void* W3, const void* b3, size_t act_offset, float* q, void* scratch,
+                               void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                               unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_critic_twin(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act, const void* W1p,
+                             const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                             const void* W1p_2, const void* b1_2, const void* W2_2, const void* b2_2,
+                             const void* W3_2, const void* b3_2, const float* act, float* q1, float* q2, float* q_min,
+                             void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_critic_twin_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                    int d_hidden, int d_act, const void* W1p, const void* b1, const void* W2,
+                                    const void* b2, const void* W3, const void* b3, const void* W1p_2,
+                                    const void* b1_2, const void* W2_2, const void* b2_2, const void* W3_2,
+                                    const void* b3_2, size_t act_offset, float* q1, float* q2, float* q_min,
+                                    void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                    unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

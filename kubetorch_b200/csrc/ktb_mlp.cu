@@ -143,10 +143,13 @@ struct MlpSmem {
 // producer (warp 8, one lane) fills the STAGES-deep ring and then returns false; each consumer thread returns true
 // with its warpgroup's 64 x BLOCK_N accumulators in acc.  A has `rows` rows (the outer dimension of map_a) and B has
 // N rows: TMA zero-fills the rows of a box past either end (and still counts the whole box toward complete_tx), so
-// the accumulators of those rows and columns are 0 and the epilogue decides what to store.
+// the accumulators of those rows and columns are 0 and the epilogue decides what to store.  map_a holds two maps of A:
+// the K blocks kb < kb_split come from map_a[0] at column 64·kb, the rest from map_a[1] at column 64·(kb − kb_split),
+// so a critic's layer 1 reads the observation rows where they are and its action tile beside them.  Every other layer
+// has kb_split = K / 64.
 template <int BLOCK_N, int STAGES>
-__device__ __forceinline__ bool mlp_tile_mainloop(const CUtensorMap* map_a, const CUtensorMap* map_b, int K, int m0,
-                                                  int n0, float (&acc)[BLOCK_N / 2]) {
+__device__ __forceinline__ bool mlp_tile_mainloop(const CUtensorMap* map_a, const CUtensorMap* map_b, int K,
+                                                  int kb_split, int m0, int n0, float (&acc)[BLOCK_N / 2]) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must be 1024-byte aligned
@@ -172,13 +175,15 @@ __device__ __forceinline__ bool mlp_tile_mainloop(const CUtensorMap* map_a, cons
     // ===== TMA producer =====
     if (lane == 0) {
       prefetch_tensormap(map_a);
+      if (kb_split < num_kb) prefetch_tensormap(map_a + 1);
       prefetch_tensormap(map_b);
       for (int kb = 0; kb < num_kb; ++kb) {
         const int s = kb % STAGES;
         mbar_wait(&empty[s], ((kb / STAGES) & 1) ^ 1);
         uint8_t* a_dst = smem + (size_t)s * S::kStageBytes;
         mbar_expect_tx(&full[s], S::kStageBytes);
-        tma_load_2d(a_dst, map_a, kb * kMlpBlockK, m0, &full[s]);
+        const bool first = kb < kb_split;
+        tma_load_2d(a_dst, map_a + !first, (first ? kb : kb - kb_split) * kMlpBlockK, m0, &full[s]);
         tma_load_2d(a_dst + S::kABytes, map_b, kb * kMlpBlockK, n0, &full[s]);
       }
     }
@@ -463,6 +468,44 @@ struct HeadEval {
     return e;
   }
 };
+
+// The outputs of a critic head, the layer kernel's last parameter (by value, like HeadEps, and for the same reason).
+// q != null marks a kGaussian head with no policy columns whose column 0 is Q(s, a): q [rows] receives it widened to
+// fp32.  The second head of a twin also reads q_other [rows], the first head's Q, and stores q_min = min(Q2, Q1)
+// (critic_epilogue).
+struct HeadQ {
+  float* q = nullptr;
+  const float* q_other = nullptr;
+  float* q_min = nullptr;
+
+  HeadQ from_row(size_t r0) const {
+    return q ? HeadQ{q + r0, q_other ? q_other + r0 : nullptr, q_min ? q_min + r0 : nullptr} : *this;
+  }
+};
+
+// The epilogue of a critic head (HeadQ) in the 64-wide kGaussian instantiation: column 0 of rows row and row + 8, held
+// by lane 0 of each quad in acc[0] and acc[2], gets the bias and one rounding to bf16 (layer_pair, as every head) and
+// is stored widened to fp32 into q.  A twin's second head also stores q_min = Q2 < Q1 ? Q2 : Q1, so a tie (±0
+// included) gives Q1, as torch.minimum of 0-d CPU tensors does, and NaN when either is NaN.  The kernel takes it in place
+// of gaussian_epilogue, so the Gaussian heads' code is what it was; the store is rolled.
+template <int BLOCK_N>
+__device__ __forceinline__ void critic_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
+                                                int row, bool st0, bool st1, const HeadQ& hq) {
+  if (col0 != 0) return;
+  __nv_bfloat162 y0, y1;
+  layer_pair<false>(acc[0], acc[1], acc[2], acc[3], bias, 0, 1, y0, y1);
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    if (!(h ? st1 : st0)) continue;
+    const int r = row + 8 * h;
+    const float v = __low2float(h ? y1 : y0);
+    hq.q[r] = v;
+    if (hq.q_other != nullptr) {
+      const float o = hq.q_other[r];
+      hq.q_min[r] = v != v ? v : v < o ? v : o;
+    }
+  }
+}
 
 // The end of the group that begins at column lo: the next set bit of `starts` past lo, or d.  The words are indexed
 // at compile time, so the bitmap stays in the kernel's parameters.
@@ -1213,23 +1256,36 @@ struct HeadOut {
 //   kSample with ev.actions and kGaussian with ev.gauss_actions: the log-probability and the entropy of given actions
 //     (evaluate_pass, gaussian_epilogue);
 //   kGaussian with sd.det: gauss_actions[row, j] = the deterministic actor's action, tanh(logit_j) (or logit_j) plus
-//     clipped noise, and no log_probs (deterministic_pass).
+//     clipped noise, and no log_probs (deterministic_pass);
+//   kGaussian with hq.q: a critic, n_valid = 1: hq.q[row] = fp32(logit_0), and a twin's second head also hq.q_min[row]
+//     (critic_epilogue).
+// A critic's layer 1 (kHidden) takes its A operand from two maps: K blocks < kb_split from maps_a.m[0] (the
+// observation rows), the last from maps_a.m[1] (the action tile); every other launch has kb_split = K / 64 and never
+// reads m[1].
 // A head runs in the smallest of 64 / 128 / 256 that holds d_out = n_valid, so that one CTA owns whole rows
 // (gridDim.x == 1) and the argmax never leaves it.  Columns >= n_valid hold TMA zero fill: they are never stored and
 // never an action.
 // `bias` is deliberately not __restrict__: with it the compiler reads the bias through the non-coherent cache in
 // batches ahead of the stores, and a biased hidden layer takes 3 % longer (H100 80GB HBM3, 700 W).
+// The A operand's maps of a layer launch, one kernel parameter: m[1] is read only by a critic's layer 1.  One object
+// rather than two parameters: with the second map a parameter of its own, taking its address made ptxas keep the
+// Gaussian epilogue's shared-memory addresses out of registers (the 256-wide instantiation grew by a quarter).
+struct AMaps {
+  CUtensorMap m[2];
+};
+
 template <int BLOCK_N, int STAGES, HeadKind KIND>
 __global__ void __launch_bounds__(kMlpThreads, 1)
-    mlp_layer_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                           const __nv_bfloat16* bias, const HeadOut out, int n_valid, int K, int rows,
-                           const HeadStd sd, const HeadEps eg, const HeadEval ev) {
+    mlp_layer_wgmma_kernel(const __grid_constant__ AMaps maps_a, const __grid_constant__ CUtensorMap map_b,
+                           const __nv_bfloat16* bias, const HeadOut out,
+                           int n_valid, int K, int kb_split, int rows, const HeadStd sd, const HeadEps eg,
+                           const HeadEval ev, const HeadQ hq) {
   const int n0 = blockIdx.x * BLOCK_N;
   const int m0 = blockIdx.y * kMlpBlockM;
   const int lane = threadIdx.x & 31;
   const int col0 = n0 + 2 * (lane & 3);
   float acc[BLOCK_N / 2];
-  if (!mlp_tile_mainloop<BLOCK_N, STAGES>(&map_a, &map_b, K, m0, n0, acc)) return;
+  if (!mlp_tile_mainloop<BLOCK_N, STAGES>(maps_a.m, &map_b, K, kb_split, m0, n0, acc)) return;
   const int warp = threadIdx.x >> 5;
   const int wg = warp >> 2;
 
@@ -1244,6 +1300,8 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
                              out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max, ev);
+  } else if (BLOCK_N == 64 && hq.q != nullptr) {   // a critic (64-wide tile): column 0 is Q, no policy columns
+    critic_epilogue<BLOCK_N>(acc, bias, col0, row, st0, st1, hq);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
                                        out.log_probs, out.seed, out.row_base, out.values, sd, ev);
@@ -1329,25 +1387,35 @@ static int ensure_smem_attr(KernelT kfn, int smem_bytes, std::atomic<unsigned>& 
   return KTB_OK;
 }
 
-// One layer through the epilogue of KIND in BLOCK_N-wide tiles: out = A[M, K] · B[N, K]ᵀ (+ bias), N columns.
+// One layer through the epilogue of KIND in BLOCK_N-wide tiles: out = A[M, K] · B[N, K]ᵀ (+ bias), N columns.  With
+// `tile` (a critic's layer 1) A is [M, K − 64] and its last K block is tile [M, 64] instead.
 template <int BLOCK_N, HeadKind KIND>
 static int launch_layer(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
                         int K, cudaStream_t stream, const HeadStd& sd = HeadStd{}, const HeadEps& eg = HeadEps{},
-                        const HeadEval& ev = HeadEval{}) {
+                        const HeadEval& ev = HeadEval{}, const HeadQ& hq = HeadQ{}, const void* tile = nullptr) {
   using S = MlpSmem<BLOCK_N, kMlpStages>;
   static_assert(S::kTotal <= 232448, "the TMA ring must fit the 227 KiB a block may own");
-  CUtensorMap ma, mb;
-  int rc = make_map(&ma, A, M, (uint64_t)K, kMlpBlockM);
+  const int k_a = tile ? K - kMlpBlockK : K;   // A's own columns
+  CUtensorMap mb;
+  AMaps am;
+  CUtensorMap& ma = am.m[0];
+  CUtensorMap& ma2 = am.m[1];
+  int rc = make_map(&ma, A, M, (uint64_t)k_a, kMlpBlockM);
   if (rc) return rc;
   rc = make_map(&mb, B, (uint64_t)N, (uint64_t)K, BLOCK_N);
   if (rc) return rc;
+  ma2 = ma;
+  if (tile) {
+    rc = make_map(&ma2, tile, M, kMlpBlockK, kMlpBlockM);
+    if (rc) return rc;
+  }
   auto kfn = mlp_layer_wgmma_kernel<BLOCK_N, kMlpStages, KIND>;
   static std::atomic<unsigned> attr_done{0};
   rc = ensure_smem_attr(kfn, S::kTotal, attr_done, dev);
   if (rc) return rc;
   dim3 grid((unsigned)((N + BLOCK_N - 1) / BLOCK_N), (unsigned)((M + kMlpBlockM - 1) / kMlpBlockM));
-  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(ma, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K, (int)M, sd,
-                                                eg, ev);
+  kfn<<<grid, kMlpThreads, S::kTotal, stream>>>(am, mb, static_cast<const __nv_bfloat16*>(bias), out, N, K,
+                                                k_a / kMlpBlockK, (int)M, sd, eg, ev, hq);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }
@@ -1356,9 +1424,33 @@ static int launch_layer(int dev, const void* A, const void* B, const void* bias,
 // head, one more with a value head).
 template <HeadKind KIND>
 static int launch_head(int dev, const void* A, const void* B, const void* bias, const HeadOut& out, size_t M, int N,
-                       int K, cudaStream_t stream, const HeadStd& sd, const HeadEps& eg, const HeadEval& ev) {
+                       int K, cudaStream_t stream, const HeadStd& sd, const HeadEps& eg, const HeadEval& ev,
+                       const HeadQ& hq) {
   const auto launch = N <= 64 ? launch_layer<64, KIND> : N <= 128 ? launch_layer<128, KIND> : launch_layer<256, KIND>;
-  return launch(dev, A, B, bias, out, M, N, K, stream, sd, eg, ev);
+  return launch(dev, A, B, bias, out, M, N, K, stream, sd, eg, ev, hq, nullptr);
+}
+
+// A critic's action tile: tile[r, j] = bf16(act[r, j]) (round to nearest even, as torch's .to(torch.bfloat16)) for
+// j < d_act and 0 for d_act <= j < 64, over `rows` rows of fp32 act [rows, d_act] (4-byte aligned; may be a peer
+// pointer).  One thread per 8 columns of a row, one 16-byte store.
+__global__ void critic_action_tile_kernel(const float* act, int d_act, __nv_bfloat16* tile, size_t rows) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= rows * 8) return;
+  const size_t r = t >> 3;
+  const int c0 = (int)(t & 7) * 8;
+  const float* a = act + r * d_act;
+  __align__(16) __nv_bfloat16 v[8];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) v[c] = __float2bfloat16_rn(c0 + c < d_act ? a[c0 + c] : 0.f);
+  *reinterpret_cast<uint4*>(tile + r * kMlpBlockK + c0) = *reinterpret_cast<const uint4*>(v);
+}
+
+static int launch_action_tile(const float* act, int d_act, void* tile, size_t rows, cudaStream_t st) {
+  const size_t threads = rows * 8;
+  critic_action_tile_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(act, d_act,
+                                                                              static_cast<__nv_bfloat16*>(tile), rows);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
 }
 
 // Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
@@ -1374,7 +1466,11 @@ static int launch_head(int dev, const void* A, const void* B, const void* bias, 
 // the _evaluate entries: ev.actions (kSample) or ev.gauss_actions (kGaussian), or in the pushed forms the bytes at
 // MlpFeed::taken_offset of the call's staging half, hold the given actions, and out.log_probs and ev.entropy receive
 // the outputs; a categorical one is grouped unless nvec == null and n_groups == 0.  std.det marks the _deterministic
-// entries: out.gauss_actions receives the actions, and mlp_run checks σ and the clip.
+// entries: out.gauss_actions receives the actions, and mlp_run checks σ and the clip.  `critic` marks the _critic
+// entries: W1 is W1p [d_hidden, d_in + 64], layer 1 reads an action tile packed from `act` (fp32 [M, d_act]; in the
+// pushed forms the bytes at MlpFeed::act_offset of the call's staging half) as its last K block, W3 / b3 are the
+// critic's [1, d_hidden] / [1], and hq receives Q; `twin` (the _twin entries) is the second critic, run on the same
+// tile after the first, whose hq also reads the first's q and stores q_min.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1390,6 +1486,23 @@ struct MlpParams {
   HeadEps eg;
   bool evaluate = false;
   HeadEval ev;
+  bool critic = false;
+  int d_act = 0;
+  const float* act = nullptr;
+  HeadQ hq;
+  const MlpParams* twin = nullptr;
+
+  // A critic, in the 64-wide kGaussian instantiation (one column, Q): act [M, d_act] fp32 (null in the pushed forms)
+  // in, q [M] fp32 out.
+  static MlpParams critic_head(const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3,
+                               const void* b3, int d_act, const float* act, float* q) {
+    MlpParams p{W1p, b1, W2, b2, W3, b3, HeadKind::kGaussian};
+    p.critic = true;
+    p.d_act = d_act;
+    p.act = act;
+    p.hq = HeadQ{q};
+    return p;
+  }
 
   // A multi-discrete head: the greedy one (logits and/or actions, ranked without noise) or the sampled one, both in
   // the kSample instantiations.
@@ -1475,12 +1588,14 @@ struct MlpParams {
 
 // Rows [r0, r0 + rows) of a call: the hidden layers h1 = relu(a1 · W1ᵀ (+ b1)) and h2 = relu(h1 · W2ᵀ (+ b2)), then
 // the head of p.kind into `out` (the call's outputs, from row 0) from h2 in the smallest tile that holds its d_out
-// columns (2·d_out for a state-dependent Gaussian head), one more with a value head.  `consumed`, unless null, is
-// recorded once layer 1 has read a1.
+// columns (2·d_out for a state-dependent Gaussian head), one more with a value head.  A critic's layer 1 reads
+// `tile` (the chunk's actions) as its last K block.  `consumed`, unless null, is recorded once layer 1 has read a1.
 static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const HeadEps& eg, const HeadEval& ev,
-                     const void* a1, void* h1, void* h2, size_t r0, size_t rows, int d_in, int d_hidden, int d_out,
-                     cudaEvent_t consumed, cudaStream_t st) {
-  int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden, d_in, st);
+                     const void* a1, const void* tile, void* h1, void* h2, size_t r0, size_t rows, int d_in,
+                     int d_hidden, int d_out, cudaEvent_t consumed, cudaStream_t st) {
+  int rc = launch_layer<256, HeadKind::kHidden>(dev, a1, p.W1, p.b1, HeadOut{h1}, rows, d_hidden,
+                                                d_in + (p.critic ? kMlpBlockK : 0), st, HeadStd{}, HeadEps{},
+                                                HeadEval{}, HeadQ{}, p.critic ? tile : nullptr);
   if (rc) return rc;
   if (consumed) KTB_CK(cudaEventRecord(consumed, st));
   rc = launch_layer<256, HeadKind::kHidden>(dev, h1, p.W2, p.b2, HeadOut{h2}, rows, d_hidden, d_hidden, st);
@@ -1491,7 +1606,7 @@ static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const Head
   const int n = (p.std.state ? 2 * d_out : d_out) + (int)p.valued;
   const size_t per_row = ev.gauss_actions ? (size_t)d_out : (size_t)std::max(out.groups.n, 1);   // given actions
   return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std, eg.from_row(r0),
-              ev.from_row(r0, per_row));
+              ev.from_row(r0, per_row), p.hq.from_row(r0));
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -1517,6 +1632,8 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
           KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
+        if (p.critic)   // a critic's act and outputs: checked by mlp_run after every other check
+          break;
         if (p.std.det)   // a deterministic actor stores its actions only
           KTB_REQUIRE(o.gauss_actions, KTB_ERR_ARG, "%s: actions is required", fn);
         else if (p.std.state)   // a state-dependent head reads its log-std from the head's own columns
@@ -1552,8 +1669,8 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //           ready[c] = seq in this rank's control block `ctrl`; layer 1 of chunk c waits in-stream for it, and the
 //           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A masked head reads
 //           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows), and
-//           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in, and an evaluating head its rows' given
-//           actions from taken_offset bytes in.
+//           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in, an evaluating head its rows' given
+//           actions from taken_offset bytes in, and a critic its rows' actions (fp32) from act_offset bytes in.
 // The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
@@ -1567,6 +1684,7 @@ struct MlpFeed {
   size_t mask_offset = 0;
   size_t epsilon_offset = 0;
   size_t taken_offset = 0;
+  size_t act_offset = 0;
 
   static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
   static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
@@ -1588,6 +1706,11 @@ struct MlpFeed {
     f.taken_offset = off;
     return f;
   }
+  MlpFeed with_act_offset(size_t off) const {
+    MlpFeed f = *this;
+    f.act_offset = off;
+    return f;
+  }
 };
 
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
@@ -1603,6 +1726,9 @@ struct MlpFeed {
 // own checks come after every check of its counterpart and its nvec: (skipped for an empty call) taken, log_probs,
 // entropy non-null and aligned, then its taken region in the pushed forms.  A deterministic entry's actions are checked
 // with the head (mlp_check), its noise and noise_clip (>= 0, not NaN; skipped for an empty call) after every check.
+// A critic entry runs every check of ktb_mlp_bf16_policy at d_out = 1 (a twin's second critic's weights and biases
+// checked as the first's, right after them), then d_act in [1, 64], then (skipped for an empty call) act and its
+// outputs non-null and 4-byte aligned, then its action region in the pushed forms.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1624,6 +1750,14 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
               "%s: chunk_rows=%zu must be a positive multiple of %d", fn, f.chunk_rows, kMlpBlockM);
   rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, f.in, scratch, f.stage);
   if (rc) return rc;
+  if (p.twin) {
+    const MlpParams& t = *p.twin;
+    KTB_REQUIRE(t.W1 && t.W2 && t.W3, KTB_ERR_ARG, "%s: null argument", fn);
+    KTB_REQUIRE(M == 0 || (((uintptr_t)t.b1 | (uintptr_t)t.b2 | (uintptr_t)t.b3) & 1) == 0, KTB_ERR_ARG,
+                "%s: logits and biases must be 2-byte aligned", fn);
+    KTB_REQUIRE((((uintptr_t)t.W1 | (uintptr_t)t.W2 | (uintptr_t)t.W3) & 15) == 0, KTB_ERR_ARG,
+                "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
+  }
   if (f.pushed) {
     const size_t n_chunks = (M + f.chunk_rows - 1) / f.chunk_rows;
     KTB_REQUIRE(n_chunks <= KTB_PUSH_MAX_CHUNKS, KTB_ERR_ARG, "%s: %zu chunks exceed %d", fn, n_chunks,
@@ -1675,6 +1809,25 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     KTB_REQUIRE(s == s && s >= 0.f, KTB_ERR_ARG, "%s: noise=%g must be >= 0, not NaN", fn, (double)s);
     KTB_REQUIRE(c == c && c >= 0.f, KTB_ERR_ARG, "%s: noise_clip=%g must be >= 0, not NaN", fn, (double)c);
   }
+  if (p.critic) {
+    KTB_REQUIRE(p.d_act >= 1, KTB_ERR_ARG, "%s: d_act=%d must be positive", fn, p.d_act);
+    KTB_REQUIRE(p.d_act <= kMlpBlockK, KTB_ERR_UNSUPPORTED, "%s: d_act=%d (actions up to %d wide)", fn, p.d_act,
+                kMlpBlockK);
+    if (M > 0) {
+      const HeadQ& q2 = p.twin ? p.twin->hq : HeadQ{};
+      KTB_REQUIRE((p.act || f.pushed) && p.hq.q && (!p.twin || (q2.q && q2.q_min)), KTB_ERR_ARG,
+                  p.twin ? "%s: act, q1, q2 and q_min are required" : "%s: act and q are required", fn);
+      KTB_REQUIRE((((uintptr_t)p.act | (uintptr_t)p.hq.q | (uintptr_t)q2.q | (uintptr_t)q2.q_min) & 3) == 0,
+                  KTB_ERR_ARG, "%s: act and the outputs must be 4-byte aligned", fn);
+    }
+    if (f.pushed) {
+      const size_t off = f.act_offset, n = M * (size_t)p.d_act * 4;
+      KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: act_offset=%zu overlaps the rows", fn, off);
+      KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG, "%s: act_offset=%zu + act exceeds stage_stride",
+                  fn, off);
+      KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: act_offset=%zu must be a multiple of 4", fn, off);
+    }
+  }
   HeadGroups groups = p.out.groups;
   if (p.grouped && M > 0) {
     KTB_REQUIRE(p.nvec, KTB_ERR_ARG, "%s: null nvec", fn);
@@ -1718,6 +1871,7 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   const size_t chunk = std::min(f.chunk_rows, M);
   __nv_bfloat16* h1 = static_cast<__nv_bfloat16*>(scratch);
   __nv_bfloat16* h2 = h1 + chunk * (size_t)d_hidden;
+  __nv_bfloat16* tile = h2 + chunk * (size_t)d_hidden;   // a critic's action tile [chunk, 64]
   // the call's rows: obs, or this call's staging half (the pull forms have seq = stride = 0)
   const __nv_bfloat16* x =
       reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride);
@@ -1735,6 +1889,9 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     else
       ev.gauss_actions = reinterpret_cast<const float*>(t);
   }
+  const float* act = p.critic && f.pushed
+                         ? reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(x) + f.act_offset)
+                         : p.act;
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
   cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
@@ -1782,9 +1939,16 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       KTB_CK(cudaStreamWaitEvent(st, evs[1 + b], 0));
       a1 = dstb;
     }
-    // evs[3..4] are null unless staged
-    rc = mlp_chunk(dev, p, out, eg, ev, a1, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)], st);
-    if (rc) return rc;
+    if (p.critic) {   // packed once per chunk; a twin's two chains both read it
+      rc = launch_action_tile(act + r0 * p.d_act, p.d_act, tile, rows, st);
+      if (rc) return rc;
+    }
+    // evs[3..4] are null unless staged; a twin records `consumed` again after its second layer 1
+    for (const MlpParams* q = &p; q != nullptr; q = q->twin) {
+      rc = mlp_chunk(dev, *q, out, eg, ev, a1, tile, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)],
+                     st);
+      if (rc) return rc;
+    }
   }
   if (!f.pushed) return KTB_OK;
   // everything before it on `st`, the peer-stored outputs included, is visible system-wide before the root sees
@@ -1801,6 +1965,11 @@ extern "C" {
 size_t ktb_mlp_scratch_bytes(size_t M, int d_hidden) {
   const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
   return 2 * rows * (size_t)d_hidden * 2;
+}
+
+size_t ktb_mlp_critic_scratch_bytes(size_t M, int d_hidden) {
+  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
+  return ktb_mlp_scratch_bytes(M, d_hidden) + rows * (size_t)kMlpBlockK * 2;
 }
 
 size_t ktb_mlp_stage_bytes(size_t M, int d_in) {
@@ -2469,6 +2638,57 @@ int ktb_mlp_bf16_policy_deterministic_pushed(int dev, const void* stage_local, s
   return mlp_run("ktb_mlp_bf16_policy_deterministic_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq), scratch,
                  stream);
+}
+
+int ktb_mlp_bf16_critic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act, const void* W1p,
+                        const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                        const float* act, float* q, void* scratch, void* stage, uintptr_t stream) {
+  const MlpParams p = MlpParams::critic_head(W1p, b1, W2, b2, W3, b3, d_act, act, q);
+  return mlp_run("ktb_mlp_bf16_critic", dev, M, d_in, d_hidden, 1, p, MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_critic_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
+                               int d_act, const void* W1p, const void* b1, const void* W2, const void* b2,
+                               const void* W3, const void* b3, size_t act_offset, float* q, void* scratch,
+                               void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                               unsigned long long seq, uintptr_t stream) {
+  const MlpParams p = MlpParams::critic_head(W1p, b1, W2, b2, W3, b3, d_act, nullptr, q);
+  return mlp_run("ktb_mlp_bf16_critic_pushed", dev, M, d_in, d_hidden, 1, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_act_offset(act_offset),
+                 scratch, stream);
+}
+
+int ktb_mlp_bf16_critic_twin(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act, const void* W1p,
+                             const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                             const void* W1p_2, const void* b1_2, const void* W2_2, const void* b2_2,
+                             const void* W3_2, const void* b3_2, const float* act, float* q1, float* q2, float* q_min,
+                             void* scratch, void* stage, uintptr_t stream) {
+  MlpParams second = MlpParams::critic_head(W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2, d_act, act, q2);
+  second.hq.q_other = q1;
+  second.hq.q_min = q_min;
+  MlpParams p = MlpParams::critic_head(W1p, b1, W2, b2, W3, b3, d_act, act, q1);
+  p.twin = &second;
+  return mlp_run("ktb_mlp_bf16_critic_twin", dev, M, d_in, d_hidden, 1, p, MlpFeed::pull(obs, stage), scratch,
+                 stream);
+}
+
+int ktb_mlp_bf16_critic_twin_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                    int d_hidden, int d_act, const void* W1p, const void* b1, const void* W2,
+                                    const void* b2, const void* W3, const void* b3, const void* W1p_2,
+                                    const void* b1_2, const void* W2_2, const void* b2_2, const void* W3_2,
+                                    const void* b3_2, size_t act_offset, float* q1, float* q2, float* q_min,
+                                    void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
+                                    unsigned long long seq, uintptr_t stream) {
+  MlpParams second = MlpParams::critic_head(W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2, d_act, nullptr, q2);
+  second.hq.q_other = q1;
+  second.hq.q_min = q_min;
+  MlpParams p = MlpParams::critic_head(W1p, b1, W2, b2, W3, b3, d_act, nullptr, q1);
+  p.twin = &second;
+  return mlp_run("ktb_mlp_bf16_critic_twin_pushed", dev, M, d_in, d_hidden, 1, p,
+                 MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                     .with_act_offset(act_offset),
+                 scratch, stream);
 }
 
 }  // extern "C"

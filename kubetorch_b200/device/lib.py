@@ -207,6 +207,14 @@ for _masked in ("", "_masked"):
 for _form, _at in (("", 18), ("_pushed", 19)):
     _restype, _args = _SIGNATURES["ktb_mlp_bf16_policy_gaussian_state" + _form]
     _SIGNATURES["ktb_mlp_bf16_policy_deterministic" + _form] = (_restype, _args[:_at] + _args[_at + 1:])
+# The _critic entries: ktb_mlp_bf16_policy's arguments up to b3 (d_act in place of d_out, W1p for W1), the second
+# critic's six after them in the _twin forms, then act (act_offset in the pushed forms) and q, or q1, q2 and q_min.
+_SIGNATURES["ktb_mlp_critic_scratch_bytes"] = (c_size_t, [c_size_t, c_int])
+for _twin in ("", "_twin"):
+    for _form, _act, _at in (("", c_void_p, 12), ("_pushed", c_size_t, 13)):
+        _args = _SIGNATURES["ktb_mlp_bf16_policy" + _form][1]
+        _head_args = [c_void_p] * (6 if _twin else 0) + [_act] + [c_void_p] * (3 if _twin else 1)
+        _SIGNATURES["ktb_mlp_bf16_critic" + _twin + _form] = (c_int, _args[:_at] + _head_args + _args[_at + 2:])
 _SIGNATURES["ktb_push_scatter_ce_sides"] = (
     c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
                                                          ctypes.c_ulonglong, c_uintptr])

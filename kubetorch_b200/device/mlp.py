@@ -6,7 +6,8 @@ mask), the _value forms of the sampled heads (a critic's state value on the same
 the greedy and sampled heads (one categorical per group of columns), the _gaussian_state forms (a per-row log-std
 head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network's ε-greedy actor), the _evaluate
 and _gaussian_evaluate forms (the log-probability and entropy of given actions), the _deterministic forms (DDPG's and
-TD3's actor: tanh actions with clipped Gaussian noise) and their scatter→exec→gather form."""
+TD3's actor: tanh actions with clipped Gaussian noise), the _critic forms (Q(s, a) critics with the actions fed into
+layer 1, single or twin) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -26,13 +27,16 @@ _scratch = {}
 _stage = {}
 _weight_cache = {}
 _stacked_heads = {}   # (device, id(w3)) -> [weakref to w3, stamp of w3 / b3 / wv / bv / w_ls / b_ls, W3, b3]
+_padded_w1s = {}      # (device, id(w1)) -> [weakref to w1, stamp of w1 and d_in, W1p]
 _pool = None
 
 
-def pushed_scratch_bytes(M: int, d_hidden: int, chunk_rows: int) -> int:
-    """Scratch of ktb_mlp_bf16_policy_pushed: two hidden activations of min(chunk_rows, M) rows.  It follows the pushed form's
-    own chunk_rows, not the tuning chunk that ktb_mlp_scratch_bytes uses for the pull forms."""
-    return 2 * min(int(chunk_rows), int(M)) * int(d_hidden) * 2
+def pushed_scratch_bytes(M: int, d_hidden: int, chunk_rows: int, critic: bool = False) -> int:
+    """Scratch of ktb_mlp_bf16_policy_pushed: two hidden activations of min(chunk_rows, M) rows, and with `critic` the
+    action tile [rows, 64] bf16 of the _critic entries.  It follows the pushed form's own chunk_rows, not the tuning
+    chunk that ktb_mlp_scratch_bytes uses for the pull forms."""
+    rows = min(int(chunk_rows), int(M))
+    return 2 * rows * int(d_hidden) * 2 + (rows * 64 * 2 if critic else 0)
 
 
 def _cached_buffer(cache: dict, key, dev: int, nbytes: int) -> torch.Tensor:
@@ -43,8 +47,10 @@ def _cached_buffer(cache: dict, key, dev: int, nbytes: int) -> torch.Tensor:
     return buf
 
 
-def _scratch_for(dev: int, M: int, d_hidden: int) -> torch.Tensor:
-    return _cached_buffer(_scratch, dev, dev, L.load().ktb_mlp_scratch_bytes(M, d_hidden))
+def _scratch_for(dev: int, M: int, d_hidden: int, critic: bool = False) -> torch.Tensor:
+    lib = L.load()
+    nbytes = lib.ktb_mlp_critic_scratch_bytes(M, d_hidden) if critic else lib.ktb_mlp_scratch_bytes(M, d_hidden)
+    return _cached_buffer(_scratch, dev, dev, nbytes)
 
 
 def _stage_for(dev: int, M: int, d_in: int) -> torch.Tensor:
@@ -198,9 +204,78 @@ def _check_deterministic(seed, noise, noise_clip, squash) -> None:
         raise ValueError(f"squash must be True or False, got {squash!r}")
 
 
+MAX_D_ACT = 64   # a critic's actions fill one 64-wide K block of layer 1
+
+
+def _check_critic(w1, w2, w3, biases, obs, action, twin) -> None:
+    """_check_policy's checks of output="critic", after its refusals, in this order: w3 one row; action given, an fp32
+    [M, d_act] CUDA tensor, contiguous, on the device of obs [M, d_in], with 1 <= d_act <= 64; w1 [d_hidden, d_in +
+    d_act]; then twin = (w1, b1, w2, b2, w3, b3) of the second critic: six entries, biases given exactly as the first
+    critic's, each weight a contiguous CUDA bfloat16 tensor of the first's shape on the device of w1."""
+    if w3.shape[0] != 1:
+        raise ValueError(f"d_out={w3.shape[0]}: a critic's w3 is [1, d_hidden] (one Q-value per row)")
+    if action is None:
+        raise ValueError('action is required with output="critic": the fp32 actions [M, d_act] it evaluates')
+    if not isinstance(action, torch.Tensor) or action.dtype != torch.float32 or action.dim() != 2:
+        raise ValueError("action must be a 2-D float32 tensor [M, d_act]")
+    if not isinstance(obs, torch.Tensor):
+        raise ValueError("action is checked against obs: pass the obs [M, d_in] it goes with")
+    M, d_in = obs.shape
+    d_act = action.shape[1]
+    if action.shape[0] != M:
+        raise ValueError(f"action must have {M} rows (one per observation), got {tuple(action.shape)}")
+    if not 1 <= d_act <= MAX_D_ACT:
+        raise ValueError(f"d_act={d_act}: a critic takes 1 to {MAX_D_ACT} action columns (one K block of layer 1)")
+    if not action.is_contiguous():
+        raise ValueError("action must be contiguous")
+    if not action.is_cuda or action.device != obs.device:
+        raise ValueError(f"action must be a CUDA tensor on the device of obs ({obs.device}), got {action.device}")
+    d_hidden = w1.shape[0]
+    if tuple(w1.shape) != (d_hidden, d_in + d_act):
+        raise ValueError(f"w1 must be [d_hidden, d_in + d_act] = [{d_hidden}, {d_in + d_act}] (the critic's layer 1 "
+                         f"over torch.cat([obs, action], -1)), got {tuple(w1.shape)}")
+    if twin is None:
+        return
+    if not isinstance(twin, (tuple, list)) or len(twin) != 6:
+        raise ValueError("twin must be (w1, b1, w2, b2, w3, b3) of the second critic (biases None without biases)")
+    for name, t, mine in zip(("b1", "b2", "b3"), twin[1::2], biases):
+        if (t is None) != (mine is None):
+            raise ValueError(f"twin: {name} is given exactly when the first critic's is")
+    for name, t, like in zip(("w1", "w2", "w3", "b1", "b2", "b3"), (*twin[0::2], *twin[1::2]), (w1, w2, w3, *biases)):
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16 or tuple(t.shape) != tuple(like.shape) \
+                or not t.is_contiguous() or not t.is_cuda or t.device != w1.device:
+            raise ValueError(f"twin: {name} must be a contiguous CUDA bfloat16 tensor of shape {tuple(like.shape)} on "
+                             f"the device of w1 ({w1.device})")
+
+
+def _padded_w1(w1: torch.Tensor, d_in: int) -> torch.Tensor:
+    """W1p = [w1 | 0] [d_hidden, d_in + 64] of a critic's layer-1 weight w1 [d_hidden, d_in + d_act], on the device of
+    w1: the action columns padded with zero columns to one 64-wide K block.  One entry per (device, w1) is kept, and
+    rewritten in place when w1 has a new data_ptr or _version: target critics are Polyak-updated in place every step.
+    Rewriting in place bumps W1p's own _version, so _weights_on copies the new weight to other devices."""
+    stamp = (w1.data_ptr(), w1._version, d_in)
+    key = (w1.device.index, id(w1))
+    entry = _padded_w1s.get(key)
+    if entry is None or entry[0]() is not w1:
+        for k, e in list(_padded_w1s.items()):   # weights that are gone, or a new w1 that reuses an old id
+            if e[0]() is None or k == key:
+                del _padded_w1s[k]
+        entry = _padded_w1s[key] = [weakref.ref(w1), None, None]
+    if entry[1] != stamp:
+        shape = (w1.shape[0], d_in + MAX_D_ACT)
+        if entry[2] is None or tuple(entry[2].shape) != shape:
+            entry[2] = torch.zeros(shape, dtype=w1.dtype, device=w1.device)
+        entry[2][:, :w1.shape[1]].copy_(w1)
+        entry[2][:, w1.shape[1]:].zero_()
+        entry[1] = stamp
+    return entry[2]
+
+
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
                   nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None, noise=None,
-                  noise_clip=None) -> None:
+                  noise_clip=None, action=None, twin=None, w2=None) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
     (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
@@ -215,9 +290,21 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     "gaussian_evaluate" take the actions to score, `taken` (_check_taken), refused with any other output; they refuse
     a seed, epsilon, squash, log_std_bounds and a log_std pair, and "gaussian_evaluate" a mask.  output="deterministic"
     takes noise, noise_clip, a seed and squash (_check_deterministic) and refuses mask, value, nvec, log_std,
-    log_std_bounds, epsilon and taken; noise and noise_clip are refused with any other output."""
+    log_std_bounds, epsilon and taken; noise and noise_clip are refused with any other output.  output="critic" takes
+    the action and an optional twin (_check_critic) and refuses seed, mask, value, nvec, log_std, log_std_bounds,
+    squash, epsilon, taken, noise and noise_clip; action and twin are refused with any other output."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
+    if output == "critic":
+        for name, v in (("seed", seed), ("mask", mask), ("value", value), ("nvec", nvec), ("log_std", log_std),
+                        ("log_std_bounds", log_std_bounds), ("squash", squash), ("epsilon", epsilon),
+                        ("taken", taken), ("noise", noise), ("noise_clip", noise_clip)):
+            if v is not None:
+                raise ValueError(f'{name} is not an argument of output="critic": a critic evaluates Q(s, a) of the '
+                                 f'given action and takes action and twin only')
+        _check_critic(w1, w2, w3, biases, obs, action, twin)
+    elif action is not None or twin is not None:
+        raise ValueError(f'action and twin are arguments of output="critic", not of output={output!r}')
     det = output == "deterministic"
     if det:
         for name, v in (("mask", mask), ("value", value), ("nvec", nvec), ("log_std", log_std),
@@ -324,12 +411,13 @@ def _stacked_head(w3, b3, wv=None, bv=None, w_ls=None, b_ls=None) -> Tuple[torch
     return entry[2], entry[3]
 
 
-def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False, nvec=None):
+def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, valued=False, nvec=None, twin=False):
     """(logits, actions, log_probs, values) of `M` rows as `output` writes them: bf16 logits [M, d_out]; int64 actions
     [M], [M, len(nvec)] with nvec, or fp32 [M, d_out] with "gaussian"; fp32 log_probs [M]; with `valued`, fp32 values
     [M].  "deterministic" writes fp32 actions [M, d_out] only.  With "epsilon_greedy" the last two slots hold its fp32
     q [M] and q_max [M]; with "evaluate" and
-    "gaussian_evaluate" the actions slot holds the fp32 entropy [M].  A buffer the mode does not
+    "gaussian_evaluate" the actions slot holds the fp32 entropy [M].  With "critic" the logits slot holds the fp32 q
+    [M] (q1 of a `twin`), and a twin's q2 and q_min ride in the actions and log_probs slots.  A buffer the mode does not
     write is None, a missing one is allocated on `device` and a given one is
     registered with the library (ops.ensure_init); given multi-discrete actions must be [M, len(nvec)]."""
     def buf(t, shape, dtype):
@@ -339,6 +427,9 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
         return t
 
     gaussian = output in ("gaussian", "deterministic")
+    if output == "critic":
+        return buf(logits, (M,), torch.float32), buf(actions, (M,), torch.float32) if twin else None, \
+            buf(log_probs, (M,), torch.float32) if twin else None, None
     if output in EVALUATE_OUTPUTS:
         return None, buf(actions, (M,), torch.float32), buf(log_probs, (M,), torch.float32), \
             buf(values, (M,), torch.float32) if valued else None
@@ -354,7 +445,7 @@ def _outputs(output, M, d_out, device, logits, actions, log_probs, values=None, 
 
 
 def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, pushed=False, mask=None, values=None,
-          nvec=None, std=None, epsilon=None, taken=None, det=None):
+          nvec=None, std=None, epsilon=None, taken=None, det=None, act=None, twin=None):
     """The C entry that computes `output` (its _pushed form with `pushed`) and the head's arguments of that entry, the
     pointers as ptr(tensor) gives them.  `mask`, unless None, picks the _masked entry and is its mask argument: the
     mask's address in the pull forms, its offset in the staging half in the pushed forms.  `values`, unless None,
@@ -364,9 +455,15 @@ def _head(output, logits, actions, log_probs, seed, row_base, log_std, ptr, push
     "epsilon_greedy", `epsilon` is ε's address (pull forms) or its offset in the staging half (pushed forms), and
     log_probs and values are its q and q_max buffers.  With "evaluate" and "gaussian_evaluate", `taken` is the given
     actions' address or offset likewise, and `actions` is the entropy buffer.  With "deterministic", `det` is the
-    entry's (noise, noise_clip, squash) (_det); a noise-free call passes seed 0, which draws nothing."""
+    entry's (noise, noise_clip, squash) (_det); a noise-free call passes seed 0, which draws nothing.  With "critic",
+    `act` is the actions' address or offset likewise, `twin` (unless None) the six weight and bias pointers of the
+    second critic, which pick the _twin entry, and logits (q1), actions (q2) and log_probs (q_min) its outputs."""
     valued = () if values is None else (ptr(values),)
     pushed_suffix = "_pushed" if pushed else ""
+    if output == "critic":
+        pair = twin is not None
+        return "ktb_mlp_bf16_critic" + ("_twin" if pair else "") + pushed_suffix, \
+            (*(twin or ()), act, ptr(logits), *((ptr(actions), ptr(log_probs)) if pair else ()))
     if output == "deterministic":
         return "ktb_mlp_bf16_policy_deterministic" + pushed_suffix, (*det, seed or 0, row_base, ptr(actions))
     if output == "gaussian_evaluate":
@@ -430,6 +527,8 @@ def _result(output, logits, actions, log_probs, values=None):
         return (log_probs, actions) if values is None else (log_probs, actions, values)
     if output == "deterministic":
         return actions
+    if output == "critic":   # q, or (q1, q2, q_min) of a twin
+        return logits if actions is None else (logits, actions, log_probs)
     return (actions, log_probs) if values is None else (actions, log_probs, values)
 
 
@@ -444,7 +543,9 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
                 epsilon=None, q: Optional[torch.Tensor] = None, q_max: Optional[torch.Tensor] = None,
                 taken: Optional[torch.Tensor] = None, entropy: Optional[torch.Tensor] = None,
-                noise: Optional[float] = None, noise_clip: Optional[float] = None, _stacked: bool = False):
+                noise: Optional[float] = None, noise_clip: Optional[float] = None,
+                action: Optional[torch.Tensor] = None, twin: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                q2: Optional[torch.Tensor] = None, q_min: Optional[torch.Tensor] = None, _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -493,9 +594,17 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     `seed`) t + (σ·normal_noise(seed, row_offset, M, d_out)).clamp(-noise_clip, noise_clip), noise_clip >= 0 defaulting
     to +inf; then clamp(-1, 1) when squashed (NaN stays NaN).  σ = 0.1 is exploration, σ = 0.2 with noise_clip = 0.5
     TD3's target policy smoothing, no noise the deterministic mode of a tanh-squashed or an unsquashed policy.
-    `_stacked` (internal, from
+    output="critic" (SAC's and TD3's Q(s, a), forward only) returns fp32 q[M], into `q` when given: with `action` an
+    fp32 [M, d_act] tensor on the device of obs (1 <= d_act <= 64), w1 the critic's [d_hidden, d_in + d_act] and w3
+    its [1, d_hidden], q = F.linear(h2, w3, b3).float() over x = torch.cat([obs, action.to(torch.bfloat16)], -1), every
+    layer rounded as above.  With `twin` = (w1, b1, w2, b2, w3, b3) of a second critic (biases given exactly as the
+    first's) it returns (q1, q2, q_min), into `q`, `q2` and `q_min` when given: q_min = torch.minimum(q1, q2) (NaN
+    when either is, q1 on ties).  Layer 1 runs over w1 padded with zero columns to d_in + 64 (_padded_w1, kept per
+    device and weight) and reads the actions, packed to bf16 once per row chunk, as its last K block; the
+    observations are never copied.  `_stacked` (internal, from
     mlp_scatter_gather, which checked the call): w3 and biases[2] are
-    already the head the C entry takes (stacked with a value head, interleaved with a log-std head)."""
+    already the head the C entry takes (stacked with a value head, interleaved with a log-std head), and a critic's
+    w1 (and its twin's) is already W1p."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -503,11 +612,13 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     ops.ensure_init({dev, obs.device.index})
     M, d_in = obs.shape
     d_hidden, d_out = w1.shape[0], w3.shape[0]
-    if w1.shape != (d_hidden, d_in) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
+    critic = output == "critic"
+    d_w1 = w1.shape[1] if critic else d_in   # a critic's layer 1 also reads the actions: checked by _check_critic
+    if w1.shape != (d_hidden, d_w1) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
     if not _stacked:
         _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon,
-                      taken, noise, noise_clip)
+                      taken, noise, noise_clip, action, twin, w2)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     valued = value is not None or (_stacked and values is not None)
     if _stacked:
@@ -520,9 +631,17 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
         log_probs, values = q, q_max
     if output in EVALUATE_OUTPUTS:   # the entropy rides in the actions slot
         actions = entropy
+    if critic:   # q (or q1), q2 and q_min ride in the logits, actions and log_probs slots
+        out, actions, log_probs = q, q2, q_min
+        d_out = action.shape[1]   # the C entry's d_act
     out, actions, log_probs, values = _outputs(output, M, d_out, f"cuda:{dev}", out, actions, log_probs, values, valued,
-                                               nvec)
+                                               nvec, twin is not None)
     s = stream if stream is not None else torch.cuda.current_stream(dev)
+    if critic and not _stacked:
+        with torch.cuda.stream(s):   # a rewrite of W1p is ordered after earlier calls on s
+            w1 = _padded_w1(w1, d_in)
+            if twin is not None:
+                twin = (_padded_w1(twin[0], d_in), *twin[1:])
     if eps and not isinstance(epsilon, torch.Tensor):
         with torch.cuda.stream(s):   # freed after the call, its memory is reused in s's order, after the kernel
             epsilon = torch.full((M,), float(epsilon), dtype=torch.float32, device=f"cuda:{dev}")
@@ -536,9 +655,10 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     entry, head = _head(output, out, actions, log_probs, seed, row_offset, log_std, ptr,
                         mask=None if mask is None else ptr(mask), values=values, nvec=nvec, std=std,
                         epsilon=ptr(epsilon) if eps else None, taken=ptr(taken),
-                        det=_det(noise, noise_clip, squash) if output == "deterministic" else None)
+                        det=_det(noise, noise_clip, squash) if output == "deterministic" else None,
+                        act=ptr(action), twin=None if twin is None else tuple(ptr(t) for t in twin))
     L.call(entry, dev, obs.data_ptr(), M, d_in, d_hidden, d_out, w1.data_ptr(), ptr(biases[0]), w2.data_ptr(),
-           ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden).data_ptr(),
+           ptr(biases[1]), w3.data_ptr(), ptr(biases[2]), *head, _scratch_for(dev, M, d_hidden, critic).data_ptr(),
            _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
     return _result(output, out, actions, log_probs, values)
 
@@ -569,7 +689,7 @@ _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pu
 
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
                                seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None,
-                               epsilon=None, taken=None, det=None) -> None:
+                               epsilon=None, taken=None, det=None, action=None, twin=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
     actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
@@ -587,14 +707,20 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     its q and q_max.  With output="evaluate" or "gaussian_evaluate", `taken` (on the root) is pushed with the rows the
     same way, each staging half rows | mask | taken with taken's offset rounded up to 8 bytes, and actions_root is the
     entropy.  With output="deterministic", `det` is the call's dict(noise=, noise_clip=, squash=), and each staging
-    half holds the rows only."""
+    half holds the rows only.  With output="critic", `action` (fp32 [M, d_act] on the root) is pushed with the rows,
+    each staging half rows | action with the action 256-byte aligned, weights[dev] holds W1p in place of w1, twin[dev]
+    (unless None) the second critic's (W1p, b1, W2, b2, W3, b3), and out_root / actions_root / log_probs_root are q
+    (q1), q2 and q_min."""
     root, n, key = devs[0], len(devs), tuple(devs)
+    critic = output == "critic"
     valued = values_root is not None and epsilon is None   # an ε-greedy head's values_root is its q_max
     d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
-    d_out = (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
+    d_out = action.shape[1] if critic else (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
     rows = max(e - b for b, e in bounds)
     mask_offset = (rows * d_in * 2 + 255) // 256 * 256
     stage_bytes = rows * d_in * 2 if mask is None else mask_offset + rows * d_out
+    if critic:   # the actions sit where a mask would
+        stage_bytes = mask_offset + rows * d_out * 4
     eps_offset = None
     if epsilon is not None:
         eps_offset = mask_offset if mask is None else (mask_offset + rows * d_out + 255) // 256 * 256
@@ -614,7 +740,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         raise
     # scratch per rank, not per device: ranks sharing a device must not share one, nor the root's own shard on the
     # side stream
-    scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS)
+    scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS, critic)
     scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], scratch_bytes) for r in range(1, n)]
     streams = [ops.current_stream_handle(d) for d in devs]
     bufs = (out_root, actions_root, log_probs_root, values_root)
@@ -630,11 +756,14 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
                     **(det or dict(squash=None if std is None else bool(std[2]))),
                     **({} if epsilon is None else dict(epsilon=epsilon[b0:e0], q=log_probs, q_max=values)),
                     **({} if taken is None else dict(taken=taken[b0:e0], entropy=actions)),
-                    _stacked=valued or std is not None)
+                    **({} if not critic else dict(action=action[b0:e0], twin=None if twin is None else twin[root],
+                                                  q=logits, q2=actions, q_min=log_probs)),
+                    _stacked=valued or std is not None or critic)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
-    if epsilon is not None or taken is not None:
+    if epsilon is not None or taken is not None or critic:
         last = (epsilon.data_ptr(), 4, eps_offset) if epsilon is not None else \
+            (action.data_ptr(), 4 * d_out, mask_offset) if critic else \
             (taken.data_ptr(), taken_row, taken_offset)
         sides = ([] if mask is None else [(mask.data_ptr(), d_out, mask_offset)]) + [last]
         src, row_bytes, offsets = zip(*sides)
@@ -656,7 +785,9 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         entry, head = _head(output, logits, actions, log_probs, seed, b,
                             None if log_std is None else log_std[devs[r]], ptr, pushed=True,
                             mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std,
-                            epsilon=eps_offset, taken=taken_offset, det=None if det is None else _det(**det))
+                            epsilon=eps_offset, taken=taken_offset, det=None if det is None else _det(**det),
+                            act=mask_offset if critic else None,
+                            twin=None if twin is None else tuple(ptr(t) for t in twin[devs[r]]))
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -675,7 +806,10 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        log_std_bounds: Optional[Tuple[float, float]] = None, squash: Optional[bool] = None,
                        epsilon=None, taken: Optional[torch.Tensor] = None,
                        entropy_root: Optional[torch.Tensor] = None, noise: Optional[float] = None,
-                       noise_clip: Optional[float] = None) -> list:
+                       noise_clip: Optional[float] = None, action: Optional[torch.Tensor] = None,
+                       twin: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                       q_root: Optional[torch.Tensor] = None, q2_root: Optional[torch.Tensor] = None,
+                       q_min_root: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -695,13 +829,20 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     a value head, into `log_probs_root`, `entropy_root` and `values_root` when given; each rank reads its rows of taken
     in place on the pull form, and the push form pushes them with the rows.  output="deterministic" with `noise`,
     `noise_clip`, `seed` and `squash` as in mlp_forward returns fp32 actions [rows, d_out] views of `actions_root`;
-    each rank draws the noise of its shard's global rows."""
+    each rank draws the noise of its shard's global rows.  output="critic" with `action` (fp32 [M, d_act] on the root)
+    and `twin` as in mlp_forward returns fp32 q [rows] views of `q_root`, or (q1, q2, q_min) triples of views of
+    `q_root`, `q2_root` and `q_min_root` with a twin; each rank reads its rows of action in place on the pull form, and
+    the push form pushes them with the rows.  W1p (and the twin's) is built on the root and copied to the other devices
+    like the other weights, again after an in-place update of w1."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
     _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon,
-                  taken, noise, noise_clip)
+                  taken, noise, noise_clip, action, twin, w2)
+    critic = output == "critic"
+    if critic:   # q (or q1), q2 and q_min ride in the logits, actions and log_probs slots
+        out_root, actions_root, log_probs_root = q_root, q2_root, q_min_root
     det = dict(noise=noise, noise_clip=noise_clip, squash=squash) if output == "deterministic" else None
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
@@ -711,11 +852,17 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     if taken is not None:   # the entropy rides in the actions slot
         actions_root = entropy_root
     bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
-                    valued, nvec)
+                    valued, nvec, twin is not None)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     if valued or std is not None:
         w3, b3 = _stacked_head(w3, biases[2], *(value or (None, None)), *(log_std if std is not None else ()))
         biases = (biases[0], biases[1], b3)
+    twins = None
+    if critic:
+        w1 = _padded_w1(w1, obs_root.shape[1])
+        if twin is not None:
+            twin = (_padded_w1(twin[0], obs_root.shape[1]), *twin[1:])
+            twins = {dev: tuple(_weights_on(dev, twin)) for dev in set(devs)}
     root_stream = torch.cuda.current_stream(root)
     ready = torch.cuda.Event()
     ready.record(root_stream)
@@ -735,10 +882,10 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
     if pushable and transfer != "pull":
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec, std, epsilon, taken, det)
+                                   nvec, std, epsilon, taken, det, action, twins)
         return views
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
-        _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0])
+        _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0], critic)
         if dev != root:
             _stage_for(dev, max(e - b for b, e in bounds), obs_root.shape[1])
     streams = {dev: torch.cuda.current_stream(dev) for dev in set(devs)}
@@ -762,7 +909,9 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                         **(det or dict(squash=None if std is None else bool(std[2]))),
                         **({} if epsilon is None else dict(epsilon=epsilon[b:e], q=log_probs, q_max=values)),
                         **({} if taken is None else dict(taken=taken[b:e], entropy=actions)),
-                        _stacked=valued or std is not None)
+                        **({} if not critic else dict(action=action[b:e], twin=None if twins is None else twins[dev],
+                                                      q=logits, q2=actions, q_min=log_probs)),
+                        _stacked=valued or std is not None or critic)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

@@ -24,7 +24,7 @@ MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
-               "gaussian_evaluate", "deterministic")   # also device.mlp.OUTPUTS
+               "gaussian_evaluate", "deterministic", "critic")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
 
 
@@ -115,13 +115,24 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     ``"gaussian"`` and ``c`` = ``noise_clip=`` (a number >= 0, default +inf), then clamped to [-1, 1] when squashed.
     ``seed=`` is required exactly when ``noise=`` is given.  Exploration is ``noise=0.1``; TD3's target policy
     smoothing is ``noise=0.2, noise_clip=0.5``.  ``mask=``, ``value=``, ``nvec=``, ``log_std=``, ``log_std_bounds=``,
-    ``epsilon=`` and ``taken=`` are refused."""
+    ``epsilon=`` and ``taken=`` are refused.
+    ``output="critic"`` is a Q(s, a) critic (SAC's and TD3's, forward only): ``action=`` names the call argument that
+    holds the fp32 actions ``[M, d_act]`` (1 <= d_act <= 64) on the device of obs (the body takes
+    ``act.chunk(WORLD_SIZE)[RANK]``), the callable is ``(obs, w1, b1, w2, b2, w3, b3, act, ...)`` (``(obs, w1, w2, w3,
+    act, ...)`` without ``bias=True``) with ``w1 [d_hidden, d_in + d_act]`` and ``w3 [1, d_hidden]``, and each rank
+    returns the fp32 ``q [rows]`` of ``torch.cat([obs, act.to(torch.bfloat16)], -1)``.  ``twin=`` names the second
+    critic's six arguments ``(w1, b1, w2, b2, w3, b3)`` (three, ``(w1, w2, w3)``, without ``bias=True``): each rank then
+    returns ``(q1, q2, q_min)`` with ``q_min = torch.minimum(q1, q2)``.  ``seed=``, ``mask=``, ``value=``, ``nvec=``,
+    ``log_std=``, ``log_std_bounds=``, ``squash=``, ``epsilon=``, ``taken=``, ``noise=`` and ``noise_clip=`` are
+    refused, and ``action=`` and ``twin=`` with every other output."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
+    if op != "mlp" and any(k in extra for k in ("action", "twin")):
+        raise ValueError(f"action= and twin= are options of the 'mlp' op, not of '{op}'")
     if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
-                                "squash", "epsilon", "taken", "noise", "noise_clip")):
+                                "squash", "epsilon", "taken", "noise", "noise_clip", "action", "twin")):
         if op != "mlp":
             raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value=, nvec=, "
                              f"epsilon=, taken=, noise= and noise_clip= are options of the 'mlp' op, not of '{op}'")
@@ -129,6 +140,11 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
+        if extra.get("output") == "critic":
+            _check_critic(extra)
+        elif "action" in extra or "twin" in extra:
+            raise ValueError(f'action= and twin= are options of output="critic", not of '
+                             f'output={extra.get("output", "logits")!r}')
         sample = extra.get("output") in ("sample", "gaussian")
         eps = extra.get("output") == "epsilon_greedy"
         det = extra.get("output") == "deterministic"
@@ -211,7 +227,7 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
 
     def deco(fn):
         params = inspect.signature(fn).parameters
-        for option in ("log_std", "mask", "value", "epsilon", "taken", "noise"):
+        for option in ("log_std", "mask", "value", "epsilon", "taken", "noise", "action", "twin"):
             names = extra.get(option)
             if option in ("epsilon", "noise") and not isinstance(names, str):   # a constant names no argument
                 continue
@@ -247,6 +263,25 @@ def _check_deterministic(extra) -> None:
             raise ValueError(f"{name} must be {what}, got {v!r}")
         if v != v or v < 0:
             raise ValueError(f"{name} must be >= 0 and not NaN, got {v!r}")
+
+
+def _check_critic(extra) -> None:
+    """mapped()'s checks of output="critic", in this order: the options it refuses, action= (required, the name of a
+    call argument), twin= (the names of six call arguments with bias=True, three without)."""
+    for name in ("seed", "mask", "value", "nvec", "log_std", "log_std_bounds", "squash", "epsilon", "taken", "noise",
+                 "noise_clip"):
+        if name in extra:
+            raise ValueError(f'{name}= is not an option of output="critic": a critic evaluates Q(s, a) of the given '
+                             f'action and takes action= and twin= only')
+    if not isinstance(extra.get("action"), str):
+        raise ValueError(f'action= is required with output="critic" and must name the call argument that holds the '
+                         f'actions, got {extra.get("action")!r}')
+    if "twin" in extra:
+        n = 6 if extra.get("bias", False) else 3
+        t = extra["twin"]
+        if not isinstance(t, (tuple, list)) or len(t) != n or not all(isinstance(x, str) for x in t):
+            what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
+            raise ValueError(f"twin must name the second critic's {n} call arguments {what}, got {t!r}")
 
 
 def check_nvec(nvec, output: str, d_out: Optional[int] = None) -> tuple:

@@ -609,13 +609,26 @@ class B200Supervisor:
             if noise not in bound:
                 raise TypeError(f"mapped mlp callable: noise argument '{noise}' not found in the call")
             noise = bound[noise]
+        action = spec.extra.get("action")
+        if action is not None:   # always the name of a call argument (the whole batch's actions), resolved per call
+            if action not in bound:
+                raise TypeError(f"mapped mlp callable: action argument '{action}' not found in the call")
+            action = bound[action]
+        twin = spec.extra.get("twin")
+        if twin is not None:   # the names of the second critic's weights (and biases), resolved per call
+            for name in twin:
+                if name not in bound:
+                    raise TypeError(f"mapped mlp callable: twin argument '{name}' not found in the call")
+            twin = tuple(bound[name] for name in twin)
+            if len(twin) == 3:   # (w1, w2, w3) of a bias-free critic
+                twin = (twin[0], None, twin[1], None, twin[2], None)
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
                                          value=value, nvec=spec.extra.get("nvec"),
                                          log_std_bounds=spec.extra.get("log_std_bounds"),
                                          squash=spec.extra.get("squash"), epsilon=epsilon, taken=taken, noise=noise,
-                                         noise_clip=spec.extra.get("noise_clip"))
+                                         noise_clip=spec.extra.get("noise_clip"), action=action, twin=twin)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

@@ -44,6 +44,11 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      actor beside output="logits", exploration (σ = 0.1) beside output="gaussian", and TD3's target policy smoothing
      (σ = 0.2, noise_clip = 0.5), at the same d_out; and the eager arm, what a user pays without the fused head: the
      logits entry, then tanh, normal_noise on the device and the two clamps in torch.
+  p  Q(s, a) critics (output="critic", SAC's and TD3's), the C4 trunk with the actions fed into layer 1 (256 + d_act ->
+     1024 -> 1024 -> 1), d_act 6, 17 and 64, single and twin, each beside output="logits" at d_out 1 on the same
+     observations (the difference is the action block and the head); and the eager twin, what a user pays without
+     the feature: torch.cat of the rows and the bf16 actions padded to d_in + 64, w1 padded likewise, the logits entry
+     per critic, .float() and torch.minimum.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -65,7 +70,10 @@ the eager arm's (the Gaussian's log-probabilities within rtol 1e-4, atol 1e-3 of
 within rtol 2^-7, atol 1e-2 of the eager critic's.  Deterministic rows: on 2048 consecutive rows, the noise-free
 actions are within tanhf's 2 ulp of fp64 tanh(y) (y the kernel's logits) and the noisy ones within
 σ·2^-19·(1 + |z|) + 2^-22·|t| + 2^-23·(|t| + |n|) of clamp(tanh(y) + clamp(σ·z, ±c), ±1) in fp64; on every row
-the smoothing actions are within rtol 1e-5, atol 1e-5 of the eager arm's.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
+the smoothing actions are within rtol 1e-5, atol 1e-5 of the eager arm's.  Critic rows: q equals the logits entry
+over [obs | bf16(act) | 0] and the padded w1 on every row, bit for bit; the twin's q1 and q2 equal the single critics'
+and its q_min the eager arm's torch.minimum (bit for bit off ties of signed zeros); q is within rtol 2^-7, atol 1e-2 of
+an fp32 evaluation on 2048 rows.  Gaussian rows: on 2048 consecutive rows, the actions are within 2^-19·σ·(1 + |z|) + 2^-23·|y| of y + σ·z (y the
 kernel's logits, σ and z = ndtri(u) in fp64) and the log-probabilities within the bar of tests/test_gpu_mlp_gaussian.py.
 The card name and its power limit are read in the same run.  Prints one JSON line."""
 import argparse
@@ -367,6 +375,41 @@ def main():
             variants[f"o_bias_{tag}_d{d}"] = (d, lambda d=d, bs=bs, kw=kw: mlp.mlp_forward(
                 obs, w1, w2, heads[d][0], biases=bs, output="deterministic", **kw))
         variants[f"o_bias_smooth_eager_d{d}"] = (d, lambda d=d: eager_deterministic(d))
+    gp = torch.Generator(device="cuda:0").manual_seed(12)   # its own generator again
+    critic_widths = (6, 17, 64)
+    critic_acts = {a: torch.rand(M, a, device="cuda:0", generator=gp) * 2 - 1 for a in critic_widths}
+    critics = {(a, i): ((torch.randn(d_hidden, d_in + a, device="cuda:0", generator=gp) * 0.02).bfloat16(),
+                        (torch.randn(d_hidden, device="cuda:0", generator=gp) * 0.1).bfloat16(),
+                        (torch.randn(d_hidden, d_hidden, device="cuda:0", generator=gp) * 0.02).bfloat16(),
+                        (torch.randn(d_hidden, device="cuda:0", generator=gp) * 0.1).bfloat16(),
+                        (torch.randn(1, d_hidden, device="cuda:0", generator=gp) * 0.02).bfloat16(),
+                        (torch.randn(1, device="cuda:0", generator=gp) * 0.1).bfloat16())
+               for a in critic_widths for i in (0, 1)}
+
+    def critic_call(a, twin):
+        c = critics[(a, 0)]
+        return mlp.mlp_forward(obs, c[0], c[2], c[4], biases=(c[1], c[3], c[5]), output="critic",
+                               action=critic_acts[a], twin=critics[(a, 1)] if twin else None)
+
+    def eager_twin(a):
+        """torch.cat and padding, the logits entry per critic, .float() and torch.minimum: what a user pays without
+        output="critic"."""
+        x = torch.cat([obs, critic_acts[a].to(torch.bfloat16), obs.new_zeros(M, 64 - a)], -1)
+        qs = []
+        for i in (0, 1):
+            c = critics[(a, i)]
+            qs.append(mlp.mlp_forward(x, F.pad(c[0], (0, 64 - a)), c[2], c[4], biases=(c[1], c[3], c[5])).float()
+                      .squeeze(-1))
+        return qs[0], qs[1], torch.minimum(qs[0], qs[1])
+
+    for a in critic_widths:
+        c = critics[(a, 0)]
+        w1_obs = c[0][:, :d_in].contiguous()   # the observation columns of w1, sliced once outside the timed calls
+        variants[f"p_bias_logits_d1_a{a}"] = (1, lambda c=c, w=w1_obs: mlp.mlp_forward(obs, w, c[2], c[4],
+                                                                                       biases=(c[1], c[3], c[5])))
+        variants[f"p_bias_critic_a{a}"] = (1, lambda a=a: critic_call(a, False))
+        variants[f"p_bias_critic_twin_a{a}"] = (1, lambda a=a: critic_call(a, True))
+        variants[f"p_bias_critic_twin_eager_a{a}"] = (1, lambda a=a: eager_twin(a))
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -574,6 +617,23 @@ def main():
         assert torch.allclose(got, want, rtol=1e-5, atol=1e-5), d
         parity[f"o_bias_deterministic_d{d}"] = "ok"
         del y, got, want
+
+    for a in critic_widths:
+        q = variants[f"p_bias_critic_a{a}"][1]()
+        q1, q2, qm = variants[f"p_bias_critic_twin_a{a}"][1]()
+        e1, e2, em = variants[f"p_bias_critic_twin_eager_a{a}"][1]()
+        assert torch.equal(q.view(torch.int32), e1.view(torch.int32)), a
+        assert torch.equal(q1.view(torch.int32), q.view(torch.int32)), a
+        assert torch.equal(q2.view(torch.int32), e2.view(torch.int32)), a
+        off_ties = ~((q1 == 0) & (q2 == 0))
+        assert torch.equal(qm[off_ties].view(torch.int32), em[off_ties].view(torch.int32)), a
+        c = critics[(a, 0)]
+        x = torch.cat([obs[idx], critic_acts[a][idx].to(torch.bfloat16)], -1)
+        ref = _fp32(x, (c[0], c[2], c[4]), (c[1], c[3], c[5])).squeeze(-1)
+        torch.testing.assert_close(q[idx], ref.bfloat16().float(), rtol=2**-7, atol=1e-2)
+        parity[f"p_bias_critic_a{a}"] = {"q_eq_logits_entry_all_rows": "ok", "twin_eq_eager_all_rows": "ok",
+                                         "q_vs_fp32_2048_rows": "ok"}
+        del q, q1, q2, qm, e1, e2, em
 
     result = {"what": "mlp_policy_c4_scale", "rows": M, "shape": f"{d_in}->{d_hidden}->{d_hidden}->d_out",
               "device": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w(),
