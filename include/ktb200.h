@@ -921,6 +921,73 @@ int ktb_mlp_bf16_critic_twin_pushed(int dev, const void* stage_local, size_t sta
                                     void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows,
                                     unsigned long long seq, uintptr_t stream);
 
+/* TD targets of TD3, DDPG and SAC in one call, forward only: the next actions of an actor, the target critics over
+ * them and the Bellman target.  For rows next_obs (bf16 [M, d_in]) with reward and done (fp32 [M]):
+ *   - Next action.  _deterministic (TD3, DDPG): a = ktb_mlp_bf16_policy_deterministic's actions, with its noise,
+ *     noise_clip, squash, seed and row_base (noise over global rows row_base + i).  _gaussian (SAC): (a, logp) =
+ *     ktb_mlp_bf16_policy_gaussian_state's actions and log-probabilities, with its interleaved head aW3s / ab3s,
+ *     log_std_min / log_std_max, squash, seed and row_base (the same Philox stream).  The actor is
+ *     (aW1, ab1, aW2, ab2, aW3, ab3) with its own d_hidden_actor, which may differ from the critics' d_hidden.
+ *   - Critics.  q1 (and q2 with a twin) are ktb_mlp_bf16_critic(_twin)'s values over a, which reaches layer 1 as the
+ *     same bf16 action tile.  t = q_min with a twin (its tie and NaN rule) and t = q1 without one (DDPG).
+ *   - SAC: t = __fsub_rn(t, __fmul_rn(alpha, logp)).  There is no alpha term in the _deterministic entries.
+ *   - y[i] = __fadd_rn(r, __fmul_rn(__fmul_rn(gamma, __fsub_rn(1.f, d)), t)), fp32 [M] (may be a peer pointer): the
+ *     evaluation order of reward + gamma * (1 - done) * (t - alpha * logp) on fp32 torch tensors with Python-float
+ *     gamma and alpha, which torch rounds to fp32 first.  No FMA contraction.  IEEE cases follow the formula: an
+ *     infinite or NaN t gives NaN where gamma * (1 - d) is 0 (done = 1, or gamma = 0), and +-inf or NaN otherwise;
+ *     alpha = 0 with an infinite logp gives NaN; a NaN reward or done gives NaN.
+ *   - Arguments: ktb_mlp_bf16_critic's up to b3 (W1p [d_hidden, d_in + 64], 1 <= d_act <= 64), the second critic's
+ *     (W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2) (all six NULL: a single critic), then d_hidden_actor and the actor's six
+ *     pointers, then the policy's arguments in the order of the standalone entry, then reward, done (reward_offset,
+ *     done_offset: byte offsets into the rank's staging half, in the pushed forms), gamma, alpha (_gaussian only), y,
+ *     then scratch and stage (or the push arguments) and stream.  scratch holds ktb_mlp_td_target_scratch_bytes(M,
+ *     d_hidden_actor, d_hidden, d_act): the two hidden activations at the wider d_hidden, the action tile, and the
+ *     chunk's fp32 actions, log-probabilities and q1.  No M-sized intermediate is written.
+ *   - Checks, in this order: every check of ktb_mlp_bf16_critic (_twin with a second critic; a second critic with a NULL
+ *     W1p_2 and another of its six pointers non-NULL is KTB_ERR_ARG there) but those of act and the Q outputs; then
+ *     every check of the actor's standalone entry at d_out = d_act and d_hidden_actor, its noise and noise_clip or its
+ *     log_std bounds included (the actor and the critics share d_in and d_act, one argument each); then a non-finite
+ *     gamma or alpha is KTB_ERR_ARG; then, with M > 0, a NULL or not 4-byte aligned reward, done (pull forms) or y is
+ *     KTB_ERR_ARG; then, in the pushed forms, a reward or done region that overlaps the rows, ends past stage_stride
+ *     or is not 4-byte aligned, or the two regions overlapping, is KTB_ERR_ARG.  An empty pushed shard (M == 0) may
+ *     pass NULL outputs and still publishes its ack.  The pushed forms read the rows, reward and done from their
+ *     staging half (ktb_push_scatter_ce_sides with two sides).  Writes stay inside y, scratch and stage. */
+size_t ktb_mlp_td_target_scratch_bytes(size_t M, int d_hidden_actor, int d_hidden, int d_act);
+int ktb_mlp_bf16_td_target_deterministic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act,
+                                         const void* W1p, const void* b1, const void* W2, const void* b2,
+                                         const void* W3, const void* b3, const void* W1p_2, const void* b1_2,
+                                         const void* W2_2, const void* b2_2, const void* W3_2, const void* b3_2,
+                                         int d_hidden_actor, const void* aW1, const void* ab1, const void* aW2,
+                                         const void* ab2, const void* aW3, const void* ab3, float noise,
+                                         float noise_clip, int squash, uint64_t seed, uint64_t row_base,
+                                         const float* reward, const float* done, float gamma, float* y, void* scratch,
+                                         void* stage, uintptr_t stream);
+int ktb_mlp_bf16_td_target_deterministic_pushed(
+    int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_act,
+    const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+    const void* W1p_2, const void* b1_2, const void* W2_2, const void* b2_2, const void* W3_2, const void* b3_2,
+    int d_hidden_actor, const void* aW1, const void* ab1, const void* aW2, const void* ab2, const void* aW3,
+    const void* ab3, float noise, float noise_clip, int squash, uint64_t seed, uint64_t row_base,
+    size_t reward_offset, size_t done_offset, float gamma, float* y, void* scratch, void* ctrl_local,
+    void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+int ktb_mlp_bf16_td_target_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act,
+                                    const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3,
+                                    const void* b3, const void* W1p_2, const void* b1_2, const void* W2_2,
+                                    const void* b2_2, const void* W3_2, const void* b3_2, int d_hidden_actor,
+                                    const void* aW1, const void* ab1, const void* aW2, const void* ab2,
+                                    const void* aW3s, const void* ab3s, float log_std_min, float log_std_max,
+                                    int squash, uint64_t seed, uint64_t row_base, const float* reward,
+                                    const float* done, float gamma, float alpha, float* y, void* scratch, void* stage,
+                                    uintptr_t stream);
+int ktb_mlp_bf16_td_target_gaussian_pushed(
+    int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_act,
+    const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+    const void* W1p_2, const void* b1_2, const void* W2_2, const void* b2_2, const void* W3_2, const void* b3_2,
+    int d_hidden_actor, const void* aW1, const void* ab1, const void* aW2, const void* ab2, const void* aW3s,
+    const void* ab3s, float log_std_min, float log_std_max, int squash, uint64_t seed, uint64_t row_base,
+    size_t reward_offset, size_t done_offset, float gamma, float alpha, float* y, void* scratch, void* ctrl_local,
+    void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

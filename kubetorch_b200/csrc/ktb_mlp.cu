@@ -472,21 +472,44 @@ struct HeadEval {
 // The outputs of a critic head, the layer kernel's last parameter (by value, like HeadEps, and for the same reason).
 // q != null marks a kGaussian head with no policy columns whose column 0 is Q(s, a): q [rows] receives it widened to
 // fp32.  The second head of a twin also reads q_other [rows], the first head's Q, and stores q_min = min(Q2, Q1)
-// (critic_epilogue).
+// (critic_epilogue).  y != null marks the last critic head of a TD target instead: it stores no Q but
+// y = r + γ·(1 − d)·(t − α·logp) (t its Q, or the twin's minimum; the α term only with logp) from reward, done and
+// logp [rows].
 struct HeadQ {
   float* q = nullptr;
   const float* q_other = nullptr;
   float* q_min = nullptr;
+  const float* reward = nullptr;
+  const float* done = nullptr;
+  const float* logp = nullptr;
+  float* y = nullptr;
+  float gamma = 0.f, alpha = 0.f;
 
-  HeadQ from_row(size_t r0) const {
-    return q ? HeadQ{q + r0, q_other ? q_other + r0 : nullptr, q_min ? q_min + r0 : nullptr} : *this;
+  // The same outputs from row r0 of the call on.  A TD target's critics (`scratch`) read and write q, q_other and
+  // logp in chunk-sized scratch from the chunk's first row, so only its reward, done and y move.
+  HeadQ from_row(size_t r0, bool scratch) const {
+    HeadQ h = *this;
+    if (scratch) {
+      if (y) {
+        h.reward += r0;
+        h.done += r0;
+        h.y += r0;
+      }
+    } else if (q) {
+      h.q += r0;
+      if (q_other) h.q_other += r0;
+      if (q_min) h.q_min += r0;
+    }
+    return h;
   }
 };
 
 // The epilogue of a critic head (HeadQ) in the 64-wide kGaussian instantiation: column 0 of rows row and row + 8, held
 // by lane 0 of each quad in acc[0] and acc[2], gets the bias and one rounding to bf16 (layer_pair, as every head) and
 // is stored widened to fp32 into q.  A twin's second head also stores q_min = Q2 < Q1 ? Q2 : Q1, so a tie (±0
-// included) gives Q1, as torch.minimum of 0-d CPU tensors does, and NaN when either is NaN.  The kernel takes it in place
+// included) gives Q1, as torch.minimum of 0-d CPU tensors does, and NaN when either is NaN.  The last head of a TD target
+// (hq.y) stores y = r + γ·(1 − d)·t in place of q and q_min, t its Q or that minimum less α·logp when it has logp,
+// each operation rounded once in the order of the torch expression (no contraction).  The kernel takes it in place
 // of gaussian_epilogue, so the Gaussian heads' code is what it was; the store is rolled.
 template <int BLOCK_N>
 __device__ __forceinline__ void critic_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
@@ -499,11 +522,18 @@ __device__ __forceinline__ void critic_epilogue(const float (&acc)[BLOCK_N / 2],
     if (!(h ? st1 : st0)) continue;
     const int r = row + 8 * h;
     const float v = __low2float(h ? y1 : y0);
-    hq.q[r] = v;
+    float t = v;
     if (hq.q_other != nullptr) {
       const float o = hq.q_other[r];
-      hq.q_min[r] = v != v ? v : v < o ? v : o;
+      t = v != v ? v : v < o ? v : o;
     }
+    if (hq.y == nullptr) {
+      hq.q[r] = v;
+      if (hq.q_other != nullptr) hq.q_min[r] = t;
+      continue;
+    }
+    if (hq.logp != nullptr) t = __fsub_rn(t, __fmul_rn(hq.alpha, hq.logp[r]));
+    hq.y[r] = __fadd_rn(hq.reward[r], __fmul_rn(__fmul_rn(hq.gamma, __fsub_rn(1.f, hq.done[r])), t));
   }
 }
 
@@ -1258,7 +1288,7 @@ struct HeadOut {
 //   kGaussian with sd.det: gauss_actions[row, j] = the deterministic actor's action, tanh(logit_j) (or logit_j) plus
 //     clipped noise, and no log_probs (deterministic_pass);
 //   kGaussian with hq.q: a critic, n_valid = 1: hq.q[row] = fp32(logit_0), and a twin's second head also hq.q_min[row]
-//     (critic_epilogue).
+//     (critic_epilogue); with hq.y the last critic of a TD target, which stores the target y[row] instead.
 // A critic's layer 1 (kHidden) takes its A operand from two maps: K blocks < kb_split from maps_a.m[0] (the
 // observation rows), the last from maps_a.m[1] (the action tile); every other launch has kb_split = K / 64 and never
 // reads m[1].
@@ -1300,7 +1330,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
                              out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max, ev);
-  } else if (BLOCK_N == 64 && hq.q != nullptr) {   // a critic (64-wide tile): column 0 is Q, no policy columns
+  } else if (BLOCK_N == 64 && (hq.q != nullptr || hq.y != nullptr)) {   // a critic (64-wide tile): column 0 is Q
     critic_epilogue<BLOCK_N>(acc, bias, col0, row, st0, st1, hq);
   } else {
     gaussian_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.log_std, out.gauss_actions,
@@ -1470,7 +1500,10 @@ static int launch_action_tile(const float* act, int d_act, void* tile, size_t ro
 // entries: W1 is W1p [d_hidden, d_in + 64], layer 1 reads an action tile packed from `act` (fp32 [M, d_act]; in the
 // pushed forms the bytes at MlpFeed::act_offset of the call's staging half) as its last K block, W3 / b3 are the
 // critic's [1, d_hidden] / [1], and hq receives Q; `twin` (the _twin entries) is the second critic, run on the same
-// tile after the first, whose hq also reads the first's q and stores q_min.
+// tile after the first, whose hq also reads the first's q and stores q_min.  `actor` marks the _td_target entries: the
+// critics' action tile is packed from the actions the actor (a deterministic or state-dependent Gaussian head,
+// `actor_hidden` wide) writes into chunk scratch, and the last critic's hq computes the target (`target` marks both
+// critics: their hq reads and writes chunk scratch).
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1491,6 +1524,9 @@ struct MlpParams {
   const float* act = nullptr;
   HeadQ hq;
   const MlpParams* twin = nullptr;
+  const MlpParams* actor = nullptr;
+  int actor_hidden = 0;
+  bool target = false;
 
   // A critic, in the 64-wide kGaussian instantiation (one column, Q): act [M, d_act] fp32 (null in the pushed forms)
   // in, q [M] fp32 out.
@@ -1606,7 +1642,7 @@ static int mlp_chunk(int dev, const MlpParams& p, const HeadOut& out, const Head
   const int n = (p.std.state ? 2 * d_out : d_out) + (int)p.valued;
   const size_t per_row = ev.gauss_actions ? (size_t)d_out : (size_t)std::max(out.groups.n, 1);   // given actions
   return head(dev, h2, p.W3, p.b3, out.from_row(r0, d_out), rows, n, d_hidden, st, p.std, eg.from_row(r0),
-              ev.from_row(r0, per_row), p.hq.from_row(r0));
+              ev.from_row(r0, per_row), p.hq.from_row(r0, p.target));
 }
 
 // The checks every MLP entry shares: the layer widths the tiles divide, the head (the outputs its kind stores, width,
@@ -1670,7 +1706,8 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A masked head reads
 //           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows), and
 //           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in, an evaluating head its rows' given
-//           actions from taken_offset bytes in, and a critic its rows' actions (fp32) from act_offset bytes in.
+//           actions from taken_offset bytes in, a critic its rows' actions (fp32) from act_offset bytes in, and a
+//           TD target its rows' reward and done (fp32) from reward_offset and done_offset bytes in.
 // The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
@@ -1685,6 +1722,7 @@ struct MlpFeed {
   size_t epsilon_offset = 0;
   size_t taken_offset = 0;
   size_t act_offset = 0;
+  size_t reward_offset = 0, done_offset = 0;
 
   static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
   static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
@@ -1711,7 +1749,57 @@ struct MlpFeed {
     f.act_offset = off;
     return f;
   }
+  MlpFeed with_target_offsets(size_t reward, size_t done) const {
+    MlpFeed f = *this;
+    f.reward_offset = reward;
+    f.done_offset = done;
+    return f;
+  }
 };
+
+// The chunk scratch of a call, in this order: two hidden activations [chunk, d_hidden] bf16 (a TD target's actor and
+// critics share them, at the wider d_hidden), a critic's action tile [chunk, 64] bf16, then a TD target's actions
+// [chunk, d_act], log-probabilities [chunk] and first Q [chunk], fp32 (ktb_mlp_td_target_scratch_bytes).
+struct MlpScratch {
+  __nv_bfloat16 *h1, *h2, *tile;
+  float *act, *logp, *q1;
+
+  static MlpScratch carve(void* scratch, size_t chunk, int d_hidden, int d_act) {
+    MlpScratch s;
+    s.h1 = static_cast<__nv_bfloat16*>(scratch);
+    s.h2 = s.h1 + chunk * (size_t)d_hidden;
+    s.tile = s.h2 + chunk * (size_t)d_hidden;
+    s.act = reinterpret_cast<float*>(s.tile + chunk * (size_t)kMlpBlockK);
+    s.logp = s.act + chunk * (size_t)d_act;
+    s.q1 = s.logp + chunk;
+    return s;
+  }
+};
+
+// The checks of a head's own options, skipped for an empty call: a value head's values and width, a state-dependent
+// Gaussian head's width and log-std bounds, a deterministic actor's noise and noise_clip.
+static int head_checks(const char* fn, size_t M, int d_out, const MlpParams& p) {
+  if (p.valued && M > 0) {
+    KTB_REQUIRE(p.out.values, KTB_ERR_ARG, "%s: null values", fn);
+    KTB_REQUIRE(((uintptr_t)p.out.values & 3) == 0, KTB_ERR_ARG, "%s: values must be 4-byte aligned", fn);
+    KTB_REQUIRE(d_out <= 255, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the policy and its value column fit one 256-wide tile)",
+                fn, d_out);
+  }
+  if (p.std.state && M > 0) {
+    KTB_REQUIRE(2 * d_out + (int)p.valued <= 256, KTB_ERR_UNSUPPORTED,
+                "%s: d_out=%d (the interleaved mean and log-std%s fit one 256-wide tile)", fn, d_out,
+                p.valued ? " and the value column" : "");
+    const float lo = p.std.lo, hi = p.std.hi;
+    KTB_REQUIRE(lo == lo && hi == hi && lo <= hi, KTB_ERR_ARG, "%s: log_std bounds [%g, %g] must be ordered, not NaN",
+                fn, (double)lo, (double)hi);
+  }
+  if (p.std.det && M > 0) {
+    const float s = p.std.noise, c = p.std.clip;
+    KTB_REQUIRE(s == s && s >= 0.f, KTB_ERR_ARG, "%s: noise=%g must be >= 0, not NaN", fn, (double)s);
+    KTB_REQUIRE(c == c && c >= 0.f, KTB_ERR_ARG, "%s: noise_clip=%g must be >= 0, not NaN", fn, (double)c);
+  }
+  return KTB_OK;
+}
 
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
 // right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
@@ -1728,7 +1816,11 @@ struct MlpFeed {
 // with the head (mlp_check), its noise and noise_clip (>= 0, not NaN; skipped for an empty call) after every check.
 // A critic entry runs every check of ktb_mlp_bf16_policy at d_out = 1 (a twin's second critic's weights and biases
 // checked as the first's, right after them), then d_act in [1, 64], then (skipped for an empty call) act and its
-// outputs non-null and 4-byte aligned, then its action region in the pushed forms.
+// outputs non-null and 4-byte aligned, then its action region in the pushed forms.  A TD target entry runs every check
+// of the critic (twin) entry but those of act and the Q outputs, then every check of its actor's standalone entry
+// (ktb_mlp_bf16_policy_deterministic or _gaussian_state at d_out = d_act, the actor's d_hidden), then gamma and alpha
+// finite, then (skipped for an empty call) reward, done and y non-null and aligned, then its reward and done regions
+// in the pushed forms.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1790,43 +1882,70 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     KTB_REQUIRE((((uintptr_t)o.epsilon | (uintptr_t)o.q | (uintptr_t)o.q_max) & 3) == 0, KTB_ERR_ARG,
                 "%s: epsilon, q and q_max must be 4-byte aligned", fn);
   }
-  if (p.valued && M > 0) {
-    KTB_REQUIRE(p.out.values, KTB_ERR_ARG, "%s: null values", fn);
-    KTB_REQUIRE(((uintptr_t)p.out.values & 3) == 0, KTB_ERR_ARG, "%s: values must be 4-byte aligned", fn);
-    KTB_REQUIRE(d_out <= 255, KTB_ERR_UNSUPPORTED, "%s: d_out=%d (the policy and its value column fit one 256-wide tile)",
-                fn, d_out);
-  }
-  if (p.std.state && M > 0) {
-    KTB_REQUIRE(2 * d_out + (int)p.valued <= 256, KTB_ERR_UNSUPPORTED,
-                "%s: d_out=%d (the interleaved mean and log-std%s fit one 256-wide tile)", fn, d_out,
-                p.valued ? " and the value column" : "");
-    const float lo = p.std.lo, hi = p.std.hi;
-    KTB_REQUIRE(lo == lo && hi == hi && lo <= hi, KTB_ERR_ARG, "%s: log_std bounds [%g, %g] must be ordered, not NaN",
-                fn, (double)lo, (double)hi);
-  }
-  if (p.std.det && M > 0) {
-    const float s = p.std.noise, c = p.std.clip;
-    KTB_REQUIRE(s == s && s >= 0.f, KTB_ERR_ARG, "%s: noise=%g must be >= 0, not NaN", fn, (double)s);
-    KTB_REQUIRE(c == c && c >= 0.f, KTB_ERR_ARG, "%s: noise_clip=%g must be >= 0, not NaN", fn, (double)c);
-  }
+  rc = head_checks(fn, M, d_out, p);
+  if (rc) return rc;
   if (p.critic) {
     KTB_REQUIRE(p.d_act >= 1, KTB_ERR_ARG, "%s: d_act=%d must be positive", fn, p.d_act);
     KTB_REQUIRE(p.d_act <= kMlpBlockK, KTB_ERR_UNSUPPORTED, "%s: d_act=%d (actions up to %d wide)", fn, p.d_act,
                 kMlpBlockK);
-    if (M > 0) {
+    if (M > 0 && !p.actor) {
       const HeadQ& q2 = p.twin ? p.twin->hq : HeadQ{};
       KTB_REQUIRE((p.act || f.pushed) && p.hq.q && (!p.twin || (q2.q && q2.q_min)), KTB_ERR_ARG,
                   p.twin ? "%s: act, q1, q2 and q_min are required" : "%s: act and q are required", fn);
       KTB_REQUIRE((((uintptr_t)p.act | (uintptr_t)p.hq.q | (uintptr_t)q2.q | (uintptr_t)q2.q_min) & 3) == 0,
                   KTB_ERR_ARG, "%s: act and the outputs must be 4-byte aligned", fn);
     }
-    if (f.pushed) {
+    if (f.pushed && !p.actor) {
       const size_t off = f.act_offset, n = M * (size_t)p.d_act * 4;
       KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: act_offset=%zu overlaps the rows", fn, off);
       KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG, "%s: act_offset=%zu + act exceeds stage_stride",
                   fn, off);
       KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: act_offset=%zu must be a multiple of 4", fn, off);
     }
+  }
+  const size_t chunk = std::min(f.chunk_rows, M);
+  const MlpScratch s = MlpScratch::carve(scratch, chunk, std::max(d_hidden, p.actor_hidden), p.d_act);
+  // a TD target's actor and critics with their chunk scratch: the actor writes its actions (and log-probabilities)
+  // there, the first of two critics its Q, and the last critic reads them
+  MlpParams actor{}, c1 = p, c2{};
+  if (p.actor) {
+    actor = *p.actor;
+    actor.out.gauss_actions = s.act;
+    if (actor.std.state) actor.out.log_probs = s.logp;
+    KTB_REQUIRE(actor.W1 && actor.W2 && actor.W3, KTB_ERR_ARG, "%s: null argument", fn);
+    rc = mlp_check(fn, M, d_in, p.actor_hidden, p.d_act, actor, f.in, scratch, f.stage);
+    if (rc) return rc;
+    rc = head_checks(fn, M, p.d_act, actor);
+    if (rc) return rc;
+    if (p.twin) {
+      c2 = *p.twin;
+      c1.hq.q = s.q1;
+      c2.hq.q_other = s.q1;
+      c1.twin = &c2;
+    }
+    HeadQ& t = (p.twin ? c2 : c1).hq;
+    KTB_REQUIRE(std::isfinite(t.gamma) && std::isfinite(t.alpha), KTB_ERR_ARG, "%s: gamma=%g and alpha=%g must be finite",
+                fn, (double)t.gamma, (double)t.alpha);
+    if (M > 0) {
+      KTB_REQUIRE(((t.reward && t.done) || f.pushed) && t.y, KTB_ERR_ARG, "%s: reward, done and y are required", fn);
+      KTB_REQUIRE((((uintptr_t)t.reward | (uintptr_t)t.done | (uintptr_t)t.y) & 3) == 0, KTB_ERR_ARG,
+                  "%s: reward, done and y must be 4-byte aligned", fn);
+    }
+    if (f.pushed) {
+      const size_t n = M * sizeof(float);
+      for (const size_t off : {f.reward_offset, f.done_offset}) {
+        KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: reward/done offset %zu overlaps the rows", fn, off);
+        KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG,
+                    "%s: reward/done offset %zu + 4*M exceeds stage_stride", fn, off);
+        KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: reward/done offset %zu must be a multiple of 4", fn, off);
+      }
+      KTB_REQUIRE(f.reward_offset + n <= f.done_offset || f.done_offset + n <= f.reward_offset, KTB_ERR_ARG,
+                  "%s: the reward and done regions overlap", fn);
+      const uint8_t* half = static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride;
+      t.reward = reinterpret_cast<const float*>(half + f.reward_offset);
+      t.done = reinterpret_cast<const float*>(half + f.done_offset);
+    }
+    if (actor.std.state) t.logp = s.logp;
   }
   HeadGroups groups = p.out.groups;
   if (p.grouped && M > 0) {
@@ -1868,10 +1987,6 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   if (rc) return rc;
   KTB_GUARD(dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const size_t chunk = std::min(f.chunk_rows, M);
-  __nv_bfloat16* h1 = static_cast<__nv_bfloat16*>(scratch);
-  __nv_bfloat16* h2 = h1 + chunk * (size_t)d_hidden;
-  __nv_bfloat16* tile = h2 + chunk * (size_t)d_hidden;   // a critic's action tile [chunk, 64]
   // the call's rows: obs, or this call's staging half (the pull forms have seq = stride = 0)
   const __nv_bfloat16* x =
       reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride);
@@ -1939,14 +2054,21 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       KTB_CK(cudaStreamWaitEvent(st, evs[1 + b], 0));
       a1 = dstb;
     }
-    if (p.critic) {   // packed once per chunk; a twin's two chains both read it
-      rc = launch_action_tile(act + r0 * p.d_act, p.d_act, tile, rows, st);
+    // evs[3..4] are null unless staged; every chain after the first records `consumed` again after its layer 1
+    cudaEvent_t consumed = evs[3 + (int)(c & 1)];
+    if (p.actor) {   // the chunk's actions into chunk scratch: pointers from its row 0, noise of its global rows
+      HeadOut ao = actor.out;
+      ao.row_base += r0;
+      rc = mlp_chunk(dev, actor, ao, HeadEps{}, HeadEval{}, a1, nullptr, s.h1, s.h2, 0, rows, d_in, p.actor_hidden,
+                     p.d_act, consumed, st);
       if (rc) return rc;
     }
-    // evs[3..4] are null unless staged; a twin records `consumed` again after its second layer 1
-    for (const MlpParams* q = &p; q != nullptr; q = q->twin) {
-      rc = mlp_chunk(dev, *q, out, eg, ev, a1, tile, h1, h2, r0, rows, d_in, d_hidden, d_out, evs[3 + (int)(c & 1)],
-                     st);
+    if (p.critic) {   // packed once per chunk; a twin's two chains both read it
+      rc = launch_action_tile(p.actor ? s.act : act + r0 * p.d_act, p.d_act, s.tile, rows, st);
+      if (rc) return rc;
+    }
+    for (const MlpParams* q = &c1; q != nullptr; q = q->twin) {
+      rc = mlp_chunk(dev, *q, out, eg, ev, a1, s.tile, s.h1, s.h2, r0, rows, d_in, d_hidden, d_out, consumed, st);
       if (rc) return rc;
     }
   }
@@ -2689,6 +2811,109 @@ int ktb_mlp_bf16_critic_twin_pushed(int dev, const void* stage_local, size_t sta
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
                      .with_act_offset(act_offset),
                  scratch, stream);
+}
+
+size_t ktb_mlp_td_target_scratch_bytes(size_t M, int d_hidden_actor, int d_hidden, int d_act) {
+  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
+  return ktb_mlp_critic_scratch_bytes(M, std::max(d_hidden_actor, d_hidden)) + rows * (4 * (size_t)d_act + 8);
+}
+
+}  // extern "C"
+
+namespace ktb {
+
+// The critics of a TD target (the first and, unless the six pointers of the second are all null, a twin's second)
+// over the actions of `actor`, the last one's HeadQ holding the target's inputs and output; mlp_run points their
+// scratch pointers into the chunk scratch.  A partly given second critic is a twin with a null weight, which mlp_run
+// refuses.
+static int td_target_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_act, const void* const (&c)[12],
+                         int d_hidden_actor, const MlpParams& actor, const float* reward, const float* done,
+                         float gamma, float alpha, float* y, const MlpFeed& f, void* scratch, uintptr_t stream) {
+  MlpParams second = MlpParams::critic_head(c[6], c[7], c[8], c[9], c[10], c[11], d_act, nullptr, nullptr);
+  MlpParams p = MlpParams::critic_head(c[0], c[1], c[2], c[3], c[4], c[5], d_act, nullptr, nullptr);
+  if (std::any_of(c + 6, c + 12, [](const void* x) { return x != nullptr; })) p.twin = &second;
+  HeadQ& t = (p.twin ? second : p).hq;
+  t.reward = reward;
+  t.done = done;
+  t.y = y;
+  t.gamma = gamma;
+  t.alpha = alpha;
+  p.target = second.target = true;
+  p.actor = &actor;
+  p.actor_hidden = d_hidden_actor;
+  return mlp_run(fn, dev, M, d_in, d_hidden, 1, p, f, scratch, stream);
+}
+
+}  // namespace ktb
+
+extern "C" {
+
+int ktb_mlp_bf16_td_target_deterministic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act,
+                                         const void* W1p, const void* b1, const void* W2, const void* b2,
+                                         const void* W3, const void* b3, const void* W1p_2, const void* b1_2,
+                                         const void* W2_2, const void* b2_2, const void* W3_2, const void* b3_2,
+                                         int d_hidden_actor, const void* aW1, const void* ab1, const void* aW2,
+                                         const void* ab2, const void* aW3, const void* ab3, float noise,
+                                         float noise_clip, int squash, uint64_t seed, uint64_t row_base,
+                                         const float* reward, const float* done, float gamma, float* y, void* scratch,
+                                         void* stage, uintptr_t stream) {
+  const MlpParams a =
+      MlpParams::deterministic(aW1, ab1, aW2, ab2, aW3, ab3, noise, noise_clip, squash, seed, row_base, nullptr);
+  return td_target_run("ktb_mlp_bf16_td_target_deterministic", dev, M, d_in, d_hidden, d_act,
+                       {W1p, b1, W2, b2, W3, b3, W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2}, d_hidden_actor, a, reward, done,
+                       gamma, 0.f, y, MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_td_target_deterministic_pushed(
+    int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_act,
+    const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+    const void* W1p_2, const void* b1_2, const void* W2_2, const void* b2_2, const void* W3_2, const void* b3_2,
+    int d_hidden_actor, const void* aW1, const void* ab1, const void* aW2, const void* ab2, const void* aW3,
+    const void* ab3, float noise, float noise_clip, int squash, uint64_t seed, uint64_t row_base,
+    size_t reward_offset, size_t done_offset, float gamma, float* y, void* scratch, void* ctrl_local,
+    void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams a =
+      MlpParams::deterministic(aW1, ab1, aW2, ab2, aW3, ab3, noise, noise_clip, squash, seed, row_base, nullptr);
+  return td_target_run("ktb_mlp_bf16_td_target_deterministic_pushed", dev, M, d_in, d_hidden, d_act,
+                       {W1p, b1, W2, b2, W3, b3, W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2}, d_hidden_actor, a, nullptr,
+                       nullptr, gamma, 0.f, y,
+                       MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                           .with_target_offsets(reward_offset, done_offset),
+                       scratch, stream);
+}
+
+int ktb_mlp_bf16_td_target_gaussian(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act,
+                                    const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3,
+                                    const void* b3, const void* W1p_2, const void* b1_2, const void* W2_2,
+                                    const void* b2_2, const void* W3_2, const void* b3_2, int d_hidden_actor,
+                                    const void* aW1, const void* ab1, const void* aW2, const void* ab2,
+                                    const void* aW3s, const void* ab3s, float log_std_min, float log_std_max,
+                                    int squash, uint64_t seed, uint64_t row_base, const float* reward,
+                                    const float* done, float gamma, float alpha, float* y, void* scratch, void* stage,
+                                    uintptr_t stream) {
+  const MlpParams a = MlpParams::gaussian_state(aW1, ab1, aW2, ab2, aW3s, ab3s, log_std_min, log_std_max, squash,
+                                                {nullptr, nullptr, nullptr, seed, row_base});
+  return td_target_run("ktb_mlp_bf16_td_target_gaussian", dev, M, d_in, d_hidden, d_act,
+                       {W1p, b1, W2, b2, W3, b3, W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2}, d_hidden_actor, a, reward, done,
+                       gamma, alpha, y, MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_td_target_gaussian_pushed(
+    int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden, int d_act,
+    const void* W1p, const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+    const void* W1p_2, const void* b1_2, const void* W2_2, const void* b2_2, const void* W3_2, const void* b3_2,
+    int d_hidden_actor, const void* aW1, const void* ab1, const void* aW2, const void* ab2, const void* aW3s,
+    const void* ab3s, float log_std_min, float log_std_max, int squash, uint64_t seed, uint64_t row_base,
+    size_t reward_offset, size_t done_offset, float gamma, float alpha, float* y, void* scratch, void* ctrl_local,
+    void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  const MlpParams a = MlpParams::gaussian_state(aW1, ab1, aW2, ab2, aW3s, ab3s, log_std_min, log_std_max, squash,
+                                                {nullptr, nullptr, nullptr, seed, row_base});
+  return td_target_run("ktb_mlp_bf16_td_target_gaussian_pushed", dev, M, d_in, d_hidden, d_act,
+                       {W1p, b1, W2, b2, W3, b3, W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2}, d_hidden_actor, a, nullptr,
+                       nullptr, gamma, alpha, y,
+                       MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                           .with_target_offsets(reward_offset, done_offset),
+                       scratch, stream);
 }
 
 }  // extern "C"

@@ -215,6 +215,16 @@ for _twin in ("", "_twin"):
         _args = _SIGNATURES["ktb_mlp_bf16_policy" + _form][1]
         _head_args = [c_void_p] * (6 if _twin else 0) + [_act] + [c_void_p] * (3 if _twin else 1)
         _SIGNATURES["ktb_mlp_bf16_critic" + _twin + _form] = (c_int, _args[:_at] + _head_args + _args[_at + 2:])
+# The _td_target entries: the _critic_twin entries' arguments up to the second critic's b3, then d_hidden_actor and the
+# actor's six pointers, the policy's five arguments, then reward and done (their offsets in the pushed forms), gamma,
+# alpha (_gaussian only) and y, then the rest of the _critic_twin entries' arguments from scratch on.
+_SIGNATURES["ktb_mlp_td_target_scratch_bytes"] = (c_size_t, [c_size_t, c_int, c_int, c_int])
+for _policy, _alpha in (("_deterministic", []), ("_gaussian", [c_float])):
+    for _form, _side, _at in (("", c_void_p, 18), ("_pushed", c_size_t, 19)):
+        _args = _SIGNATURES["ktb_mlp_bf16_critic_twin" + _form][1]
+        _SIGNATURES["ktb_mlp_bf16_td_target" + _policy + _form] = (
+            c_int, _args[:_at] + [c_int] + [c_void_p] * 6 + [c_float, c_float, c_int, ctypes.c_uint64, ctypes.c_uint64]
+            + [_side, _side, c_float] + _alpha + [c_void_p] + _args[_at + 4:])
 _SIGNATURES["ktb_push_scatter_ce_sides"] = (
     c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
                                                          ctypes.c_ulonglong, c_uintptr])

@@ -7,7 +7,8 @@ the greedy and sampled heads (one categorical per group of columns), the _gaussi
 head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network's ε-greedy actor), the _evaluate
 and _gaussian_evaluate forms (the log-probability and entropy of given actions), the _deterministic forms (DDPG's and
 TD3's actor: tanh actions with clipped Gaussian noise), the _critic forms (Q(s, a) critics with the actions fed into
-layer 1, single or twin) and their scatter→exec→gather form."""
+layer 1, single or twin), the _td_target forms (TD3's, DDPG's and SAC's Bellman target: the actor, the target critics
+and the target in one call) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -37,6 +38,12 @@ def pushed_scratch_bytes(M: int, d_hidden: int, chunk_rows: int, critic: bool = 
     chunk that ktb_mlp_scratch_bytes uses for the pull forms."""
     rows = min(int(chunk_rows), int(M))
     return 2 * rows * int(d_hidden) * 2 + (rows * 64 * 2 if critic else 0)
+
+
+def pushed_td_scratch_bytes(M: int, d_hidden_actor: int, d_hidden: int, d_act: int, chunk_rows: int) -> int:
+    """Scratch of the _td_target _pushed entries: ktb_mlp_td_target_scratch_bytes at the pushed form's chunk_rows."""
+    rows = min(int(chunk_rows), int(M))
+    return pushed_scratch_bytes(M, max(d_hidden_actor, d_hidden), chunk_rows, True) + rows * (4 * int(d_act) + 8)
 
 
 def _cached_buffer(cache: dict, key, dev: int, nbytes: int) -> torch.Tensor:
@@ -234,20 +241,8 @@ def _check_critic(w1, w2, w3, biases, obs, action, twin) -> None:
     if tuple(w1.shape) != (d_hidden, d_in + d_act):
         raise ValueError(f"w1 must be [d_hidden, d_in + d_act] = [{d_hidden}, {d_in + d_act}] (the critic's layer 1 "
                          f"over torch.cat([obs, action], -1)), got {tuple(w1.shape)}")
-    if twin is None:
-        return
-    if not isinstance(twin, (tuple, list)) or len(twin) != 6:
-        raise ValueError("twin must be (w1, b1, w2, b2, w3, b3) of the second critic (biases None without biases)")
-    for name, t, mine in zip(("b1", "b2", "b3"), twin[1::2], biases):
-        if (t is None) != (mine is None):
-            raise ValueError(f"twin: {name} is given exactly when the first critic's is")
-    for name, t, like in zip(("w1", "w2", "w3", "b1", "b2", "b3"), (*twin[0::2], *twin[1::2]), (w1, w2, w3, *biases)):
-        if t is None:
-            continue
-        if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16 or tuple(t.shape) != tuple(like.shape) \
-                or not t.is_contiguous() or not t.is_cuda or t.device != w1.device:
-            raise ValueError(f"twin: {name} must be a contiguous CUDA bfloat16 tensor of shape {tuple(like.shape)} on "
-                             f"the device of w1 ({w1.device})")
+    if twin is not None:
+        _check_twin(twin, w1, w2, w3, biases)
 
 
 def _padded_w1(w1: torch.Tensor, d_in: int) -> torch.Tensor:
@@ -273,9 +268,108 @@ def _padded_w1(w1: torch.Tensor, d_in: int) -> torch.Tensor:
     return entry[2]
 
 
+def _check_twin(twin, w1, w2, w3, biases) -> None:
+    """_check_critic's checks of twin = (w1, b1, w2, b2, w3, b3) of a second critic: six entries, biases given exactly
+    as the first critic's, each weight a contiguous CUDA bfloat16 tensor of the first's shape on the device of w1."""
+    if not isinstance(twin, (tuple, list)) or len(twin) != 6:
+        raise ValueError("twin must be (w1, b1, w2, b2, w3, b3) of the second critic (biases None without biases)")
+    for name, t, mine in zip(("b1", "b2", "b3"), twin[1::2], biases):
+        if (t is None) != (mine is None):
+            raise ValueError(f"twin: {name} is given exactly when the first critic's is")
+    for name, t, like in zip(("w1", "w2", "w3", "b1", "b2", "b3"), (*twin[0::2], *twin[1::2]), (w1, w2, w3, *biases)):
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16 or tuple(t.shape) != tuple(like.shape) \
+                or not t.is_contiguous() or not t.is_cuda or t.device != w1.device:
+            raise ValueError(f"twin: {name} must be a contiguous CUDA bfloat16 tensor of shape {tuple(like.shape)} on "
+                             f"the device of w1 ({w1.device})")
+
+
+TD_POLICIES = ("deterministic", "gaussian")
+
+
+def _check_td_target(w1, w2, w3, biases, obs, twin, seed, log_std, log_std_bounds, squash, noise, noise_clip, actor,
+                     policy, reward, done, gamma, alpha) -> None:
+    """_check_policy's checks of output="td_target", after its refusals, in this order: policy; the policy's options
+    (noise, noise_clip, seed and squash with "deterministic", which refuses log_std, log_std_bounds and alpha; a seed,
+    alpha and the pair log_std = (w_ls, b_ls) with "gaussian", which refuses noise and noise_clip); actor = (w1, b1,
+    w2, b2, w3, b3): six entries, biases given exactly as the critic's, contiguous CUDA bfloat16 on the device of w1,
+    w1 [d_ha, d_in], w2 [d_ha, d_ha], w3 [d_act, d_ha] with 1 <= d_act <= 64; the critic's w3 one row and w1 [d_hidden,
+    d_in + d_act]; the twin; the log-std head against the actor; reward and done fp32 [M] or [M, 1] of one shape,
+    contiguous, on the device of obs [M, d_in]; gamma and alpha finite numbers."""
+    if policy not in TD_POLICIES:
+        raise ValueError(f'policy must be one of {TD_POLICIES} with output="td_target" (the actor of the next '
+                         f'actions), got {policy!r}')
+    if policy == "deterministic":
+        for name, v in (("log_std", log_std), ("log_std_bounds", log_std_bounds), ("alpha", alpha)):
+            if v is not None:
+                raise ValueError(f'{name} is not an argument of policy="deterministic": TD3 and DDPG targets take '
+                                 f'noise, noise_clip, seed and squash, and no entropy term')
+        _check_deterministic(seed, noise, noise_clip, squash)
+    else:
+        for name, v in (("noise", noise), ("noise_clip", noise_clip)):
+            if v is not None:
+                raise ValueError(f'{name} is not an argument of policy="gaussian": SAC\'s next actions are sampled '
+                                 f'with the log-std head, not with added noise')
+        _check_seed(seed)
+        if alpha is None:
+            raise ValueError('alpha is required with policy="gaussian": the entropy coefficient of SAC\'s target')
+        if not isinstance(log_std, (tuple, list)):
+            raise ValueError('log_std=(w_ls, b_ls) is required with policy="gaussian": the actor\'s state-dependent '
+                             'log-std head')
+    if not isinstance(actor, (tuple, list)) or len(actor) != 6:
+        raise ValueError("actor must be (w1, b1, w2, b2, w3, b3) of the actor (biases None without biases)")
+    for name, t, mine in zip(("b1", "b2", "b3"), actor[1::2], biases):
+        if (t is None) != (mine is None):
+            raise ValueError(f"actor: {name} is given exactly when the critic's is")
+    for name, t in zip(("w1", "w2", "w3"), actor[0::2]):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16 or t.dim() != 2 or not t.is_contiguous() \
+                or not t.is_cuda or t.device != w1.device:
+            raise ValueError(f"actor: {name} must be a 2-D contiguous CUDA bfloat16 tensor on the device of w1 "
+                             f"({w1.device})")
+    if not isinstance(obs, torch.Tensor):
+        raise ValueError("a TD target is checked against obs: pass the next observations [M, d_in] it goes with")
+    M, d_in = obs.shape
+    aw1, _, aw2, _, aw3, _ = actor
+    d_ha, d_act = aw1.shape[0], aw3.shape[0]
+    if tuple(aw1.shape) != (d_ha, d_in) or tuple(aw2.shape) != (d_ha, d_ha) or aw3.shape[1] != d_ha:
+        raise ValueError(f"actor: weight shapes must be w1 [d_h, {d_in}], w2 [d_h, d_h], w3 [d_act, d_h] (nn.Linear "
+                         f"layout), got {tuple(aw1.shape)}, {tuple(aw2.shape)}, {tuple(aw3.shape)}")
+    if not 1 <= d_act <= MAX_D_ACT:
+        raise ValueError(f"d_act={d_act}: a TD target's actor takes 1 to {MAX_D_ACT} actions (one K block of the "
+                         f"critic's layer 1)")
+    _check_biases(actor[1::2], d_ha, d_act, "actor: ")
+    if w3.shape[0] != 1:
+        raise ValueError(f"d_out={w3.shape[0]}: a critic's w3 is [1, d_hidden] (one Q-value per row)")
+    if tuple(w1.shape) != (w1.shape[0], d_in + d_act):
+        raise ValueError(f"w1 must be [d_hidden, d_in + d_act] = [{w1.shape[0]}, {d_in + d_act}] (the critic's layer "
+                         f"1 over torch.cat([next_obs, actor(next_obs)], -1)), got {tuple(w1.shape)}")
+    if twin is not None:
+        _check_twin(twin, w1, w2, w3, biases)
+    if policy == "gaussian":
+        _check_state_std(log_std, log_std_bounds, squash, aw3, actor[5], d_ha, d_act, False)
+    for name, t in (("reward", reward), ("done", done)):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) not in ((M,), (M, 1)):
+            raise ValueError(f"{name} must be a float32 tensor of shape ({M},) or ({M}, 1), got "
+                             f"{getattr(t, 'dtype', type(t).__name__)} {tuple(getattr(t, 'shape', ()))}")
+        if not t.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+        if not t.is_cuda or t.device != obs.device:
+            raise ValueError(f"{name} must be a CUDA tensor on the device of obs ({obs.device}), got {t.device}")
+    if reward.shape != done.shape:
+        raise ValueError(f"reward and done must have one shape, got {tuple(reward.shape)} and {tuple(done.shape)}")
+    for name, v in (("gamma", gamma), ("alpha", alpha)):
+        if v is None and name == "alpha":
+            continue
+        if isinstance(v, bool) or not isinstance(v, (int, float)):
+            raise ValueError(f"{name} must be a number, got {v!r}")
+        if not math.isfinite(v):
+            raise ValueError(f"{name} must be finite, got {v!r}")
+
+
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
                   nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None, noise=None,
-                  noise_clip=None, action=None, twin=None, w2=None) -> None:
+                  noise_clip=None, action=None, twin=None, w2=None, td=(None,) * 6) -> None:
     """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
     (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
     a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
@@ -292,9 +386,23 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
     takes noise, noise_clip, a seed and squash (_check_deterministic) and refuses mask, value, nvec, log_std,
     log_std_bounds, epsilon and taken; noise and noise_clip are refused with any other output.  output="critic" takes
     the action and an optional twin (_check_critic) and refuses seed, mask, value, nvec, log_std, log_std_bounds,
-    squash, epsilon, taken, noise and noise_clip; action and twin are refused with any other output."""
+    squash, epsilon, taken, noise and noise_clip; action and twin are refused with any other output.
+    output="td_target" refuses mask, value, nvec, epsilon, taken and action, and checks the rest with _check_td_target;
+    td = (actor, policy, reward, done, gamma, alpha), each refused with any other output."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
+    if output == "td_target":
+        for name, v in (("mask", mask), ("value", value), ("nvec", nvec), ("epsilon", epsilon), ("taken", taken),
+                        ("action", action)):
+            if v is not None:
+                raise ValueError(f'{name} is not an argument of output="td_target": a TD target takes twin, actor, '
+                                 f'policy and its options, reward, done, gamma and alpha only')
+        _check_td_target(w1, w2, w3, biases, obs, twin, seed, log_std, log_std_bounds, squash, noise, noise_clip, *td)
+        _check_biases(biases, w1.shape[0], w3.shape[0])
+        return
+    if any(v is not None for v in td):
+        raise ValueError(f'actor, policy, reward, done, gamma and alpha are arguments of output="td_target", not of '
+                         f'output={output!r}')
     if output == "critic":
         for name, v in (("seed", seed), ("mask", mask), ("value", value), ("nvec", nvec), ("log_std", log_std),
                         ("log_std_bounds", log_std_bounds), ("squash", squash), ("epsilon", epsilon),
@@ -368,12 +476,17 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
             raise ValueError(f"mask must be a CUDA tensor on the device of obs ({obs.device}), got {mask.device}")
     if value is not None:
         _check_value(value, output, w3, biases[2], d_hidden, d_out)
+    _check_biases(biases, d_hidden, d_out)
+
+
+def _check_biases(biases, d_hidden, d_out, what="") -> None:
+    """Each bias given is a 1-D contiguous CUDA bfloat16 tensor of its layer's width."""
     for name, b, n in zip(("b1", "b2", "b3"), biases, (d_hidden, d_hidden, d_out)):
         if b is None:
             continue
         if not isinstance(b, torch.Tensor) or b.dtype != torch.bfloat16 or not b.is_cuda or not b.is_contiguous() \
                 or b.dim() != 1 or b.shape[0] != n:
-            raise ValueError(f"{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
+            raise ValueError(f"{what}{name} must be a 1-D contiguous CUDA bfloat16 tensor of length {n}")
 
 
 def _stacked_head(w3, b3, wv=None, bv=None, w_ls=None, b_ls=None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
@@ -545,7 +658,11 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 taken: Optional[torch.Tensor] = None, entropy: Optional[torch.Tensor] = None,
                 noise: Optional[float] = None, noise_clip: Optional[float] = None,
                 action: Optional[torch.Tensor] = None, twin: Optional[Sequence[Optional[torch.Tensor]]] = None,
-                q2: Optional[torch.Tensor] = None, q_min: Optional[torch.Tensor] = None, _stacked: bool = False):
+                q2: Optional[torch.Tensor] = None, q_min: Optional[torch.Tensor] = None,
+                actor: Optional[Sequence[Optional[torch.Tensor]]] = None, policy: Optional[str] = None,
+                reward: Optional[torch.Tensor] = None, done: Optional[torch.Tensor] = None,
+                gamma: Optional[float] = None, alpha: Optional[float] = None, target: Optional[torch.Tensor] = None,
+                _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -601,10 +718,21 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     first's) it returns (q1, q2, q_min), into `q`, `q2` and `q_min` when given: q_min = torch.minimum(q1, q2) (NaN
     when either is, q1 on ties).  Layer 1 runs over w1 padded with zero columns to d_in + 64 (_padded_w1, kept per
     device and weight) and reads the actions, packed to bf16 once per row chunk, as its last K block; the
-    observations are never copied.  `_stacked` (internal, from
+    observations are never copied.  output="td_target" (the Bellman target of TD3, DDPG and SAC, forward only)
+    returns fp32 y of the shape of `reward`, into `target` when given: obs are the next observations, w1, w2, w3 and
+    biases the (target) critic's and `twin` an optional second one, as with "critic"; `actor` = (w1, b1, w2, b2, w3,
+    b3) is the (target) actor, biases given exactly when the critic's are, w3 [d_act, d_ha] with its own d_ha.  With
+    policy="deterministic" (TD3, DDPG) the next actions are output="deterministic"'s with `noise`, `noise_clip`,
+    `seed` and `squash`; with policy="gaussian" (SAC) they and their log-probabilities are output="gaussian"'s with
+    log_std = (w_ls, b_ls), `log_std_bounds`, `squash` and `seed`, the noise of global rows row_offset, ....  Then
+    t = q (q_min with a twin), less alpha * logp with "gaussian", and y = reward + gamma * (1 - done) * t evaluated in
+    fp32 as torch evaluates that expression; `reward` and `done` are fp32 [M] or [M, 1] on the device of obs, and gamma
+    and alpha finite numbers (alpha required with "gaussian" and refused with "deterministic").  Per row chunk the
+    actor's actions stay in scratch and feed the critics' action tile; nothing M-sized but y is written.
+    `_stacked` (internal, from
     mlp_scatter_gather, which checked the call): w3 and biases[2] are
     already the head the C entry takes (stacked with a value head, interleaved with a log-std head), and a critic's
-    w1 (and its twin's) is already W1p."""
+    w1 (and its twin's) is already W1p; a TD target's actor w3 and b3 are already interleaved with its log-std head."""
     for name, t in (("obs", obs), ("w1", w1), ("w2", w2), ("w3", w3)):
         if t.dtype != torch.bfloat16 or not t.is_cuda or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous CUDA bfloat16 tensor")
@@ -613,12 +741,18 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     M, d_in = obs.shape
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     critic = output == "critic"
-    d_w1 = w1.shape[1] if critic else d_in   # a critic's layer 1 also reads the actions: checked by _check_critic
+    td = (actor, policy, reward, done, gamma, alpha)
+    # a critic's layer 1 also reads the actions: checked by _check_critic and _check_td_target
+    d_w1 = w1.shape[1] if critic or output == "td_target" else d_in
     if w1.shape != (d_hidden, d_w1) or w2.shape != (d_hidden, d_hidden) or w3.shape != (d_out, d_hidden):
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
     if not _stacked:
         _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon,
-                      taken, noise, noise_clip, action, twin, w2)
+                      taken, noise, noise_clip, action, twin, w2, td)
+    if output == "td_target":
+        return _td_target(obs, w1, w2, w3, biases, twin, td, seed, log_std, log_std_bounds, squash, noise, noise_clip,
+                          row_offset, target, dev, stream if stream is not None else torch.cuda.current_stream(dev),
+                          staged, _stacked)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     valued = value is not None or (_stacked and values is not None)
     if _stacked:
@@ -663,6 +797,51 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     return _result(output, out, actions, log_probs, values)
 
 
+def _td_args(policy, seed, log_std, log_std_bounds, squash, noise, noise_clip, row_offset):
+    """The policy's arguments of a _td_target entry: those of the standalone _deterministic or _gaussian_state entry,
+    (noise, noise_clip, squash) or (log_std_min, log_std_max, squash), then seed (0 for a noise-free actor, which draws
+    nothing) and row_base."""
+    if policy == "deterministic":
+        return (*_det(noise, noise_clip, squash), seed or 0, row_offset)
+    return (*_std(log_std, log_std_bounds, squash), seed, row_offset)
+
+
+def _td_target(obs, w1, w2, w3, biases, twin, td, seed, log_std, log_std_bounds, squash, noise, noise_clip,
+               row_offset, target, dev, s, staged, stacked):
+    """mlp_forward's output="td_target" on `dev` and stream `s`: y of the shape of reward, into `target` when given."""
+    actor, policy, reward, done, gamma, alpha = td
+    if isinstance(row_offset, bool) or not isinstance(row_offset, int) or row_offset < 0:
+        raise ValueError(f"row_offset must be a non-negative int, got {row_offset!r}")
+    M, d_in = obs.shape
+    gaussian = policy == "gaussian"
+    aw1, ab1, aw2, ab2, aw3, ab3 = actor
+    if target is None:
+        target = torch.empty(reward.shape, dtype=torch.float32, device=f"cuda:{dev}")
+    else:
+        ops.ensure_init({target.device.index})
+    if not stacked:
+        with torch.cuda.stream(s):   # a rewrite of W1p or of the interleaved head is ordered after earlier calls on s
+            w1 = _padded_w1(w1, d_in)
+            if twin is not None:
+                twin = (_padded_w1(twin[0], d_in), *twin[1:])
+            if gaussian:
+                aw3, ab3 = _stacked_head(aw3, ab3, None, None, *log_std)
+    d_act = aw3.shape[0] // (2 if gaussian else 1)
+    if staged is None:
+        staged = obs.device.index != dev
+    ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+    lib = L.load()
+    scratch = _cached_buffer(_scratch, dev, dev,
+                             lib.ktb_mlp_td_target_scratch_bytes(M, aw1.shape[0], w1.shape[0], d_act))
+    L.call("ktb_mlp_bf16_td_target_" + policy, dev, obs.data_ptr(), M, d_in, w1.shape[0], d_act, w1.data_ptr(),
+           ptr(biases[0]), w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]),
+           *(ptr(t) for t in (twin or (None,) * 6)), aw1.shape[0], *(ptr(t) for t in (aw1, ab1, aw2, ab2, aw3, ab3)),
+           *_td_args(policy, seed, log_std, log_std_bounds, squash, noise, noise_clip, row_offset), reward.data_ptr(),
+           done.data_ptr(), float(gamma), *((float(alpha),) if gaussian else ()), target.data_ptr(),
+           scratch.data_ptr(), _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
+    return target
+
+
 def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     """Weights are shared by all ranks: broadcast once per (weights, device) and kept resident
     (excluded from per-call bytes, SURVEY.md §8(d) C4)."""
@@ -683,6 +862,17 @@ def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
 
 
 PUSH_CHUNK_ROWS = 16896      # 132 SMs x 128 rows: each 256-wide layer of a chunk is whole waves of 128 x 256 tiles
+
+
+def _use_push(devs, bounds, transfer) -> bool:
+    """Whether a scatter→exec→gather call takes the push form: distinct devices, shards of whole 128-row blocks and at
+    most 64 chunks each, unless transfer="pull"; transfer="push" without them is a ValueError."""
+    distinct = len(set(devs)) == len(devs) and len(devs) > 1
+    pushable = distinct and all((e - b) % 128 == 0 for b, e in bounds) and \
+        -(-max(e - b for b, e in bounds) // PUSH_CHUNK_ROWS) <= 64
+    if transfer == "push" and not pushable:
+        raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
+    return pushable and transfer != "pull"
 _push_sessions = {}          # device tuple -> ops.PushSession
 _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pushed GEMMs
 
@@ -809,7 +999,11 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        noise_clip: Optional[float] = None, action: Optional[torch.Tensor] = None,
                        twin: Optional[Sequence[Optional[torch.Tensor]]] = None,
                        q_root: Optional[torch.Tensor] = None, q2_root: Optional[torch.Tensor] = None,
-                       q_min_root: Optional[torch.Tensor] = None) -> list:
+                       q_min_root: Optional[torch.Tensor] = None,
+                       actor: Optional[Sequence[Optional[torch.Tensor]]] = None, policy: Optional[str] = None,
+                       reward: Optional[torch.Tensor] = None, done: Optional[torch.Tensor] = None,
+                       gamma: Optional[float] = None, alpha: Optional[float] = None,
+                       target_root: Optional[torch.Tensor] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -833,13 +1027,22 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     and `twin` as in mlp_forward returns fp32 q [rows] views of `q_root`, or (q1, q2, q_min) triples of views of
     `q_root`, `q2_root` and `q_min_root` with a twin; each rank reads its rows of action in place on the pull form, and
     the push form pushes them with the rows.  W1p (and the twin's) is built on the root and copied to the other devices
-    like the other weights, again after an in-place update of w1."""
+    like the other weights, again after an in-place update of w1.  output="td_target" with `actor`, `policy`, its
+    options, `twin`, `reward`, `done` (on the root), `gamma` and `alpha` as in mlp_forward returns fp32 y views of
+    `target_root` (of reward's shape, allocated on the root when None); each rank draws the noise of its shard's global
+    rows, reads its rows of reward and done in place on the pull form, and the push form pushes them with the rows."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
+    td = (actor, policy, reward, done, gamma, alpha)
     _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon,
-                  taken, noise, noise_clip, action, twin, w2)
+                  taken, noise, noise_clip, action, twin, w2, td)
+    if transfer not in ("auto", "pull", "push"):
+        raise ValueError("transfer must be 'auto', 'pull' or 'push'")
+    if output == "td_target":
+        return _td_scatter_gather(obs_root, w1, w2, w3, devs, transfer, biases, twin, td, seed, log_std,
+                                  log_std_bounds, squash, noise, noise_clip, target_root)
     critic = output == "critic"
     if critic:   # q (or q1), q2 and q_min ride in the logits, actions and log_probs slots
         out_root, actions_root, log_probs_root = q_root, q2_root, q_min_root
@@ -873,14 +1076,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         log_stds = {dev: log_std for dev in set(devs)}
     else:
         log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
-    distinct = len(set(devs)) == len(devs) and len(devs) > 1
-    pushable = distinct and all((e - b) % 128 == 0 for b, e in bounds) and \
-        -(-max(e - b for b, e in bounds) // PUSH_CHUNK_ROWS) <= 64
-    if transfer not in ("auto", "pull", "push"):
-        raise ValueError("transfer must be 'auto', 'pull' or 'push'")
-    if transfer == "push" and not pushable:
-        raise ValueError("push transfer needs distinct devices and shards of a multiple of 128 rows")
-    if pushable and transfer != "pull":
+    if _use_push(devs, bounds, transfer):
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
                                    nvec, std, epsilon, taken, det, action, twins)
         return views
@@ -923,6 +1119,117 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     else:
         done = [issue(r) for r in range(len(devs))]
     for ev in done:
+        if ev is not None:
+            root_stream.wait_event(ev)
+    return views
+
+
+def _td_scatter_gather(obs_root, w1, w2, w3, devs, transfer, biases, twin, td, seed, log_std, log_std_bounds, squash,
+                       noise, noise_clip, target_root) -> list:
+    """mlp_scatter_gather's output="td_target" (checked): the critics' W1p and the SAC actor's interleaved head are
+    built on the root and copied to the other devices like the other weights; rank r computes y of rows b_r .. e_r - 1
+    with row_offset b_r, pulling its rows of obs, reward and done in place or having them pushed with ktb_push_scatter_ce_sides
+    (each staging half rows | reward | done, each 256-byte aligned), and stores them into the root's y."""
+    actor, policy, reward, done, gamma, alpha = td
+    root, n = devs[0], len(devs)
+    M, d_in = obs_root.shape
+    ops.ensure_init(set(devs))
+    gaussian = policy == "gaussian"
+    if target_root is None:
+        target_root = torch.empty(reward.shape, dtype=torch.float32, device=obs_root.device)
+    else:
+        ops.ensure_init({target_root.device.index})
+    w1 = _padded_w1(w1, d_in)
+    if twin is not None:
+        twin = (_padded_w1(twin[0], d_in), *twin[1:])
+    actor = tuple(actor)
+    if gaussian:
+        actor = actor[:4] + _stacked_head(actor[4], actor[5], None, None, *log_std)
+    d_hidden, d_ha, d_act = w1.shape[0], actor[0].shape[0], actor[4].shape[0] // (2 if gaussian else 1)
+    weights = {dev: _weights_on(dev, (w1, biases[0], w2, biases[1], w3, biases[2])) for dev in set(devs)}
+    twins = {dev: None if twin is None else tuple(_weights_on(dev, twin)) for dev in set(devs)}
+    actors = {dev: tuple(_weights_on(dev, actor)) for dev in set(devs)}
+    bounds = [ops.shard_bounds(M, n, r) for r in range(n)]
+    views = [target_root[b:e] for b, e in bounds]
+    rows = max(e - b for b, e in bounds)
+    opts = dict(output="td_target", policy=policy, gamma=gamma, alpha=alpha, seed=seed, log_std=log_std,
+                log_std_bounds=log_std_bounds, squash=squash, noise=noise, noise_clip=noise_clip, _stacked=True)
+
+    def run(dev, b, e, stream, staged):
+        ws = weights[dev]
+        mlp_forward(obs_root[b:e], ws[0], ws[2], ws[4], device=dev, stream=stream, staged=staged,
+                    biases=(ws[1], ws[3], ws[5]), twin=twins[dev], actor=actors[dev], reward=reward[b:e],
+                    done=done[b:e], target=target_root[b:e], row_offset=b, **opts)
+
+    if _use_push(devs, bounds, transfer):
+        key = tuple(devs)
+        reward_offset = (rows * d_in * 2 + 255) // 256 * 256
+        done_offset = reward_offset + (rows * 4 + 255) // 256 * 256
+        stage_bytes = done_offset + rows * 4
+        sess = _push_sessions.get(key)
+        if sess is None or sess.stride < stage_bytes:
+            sess = _push_sessions[key] = ops.PushSession(devs, stage_bytes)
+        try:
+            seq = sess.begin()
+        except ops.PushTimeout:
+            del _push_sessions[key]
+            raise
+        nbytes = pushed_td_scratch_bytes(rows, d_ha, d_hidden, d_act, PUSH_CHUNK_ROWS)
+        scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], nbytes) for r in range(1, n)]
+        streams = [ops.current_stream_handle(d) for d in devs]
+        b0, e0 = bounds[0]
+        own = e0 > b0
+        if own:
+            run(root, b0, e0, sess.fork(), False)
+        L.call("ktb_push_scatter_ce_sides", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
+               L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
+               PUSH_CHUNK_ROWS * d_in, 2, L.arr(ctypes.c_void_p, [reward.data_ptr(), done.data_ptr()]),
+               L.arr(ctypes.c_size_t, [4, 4]), L.arr(ctypes.c_size_t, [reward_offset, done_offset]), seq, streams[0])
+
+        def issue(r):
+            b, e = bounds[r]
+            ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+            ws, tw = weights[devs[r]], twins[devs[r]]
+            L.call("ktb_mlp_bf16_td_target_" + policy + "_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride,
+                   e - b, d_in, d_hidden, d_act, *(ptr(t) for t in ws), *(ptr(t) for t in (tw or (None,) * 6)), d_ha,
+                   *(ptr(t) for t in actors[devs[r]]),
+                   *_td_args(policy, seed, log_std, log_std_bounds, squash, noise, noise_clip, b), reward_offset,
+                   done_offset, float(gamma), *((float(alpha),) if gaussian else ()),
+                   target_root.data_ptr() + 4 * b if e > b else 0,
+                   scratch[r].data_ptr(), sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq,
+                   streams[r])
+
+        list(_thread_pool().map(issue, range(1, n)))
+        sess.finish(seq, joined=own)
+        return views
+    lib = L.load()
+    for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
+        _cached_buffer(_scratch, dev, dev, lib.ktb_mlp_td_target_scratch_bytes(rows, d_ha, d_hidden, d_act))
+        if dev != root:
+            _stage_for(dev, rows, d_in)
+    root_stream = torch.cuda.current_stream(root)
+    ready = torch.cuda.Event()
+    ready.record(root_stream)
+    streams = {dev: torch.cuda.current_stream(dev) for dev in set(devs)}
+
+    def issue_pull(r):
+        dev = devs[r]
+        b, e = bounds[r]
+        if e == b:
+            return None
+        st = streams[dev]
+        with torch.cuda.device(dev):
+            if dev != root:
+                st.wait_event(ready)
+            run(dev, b, e, st, None)
+            if dev != root:
+                ev = torch.cuda.Event()
+                ev.record(st)
+                return ev
+        return None
+
+    done_evs = list(_thread_pool().map(issue_pull, range(n))) if len(set(devs)) > 1 else [issue_pull(r) for r in range(n)]
+    for ev in done_evs:
         if ev is not None:
             root_stream.wait_event(ev)
     return views

@@ -24,8 +24,9 @@ MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
-               "gaussian_evaluate", "deterministic", "critic")   # also device.mlp.OUTPUTS
+               "gaussian_evaluate", "deterministic", "critic", "td_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
+TD_OPTIONS = ("actor", "policy", "reward", "done", "gamma", "alpha")   # the options of output="td_target" alone
 
 
 @dataclass
@@ -66,7 +67,10 @@ class MappedSpec:
         return arguments[tensor_name], resolve(self.alpha), resolve(self.beta), arguments
 
 
-def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = None, arg: str = None, **extra):
+_UNSET = object()   # mapped()'s alpha when not given: 1.0, and no entropy coefficient of a TD target
+
+
+def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] = None, arg: str = None, **extra):
     """Declare that the decorated function is computed by device op `op` (see module docstring).
 
     The "mlp" op takes more options.  ``bias=True``: the callable is ``(obs, w1, b1, w2, b2, w3, b3, ...)``, an
@@ -124,13 +128,32 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
     critic's six arguments ``(w1, b1, w2, b2, w3, b3)`` (three, ``(w1, w2, w3)``, without ``bias=True``): each rank then
     returns ``(q1, q2, q_min)`` with ``q_min = torch.minimum(q1, q2)``.  ``seed=``, ``mask=``, ``value=``, ``nvec=``,
     ``log_std=``, ``log_std_bounds=``, ``squash=``, ``epsilon=``, ``taken=``, ``noise=`` and ``noise_clip=`` are
-    refused, and ``action=`` and ``twin=`` with every other output."""
+    refused, and ``action=`` and ``twin=`` with every other output.
+    ``output="td_target"`` is the Bellman target of TD3, DDPG and SAC (forward only): the callable is ``(next_obs,
+    w1, b1, w2, b2, w3, b3, ...)``, the (target) critic as with ``"critic"``, and each rank returns the fp32 ``y`` of
+    its rows, ``reward + gamma * (1 - done) * t``.  ``actor=`` names the (target) actor's six arguments (three without
+    ``bias=True``); ``policy="deterministic"`` takes its next actions as ``output="deterministic"`` does, with
+    ``noise=``, ``noise_clip=``, ``seed=`` and ``squash=`` (TD3: ``noise=0.2, noise_clip=0.5``; DDPG: no noise), and
+    ``t`` is the critic's ``q``, or with ``twin=`` the minimum of the two; ``policy="gaussian"`` samples them as
+    ``output="gaussian"`` with ``log_std=(w_ls, b_ls)``, ``log_std_bounds=``, ``squash=`` and ``seed=`` (SAC), and
+    ``t`` less ``alpha * log_prob``.  ``reward=`` and ``done=`` name fp32 ``[M]`` or ``[M, 1]`` arguments on the device
+    of obs (the body takes their ``chunk(WORLD_SIZE)[RANK]``), ``gamma=`` is a finite number and ``alpha=`` (with
+    ``"gaussian"`` only, required there) a finite number or the name of a call argument that holds a number or a
+    one-element tensor; a CUDA tensor is read with ``float()``, one host synchronisation per call.  ``mask=``,
+    ``value=``, ``nvec=``, ``epsilon=``, ``taken=`` and ``action=`` are refused, and these options with every other
+    output."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
+    if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
+        extra["alpha"] = alpha
+    alpha = 1.0 if alpha is _UNSET or op == "mlp" and "alpha" in extra else alpha
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
     if op != "mlp" and any(k in extra for k in ("action", "twin")):
         raise ValueError(f"action= and twin= are options of the 'mlp' op, not of '{op}'")
+    if op != "mlp" and any(k in extra for k in TD_OPTIONS):
+        raise ValueError(f"actor=, policy=, reward=, done=, gamma= and alpha= are options of the 'mlp' op, not of "
+                         f"'{op}'")
     if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
                                 "squash", "epsilon", "taken", "noise", "noise_clip", "action", "twin")):
         if op != "mlp":
@@ -140,96 +163,103 @@ def mapped(op: str, alpha: Any = 1.0, beta: Any = 0.0, reduce: Optional[str] = N
             raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
         if extra.get("output", "logits") not in MLP_OUTPUTS:
             raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
-        if extra.get("output") == "critic":
-            _check_critic(extra)
-        elif "action" in extra or "twin" in extra:
-            raise ValueError(f'action= and twin= are options of output="critic", not of '
-                             f'output={extra.get("output", "logits")!r}')
-        sample = extra.get("output") in ("sample", "gaussian")
-        eps = extra.get("output") == "epsilon_greedy"
-        det = extra.get("output") == "deterministic"
-        if det:
-            _check_deterministic(extra)
-        elif "noise" in extra or "noise_clip" in extra:
-            raise ValueError(f'noise= and noise_clip= are options of output="deterministic", not of '
-                             f'output={extra.get("output", "logits")!r}')
-        evaluate = extra.get("output") in EVALUATE_OUTPUTS
-        if evaluate != ("taken" in extra):
-            raise ValueError('taken= is required with output="evaluate" and "gaussian_evaluate" and is an option of '
-                             'those outputs only')
-        if evaluate and not isinstance(extra["taken"], str):
-            raise ValueError(f"taken must be the name of a call argument, got {extra['taken']!r}")
-        if evaluate and "seed" in extra:
-            raise ValueError(f'seed= is not an option of output={extra["output"]!r}: evaluating given actions draws '
-                             f'no noise')
-        if not det and (sample or eps) != ("seed" in extra):
-            raise ValueError('seed= is required with output="sample" or "gaussian" (or "epsilon_greedy") and is an '
-                             'option of those only')
-        if (sample or eps or det) and "seed" in extra and not isinstance(extra["seed"], str):
-            from .sampling import _check_seed
+        if extra.get("output") == "td_target":
+            _check_td_target(extra)
+        elif any(k in extra for k in TD_OPTIONS):
+            raise ValueError(f'actor=, policy=, reward=, done=, gamma= and alpha= are options of output="td_target", '
+                             f'not of output={extra.get("output", "logits")!r}')
+        else:
+            if extra.get("output") == "critic":
+                _check_critic(extra)
+            elif "action" in extra or "twin" in extra:
+                raise ValueError(f'action= and twin= are options of output="critic", not of '
+                                 f'output={extra.get("output", "logits")!r}')
+            sample = extra.get("output") in ("sample", "gaussian")
+            eps = extra.get("output") == "epsilon_greedy"
+            det = extra.get("output") == "deterministic"
+            if det:
+                _check_deterministic(extra)
+            elif "noise" in extra or "noise_clip" in extra:
+                raise ValueError(f'noise= and noise_clip= are options of output="deterministic", not of '
+                                 f'output={extra.get("output", "logits")!r}')
+            evaluate = extra.get("output") in EVALUATE_OUTPUTS
+            if evaluate != ("taken" in extra):
+                raise ValueError('taken= is required with output="evaluate" and "gaussian_evaluate" and is an option of '
+                                 'those outputs only')
+            if evaluate and not isinstance(extra["taken"], str):
+                raise ValueError(f"taken must be the name of a call argument, got {extra['taken']!r}")
+            if evaluate and "seed" in extra:
+                raise ValueError(f'seed= is not an option of output={extra["output"]!r}: evaluating given actions draws '
+                                 f'no noise')
+            if not det and (sample or eps) != ("seed" in extra):
+                raise ValueError('seed= is required with output="sample" or "gaussian" (or "epsilon_greedy") and is an '
+                                 'option of those only')
+            if (sample or eps or det) and "seed" in extra and not isinstance(extra["seed"], str):
+                from .sampling import _check_seed
 
-            _check_seed(extra["seed"])
-        gaussian = extra.get("output") in ("gaussian", "gaussian_evaluate")
-        if gaussian != ("log_std" in extra):
-            raise ValueError('log_std= is required with output="gaussian" (and "gaussian_evaluate") and is an option of '
-                             'those outputs only')
-        state = gaussian and isinstance(extra["log_std"], (tuple, list))
-        if state and evaluate:
-            raise ValueError('output="gaussian_evaluate" takes a state-independent log_std (the name of one call '
-                             'argument), not a log_std=(w_ls, b_ls) pair')
-        if state:
-            ls = extra["log_std"]
-            if len(ls) != 2 or not all(isinstance(n, str) for n in ls):
-                raise ValueError(f"log_std must name one call argument or two (w_ls, b_ls), got {ls!r}")
-            if not extra.get("bias", False):
-                raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when "
-                                 "b3 is")
-        elif gaussian and not isinstance(extra["log_std"], str):
-            raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
-        if not state and ("log_std_bounds" in extra or "squash" in extra and not det):
-            raise ValueError("log_std_bounds= and squash= are options of a state-dependent log_std=(w_ls, b_ls) only")
-        if "log_std_bounds" in extra:
-            lb = extra["log_std_bounds"]
-            if not isinstance(lb, (tuple, list)) or len(lb) != 2 or \
-                    not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in lb):
-                raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {lb!r}")
-            if lb[0] != lb[0] or lb[1] != lb[1]:
-                raise ValueError(f"log_std_bounds must not be NaN, got {lb!r}")
-            if lb[0] > lb[1]:
-                raise ValueError(f"log_std_bounds must have low <= high, got {lb!r}")
-            extra["log_std_bounds"] = (float(lb[0]), float(lb[1]))
-        if "squash" in extra and not isinstance(extra["squash"], bool):
-            raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
-        if "mask" in extra:
-            if gaussian:
-                raise ValueError(f'mask= is an option of the categorical outputs, not of output={extra["output"]!r}')
-            if not isinstance(extra["mask"], str):
-                raise ValueError(f"mask must be the name of a call argument, got {extra['mask']!r}")
-        if "value" in extra:
-            if not (sample or evaluate):
-                raise ValueError('value= is an option of output="sample", "gaussian", "evaluate" and '
-                                 '"gaussian_evaluate" only')
-            if not extra.get("bias", False):
-                raise ValueError("value= needs bias=True: the critic's bias is given exactly when b3 is")
-            v = extra["value"]
-            if not isinstance(v, (tuple, list)) or len(v) != 2 or not all(isinstance(n, str) for n in v):
-                raise ValueError(f"value must name two call arguments (wv, bv), got {v!r}")
-        if "nvec" in extra:
-            extra["nvec"] = check_nvec(extra["nvec"], extra.get("output", "logits"))
-        if eps != ("epsilon" in extra):
-            raise ValueError('epsilon= is required with output="epsilon_greedy" and is an option of that output only')
-        if eps and not isinstance(extra["epsilon"], str):
-            e = extra["epsilon"]
-            if isinstance(e, bool) or not isinstance(e, (int, float)):
-                raise ValueError(f"epsilon must be a number or the name of a call argument, got {e!r}")
-            if e != e:
-                raise ValueError("epsilon must not be NaN (a NaN never explores: pass 0.0 for that)")
+                _check_seed(extra["seed"])
+            gaussian = extra.get("output") in ("gaussian", "gaussian_evaluate")
+            if gaussian != ("log_std" in extra):
+                raise ValueError('log_std= is required with output="gaussian" (and "gaussian_evaluate") and is an option of '
+                                 'those outputs only')
+            state = gaussian and isinstance(extra["log_std"], (tuple, list))
+            if state and evaluate:
+                raise ValueError('output="gaussian_evaluate" takes a state-independent log_std (the name of one call '
+                                 'argument), not a log_std=(w_ls, b_ls) pair')
+            if state:
+                ls = extra["log_std"]
+                if len(ls) != 2 or not all(isinstance(n, str) for n in ls):
+                    raise ValueError(f"log_std must name one call argument or two (w_ls, b_ls), got {ls!r}")
+                if not extra.get("bias", False):
+                    raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when "
+                                     "b3 is")
+            elif gaussian and not isinstance(extra["log_std"], str):
+                raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
+            if not state and ("log_std_bounds" in extra or "squash" in extra and not det):
+                raise ValueError("log_std_bounds= and squash= are options of a state-dependent log_std=(w_ls, b_ls) only")
+            if "log_std_bounds" in extra:
+                lb = extra["log_std_bounds"]
+                if not isinstance(lb, (tuple, list)) or len(lb) != 2 or \
+                        not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in lb):
+                    raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {lb!r}")
+                if lb[0] != lb[0] or lb[1] != lb[1]:
+                    raise ValueError(f"log_std_bounds must not be NaN, got {lb!r}")
+                if lb[0] > lb[1]:
+                    raise ValueError(f"log_std_bounds must have low <= high, got {lb!r}")
+                extra["log_std_bounds"] = (float(lb[0]), float(lb[1]))
+            if "squash" in extra and not isinstance(extra["squash"], bool):
+                raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
+            if "mask" in extra:
+                if gaussian:
+                    raise ValueError(f'mask= is an option of the categorical outputs, not of output={extra["output"]!r}')
+                if not isinstance(extra["mask"], str):
+                    raise ValueError(f"mask must be the name of a call argument, got {extra['mask']!r}")
+            if "value" in extra:
+                if not (sample or evaluate):
+                    raise ValueError('value= is an option of output="sample", "gaussian", "evaluate" and '
+                                     '"gaussian_evaluate" only')
+                if not extra.get("bias", False):
+                    raise ValueError("value= needs bias=True: the critic's bias is given exactly when b3 is")
+                v = extra["value"]
+                if not isinstance(v, (tuple, list)) or len(v) != 2 or not all(isinstance(n, str) for n in v):
+                    raise ValueError(f"value must name two call arguments (wv, bv), got {v!r}")
+            if "nvec" in extra:
+                extra["nvec"] = check_nvec(extra["nvec"], extra.get("output", "logits"))
+            if eps != ("epsilon" in extra):
+                raise ValueError('epsilon= is required with output="epsilon_greedy" and is an option of that output only')
+            if eps and not isinstance(extra["epsilon"], str):
+                e = extra["epsilon"]
+                if isinstance(e, bool) or not isinstance(e, (int, float)):
+                    raise ValueError(f"epsilon must be a number or the name of a call argument, got {e!r}")
+                if e != e:
+                    raise ValueError("epsilon must not be NaN (a NaN never explores: pass 0.0 for that)")
 
     def deco(fn):
         params = inspect.signature(fn).parameters
-        for option in ("log_std", "mask", "value", "epsilon", "taken", "noise", "action", "twin"):
+        for option in ("log_std", "mask", "value", "epsilon", "taken", "noise", "action", "twin", "actor", "reward",
+                       "done", "alpha"):
             names = extra.get(option)
-            if option in ("epsilon", "noise") and not isinstance(names, str):   # a constant names no argument
+            if option in ("epsilon", "noise", "alpha") and not isinstance(names, str):   # a constant names no argument
                 continue
             for name in (names,) if isinstance(names, str) or names is None else names:
                 if name is not None and name not in params:
@@ -282,6 +312,79 @@ def _check_critic(extra) -> None:
         if not isinstance(t, (tuple, list)) or len(t) != n or not all(isinstance(x, str) for x in t):
             what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
             raise ValueError(f"twin must name the second critic's {n} call arguments {what}, got {t!r}")
+
+
+def _check_td_target(extra) -> None:
+    """mapped()'s checks of output="td_target", in this order: the options it refuses, policy=, the policy's options
+    (noise=, noise_clip= and seed= as output="deterministic" takes them, refusing log_std=, log_std_bounds= and alpha=;
+    or seed=, alpha=, log_std=(w_ls, b_ls) with bias=True, log_std_bounds= and squash=, refusing noise= and
+    noise_clip=), actor= (six names with bias=True, three without), twin= as output="critic" takes it, reward= and
+    done= (names), gamma= (a finite number)."""
+    for name in ("mask", "value", "nvec", "epsilon", "taken", "action"):
+        if name in extra:
+            raise ValueError(f'{name}= is not an option of output="td_target": a TD target takes actor=, policy= and '
+                             f'its options, twin=, reward=, done=, gamma= and alpha= only')
+    policy = extra.get("policy")
+    if policy not in ("deterministic", "gaussian"):
+        raise ValueError(f'policy= must be "deterministic" or "gaussian" with output="td_target", got {policy!r}')
+    if policy == "deterministic":
+        for name in ("log_std", "log_std_bounds", "alpha"):
+            if name in extra:
+                raise ValueError(f'{name}= is not an option of policy="deterministic": TD3 and DDPG targets take '
+                                 f'noise=, noise_clip=, seed= and squash=, and no entropy term')
+        _check_deterministic(extra)
+        if "seed" in extra and not isinstance(extra["seed"], str):
+            from .sampling import _check_seed
+
+            _check_seed(extra["seed"])
+    else:
+        for name in ("noise", "noise_clip"):
+            if name in extra:
+                raise ValueError(f'{name}= is not an option of policy="gaussian": SAC\'s next actions are sampled with '
+                                 f'the log-std head')
+        if "seed" not in extra:
+            raise ValueError('seed= is required with policy="gaussian"')
+        if not isinstance(extra["seed"], str):
+            from .sampling import _check_seed
+
+            _check_seed(extra["seed"])
+        a = extra.get("alpha")
+        if a is None:
+            raise ValueError('alpha= is required with policy="gaussian": a number or the name of a call argument')
+        if not isinstance(a, str) and (isinstance(a, bool) or not isinstance(a, (int, float)) or a != a
+                                       or a in (float("inf"), float("-inf"))):
+            raise ValueError(f"alpha must be a finite number or the name of a call argument, got {a!r}")
+        ls = extra.get("log_std")
+        if not isinstance(ls, (tuple, list)) or len(ls) != 2 or not all(isinstance(n, str) for n in ls):
+            raise ValueError(f'log_std= must name the two call arguments (w_ls, b_ls) of the actor\'s log-std head '
+                             f'with policy="gaussian", got {ls!r}')
+        if not extra.get("bias", False):
+            raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when b3 is")
+        if "log_std_bounds" in extra:
+            lb = extra["log_std_bounds"]
+            if not isinstance(lb, (tuple, list)) or len(lb) != 2 or \
+                    not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in lb) or \
+                    lb[0] != lb[0] or lb[1] != lb[1] or lb[0] > lb[1]:
+                raise ValueError(f"log_std_bounds must be (low, high), two numbers, not NaN, low <= high, got {lb!r}")
+            extra["log_std_bounds"] = (float(lb[0]), float(lb[1]))
+    if "squash" in extra and not isinstance(extra["squash"], bool):
+        raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
+    n = 6 if extra.get("bias", False) else 3
+    for option in ("actor", "twin"):
+        if option not in extra and option == "twin":
+            continue
+        t = extra.get(option)
+        if not isinstance(t, (tuple, list)) or len(t) != n or not all(isinstance(x, str) for x in t):
+            what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
+            whose = "the actor's" if option == "actor" else "the second critic's"
+            raise ValueError(f"{option} must name {whose} {n} call arguments {what}, got {t!r}")
+    for option in ("reward", "done"):
+        if not isinstance(extra.get(option), str):
+            raise ValueError(f'{option}= is required with output="td_target" and must name a call argument, got '
+                             f'{extra.get(option)!r}')
+    g = extra.get("gamma")
+    if isinstance(g, bool) or not isinstance(g, (int, float)) or g != g or g in (float("inf"), float("-inf")):
+        raise ValueError(f'gamma= is required with output="td_target" and must be a finite number, got {g!r}')
 
 
 def check_nvec(nvec, output: str, d_out: Optional[int] = None) -> tuple:

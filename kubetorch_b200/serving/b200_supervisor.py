@@ -622,13 +622,28 @@ class B200Supervisor:
             twin = tuple(bound[name] for name in twin)
             if len(twin) == 3:   # (w1, w2, w3) of a bias-free critic
                 twin = (twin[0], None, twin[1], None, twin[2], None)
+        td = {}
+        if output == "td_target":   # the actor's weights, reward, done and a named alpha, resolved per call
+            for name in (*spec.extra["actor"], spec.extra["reward"], spec.extra["done"]):
+                if name not in bound:
+                    raise TypeError(f"mapped mlp callable: td_target argument '{name}' not found in the call")
+            actor = tuple(bound[name] for name in spec.extra["actor"])
+            if len(actor) == 3:   # (w1, w2, w3) of a bias-free actor
+                actor = (actor[0], None, actor[1], None, actor[2], None)
+            alpha = spec.extra.get("alpha")
+            if isinstance(alpha, str):
+                if alpha not in bound:
+                    raise TypeError(f"mapped mlp callable: alpha argument '{alpha}' not found in the call")
+                alpha = float(bound[alpha])   # a number or a one-element tensor (on a GPU: one host synchronisation)
+            td = dict(actor=actor, policy=spec.extra["policy"], reward=bound[spec.extra["reward"]],
+                      done=bound[spec.extra["done"]], gamma=spec.extra["gamma"], alpha=alpha)
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
                                          biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
                                          value=value, nvec=spec.extra.get("nvec"),
                                          log_std_bounds=spec.extra.get("log_std_bounds"),
                                          squash=spec.extra.get("squash"), epsilon=epsilon, taken=taken, noise=noise,
-                                         noise_clip=spec.extra.get("noise_clip"), action=action, twin=twin)
+                                         noise_clip=spec.extra.get("noise_clip"), action=action, twin=twin, **td)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

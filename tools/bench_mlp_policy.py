@@ -49,6 +49,12 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      observations (the difference is the action block and the head); and the eager twin, what a user pays without
      the feature: torch.cat of the rows and the bf16 actions padded to d_in + 64, w1 padded likewise, the logits entry
      per critic, .float() and torch.minimum.
+  q  TD targets (output="td_target") over the twin critics of p and a 256 -> 1024 -> 1024 -> d_act actor, d_act 6, 17
+     and 64: TD3's (σ 0.2, clip 0.5) and SAC's (squashed, α 0.2), each beside the two-call arm (the actor entry, the
+     twin critic entry, then reward + 0.99 * (1 - done) * t in eager torch) and the eager arm (the logits entries, the
+     actor's head, the padded concatenation and the minimum in torch).  Before timing, the fused y equals the two-call
+     arm's bit for bit on every row, and is within rtol 2^-7, atol 1e-2 of the eager arm's on at least 99 % of the rows
+     (the eager arm's tanh and log rounding move some bf16 actions by an ulp).
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -144,6 +150,7 @@ def main():
                heads[64][0].data_ptr(), 0, out.data_ptr(), 0, scratch.data_ptr(), 0, stream)
         return out
 
+    parity = {}
     out_a = torch.empty(M, 64, dtype=torch.bfloat16, device="cuda:0")
     out_b = torch.empty(M, 64, dtype=torch.bfloat16, device="cuda:0")
     variants = {
@@ -410,6 +417,81 @@ def main():
         variants[f"p_bias_critic_a{a}"] = (1, lambda a=a: critic_call(a, False))
         variants[f"p_bias_critic_twin_a{a}"] = (1, lambda a=a: critic_call(a, True))
         variants[f"p_bias_critic_twin_eager_a{a}"] = (1, lambda a=a: eager_twin(a))
+    # q: TD targets over the twin critics of p, with a 256 -> 1024 -> 1024 -> d_act actor (its own weights)
+    gq = torch.Generator(device="cuda:0").manual_seed(13)
+    qr = lambda *s, scale=1.0: (torch.randn(*s, device="cuda:0", generator=gq) * scale).bfloat16()   # noqa: E731
+    actors = {a: (qr(d_hidden, d_in, scale=0.02), qr(d_hidden, scale=0.1), qr(d_hidden, d_hidden, scale=0.02),
+                  qr(d_hidden, scale=0.1), qr(a, d_hidden, scale=0.02), qr(a, scale=0.1)) for a in critic_widths}
+    actor_ls = {a: (qr(a, d_hidden, scale=0.02), torch.linspace(-2.0, 0.5, a, device="cuda:0").bfloat16())
+                for a in critic_widths}
+    reward = torch.randn(M, device="cuda:0", generator=gq)
+    done = (torch.rand(M, device="cuda:0", generator=gq) < 0.05).float()
+    td_opts = {"td3": dict(policy="deterministic", noise=0.2, noise_clip=0.5, seed=SEED),
+               "sac": dict(policy="gaussian", squash=True, seed=SEED, alpha=0.2)}
+
+    def td_fused(a, tag):
+        c, kw = critics[(a, 0)], dict(td_opts[tag])
+        if tag == "sac":
+            kw["log_std"] = actor_ls[a]
+        return mlp.mlp_forward(obs, c[0], c[2], c[4], biases=(c[1], c[3], c[5]), output="td_target",
+                               twin=critics[(a, 1)], actor=actors[a], reward=reward, done=done, gamma=0.99, **kw)
+
+    def td_two_call(a, tag):
+        """The actor entry, the twin critic entry, then the target in eager torch."""
+        ac, c, kw = actors[a], critics[(a, 0)], dict(td_opts[tag])
+        if tag == "td3":
+            kw.pop("policy")
+            act = mlp.mlp_forward(obs, ac[0], ac[2], ac[4], biases=(ac[1], ac[3], ac[5]), output="deterministic", **kw)
+        else:
+            act, logp = mlp.mlp_forward(obs, ac[0], ac[2], ac[4], biases=(ac[1], ac[3], ac[5]), output="gaussian",
+                                        seed=SEED, log_std=actor_ls[a], squash=True)
+        t = mlp.mlp_forward(obs, c[0], c[2], c[4], biases=(c[1], c[3], c[5]), output="critic", action=act,
+                            twin=critics[(a, 1)])[2]
+        if tag == "sac":
+            t = t - 0.2 * logp
+        return reward + 0.99 * (1 - done) * t
+
+    def td_eager(a, tag):
+        """Logits entries and torch: the actor's logits (over [w3; w_ls] for SAC), its head in torch, then the eager
+        twin of p over those actions and the target in torch."""
+        ac = actors[a]
+        z = normal_noise(SEED, 0, M, a, device="cuda:0")
+        if tag == "td3":
+            y = mlp.mlp_forward(obs, ac[0], ac[2], ac[4], biases=(ac[1], ac[3], ac[5])).float()
+            act = (y.tanh() + (0.2 * z).clamp(-0.5, 0.5)).clamp(-1.0, 1.0)
+        else:
+            y = mlp.mlp_forward(obs, ac[0], ac[2], torch.cat((ac[4], actor_ls[a][0])),
+                                biases=(ac[1], ac[3], torch.cat((ac[5], actor_ls[a][1])))).float()
+            mu, ls = y[:, :a], y[:, a:].clamp(-20.0, 2.0)
+            u = mu + torch.exp(ls) * z
+            au = u.abs()
+            logp = (-0.5 * z * z - ls - HALF_LOG_2PI).sum(-1) - (2 * (LN2 - au - torch.log1p(torch.exp(-2 * au)))).sum(-1)
+            act = torch.tanh(u)
+        x = torch.cat([obs, act.to(torch.bfloat16), obs.new_zeros(M, 64 - a)], -1)
+        qs = [mlp.mlp_forward(x, F.pad(critics[(a, i)][0], (0, 64 - a)), critics[(a, i)][2], critics[(a, i)][4],
+                              biases=critics[(a, i)][1::2]).float().squeeze(-1) for i in (0, 1)]
+        t = torch.minimum(qs[0], qs[1])
+        if tag == "sac":
+            t = t - 0.2 * logp
+        return reward + 0.99 * (1 - done) * t
+
+    for a in critic_widths:
+        for tag in td_opts:
+            variants[f"q_bias_{tag}_target_a{a}"] = (1, lambda a=a, tag=tag: td_fused(a, tag))
+            variants[f"q_bias_{tag}_two_call_a{a}"] = (1, lambda a=a, tag=tag: td_two_call(a, tag))
+            variants[f"q_bias_{tag}_eager_a{a}"] = (1, lambda a=a, tag=tag: td_eager(a, tag))
+    for a in critic_widths:   # parity before timing: the fused target equals the two-call arm bit for bit
+        for tag in td_opts:
+            got, two = td_fused(a, tag), td_two_call(a, tag)
+            assert torch.equal(got.view(torch.int32), two.view(torch.int32)), (tag, a)
+            eager = td_eager(a, tag)
+            close = torch.isclose(got, eager, rtol=2.0 ** -7, atol=1e-2)
+            assert float(close.float().mean()) > 0.99, (tag, a)
+            parity[f"q_bias_{tag}_a{a}"] = {"target_eq_two_call_all_rows": "ok",
+                                            "target_vs_eager_frac_close": round(float(close.float().mean()), 6),
+                                            "target_eq_eager_bits_frac": round(float(
+                                                (got.view(torch.int32) == eager.view(torch.int32)).float().mean()), 6)}
+            del got, two, eager
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
@@ -429,7 +511,7 @@ def main():
     a = variants["a_original_d64"][1]()
     b = variants["b_policy_nobias_d64"][1]()
     torch.cuda.synchronize(0)
-    parity = {"b_equals_a_bitwise": bool(torch.equal(a, b))}
+    parity["b_equals_a_bitwise"] = bool(torch.equal(a, b))
     idx = torch.randint(0, M, (2048,), device="cuda:0", generator=g)
     for name, d, bias in (("a_original_d64", 64, False), ("e_bias_both_d64", 64, True), ("f_bias_both_d18", 18, True),
                           ("f_bias_both_d256", 256, True)):
