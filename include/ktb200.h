@@ -241,13 +241,13 @@ int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elem
                                size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
                                const void* mask_root, size_t row_bytes, size_t mask_offset, unsigned long long seq,
                                uintptr_t stream);
-/* ktb_push_scatter_ce with n_sides (1 or 2) per-row side sources, for the masked and epsilon-greedy MLP heads (the
- * legal-action mask and the per-row epsilon): row i of obs has side_row_bytes[k] bytes at side_src[k] +
+/* ktb_push_scatter_ce with n_sides (1 or 2) per-row side sources, the side inputs of the push-fed MLP heads
+ * (ktb_mlp_bf16_pushed): row i of obs has side_row_bytes[k] bytes at side_src[k] +
  * i*side_row_bytes[k], copied chunk by chunk, after the same wait for ack[r] >= seq-2, to stage_peer[r] +
  * (seq&1)*stage_stride + side_offset[k] + (the chunk's first row in the shard)*side_row_bytes[k]; ready[c] is
  * published behind every copy of chunk c.  ktb_push_scatter_ce_masked is its one-side case.  After every check of
  * ktb_push_scatter_ce, in its order: n_sides outside [1, 2] or a NULL array; then per side in order a NULL source with
- * n_elems > 0, side_row_bytes == 0 or chunk_elems not a multiple of granule, and for a served rank a side that
+ * n_elems > 0, side_row_bytes == 0 or chunk_elems not a multiple of granule; then for each served rank a side that
  * overlaps its shard's rows, ends past stage_stride, or overlaps an earlier side, are KTB_ERR_ARG. */
 int ktb_push_scatter_ce_sides(int root_dev, const void* src_root, size_t n_elems, size_t granule, int dtype,
                               int n_ranks, int root_rank, const int* devs, void* const* stage_peer, size_t stage_stride,
@@ -321,7 +321,14 @@ int ktb_mlp_bf16_staged(int dev, const void* obs_peer, size_t M, int d_in, int d
  * 16-byte aligned) and stage_local, weights and scratch 16-byte aligned (KTB_ERR_ARG otherwise, before anything
  * is enqueued); d_out == 64 (KTB_ERR_UNSUPPORTED otherwise).  `scratch`
  * holds 2*min(chunk_rows, M)*d_hidden bf16: it follows this call's chunk_rows, not the chunk of
- * ktb_mlp_scratch_bytes. */
+ * ktb_mlp_scratch_bytes.
+ * Side inputs of the push-fed heads: a head's per-row inputs (its sides, up to two, named by each family below) are
+ * pushed beside the rows into the same staging half (ktb_push_scatter_ce_sides puts them there), and the rank reads
+ * them at stage_local + (seq & 1)*stage_stride + the side's offset argument, never from a peer.  Each side holds M rows
+ * of its bytes per row and needs its alignment; a side that starts inside the rows (offset < M*d_in*2), ends past
+ * stage_stride, starts at an offset that is not a multiple of its alignment, or overlaps an earlier side is
+ * KTB_ERR_ARG.  These checks come right after those of stage_stride, before every check of the head's own arguments, so
+ * a call with a bad side and another defect (say an unsupported d_out) may report the side's KTB_ERR_ARG first. */
 int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in, int d_hidden,
                         int d_out, const void* W1, const void* W2, const void* W3, void* logits, void* scratch,
                         void* ctrl_local, void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
@@ -444,10 +451,8 @@ int ktb_mlp_bf16_policy_sample_masked(int dev, const void* obs, size_t M, int d_
                                       const void* b3, const uint8_t* mask, uint64_t seed, uint64_t row_base,
                                       int64_t* actions, float* log_probs, void* scratch, void* stage,
                                       uintptr_t stream);
-/* Push-fed masked forms: the _pushed entries' arguments with mask_offset after b3.  The rank's mask rows are read
- * from its own staging half, at stage_local + (seq & 1)*stage_stride + mask_offset (ktb_push_scatter_ce_masked puts
- * them there), never from a peer.  mask_offset < M*d_in*2 (overlapping the rows) or mask_offset + M*d_out >
- * stage_stride is KTB_ERR_ARG, checked after every check of the unmasked pushed entry. */
+/* Push-fed masked forms: the _pushed entries' arguments with mask_offset after b3, the offset of their one side
+ * (ktb_mlp_bf16_pushed): the mask, d_out bytes per row, any alignment. */
 int ktb_mlp_bf16_policy_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
                                       int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
                                       const void* b2, const void* W3, const void* b3, size_t mask_offset, void* logits,
@@ -698,11 +703,9 @@ int ktb_mlp_bf16_policy_epsilon_greedy_masked(int dev, const void* obs, size_t M
                                               int64_t* actions, float* q, float* q_max, void* scratch, void* stage,
                                               uintptr_t stream);
 /* Push-fed epsilon-greedy forms: the _pushed entries' arguments with (mask_offset,) epsilon_offset after b3 in place of
- * the pointers.  The rank reads its rows' epsilon (fp32, M*4 bytes) and mask from its own staging half, at
- * stage_local + (seq & 1)*stage_stride + the offset (ktb_push_scatter_ce_sides puts them there), never from a peer.
- * After the counterpart's checks: an epsilon region that overlaps the rows (epsilon_offset < M*d_in*2) or the mask
- * region, that ends past stage_stride, or whose offset is not a multiple of 4, is KTB_ERR_ARG; then the output checks
- * above.  An empty shard (M == 0) may pass NULL outputs and still publishes its ack. */
+ * the pointers, the offsets of their sides (ktb_mlp_bf16_pushed): the mask (masked form; d_out bytes per row, any
+ * alignment), then epsilon (fp32, 4 bytes per row, 4-byte aligned).  An empty shard (M == 0) may pass NULL outputs and
+ * still publishes its ack. */
 int ktb_mlp_bf16_policy_epsilon_greedy_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
                                               int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
                                               const void* b2, const void* W3, const void* b3, size_t epsilon_offset,
@@ -787,11 +790,9 @@ int ktb_mlp_bf16_policy_gaussian_evaluate_value(int dev, const void* obs, size_t
                                                 const float* taken, float* log_probs, float* entropy, float* values,
                                                 void* scratch, void* stage, uintptr_t stream);
 /* Push-fed evaluating forms: the _pushed entries' arguments with the evaluating arguments above after b3 (b3v), and
- * (mask_offset,) taken_offset in place of the pointers.  The rank reads its rows' actions (M*8*max(n_groups, 1) bytes
- * categorical, M*4*d_out Gaussian) and mask from its own staging half, at stage_local + (seq & 1)*stage_stride + the
- * offset (ktb_push_scatter_ce_sides puts them there), never from a peer.  After the checks above: a taken region that
- * overlaps the rows (taken_offset < M*d_in*2) or the mask region, that ends past stage_stride, or whose offset is not a
- * multiple of 8 (categorical) or 4 (Gaussian), is KTB_ERR_ARG.  An empty shard (M == 0) may pass NULL outputs and a
+ * (mask_offset,) taken_offset in place of the pointers, the offsets of their sides (ktb_mlp_bf16_pushed): the mask
+ * (masked forms; d_out bytes per row, any alignment), then taken (8*max(n_groups, 1) bytes per row, 8-byte aligned,
+ * categorical; 4*d_out bytes per row, 4-byte aligned, Gaussian).  An empty shard (M == 0) may pass NULL outputs and a
  * NULL nvec and still publishes its ack. */
 int ktb_mlp_bf16_policy_evaluate_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
                                         int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
@@ -892,13 +893,12 @@ int ktb_mlp_bf16_policy_deterministic_pushed(int dev, const void* stage_local, s
  *     adds to it as +0, so no signed-zero tie of q1 and q2 arises from the kernel.  The action tile is packed once
  *     per chunk for both.
  *   - scratch holds ktb_mlp_critic_scratch_bytes(M, d_hidden): the two hidden activations and the action tile.
- *   - act and the outputs may be peer pointers.  The pushed forms read the actions from their staging half (pushed
- *     there beside the rows by ktb_push_scatter_ce_sides), act_offset bytes in.
+ *   - act and the outputs may be peer pointers.  The pushed forms read the actions from their one side
+ *     (ktb_mlp_bf16_pushed), act: 4*d_act bytes per row, 4-byte aligned, act_offset bytes into the staging half.
  *   - Checks: every check ktb_mlp_bf16_policy runs first, at d_out = 1 (a twin's second weights and biases as the
  *     first's, right after them); then d_act < 1 is KTB_ERR_ARG and d_act > 64 KTB_ERR_UNSUPPORTED; then, with M > 0, a
- *     NULL or not 4-byte aligned act, q, q1, q2 or q_min is KTB_ERR_ARG; then, in the pushed forms, an action region
- *     that overlaps the rows, ends past stage_stride or is not 4-byte aligned is KTB_ERR_ARG.  An empty pushed shard
- *     (M == 0) may pass NULL outputs and still publishes its ack.  Writes stay inside the outputs, scratch and stage. */
+ *     NULL or not 4-byte aligned act, q, q1, q2 or q_min is KTB_ERR_ARG.  An empty pushed shard (M == 0) may pass NULL
+ *     outputs and still publishes its ack.  Writes stay inside the outputs, scratch and stage. */
 size_t ktb_mlp_critic_scratch_bytes(size_t M, int d_hidden);
 int ktb_mlp_bf16_critic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act, const void* W1p,
                         const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
@@ -948,10 +948,9 @@ int ktb_mlp_bf16_critic_twin_pushed(int dev, const void* stage_local, size_t sta
  *     every check of the actor's standalone entry at d_out = d_act and d_hidden_actor, its noise and noise_clip or its
  *     log_std bounds included (the actor and the critics share d_in and d_act, one argument each); then a non-finite
  *     gamma or alpha is KTB_ERR_ARG; then, with M > 0, a NULL or not 4-byte aligned reward, done (pull forms) or y is
- *     KTB_ERR_ARG; then, in the pushed forms, a reward or done region that overlaps the rows, ends past stage_stride
- *     or is not 4-byte aligned, or the two regions overlapping, is KTB_ERR_ARG.  An empty pushed shard (M == 0) may
- *     pass NULL outputs and still publishes its ack.  The pushed forms read the rows, reward and done from their
- *     staging half (ktb_push_scatter_ce_sides with two sides).  Writes stay inside y, scratch and stage. */
+ *     KTB_ERR_ARG.  An empty pushed shard (M == 0) may pass NULL outputs and still publishes its ack.  The pushed forms
+ *     read reward and done from their two sides (ktb_mlp_bf16_pushed): reward, then done, each fp32, 4 bytes per row,
+ *     4-byte aligned.  Writes stay inside y, scratch and stage. */
 size_t ktb_mlp_td_target_scratch_bytes(size_t M, int d_hidden_actor, int d_hidden, int d_act);
 int ktb_mlp_bf16_td_target_deterministic(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_act,
                                          const void* W1p, const void* b1, const void* W2, const void* b2,

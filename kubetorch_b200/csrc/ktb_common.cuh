@@ -437,6 +437,36 @@ __device__ __forceinline__ bool spin_until(const unsigned long long* flag, unsig
 #define KTB_CTRL_CHUNK_DONE 2048
 #define KTB_PUSH_MAX_CHUNKS 64
 
+// A per-row input pushed with the rows into a rank's staging half (the MLP heads' side inputs): row i of a shard has
+// row_bytes bytes at `offset + i·row_bytes` of the half, and on the root at `src + i·row_bytes` (null on the ranks).
+// `name` names it in the errors.
+struct PushSide {
+  const void* src;
+  size_t row_bytes, offset, align;
+  const char* name;
+};
+
+// The side regions of a staging half that holds `rows` rows of `row_bytes` bytes and is `stride` bytes long
+// (KTB_ERR_ARG naming `who` otherwise): each starts at or past the rows, ends within the stride, starts at a multiple
+// of its alignment and overlaps no earlier region.
+inline int check_push_sides(const char* who, const PushSide* sides, int n_sides, size_t rows, size_t row_bytes,
+                            size_t stride) {
+  for (int k = 0; k < n_sides; ++k) {
+    const PushSide& sd = sides[k];
+    const size_t n = rows * sd.row_bytes;
+    KTB_REQUIRE(sd.offset >= rows * row_bytes, KTB_ERR_ARG, "%s: %s offset %zu overlaps the rows", who, sd.name,
+                sd.offset);
+    KTB_REQUIRE(sd.offset <= stride && n <= stride - sd.offset, KTB_ERR_ARG,
+                "%s: %s offset %zu + %zu exceeds stage_stride", who, sd.name, sd.offset, n);
+    KTB_REQUIRE(sd.offset % sd.align == 0, KTB_ERR_ARG, "%s: %s offset %zu must be a multiple of %zu", who, sd.name,
+                sd.offset, sd.align);
+    for (int o = 0; o < k; ++o)
+      KTB_REQUIRE(sd.offset >= sides[o].offset + rows * sides[o].row_bytes || sd.offset + n <= sides[o].offset,
+                  KTB_ERR_ARG, "%s: %s overlaps %s", who, sd.name, sides[o].name);
+  }
+  return KTB_OK;
+}
+
 
 // ---- kernel-launch entry points shared between translation units --------------------------------
 // (ktb_map.cu) enqueue dst = op(src) on the current device.

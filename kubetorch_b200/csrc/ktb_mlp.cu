@@ -1483,27 +1483,25 @@ static int launch_action_tile(const float* act, int d_act, void* tile, size_t ro
   return KTB_OK;
 }
 
-// Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged
-// and _pushed: no biases and a 64-wide greedy head that stores logits only.  `masked` marks the _masked entries: the
-// head applies a legal-action mask, out.mask in the pull forms and the bytes at MlpFeed::mask_offset of the call's
-// staging half in the pushed forms.  `valued` marks the _value entries: W3 / b3 are the stacked W3v [d_out + 1,
-// d_hidden] / b3v [d_out + 1] of the policy and its value head, and out.values receives the value of each row.
-// `nvec` (n_groups entries, a host array) marks the _multidiscrete entries: mlp_run checks it and builds out.groups.
-// std.state marks the _gaussian_state entries: W3 / b3 are the interleaved W3s [2·d_out, d_hidden] / b3s (with a
-// value head W3sv / b3sv, one more row), log_std is null, and mlp_run checks the bounds.  `eps` marks the
-// _epsilon_greedy entries: eg.epsilon (the pull forms) or the bytes at MlpFeed::epsilon_offset of the call's staging
-// half (the pushed forms) hold each row's ε, and out.actions, eg.q and eg.q_max receive the outputs.  `evaluate` marks
-// the _evaluate entries: ev.actions (kSample) or ev.gauss_actions (kGaussian), or in the pushed forms the bytes at
-// MlpFeed::taken_offset of the call's staging half, hold the given actions, and out.log_probs and ev.entropy receive
-// the outputs; a categorical one is grouped unless nvec == null and n_groups == 0.  std.det marks the _deterministic
-// entries: out.gauss_actions receives the actions, and mlp_run checks σ and the clip.  `critic` marks the _critic
-// entries: W1 is W1p [d_hidden, d_in + 64], layer 1 reads an action tile packed from `act` (fp32 [M, d_act]; in the
-// pushed forms the bytes at MlpFeed::act_offset of the call's staging half) as its last K block, W3 / b3 are the
-// critic's [1, d_hidden] / [1], and hq receives Q; `twin` (the _twin entries) is the second critic, run on the same
-// tile after the first, whose hq also reads the first's q and stores q_min.  `actor` marks the _td_target entries: the
-// critics' action tile is packed from the actions the actor (a deterministic or state-dependent Gaussian head,
-// `actor_hidden` wide) writes into chunk scratch, and the last critic's hq computes the target (`target` marks both
-// critics: their hq reads and writes chunk scratch).
+// Weights and biases (each bias may be null) of one MLP call, and its head.  `logits64` marks ktb_mlp_bf16, _staged and
+// _pushed: no biases and a 64-wide greedy head that stores logits only.  `masked` marks the _masked entries: the head
+// applies a legal-action mask, out.mask in the pull forms and the call's "mask" side (MlpFeed) in the pushed forms.
+// `valued` marks the _value entries: W3 / b3 are the stacked W3v [d_out + 1, d_hidden] / b3v [d_out + 1] of the policy
+// and its value head, and out.values receives the value of each row. `nvec` (n_groups entries, a host array) marks the
+// _multidiscrete entries: mlp_run checks it and builds out.groups. std.state marks the _gaussian_state entries: W3 / b3
+// are the interleaved W3s [2·d_out, d_hidden] / b3s (with a value head W3sv / b3sv, one more row), log_std is null, and
+// mlp_run checks the bounds.  `eps` marks the _epsilon_greedy entries: eg.epsilon (the pull forms) or the call's
+// "epsilon" side (the pushed forms) hold each row's ε, and out.actions, eg.q and eg.q_max receive the outputs.
+// `evaluate` marks the _evaluate entries: ev.actions (kSample) or ev.gauss_actions (kGaussian), or in the pushed forms
+// the call's "taken" side, hold the given actions, and out.log_probs and ev.entropy receive the outputs; a categorical
+// one is grouped unless nvec == null and n_groups == 0.  std.det marks the _deterministic entries: out.gauss_actions
+// receives the actions, and mlp_run checks σ and the clip.  `critic` marks the _critic entries: W1 is W1p [d_hidden,
+// d_in + 64], layer 1 reads an action tile packed from `act` (fp32 [M, d_act]; in the pushed forms the call's "act"
+// side) as its last K block, W3 / b3 are the critic's [1, d_hidden] / [1], and hq receives Q; `twin` (the _twin
+// entries) is the second critic, run on the same tile after the first, whose hq also reads the first's q and stores
+// q_min.  `actor` marks the _td_target entries: the critics' action tile is packed from the actions the actor (a
+// deterministic or state-dependent Gaussian head, `actor_hidden` wide) writes into chunk scratch, and the last critic's
+// hq computes the target (`target` marks both critics: their hq reads and writes chunk scratch).
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1703,11 +1701,11 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //           stage stream while the previous chunk computes, and layer 1 reads it there.
 //   pushed: the root pushes the rows into half seq & 1 of `in` (stage_local, halves `stride` bytes apart) and publishes
 //           ready[c] = seq in this rank's control block `ctrl`; layer 1 of chunk c waits in-stream for it, and the
-//           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A masked head reads
-//           the rows' legal-action mask from the same half, mask_offset bytes in (pushed there beside the rows), and
-//           an ε-greedy head its rows' ε (fp32) from epsilon_offset bytes in, an evaluating head its rows' given
-//           actions from taken_offset bytes in, a critic its rows' actions (fp32) from act_offset bytes in, and a
-//           TD target its rows' reward and done (fp32) from reward_offset and done_offset bytes in.
+//           call ends by publishing ack[rank] = seq in the root's control block `ctrl_root`.  A head's per-row
+//           inputs were pushed into the same half beside the rows: `sides`, up to two regions (PushSide, src null)
+//           named for what they hold, "mask" (a masked head's legal-action mask), "epsilon" (an ε-greedy head's ε,
+//           fp32), "taken" (an evaluating head's given actions), "act" (a critic's actions, fp32), or "reward" and
+//           "done" (a TD target's, fp32).
 // The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
@@ -1718,42 +1716,25 @@ struct MlpFeed {
   void *ctrl = nullptr, *ctrl_root = nullptr;
   int rank = 0;
   unsigned long long seq = 0;
-  size_t mask_offset = 0;
-  size_t epsilon_offset = 0;
-  size_t taken_offset = 0;
-  size_t act_offset = 0;
-  size_t reward_offset = 0, done_offset = 0;
+  PushSide sides[2] = {};
+  int n_sides = 0;
 
   static MlpFeed pull(const void* obs, void* stage) { return {obs, (size_t)g_mlp_chunk_rows, stage}; }
   static MlpFeed push(const void* stage_local, size_t stride, void* ctrl, void* ctrl_root, int rank, size_t chunk_rows,
                       unsigned long long seq) {
     return {stage_local, chunk_rows, nullptr, true, stride, ctrl, ctrl_root, rank, seq};
   }
-  MlpFeed with_mask_offset(size_t off) const {
+  // the feed with one more side region: `name`, `offset` bytes into the half, row_bytes per row, `align`-aligned
+  MlpFeed with_side(const char* name, size_t offset, size_t row_bytes, size_t align) const {
     MlpFeed f = *this;
-    f.mask_offset = off;
+    f.sides[f.n_sides++] = PushSide{nullptr, row_bytes, offset, align, name};
     return f;
   }
-  MlpFeed with_epsilon_offset(size_t off) const {
-    MlpFeed f = *this;
-    f.epsilon_offset = off;
-    return f;
-  }
-  MlpFeed with_taken_offset(size_t off) const {
-    MlpFeed f = *this;
-    f.taken_offset = off;
-    return f;
-  }
-  MlpFeed with_act_offset(size_t off) const {
-    MlpFeed f = *this;
-    f.act_offset = off;
-    return f;
-  }
-  MlpFeed with_target_offsets(size_t reward, size_t done) const {
-    MlpFeed f = *this;
-    f.reward_offset = reward;
-    f.done_offset = done;
-    return f;
+  // the side named `name` in staging half `half`
+  const void* side(const uint8_t* half, const char* name) const {
+    for (int k = 0; k < n_sides; ++k)
+      if (strcmp(sides[k].name, name) == 0) return half + sides[k].offset;
+    return nullptr;
   }
 };
 
@@ -1803,24 +1784,23 @@ static int head_checks(const char* fn, size_t M, int d_out, const MlpParams& p) 
 
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
 // right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
-// ktb_push_wait waits for.  A masked entry's own checks (a mask in the pull forms, mask_offset inside the staging half
-// and past the rows in the pushed forms) come after every check of the unmasked entry, and a value entry's (values,
-// d_out <= 255; skipped for an empty call) after every check of the entry without a value head.  A multi-discrete
-// entry's nvec (skipped for an empty call) is checked last, and read into the launch's HeadGroups before the call
-// returns.  A state-dependent Gaussian entry's head width (2·d_out, one more with a value head, <= 256) and log-std
-// bounds (skipped for an empty call) come after every check of its state-independent counterpart.  An ε-greedy entry's
-// own checks come after every check of its greedy counterpart (ktb_mlp_bf16_policy or _masked): its ε region in the
-// pushed forms, then (skipped for an empty call) ε, actions, q and q_max non-null and aligned.  An evaluating entry's
-// own checks come after every check of its counterpart and its nvec: (skipped for an empty call) taken, log_probs,
-// entropy non-null and aligned, then its taken region in the pushed forms.  A deterministic entry's actions are checked
-// with the head (mlp_check), its noise and noise_clip (>= 0, not NaN; skipped for an empty call) after every check.
-// A critic entry runs every check of ktb_mlp_bf16_policy at d_out = 1 (a twin's second critic's weights and biases
-// checked as the first's, right after them), then d_act in [1, 64], then (skipped for an empty call) act and its
-// outputs non-null and 4-byte aligned, then its action region in the pushed forms.  A TD target entry runs every check
-// of the critic (twin) entry but those of act and the Q outputs, then every check of its actor's standalone entry
-// (ktb_mlp_bf16_policy_deterministic or _gaussian_state at d_out = d_act, the actor's d_hidden), then gamma and alpha
-// finite, then (skipped for an empty call) reward, done and y non-null and aligned, then its reward and done regions
-// in the pushed forms.
+// ktb_push_wait waits for.  A pushed entry's side regions (check_push_sides) are checked right after its stage_stride,
+// before every check of the head's own arguments, so a call with a bad region and another defect may report the
+// region's KTB_ERR_ARG first.  A masked entry's own checks (a mask in the pull forms) come after every check of the
+// unmasked entry, and a value entry's (values, d_out <= 255; skipped for an empty call) after every check of the entry
+// without a value head.  A multi-discrete entry's nvec (skipped for an empty call) is checked last, and read into the
+// launch's HeadGroups before the call returns.  A state-dependent Gaussian entry's head width (2·d_out, one more with a
+// value head, <= 256) and log-std bounds (skipped for an empty call) come after every check of its state-independent
+// counterpart.  An ε-greedy entry's own checks come after every check of its greedy counterpart (ktb_mlp_bf16_policy or
+// _masked): (skipped for an empty call) ε, actions, q and q_max non-null and aligned.  An evaluating entry's own checks
+// come after every check of its counterpart and its nvec: (skipped for an empty call) taken, log_probs, entropy
+// non-null and aligned.  A deterministic entry's actions are checked with the head (mlp_check), its noise and
+// noise_clip (>= 0, not NaN; skipped for an empty call) after every check.  A critic entry runs every check of
+// ktb_mlp_bf16_policy at d_out = 1 (a twin's second critic's weights and biases checked as the first's, right after
+// them), then d_act in [1, 64], then (skipped for an empty call) act and its outputs non-null and 4-byte aligned.  A TD
+// target entry runs every check of the critic (twin) entry but those of act and the Q outputs, then every check of its
+// actor's standalone entry (ktb_mlp_bf16_policy_deterministic or _gaussian_state at d_out = d_act, the actor's
+// d_hidden), then gamma and alpha finite, then (skipped for an empty call) reward, done and y non-null and aligned.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1857,24 +1837,11 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     KTB_REQUIRE(M * (size_t)d_in * 2 <= f.stride, KTB_ERR_ARG, "%s: shard exceeds stage_stride", fn);
     // layer 1 reads half seq & 1 through a tensor map, whose base TMA needs 16-byte aligned
     KTB_REQUIRE(f.stride % 16 == 0, KTB_ERR_ARG, "%s: stage_stride=%zu must be a multiple of 16", fn, f.stride);
+    rc = check_push_sides(fn, f.sides, f.n_sides, M, (size_t)d_in * 2, f.stride);
+    if (rc) return rc;
   }
-  if (p.masked && f.pushed) {
-    KTB_REQUIRE(f.mask_offset >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: mask_offset=%zu overlaps the rows", fn,
-                f.mask_offset);
-    KTB_REQUIRE(f.mask_offset <= f.stride && M * (size_t)d_out <= f.stride - f.mask_offset, KTB_ERR_ARG,
-                "%s: mask_offset=%zu + M*d_out exceeds stage_stride", fn, f.mask_offset);
-  } else if (p.masked) {
+  if (p.masked && !f.pushed)
     KTB_REQUIRE(p.out.mask, KTB_ERR_ARG, "%s: null mask", fn);   // M > 0 here: an empty pull call has returned
-  }
-  if (p.eps && f.pushed) {
-    const size_t off = f.epsilon_offset, n = M * sizeof(float);
-    KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: epsilon_offset=%zu overlaps the rows", fn, off);
-    KTB_REQUIRE(!p.masked || off >= f.mask_offset + M * (size_t)d_out || off + n <= f.mask_offset, KTB_ERR_ARG,
-                "%s: epsilon_offset=%zu overlaps the mask", fn, off);
-    KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG,
-                "%s: epsilon_offset=%zu + 4*M exceeds stage_stride", fn, off);
-    KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: epsilon_offset=%zu must be a multiple of 4", fn, off);
-  }
   if (p.eps && M > 0) {
     const HeadEps& o = p.eg;
     KTB_REQUIRE((o.epsilon || f.pushed) && p.out.actions && o.q && o.q_max, KTB_ERR_ARG,
@@ -1894,13 +1861,6 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
                   p.twin ? "%s: act, q1, q2 and q_min are required" : "%s: act and q are required", fn);
       KTB_REQUIRE((((uintptr_t)p.act | (uintptr_t)p.hq.q | (uintptr_t)q2.q | (uintptr_t)q2.q_min) & 3) == 0,
                   KTB_ERR_ARG, "%s: act and the outputs must be 4-byte aligned", fn);
-    }
-    if (f.pushed && !p.actor) {
-      const size_t off = f.act_offset, n = M * (size_t)p.d_act * 4;
-      KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: act_offset=%zu overlaps the rows", fn, off);
-      KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG, "%s: act_offset=%zu + act exceeds stage_stride",
-                  fn, off);
-      KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: act_offset=%zu must be a multiple of 4", fn, off);
     }
   }
   const size_t chunk = std::min(f.chunk_rows, M);
@@ -1931,20 +1891,6 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       KTB_REQUIRE((((uintptr_t)t.reward | (uintptr_t)t.done | (uintptr_t)t.y) & 3) == 0, KTB_ERR_ARG,
                   "%s: reward, done and y must be 4-byte aligned", fn);
     }
-    if (f.pushed) {
-      const size_t n = M * sizeof(float);
-      for (const size_t off : {f.reward_offset, f.done_offset}) {
-        KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: reward/done offset %zu overlaps the rows", fn, off);
-        KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG,
-                    "%s: reward/done offset %zu + 4*M exceeds stage_stride", fn, off);
-        KTB_REQUIRE(off % 4 == 0, KTB_ERR_ARG, "%s: reward/done offset %zu must be a multiple of 4", fn, off);
-      }
-      KTB_REQUIRE(f.reward_offset + n <= f.done_offset || f.done_offset + n <= f.reward_offset, KTB_ERR_ARG,
-                  "%s: the reward and done regions overlap", fn);
-      const uint8_t* half = static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride;
-      t.reward = reinterpret_cast<const float*>(half + f.reward_offset);
-      t.done = reinterpret_cast<const float*>(half + f.done_offset);
-    }
     if (actor.std.state) t.logp = s.logp;
   }
   HeadGroups groups = p.out.groups;
@@ -1972,41 +1918,31 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       KTB_REQUIRE((((uintptr_t)p.out.log_probs | (uintptr_t)p.ev.entropy) & 3) == 0, KTB_ERR_ARG,
                   "%s: log_probs and entropy must be 4-byte aligned", fn);
     }
-    if (f.pushed) {
-      const size_t off = f.taken_offset;
-      const size_t n = M * (cat ? 8 * (size_t)std::max(groups.n, 1) : 4 * (size_t)d_out);
-      KTB_REQUIRE(off >= M * (size_t)d_in * 2, KTB_ERR_ARG, "%s: taken_offset=%zu overlaps the rows", fn, off);
-      KTB_REQUIRE(!p.masked || off >= f.mask_offset + M * (size_t)d_out || off + n <= f.mask_offset, KTB_ERR_ARG,
-                  "%s: taken_offset=%zu overlaps the mask", fn, off);
-      KTB_REQUIRE(off <= f.stride && n <= f.stride - off, KTB_ERR_ARG, "%s: taken_offset=%zu + taken exceeds stage_stride",
-                  fn, off);
-      KTB_REQUIRE(off % align == 0, KTB_ERR_ARG, "%s: taken_offset=%zu must be a multiple of %zu", fn, off, align);
-    }
   }
   rc = get_encoder();
   if (rc) return rc;
   KTB_GUARD(dev);
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   // the call's rows: obs, or this call's staging half (the pull forms have seq = stride = 0)
-  const __nv_bfloat16* x =
-      reinterpret_cast<const __nv_bfloat16*>(static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride);
+  const uint8_t* half = static_cast<const uint8_t*>(f.in) + (size_t)(f.seq & 1) * f.stride;
+  const __nv_bfloat16* x = reinterpret_cast<const __nv_bfloat16*>(half);
   HeadOut out = p.out;
   out.groups = groups;
-  if (p.masked && f.pushed) out.mask = reinterpret_cast<const uint8_t*>(x) + f.mask_offset;
   HeadEps eg = p.eg;
-  if (p.eps && f.pushed)
-    eg.epsilon = reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(x) + f.epsilon_offset);
   HeadEval ev = p.ev;
-  if (p.evaluate && f.pushed) {
-    const uint8_t* t = reinterpret_cast<const uint8_t*>(x) + f.taken_offset;
-    if (p.kind == HeadKind::kSample)
-      ev.actions = reinterpret_cast<const int64_t*>(t);
-    else
-      ev.gauss_actions = reinterpret_cast<const float*>(t);
+  const float* act = p.act;
+  if (f.pushed) {   // the head's per-row inputs, pushed into the same half
+    if (p.masked) out.mask = static_cast<const uint8_t*>(f.side(half, "mask"));
+    if (p.eps) eg.epsilon = static_cast<const float*>(f.side(half, "epsilon"));
+    if (p.evaluate && p.kind == HeadKind::kSample) ev.actions = static_cast<const int64_t*>(f.side(half, "taken"));
+    if (p.evaluate && p.kind != HeadKind::kSample) ev.gauss_actions = static_cast<const float*>(f.side(half, "taken"));
+    if (p.critic && !p.actor) act = static_cast<const float*>(f.side(half, "act"));
+    if (p.actor) {
+      HeadQ& t = (p.twin ? c2 : c1).hq;
+      t.reward = static_cast<const float*>(f.side(half, "reward"));
+      t.done = static_cast<const float*>(f.side(half, "done"));
+    }
   }
-  const float* act = p.critic && f.pushed
-                         ? reinterpret_cast<const float*>(reinterpret_cast<const uint8_t*>(x) + f.act_offset)
-                         : p.act;
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
   cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
@@ -2157,7 +2093,7 @@ int ktb_mlp_bf16_policy_masked_pushed(int dev, const void* stage_local, size_t s
   const MlpParams p = MlpParams{W1, b1, W2, b2, W3, b3, HeadKind::kGreedy, {logits, actions}}.with_mask(nullptr);
   return mlp_run("ktb_mlp_bf16_policy_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset),
+                     .with_side("mask", mask_offset, d_out, 1),
                  scratch, stream);
 }
 
@@ -2203,7 +2139,7 @@ int ktb_mlp_bf16_policy_sample_masked_pushed(int dev, const void* stage_local, s
                           .with_mask(nullptr);
   return mlp_run("ktb_mlp_bf16_policy_sample_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset),
+                     .with_side("mask", mask_offset, d_out, 1),
                  scratch, stream);
 }
 
@@ -2277,7 +2213,7 @@ int ktb_mlp_bf16_policy_sample_masked_value_pushed(int dev, const void* stage_lo
                           .with_values(values);
   return mlp_run("ktb_mlp_bf16_policy_sample_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset),
+                     .with_side("mask", mask_offset, d_out, 1),
                  scratch, stream);
 }
 
@@ -2404,7 +2340,7 @@ int ktb_mlp_bf16_policy_multidiscrete_masked_pushed(int dev, const void* stage_l
       MlpParams::multidiscrete(W1, b1, W2, b2, W3, b3, nvec, n_groups, {logits, actions}, true).with_mask(nullptr);
   return mlp_run("ktb_mlp_bf16_policy_multidiscrete_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset),
+                     .with_side("mask", mask_offset, d_out, 1),
                  scratch, stream);
 }
 
@@ -2460,7 +2396,7 @@ int ktb_mlp_bf16_policy_sample_multidiscrete_masked_pushed(int dev, const void* 
                           .with_mask(nullptr);
   return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset),
+                     .with_side("mask", mask_offset, d_out, 1),
                  scratch, stream);
 }
 
@@ -2521,7 +2457,7 @@ int ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed(
                           .with_values(values);
   return mlp_run("ktb_mlp_bf16_policy_sample_multidiscrete_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset),
+                     .with_side("mask", mask_offset, d_out, 1),
                  scratch, stream);
 }
 
@@ -2544,7 +2480,7 @@ int ktb_mlp_bf16_policy_epsilon_greedy_pushed(int dev, const void* stage_local, 
   const MlpParams p = MlpParams::epsilon_greedy(W1, b1, W2, b2, W3, b3, nullptr, seed, row_base, actions, q, q_max);
   return mlp_run("ktb_mlp_bf16_policy_epsilon_greedy_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_epsilon_offset(epsilon_offset),
+                     .with_side("epsilon", epsilon_offset, 4, 4),
                  scratch, stream);
 }
 
@@ -2571,8 +2507,8 @@ int ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed(int dev, const void* stage_
       MlpParams::epsilon_greedy(W1, b1, W2, b2, W3, b3, nullptr, seed, row_base, actions, q, q_max).with_mask(nullptr);
   return mlp_run("ktb_mlp_bf16_policy_epsilon_greedy_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset)
-                     .with_epsilon_offset(epsilon_offset),
+                     .with_side("mask", mask_offset, d_out, 1)
+                     .with_side("epsilon", epsilon_offset, 4, 4),
                  scratch, stream);
 }
 
@@ -2596,7 +2532,7 @@ int ktb_mlp_bf16_policy_evaluate_pushed(int dev, const void* stage_local, size_t
       MlpParams::evaluate_categorical(W1, b1, W2, b2, W3, b3, nvec, n_groups, nullptr, log_probs, entropy);
   return mlp_run("ktb_mlp_bf16_policy_evaluate_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_taken_offset(taken_offset),
+                     .with_side("taken", taken_offset, 8 * (size_t)std::max(n_groups, 1), 8),
                  scratch, stream);
 }
 
@@ -2624,7 +2560,7 @@ int ktb_mlp_bf16_policy_evaluate_value_pushed(int dev, const void* stage_local, 
                           .with_values(values);
   return mlp_run("ktb_mlp_bf16_policy_evaluate_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_taken_offset(taken_offset),
+                     .with_side("taken", taken_offset, 8 * (size_t)std::max(n_groups, 1), 8),
                  scratch, stream);
 }
 
@@ -2651,8 +2587,8 @@ int ktb_mlp_bf16_policy_evaluate_masked_pushed(int dev, const void* stage_local,
                           .with_mask(nullptr);
   return mlp_run("ktb_mlp_bf16_policy_evaluate_masked_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset)
-                     .with_taken_offset(taken_offset),
+                     .with_side("mask", mask_offset, d_out, 1)
+                     .with_side("taken", taken_offset, 8 * (size_t)std::max(n_groups, 1), 8),
                  scratch, stream);
 }
 
@@ -2684,8 +2620,8 @@ int ktb_mlp_bf16_policy_evaluate_masked_value_pushed(int dev, const void* stage_
                           .with_values(values);
   return mlp_run("ktb_mlp_bf16_policy_evaluate_masked_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_mask_offset(mask_offset)
-                     .with_taken_offset(taken_offset),
+                     .with_side("mask", mask_offset, d_out, 1)
+                     .with_side("taken", taken_offset, 8 * (size_t)std::max(n_groups, 1), 8),
                  scratch, stream);
 }
 
@@ -2709,7 +2645,7 @@ int ktb_mlp_bf16_policy_gaussian_evaluate_pushed(int dev, const void* stage_loca
   const MlpParams p = MlpParams::evaluate_gaussian(W1, b1, W2, b2, W3, b3, log_std, nullptr, log_probs, entropy);
   return mlp_run("ktb_mlp_bf16_policy_gaussian_evaluate_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_taken_offset(taken_offset),
+                     .with_side("taken", taken_offset, 4 * (size_t)d_out, 4),
                  scratch, stream);
 }
 
@@ -2735,7 +2671,7 @@ int ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed(int dev, const void* stag
                           .with_values(values);
   return mlp_run("ktb_mlp_bf16_policy_gaussian_evaluate_value_pushed", dev, M, d_in, d_hidden, d_out, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_taken_offset(taken_offset),
+                     .with_side("taken", taken_offset, 4 * (size_t)d_out, 4),
                  scratch, stream);
 }
 
@@ -2777,7 +2713,7 @@ int ktb_mlp_bf16_critic_pushed(int dev, const void* stage_local, size_t stage_st
   const MlpParams p = MlpParams::critic_head(W1p, b1, W2, b2, W3, b3, d_act, nullptr, q);
   return mlp_run("ktb_mlp_bf16_critic_pushed", dev, M, d_in, d_hidden, 1, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_act_offset(act_offset),
+                     .with_side("act", act_offset, 4 * (size_t)d_act, 4),
                  scratch, stream);
 }
 
@@ -2809,7 +2745,7 @@ int ktb_mlp_bf16_critic_twin_pushed(int dev, const void* stage_local, size_t sta
   p.twin = &second;
   return mlp_run("ktb_mlp_bf16_critic_twin_pushed", dev, M, d_in, d_hidden, 1, p,
                  MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                     .with_act_offset(act_offset),
+                     .with_side("act", act_offset, 4 * (size_t)d_act, 4),
                  scratch, stream);
 }
 
@@ -2878,7 +2814,7 @@ int ktb_mlp_bf16_td_target_deterministic_pushed(
                        {W1p, b1, W2, b2, W3, b3, W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2}, d_hidden_actor, a, nullptr,
                        nullptr, gamma, 0.f, y,
                        MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                           .with_target_offsets(reward_offset, done_offset),
+                           .with_side("reward", reward_offset, 4, 4).with_side("done", done_offset, 4, 4),
                        scratch, stream);
 }
 
@@ -2912,7 +2848,7 @@ int ktb_mlp_bf16_td_target_gaussian_pushed(
                        {W1p, b1, W2, b2, W3, b3, W1p_2, b1_2, W2_2, b2_2, W3_2, b3_2}, d_hidden_actor, a, nullptr,
                        nullptr, gamma, alpha, y,
                        MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
-                           .with_target_offsets(reward_offset, done_offset),
+                           .with_side("reward", reward_offset, 4, 4).with_side("done", done_offset, 4, 4),
                        scratch, stream);
 }
 

@@ -337,19 +337,10 @@ int ktb_push_scatter_chunked(int root_dev, const void* src_root, size_t n_elems,
 }
 
 // ---- copy-engine form of the root side: no SM of the root is used ------------------------------------------------
-// A per-row source that rides along with the rows (the masked and ε-greedy MLP heads): row i of the shard (granule
-// elements) has row_bytes bytes at src + i·row_bytes, and they land `offset` bytes into the rank's staging half.
-// `name` names it in the errors.
-struct PushSide {
-  const void* src;
-  size_t row_bytes, offset;
-  const char* name;
-};
-
-// With n_sides (0 to 2; anything else, or null sides, is KTB_ERR_ARG) side sources, each rides along chunk by chunk
-// beside the rows and behind the same ack wait, with ready[c] published after every copy of chunk c.  Their checks come
-// after every check of the plain form: per side in order a null source, then row_bytes and whole-row chunks, then per
-// served rank the side's overlap with the rows, its end past stage_stride, and its overlap with an earlier side.
+// With n_sides (0 to 2; anything else, or null sides, is KTB_ERR_ARG) side sources (PushSide, a shard row being
+// `granule` elements), each rides along chunk by chunk beside the rows and behind the same ack wait, with ready[c]
+// published after every copy of chunk c.  Their checks come after every check of the plain form: per side in order a
+// null source, then row_bytes and whole-row chunks, then per served rank its regions (check_push_sides).
 static int push_scatter_ce_impl(const char* who, int root_dev, const void* src_root, size_t n_elems, size_t granule,
                                 int dtype, int n_ranks, int root_rank, const int* devs, void* const* stage_peer,
                                 size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
@@ -368,19 +359,13 @@ static int push_scatter_ce_impl(const char* who, int root_dev, const void* src_r
     KTB_REQUIRE(sd.src || n_elems == 0, KTB_ERR_ARG, "%s: null %s", who, sd.name);
     KTB_REQUIRE(sd.row_bytes > 0 && chunk_elems % granule == 0, KTB_ERR_ARG,
                 "%s: row_bytes must be positive and chunk_elems whole rows", who);
-    for (int r = 0; r < n_ranks; ++r) {
-      if (r == root_rank || !stage_peer[r]) continue;
-      size_t b = 0, e = 0;
-      ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
-      KTB_REQUIRE(sd.offset >= (e - b) * granule * es, KTB_ERR_ARG, "%s: %s_offset overlaps the rows of rank %d", who,
-                  sd.name, r);
-      KTB_REQUIRE(sd.offset <= stage_stride && (e - b) * sd.row_bytes <= stage_stride - sd.offset, KTB_ERR_ARG,
-                  "%s: %s of rank %d exceeds stage_stride", who, sd.name, r);
-      for (int o = 0; o < k; ++o)
-        KTB_REQUIRE(sd.offset >= sides[o].offset + (e - b) * sides[o].row_bytes ||
-                        sd.offset + (e - b) * sd.row_bytes <= sides[o].offset,
-                    KTB_ERR_ARG, "%s: %s of rank %d overlaps %s", who, sd.name, r, sides[o].name);
-    }
+  }
+  for (int r = 0; n_sides > 0 && r < n_ranks; ++r) {
+    if (r == root_rank || !stage_peer[r]) continue;
+    size_t b = 0, e = 0;
+    ktb_shard_bounds(n_elems / granule, n_ranks, r, &b, &e);
+    rc = check_push_sides(who, sides, n_sides, e - b, granule * es, stage_stride);
+    if (rc) return rc;
   }
   KTB_GUARD(root_dev);
   // one library stream (and fork/join event pair) per destination rank on the root device, created on first use:
@@ -455,7 +440,7 @@ int ktb_push_scatter_ce_masked(int root_dev, const void* src_root, size_t n_elem
                                size_t stage_stride, void* const* ctrl_peer, void* ctrl_root, size_t chunk_elems,
                                const void* mask_root, size_t row_bytes, size_t mask_offset, unsigned long long seq,
                                uintptr_t stream) {
-  const PushSide side{mask_root, row_bytes, mask_offset, "mask"};
+  const PushSide side{mask_root, row_bytes, mask_offset, 1, "mask"};
   return push_scatter_ce_impl("ktb_push_scatter_ce_masked", root_dev, src_root, n_elems, granule, dtype, n_ranks,
                               root_rank, devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems, 1, &side,
                               seq, stream);
@@ -470,7 +455,7 @@ int ktb_push_scatter_ce_sides(int root_dev, const void* src_root, size_t n_elems
   // a bad count or null arrays reach the impl as no sides at all, which it refuses after the plain form's checks
   const bool ok = n_sides >= 1 && n_sides <= 2 && side_src && side_row_bytes && side_offset;
   PushSide sides[2];
-  for (int k = 0; ok && k < n_sides; ++k) sides[k] = {side_src[k], side_row_bytes[k], side_offset[k], kNames[k]};
+  for (int k = 0; ok && k < n_sides; ++k) sides[k] = {side_src[k], side_row_bytes[k], side_offset[k], 1, kNames[k]};
   return push_scatter_ce_impl("ktb_push_scatter_ce_sides", root_dev, src_root, n_elems, granule, dtype, n_ranks,
                               root_rank, devs, stage_peer, stage_stride, ctrl_peer, ctrl_root, chunk_elems,
                               ok ? n_sides : -1, ok ? sides : nullptr, seq, stream);

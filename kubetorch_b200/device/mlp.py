@@ -877,49 +877,78 @@ _push_sessions = {}          # device tuple -> ops.PushSession
 _push_scratch = {}           # (device tuple, rank) -> scratch of that rank's pushed GEMMs
 
 
+def _stage_layout(rows: int, d_in: int, sides) -> Tuple[dict, int]:
+    """The staging half of a pushed call whose largest shard has `rows` rows of d_in bf16 observations: the rows, then
+    each side input (name, bytes per row) of `sides` in order, 256-byte aligned after the previous region.  Returns the
+    sides' offsets by name and the half's bytes."""
+    offsets, end = {}, rows * d_in * 2
+    for name, row_bytes in sides:
+        offsets[name] = (end + 255) // 256 * 256
+        end = offsets[name] + rows * row_bytes
+    return offsets, end
+
+
+def _forward_rows(obs_root, b, e, dev, stream, staged, ws, bufs, output, seed, log_std, mask, nvec, std, epsilon,
+                  taken, det, action, twin, td) -> None:
+    """mlp_forward of rows b .. e - 1 of a scatter→exec→gather call on `dev` and `stream`, into those rows of `bufs`:
+    the arguments of _mlp_scatter_gather_pushed, with ws, log_std and twin those on `dev`."""
+    logits, actions, log_probs, values = _rows(bufs, b, e)
+    valued = values is not None and epsilon is None   # an ε-greedy head's values slot is its q_max
+    mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=stream, staged=staged,
+                biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
+                log_std=log_std, mask=None if mask is None else mask[b:e], values=values, nvec=nvec,
+                log_std_bounds=None if std is None else std[:2],
+                **(det or dict(squash=None if std is None else bool(std[2]))),
+                **({} if epsilon is None else dict(epsilon=epsilon[b:e], q=log_probs, q_max=values)),
+                **({} if taken is None else dict(taken=taken[b:e], entropy=actions)),
+                **({} if output != "critic" else dict(action=action[b:e], twin=twin, q=logits, q2=actions,
+                                                       q_min=log_probs)),
+                **({} if td is None else dict(actor=td[0][dev], policy=td[1], reward=td[2][b:e], done=td[3][b:e],
+                                              gamma=td[4], alpha=td[5], twin=twin, target=logits)),
+                _stacked=valued or std is not None or output == "critic" or td is not None)
+
+
 def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root, actions_root, log_probs_root=None,
                                seed=None, log_std=None, mask=None, values_root=None, nvec=None, std=None,
-                               epsilon=None, taken=None, det=None, action=None, twin=None) -> None:
+                               epsilon=None, taken=None, det=None, action=None, twin=None, td=None) -> None:
     """The root PUSHES each rank's observation rows in GEMM-sized chunks (copy engines, posted NVLink writes, flags in
     device memory); every rank's GEMM chain consumes chunk c as soon as it has landed and stores its logits (and/or
-    actions) straight into the root's result; the root's own shard runs on the session's side stream beside the
-    scatter.  No host synchronisation, no events between devices.  weights[dev] = (w1, w2, w3, b1, b2, b3) on that
-    device (biases may be None); out_root / actions_root / log_probs_root are None when `output` does not want them
-    (with "gaussian", actions_root holds the fp32 actions [M, d_out]).  log_std[dev] is the Gaussian head's log_std on
-    that device.  With output="sample" or "gaussian" rank r draws the noise of global rows b_r .. e_r - 1 (its shard's
-    place in obs_root).  A legal-action `mask` [M, d_out] on the root travels with its rows: the copy engines push each
-    rank's mask rows into the same staging half, 256-byte aligned after the largest shard's observation rows, so no
-    rank reads the root's memory.  With `values_root` (fp32 [M]) weights[dev] holds the stacked W3v and b3v in place of
-    w3 and b3, and each rank stores its values there too.  `nvec` picks every rank's multi-discrete entry.  `std`
-    (_std) picks every rank's _gaussian_state entry, weights[dev] then holding the interleaved head.  With
-    output="epsilon_greedy", `epsilon` is the fp32 [M] on the root, pushed with the rows like the mask: each staging
-    half is rows | mask | ε, each 256-byte aligned (ktb_push_scatter_ce_sides), and log_probs_root / values_root are
-    its q and q_max.  With output="evaluate" or "gaussian_evaluate", `taken` (on the root) is pushed with the rows the
-    same way, each staging half rows | mask | taken with taken's offset rounded up to 8 bytes, and actions_root is the
-    entropy.  With output="deterministic", `det` is the call's dict(noise=, noise_clip=, squash=), and each staging
-    half holds the rows only.  With output="critic", `action` (fp32 [M, d_act] on the root) is pushed with the rows,
-    each staging half rows | action with the action 256-byte aligned, weights[dev] holds W1p in place of w1, twin[dev]
-    (unless None) the second critic's (W1p, b1, W2, b2, W3, b3), and out_root / actions_root / log_probs_root are q
-    (q1), q2 and q_min."""
+    actions) straight into the root's result; the root's own shard runs on the session's side stream beside the scatter.
+    No host synchronisation, no events between devices.  weights[dev] = (w1, w2, w3, b1, b2, b3) on that device (biases
+    may be None); out_root / actions_root / log_probs_root are None when `output` does not want them (with "gaussian",
+    actions_root holds the fp32 actions [M, d_out]).  log_std[dev] is the Gaussian head's log_std on that device.  With
+    output="sample" or "gaussian" rank r draws the noise of global rows b_r .. e_r - 1 (its shard's place in obs_root).
+    A legal-action `mask` [M, d_out] on the root travels with its rows: the copy engines push each rank's mask rows into
+    the same staging half (_stage_layout), so no rank reads the root's memory; every other per-row input below travels
+    the same way.  With `values_root` (fp32 [M]) weights[dev] holds the stacked W3v and b3v in place of w3 and b3, and
+    each rank stores its values there too.  `nvec` picks every rank's multi-discrete entry.  `std` (_std) picks every
+    rank's _gaussian_state entry, weights[dev] then holding the interleaved head.  With output="epsilon_greedy",
+    `epsilon` is the fp32 [M] on the root, pushed with the rows like the mask, and log_probs_root / values_root are its
+    q and q_max.  With output="evaluate" or "gaussian_evaluate", `taken` (on the root) is pushed with the rows, and
+    actions_root is the entropy.  With output="deterministic", `det` is the call's dict(noise=, noise_clip=, squash=),
+    and each staging half holds the rows only.  With output="critic", `action` (fp32 [M, d_act] on the root) is pushed
+    with the rows, weights[dev] holds W1p in place of w1, twin[dev] (unless None) the second critic's (W1p, b1, W2, b2,
+    W3, b3), and out_root / actions_root / log_probs_root are q (q1), q2 and q_min.  With output="td_target", td =
+    (actors, policy, reward, done, gamma, alpha): actors[dev] is the actor's six weights and biases on that device (its
+    head interleaved with the log-std head for policy="gaussian", picked by `std`; "deterministic" by `det`), reward and
+    done (on the root) are pushed with the rows, weights[dev] and twin[dev] are the target critics as with "critic", and
+    out_root is y."""
     root, n, key = devs[0], len(devs), tuple(devs)
     critic = output == "critic"
     valued = values_root is not None and epsilon is None   # an ε-greedy head's values_root is its q_max
     d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
-    d_out = action.shape[1] if critic else (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
+    actors, policy, reward, done, gamma, alpha = td or (None,) * 6
+    if td is not None:   # the entry's d_act
+        d_out = actors[root][4].shape[0] // (2 if std is not None else 1)
+    else:
+        d_out = action.shape[1] if critic else (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
     rows = max(e - b for b, e in bounds)
-    mask_offset = (rows * d_in * 2 + 255) // 256 * 256
-    stage_bytes = rows * d_in * 2 if mask is None else mask_offset + rows * d_out
-    if critic:   # the actions sit where a mask would
-        stage_bytes = mask_offset + rows * d_out * 4
-    eps_offset = None
-    if epsilon is not None:
-        eps_offset = mask_offset if mask is None else (mask_offset + rows * d_out + 255) // 256 * 256
-        stage_bytes = eps_offset + rows * 4
-    taken_offset = None
-    if taken is not None:
-        taken_row = taken[0].numel() * taken.element_size() if taken.dim() > 1 else taken.element_size()
-        taken_offset = (stage_bytes + 7) // 8 * 8
-        stage_bytes = taken_offset + rows * taken_row
+    taken_row = None if taken is None else taken[0].numel() * taken.element_size() if taken.dim() > 1 else \
+        taken.element_size()
+    sides = [(name, t, row_bytes) for name, t, row_bytes in
+             (("mask", mask, d_out), ("epsilon", epsilon, 4), ("taken", taken, taken_row), ("act", action, 4 * d_out),
+              ("reward", reward, 4), ("done", done, 4)) if t is not None]
+    offsets, stage_bytes = _stage_layout(rows, d_in, [(name, row_bytes) for name, _, row_bytes in sides])
     sess = _push_sessions.get(key)
     if sess is None or sess.stride < stage_bytes:
         sess = _push_sessions[key] = ops.PushSession(devs, stage_bytes)
@@ -930,54 +959,54 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         raise
     # scratch per rank, not per device: ranks sharing a device must not share one, nor the root's own shard on the
     # side stream
-    scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS, critic)
+    if td is not None:
+        scratch_bytes = pushed_td_scratch_bytes(rows, actors[root][0].shape[0], d_hidden, d_out, PUSH_CHUNK_ROWS)
+    else:
+        scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS, critic)
     scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], scratch_bytes) for r in range(1, n)]
     streams = [ops.current_stream_handle(d) for d in devs]
     bufs = (out_root, actions_root, log_probs_root, values_root)
     b0, e0 = bounds[0]
     own = e0 > b0
     if own:
-        ws = weights[root]
-        logits, actions, log_probs, values = _rows(bufs, b0, e0)
-        mlp_forward(obs_root[b0:e0], ws[0], ws[1], ws[2], out=logits, device=root, stream=sess.fork(), staged=False,
-                    biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b0, log_probs=log_probs,
-                    log_std=None if log_std is None else log_std[root], mask=None if mask is None else mask[b0:e0],
-                    values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
-                    **(det or dict(squash=None if std is None else bool(std[2]))),
-                    **({} if epsilon is None else dict(epsilon=epsilon[b0:e0], q=log_probs, q_max=values)),
-                    **({} if taken is None else dict(taken=taken[b0:e0], entropy=actions)),
-                    **({} if not critic else dict(action=action[b0:e0], twin=None if twin is None else twin[root],
-                                                  q=logits, q2=actions, q_min=log_probs)),
-                    _stacked=valued or std is not None or critic)
+        _forward_rows(obs_root, b0, e0, root, sess.fork(), False, weights[root], bufs, output, seed,
+                      None if log_std is None else log_std[root], mask, nvec, std, epsilon, taken, det, action,
+                      None if twin is None else twin[root], td)
     scatter = (L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
                PUSH_CHUNK_ROWS * d_in)
-    if epsilon is not None or taken is not None or critic:
-        last = (epsilon.data_ptr(), 4, eps_offset) if epsilon is not None else \
-            (action.data_ptr(), 4 * d_out, mask_offset) if critic else \
-            (taken.data_ptr(), taken_row, taken_offset)
-        sides = ([] if mask is None else [(mask.data_ptr(), d_out, mask_offset)]) + [last]
-        src, row_bytes, offsets = zip(*sides)
+    if sides:
         L.call("ktb_push_scatter_ce_sides", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, *scatter,
-               len(sides), L.arr(ctypes.c_void_p, src), L.arr(ctypes.c_size_t, row_bytes),
-               L.arr(ctypes.c_size_t, offsets), seq, streams[0])
-    elif mask is None:
+               len(sides), L.arr(ctypes.c_void_p, [t.data_ptr() for _, t, _ in sides]),
+               L.arr(ctypes.c_size_t, [row_bytes for _, _, row_bytes in sides]),
+               L.arr(ctypes.c_size_t, [offsets[name] for name, _, _ in sides]), seq, streams[0])
+    else:
         L.call("ktb_push_scatter_ce", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0, *scatter, seq,
                streams[0])
-    else:
-        L.call("ktb_push_scatter_ce_masked", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
-               *scatter, mask.data_ptr(), d_out, mask_offset, seq, streams[0])
+
+    # a TD target's actor options as mlp_forward takes them
+    pol = det or dict(log_std_bounds=None if std is None else std[:2], squash=None if std is None else std[2])
 
     def issue(r):
         b, e = bounds[r]
         ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
         logits, actions, log_probs, values = _rows(bufs, b, e)
-        entry, head = _head(output, logits, actions, log_probs, seed, b,
-                            None if log_std is None else log_std[devs[r]], ptr, pushed=True,
-                            mask=None if mask is None else mask_offset, values=values, nvec=nvec, std=std,
-                            epsilon=eps_offset, taken=taken_offset, det=None if det is None else _det(**det),
-                            act=mask_offset if critic else None,
-                            twin=None if twin is None else tuple(ptr(t) for t in twin[devs[r]]))
+        if td is not None:   # y rides in the logits slot
+            wptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+            entry = "ktb_mlp_bf16_td_target_" + policy + "_pushed"
+            head = (*(wptr(t) for t in (twin[devs[r]] if twin is not None else (None,) * 6)),
+                    actors[root][0].shape[0], *(wptr(t) for t in actors[devs[r]]),
+                    *_td_args(policy, seed, None if log_std is None else log_std[devs[r]], pol.get("log_std_bounds"),
+                              pol["squash"], pol.get("noise"), pol.get("noise_clip"), b),
+                    offsets["reward"], offsets["done"], float(gamma), *((float(alpha),) if policy == "gaussian" else ()),
+                    ptr(logits))
+        else:
+            entry, head = _head(output, logits, actions, log_probs, seed, b,
+                                None if log_std is None else log_std[devs[r]], ptr, pushed=True,
+                                mask=offsets.get("mask"), values=values, nvec=nvec, std=std,
+                                epsilon=offsets.get("epsilon"), taken=offsets.get("taken"),
+                                det=None if det is None else _det(**det), act=offsets.get("act"),
+                                twin=None if twin is None else tuple(ptr(t) for t in twin[devs[r]]))
         L.call(entry, devs[r], sess.stage[r].data_ptr(), sess.stride, e - b, d_in, d_hidden, d_out, ws[0].data_ptr(),
                ptr(ws[3]), ws[1].data_ptr(), ptr(ws[4]), ws[2].data_ptr(), ptr(ws[5]), *head, scratch[r].data_ptr(),
                sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq, streams[r])
@@ -1040,13 +1069,11 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                   taken, noise, noise_clip, action, twin, w2, td)
     if transfer not in ("auto", "pull", "push"):
         raise ValueError("transfer must be 'auto', 'pull' or 'push'")
-    if output == "td_target":
-        return _td_scatter_gather(obs_root, w1, w2, w3, devs, transfer, biases, twin, td, seed, log_std,
-                                  log_std_bounds, squash, noise, noise_clip, target_root)
-    critic = output == "critic"
+    critic, target = output == "critic", output == "td_target"
     if critic:   # q (or q1), q2 and q_min ride in the logits, actions and log_probs slots
         out_root, actions_root, log_probs_root = q_root, q2_root, q_min_root
-    det = dict(noise=noise, noise_clip=noise_clip, squash=squash) if output == "deterministic" else None
+    det = dict(noise=noise, noise_clip=noise_clip, squash=squash) \
+        if output == "deterministic" or target and policy == "deterministic" else None
     ops.ensure_init(set(devs))
     M = obs_root.shape[0]
     if output == "epsilon_greedy" and not isinstance(epsilon, torch.Tensor):   # before `ready`: every rank reads it
@@ -1054,14 +1081,23 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     valued = value is not None
     if taken is not None:   # the entropy rides in the actions slot
         actions_root = entropy_root
-    bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
-                    valued, nvec, twin is not None)
-    std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
-    if valued or std is not None:
+    if target:   # y, of reward's shape, rides in the logits slot
+        if target_root is None:
+            target_root = torch.empty(reward.shape, dtype=torch.float32, device=obs_root.device)
+        else:
+            ops.ensure_init({target_root.device.index})
+        bufs = (target_root, None, None, None)
+    else:
+        bufs = _outputs(output, M, w3.shape[0], obs_root.device, out_root, actions_root, log_probs_root, values_root,
+                        valued, nvec, twin is not None)
+    std = _std(log_std, log_std_bounds, squash) if output == "gaussian" or target and policy == "gaussian" else None
+    if target and std is not None:   # the SAC actor's head interleaved with its log-std head
+        actor = (*actor[:4], *_stacked_head(actor[4], actor[5], None, None, *log_std))
+    elif valued or std is not None:
         w3, b3 = _stacked_head(w3, biases[2], *(value or (None, None)), *(log_std if std is not None else ()))
         biases = (biases[0], biases[1], b3)
     twins = None
-    if critic:
+    if critic or target:
         w1 = _padded_w1(w1, obs_root.shape[1])
         if twin is not None:
             twin = (_padded_w1(twin[0], obs_root.shape[1]), *twin[1:])
@@ -1070,20 +1106,28 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     ready = torch.cuda.Event()
     ready.record(root_stream)
     bounds = [ops.shard_bounds(M, len(devs), r) for r in range(len(devs))]
-    views = [_result(output, *_rows(bufs, b, e)) for b, e in bounds]
+    views = [target_root[b:e] if target else _result(output, *_rows(bufs, b, e)) for b, e in bounds]
     weights = {dev: _weights_on(dev, (w1, w2, w3)) + _weights_on(dev, biases) for dev in set(devs)}
     if std is not None:   # the pair only marks the form on each rank: its rows are in the interleaved head
         log_stds = {dev: log_std for dev in set(devs)}
     else:
         log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
+    if target:
+        td = ({dev: tuple(_weights_on(dev, actor)) for dev in set(devs)}, *td[1:])
     if _use_push(devs, bounds, transfer):
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec, std, epsilon, taken, det, action, twins)
+                                   nvec, std, epsilon, taken, det, action, twins, td if target else None)
         return views
+    rows = max(e - b for b, e in bounds)
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
-        _scratch_for(dev, max(e - b for b, e in bounds), w1.shape[0], critic)
+        if target:
+            d_act = actor[4].shape[0] // (2 if std is not None else 1)
+            _cached_buffer(_scratch, dev, dev,
+                           L.load().ktb_mlp_td_target_scratch_bytes(rows, actor[0].shape[0], w1.shape[0], d_act))
+        else:
+            _scratch_for(dev, rows, w1.shape[0], critic)
         if dev != root:
-            _stage_for(dev, max(e - b for b, e in bounds), obs_root.shape[1])
+            _stage_for(dev, rows, obs_root.shape[1])
     streams = {dev: torch.cuda.current_stream(dev) for dev in set(devs)}
 
     def issue(r):
@@ -1092,22 +1136,13 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         b, e = bounds[r]
         if e == b:
             return None
-        ws = weights[dev]
         st = streams[dev]
         with torch.cuda.device(dev):
             if dev != root:
                 st.wait_event(ready)
-            logits, actions, log_probs, values = _rows(bufs, b, e)
-            mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=st, biases=ws[3:],
-                        output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
-                        log_std=None if log_stds is None else log_stds[dev], mask=None if mask is None else mask[b:e],
-                        values=values, nvec=nvec, log_std_bounds=None if std is None else std[:2],
-                        **(det or dict(squash=None if std is None else bool(std[2]))),
-                        **({} if epsilon is None else dict(epsilon=epsilon[b:e], q=log_probs, q_max=values)),
-                        **({} if taken is None else dict(taken=taken[b:e], entropy=actions)),
-                        **({} if not critic else dict(action=action[b:e], twin=None if twins is None else twins[dev],
-                                                      q=logits, q2=actions, q_min=log_probs)),
-                        _stacked=valued or std is not None or critic)
+            _forward_rows(obs_root, b, e, dev, st, None, weights[dev], bufs, output, seed,
+                          None if log_stds is None else log_stds[dev], mask, nvec, std, epsilon, taken, det, action,
+                          None if twins is None else twins[dev], td if target else None)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)
@@ -1115,120 +1150,9 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         return None
 
     if len(set(devs)) > 1:
-        done = list(_thread_pool().map(issue, range(len(devs))))
+        done_evs = list(_thread_pool().map(issue, range(len(devs))))
     else:
-        done = [issue(r) for r in range(len(devs))]
-    for ev in done:
-        if ev is not None:
-            root_stream.wait_event(ev)
-    return views
-
-
-def _td_scatter_gather(obs_root, w1, w2, w3, devs, transfer, biases, twin, td, seed, log_std, log_std_bounds, squash,
-                       noise, noise_clip, target_root) -> list:
-    """mlp_scatter_gather's output="td_target" (checked): the critics' W1p and the SAC actor's interleaved head are
-    built on the root and copied to the other devices like the other weights; rank r computes y of rows b_r .. e_r - 1
-    with row_offset b_r, pulling its rows of obs, reward and done in place or having them pushed with ktb_push_scatter_ce_sides
-    (each staging half rows | reward | done, each 256-byte aligned), and stores them into the root's y."""
-    actor, policy, reward, done, gamma, alpha = td
-    root, n = devs[0], len(devs)
-    M, d_in = obs_root.shape
-    ops.ensure_init(set(devs))
-    gaussian = policy == "gaussian"
-    if target_root is None:
-        target_root = torch.empty(reward.shape, dtype=torch.float32, device=obs_root.device)
-    else:
-        ops.ensure_init({target_root.device.index})
-    w1 = _padded_w1(w1, d_in)
-    if twin is not None:
-        twin = (_padded_w1(twin[0], d_in), *twin[1:])
-    actor = tuple(actor)
-    if gaussian:
-        actor = actor[:4] + _stacked_head(actor[4], actor[5], None, None, *log_std)
-    d_hidden, d_ha, d_act = w1.shape[0], actor[0].shape[0], actor[4].shape[0] // (2 if gaussian else 1)
-    weights = {dev: _weights_on(dev, (w1, biases[0], w2, biases[1], w3, biases[2])) for dev in set(devs)}
-    twins = {dev: None if twin is None else tuple(_weights_on(dev, twin)) for dev in set(devs)}
-    actors = {dev: tuple(_weights_on(dev, actor)) for dev in set(devs)}
-    bounds = [ops.shard_bounds(M, n, r) for r in range(n)]
-    views = [target_root[b:e] for b, e in bounds]
-    rows = max(e - b for b, e in bounds)
-    opts = dict(output="td_target", policy=policy, gamma=gamma, alpha=alpha, seed=seed, log_std=log_std,
-                log_std_bounds=log_std_bounds, squash=squash, noise=noise, noise_clip=noise_clip, _stacked=True)
-
-    def run(dev, b, e, stream, staged):
-        ws = weights[dev]
-        mlp_forward(obs_root[b:e], ws[0], ws[2], ws[4], device=dev, stream=stream, staged=staged,
-                    biases=(ws[1], ws[3], ws[5]), twin=twins[dev], actor=actors[dev], reward=reward[b:e],
-                    done=done[b:e], target=target_root[b:e], row_offset=b, **opts)
-
-    if _use_push(devs, bounds, transfer):
-        key = tuple(devs)
-        reward_offset = (rows * d_in * 2 + 255) // 256 * 256
-        done_offset = reward_offset + (rows * 4 + 255) // 256 * 256
-        stage_bytes = done_offset + rows * 4
-        sess = _push_sessions.get(key)
-        if sess is None or sess.stride < stage_bytes:
-            sess = _push_sessions[key] = ops.PushSession(devs, stage_bytes)
-        try:
-            seq = sess.begin()
-        except ops.PushTimeout:
-            del _push_sessions[key]
-            raise
-        nbytes = pushed_td_scratch_bytes(rows, d_ha, d_hidden, d_act, PUSH_CHUNK_ROWS)
-        scratch = [None] + [_cached_buffer(_push_scratch, (key, r), devs[r], nbytes) for r in range(1, n)]
-        streams = [ops.current_stream_handle(d) for d in devs]
-        b0, e0 = bounds[0]
-        own = e0 > b0
-        if own:
-            run(root, b0, e0, sess.fork(), False)
-        L.call("ktb_push_scatter_ce_sides", root, obs_root.data_ptr(), obs_root.numel(), d_in, L.BF16, n, 0,
-               L.arr(ctypes.c_int, devs), sess.stage_ptrs, sess.stride, sess.ctrl_ptrs, sess.ctrl[0].data_ptr(),
-               PUSH_CHUNK_ROWS * d_in, 2, L.arr(ctypes.c_void_p, [reward.data_ptr(), done.data_ptr()]),
-               L.arr(ctypes.c_size_t, [4, 4]), L.arr(ctypes.c_size_t, [reward_offset, done_offset]), seq, streams[0])
-
-        def issue(r):
-            b, e = bounds[r]
-            ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
-            ws, tw = weights[devs[r]], twins[devs[r]]
-            L.call("ktb_mlp_bf16_td_target_" + policy + "_pushed", devs[r], sess.stage[r].data_ptr(), sess.stride,
-                   e - b, d_in, d_hidden, d_act, *(ptr(t) for t in ws), *(ptr(t) for t in (tw or (None,) * 6)), d_ha,
-                   *(ptr(t) for t in actors[devs[r]]),
-                   *_td_args(policy, seed, log_std, log_std_bounds, squash, noise, noise_clip, b), reward_offset,
-                   done_offset, float(gamma), *((float(alpha),) if gaussian else ()),
-                   target_root.data_ptr() + 4 * b if e > b else 0,
-                   scratch[r].data_ptr(), sess.ctrl[r].data_ptr(), sess.ctrl[0].data_ptr(), r, PUSH_CHUNK_ROWS, seq,
-                   streams[r])
-
-        list(_thread_pool().map(issue, range(1, n)))
-        sess.finish(seq, joined=own)
-        return views
-    lib = L.load()
-    for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
-        _cached_buffer(_scratch, dev, dev, lib.ktb_mlp_td_target_scratch_bytes(rows, d_ha, d_hidden, d_act))
-        if dev != root:
-            _stage_for(dev, rows, d_in)
-    root_stream = torch.cuda.current_stream(root)
-    ready = torch.cuda.Event()
-    ready.record(root_stream)
-    streams = {dev: torch.cuda.current_stream(dev) for dev in set(devs)}
-
-    def issue_pull(r):
-        dev = devs[r]
-        b, e = bounds[r]
-        if e == b:
-            return None
-        st = streams[dev]
-        with torch.cuda.device(dev):
-            if dev != root:
-                st.wait_event(ready)
-            run(dev, b, e, st, None)
-            if dev != root:
-                ev = torch.cuda.Event()
-                ev.record(st)
-                return ev
-        return None
-
-    done_evs = list(_thread_pool().map(issue_pull, range(n))) if len(set(devs)) > 1 else [issue_pull(r) for r in range(n)]
+        done_evs = [issue(r) for r in range(len(devs))]
     for ev in done_evs:
         if ev is not None:
             root_stream.wait_event(ev)

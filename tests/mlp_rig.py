@@ -270,48 +270,77 @@ class PushRig:
     """What PushSession does for the MLP, for one head: ranks [0, 0, 0] on cuda:0 and ONE stream, the head's pushed
     entry on ranks 1.. and its plain entry on the root's shard.  Every flag a kernel waits on is published by work
     enqueued before it on that stream (or on library streams that stream already waits for), so no wait can block.
-    Staging and scratch are guarded buffers of the documented sizes."""
+    Staging and scratch are guarded buffers of the documented sizes; `scratch_bytes(rows)` sizes a rank's scratch (the
+    policy entries' by default).  The head's per-row inputs, `sides` ((name, bytes per row) in order), ride with the
+    rows (ktb_push_scatter_ce_sides) into each staging half, laid out here and not by the package: the rows, then each
+    side 8-byte aligned after the previous region, tighter than the package's 256-byte layout, since the pushed
+    entries take any valid set of regions."""
 
-    def __init__(self, K, M, d_in, d_hidden, chunk_rows, engine, head, n_ranks=3):
+    def __init__(self, K, M, d_in, d_hidden, chunk_rows, engine, head=None, n_ranks=3, sides=(), scratch_bytes=None):
         self.d_in, self.d_hidden, self.chunk_rows, self.engine, self.head = d_in, d_hidden, chunk_rows, engine, head
         self.n = n_ranks
         self.bounds = [K.shard_bounds(M, n_ranks, r) for r in range(n_ranks)]
         shard = max(e - b for b, e in self.bounds)
-        self.stride = (shard * d_in * 2 + 255) // 256 * 256
+        end, self.offsets, self.row_bytes = shard * d_in * 2, {}, dict(sides)
+        for name, row_bytes in sides:
+            self.offsets[name] = (end + 7) // 8 * 8
+            end = self.offsets[name] + shard * row_bytes
+        self.stride = (end + 255) // 256 * 256
         self.ctrl = [torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda")
                      for _ in range(n_ranks)]
         self.stage = [None] + [Guarded(2 * self.stride) for _ in range(1, n_ranks)]
-        self.scratch = [None] + [Guarded(mlp.pushed_scratch_bytes(e - b, d_hidden, chunk_rows))
-                                 for b, e in self.bounds[1:]]
+        size = scratch_bytes or (lambda rows: mlp.pushed_scratch_bytes(rows, d_hidden, chunk_rows))
+        self.scratch = [None] + [Guarded(size(e - b)) for b, e in self.bounds[1:]]
         torch.cuda.synchronize()
         self.seq = 0
 
-    def call(self, obs, w, b, out, seed=0, log_std=None):
-        """One call over the M rows of obs; `out` maps the head's outputs to the addresses of their M-row buffers."""
+    def push(self, obs, sides, rank_entry, root_entry):
+        """One call over the M rows of obs with the side tensors `sides` (by name): the scatter, then
+        rank_entry(r, lo, hi, push) on ranks 1.., `push` holding the pushed entry's arguments (stage, stride, scratch,
+        ctrl, ctrl_root, rank, chunk_rows, seq) and each side's offset by name, then root_entry(lo, hi, rows) on the
+        root's shard, `rows` holding each side's address at row lo by name, then ktb_push_wait."""
         self.seq += 1
         seq, n, d_in, st = self.seq, self.n, self.d_in, stream()
         stage_ptrs = L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in self.stage[1:]])
         ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
         root = self.ctrl[0].data_ptr()
-        if self.engine == "sm":
+        names = list(self.offsets)
+        if names:
+            L.call("ktb_push_scatter_ce_sides", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
+                   L.arr(ctypes.c_int, [0] * n), stage_ptrs, self.stride, ctrl_ptrs, root, self.chunk_rows * d_in,
+                   len(names), L.arr(ctypes.c_void_p, [sides[k].data_ptr() for k in names]),
+                   L.arr(ctypes.c_size_t, [self.row_bytes[k] for k in names]),
+                   L.arr(ctypes.c_size_t, [self.offsets[k] for k in names]), seq, st)
+        elif self.engine == "sm":
             L.call("ktb_push_scatter_chunked", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0, stage_ptrs,
                    self.stride, ctrl_ptrs, root, self.chunk_rows * d_in, 0, seq, st)
         else:
             L.call("ktb_push_scatter_ce", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
                    L.arr(ctypes.c_int, [0] * n), stage_ptrs, self.stride, ctrl_ptrs, root, self.chunk_rows * d_in,
                    seq, st)
-        a = named_args(obs, w, b, out, seed, log_std)
         for r in range(1, n):
             lo, hi = self.bounds[r]
-            L.call(*entry_args(self.head, dict(
-                from_row(self.head, a, lo), M=hi - lo, stage=self.stage[r].ptr(), stride=self.stride,
-                scratch=self.scratch[r].ptr(), ctrl=self.ctrl[r].data_ptr(), ctrl_root=root, rank=r,
-                chunk_rows=self.chunk_rows, seq=seq), push=True))
+            rank_entry(r, lo, hi, dict(self.offsets, stage=self.stage[r].ptr(), stride=self.stride,
+                                       scratch=self.scratch[r].ptr(), ctrl=self.ctrl[r].data_ptr(), ctrl_root=root,
+                                       rank=r, chunk_rows=self.chunk_rows, seq=seq))
         lo, hi = self.bounds[0]
-        scratch = mlp._scratch_for(0, hi - lo, self.d_hidden)
-        L.call(*entry_args(self.head, dict(from_row(self.head, a, lo), M=hi - lo, obs=a["obs"] + lo * d_in * 2,
-                                           scratch=scratch.data_ptr())))
+        root_entry(lo, hi, {k: sides[k].data_ptr() + lo * self.row_bytes[k] for k in names})
         L.call("ktb_push_wait", 0, root, n, 0, seq, st)
+
+    def call(self, obs, w, b, out, seed=0, log_std=None, sides=None, **more):
+        """One call of the head over the M rows of obs; `out` maps the head's outputs to the addresses of their M-row
+        buffers, `sides` its side tensors by name, `more` adds named arguments (named_args)."""
+        a = named_args(obs, w, b, out, seed, log_std, **more)
+
+        def rank(r, lo, hi, push):
+            L.call(*entry_args(self.head, dict(from_row(self.head, a, lo), M=hi - lo, **push), push=True))
+
+        def root(lo, hi, rows):
+            scratch = mlp._scratch_for(0, hi - lo, self.d_hidden)
+            L.call(*entry_args(self.head, dict(from_row(self.head, a, lo), M=hi - lo, obs=a["obs"] + lo * self.d_in * 2,
+                                               scratch=scratch.data_ptr(), **rows)))
+
+        self.push(obs, sides or {}, rank, root)
 
     def statuses(self):
         out = []
@@ -320,6 +349,14 @@ class PushRig:
             L.call("ktb_push_status", 0, c.data_ptr(), ctypes.byref(s))
             out.append(s.value)
         return out
+
+    def check(self):
+        """After the calls: every status 0, and no write past a rank's staging or scratch."""
+        torch.cuda.synchronize()
+        assert self.statuses() == [0] * self.n
+        for r in range(1, self.n):
+            self.stage[r].check(f"stage[{r}]")
+            self.scratch[r].check(f"scratch[{r}]")
 
 
 def run_guarded(form, head, K, chunk, obs, w, b, seed=0, log_std=None, offsets=None):

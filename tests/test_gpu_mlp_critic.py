@@ -11,7 +11,7 @@ import torch
 
 from kubetorch_b200.device import lib as L
 from kubetorch_b200.device import mlp
-from mlp_rig import K, Guarded, deployed, expect_status, stream, tuning  # noqa: F401
+from mlp_rig import K, Guarded, PushRig, deployed, expect_status, stream, tuning  # noqa: F401
 from oracle import ref_dispatch
 from policy_critic_cases import critic_q, mlp_critic, mlp_critic_nobias, mlp_critic_twin, q_min
 
@@ -125,50 +125,31 @@ def test_nan_and_infinite_actions_follow_the_policy_entry(K):
 
 
 def _push_call(K, obs, act, c, twin, chunk_rows, n=3):
-    """The pushed forms as a PushSession runs them, ranks [0, 0, 0] on cuda:0 and one stream: the rows and the actions
-    pushed by ktb_push_scatter_ce_sides (each staging half rows | action), ranks 1.. on the _pushed entry, the root's
-    shard on the plain one."""
+    """The pushed forms through the push rig, ranks [0] * n on cuda:0 and one stream, the actions a side input beside
+    the rows: ranks 1.. on the _pushed entry, the root's shard on the plain one."""
     M, d_in = obs.shape
-    d_act = act.shape[1]
-    bounds = [K.shard_bounds(M, n, r) for r in range(n)]
-    shard = max(e - b for b, e in bounds)
-    act_off = (shard * d_in * 2 + 255) // 256 * 256
-    stride = (act_off + shard * d_act * 4 + 255) // 256 * 256
-    ctrl = [torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda") for _ in range(n)]
-    stage = [None] + [Guarded(2 * stride) for _ in range(1, n)]
-    scratch = [None] + [Guarded(mlp.pushed_scratch_bytes(e - b, c[0].shape[0], chunk_rows, True))
-                        for b, e in bounds[1:]]
+    d_act, d_h = act.shape[1], c[0].shape[0]
+    rig = PushRig(K, M, d_in, d_h, chunk_rows, "ce", n_ranks=n, sides=[("act", d_act * 4)],
+                  scratch_bytes=lambda rows: mlp.pushed_scratch_bytes(rows, d_h, chunk_rows, True))
     outs = [torch.full((M,), 7.0, device="cuda") for _ in range(3 if twin else 1)]
     w1p = [mlp._padded_w1(c[0], d_in)] + ([mlp._padded_w1(twin[0], d_in)] if twin else [])
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     weights = [ptr(t) for t in (w1p[0],) + c[1:]]
     twin_ptrs = [ptr(t) for t in (w1p[1],) + tuple(twin[1:])] if twin else []
     entry = "ktb_mlp_bf16_critic" + ("_twin" if twin else "")
-    st = stream()
-    root = ctrl[0].data_ptr()
-    for seq in (1, 2):
-        L.call("ktb_push_scatter_ce_sides", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
-               L.arr(ctypes.c_int, [0] * n), L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in stage[1:]]), stride,
-               L.arr(ctypes.c_void_p, [t.data_ptr() for t in ctrl]), root, chunk_rows * d_in, 1,
-               L.arr(ctypes.c_void_p, [act.data_ptr()]), L.arr(ctypes.c_size_t, [d_act * 4]),
-               L.arr(ctypes.c_size_t, [act_off]), seq, st)
-        for r in range(1, n):
-            b, e = bounds[r]
-            L.call(entry + "_pushed", 0, stage[r].ptr(), stride, e - b, d_in, c[0].shape[0], d_act, *weights,
-                   *twin_ptrs, act_off, *[o.data_ptr() + 4 * b for o in outs], scratch[r].ptr(), ctrl[r].data_ptr(),
-                   root, r, chunk_rows, seq, st)
-        b, e = bounds[0]
-        L.call(entry, 0, obs.data_ptr() + b * d_in * 2, e - b, d_in, c[0].shape[0], d_act, *weights, *twin_ptrs,
-               act.data_ptr() + b * d_act * 4, *[o.data_ptr() + 4 * b for o in outs],
-               mlp._scratch_for(0, e - b, c[0].shape[0], True).data_ptr(), 0, st)
-        L.call("ktb_push_wait", 0, root, n, 0, seq, st)
-    torch.cuda.synchronize()
-    for r in range(1, n):
-        s = ctypes.c_uint(0)
-        L.call("ktb_push_status", 0, ctrl[r].data_ptr(), ctypes.byref(s))
-        assert s.value == 0
-        stage[r].check(f"stage[{r}]")
-        scratch[r].check(f"scratch[{r}]")
+
+    def rank(r, b, e, p):
+        L.call(entry + "_pushed", 0, p["stage"], p["stride"], e - b, d_in, d_h, d_act, *weights, *twin_ptrs, p["act"],
+               *[o.data_ptr() + 4 * b for o in outs], p["scratch"], p["ctrl"], p["ctrl_root"], r, chunk_rows, p["seq"],
+               stream())
+
+    def root(b, e, rows):
+        L.call(entry, 0, obs.data_ptr() + b * d_in * 2, e - b, d_in, d_h, d_act, *weights, *twin_ptrs, rows["act"],
+               *[o.data_ptr() + 4 * b for o in outs], mlp._scratch_for(0, e - b, d_h, True).data_ptr(), 0, stream())
+
+    for _ in (1, 2):
+        rig.push(obs, {"act": act}, rank, root)
+    rig.check()
     return outs
 
 
@@ -292,7 +273,7 @@ def test_twin_statuses_cover_the_second_critic(K):
 
 @pytest.mark.parametrize("entry", ["ktb_mlp_bf16_critic", "ktb_mlp_bf16_critic_twin"])
 @pytest.mark.parametrize("case,over,status", [
-    ("d_act_first", dict(d_act=65, act_off=2), L.ERR_UNSUPPORTED),
+    ("region_before_d_act", dict(d_act=65, act_off=2), L.ERR_ARG),
     ("act_overlaps_rows", dict(act_off=256 * 256 * 2 - 4), L.ERR_ARG),
     ("act_past_stride", dict(act_off=(1 << 20) - 4), L.ERR_ARG),
     ("act_align", dict(act_off=(1 << 17) + 2), L.ERR_ARG),

@@ -214,57 +214,6 @@ def test_edge_rows(K):
 
 
 # ---- 6. forms -----------------------------------------------------------------------------------------------------------------
-class EpsPushRig(PushRig):
-    """What mlp._mlp_scatter_gather_pushed does for an ε-greedy head, on ranks [0, 0, 0] of cuda:0 and ONE stream: the
-    copy-engine scatter (ktb_push_scatter_ce_sides) pushes each rank's rows, mask rows (masked heads) and ε rows into
-    its guarded staging half, laid out rows | mask | ε, each 256-byte aligned; the pushed entry runs on ranks 1.. and
-    the plain entry on the root's shard."""
-
-    def __init__(self, K, M, d_in, d_hidden, d_out, chunk_rows, head, n_ranks=3):
-        self.d_in, self.d_hidden, self.d_out, self.chunk_rows, self.head, self.n = \
-            d_in, d_hidden, d_out, chunk_rows, head, n_ranks
-        self.masked = head is EPS_MASKED
-        self.bounds = [K.shard_bounds(M, n_ranks, r) for r in range(n_ranks)]
-        shard = max(e - b for b, e in self.bounds)
-        self.mask_offset = (shard * d_in * 2 + 255) // 256 * 256
-        self.eps_offset = (self.mask_offset + shard * d_out + 255) // 256 * 256 if self.masked else self.mask_offset
-        self.stride = (self.eps_offset + shard * 4 + 255) // 256 * 256
-        self.ctrl = [torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda")
-                     for _ in range(n_ranks)]
-        self.stage = [None] + [Guarded(2 * self.stride) for _ in range(1, n_ranks)]
-        self.scratch = [None] + [Guarded(mlp.pushed_scratch_bytes(e - b, d_hidden, chunk_rows))
-                                 for b, e in self.bounds[1:]]
-        torch.cuda.synchronize()
-        self.seq = 0
-
-    def call(self, obs, w, b, legal, eps, out, seed=0):
-        self.seq += 1
-        seq, n, d_in, d_out, st = self.seq, self.n, self.d_in, self.d_out, stream()
-        stage_ptrs = L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in self.stage[1:]])
-        ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
-        root = self.ctrl[0].data_ptr()
-        sides = ([(legal.data_ptr(), d_out, self.mask_offset)] if self.masked else []) + \
-            [(eps.data_ptr(), 4, self.eps_offset)]
-        src, row_bytes, offsets = zip(*sides)
-        L.call("ktb_push_scatter_ce_sides", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
-               L.arr(ctypes.c_int, [0] * n), stage_ptrs, self.stride, ctrl_ptrs, root, self.chunk_rows * d_in,
-               len(sides), L.arr(ctypes.c_void_p, src), L.arr(ctypes.c_size_t, row_bytes),
-               L.arr(ctypes.c_size_t, offsets), seq, st)
-        a = named_args(obs, w, b, out, seed)
-        for r in range(1, n):
-            lo, hi = self.bounds[r]
-            L.call(*entry_args(self.head, dict(
-                from_row(self.head, a, lo), M=hi - lo, mask=self.mask_offset, epsilon=self.eps_offset,
-                stage=self.stage[r].ptr(), stride=self.stride, scratch=self.scratch[r].ptr(),
-                ctrl=self.ctrl[r].data_ptr(), ctrl_root=root, rank=r, chunk_rows=self.chunk_rows, seq=seq), push=True))
-        lo, hi = self.bounds[0]
-        scratch = mlp._scratch_for(0, hi - lo, self.d_hidden)
-        L.call(*entry_args(self.head, dict(from_row(self.head, a, lo), M=hi - lo, obs=a["obs"] + lo * d_in * 2,
-                                           mask=0 if legal is None else legal.data_ptr() + lo * d_out,
-                                           epsilon=eps.data_ptr() + lo * 4, scratch=scratch.data_ptr())))
-        L.call("ktb_push_wait", 0, root, n, 0, seq, st)
-
-
 def _fresh(M):
     return {"actions": torch.full((M,), -1, dtype=torch.int64, device="cuda"),
             "q": torch.full((M,), -1, dtype=torch.int32, device="cuda"),
@@ -299,14 +248,16 @@ def test_every_form_chunking_and_row_split_gives_identical_bits(K, head, d_out):
         same([torch.cat([x, y]) for x, y in zip(lo, hi)], want, split)
     assert torch.equal(eps, keep)
     Mp = 3 * 1408
-    rig = EpsPushRig(K, Mp, 256, 1024, d_out, 512, head)
+    masked = [("mask", d_out)] if head is EPS_MASKED else []
+    rig = PushRig(K, Mp, 256, 1024, 512, "ce", head, sides=masked + [("epsilon", 4)])
     for it in range(3):
         obs_p = randn((Mp, 256), 710 + it)
         legal_p = random_legal(Mp, d_out, 720 + it) if head is EPS_MASKED else None
         eps_p = _mixed_eps(Mp, 730 + it)
         want_p = run(obs_p, w, b, eps_p, seed, legal_p)
         out = _fresh(Mp)
-        rig.call(obs_p, w, b, legal_p, eps_p, {k: t.data_ptr() for k, t in out.items()}, seed)
+        rig.call(obs_p, w, b, {k: t.data_ptr() for k, t in out.items()}, seed,
+                 sides=dict(epsilon=eps_p, **({} if legal_p is None else dict(mask=legal_p))))
         torch.cuda.synchronize()
         same([out["actions"], out["q"].view(torch.float32), out["q_max"].view(torch.float32)], want_p, ("pushed", it))
     assert rig.statuses() == [0] * rig.n
@@ -363,10 +314,11 @@ def test_writes_stay_inside_the_outputs(K, head, form, M, chunk, d_out):
     out = {name: buf.ptr() for name, buf in bufs.items()}
     with tuning(chunk):
         if form == "pushed":
-            rig = EpsPushRig(K, M, 256, 1024, d_out, 512, head)
+            masked = [("mask", d_out)] if legal is not None else []
+            rig = PushRig(K, M, 256, 1024, 512, "ce", head, sides=masked + [("epsilon", 4)])
+            sides = dict(epsilon=geps.view(torch.float32), **({} if legal is None else dict(mask=gmask.view())))
             for _ in range(3):
-                rig.call(obs, w, b, None if legal is None else gmask.view().view(torch.bool).view(M, d_out),
-                         geps.view(torch.float32), out, seed)
+                rig.call(obs, w, b, out, seed, sides=sides)
             torch.cuda.synchronize()
             assert rig.statuses() == [0] * rig.n
             bufs.update({f"stage[{r}]": rig.stage[r] for r in range(1, rig.n)})

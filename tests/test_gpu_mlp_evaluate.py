@@ -14,7 +14,7 @@ import torch
 from conftest import mapped_copy
 from kubetorch_b200.device import lib as L
 from kubetorch_b200.device import mlp
-from mlp_rig import (SHIPPED_CHUNK, Guarded, Head, K, config, deployed, entry_args,  # noqa: F401
+from mlp_rig import (SHIPPED_CHUNK, Guarded, Head, K, PushRig, config, deployed, entry_args,  # noqa: F401
                      expect_status, from_row, named_args, plain, pushed, randn, stream, tuning)
 
 pytestmark = pytest.mark.gpu
@@ -280,64 +280,6 @@ def test_gaussian_round_trip_and_values(K, d_out):
 
 
 # ---- 6. forms, chunkings and row splits ---------------------------------------------------------------------------------
-class EvalPushRig:
-    """What mlp._mlp_scatter_gather_pushed does for an evaluating head, on ranks [0, 0, 0] of cuda:0 and ONE stream:
-    ktb_push_scatter_ce_sides pushes each rank's rows, mask rows (masked heads) and actions into its guarded staging
-    half, laid out rows | mask | taken (taken 8-byte aligned); the pushed entry runs on ranks 1.. and the plain entry
-    on the root's shard."""
-
-    def __init__(self, K, M, d_out, taken_row, head, masked, chunk_rows=512, n_ranks=3):
-        self.d_out, self.head, self.masked, self.n, self.chunk_rows = d_out, head, masked, n_ranks, chunk_rows
-        self.taken_row = taken_row
-        self.bounds = [K.shard_bounds(M, n_ranks, r) for r in range(n_ranks)]
-        shard = max(e - b for b, e in self.bounds)
-        self.mask_offset = (shard * 256 * 2 + 255) // 256 * 256
-        end = self.mask_offset + shard * d_out if masked else self.mask_offset
-        self.taken_offset = (end + 7) // 8 * 8
-        self.stride = (self.taken_offset + shard * taken_row + 255) // 256 * 256
-        self.ctrl = [torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda")
-                     for _ in range(n_ranks)]
-        self.stage = [None] + [Guarded(2 * self.stride) for _ in range(1, n_ranks)]
-        self.scratch = [None] + [Guarded(mlp.pushed_scratch_bytes(e - b, 1024, chunk_rows)) for b, e in self.bounds[1:]]
-        torch.cuda.synchronize()
-        self.seq = 0
-
-    def call(self, obs, w, b, legal, taken, out, **more):
-        self.seq += 1
-        seq, n, st = self.seq, self.n, stream()
-        stage_ptrs = L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in self.stage[1:]])
-        ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
-        root = self.ctrl[0].data_ptr()
-        sides = ([(legal.data_ptr(), self.d_out, self.mask_offset)] if self.masked else []) + \
-            [(taken.data_ptr(), self.taken_row, self.taken_offset)]
-        src, row_bytes, offsets = zip(*sides)
-        L.call("ktb_push_scatter_ce_sides", 0, obs.data_ptr(), obs.numel(), 256, L.BF16, n, 0,
-               L.arr(ctypes.c_int, [0] * n), stage_ptrs, self.stride, ctrl_ptrs, root, self.chunk_rows * 256,
-               len(sides), L.arr(ctypes.c_void_p, src), L.arr(ctypes.c_size_t, row_bytes),
-               L.arr(ctypes.c_size_t, offsets), seq, st)
-        a = named_args(obs, w, b, out, **more)
-        for r in range(1, n):
-            lo, hi = self.bounds[r]
-            L.call(*entry_args(self.head, dict(
-                from_row(self.head, a, lo), M=hi - lo, mask=self.mask_offset, taken=self.taken_offset,
-                stage=self.stage[r].ptr(), stride=self.stride, scratch=self.scratch[r].ptr(),
-                ctrl=self.ctrl[r].data_ptr(), ctrl_root=root, rank=r, chunk_rows=self.chunk_rows, seq=seq), push=True))
-        lo, hi = self.bounds[0]
-        scratch = mlp._scratch_for(0, hi - lo, 1024)
-        L.call(*entry_args(self.head, dict(from_row(self.head, a, lo), M=hi - lo, obs=a["obs"] + lo * 512,
-                                           mask=0 if legal is None else legal.data_ptr() + lo * self.d_out,
-                                           taken=taken.data_ptr() + lo * self.taken_row, scratch=scratch.data_ptr())))
-        L.call("ktb_push_wait", 0, root, n, 0, seq, st)
-
-    def statuses(self):
-        out = []
-        for c in self.ctrl:
-            s = ctypes.c_uint(0)
-            L.call("ktb_push_status", 0, c.data_ptr(), ctypes.byref(s))
-            out.append(s.value)
-        return out
-
-
 def _fresh(M, valued):
     return {k: torch.full((M,), -1, dtype=torch.int32, device="cuda").view(torch.float32)
             for k in ("log_probs", "entropy") + (("values",) if valued else ())}
@@ -382,7 +324,8 @@ def test_every_form_chunking_and_row_split_gives_identical_bits(K, kind, d_out):
     assert torch.equal(taken, keep)
     Mp = 3 * 1408
     taken_row = taken[0].numel() * taken.element_size()
-    rig = EvalPushRig(K, Mp, d_out, taken_row, head, legal is not None)
+    masked = [("mask", d_out)] if legal is not None else []
+    rig = PushRig(K, Mp, 256, 1024, 512, "ce", head, sides=masked + [("taken", taken_row)])
     w3v, b3v = mlp._stacked_head(w[2], b[2], *value)
     wv = (w[0], w[1], w3v)
     bv = (b[0], b[1], b3v)
@@ -392,8 +335,8 @@ def test_every_form_chunking_and_row_split_gives_identical_bits(K, kind, d_out):
         want_p = run(obs_p, taken_p, legal_p)
         out = _fresh(Mp, True)
         groups = {} if nvec is None else dict(nvec=L.arr(ctypes.c_int32, nvec), n_groups=len(nvec))
-        rig.call(obs_p, wv, bv, legal_p, taken_p, {k: t.data_ptr() for k, t in out.items()},
-                 d_out=d_out, log_std=ls, **groups)
+        rig.call(obs_p, wv, bv, {k: t.data_ptr() for k, t in out.items()}, log_std=ls,
+                 sides=dict(taken=taken_p, **({} if legal_p is None else dict(mask=legal_p))), d_out=d_out, **groups)
         torch.cuda.synchronize()
         same([out["log_probs"], out["entropy"], out["values"]], want_p, ("rig", it))
         devs = [0, 0, 0]
@@ -435,9 +378,12 @@ def test_writes_stay_inside_the_outputs(K, kind, form, M, chunk, d_out):
     more = dict(d_out=d_out, log_std=ls, **groups)
     with tuning(chunk):
         if form == "pushed":
-            rig = EvalPushRig(K, M, d_out, taken[0].numel() * taken.element_size(), head, legal is not None)
+            masked = [("mask", d_out)] if legal is not None else []
+            rig = PushRig(K, M, 256, 1024, 512, "ce", head,
+                          sides=masked + [("taken", taken[0].numel() * taken.element_size())])
+            sides = dict(taken=gt.view(taken.dtype), **({} if legal is None else dict(mask=legal)))
             for _ in range(3):
-                rig.call(obs, wv, bv, legal, gt.view(taken.dtype).view(taken.shape), out, **more)
+                rig.call(obs, wv, bv, out, sides=sides, **more)
             torch.cuda.synchronize()
             assert rig.statuses() == [0] * rig.n
             bufs.update({f"stage[{r}]": rig.stage[r] for r in range(1, rig.n)})

@@ -228,51 +228,6 @@ def test_all_true_mask_gives_the_unmasked_bits(K, d_out):
 
 
 # ---- 6. forms --------------------------------------------------------------------------------------------------------------
-class MaskedPushRig(PushRig):
-    """What mlp._mlp_scatter_gather_pushed does for a masked head, on ranks [0, 0, 0] of cuda:0 and ONE stream: the
-    copy-engine scatter pushes each rank's rows and mask rows into its guarded staging half (mask 256-byte aligned
-    after the largest shard's rows), the head's masked pushed entry runs on ranks 1.. and its plain entry on the root's
-    shard."""
-
-    def __init__(self, K, M, d_in, d_hidden, d_out, chunk_rows, head, n_ranks=3):
-        self.d_in, self.d_hidden, self.d_out, self.chunk_rows, self.head, self.n = \
-            d_in, d_hidden, d_out, chunk_rows, head, n_ranks
-        self.bounds = [K.shard_bounds(M, n_ranks, r) for r in range(n_ranks)]
-        shard = max(e - b for b, e in self.bounds)
-        self.mask_offset = (shard * d_in * 2 + 255) // 256 * 256
-        self.stride = (self.mask_offset + shard * d_out + 255) // 256 * 256
-        self.ctrl = [torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda")
-                     for _ in range(n_ranks)]
-        self.stage = [None] + [Guarded(2 * self.stride) for _ in range(1, n_ranks)]
-        self.scratch = [None] + [Guarded(mlp.pushed_scratch_bytes(e - b, d_hidden, chunk_rows))
-                                 for b, e in self.bounds[1:]]
-        torch.cuda.synchronize()
-        self.seq = 0
-
-    def call(self, obs, w, b, legal, out, seed=0):
-        self.seq += 1
-        seq, n, d_in, d_out, st = self.seq, self.n, self.d_in, self.d_out, stream()
-        stage_ptrs = L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in self.stage[1:]])
-        ctrl_ptrs = L.arr(ctypes.c_void_p, [c.data_ptr() for c in self.ctrl])
-        root = self.ctrl[0].data_ptr()
-        L.call("ktb_push_scatter_ce_masked", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
-               L.arr(ctypes.c_int, [0] * n), stage_ptrs, self.stride, ctrl_ptrs, root, self.chunk_rows * d_in,
-               legal.data_ptr(), d_out, self.mask_offset, seq, st)
-        a = named_args(obs, w, b, out, seed)
-        for r in range(1, n):
-            lo, hi = self.bounds[r]
-            L.call(*entry_args(self.head, dict(
-                from_row(self.head, a, lo), M=hi - lo, mask=self.mask_offset, stage=self.stage[r].ptr(),
-                stride=self.stride, scratch=self.scratch[r].ptr(), ctrl=self.ctrl[r].data_ptr(), ctrl_root=root,
-                rank=r, chunk_rows=self.chunk_rows, seq=seq), push=True))
-        lo, hi = self.bounds[0]
-        scratch = mlp._scratch_for(0, hi - lo, self.d_hidden)
-        L.call(*entry_args(self.head, dict(from_row(self.head, a, lo), M=hi - lo, obs=a["obs"] + lo * d_in * 2,
-                                           mask=legal.data_ptr() + lo * d_out, scratch=scratch.data_ptr())))
-        L.call("ktb_push_wait", 0, root, n, 0, seq, st)
-
-
-
 def _outputs(head, M, d_out):
     if head is MASKED_GREEDY:
         return {"logits": torch.full((M, d_out), -1, dtype=torch.int16, device="cuda"),
@@ -317,14 +272,14 @@ def test_every_form_chunking_and_row_split_gives_identical_bits(K, head, d_out):
         _same({k: torch.cat([lo[k], hi[k]]) for k in want}, want, split)
     assert torch.equal(legal, keep)
     Mp = 3 * 1408
-    rig = MaskedPushRig(K, Mp, 256, 1024, d_out, 512, head)
+    rig = PushRig(K, Mp, 256, 1024, 512, "ce", head, sides=[("mask", d_out)])
     for it in range(3):
         obs_p = randn((Mp, 256), 1410 + it)
         legal_p = random_legal(Mp, d_out, 1420 + it)
         keep_p = legal_p.clone()
         want_p = _want(head, obs_p, w, b, legal_p, seed)
         out = _outputs(head, Mp, d_out)
-        rig.call(obs_p, w, b, legal_p, {k: t.data_ptr() for k, t in out.items()}, seed)
+        rig.call(obs_p, w, b, {k: t.data_ptr() for k, t in out.items()}, seed, sides={"mask": legal_p})
         torch.cuda.synchronize()
         _same(out, want_p, ("pushed", it))
         assert torch.equal(legal_p, keep_p)
@@ -377,9 +332,9 @@ def test_writes_stay_inside_the_outputs(K, head, form, M, chunk, d_out):
     out = {name: buf.ptr() for name, buf in bufs.items()}
     with tuning(chunk):
         if form == "pushed":
-            rig = MaskedPushRig(K, M, 256, 1024, d_out, 512, head)
+            rig = PushRig(K, M, 256, 1024, 512, "ce", head, sides=[("mask", d_out)])
             for _ in range(3):
-                rig.call(obs, w, b, gmask.view().view(torch.bool).view(M, d_out), out, seed)
+                rig.call(obs, w, b, out, seed, sides={"mask": gmask.view()})
             torch.cuda.synchronize()
             assert rig.statuses() == [0] * rig.n
             bufs.update({f"stage[{r}]": rig.stage[r] for r in range(1, rig.n)})

@@ -12,7 +12,7 @@ import torch
 
 from kubetorch_b200.device import lib as L
 from kubetorch_b200.device import mlp
-from mlp_rig import K, Guarded, deployed, expect_status, stream, tuning  # noqa: F401
+from mlp_rig import K, Guarded, PushRig, deployed, expect_status, stream, tuning  # noqa: F401
 from oracle import ref_dispatch
 from policy_td_target_cases import header_y, mlp_ddpg_target, mlp_sac_target, mlp_td3_target
 
@@ -146,56 +146,38 @@ def test_special_values_follow_the_header(K, name, case):
         assert bool(y[1::3].isnan().all()) and bool((y[0::3] == math.inf).all())
 
 
-def _push_call(obs, c1, kw, chunk_rows, n):
-    """The pushed forms as a PushSession runs them, ranks [0] * n on cuda:0 and one stream: the rows, reward and done
-    pushed by ktb_push_scatter_ce_sides (each staging half rows | reward | done), ranks 1.. on the _pushed entry, the
-    root's shard on the plain one through mlp_forward.  Staging halves and scratch are guarded."""
+def _push_call(K, obs, c1, kw, chunk_rows, n):
+    """The pushed forms through the push rig, ranks [0] * n on cuda:0 and one stream, reward and done side inputs
+    beside the rows: ranks 1.. on the _pushed entry, the root's shard on the plain one through mlp_forward."""
     M, d_in = obs.shape
     policy, gaussian = kw["policy"], kw["policy"] == "gaussian"
     a = list(kw["actor"])
     if gaussian:
         a[4], a[5] = mlp._stacked_head(a[4], a[5], None, None, *kw["log_std"])
     d_act, d_ha, d_h = a[4].shape[0] // (2 if gaussian else 1), a[0].shape[0], c1[0].shape[0]
-    bounds = [mlp.ops.shard_bounds(M, n, r) for r in range(n)]
-    shard = max(e - b for b, e in bounds)
-    r_off = (shard * d_in * 2 + 255) // 256 * 256
-    d_off = r_off + (shard * 4 + 255) // 256 * 256
-    stride = (d_off + shard * 4 + 255) // 256 * 256
-    ctrl = [torch.zeros(L.load().ktb_push_control_bytes(), dtype=torch.uint8, device="cuda") for _ in range(n)]
-    stage = [None] + [Guarded(2 * stride) for _ in range(1, n)]
-    scratch = [None] + [Guarded(mlp.pushed_td_scratch_bytes(e - b, d_ha, d_h, d_act, chunk_rows)) for b, e in bounds[1:]]
+    rig = PushRig(K, M, d_in, d_h, chunk_rows, "ce", n_ranks=n, sides=[("reward", 4), ("done", 4)],
+                  scratch_bytes=lambda rows: mlp.pushed_td_scratch_bytes(rows, d_ha, d_h, d_act, chunk_rows))
     y = torch.full((M,), 7.0, device="cuda")
     ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
     crit = [ptr(t) for t in (mlp._padded_w1(c1[0], d_in),) + c1[1:]]
     tw = kw["twin"]
     twin = [ptr(t) for t in (mlp._padded_w1(tw[0], d_in),) + tuple(tw[1:])] if tw else [0] * 6
-    st = stream()
-    root = ctrl[0].data_ptr()
-    for seq in (1, 2):
-        L.call("ktb_push_scatter_ce_sides", 0, obs.data_ptr(), obs.numel(), d_in, L.BF16, n, 0,
-               L.arr(ctypes.c_int, [0] * n), L.arr(ctypes.c_void_p, [0] + [s.ptr() for s in stage[1:]]), stride,
-               L.arr(ctypes.c_void_p, [t.data_ptr() for t in ctrl]), root, chunk_rows * d_in, 2,
-               L.arr(ctypes.c_void_p, [kw["reward"].data_ptr(), kw["done"].data_ptr()]),
-               L.arr(ctypes.c_size_t, [4, 4]), L.arr(ctypes.c_size_t, [r_off, d_off]), seq, st)
-        for r in range(1, n):
-            b, e = bounds[r]
-            args = mlp._td_args(policy, kw.get("seed"), kw.get("log_std"), kw.get("log_std_bounds"), kw.get("squash"),
-                                kw.get("noise"), kw.get("noise_clip"), b)
-            L.call("ktb_mlp_bf16_td_target_" + policy + "_pushed", 0, stage[r].ptr(), stride, e - b, d_in, d_h, d_act,
-                   *crit, *twin, d_ha, *[ptr(t) for t in a], *args, r_off, d_off, float(kw["gamma"]),
-                   *((float(kw["alpha"]),) if gaussian else ()), y.data_ptr() + 4 * b, scratch[r].ptr(),
-                   ctrl[r].data_ptr(), root, r, chunk_rows, seq, st)
-        b, e = bounds[0]
+
+    def rank(r, b, e, p):
+        args = mlp._td_args(policy, kw.get("seed"), kw.get("log_std"), kw.get("log_std_bounds"), kw.get("squash"),
+                            kw.get("noise"), kw.get("noise_clip"), b)
+        L.call("ktb_mlp_bf16_td_target_" + policy + "_pushed", 0, p["stage"], p["stride"], e - b, d_in, d_h, d_act,
+               *crit, *twin, d_ha, *[ptr(t) for t in a], *args, p["reward"], p["done"], float(kw["gamma"]),
+               *((float(kw["alpha"]),) if gaussian else ()), y.data_ptr() + 4 * b, p["scratch"], p["ctrl"],
+               p["ctrl_root"], r, chunk_rows, p["seq"], stream())
+
+    def root(b, e, rows):
         sub = dict(kw, reward=kw["reward"][b:e], done=kw["done"][b:e], target=y[b:e], row_offset=b)
         _fused(obs[b:e], c1, dict(sub, stream=torch.cuda.current_stream()))
-        L.call("ktb_push_wait", 0, root, n, 0, seq, st)
-    torch.cuda.synchronize()
-    for r in range(1, n):
-        s = ctypes.c_uint(0)
-        L.call("ktb_push_status", 0, ctrl[r].data_ptr(), ctypes.byref(s))
-        assert s.value == 0
-        stage[r].check(f"stage[{r}]")
-        scratch[r].check(f"scratch[{r}]")
+
+    for _ in (1, 2):
+        rig.push(obs, {"reward": kw["reward"], "done": kw["done"]}, rank, root)
+    rig.check()
     return y
 
 
@@ -213,7 +195,7 @@ def test_every_form_gives_the_same_bits(K, name, chunk, ranks):
         staged = _fused(obs, c1, dict(kw, staged=True))
         split = torch.cat([_fused(obs[b:e], c1, dict(kw, reward=r[b:e], done=d[b:e], row_offset=b))
                            for b, e in ((0, 384), (384, 1000), (1000, M))])
-        pushed = _push_call(obs, c1, kw, chunk or 16896, ranks)
+        pushed = _push_call(K, obs, c1, kw, chunk or 16896, ranks)
     same(plain, _composed(obs, c1, kw), "composed")
     for what, got in (("staged", staged), ("split", split), ("pushed", pushed)):
         same(got, plain, what)
@@ -230,6 +212,34 @@ def test_pull_scatter_gather_over_uneven_and_empty_shards(K, name, M):
     torch.cuda.synchronize()
     want = _fused(obs, c1, dict(kw, biases=(c1[1], c1[3], c1[5])))
     same(torch.cat(got), want, M)
+
+
+@pytest.mark.parametrize("name", ["td3", "ddpg", "sac"])
+def test_package_push_path_on_one_gpu_matches_plain_bits(K, name):
+    """mlp_scatter_gather's pushed form (the rows, reward and done pushed into each staging half, the root's shard on
+    the side stream) with ranks [0, 0, 0] on cuda:0, back to back with fresh inputs: equal to one plain call over all
+    rows."""
+    devs, M, d_in = [0, 0, 0], 3 * 1280, 128
+    bounds = [K.shard_bounds(M, 3, r) for r in range(3)]
+    c1, c2, actor, ls = _nets(d_in, 17, 512, 256, True, 4)
+    policy, opts, twin, alpha = POLICIES[name]
+    gaussian = policy == "gaussian"
+    a = (*actor[:4], *mlp._stacked_head(actor[4], actor[5], None, None, *ls)) if gaussian else actor
+    weights = {0: (mlp._padded_w1(c1[0], d_in), c1[2], c1[4], c1[1], c1[3], c1[5])}
+    tw = {0: (mlp._padded_w1(c2[0], d_in), *c2[1:])} if twin else None
+    std = mlp._std(ls, None, opts.get("squash")) if gaussian else None
+    det = None if gaussian else dict(noise=opts.get("noise"), noise_clip=opts.get("noise_clip"),
+                                     squash=opts.get("squash"))
+    for it in range(3):
+        obs, r, d = _inputs(M, d_in, seed=20 + it)
+        want = _fused(obs, c1, _kw(name, c1, c2, actor, ls, r, d))
+        y = torch.full((M,), 7.0, device="cuda")
+        mlp._mlp_scatter_gather_pushed(obs, devs, bounds, weights, "td_target", y, None, None, opts.get("seed"),
+                                       {0: ls} if gaussian else None, std=std, det=det, twin=tw,
+                                       td=({0: a}, policy, r, d, 0.99, alpha))
+        torch.cuda.synchronize()
+        same(y, want, (name, it))
+    mlp._push_sessions[tuple(devs)].check()
 
 
 @pytest.mark.parametrize("name", ["td3", "ddpg", "sac"])
@@ -317,7 +327,7 @@ def test_policy_statuses(K, policy, over):
 
 @pytest.mark.parametrize("policy", ["deterministic", "gaussian"])
 @pytest.mark.parametrize("case,over,status", [
-    ("d_act_first", dict(d_act=65, r_off=2), L.ERR_UNSUPPORTED),
+    ("region_before_d_act", dict(d_act=65, r_off=2), L.ERR_ARG),
     ("gamma_first", dict(gamma=math.nan, r_off=2), L.ERR_ARG),
     ("reward_overlaps_rows", dict(r_off=256 * 256 * 2 - 4), L.ERR_ARG),
     ("done_past_stride", dict(d_off=(1 << 20) - 4), L.ERR_ARG),
