@@ -21,8 +21,7 @@ import torch
 from . import lib as L
 from . import ops
 from ..mapped import MLP_OUTPUTS as OUTPUTS
-from ..mapped import EVALUATE_OUTPUTS, check_nvec
-from ..sampling import _check_seed
+from ..mapped import CONSTANT_CHECKS, EVALUATE_OUTPUTS, TD_OPTIONS, check_mlp_options, check_mlp_rules, check_nvec
 
 _scratch = {}
 _stage = {}
@@ -78,12 +77,9 @@ MAX_D_OUT = 256
 LOG_STD_BOUNDS = (-20.0, 2.0)   # SB3's and Spinning Up's clamp of a SAC actor's log-std
 
 
-def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
-    """_check_policy's checks of a value head (wv, bv), in this order: the output, the pair, the head width, bv given
-    exactly when b3 is, then wv's dtype and shape, layout and device, then bv."""
-    if output not in ("sample", "gaussian") + EVALUATE_OUTPUTS:
-        raise ValueError(f'value is an argument of output="sample" and "gaussian" (and "evaluate" and '
-                         f'"gaussian_evaluate"), not of output={output!r}')
+def _check_value(value, w3, b3, d_hidden, d_out) -> None:
+    """_check_policy's checks of a value head (wv, bv), in this order: the pair, the head width, bv given exactly when
+    b3 is, then wv's dtype and shape, layout and device, then bv."""
     if not isinstance(value, (tuple, list)) or len(value) != 2:
         raise ValueError("value must be (wv, bv): the critic's weight [1, d_hidden] and its bias [1] or None")
     wv, bv = value
@@ -105,10 +101,10 @@ def _check_value(value, output, w3, b3, d_hidden, d_out) -> None:
                          f"({w3.device})")
 
 
-def _check_state_std(log_std, log_std_bounds, squash, w3, b3, d_hidden, d_out, valued) -> None:
+def _check_state_std(log_std, w3, b3, d_hidden, d_out, valued) -> None:
     """_check_policy's checks of a state-dependent log-std head log_std = (w_ls, b_ls), in this order: the pair, the
     head width (2·d_out columns, one more with a value head, in one 256-wide tile), b_ls given exactly when b3 is,
-    w_ls's dtype and shape, layout and device, b_ls, then the bounds and squash."""
+    w_ls's dtype and shape, layout and device, then b_ls."""
     if len(log_std) != 2:
         raise ValueError("log_std must be a tensor or (w_ls, b_ls): the log-std head's weight [d_out, d_hidden] and "
                          "its bias [d_out] or None")
@@ -130,47 +126,26 @@ def _check_state_std(log_std, log_std_bounds, squash, w3, b3, d_hidden, d_out, v
                              or tuple(b_ls.shape) != (d_out,) or not b_ls.is_contiguous() or b_ls.device != w3.device):
         raise ValueError(f"log_std: b_ls must be a contiguous bfloat16 tensor of shape ({d_out},) on the device of w3 "
                          f"({w3.device})")
-    if log_std_bounds is not None:
-        if not isinstance(log_std_bounds, (tuple, list)) or len(log_std_bounds) != 2 or \
-                not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in log_std_bounds):
-            raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {log_std_bounds!r}")
-        lo, hi = (float(b) for b in log_std_bounds)
-        if lo != lo or hi != hi:
-            raise ValueError(f"log_std_bounds must not be NaN, got {log_std_bounds!r}")
-        if lo > hi:
-            raise ValueError(f"log_std_bounds must have low <= high, got {log_std_bounds!r}")
-    if squash is not None and not isinstance(squash, bool):
-        raise ValueError(f"squash must be True or False, got {squash!r}")
 
 
 def _check_epsilon(epsilon, obs) -> None:
-    """_check_policy's checks of output="epsilon_greedy"'s epsilon: given; a number (not a bool) that is not NaN, or a
-    contiguous CUDA float32 tensor [M] on the device of obs [M, d_in]."""
-    if epsilon is None:
-        raise ValueError('epsilon is required with output="epsilon_greedy": a float or a float32 tensor [M]')
-    if isinstance(epsilon, torch.Tensor):
-        if not isinstance(obs, torch.Tensor):
-            raise ValueError("an epsilon tensor is checked against obs: pass the obs [M, d_in] it goes with")
-        if epsilon.dtype != torch.float32 or tuple(epsilon.shape) != (obs.shape[0],):
-            raise ValueError(f"epsilon must be a float32 tensor of shape ({obs.shape[0]},), got {epsilon.dtype} "
-                             f"{tuple(epsilon.shape)}")
-        if not epsilon.is_contiguous():
-            raise ValueError("epsilon must be contiguous")
-        if not epsilon.is_cuda or epsilon.device != obs.device:
-            raise ValueError(f"epsilon must be a CUDA tensor on the device of obs ({obs.device}), got {epsilon.device}")
-        return
-    if isinstance(epsilon, bool) or not isinstance(epsilon, (int, float)):
-        raise ValueError(f"epsilon must be a float or a float32 tensor [M], got {epsilon!r}")
-    if math.isnan(epsilon):
-        raise ValueError("epsilon must not be NaN (a NaN float never explores: pass 0.0 for that)")
+    """_check_policy's checks of an epsilon tensor: a contiguous CUDA float32 tensor [M] on the device of obs [M,
+    d_in]."""
+    if not isinstance(obs, torch.Tensor):
+        raise ValueError("an epsilon tensor is checked against obs: pass the obs [M, d_in] it goes with")
+    if epsilon.dtype != torch.float32 or tuple(epsilon.shape) != (obs.shape[0],):
+        raise ValueError(f"epsilon must be a float32 tensor of shape ({obs.shape[0]},), got {epsilon.dtype} "
+                         f"{tuple(epsilon.shape)}")
+    if not epsilon.is_contiguous():
+        raise ValueError("epsilon must be contiguous")
+    if not epsilon.is_cuda or epsilon.device != obs.device:
+        raise ValueError(f"epsilon must be a CUDA tensor on the device of obs ({obs.device}), got {epsilon.device}")
 
 
 def _check_taken(taken, output, obs, d_out, nvec) -> None:
-    """_check_policy's checks of an evaluate output's given actions `taken`, in this order: given; the dtype and shape
-    (int64 [M], [M, len(nvec)] with nvec, for "evaluate"; float32 [M, d_out] for "gaussian_evaluate"; obs [M, d_in]);
-    contiguous; a CUDA tensor on the device of obs."""
-    if taken is None:
-        raise ValueError(f"taken is required with output={output!r}: the actions to evaluate")
+    """_check_policy's checks of an evaluate output's given actions `taken`, in this order: a tensor; the dtype and
+    shape (int64 [M], [M, len(nvec)] with nvec, for "evaluate"; float32 [M, d_out] for "gaussian_evaluate"; obs [M,
+    d_in]); contiguous; a CUDA tensor on the device of obs."""
     if not isinstance(taken, torch.Tensor):
         raise ValueError(f"taken must be a tensor, got {type(taken).__name__}")
     if not isinstance(obs, torch.Tensor):
@@ -189,40 +164,15 @@ def _check_taken(taken, output, obs, d_out, nvec) -> None:
         raise ValueError(f"taken must be a CUDA tensor on the device of obs ({obs.device}), got {taken.device}")
 
 
-def _check_deterministic(seed, noise, noise_clip, squash) -> None:
-    """_check_policy's checks of output="deterministic"'s own options, in this order: a seed exactly when noise is
-    given (then _check_seed), noise_clip with noise only, noise and noise_clip numbers (not bools) >= 0 and not NaN,
-    squash True or False."""
-    if (noise is None) != (seed is None):
-        raise ValueError('output="deterministic" takes a seed exactly when it takes noise: the noise-free actor draws '
-                         'nothing')
-    if noise_clip is not None and noise is None:
-        raise ValueError("noise_clip is an option of noise only: it clips the noise")
-    if seed is not None:
-        _check_seed(seed)
-    for name, v in (("noise", noise), ("noise_clip", noise_clip)):
-        if v is None:
-            continue
-        if isinstance(v, bool) or not isinstance(v, (int, float)):
-            raise ValueError(f"{name} must be a number, got {v!r}")
-        if v != v or v < 0:
-            raise ValueError(f"{name} must be >= 0 and not NaN, got {v!r}")
-    if squash is not None and not isinstance(squash, bool):
-        raise ValueError(f"squash must be True or False, got {squash!r}")
-
-
 MAX_D_ACT = 64   # a critic's actions fill one 64-wide K block of layer 1
 
 
 def _check_critic(w1, w2, w3, biases, obs, action, twin) -> None:
-    """_check_policy's checks of output="critic", after its refusals, in this order: w3 one row; action given, an fp32
-    [M, d_act] CUDA tensor, contiguous, on the device of obs [M, d_in], with 1 <= d_act <= 64; w1 [d_hidden, d_in +
-    d_act]; then twin = (w1, b1, w2, b2, w3, b3) of the second critic: six entries, biases given exactly as the first
-    critic's, each weight a contiguous CUDA bfloat16 tensor of the first's shape on the device of w1."""
+    """_check_policy's checks of output="critic", in this order: w3 one row; action an fp32 [M, d_act] CUDA tensor,
+    contiguous, on the device of obs [M, d_in], with 1 <= d_act <= 64; w1 [d_hidden, d_in + d_act]; then twin = (w1,
+    b1, w2, b2, w3, b3) of the second critic (_check_twin)."""
     if w3.shape[0] != 1:
         raise ValueError(f"d_out={w3.shape[0]}: a critic's w3 is [1, d_hidden] (one Q-value per row)")
-    if action is None:
-        raise ValueError('action is required with output="critic": the fp32 actions [M, d_act] it evaluates')
     if not isinstance(action, torch.Tensor) or action.dtype != torch.float32 or action.dim() != 2:
         raise ValueError("action must be a 2-D float32 tensor [M, d_act]")
     if not isinstance(obs, torch.Tensor):
@@ -285,38 +235,12 @@ def _check_twin(twin, w1, w2, w3, biases) -> None:
                              f"the device of w1 ({w1.device})")
 
 
-TD_POLICIES = ("deterministic", "gaussian")
-
-
-def _check_td_target(w1, w2, w3, biases, obs, twin, seed, log_std, log_std_bounds, squash, noise, noise_clip, actor,
-                     policy, reward, done, gamma, alpha) -> None:
-    """_check_policy's checks of output="td_target", after its refusals, in this order: policy; the policy's options
-    (noise, noise_clip, seed and squash with "deterministic", which refuses log_std, log_std_bounds and alpha; a seed,
-    alpha and the pair log_std = (w_ls, b_ls) with "gaussian", which refuses noise and noise_clip); actor = (w1, b1,
-    w2, b2, w3, b3): six entries, biases given exactly as the critic's, contiguous CUDA bfloat16 on the device of w1,
-    w1 [d_ha, d_in], w2 [d_ha, d_ha], w3 [d_act, d_ha] with 1 <= d_act <= 64; the critic's w3 one row and w1 [d_hidden,
-    d_in + d_act]; the twin; the log-std head against the actor; reward and done fp32 [M] or [M, 1] of one shape,
-    contiguous, on the device of obs [M, d_in]; gamma and alpha finite numbers."""
-    if policy not in TD_POLICIES:
-        raise ValueError(f'policy must be one of {TD_POLICIES} with output="td_target" (the actor of the next '
-                         f'actions), got {policy!r}')
-    if policy == "deterministic":
-        for name, v in (("log_std", log_std), ("log_std_bounds", log_std_bounds), ("alpha", alpha)):
-            if v is not None:
-                raise ValueError(f'{name} is not an argument of policy="deterministic": TD3 and DDPG targets take '
-                                 f'noise, noise_clip, seed and squash, and no entropy term')
-        _check_deterministic(seed, noise, noise_clip, squash)
-    else:
-        for name, v in (("noise", noise), ("noise_clip", noise_clip)):
-            if v is not None:
-                raise ValueError(f'{name} is not an argument of policy="gaussian": SAC\'s next actions are sampled '
-                                 f'with the log-std head, not with added noise')
-        _check_seed(seed)
-        if alpha is None:
-            raise ValueError('alpha is required with policy="gaussian": the entropy coefficient of SAC\'s target')
-        if not isinstance(log_std, (tuple, list)):
-            raise ValueError('log_std=(w_ls, b_ls) is required with policy="gaussian": the actor\'s state-dependent '
-                             'log-std head')
+def _check_td_target(w1, w2, w3, biases, obs, twin, log_std, actor, reward, done) -> None:
+    """_check_policy's checks of output="td_target"'s tensors, in this order: actor = (w1, b1, w2, b2, w3, b3): six
+    entries, biases given exactly as the critic's, contiguous CUDA bfloat16 on the device of w1, w1 [d_ha, d_in], w2
+    [d_ha, d_ha], w3 [d_act, d_ha] with 1 <= d_act <= 64; the critic's w3 one row and w1 [d_hidden, d_in + d_act]; the
+    twin; with a log_std = (w_ls, b_ls) pair the log-std head against the actor; reward and done fp32 [M] or [M, 1] of
+    one shape, contiguous, on the device of obs [M, d_in]."""
     if not isinstance(actor, (tuple, list)) or len(actor) != 6:
         raise ValueError("actor must be (w1, b1, w2, b2, w3, b3) of the actor (biases None without biases)")
     for name, t, mine in zip(("b1", "b2", "b3"), actor[1::2], biases):
@@ -346,8 +270,8 @@ def _check_td_target(w1, w2, w3, biases, obs, twin, seed, log_std, log_std_bound
                          f"1 over torch.cat([next_obs, actor(next_obs)], -1)), got {tuple(w1.shape)}")
     if twin is not None:
         _check_twin(twin, w1, w2, w3, biases)
-    if policy == "gaussian":
-        _check_state_std(log_std, log_std_bounds, squash, aw3, actor[5], d_ha, d_act, False)
+    if log_std is not None:
+        _check_state_std(log_std, aw3, actor[5], d_ha, d_act, False)
     for name, t in (("reward", reward), ("done", done)):
         if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) not in ((M,), (M, 1)):
             raise ValueError(f"{name} must be a float32 tensor of shape ({M},) or ({M}, 1), got "
@@ -358,110 +282,55 @@ def _check_td_target(w1, w2, w3, biases, obs, twin, seed, log_std, log_std_bound
             raise ValueError(f"{name} must be a CUDA tensor on the device of obs ({obs.device}), got {t.device}")
     if reward.shape != done.shape:
         raise ValueError(f"reward and done must have one shape, got {tuple(reward.shape)} and {tuple(done.shape)}")
-    for name, v in (("gamma", gamma), ("alpha", alpha)):
-        if v is None and name == "alpha":
-            continue
-        if isinstance(v, bool) or not isinstance(v, (int, float)):
-            raise ValueError(f"{name} must be a number, got {v!r}")
-        if not math.isfinite(v):
-            raise ValueError(f"{name} must be finite, got {v!r}")
+
+
+_ARGUMENTS = ("seed", "log_std", "mask", "value", "nvec", "log_std_bounds", "squash", "epsilon", "taken", "noise",
+              "noise_clip", "action", "twin") + TD_OPTIONS   # _check_policy's options, td's last
 
 
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
                   nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None, noise=None,
                   noise_clip=None, action=None, twin=None, w2=None, td=(None,) * 6) -> None:
-    """Raise ValueError for an output mode, a head width, a bias, (output="sample" or "gaussian") a seed,
-    (output="gaussian") a log_std, a legal-action mask, a value head or a multi-discrete nvec the kernels do not take.  A seed is an int (not
-    a bool) in [0, 2**64); log_std is a 1-D contiguous CUDA float32 tensor of length d_out, given with
-    output="gaussian" only; a mask is a contiguous CUDA torch.bool tensor [M, d_out] on the device of obs [M, d_in],
-    given with any output but "gaussian"; a value head (wv, bv), given with output="sample" or "gaussian" only, is a
-    contiguous bfloat16 wv [1, d_hidden] and a contiguous bfloat16 bv [1] (given exactly when b3 is), both on the
-    device of w3, beside a policy at most 255 wide; nvec (output="actions", "both" or "sample" only) is a non-empty
-    tuple or list of ints >= 1 that sums to d_out (mapped.check_nvec).  With output="gaussian", log_std may instead
-    be a state-dependent head (w_ls, b_ls) (_check_state_std), and log_std_bounds and squash are taken with that form
-    only.  output="epsilon_greedy" takes a seed and an epsilon (_check_epsilon), and epsilon is refused with any other
-    output; its value=, nvec= and log_std= are refused by the checks of those options.  output="evaluate" and
-    "gaussian_evaluate" take the actions to score, `taken` (_check_taken), refused with any other output; they refuse
-    a seed, epsilon, squash, log_std_bounds and a log_std pair, and "gaussian_evaluate" a mask.  output="deterministic"
-    takes noise, noise_clip, a seed and squash (_check_deterministic) and refuses mask, value, nvec, log_std,
-    log_std_bounds, epsilon and taken; noise and noise_clip are refused with any other output.  output="critic" takes
-    the action and an optional twin (_check_critic) and refuses seed, mask, value, nvec, log_std, log_std_bounds,
-    squash, epsilon, taken, noise and noise_clip; action and twin are refused with any other output.
-    output="td_target" refuses mask, value, nvec, epsilon, taken and action, and checks the rest with _check_td_target;
-    td = (actor, policy, reward, done, gamma, alpha), each refused with any other output."""
+    """Raise ValueError for a call the kernels do not take, td = (actor, policy, reward, done, gamma, alpha) and None
+    an option not given.  The options each output takes and requires are those of the table mapped.MLP_TAKES
+    (check_mlp_options, check_mlp_rules), and a constant's value is checked as mapped() checks it (CONSTANT_CHECKS).
+    Then the tensors: a TD target's (_check_td_target) and a critic's (_check_critic); a head 1 to 256 wide; nvec
+    summing to d_out; taken (_check_taken); an epsilon tensor (_check_epsilon); log_std, a 1-D contiguous CUDA float32
+    tensor of length d_out or a state-dependent head (w_ls, b_ls) (_check_state_std); a mask, a contiguous CUDA
+    torch.bool tensor [M, d_out] on the device of obs [M, d_in]; a value head (_check_value); the biases."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
+    values = (seed, log_std, mask, value, nvec, log_std_bounds, squash, epsilon, taken, noise, noise_clip, action, twin,
+              *td)
+    given = {name: v for name, v in zip(_ARGUMENTS, values) if v is not None}
+    actor, policy, reward, done = td[:4]
+    row = check_mlp_options(output, policy, given, argument=True)
+    check_mlp_rules(row, output, policy, log_std, given, argument=True)
+    for name, v in given.items():   # an epsilon may also be a per-row tensor (_check_epsilon)
+        if name in CONSTANT_CHECKS and not (name == "epsilon" and isinstance(v, torch.Tensor)):
+            CONSTANT_CHECKS[name](v)
     if output == "td_target":
-        for name, v in (("mask", mask), ("value", value), ("nvec", nvec), ("epsilon", epsilon), ("taken", taken),
-                        ("action", action)):
-            if v is not None:
-                raise ValueError(f'{name} is not an argument of output="td_target": a TD target takes twin, actor, '
-                                 f'policy and its options, reward, done, gamma and alpha only')
-        _check_td_target(w1, w2, w3, biases, obs, twin, seed, log_std, log_std_bounds, squash, noise, noise_clip, *td)
+        _check_td_target(w1, w2, w3, biases, obs, twin, log_std, actor, reward, done)
         _check_biases(biases, w1.shape[0], w3.shape[0])
         return
-    if any(v is not None for v in td):
-        raise ValueError(f'actor, policy, reward, done, gamma and alpha are arguments of output="td_target", not of '
-                         f'output={output!r}')
     if output == "critic":
-        for name, v in (("seed", seed), ("mask", mask), ("value", value), ("nvec", nvec), ("log_std", log_std),
-                        ("log_std_bounds", log_std_bounds), ("squash", squash), ("epsilon", epsilon),
-                        ("taken", taken), ("noise", noise), ("noise_clip", noise_clip)):
-            if v is not None:
-                raise ValueError(f'{name} is not an argument of output="critic": a critic evaluates Q(s, a) of the '
-                                 f'given action and takes action and twin only')
         _check_critic(w1, w2, w3, biases, obs, action, twin)
-    elif action is not None or twin is not None:
-        raise ValueError(f'action and twin are arguments of output="critic", not of output={output!r}')
-    det = output == "deterministic"
-    if det:
-        for name, v in (("mask", mask), ("value", value), ("nvec", nvec), ("log_std", log_std),
-                        ("log_std_bounds", log_std_bounds), ("epsilon", epsilon), ("taken", taken)):
-            if v is not None:
-                raise ValueError(f'{name} is not an argument of output="deterministic": the deterministic actor takes '
-                                 f'noise, noise_clip, seed and squash only')
-        _check_deterministic(seed, noise, noise_clip, squash)
-    elif noise is not None or noise_clip is not None:
-        raise ValueError(f'noise and noise_clip are arguments of output="deterministic", not of output={output!r}')
-    evaluate = output in EVALUATE_OUTPUTS
-    if evaluate:
-        for name, v in (("seed", seed), ("epsilon", epsilon), ("squash", squash), ("log_std_bounds", log_std_bounds)):
-            if v is not None:
-                raise ValueError(f"{name} is not an argument of output={output!r}: evaluating given actions draws no "
-                                 f"noise")
-        if isinstance(log_std, (tuple, list)):
-            raise ValueError('output="gaussian_evaluate" takes a state-independent log_std tensor, not a log_std=(w_ls, '
-                             'b_ls) pair (evaluating a state-dependent or squashed head is not supported)')
-    elif taken is not None:
-        raise ValueError(f'taken is an argument of output="evaluate" and "gaussian_evaluate", not of output={output!r}')
-    if output in ("sample", "gaussian", "epsilon_greedy"):
-        _check_seed(seed)
-    if output == "epsilon_greedy":
-        _check_epsilon(epsilon, obs)
-    elif epsilon is not None:
-        raise ValueError(f'epsilon is an argument of output="epsilon_greedy", not of output={output!r}')
-    if mask is not None and output in ("gaussian", "gaussian_evaluate"):
-        raise ValueError(f'mask is an argument of the categorical outputs, not of output={output!r}')
     if len(biases) != 3:
         raise ValueError("biases must be (b1, b2, b3), each a tensor or None")
     d_hidden, d_out = w1.shape[0], w3.shape[0]
     if not 1 <= d_out <= MAX_D_OUT:
         raise ValueError(f"d_out={d_out}: the policy head is 1 to {MAX_D_OUT} wide")
     if nvec is not None:
-        check_nvec(nvec, output, d_out)
-    if evaluate:
+        check_nvec(nvec, d_out)
+    if taken is not None:
         _check_taken(taken, output, obs, d_out, nvec)
-    state = isinstance(log_std, (tuple, list))
-    gaussian = output in ("gaussian", "gaussian_evaluate")
-    if not gaussian and log_std is not None:
-        raise ValueError('log_std is an argument of output="gaussian" only (and of "gaussian_evaluate")')
-    if not state and (log_std_bounds is not None or squash is not None and not det):
-        raise ValueError("log_std_bounds and squash are options of a state-dependent log_std=(w_ls, b_ls) only")
-    if output == "gaussian" and state:
-        _check_state_std(log_std, log_std_bounds, squash, w3, biases[2], d_hidden, d_out, value is not None)
-    elif gaussian and (not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32
-                                   or not log_std.is_cuda or not log_std.is_contiguous() or log_std.dim() != 1
-                                   or log_std.shape[0] != d_out):
+    if isinstance(epsilon, torch.Tensor):
+        _check_epsilon(epsilon, obs)
+    if isinstance(log_std, (tuple, list)):
+        _check_state_std(log_std, w3, biases[2], d_hidden, d_out, value is not None)
+    elif log_std is not None and (not isinstance(log_std, torch.Tensor) or log_std.dtype != torch.float32
+                                  or not log_std.is_cuda or not log_std.is_contiguous() or log_std.dim() != 1
+                                  or log_std.shape[0] != d_out):
         raise ValueError(f"log_std must be a 1-D contiguous CUDA float32 tensor of length {d_out}")
     if mask is not None:
         if not isinstance(obs, torch.Tensor):
@@ -475,7 +344,7 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
         if not mask.is_cuda or mask.device != obs.device:
             raise ValueError(f"mask must be a CUDA tensor on the device of obs ({obs.device}), got {mask.device}")
     if value is not None:
-        _check_value(value, output, w3, biases[2], d_hidden, d_out)
+        _check_value(value, w3, biases[2], d_hidden, d_out)
     _check_biases(biases, d_hidden, d_out)
 
 

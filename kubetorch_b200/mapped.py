@@ -17,8 +17,11 @@ Parameter values may be constants or the *name* of a call argument (``alpha="alp
 from __future__ import annotations
 
 import inspect
+import math
 from dataclasses import dataclass, field
 from typing import Any, Callable, Dict, Optional
+
+from .sampling import _check_seed
 
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
@@ -27,6 +30,134 @@ MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greed
                "gaussian_evaluate", "deterministic", "critic", "td_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
 TD_OPTIONS = ("actor", "policy", "reward", "done", "gamma", "alpha")   # the options of output="td_target" alone
+
+# The options each MLP output takes beside bias= and output=, True for those it requires, keyed by (output, policy):
+# a TD target's depend on its policy=, and every other output has none.  mapped() and device.mlp._check_policy refuse
+# every other option and report every missing one (check_mlp_options).
+MLP_TAKES = {
+    ("logits", None): dict(mask=False),
+    ("actions", None): dict(mask=False, nvec=False),
+    ("both", None): dict(mask=False, nvec=False),
+    ("sample", None): dict(seed=True, mask=False, value=False, nvec=False),
+    ("gaussian", None): dict(seed=True, log_std=True, value=False, log_std_bounds=False, squash=False),
+    ("epsilon_greedy", None): dict(seed=True, epsilon=True, mask=False),
+    ("evaluate", None): dict(taken=True, mask=False, value=False, nvec=False),
+    ("gaussian_evaluate", None): dict(taken=True, log_std=True, value=False),
+    ("deterministic", None): dict(noise=False, noise_clip=False, seed=False, squash=False),
+    ("critic", None): dict(action=True, twin=False),
+    ("td_target", "deterministic"): dict(actor=True, policy=True, reward=True, done=True, gamma=True, twin=False,
+                                         noise=False, noise_clip=False, seed=False, squash=False),
+    ("td_target", "gaussian"): dict(actor=True, policy=True, reward=True, done=True, gamma=True, twin=False, seed=True,
+                                    alpha=True, log_std=True, log_std_bounds=False, squash=False),
+}
+
+# Each MLP option's form at decoration: "name", the name of a call argument; "names", a tuple of such names
+# (_NAMES); "name or constant", either; "constant", a value fixed at decoration.  The supervisor binds the names to
+# the call's arguments on every call.
+MLP_FORMS = dict(seed="name or constant", log_std="names", mask="name", value="names", nvec="constant",
+                 log_std_bounds="constant", squash="constant", epsilon="name or constant", taken="name",
+                 noise="name or constant", noise_clip="constant", action="name", twin="names", actor="names",
+                 policy="constant", reward="name", done="name", gamma="constant", alpha="name or constant")
+
+# What each "names" option names, for the message that refuses a wrong count (log_std may also be one name)
+_NAMES =dict(log_std="one call argument or two (w_ls, b_ls)", value="two call arguments (wv, bv)",
+              twin="the second critic's {n} call arguments {what}", actor="the actor's {n} call arguments {what}")
+
+
+def check_mlp_options(output: str, policy, given, argument: bool = False) -> dict:
+    """MLP_TAKES's row of `output` (with a TD target's `policy`), or ValueError naming the first option of `given` that
+    the row does not take, else the first option it requires that `given` lacks.  mapped() says "mask= is not an
+    option of output=...", and with `argument` the device layer "mask is not an argument of output=..."."""
+    eq, what = ("", "an argument") if argument else ("=", "an option")
+    row = MLP_TAKES.get((output, policy if isinstance(policy, str) else None)) or MLP_TAKES.get((output, None))
+    if row is None:
+        policies = tuple(p for o, p in MLP_TAKES if o == output)
+        if policy is None:
+            raise ValueError(f'policy{eq} is required with output="{output}": one of {policies}')
+        raise ValueError(f'policy{eq} must be one of {policies} with output="{output}", got {policy!r}')
+    where = f'output="{output}"' + (f', policy="{policy}"' if "policy" in row else "")
+    for name in given:
+        if name not in row:
+            raise ValueError(f'{name}{eq} is not {what} of {where}, which takes {", ".join(o + eq for o in row)}')
+    for name, required in row.items():
+        if required and name not in given:
+            raise ValueError(f"{name}{eq} is required with {where}")
+    return row
+
+
+def check_noise(name: str, v) -> float:
+    """noise or noise_clip of a deterministic actor: a number (not a bool) >= 0, not NaN."""
+    if isinstance(v, bool) or not isinstance(v, (int, float)):
+        raise ValueError(f"{name} must be a number, got {v!r}")
+    if v != v or v < 0:
+        raise ValueError(f"{name} must be >= 0 and not NaN, got {v!r}")
+    return v
+
+
+def check_squash(v) -> bool:
+    if not isinstance(v, bool):
+        raise ValueError(f"squash must be True or False, got {v!r}")
+    return v
+
+
+def check_log_std_bounds(v) -> tuple:
+    """log_std_bounds as a pair of floats: two numbers (not bools), not NaN, low <= high."""
+    if not isinstance(v, (tuple, list)) or len(v) != 2 or \
+            not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in v):
+        raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {v!r}")
+    lo, hi = float(v[0]), float(v[1])
+    if lo != lo or hi != hi:
+        raise ValueError(f"log_std_bounds must not be NaN, got {v!r}")
+    if lo > hi:
+        raise ValueError(f"log_std_bounds must have low <= high, got {v!r}")
+    return lo, hi
+
+
+def check_epsilon(v):
+    """A constant ε: a number (not a bool), not NaN."""
+    if isinstance(v, bool) or not isinstance(v, (int, float)):
+        raise ValueError(f"epsilon must be a number, got {v!r}")
+    if v != v:
+        raise ValueError("epsilon must not be NaN (a NaN never explores: pass 0.0 for that)")
+    return v
+
+
+def check_finite(name: str, v):
+    """gamma or alpha of a TD target: a finite number (not a bool)."""
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+        raise ValueError(f"{name} must be a finite number, got {v!r}")
+    return v
+
+
+# The check of each MLP option's constant value, which returns the value as MappedSpec.extra keeps it
+CONSTANT_CHECKS = dict(seed=_check_seed, noise=lambda v: check_noise("noise", v),
+                        noise_clip=lambda v: check_noise("noise_clip", v), squash=check_squash,
+                        log_std_bounds=check_log_std_bounds, epsilon=check_epsilon,
+                        gamma=lambda v: check_finite("gamma", v), alpha=lambda v: check_finite("alpha", v),
+                        nvec=lambda v: check_nvec(v))
+
+
+def check_mlp_rules(row: dict, output: str, policy, log_std, given, argument: bool = False) -> None:
+    """The rules of the MLP options that are not rows of MLP_TAKES, with the option names `given` and `row` as
+    check_mlp_options returned it: seed is given exactly when noise is and noise_clip only with noise (where noise is an
+    option); log_std_bounds and squash only with a log_std=(w_ls, b_ls) pair (where log_std is an option); a pair is
+    refused by output="gaussian_evaluate" and required by policy="gaussian"."""
+    eq = "" if argument else "="
+    pair = isinstance(log_std, (tuple, list))
+    if "noise" in row:
+        if ("noise" in given) != ("seed" in given):
+            raise ValueError(f'output="{output}" takes {"a seed" if argument else "seed="} exactly when it takes '
+                             f'noise{eq}: the noise-free actor draws nothing')
+        if "noise_clip" in given and "noise" not in given:
+            raise ValueError(f"noise_clip{eq} is an option of noise{eq} only: it clips the noise")
+    if "log_std" in row and not pair and ("log_std_bounds" in given or "squash" in given):
+        raise ValueError(f"log_std_bounds{eq} and squash{eq} are options of a state-dependent log_std=(w_ls, b_ls) only")
+    if pair and output == "gaussian_evaluate":
+        raise ValueError('output="gaussian_evaluate" takes a state-independent log_std, not a log_std=(w_ls, b_ls) '
+                         'pair (evaluating a state-dependent or squashed head is not supported)')
+    if policy == "gaussian" and not pair:
+        raise ValueError(f'log_std=(w_ls, b_ls) is required with policy="gaussian": the actor\'s state-dependent '
+                         f'log-std head')
 
 
 @dataclass
@@ -149,120 +280,43 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
     alpha = 1.0 if alpha is _UNSET or op == "mlp" and "alpha" in extra else alpha
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if op != "mlp" and any(k in extra for k in ("action", "twin")):
-        raise ValueError(f"action= and twin= are options of the 'mlp' op, not of '{op}'")
-    if op != "mlp" and any(k in extra for k in TD_OPTIONS):
-        raise ValueError(f"actor=, policy=, reward=, done=, gamma= and alpha= are options of the 'mlp' op, not of "
-                         f"'{op}'")
-    if any(k in extra for k in ("bias", "output", "seed", "log_std", "mask", "value", "nvec", "log_std_bounds",
-                                "squash", "epsilon", "taken", "noise", "noise_clip", "action", "twin")):
-        if op != "mlp":
-            raise ValueError(f"bias=, output=, seed=, log_std=, log_std_bounds=, squash=, mask=, value=, nvec=, "
-                             f"epsilon=, taken=, noise= and noise_clip= are options of the 'mlp' op, not of '{op}'")
-        if not isinstance(extra.get("bias", False), bool):
-            raise ValueError(f"bias must be True or False, got {extra['bias']!r}")
-        if extra.get("output", "logits") not in MLP_OUTPUTS:
-            raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {extra['output']!r}")
-        if extra.get("output") == "td_target":
-            _check_td_target(extra)
-        elif any(k in extra for k in TD_OPTIONS):
-            raise ValueError(f'actor=, policy=, reward=, done=, gamma= and alpha= are options of output="td_target", '
-                             f'not of output={extra.get("output", "logits")!r}')
-        else:
-            if extra.get("output") == "critic":
-                _check_critic(extra)
-            elif "action" in extra or "twin" in extra:
-                raise ValueError(f'action= and twin= are options of output="critic", not of '
-                                 f'output={extra.get("output", "logits")!r}')
-            sample = extra.get("output") in ("sample", "gaussian")
-            eps = extra.get("output") == "epsilon_greedy"
-            det = extra.get("output") == "deterministic"
-            if det:
-                _check_deterministic(extra)
-            elif "noise" in extra or "noise_clip" in extra:
-                raise ValueError(f'noise= and noise_clip= are options of output="deterministic", not of '
-                                 f'output={extra.get("output", "logits")!r}')
-            evaluate = extra.get("output") in EVALUATE_OUTPUTS
-            if evaluate != ("taken" in extra):
-                raise ValueError('taken= is required with output="evaluate" and "gaussian_evaluate" and is an option of '
-                                 'those outputs only')
-            if evaluate and not isinstance(extra["taken"], str):
-                raise ValueError(f"taken must be the name of a call argument, got {extra['taken']!r}")
-            if evaluate and "seed" in extra:
-                raise ValueError(f'seed= is not an option of output={extra["output"]!r}: evaluating given actions draws '
-                                 f'no noise')
-            if not det and (sample or eps) != ("seed" in extra):
-                raise ValueError('seed= is required with output="sample" or "gaussian" (or "epsilon_greedy") and is an '
-                                 'option of those only')
-            if (sample or eps or det) and "seed" in extra and not isinstance(extra["seed"], str):
-                from .sampling import _check_seed
-
-                _check_seed(extra["seed"])
-            gaussian = extra.get("output") in ("gaussian", "gaussian_evaluate")
-            if gaussian != ("log_std" in extra):
-                raise ValueError('log_std= is required with output="gaussian" (and "gaussian_evaluate") and is an option of '
-                                 'those outputs only')
-            state = gaussian and isinstance(extra["log_std"], (tuple, list))
-            if state and evaluate:
-                raise ValueError('output="gaussian_evaluate" takes a state-independent log_std (the name of one call '
-                                 'argument), not a log_std=(w_ls, b_ls) pair')
-            if state:
-                ls = extra["log_std"]
-                if len(ls) != 2 or not all(isinstance(n, str) for n in ls):
-                    raise ValueError(f"log_std must name one call argument or two (w_ls, b_ls), got {ls!r}")
-                if not extra.get("bias", False):
-                    raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when "
-                                     "b3 is")
-            elif gaussian and not isinstance(extra["log_std"], str):
-                raise ValueError(f"log_std must be the name of a call argument, got {extra['log_std']!r}")
-            if not state and ("log_std_bounds" in extra or "squash" in extra and not det):
-                raise ValueError("log_std_bounds= and squash= are options of a state-dependent log_std=(w_ls, b_ls) only")
-            if "log_std_bounds" in extra:
-                lb = extra["log_std_bounds"]
-                if not isinstance(lb, (tuple, list)) or len(lb) != 2 or \
-                        not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in lb):
-                    raise ValueError(f"log_std_bounds must be (low, high), two numbers, got {lb!r}")
-                if lb[0] != lb[0] or lb[1] != lb[1]:
-                    raise ValueError(f"log_std_bounds must not be NaN, got {lb!r}")
-                if lb[0] > lb[1]:
-                    raise ValueError(f"log_std_bounds must have low <= high, got {lb!r}")
-                extra["log_std_bounds"] = (float(lb[0]), float(lb[1]))
-            if "squash" in extra and not isinstance(extra["squash"], bool):
-                raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
-            if "mask" in extra:
-                if gaussian:
-                    raise ValueError(f'mask= is an option of the categorical outputs, not of output={extra["output"]!r}')
-                if not isinstance(extra["mask"], str):
-                    raise ValueError(f"mask must be the name of a call argument, got {extra['mask']!r}")
-            if "value" in extra:
-                if not (sample or evaluate):
-                    raise ValueError('value= is an option of output="sample", "gaussian", "evaluate" and '
-                                     '"gaussian_evaluate" only')
-                if not extra.get("bias", False):
-                    raise ValueError("value= needs bias=True: the critic's bias is given exactly when b3 is")
-                v = extra["value"]
-                if not isinstance(v, (tuple, list)) or len(v) != 2 or not all(isinstance(n, str) for n in v):
-                    raise ValueError(f"value must name two call arguments (wv, bv), got {v!r}")
-            if "nvec" in extra:
-                extra["nvec"] = check_nvec(extra["nvec"], extra.get("output", "logits"))
-            if eps != ("epsilon" in extra):
-                raise ValueError('epsilon= is required with output="epsilon_greedy" and is an option of that output only')
-            if eps and not isinstance(extra["epsilon"], str):
-                e = extra["epsilon"]
-                if isinstance(e, bool) or not isinstance(e, (int, float)):
-                    raise ValueError(f"epsilon must be a number or the name of a call argument, got {e!r}")
-                if e != e:
-                    raise ValueError("epsilon must not be NaN (a NaN never explores: pass 0.0 for that)")
+    if op != "mlp":
+        if any(k in extra for k in ("bias", "output", *MLP_FORMS)):
+            raise ValueError(f"{', '.join(k + '=' for k in ('bias', 'output', *MLP_FORMS))} are options of the 'mlp' "
+                             f"op, not of '{op}'")
+    else:
+        bias = extra.get("bias", False)
+        if not isinstance(bias, bool):
+            raise ValueError(f"bias must be True or False, got {bias!r}")
+        output = extra.get("output", "logits")
+        if output not in MLP_OUTPUTS:
+            raise ValueError(f"output must be one of {MLP_OUTPUTS}, got {output!r}")
+        given = [k for k in extra if k in MLP_FORMS]
+        row = check_mlp_options(output, extra.get("policy"), given)
+        check_mlp_rules(row, output, extra.get("policy"), extra.get("log_std"), given)
+        for name in given:
+            form, v = MLP_FORMS[name], extra[name]
+            if form == "name" and not isinstance(v, str):
+                raise ValueError(f"{name} must be the name of a call argument, got {v!r}")
+            if form == "names" and not (name == "log_std" and isinstance(v, str)):
+                n = (6 if bias else 3) if name in ("twin", "actor") else 2
+                if not isinstance(v, (tuple, list)) or len(v) != n or not all(isinstance(x, str) for x in v):
+                    what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
+                    raise ValueError(f"{name} must name {_NAMES[name].format(n=n, what=what)}, got {v!r}")
+            if name in CONSTANT_CHECKS and not names_arguments(name, v):
+                extra[name] = CONSTANT_CHECKS[name](v)
+        if not bias and "value" in extra:
+            raise ValueError("value= needs bias=True: the critic's bias is given exactly when b3 is")
+        if not bias and isinstance(extra.get("log_std"), (tuple, list)):
+            raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when b3 is")
 
     def deco(fn):
         params = inspect.signature(fn).parameters
-        for option in ("log_std", "mask", "value", "epsilon", "taken", "noise", "action", "twin", "actor", "reward",
-                       "done", "alpha"):
-            names = extra.get(option)
-            if option in ("epsilon", "noise", "alpha") and not isinstance(names, str):   # a constant names no argument
+        for option, names in extra.items():
+            if not names_arguments(option, names):
                 continue
-            for name in (names,) if isinstance(names, str) or names is None else names:
-                if name is not None and name not in params:
+            for name in (names,) if isinstance(names, str) else names:
+                if name not in params:
                     raise ValueError(f"{option}={names!r}: {name!r} is not an argument of "
                                      f"{getattr(fn, '__name__', fn)!r}")
         setattr(fn, MAPPED_ATTR, MappedSpec(op=op, alpha=alpha, beta=beta, reduce=reduce, arg=arg, extra=extra))
@@ -271,129 +325,16 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
     return deco
 
 
-def _check_deterministic(extra) -> None:
-    """mapped()'s checks of output="deterministic", in this order: the options it refuses, seed= given exactly when
-    noise= is, noise (a number that is not NaN and >= 0, or the name of a call argument), noise_clip (with noise= only;
-    a number that is not NaN and >= 0)."""
-    for name in ("mask", "value", "nvec", "log_std", "log_std_bounds", "epsilon", "taken"):
-        if name in extra:
-            raise ValueError(f'{name}= is not an option of output="deterministic": the deterministic actor takes '
-                             f'noise=, noise_clip=, seed= and squash= only')
-    if ("noise" in extra) != ("seed" in extra):
-        raise ValueError('output="deterministic" takes seed= exactly when it takes noise=: the noise-free actor draws '
-                         'nothing')
-    if "noise_clip" in extra and "noise" not in extra:
-        raise ValueError("noise_clip= is an option of noise= only: it clips the noise")
-    for name in ("noise", "noise_clip"):
-        v = extra.get(name)
-        if v is None or name == "noise" and isinstance(v, str):
-            continue
-        if isinstance(v, bool) or not isinstance(v, (int, float)):
-            what = "a number or the name of a call argument" if name == "noise" else "a number"
-            raise ValueError(f"{name} must be {what}, got {v!r}")
-        if v != v or v < 0:
-            raise ValueError(f"{name} must be >= 0 and not NaN, got {v!r}")
+def names_arguments(option: str, v) -> bool:
+    """Whether the value v of an MLP option names call arguments (one name, or the tuple of a "names" option) rather
+    than being a constant."""
+    form = MLP_FORMS.get(option, "constant")
+    return form == "names" or form != "constant" and isinstance(v, str)
 
 
-def _check_critic(extra) -> None:
-    """mapped()'s checks of output="critic", in this order: the options it refuses, action= (required, the name of a
-    call argument), twin= (the names of six call arguments with bias=True, three without)."""
-    for name in ("seed", "mask", "value", "nvec", "log_std", "log_std_bounds", "squash", "epsilon", "taken", "noise",
-                 "noise_clip"):
-        if name in extra:
-            raise ValueError(f'{name}= is not an option of output="critic": a critic evaluates Q(s, a) of the given '
-                             f'action and takes action= and twin= only')
-    if not isinstance(extra.get("action"), str):
-        raise ValueError(f'action= is required with output="critic" and must name the call argument that holds the '
-                         f'actions, got {extra.get("action")!r}')
-    if "twin" in extra:
-        n = 6 if extra.get("bias", False) else 3
-        t = extra["twin"]
-        if not isinstance(t, (tuple, list)) or len(t) != n or not all(isinstance(x, str) for x in t):
-            what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
-            raise ValueError(f"twin must name the second critic's {n} call arguments {what}, got {t!r}")
-
-
-def _check_td_target(extra) -> None:
-    """mapped()'s checks of output="td_target", in this order: the options it refuses, policy=, the policy's options
-    (noise=, noise_clip= and seed= as output="deterministic" takes them, refusing log_std=, log_std_bounds= and alpha=;
-    or seed=, alpha=, log_std=(w_ls, b_ls) with bias=True, log_std_bounds= and squash=, refusing noise= and
-    noise_clip=), actor= (six names with bias=True, three without), twin= as output="critic" takes it, reward= and
-    done= (names), gamma= (a finite number)."""
-    for name in ("mask", "value", "nvec", "epsilon", "taken", "action"):
-        if name in extra:
-            raise ValueError(f'{name}= is not an option of output="td_target": a TD target takes actor=, policy= and '
-                             f'its options, twin=, reward=, done=, gamma= and alpha= only')
-    policy = extra.get("policy")
-    if policy not in ("deterministic", "gaussian"):
-        raise ValueError(f'policy= must be "deterministic" or "gaussian" with output="td_target", got {policy!r}')
-    if policy == "deterministic":
-        for name in ("log_std", "log_std_bounds", "alpha"):
-            if name in extra:
-                raise ValueError(f'{name}= is not an option of policy="deterministic": TD3 and DDPG targets take '
-                                 f'noise=, noise_clip=, seed= and squash=, and no entropy term')
-        _check_deterministic(extra)
-        if "seed" in extra and not isinstance(extra["seed"], str):
-            from .sampling import _check_seed
-
-            _check_seed(extra["seed"])
-    else:
-        for name in ("noise", "noise_clip"):
-            if name in extra:
-                raise ValueError(f'{name}= is not an option of policy="gaussian": SAC\'s next actions are sampled with '
-                                 f'the log-std head')
-        if "seed" not in extra:
-            raise ValueError('seed= is required with policy="gaussian"')
-        if not isinstance(extra["seed"], str):
-            from .sampling import _check_seed
-
-            _check_seed(extra["seed"])
-        a = extra.get("alpha")
-        if a is None:
-            raise ValueError('alpha= is required with policy="gaussian": a number or the name of a call argument')
-        if not isinstance(a, str) and (isinstance(a, bool) or not isinstance(a, (int, float)) or a != a
-                                       or a in (float("inf"), float("-inf"))):
-            raise ValueError(f"alpha must be a finite number or the name of a call argument, got {a!r}")
-        ls = extra.get("log_std")
-        if not isinstance(ls, (tuple, list)) or len(ls) != 2 or not all(isinstance(n, str) for n in ls):
-            raise ValueError(f'log_std= must name the two call arguments (w_ls, b_ls) of the actor\'s log-std head '
-                             f'with policy="gaussian", got {ls!r}')
-        if not extra.get("bias", False):
-            raise ValueError("log_std=(w_ls, b_ls) needs bias=True: the log-std head's bias is given exactly when b3 is")
-        if "log_std_bounds" in extra:
-            lb = extra["log_std_bounds"]
-            if not isinstance(lb, (tuple, list)) or len(lb) != 2 or \
-                    not all(isinstance(b, (int, float)) and not isinstance(b, bool) for b in lb) or \
-                    lb[0] != lb[0] or lb[1] != lb[1] or lb[0] > lb[1]:
-                raise ValueError(f"log_std_bounds must be (low, high), two numbers, not NaN, low <= high, got {lb!r}")
-            extra["log_std_bounds"] = (float(lb[0]), float(lb[1]))
-    if "squash" in extra and not isinstance(extra["squash"], bool):
-        raise ValueError(f"squash must be True or False, got {extra['squash']!r}")
-    n = 6 if extra.get("bias", False) else 3
-    for option in ("actor", "twin"):
-        if option not in extra and option == "twin":
-            continue
-        t = extra.get(option)
-        if not isinstance(t, (tuple, list)) or len(t) != n or not all(isinstance(x, str) for x in t):
-            what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
-            whose = "the actor's" if option == "actor" else "the second critic's"
-            raise ValueError(f"{option} must name {whose} {n} call arguments {what}, got {t!r}")
-    for option in ("reward", "done"):
-        if not isinstance(extra.get(option), str):
-            raise ValueError(f'{option}= is required with output="td_target" and must name a call argument, got '
-                             f'{extra.get(option)!r}')
-    g = extra.get("gamma")
-    if isinstance(g, bool) or not isinstance(g, (int, float)) or g != g or g in (float("inf"), float("-inf")):
-        raise ValueError(f'gamma= is required with output="td_target" and must be a finite number, got {g!r}')
-
-
-def check_nvec(nvec, output: str, d_out: Optional[int] = None) -> tuple:
-    """nvec as a tuple, or ValueError naming what is wrong with it: given with an output other than "actions", "both",
-    "sample" and "evaluate"; not a tuple or list of ints (bools refused); empty; an entry below 1; (with d_out) a sum
-    other than d_out."""
-    if output not in ("actions", "both", "sample", "evaluate"):
-        raise ValueError(f'nvec is an option of output="actions", "both", "sample" and "evaluate", not of '
-                         f'output={output!r}')
+def check_nvec(nvec, d_out: Optional[int] = None) -> tuple:
+    """nvec as a tuple, or ValueError naming what is wrong with it: not a tuple or list of ints (bools refused); empty;
+    an entry below 1; (with d_out) a sum other than d_out."""
     if not isinstance(nvec, (tuple, list)) or not all(isinstance(n, int) and not isinstance(n, bool) for n in nvec):
         raise ValueError(f"nvec must be a tuple of ints, got {nvec!r}")
     if len(nvec) == 0:

@@ -50,7 +50,7 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import ELEMENTWISE_OPS, mapped_spec
+from ..mapped import ELEMENTWISE_OPS, MLP_FORMS, TD_OPTIONS, mapped_spec, names_arguments
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -572,78 +572,21 @@ class B200Supervisor:
         else:
             obs, w1, w2, w3 = (bound[n] for n in names[:4])
             biases = (None, None, None)
-        seed = spec.extra.get("seed")
-        if isinstance(seed, str):   # the name of a call argument, resolved per call
-            if seed not in bound:
-                raise TypeError(f"mapped mlp callable: seed argument '{seed}' not found in the call")
-            seed = bound[seed]
-        log_std = spec.extra.get("log_std")
-        if log_std is not None:   # the name of a call argument, or the names (w_ls, b_ls) of two, resolved per call
-            for name in (log_std,) if isinstance(log_std, str) else log_std:
-                if name not in bound:
-                    raise TypeError(f"mapped mlp callable: log_std argument '{name}' not found in the call")
-            log_std = bound[log_std] if isinstance(log_std, str) else tuple(bound[name] for name in log_std)
-        mask = spec.extra.get("mask")
-        if mask is not None:   # always the name of a call argument, resolved per call
-            if mask not in bound:
-                raise TypeError(f"mapped mlp callable: mask argument '{mask}' not found in the call")
-            mask = bound[mask]
-        value = spec.extra.get("value")
-        if value is not None:   # always the names (wv, bv) of two call arguments, resolved per call
-            for name in value:
-                if name not in bound:
-                    raise TypeError(f"mapped mlp callable: value argument '{name}' not found in the call")
-            value = tuple(bound[name] for name in value)
-        epsilon = spec.extra.get("epsilon")
-        if isinstance(epsilon, str):   # the name of a call argument (a float or a per-row tensor), resolved per call
-            if epsilon not in bound:
-                raise TypeError(f"mapped mlp callable: epsilon argument '{epsilon}' not found in the call")
-            epsilon = bound[epsilon]
-        taken = spec.extra.get("taken")
-        if taken is not None:   # always the name of a call argument (the whole batch's actions), resolved per call
-            if taken not in bound:
-                raise TypeError(f"mapped mlp callable: taken argument '{taken}' not found in the call")
-            taken = bound[taken]
-        noise = spec.extra.get("noise")
-        if isinstance(noise, str):   # the name of a call argument (a float), resolved per call
-            if noise not in bound:
-                raise TypeError(f"mapped mlp callable: noise argument '{noise}' not found in the call")
-            noise = bound[noise]
-        action = spec.extra.get("action")
-        if action is not None:   # always the name of a call argument (the whole batch's actions), resolved per call
-            if action not in bound:
-                raise TypeError(f"mapped mlp callable: action argument '{action}' not found in the call")
-            action = bound[action]
-        twin = spec.extra.get("twin")
-        if twin is not None:   # the names of the second critic's weights (and biases), resolved per call
-            for name in twin:
-                if name not in bound:
-                    raise TypeError(f"mapped mlp callable: twin argument '{name}' not found in the call")
-            twin = tuple(bound[name] for name in twin)
-            if len(twin) == 3:   # (w1, w2, w3) of a bias-free critic
-                twin = (twin[0], None, twin[1], None, twin[2], None)
-        td = {}
-        if output == "td_target":   # the actor's weights, reward, done and a named alpha, resolved per call
-            for name in (*spec.extra["actor"], spec.extra["reward"], spec.extra["done"]):
-                if name not in bound:
-                    raise TypeError(f"mapped mlp callable: td_target argument '{name}' not found in the call")
-            actor = tuple(bound[name] for name in spec.extra["actor"])
-            if len(actor) == 3:   # (w1, w2, w3) of a bias-free actor
-                actor = (actor[0], None, actor[1], None, actor[2], None)
-            alpha = spec.extra.get("alpha")
-            if isinstance(alpha, str):
-                if alpha not in bound:
-                    raise TypeError(f"mapped mlp callable: alpha argument '{alpha}' not found in the call")
-                alpha = float(bound[alpha])   # a number or a one-element tensor (on a GPU: one host synchronisation)
-            td = dict(actor=actor, policy=spec.extra["policy"], reward=bound[spec.extra["reward"]],
-                      done=bound[spec.extra["done"]], gamma=spec.extra["gamma"], alpha=alpha)
+        # every option mlp_scatter_gather takes, a TD target's only with output="td_target"; None unless given
+        args = {name: None for name in MLP_FORMS if name not in TD_OPTIONS or output == "td_target"}
+        for option, v in spec.extra.items():
+            if option not in MLP_FORMS:
+                continue
+            if names_arguments(option, v):   # resolved per call: mapped() checked that each names an argument
+                v = bound[v] if isinstance(v, str) else tuple(bound[name] for name in v)
+                if option in ("twin", "actor") and len(v) == 3:   # (w1, w2, w3) of a bias-free network
+                    v = (v[0], None, v[1], None, v[2], None)
+                elif option == "alpha":
+                    v = float(v)   # a number or a one-element tensor (on a GPU: one host synchronisation)
+            args[option] = v
         try:
             out = mlp.mlp_scatter_gather(obs, w1, w2, w3, devices=self.devices, transfer=self.transfer,
-                                         biases=biases, output=output, seed=seed, log_std=log_std, mask=mask,
-                                         value=value, nvec=spec.extra.get("nvec"),
-                                         log_std_bounds=spec.extra.get("log_std_bounds"),
-                                         squash=spec.extra.get("squash"), epsilon=epsilon, taken=taken, noise=noise,
-                                         noise_clip=spec.extra.get("noise_clip"), action=action, twin=twin, **td)
+                                         biases=biases, output=output, **args)
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]

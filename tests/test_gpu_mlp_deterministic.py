@@ -301,7 +301,7 @@ def test_empty_pushed_shard_runs_its_checks_and_acks(K):
 
 
 # ---- Python checks -----------------------------------------------------------------------------------------------------------
-def test_python_checks_reach_mlp_forward_and_scatter_gather(K):
+def test_python_checks_name_the_output_in_mlp_forward_and_scatter_gather(K):
     (w1, w2, w3), b = config(5700, 18)
     obs = randn((256, 256), 5701)
     bad = [
@@ -313,7 +313,8 @@ def test_python_checks_reach_mlp_forward_and_scatter_gather(K):
         (dict(squash=1), "True or False"),
         (dict(mask=torch.ones(256, 18, dtype=torch.bool, device="cuda")), "mask is not an argument"),
         (dict(log_std=torch.zeros(18, device="cuda")), "log_std is not an argument"),
-        (dict(output="gaussian", noise=0.1, seed=1, log_std=torch.zeros(18, device="cuda")), "arguments of output="),
+        (dict(output="gaussian", noise=0.1, seed=1, log_std=torch.zeros(18, device="cuda")),
+         'noise is not an argument of output="gaussian"'),
     ]
     for kw, reason in bad:
         kw = dict(dict(output="deterministic"), **kw)

@@ -410,12 +410,12 @@ def test_empty_pushed_shard_runs_its_checks_and_acks(K, valued):
 
 
 # ---- Python checks and in-place updates ------------------------------------------------------------------------------------
-def test_python_checks_reach_mlp_forward_and_scatter_gather(K):
+def test_python_checks_name_the_output_in_mlp_forward_and_scatter_gather(K):
     (w1, w2, w3), b = config(4600, 18)
     obs = randn((256, 256), 4601)
     w_ls, b_ls = randn((18, 1024), 4602), randn((18,), 4603)
     bad = [
-        (dict(log_std=(w_ls, b_ls), output="sample"), 'output="gaussian" only'),
+        (dict(log_std=(w_ls, b_ls), output="sample"), 'log_std is not an argument of output="sample"'),
         (dict(log_std=(w_ls,)), "tensor or"),
         (dict(log_std=(w_ls, None)), "b_ls is given exactly when b3 is"),
         (dict(log_std=(w_ls[:17], b_ls)), "shape"),

@@ -346,12 +346,13 @@ def test_empty_pushed_shard_runs_its_checks_and_acks(K, kind):
 
 
 # ---- 6. Python checks ---------------------------------------------------------------------------------------------------
-def test_python_checks_reach_mlp_forward_and_scatter_gather(K):
+def test_python_checks_name_the_output_in_mlp_forward_and_scatter_gather(K):
     (w1, w2, w3), b = config(3400, 18)
     obs = randn((256, 256), 3401)
     bad = [
-        ("logits", {}, (9, 9), "nvec is an option"),
-        ("gaussian", dict(seed=1, log_std=torch.zeros(18, device="cuda")), (9, 9), "nvec is an option"),
+        ("logits", {}, (9, 9), 'nvec is not an argument of output="logits"'),
+        ("gaussian", dict(seed=1, log_std=torch.zeros(18, device="cuda")), (9, 9),
+         'nvec is not an argument of output="gaussian"'),
         ("actions", {}, (9.0, 9), "tuple of ints"),
         ("both", {}, (True, 17), "tuple of ints"),
         ("sample", dict(seed=1), "99", "tuple of ints"),

@@ -234,15 +234,15 @@ def test_empty_pushed_shard_runs_its_checks_and_acks(K, head):
 
 
 # ---- 4. Python checks ---------------------------------------------------------------------------------------------------
-def test_python_checks_reach_mlp_forward_and_scatter_gather(K):
+def test_python_checks_name_the_output_in_mlp_forward_and_scatter_gather(K):
     (w1, w2, w3), b = config(2200, 18)
     obs = randn((256, 256), 2201)
     wv, bv = randn((1, 1024), 2202), randn((1,), 2203)
     log_std = torch.zeros(18, device="cuda")
     bad = [
-        ("actions", {}, b, (wv, bv), "value is an argument"),
-        ("both", {}, b, (wv, bv), "value is an argument"),
-        ("logits", {}, b, (wv, bv), "value is an argument"),
+        ("actions", {}, b, (wv, bv), 'value is not an argument of output="actions"'),
+        ("both", {}, b, (wv, bv), 'value is not an argument of output="both"'),
+        ("logits", {}, b, (wv, bv), 'value is not an argument of output="logits"'),
         ("sample", dict(seed=1), b, (wv,), "value must be"),
         ("sample", dict(seed=1), b, (wv, None), "bv is given exactly when b3 is"),
         ("gaussian", dict(seed=1, log_std=log_std), (b[0], b[1], None), (wv, bv), "bv is given exactly when b3 is"),

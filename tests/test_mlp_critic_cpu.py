@@ -99,18 +99,18 @@ def test_mapped_critic_refuses_the_options_of_other_heads(option):
         kt.mapped("mlp", bias=True, output="critic", action="act", **{option: REFUSED[option]})
 
 
-def test_mapped_critic_requires_action_by_name():
+def test_mapped_critic_requires_action_as_a_name():
     with pytest.raises(ValueError, match='action= is required with output="critic"'):
         kt.mapped("mlp", bias=True, output="critic")
-    with pytest.raises(ValueError, match='action= is required with output="critic"'):
+    with pytest.raises(ValueError, match="action must be the name of a call argument"):
         kt.mapped("mlp", bias=True, output="critic", action=3)
 
 
 @pytest.mark.parametrize("output", ["logits", "actions", "sample", "deterministic"])
 @pytest.mark.parametrize("option", ["action", "twin"])
-def test_mapped_refuses_action_and_twin_with_other_outputs(output, option):
+def test_mapped_refuses_action_and_twin_naming_the_output(output, option):
     extra = dict(seed=1) if output == "sample" else {}
-    with pytest.raises(ValueError, match='action= and twin= are options of output="critic"'):
+    with pytest.raises(ValueError, match=f'{option}= is not an option of output="{output}"'):
         kt.mapped("mlp", bias=True, output=output, **extra, **{option: "act" if option == "action" else ("a",) * 6})
 
 
@@ -150,15 +150,16 @@ def test_check_policy_critic_refuses_the_options_of_other_heads(option):
         _check(**{option: REFUSED[option]})
 
 
-def test_check_policy_critic_refuses_a_wide_head_and_a_missing_action():
+def test_check_policy_critic_refuses_a_wide_head_and_requires_action():
+    obs, act, _, _ = _case()
     with pytest.raises(ValueError, match=r"d_out=4: a critic's w3 is \[1, d_hidden\]"):
-        _check(w3_rows=4)
+        _check(w3_rows=4, action=act)
     with pytest.raises(ValueError, match='action is required with output="critic"'):
         _check()
 
 
 @pytest.mark.parametrize("output", ["logits", "sample", "deterministic"])
-def test_check_policy_refuses_action_and_twin_with_other_outputs(output):
+def test_check_policy_refuses_action_naming_the_output(output):
     extra = dict(seed=1) if output == "sample" else {}
-    with pytest.raises(ValueError, match='action and twin are arguments of output="critic"'):
+    with pytest.raises(ValueError, match=f'action is not an argument of output="{output}"'):
         _check(output=output, action=torch.zeros(37, 6), **extra)

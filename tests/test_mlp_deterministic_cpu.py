@@ -117,8 +117,8 @@ D = dict(output="deterministic")
     (dict(**D, noise_clip=0.5), "noise_clip= is an option of noise= only"),
     (dict(**D, noise=-0.1, seed="seed"), ">= 0 and not NaN"),
     (dict(**D, noise=float("nan"), seed="seed"), ">= 0 and not NaN"),
-    (dict(**D, noise=True, seed="seed"), "a number or the name of a call argument"),
-    (dict(**D, noise=[0.1], seed="seed"), "a number or the name of a call argument"),
+    (dict(**D, noise=True, seed="seed"), "noise must be a number"),
+    (dict(**D, noise=[0.1], seed="seed"), "noise must be a number"),
     (dict(**D, noise=0.1, seed="seed", noise_clip=-1.0), ">= 0 and not NaN"),
     (dict(**D, noise=0.1, seed="seed", noise_clip="clip"), "noise_clip must be a number"),
     (dict(**D, noise=0.1, seed=-1), "seed must be an int"),
@@ -130,9 +130,9 @@ D = dict(output="deterministic")
     (dict(**D, log_std_bounds=(-1, 1)), 'log_std_bounds= is not an option of output="deterministic"'),
     (dict(**D, epsilon=0.1), 'epsilon= is not an option of output="deterministic"'),
     (dict(**D, taken="acts"), 'taken= is not an option of output="deterministic"'),
-    (dict(output="gaussian", seed="seed", log_std="log_std", noise=0.1), 'options of output="deterministic"'),
-    (dict(output="sample", seed="seed", noise_clip=0.5), 'options of output="deterministic"'),
-    (dict(output="sample", seed="seed", squash=True), "state-dependent"),
+    (dict(output="gaussian", seed="seed", log_std="log_std", noise=0.1), 'noise= is not an option of output="gaussian"'),
+    (dict(output="sample", seed="seed", noise_clip=0.5), 'noise_clip= is not an option of output="sample"'),
+    (dict(output="sample", seed="seed", squash=True), 'squash= is not an option of output="sample"'),
 ])
 def test_bad_deterministic_options_raise_at_decoration(kwargs, reason):
     import kubetorch_b200 as kt
@@ -187,9 +187,9 @@ def _check(**kw):
     (dict(log_std_bounds=(-1.0, 1.0)), "log_std_bounds is not an argument"),
     (dict(epsilon=0.5), "epsilon is not an argument"),
     (dict(taken=torch.zeros(4, 18)), "taken is not an argument"),
-    (dict(output="gaussian", seed=1, noise=0.1), 'arguments of output="deterministic"'),
-    (dict(output="logits", noise_clip=1.0), 'arguments of output="deterministic"'),
-    (dict(output="sample", seed=1, squash=True), "state-dependent"),
+    (dict(output="gaussian", seed=1, noise=0.1), 'noise is not an argument of output="gaussian"'),
+    (dict(output="logits", noise_clip=1.0), 'noise_clip is not an argument of output="logits"'),
+    (dict(output="sample", seed=1, squash=True), 'squash is not an argument of output="sample"'),
 ])
 def test_check_policy_rejects_bad_deterministic_arguments(kw, reason):
     with pytest.raises(ValueError, match=reason):

@@ -144,18 +144,18 @@ GEV = dict(bias=True, output="gaussian_evaluate", taken="acts", log_std="log_std
 @pytest.mark.parametrize("kwargs,reason", [
     (dict(bias=True, output="evaluate"), "taken= is required"),
     (dict(bias=True, output="gaussian_evaluate", log_std="log_std"), "taken= is required"),
-    (dict(bias=True, output="sample", seed=1, taken="acts"), "taken= is required"),
-    (dict(bias=True, output="actions", taken="acts"), "taken= is required"),
+    (dict(bias=True, output="sample", seed=1, taken="acts"), 'taken= is not an option of output="sample"'),
+    (dict(bias=True, output="actions", taken="acts"), 'taken= is not an option of output="actions"'),
     (dict(EV, taken=3), "taken must be the name of a call argument"),
     (dict(EV, seed=1), "seed= is not an option"),
     (dict(GEV, seed="seed"), "seed= is not an option"),
-    (dict(EV, epsilon=0.1), "epsilon= is required with output=\"epsilon_greedy\""),
-    (dict(GEV, squash=True), "options of a state-dependent"),
-    (dict(GEV, log_std_bounds=(-5, 2)), "options of a state-dependent"),
+    (dict(EV, epsilon=0.1), 'epsilon= is not an option of output="evaluate"'),
+    (dict(GEV, squash=True), 'squash= is not an option of output="gaussian_evaluate"'),
+    (dict(GEV, log_std_bounds=(-5, 2)), 'log_std_bounds= is not an option of output="gaussian_evaluate"'),
     (dict(GEV, log_std=("w_ls", "b_ls")), "not a log_std=\\(w_ls, b_ls\\) pair"),
-    (dict(GEV, mask="legal"), "mask= is an option of the categorical outputs"),
-    (dict(EV, log_std="log_std"), "log_std= is required with output=\"gaussian\""),
-    (dict(GEV, nvec=(3, 3)), "nvec is an option"),
+    (dict(GEV, mask="legal"), 'mask= is not an option of output="gaussian_evaluate"'),
+    (dict(EV, log_std="log_std"), 'log_std= is not an option of output="evaluate"'),
+    (dict(GEV, nvec=(3, 3)), 'nvec= is not an option of output="gaussian_evaluate"'),
 ])
 def test_bad_evaluate_options_raise_at_decoration(kwargs, reason):
     with pytest.raises(ValueError, match=reason):
@@ -186,6 +186,9 @@ def _check(output="evaluate", taken="default", obs=None, **kw):
                       taken=taken, **kw)
 
 
+LS = torch.zeros(18)   # a CPU log_std: the checks of taken come first
+
+
 @pytest.mark.parametrize("case,reason", [
     (dict(taken=None), "taken is required"),
     (dict(taken=[0] * 8), "taken must be a tensor"),
@@ -195,24 +198,24 @@ def _check(output="evaluate", taken="default", obs=None, **kw):
     (dict(taken=torch.zeros(16, dtype=torch.int64)[::2]), "taken must be contiguous"),
     (dict(taken=torch.zeros(2, 8, dtype=torch.int64).t(), nvec=(9, 9)), "taken must be contiguous"),
     (dict(), "taken must be a CUDA tensor on the device of obs"),
-    (dict(output="gaussian_evaluate", taken=torch.zeros(8, 18, dtype=torch.float64)),
+    (dict(output="gaussian_evaluate", log_std=LS, taken=torch.zeros(8, 18, dtype=torch.float64)),
      "float32 tensor of shape \\(8, 18\\)"),
-    (dict(output="gaussian_evaluate", taken=torch.zeros(8, 17)), "float32 tensor of shape \\(8, 18\\)"),
-    (dict(output="gaussian_evaluate", taken=torch.zeros(18, 8).t()), "taken must be contiguous"),
-    (dict(output="gaussian_evaluate"), "taken must be a CUDA tensor on the device of obs"),
-    (dict(seed=1), "seed is not an argument of output='evaluate'"),
+    (dict(output="gaussian_evaluate", log_std=LS, taken=torch.zeros(8, 17)), "float32 tensor of shape \\(8, 18\\)"),
+    (dict(output="gaussian_evaluate", log_std=LS, taken=torch.zeros(18, 8).t()), "taken must be contiguous"),
+    (dict(output="gaussian_evaluate", log_std=LS), "taken must be a CUDA tensor on the device of obs"),
+    (dict(seed=1), 'seed is not an argument of output="evaluate"'),
     (dict(epsilon=0.1), "epsilon is not an argument"),
     (dict(output="gaussian_evaluate", squash=True), "squash is not an argument"),
     (dict(output="gaussian_evaluate", log_std_bounds=(-5.0, 2.0)), "log_std_bounds is not an argument"),
     (dict(output="gaussian_evaluate", log_std=(torch.zeros(18, 1024), None)), "not a log_std=\\(w_ls, b_ls\\) pair"),
     (dict(output="gaussian_evaluate", mask=torch.zeros(8, 18, dtype=torch.bool)),
-     "mask is an argument of the categorical outputs"),
-    (dict(output="sample", seed=1), 'taken is an argument of output="evaluate"'),
-    (dict(output="actions"), 'taken is an argument of output="evaluate"'),
-    (dict(output="gaussian", seed=1), 'taken is an argument of output="evaluate"'),
-    (dict(output="epsilon_greedy", seed=1, epsilon=0.1), 'taken is an argument of output="evaluate"'),
+     'mask is not an argument of output="gaussian_evaluate"'),
+    (dict(output="sample", seed=1), 'taken is not an argument of output="sample"'),
+    (dict(output="actions"), 'taken is not an argument of output="actions"'),
+    (dict(output="gaussian", seed=1), 'taken is not an argument of output="gaussian"'),
+    (dict(output="epsilon_greedy", seed=1, epsilon=0.1), 'taken is not an argument of output="epsilon_greedy"'),
 ])
-def test_check_policy_rejects_bad_evaluate_options(case, reason):
+def test_check_policy_rejects_bad_evaluate_arguments(case, reason):
     with pytest.raises(ValueError, match=reason):
         _check(**case)
 

@@ -178,7 +178,7 @@ G = dict(output="gaussian", seed="seed")
     (dict(bias=False, **G, log_std=("w_ls", "b_ls")), "bias=True"),
     (dict(bias=True, **G, log_std="log_std", squash=True), "state-dependent"),
     (dict(bias=True, **G, log_std="log_std", log_std_bounds=(-5, 1)), "state-dependent"),
-    (dict(bias=True, output="sample", seed="seed", squash=True), "state-dependent"),
+    (dict(bias=True, output="sample", seed="seed", squash=True), 'squash= is not an option of output="sample"'),
     (dict(bias=True, **G, log_std=("w_ls", "b_ls"), log_std_bounds=(1.0,)), "two numbers"),
     (dict(bias=True, **G, log_std=("w_ls", "b_ls"), log_std_bounds=(True, 2.0)), "two numbers"),
     (dict(bias=True, **G, log_std=("w_ls", "b_ls"), log_std_bounds="(-20, 2)"), "two numbers"),
@@ -230,7 +230,7 @@ def _zw(*shape, dtype=torch.bfloat16):
 
 
 @pytest.mark.parametrize("case,reason", [
-    (dict(output="sample"), 'output="gaussian" only'),
+    (dict(output="sample"), 'log_std is not an argument of output="sample"'),
     (dict(log_std=(_zw(18, 1024),)), "tensor or \\(w_ls, b_ls\\)"),
     (dict(log_std=(_zw(18, 1024), _zw(18), _zw(18))), "tensor or \\(w_ls, b_ls\\)"),
     (dict(d_out=129), "1 to 128 actions"),
@@ -254,13 +254,13 @@ def test_check_policy_rejects_a_bad_log_std_pair(case, reason):
     (dict(squash=True), "state-dependent"),
     (dict(squash=False), "state-dependent"),
 ])
-def test_bounds_and_squash_are_refused_with_a_tensor_log_std(kw, reason):
+def test_bounds_and_squash_need_a_log_std_pair(kw, reason):
     from kubetorch_b200.device import mlp
 
     w1, w3 = _w()
     with pytest.raises(ValueError, match=reason):
         mlp._check_policy(w1, w3, (None, None, None), "gaussian", 1, torch.zeros(18), **kw)
-    with pytest.raises(ValueError, match=reason):
+    with pytest.raises(ValueError, match=f'{next(iter(kw))} is not an argument of output="sample"'):
         mlp._check_policy(w1, w3, (None, None, None), "sample", 1, None, **kw)
 
 

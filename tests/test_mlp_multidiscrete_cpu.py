@@ -166,10 +166,10 @@ def test_bad_nvec_raises_at_decoration(nvec, reason):
 
 
 @pytest.mark.parametrize("kwargs", [{}, {"output": "logits"}, {"output": "gaussian", "seed": 1, "log_std": "s"}])
-def test_nvec_is_refused_with_logits_and_gaussian(kwargs):
+def test_mapped_refuses_nvec_naming_the_output(kwargs):
     import kubetorch_b200 as kt
 
-    with pytest.raises(ValueError, match="nvec is an option"):
+    with pytest.raises(ValueError, match=f'nvec= is not an option of output="{kwargs.get("output", "logits")}"'):
         kt.mapped("mlp", bias=True, nvec=(3, 3), **kwargs)
 
 
@@ -201,11 +201,11 @@ def test_check_policy_rejects_a_bad_nvec(nvec, reason, output):
 
 
 @pytest.mark.parametrize("output,extra", [("logits", {}), ("gaussian", {"seed": 1})])
-def test_check_policy_refuses_nvec_with_logits_and_gaussian(output, extra):
+def test_check_policy_refuses_nvec_naming_the_output(output, extra):
     from kubetorch_b200.device import mlp
 
     w1, w3 = _w()
-    with pytest.raises(ValueError, match="nvec is an option"):
+    with pytest.raises(ValueError, match=f'nvec is not an argument of output="{output}"'):
         mlp._check_policy(w1, w3, (None, None, None), output, nvec=(9, 9), **extra)
 
 

@@ -125,20 +125,21 @@ REFUSALS = [
     (dict(taken=torch.zeros(37, dtype=torch.int64)), "taken is not an argument"),
     (dict(action=torch.zeros(37, 6)), "action is not an argument"),
     (dict(td=_td(policy="greedy")), "policy must be one of"),
-    (dict(td=_td(alpha=0.2)), "alpha is not an argument of policy=\"deterministic\""),
-    (dict(log_std_bounds=(-5, 2)), "log_std_bounds is not an argument of policy=\"deterministic\""),
+    (dict(td=_td(alpha=0.2)), 'alpha is not an argument of output="td_target", policy="deterministic"'),
+    (dict(log_std_bounds=(-5, 2)), 'log_std_bounds is not an argument of output="td_target", policy="deterministic"'),
     (dict(seed=None), "takes a seed exactly when it takes noise"),
     (dict(noise=-1.0), "noise must be >= 0"),
-    (dict(td=_td(policy="gaussian", alpha=0.2)), "noise is not an argument of policy=\"gaussian\""),
+    (dict(td=_td(policy="gaussian", alpha=0.2)), 'noise is not an argument of output="td_target", policy="gaussian"'),
     (dict(td=_td(policy="gaussian"), noise=None, noise_clip=None), "alpha is required"),
-    (dict(td=_td(policy="gaussian", alpha=0.2), noise=None, noise_clip=None), "log_std=(w_ls, b_ls) is required"),
+    (dict(td=_td(policy="gaussian", alpha=0.2), noise=None, noise_clip=None),
+     'log_std is required with output="td_target", policy="gaussian"'),
     (dict(td=_td(actor=(None,) * 5)), "actor must be (w1, b1, w2, b2, w3, b3)"),
     (dict(td=_td(reward=torch.zeros(37, dtype=torch.float64))), "reward must be a float32 tensor"),
     (dict(td=_td(done=torch.zeros(37, dtype=torch.bfloat16))), "done must be a float32 tensor"),
     (dict(td=_td(done=torch.zeros(37, 1))), "reward and done must have one shape"),
     (dict(td=_td(reward=torch.zeros(36))), "reward must be a float32 tensor of shape (37,)"),
-    (dict(td=_td(gamma=math.nan)), "gamma must be finite"),
-    (dict(td=_td(gamma="0.99")), "gamma must be a number"),
+    (dict(td=_td(gamma=math.nan)), "gamma must be a finite number"),
+    (dict(td=_td(gamma="0.99")), "gamma must be a finite number, got '0.99'"),
     (dict(twin=(None,) * 3), "twin must be (w1, b1, w2, b2, w3, b3)"),
 ]
 
@@ -157,10 +158,10 @@ def test_the_actor_width_must_match_the_critic():
         _check(td=(bad, "deterministic", r, d, 0.99, None))
 
 
-def test_td_options_are_refused_with_other_outputs():
+def test_check_policy_refuses_td_arguments_naming_the_output():
     obs, c1, c2, actor, ls, r, d = _case()
     with mock.patch.object(torch.Tensor, "is_cuda", property(lambda self: True)):
-        with pytest.raises(ValueError, match='are arguments of output="td_target"'):
+        with pytest.raises(ValueError, match='actor is not an argument of output="logits"'):
             mlp._check_policy(c1[0], c1[4], (c1[1], c1[3], c1[5]), "logits", obs=obs, w2=c1[2],
                               td=(actor, None, None, None, None, None))
 
@@ -189,35 +190,38 @@ MAPPED_REFUSALS = [
     (dict(taken="r"), "taken= is not an option"),
     (dict(action="r"), "action= is not an option"),
     (dict(policy="sample"), "policy= must be"),
-    (dict(alpha=0.2), "alpha= is not an option of policy=\"deterministic\""),
-    (dict(log_std=("a", "b")), "log_std= is not an option of policy=\"deterministic\""),
+    (dict(alpha=0.2), 'alpha= is not an option of output="td_target", policy="deterministic"'),
+    (dict(log_std=("a", "b")), 'log_std= is not an option of output="td_target", policy="deterministic"'),
     (dict(seed=None), "seed= exactly when it takes noise="),
     (dict(noise=-1.0), "noise must be >= 0"),
-    (dict(policy="gaussian"), "noise= is not an option of policy=\"gaussian\""),
-    (dict(policy="gaussian", noise=None, noise_clip=None, seed=None), "seed= is required with policy=\"gaussian\""),
+    (dict(policy="gaussian"), 'noise= is not an option of output="td_target", policy="gaussian"'),
+    (dict(policy="gaussian", noise=None, noise_clip=None, seed=None),
+     'seed= is required with output="td_target", policy="gaussian"'),
     (dict(policy="gaussian", noise=None, noise_clip=None), "alpha= is required"),
-    (dict(policy="gaussian", noise=None, noise_clip=None, alpha=math.inf), "alpha must be a finite number"),
-    (dict(policy="gaussian", noise=None, noise_clip=None, alpha=0.2), "log_std= must name the two"),
+    (dict(policy="gaussian", noise=None, noise_clip=None, alpha=math.inf, log_std=("a", "b")),
+     "alpha must be a finite number"),
+    (dict(policy="gaussian", noise=None, noise_clip=None, alpha=0.2),
+     'log_std= is required with output="td_target", policy="gaussian"'),
     (dict(squash=1), "squash must be True or False"),
     (dict(actor=("a1", "a2", "a3")), "actor must name the actor's 6 call arguments"),
     (dict(twin=("v1",)), "twin must name the second critic's 6"),
     (dict(reward=None), "reward= is required"),
-    (dict(done=3), "done= is required"),
+    (dict(done=3), "done must be the name of a call argument"),
     (dict(gamma=None), "gamma= is required"),
-    (dict(gamma=math.nan), "gamma= is required with output=\"td_target\" and must be a finite number"),
+    (dict(gamma=math.nan), "gamma must be a finite number, got nan"),
     (dict(reward="nope"), "'nope' is not an argument"),
 ]
 
 
 @pytest.mark.parametrize("over,msg", MAPPED_REFUSALS, ids=[m for _, m in MAPPED_REFUSALS])
-def test_mapped_refuses_with_a_reason(over, msg):
+def test_mapped_refuses_td_options_with_a_reason(over, msg):
     with pytest.raises(ValueError) as e:
         _mapped(**over)
     assert msg in str(e.value), str(e.value)
 
 
-def test_mapped_refuses_td_options_elsewhere():
-    with pytest.raises(ValueError, match='options of output="td_target"'):
+def test_mapped_refuses_td_options_naming_the_output():
+    with pytest.raises(ValueError, match='gamma= is not an option of output="critic"'):
         kt.mapped("mlp", output="critic", action="act", gamma=0.99)(lambda obs, w1, w2, w3, act: None)
     with pytest.raises(ValueError, match="options of the 'mlp' op"):
         kt.mapped("scale", reward="r")(lambda x, r: None)

@@ -97,10 +97,10 @@ def test_value_option_is_recorded_on_the_spec(output, extra):
 
 
 @pytest.mark.parametrize("kwargs,reason", [
-    ({"bias": True, "output": "actions"}, "sample"),
-    ({"bias": True, "output": "logits"}, "sample"),
-    ({"bias": True, "output": "both"}, "sample"),
-    ({"bias": True}, "sample"),
+    ({"bias": True, "output": "actions"}, 'value= is not an option of output="actions"'),
+    ({"bias": True, "output": "logits"}, 'value= is not an option of output="logits"'),
+    ({"bias": True, "output": "both"}, 'value= is not an option of output="both"'),
+    ({"bias": True}, 'value= is not an option of output="logits"'),
     ({"bias": False, "output": "sample", "seed": 1}, "bias=True"),
     ({"output": "sample", "seed": 1}, "bias=True"),
     ({"bias": True, "output": "sample", "seed": 1, "value_": "wv"}, "two call arguments"),
@@ -199,11 +199,11 @@ BIASED = (None, None, torch.zeros(18, dtype=torch.bfloat16))
 
 
 @pytest.mark.parametrize("output", ["logits", "actions", "both"])
-def test_check_policy_refuses_a_value_with_greedy_outputs(output):
+def test_check_policy_refuses_a_value_naming_the_output(output):
     from kubetorch_b200.device import mlp
 
     w1, w3 = _w()
-    with pytest.raises(ValueError, match="value is an argument"):
+    with pytest.raises(ValueError, match=f'value is not an argument of output="{output}"'):
         mlp._check_policy(w1, w3, (None, None, None), output, value=(torch.zeros(1, 1024, dtype=torch.bfloat16), None))
 
 
