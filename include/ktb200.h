@@ -338,7 +338,12 @@ int ktb_mlp_bf16_pushed(int dev, const void* stage_local, size_t stage_stride, s
  * Linear(d_hidden, d_out)  with biases, a head of any width 1 <= d_out <= 256, and greedy actions.
  *   - Layer l is act(fp32 sum of the exact bf16 products + b_l) rounded ONCE to nearest-even bf16: the bias
  *     joins the fp32 accumulator before the ReLU (F.linear / nn.Linear, one rounding).  This differs from
- *     `x @ w.t() + b` written as two eager ops, which rounds twice.  ReLU is fmaxf, as in ktb_mlp_bf16.
+ *     `x @ w.t() + b` written as two eager ops, which rounds twice.  ReLU is torch.relu, as in ktb_mlp_bf16: a NaN
+ *     pre-activation stays NaN (max.NaN, not fmaxf), +inf stays +inf, -inf becomes 0.
+ *   - IEEE special values follow torch (measured on H100 80GB HBM3): the tensor cores keep NaN and +-inf from their
+ *     bf16 inputs and give NaN for inf * 0 and +inf - inf; an fp32 sum past FLT_MAX is +-inf; a result on the bf16
+ *     overflow tie rounds to +-inf; subnormal inputs and results are not flushed.  So a NaN observation row gives NaN
+ *     outputs in that row only, and a NaN weight or bias of any layer gives NaN outputs in every row it reaches.
  *   - b1 [d_hidden], b2 [d_hidden], b3 [d_out] bf16; each may be NULL (no bias on that layer).
  *   - logits [M, d_out] bf16 and/or actions [M] int64; either may be NULL, not both.  actions[i] =
  *     torch.argmax(logits[i]) over the ROUNDED logits: ties go to the lowest index, NaN is greater than any
@@ -877,7 +882,8 @@ int ktb_mlp_bf16_policy_deterministic_pushed(int dev, const void* stage_local, s
  *     x = [obs | bf16(act)]                     obs bf16 [M, d_in], act fp32 [M, d_act]
  *     h = relu(x W1ᵀ + b1), h = relu(h W2ᵀ + b2), q = fp32(h W3ᵀ + b3)      q fp32 [M]
  *   - Every layer follows ktb_mlp_bf16_policy's rules: the bias joins the fp32 accumulator, each layer rounds once to
- *     bf16, ReLU is fmaxf (so a NaN or infinite action need not give a NaN q: a NaN pre-activation becomes 0).
+ *     bf16, ReLU keeps NaN as torch.relu does (so a NaN action gives a NaN q, and an infinite one a NaN q wherever
+ *     the torch definition gives one).
  *   - The action is rounded to bf16 once, to nearest even, as .to(torch.bfloat16) does.  q is the bf16 head output
  *     widened exactly.
  *   - W1p is the user's W1 [d_hidden, d_in + d_act] padded with zero columns to [d_hidden, d_in + 64]; layer 1 runs

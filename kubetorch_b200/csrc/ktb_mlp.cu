@@ -241,9 +241,18 @@ __device__ __forceinline__ float gumbel_of(uint32_t x) {
   return -logf(-logf(u));
 }
 
+// torch.relu: max.NaN returns NaN when an operand is NaN (fmaxf would return the 0), +inf stays +inf and -inf gives
+// +0.0.  Before a bf16 rounding ptxas folds it into the conversion (F2FP.RELU, which keeps NaN), so it costs no
+// instruction.  A zero's sign may differ from torch's; a hidden zero's sign never reaches an output.
+__device__ __forceinline__ float relu_keep_nan(float v) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(v));
+  return r;
+}
+
 // One column pair (col, col + 1) of a layer in rows r and r + 8: y0 = act(a0 + bias, a1 + bias) of row r, y1 of row
-// r + 8, each rounded once to bf16; act is ReLU in the hidden layers and the identity in the head.  A column >= n_valid
-// gets no bias.
+// r + 8, each rounded once to bf16; act is ReLU (relu_keep_nan: a NaN stays NaN, as in torch) in the hidden layers
+// and the identity in the head.  A column >= n_valid gets no bias.
 template <bool RELU>
 __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a3, const __nv_bfloat16* bias, int col,
                                            int n_valid, __nv_bfloat162& y0, __nv_bfloat162& y1) {
@@ -262,7 +271,7 @@ __device__ __forceinline__ void layer_pair(float a0, float a1, float a2, float a
   }
   if constexpr (RELU) {
 #pragma unroll
-    for (int q = 0; q < 4; ++q) v[q] = fmaxf(v[q], 0.f);
+    for (int q = 0; q < 4; ++q) v[q] = relu_keep_nan(v[q]);
   }
   y0 = __floats2bfloat162_rn(v[0], v[1]);
   y1 = __floats2bfloat162_rn(v[2], v[3]);
