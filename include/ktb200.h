@@ -993,6 +993,66 @@ int ktb_mlp_bf16_td_target_gaussian_pushed(
     size_t reward_offset, size_t done_offset, float gamma, float alpha, float* y, void* scratch, void* ctrl_local,
     void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* DQN and Double DQN targets in one call, forward only: the greedy next action, the target network's Q at it and the
+ * Bellman target.  For rows next_obs (bf16 [M, d_in]) with reward and done (fp32 [M]), the target Q-network (W1, b1,
+ * W2, b2, W3, b3) and, for Double DQN, an online Q-network (oW1, ob1, oW2, ob2, oW3, ob3) of the same d_in, d_hidden
+ * and d_out:
+ *   - Qt and Qo are the bf16 logits ktb_mlp_bf16_policy computes for the target and the online network.
+ *   - The selector S is Qo with an online network (Double DQN) and Qt without one (DQN); the _masked entries rank
+ *     S.masked_fill(~legal, -inf) with the legal-action mask of the next states (uint8 [M, d_out], nonzero: legal).
+ *   - a*[i] = torch.argmax(S[i]) with the greedy entries' rules (ties to the lowest column, the first NaN wins, -0 equals
+ *     +0, a row whose ranked values are all -inf or that has no legal column gets 0): bit for bit the actions of
+ *     ktb_mlp_bf16_policy(_masked) on the selecting network.
+ *   - q[i] = fp32(Qt[i, a*[i]]), read from the UNMASKED target logits and widened exactly.  A terminal next state
+ *     often has no legal action, and there done = 1: the unmasked read gives Qt[i, 0] and y = r exactly, where a masked
+ *     one would give 0 * -inf = NaN.
+ *   - y[i] = __fadd_rn(r, __fmul_rn(__fmul_rn(gamma, __fsub_rn(1.f, d)), q)), fp32 [M] (may be a peer pointer): the TD
+ *     targets' expression and rounding, no FMA contraction.  IEEE cases follow: a NaN in the selector picks that
+ *     column (DQN's y is then NaN; Double DQN's is the target's value there), and an infinite q with done = 1 or with
+ *     gamma = 0 gives NaN.  Nothing is drawn, so y does not depend on the chunk size, the form or the rank split, and
+ *     DQN's y equals Double DQN's with online = target bit for bit.
+ *   - Per row chunk on one stream: Double DQN runs the online network with the greedy head (actions only) into chunk
+ *     scratch, then the target network, whose head reads a* there; DQN runs the target network alone.  scratch holds
+ *     ktb_mlp_dqn_target_scratch_bytes(M, d_hidden): the two hidden activations and the chunk's int64 a*.  No M-sized
+ *     intermediate is written.
+ *   - Arguments: ktb_mlp_bf16_policy's up to b3 (the target network), the online network's six pointers (all six NULL:
+ *     DQN), mask (the _masked entries), reward, done (rd_offset in the pushed forms), gamma, y, then scratch and stage
+ *     (or the push arguments) and stream.
+ *   - Checks, in this order: every check of ktb_mlp_bf16_policy (_masked) on the target network, d_out > 256 being
+ *     KTB_ERR_UNSUPPORTED; then the online network's pointers and alignment, checked as a twin critic's second (a NULL
+ *     oW1 with another of its six pointers non-NULL is KTB_ERR_ARG); then a non-finite gamma is KTB_ERR_ARG; then, with
+ *     M > 0, a NULL or not 4-byte aligned reward, done (pull forms) or y is KTB_ERR_ARG.  An empty pushed shard
+ *     (M == 0) may pass NULL outputs and still publishes its ack.  The pushed forms read (mask, then) rd from their
+ *     sides (ktb_mlp_bf16_pushed): mask d_out bytes per row, and rd one side of interleaved fp32 (reward, done) pairs,
+ *     8 bytes per row, 8-byte aligned (the kernel reads reward[2i] and done[2i] there).  Writes stay inside y[M],
+ *     scratch and stage. */
+size_t ktb_mlp_dqn_target_scratch_bytes(size_t M, int d_hidden);
+int ktb_mlp_bf16_dqn_target(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                            const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                            const void* oW1, const void* ob1, const void* oW2, const void* ob2, const void* oW3,
+                            const void* ob3, const float* reward, const float* done, float gamma, float* y,
+                            void* scratch, void* stage, uintptr_t stream);
+int ktb_mlp_bf16_dqn_target_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                   int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                   const void* b2, const void* W3, const void* b3, const void* oW1, const void* ob1,
+                                   const void* oW2, const void* ob2, const void* oW3, const void* ob3,
+                                   size_t rd_offset, float gamma, float* y, void* scratch, void* ctrl_local,
+                                   void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
+                                   uintptr_t stream);
+int ktb_mlp_bf16_dqn_target_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                   const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                   const void* b3, const void* oW1, const void* ob1, const void* oW2, const void* ob2,
+                                   const void* oW3, const void* ob3, const uint8_t* mask, const float* reward,
+                                   const float* done, float gamma, float* y, void* scratch, void* stage,
+                                   uintptr_t stream);
+int ktb_mlp_bf16_dqn_target_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                          int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                          const void* b2, const void* W3, const void* b3, const void* oW1,
+                                          const void* ob1, const void* oW2, const void* ob2, const void* oW3,
+                                          const void* ob3, size_t mask_offset, size_t rd_offset, float gamma, float* y,
+                                          void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                          size_t chunk_rows, unsigned long long seq, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

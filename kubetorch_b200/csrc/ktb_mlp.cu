@@ -483,7 +483,9 @@ struct HeadEval {
 // fp32.  The second head of a twin also reads q_other [rows], the first head's Q, and stores q_min = min(Q2, Q1)
 // (critic_epilogue).  y != null marks the last critic head of a TD target instead: it stores no Q but
 // y = r + γ·(1 − d)·(t − α·logp) (t its Q, or the twin's minimum; the α term only with logp) from reward, done and
-// logp [rows].
+// logp [rows].  In a kSample head y != null marks a DQN target's target network (dqn_pass): y = r + γ·(1 − d)·q with
+// q its value at the action sel [rows] (Double DQN's, chosen by the online network) or at its own greedy action
+// (sel null), reading reward[r·rd_stride] and done[r·rd_stride] (2: the interleaved pairs of the pushed forms).
 struct HeadQ {
   float* q = nullptr;
   const float* q_other = nullptr;
@@ -493,15 +495,17 @@ struct HeadQ {
   const float* logp = nullptr;
   float* y = nullptr;
   float gamma = 0.f, alpha = 0.f;
+  const int64_t* sel = nullptr;
+  int rd_stride = 1;
 
-  // The same outputs from row r0 of the call on.  A TD target's critics (`scratch`) read and write q, q_other and
-  // logp in chunk-sized scratch from the chunk's first row, so only its reward, done and y move.
+  // The same outputs from row r0 of the call on.  A TD or DQN target's heads (`scratch`) read and write q, q_other,
+  // logp and sel in chunk-sized scratch from the chunk's first row, so only its reward, done and y move.
   HeadQ from_row(size_t r0, bool scratch) const {
     HeadQ h = *this;
     if (scratch) {
       if (y) {
-        h.reward += r0;
-        h.done += r0;
+        h.reward += r0 * rd_stride;
+        h.done += r0 * rd_stride;
         h.y += r0;
       }
     } else if (q) {
@@ -512,6 +516,12 @@ struct HeadQ {
     return h;
   }
 };
+
+// The Bellman target of both target heads: y = r + γ·(1 − d)·t, each operation rounded once in the order torch
+// evaluates reward + gamma * (1 - done) * t on fp32 tensors with a Python-float γ (no contraction).
+__device__ __forceinline__ float bellman_target(float r, float d, float gamma, float t) {
+  return __fadd_rn(r, __fmul_rn(__fmul_rn(gamma, __fsub_rn(1.f, d)), t));
+}
 
 // The epilogue of a critic head (HeadQ) in the 64-wide kGaussian instantiation: column 0 of rows row and row + 8, held
 // by lane 0 of each quad in acc[0] and acc[2], gets the bias and one rounding to bf16 (layer_pair, as every head) and
@@ -542,7 +552,7 @@ __device__ __forceinline__ void critic_epilogue(const float (&acc)[BLOCK_N / 2],
       continue;
     }
     if (hq.logp != nullptr) t = __fsub_rn(t, __fmul_rn(hq.alpha, hq.logp[r]));
-    hq.y[r] = __fadd_rn(hq.reward[r], __fmul_rn(__fmul_rn(hq.gamma, __fsub_rn(1.f, hq.done[r])), t));
+    hq.y[r] = bellman_target(hq.reward[r], hq.done[r], hq.gamma, t);
   }
 }
 
@@ -894,6 +904,78 @@ __device__ __forceinline__ void epsilon_pass(Slot slot, const ColBits<BLOCK_N> (
   }
 }
 
+// The DQN target's pass of sample_epilogue (hq.y != null) over the bf16 pairs that its pass 1 parked in the ring: the
+// target network's head.  For each of the thread's rows r = row + 8h:
+//   * the action a: hq.sel[r] (Double DQN: the online network's greedy action, which every lane of the quad reads), or
+//     with sel null (DQN) the greedy action of this head's live columns, ranked as epsilon_pass ranks g (argmax_before
+//     in the greedy epilogue's per-thread and quad order; 0 when their values are all -inf or there are none);
+//   * q: the lane whose columns include a reads its parked value with no live-bit test, so q is the UNMASKED target
+//     value widened exactly (a terminal state with no legal action reads column 0, and done = 1 then gives y = r
+//     rather than 0·(−inf)), and shfl.xor shares it across the quad, as evaluate_pass shares y_a;
+//   * lane 0 of the quad stores y[r] = bellman_target(reward[r·s], done[r·s], γ, q), s = hq.rd_stride.
+template <int BLOCK_N, typename Slot>
+__device__ __forceinline__ void dqn_pass(Slot slot, const ColBits<BLOCK_N> (&live)[2], int d, int col0, int row,
+                                         bool st0, bool st1, const HeadQ& hq) {
+  const int lane = threadIdx.x & 31;
+  int a[2] = {0, 0};
+  if (hq.sel != nullptr) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (h ? st1 : st0) a[h] = (int)hq.sel[row + 8 * h];
+  } else {
+    float best[2] = {-INFINITY, -INFINITY};
+    int best_col[2] = {INT_MAX, INT_MAX};
+#pragma unroll 1
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int col = col0 + 8 * j;
+      if (col >= d) break;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const __nv_bfloat162 y = *slot(2 * j + h);
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const float v = c ? __high2float(y) : __low2float(y);
+          if (((live[h] >> (2 * j + c)) & 1) && argmax_before(v, col + c, best[h], best_col[h])) {
+            best[h] = v;
+            best_col[h] = col + c;
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int m = 1; m <= 2; m <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best[h], m);
+        const int oc = __shfl_xor_sync(0xffffffffu, best_col[h], m);
+        if (argmax_before(ov, oc, best[h], best_col[h])) {
+          best[h] = ov;
+          best_col[h] = oc;
+        }
+      }
+      a[h] = best[h] == -INFINITY ? 0 : best_col[h];
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int owner = (a[h] >> 1) & 3;
+    float q = 0.f;
+    if (owner == (lane & 3)) {
+      const __nv_bfloat162 y = *slot(2 * ((a[h] - col0) >> 3) + h);
+      q = a[h] & 1 ? __high2float(y) : __low2float(y);
+    }
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      const float oq = __shfl_xor_sync(0xffffffffu, q, m);
+      if ((lane ^ owner) & m) q = oq;   // the partner is nearer the owner: after m = 1, 2 every lane holds q
+    }
+    if ((lane & 3) == 0 && (h ? st1 : st0)) {
+      const size_t r = (size_t)(row + 8 * h) * hq.rd_stride;
+      hq.y[row + 8 * h] = bellman_target(hq.reward[r], hq.done[r], hq.gamma, q);
+    }
+  }
+}
+
 // The sampling epilogue of a head tile (HeadKind::kSample): rows r = row and row + 8 of the thread, global rows
 // row_base + r.  Pass 1 (unrolled over the accumulators) rounds the logits once, parks them as bf16 pairs in the TMA
 // ring as gaussian_epilogue does, and takes each row's largest logit m across the quad (NaN skipped: it reaches the sum
@@ -911,15 +993,15 @@ __device__ __forceinline__ void epsilon_pass(Slot slot, const ColBits<BLOCK_N> (
 // Pass 1 parks column d with the rest; everything ranked, drawn, summed or masked stops at d; store_values reads it.
 // A multi-discrete head (groups.n > 0) takes group_pass in place of the rolled pass: the greedy one as well, whose
 // logits (C, unless null) it also stores.  An ε-greedy head (epsilon != null) takes epsilon_pass in its place, and an
-// evaluating head (ev.actions != null), grouped or not, evaluate_pass.  The single categorical's rolled pass stays as
-// it is.
+// evaluating head (ev.actions != null), grouped or not, evaluate_pass, and a DQN target's target network (hq.y != null)
+// dqn_pass.  The single categorical's rolled pass stays as it is.
 template <int BLOCK_N, int STAGES>
 __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2], const __nv_bfloat16* bias, int col0,
                                                 int n_valid, int row, bool st0, bool st1, int64_t* actions,
                                                 float* log_probs, const uint8_t* mask, uint64_t seed,
                                                 uint64_t row_base, float* values, const HeadGroups& groups,
                                                 __nv_bfloat16* C, const float* epsilon, float* q, float* q_max,
-                                                const HeadEval& ev) {
+                                                const HeadEval& ev, const HeadQ& hq) {
   using S = MlpSmem<BLOCK_N, STAGES>;
   static_assert(BLOCK_N / 64 <= STAGES, "each warp's bf16 pairs fill its 16 A rows of BLOCK_N / 64 stages");
   extern __shared__ uint8_t smem_raw[];
@@ -966,6 +1048,10 @@ __device__ __forceinline__ void sample_epilogue(const float (&acc)[BLOCK_N / 2],
   }
   if (epsilon != nullptr) {
     epsilon_pass<BLOCK_N>(slot, live, d, col0, row, st0, st1, epsilon, actions, q, q_max, seed, row_base);
+    return;
+  }
+  if (hq.y != nullptr) {
+    dqn_pass<BLOCK_N>(slot, live, d, col0, row, st0, st1, hq);
     return;
   }
   const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
@@ -1237,7 +1323,7 @@ enum class HeadKind {
   kGreedy,     // bf16 logits and/or int64 argmax actions (unrolled; the single categorical)
   kSample,     // the rolled categorical head: Gumbel-max int64 actions and fp32 log_probs, or with groups (HeadGroups)
                // greedy or Gumbel-max actions per group, with the logits of "both" or the summed log_probs, or with
-               // epsilon ε-greedy actions and their fp32 Q-values
+               // epsilon ε-greedy actions and their fp32 Q-values, or with hq.y a DQN target
   kGaussian,   // fp32 actions [rows, d_out] (gauss_actions) drawn with log_std, and fp32 log_probs
 };
 
@@ -1292,6 +1378,8 @@ struct HeadOut {
 //     log-probability of the sampled ones, and the logits of a greedy head that stores them (group_pass);
 //   kSample with eg.epsilon: the ε-greedy action of each row with the Q-values of the taken and the greedy action
 //     (epsilon_pass);
+//   kSample with hq.y: a DQN target's target network, y[row] = r + γ·(1 − d)·q with q its unmasked value at the
+//     online network's action hq.sel[row] or at its own (masked) greedy action (dqn_pass);
 //   kSample with ev.actions and kGaussian with ev.gauss_actions: the log-probability and the entropy of given actions
 //     (evaluate_pass, gaussian_epilogue);
 //   kGaussian with sd.det: gauss_actions[row, j] = the deterministic actor's action, tanh(logit_j) (or logit_j) plus
@@ -1338,7 +1426,7 @@ __global__ void __launch_bounds__(kMlpThreads, 1)
     greedy_epilogue<BLOCK_N>(acc, bias, C, out.actions, out.mask, col0, n_valid, row, st0, st1);
   } else if constexpr (KIND == HeadKind::kSample) {
     sample_epilogue<BLOCK_N, STAGES>(acc, bias, col0, n_valid, row, st0, st1, out.actions, out.log_probs, out.mask, out.seed,
-                             out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max, ev);
+                             out.row_base, out.values, out.groups, C, eg.epsilon, eg.q, eg.q_max, ev, hq);
   } else if (BLOCK_N == 64 && (hq.q != nullptr || hq.y != nullptr)) {   // a critic (64-wide tile): column 0 is Q
     critic_epilogue<BLOCK_N>(acc, bias, col0, row, st0, st1, hq);
   } else {
@@ -1510,7 +1598,10 @@ static int launch_action_tile(const float* act, int d_act, void* tile, size_t ro
 // entries) is the second critic, run on the same tile after the first, whose hq also reads the first's q and stores
 // q_min.  `actor` marks the _td_target entries: the critics' action tile is packed from the actions the actor (a
 // deterministic or state-dependent Gaussian head, `actor_hidden` wide) writes into chunk scratch, and the last critic's
-// hq computes the target (`target` marks both critics: their hq reads and writes chunk scratch).
+// hq computes the target (`target` marks both critics: their hq reads and writes chunk scratch).  `dqn` marks the
+// _dqn_target entries: a kSample head whose hq computes the target from the target network's logits (`target` set too),
+// at the actions that `online` (Double DQN; a greedy head, masked with the call's mask) writes into chunk scratch, or
+// without `online` at its own greedy actions under the call's mask.
 struct MlpParams {
   const void *W1, *b1, *W2, *b2, *W3, *b3;
   HeadKind kind;
@@ -1534,6 +1625,8 @@ struct MlpParams {
   const MlpParams* actor = nullptr;
   int actor_hidden = 0;
   bool target = false;
+  bool dqn = false;
+  const MlpParams* online = nullptr;
 
   // A critic, in the 64-wide kGaussian instantiation (one column, Q): act [M, d_act] fp32 (null in the pushed forms)
   // in, q [M] fp32 out.
@@ -1671,7 +1764,7 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
       case HeadKind::kSample:
         if (o.groups.greedy)   // a greedy multi-discrete head takes what the greedy entries take
           KTB_REQUIRE(o.logits || o.actions, KTB_ERR_ARG, "%s: logits and actions are both null", fn);
-        else if (!p.eps && !p.evaluate)   // ε-greedy and evaluating heads: checked by mlp_run after every other check
+        else if (!p.eps && !p.evaluate && !p.dqn)   // ε-greedy, evaluating and DQN target heads: checked by mlp_run
           KTB_REQUIRE(o.actions && o.log_probs, KTB_ERR_ARG, "%s: actions and log_probs are required", fn);
         break;
       case HeadKind::kGaussian:
@@ -1714,7 +1807,7 @@ static int mlp_check(const char* fn, size_t M, int d_in, int d_hidden, int d_out
 //           inputs were pushed into the same half beside the rows: `sides`, up to two regions (PushSide, src null)
 //           named for what they hold, "mask" (a masked head's legal-action mask), "epsilon" (an ε-greedy head's ε,
 //           fp32), "taken" (an evaluating head's given actions), "act" (a critic's actions, fp32), or "reward" and
-//           "done" (a TD target's, fp32).
+//           "done" (a TD target's, fp32), or "rd" (a DQN target's interleaved fp32 (reward, done) pairs).
 // The pull forms read a mask in place (MlpParams::out.mask), a peer pointer where obs is one: it is read once per row.
 struct MlpFeed {
   const void* in;
@@ -1748,11 +1841,14 @@ struct MlpFeed {
 };
 
 // The chunk scratch of a call, in this order: two hidden activations [chunk, d_hidden] bf16 (a TD target's actor and
-// critics share them, at the wider d_hidden), a critic's action tile [chunk, 64] bf16, then a TD target's actions
-// [chunk, d_act], log-probabilities [chunk] and first Q [chunk], fp32 (ktb_mlp_td_target_scratch_bytes).
+// critics share them, at the wider d_hidden, and a DQN target's two networks), a critic's action tile [chunk, 64] bf16,
+// then a TD target's actions [chunk, d_act], log-probabilities [chunk] and first Q [chunk], fp32
+// (ktb_mlp_td_target_scratch_bytes).  A DQN target's selected actions [chunk] int64 take the place of the action tile
+// (ktb_mlp_dqn_target_scratch_bytes).
 struct MlpScratch {
   __nv_bfloat16 *h1, *h2, *tile;
   float *act, *logp, *q1;
+  int64_t* sel;
 
   static MlpScratch carve(void* scratch, size_t chunk, int d_hidden, int d_act) {
     MlpScratch s;
@@ -1762,6 +1858,7 @@ struct MlpScratch {
     s.act = reinterpret_cast<float*>(s.tile + chunk * (size_t)kMlpBlockK);
     s.logp = s.act + chunk * (size_t)d_act;
     s.q1 = s.logp + chunk;
+    s.sel = reinterpret_cast<int64_t*>(s.tile);
     return s;
   }
 };
@@ -1791,6 +1888,17 @@ static int head_checks(const char* fn, size_t M, int d_out, const MlpParams& p) 
   return KTB_OK;
 }
 
+// The weights and biases of a second network of the same shapes (a twin's second critic, a Double DQN target's online
+// network): non-null weights, and the alignment mlp_check asks of the first's.
+static int second_network_check(const char* fn, size_t M, const MlpParams& t) {
+  KTB_REQUIRE(t.W1 && t.W2 && t.W3, KTB_ERR_ARG, "%s: null argument", fn);
+  KTB_REQUIRE(M == 0 || (((uintptr_t)t.b1 | (uintptr_t)t.b2 | (uintptr_t)t.b3) & 1) == 0, KTB_ERR_ARG,
+              "%s: logits and biases must be 2-byte aligned", fn);
+  KTB_REQUIRE((((uintptr_t)t.W1 | (uintptr_t)t.W2 | (uintptr_t)t.W3) & 15) == 0, KTB_ERR_ARG,
+              "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
+  return KTB_OK;
+}
+
 // One MLP call of any head and form: every entry's checks, then one chunk loop.  An empty plain or staged call returns
 // right after the device check; an empty pushed shard runs every check and still publishes its ack, which the root's
 // ktb_push_wait waits for.  A pushed entry's side regions (check_push_sides) are checked right after its stage_stride,
@@ -1809,7 +1917,10 @@ static int head_checks(const char* fn, size_t M, int d_out, const MlpParams& p) 
 // them), then d_act in [1, 64], then (skipped for an empty call) act and its outputs non-null and 4-byte aligned.  A TD
 // target entry runs every check of the critic (twin) entry but those of act and the Q outputs, then every check of its
 // actor's standalone entry (ktb_mlp_bf16_policy_deterministic or _gaussian_state at d_out = d_act, the actor's
-// d_hidden), then gamma and alpha finite, then (skipped for an empty call) reward, done and y non-null and aligned.
+// d_hidden), then gamma and alpha finite, then (skipped for an empty call) reward, done and y non-null and aligned.  A
+// DQN target entry runs every check of ktb_mlp_bf16_policy (_masked) on the target network, then the online network's
+// as a twin's second critic's, then gamma finite, then (skipped for an empty call) reward, done and y non-null and
+// aligned.
 static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out, const MlpParams& p,
                    const MlpFeed& f, void* scratch, uintptr_t stream) {
   int rc = require_device(dev);
@@ -1832,12 +1943,8 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
   rc = mlp_check(fn, M, d_in, d_hidden, d_out, p, f.in, scratch, f.stage);
   if (rc) return rc;
   if (p.twin) {
-    const MlpParams& t = *p.twin;
-    KTB_REQUIRE(t.W1 && t.W2 && t.W3, KTB_ERR_ARG, "%s: null argument", fn);
-    KTB_REQUIRE(M == 0 || (((uintptr_t)t.b1 | (uintptr_t)t.b2 | (uintptr_t)t.b3) & 1) == 0, KTB_ERR_ARG,
-                "%s: logits and biases must be 2-byte aligned", fn);
-    KTB_REQUIRE((((uintptr_t)t.W1 | (uintptr_t)t.W2 | (uintptr_t)t.W3) & 15) == 0, KTB_ERR_ARG,
-                "%s: obs, weights, scratch and stage must be 16-byte aligned", fn);
+    rc = second_network_check(fn, M, *p.twin);
+    if (rc) return rc;
   }
   if (f.pushed) {
     const size_t n_chunks = (M + f.chunk_rows - 1) / f.chunk_rows;
@@ -1872,6 +1979,19 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
                   KTB_ERR_ARG, "%s: act and the outputs must be 4-byte aligned", fn);
     }
   }
+  if (p.dqn) {
+    if (p.online) {
+      rc = second_network_check(fn, M, *p.online);
+      if (rc) return rc;
+    }
+    const HeadQ& t = p.hq;
+    KTB_REQUIRE(std::isfinite(t.gamma), KTB_ERR_ARG, "%s: gamma=%g must be finite", fn, (double)t.gamma);
+    if (M > 0) {
+      KTB_REQUIRE(((t.reward && t.done) || f.pushed) && t.y, KTB_ERR_ARG, "%s: reward, done and y are required", fn);
+      KTB_REQUIRE((((uintptr_t)t.reward | (uintptr_t)t.done | (uintptr_t)t.y) & 3) == 0, KTB_ERR_ARG,
+                  "%s: reward, done and y must be 4-byte aligned", fn);
+    }
+  }
   const size_t chunk = std::min(f.chunk_rows, M);
   const MlpScratch s = MlpScratch::carve(scratch, chunk, std::max(d_hidden, p.actor_hidden), p.d_act);
   // a TD target's actor and critics with their chunk scratch: the actor writes its actions (and log-probabilities)
@@ -1901,6 +2021,14 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
                   "%s: reward, done and y must be 4-byte aligned", fn);
     }
     if (actor.std.state) t.logp = s.logp;
+  }
+  // a Double DQN target's online network writes the chunk's actions into chunk scratch, where the target's head reads
+  // them
+  MlpParams online{};
+  if (p.online) {
+    online = *p.online;
+    online.out.actions = s.sel;
+    c1.hq.sel = s.sel;
   }
   HeadGroups groups = p.out.groups;
   if (p.grouped && M > 0) {
@@ -1951,7 +2079,15 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
       t.reward = static_cast<const float*>(f.side(half, "reward"));
       t.done = static_cast<const float*>(f.side(half, "done"));
     }
+    if (p.dqn) {   // interleaved (reward, done) pairs
+      c1.hq.reward = static_cast<const float*>(f.side(half, "rd"));
+      c1.hq.done = c1.hq.reward + 1;
+      c1.hq.rd_stride = 2;
+    }
   }
+  // Double DQN masks the online network's ranking; the target's value is read unmasked
+  const uint8_t* online_mask = out.mask;
+  if (p.online) out.mask = nullptr;
   uint8_t* ctrl = static_cast<uint8_t*>(f.ctrl);
   __nv_bfloat16* stg = static_cast<__nv_bfloat16*>(f.stage);
   cudaStream_t side = device_info(dev)->stream_stage;   // pulls the next chunk while this one computes
@@ -2001,6 +2137,13 @@ static int mlp_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, in
     }
     // evs[3..4] are null unless staged; every chain after the first records `consumed` again after its layer 1
     cudaEvent_t consumed = evs[3 + (int)(c & 1)];
+    if (p.online) {   // the chunk's greedy actions into chunk scratch: pointers from its row 0
+      HeadOut so = online.out;
+      so.mask = online_mask ? online_mask + r0 * d_out : nullptr;
+      rc = mlp_chunk(dev, online, so, HeadEps{}, HeadEval{}, a1, nullptr, s.h1, s.h2, 0, rows, d_in, d_hidden, d_out,
+                     consumed, st);
+      if (rc) return rc;
+    }
     if (p.actor) {   // the chunk's actions into chunk scratch: pointers from its row 0, noise of its global rows
       HeadOut ao = actor.out;
       ao.row_base += r0;
@@ -2763,6 +2906,11 @@ size_t ktb_mlp_td_target_scratch_bytes(size_t M, int d_hidden_actor, int d_hidde
   return ktb_mlp_critic_scratch_bytes(M, std::max(d_hidden_actor, d_hidden)) + rows * (4 * (size_t)d_act + 8);
 }
 
+size_t ktb_mlp_dqn_target_scratch_bytes(size_t M, int d_hidden) {
+  const size_t rows = std::min<size_t>(M, (size_t)g_mlp_chunk_rows);
+  return ktb_mlp_scratch_bytes(M, d_hidden) + rows * 8;
+}
+
 }  // extern "C"
 
 namespace ktb {
@@ -2787,6 +2935,24 @@ static int td_target_run(const char* fn, int dev, size_t M, int d_in, int d_hidd
   p.actor = &actor;
   p.actor_hidden = d_hidden_actor;
   return mlp_run(fn, dev, M, d_in, d_hidden, 1, p, f, scratch, stream);
+}
+
+// A DQN target: the target network (w[0..5]) in the kSample instantiations, whose hq computes y, and unless the six
+// pointers w[6..11] are all null Double DQN's online network, a greedy head; `masked` marks the _masked entries (mask
+// null in the pushed forms).  A partly given online network has a null weight, which mlp_run refuses.
+static int dqn_target_run(const char* fn, int dev, size_t M, int d_in, int d_hidden, int d_out,
+                          const void* const (&w)[12], bool masked, const uint8_t* mask, const float* reward,
+                          const float* done, float gamma, float* y, const MlpFeed& f, void* scratch, uintptr_t stream) {
+  const MlpParams online{w[6], w[7], w[8], w[9], w[10], w[11], HeadKind::kGreedy};
+  MlpParams p{w[0], w[1], w[2], w[3], w[4], w[5], HeadKind::kSample};
+  if (masked) p = p.with_mask(mask);
+  if (std::any_of(w + 6, w + 12, [](const void* x) { return x != nullptr; })) p.online = &online;
+  p.dqn = p.target = true;
+  p.hq.reward = reward;
+  p.hq.done = done;
+  p.hq.gamma = gamma;
+  p.hq.y = y;
+  return mlp_run(fn, dev, M, d_in, d_hidden, d_out, p, f, scratch, stream);
 }
 
 }  // namespace ktb
@@ -2859,6 +3025,58 @@ int ktb_mlp_bf16_td_target_gaussian_pushed(
                        MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
                            .with_side("reward", reward_offset, 4, 4).with_side("done", done_offset, 4, 4),
                        scratch, stream);
+}
+
+int ktb_mlp_bf16_dqn_target(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out, const void* W1,
+                            const void* b1, const void* W2, const void* b2, const void* W3, const void* b3,
+                            const void* oW1, const void* ob1, const void* oW2, const void* ob2, const void* oW3,
+                            const void* ob3, const float* reward, const float* done, float gamma, float* y,
+                            void* scratch, void* stage, uintptr_t stream) {
+  return dqn_target_run("ktb_mlp_bf16_dqn_target", dev, M, d_in, d_hidden, d_out,
+                        {W1, b1, W2, b2, W3, b3, oW1, ob1, oW2, ob2, oW3, ob3}, false, nullptr, reward, done, gamma, y,
+                        MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_dqn_target_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                   int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                   const void* b2, const void* W3, const void* b3, const void* oW1, const void* ob1,
+                                   const void* oW2, const void* ob2, const void* oW3, const void* ob3,
+                                   size_t rd_offset, float gamma, float* y, void* scratch, void* ctrl_local,
+                                   void* ctrl_root_peer, int rank, size_t chunk_rows, unsigned long long seq,
+                                   uintptr_t stream) {
+  return dqn_target_run("ktb_mlp_bf16_dqn_target_pushed", dev, M, d_in, d_hidden, d_out,
+                        {W1, b1, W2, b2, W3, b3, oW1, ob1, oW2, ob2, oW3, ob3}, false, nullptr, nullptr, nullptr, gamma,
+                        y,
+                        MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                            .with_side("rd", rd_offset, 8, 8),
+                        scratch, stream);
+}
+
+int ktb_mlp_bf16_dqn_target_masked(int dev, const void* obs, size_t M, int d_in, int d_hidden, int d_out,
+                                   const void* W1, const void* b1, const void* W2, const void* b2, const void* W3,
+                                   const void* b3, const void* oW1, const void* ob1, const void* oW2, const void* ob2,
+                                   const void* oW3, const void* ob3, const uint8_t* mask, const float* reward,
+                                   const float* done, float gamma, float* y, void* scratch, void* stage,
+                                   uintptr_t stream) {
+  return dqn_target_run("ktb_mlp_bf16_dqn_target_masked", dev, M, d_in, d_hidden, d_out,
+                        {W1, b1, W2, b2, W3, b3, oW1, ob1, oW2, ob2, oW3, ob3}, true, mask, reward, done, gamma, y,
+                        MlpFeed::pull(obs, stage), scratch, stream);
+}
+
+int ktb_mlp_bf16_dqn_target_masked_pushed(int dev, const void* stage_local, size_t stage_stride, size_t M, int d_in,
+                                          int d_hidden, int d_out, const void* W1, const void* b1, const void* W2,
+                                          const void* b2, const void* W3, const void* b3, const void* oW1,
+                                          const void* ob1, const void* oW2, const void* ob2, const void* oW3,
+                                          const void* ob3, size_t mask_offset, size_t rd_offset, float gamma, float* y,
+                                          void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
+                                          size_t chunk_rows, unsigned long long seq, uintptr_t stream) {
+  return dqn_target_run("ktb_mlp_bf16_dqn_target_masked_pushed", dev, M, d_in, d_hidden, d_out,
+                        {W1, b1, W2, b2, W3, b3, oW1, ob1, oW2, ob2, oW3, ob3}, true, nullptr, nullptr, nullptr, gamma,
+                        y,
+                        MlpFeed::push(stage_local, stage_stride, ctrl_local, ctrl_root_peer, rank, chunk_rows, seq)
+                            .with_side("mask", mask_offset, d_out, 1)
+                            .with_side("rd", rd_offset, 8, 8),
+                        scratch, stream);
 }
 
 }  // extern "C"

@@ -225,6 +225,15 @@ for _policy, _alpha in (("_deterministic", []), ("_gaussian", [c_float])):
         _SIGNATURES["ktb_mlp_bf16_td_target" + _policy + _form] = (
             c_int, _args[:_at] + [c_int] + [c_void_p] * 6 + [c_float, c_float, c_int, ctypes.c_uint64, ctypes.c_uint64]
             + [_side, _side, c_float] + _alpha + [c_void_p] + _args[_at + 4:])
+# The _dqn_target entries: ktb_mlp_bf16_policy's arguments up to b3 (the target network), the online network's six
+# pointers, ([mask,] reward, done, gamma, y) with (mask_offset,) rd_offset in place of (mask, reward, done) in the pushed
+# forms, then ktb_mlp_bf16_policy's arguments from scratch on.
+_SIGNATURES["ktb_mlp_dqn_target_scratch_bytes"] = (c_size_t, [c_size_t, c_int])
+for _masked in ("", "_masked"):
+    for _form, _in, _rd, _at in (("", c_void_p, [c_void_p, c_void_p], 12), ("_pushed", c_size_t, [c_size_t], 13)):
+        _args = _SIGNATURES["ktb_mlp_bf16_policy" + _form][1]
+        _SIGNATURES["ktb_mlp_bf16_dqn_target" + _masked + _form] = (
+            c_int, _args[:_at] + [c_void_p] * 6 + [_in] * bool(_masked) + _rd + [c_float, c_void_p] + _args[_at + 2:])
 _SIGNATURES["ktb_push_scatter_ce_sides"] = (
     c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
                                                          ctypes.c_ulonglong, c_uintptr])

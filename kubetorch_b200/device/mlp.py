@@ -8,7 +8,8 @@ head, optionally tanh-squashed actions), the _epsilon_greedy forms (a Q-network'
 and _gaussian_evaluate forms (the log-probability and entropy of given actions), the _deterministic forms (DDPG's and
 TD3's actor: tanh actions with clipped Gaussian noise), the _critic forms (Q(s, a) critics with the actions fed into
 layer 1, single or twin), the _td_target forms (TD3's, DDPG's and SAC's Bellman target: the actor, the target critics
-and the target in one call) and their scatter→exec→gather form."""
+and the target in one call), the _dqn_target forms (DQN's and Double DQN's Bellman target: the greedy next action, the
+target network's Q at it and the target in one call) and their scatter→exec→gather form."""
 from __future__ import annotations
 
 import ctypes
@@ -218,21 +219,22 @@ def _padded_w1(w1: torch.Tensor, d_in: int) -> torch.Tensor:
     return entry[2]
 
 
-def _check_twin(twin, w1, w2, w3, biases) -> None:
-    """_check_critic's checks of twin = (w1, b1, w2, b2, w3, b3) of a second critic: six entries, biases given exactly
-    as the first critic's, each weight a contiguous CUDA bfloat16 tensor of the first's shape on the device of w1."""
+def _check_twin(twin, w1, w2, w3, biases, what="twin", of=("the second critic", "the first critic's")) -> None:
+    """_check_critic's checks of twin = (w1, b1, w2, b2, w3, b3) of a second critic (or of a Double DQN target's online
+    network, `what` naming the option and `of` the networks in the messages): six entries, biases given exactly as the
+    first critic's, each weight a contiguous CUDA bfloat16 tensor of the first's shape on the device of w1."""
     if not isinstance(twin, (tuple, list)) or len(twin) != 6:
-        raise ValueError("twin must be (w1, b1, w2, b2, w3, b3) of the second critic (biases None without biases)")
+        raise ValueError(f"{what} must be (w1, b1, w2, b2, w3, b3) of {of[0]} (biases None without biases)")
     for name, t, mine in zip(("b1", "b2", "b3"), twin[1::2], biases):
         if (t is None) != (mine is None):
-            raise ValueError(f"twin: {name} is given exactly when the first critic's is")
+            raise ValueError(f"{what}: {name} is given exactly when {of[1]} is")
     for name, t, like in zip(("w1", "w2", "w3", "b1", "b2", "b3"), (*twin[0::2], *twin[1::2]), (w1, w2, w3, *biases)):
         if t is None:
             continue
         if not isinstance(t, torch.Tensor) or t.dtype != torch.bfloat16 or tuple(t.shape) != tuple(like.shape) \
                 or not t.is_contiguous() or not t.is_cuda or t.device != w1.device:
-            raise ValueError(f"twin: {name} must be a contiguous CUDA bfloat16 tensor of shape {tuple(like.shape)} on "
-                             f"the device of w1 ({w1.device})")
+            raise ValueError(f"{what}: {name} must be a contiguous CUDA bfloat16 tensor of shape {tuple(like.shape)} "
+                             f"on the device of w1 ({w1.device})")
 
 
 def _check_td_target(w1, w2, w3, biases, obs, twin, log_std, actor, reward, done) -> None:
@@ -253,7 +255,7 @@ def _check_td_target(w1, w2, w3, biases, obs, twin, log_std, actor, reward, done
                              f"({w1.device})")
     if not isinstance(obs, torch.Tensor):
         raise ValueError("a TD target is checked against obs: pass the next observations [M, d_in] it goes with")
-    M, d_in = obs.shape
+    d_in = obs.shape[1]
     aw1, _, aw2, _, aw3, _ = actor
     d_ha, d_act = aw1.shape[0], aw3.shape[0]
     if tuple(aw1.shape) != (d_ha, d_in) or tuple(aw2.shape) != (d_ha, d_ha) or aw3.shape[1] != d_ha:
@@ -272,6 +274,13 @@ def _check_td_target(w1, w2, w3, biases, obs, twin, log_std, actor, reward, done
         _check_twin(twin, w1, w2, w3, biases)
     if log_std is not None:
         _check_state_std(log_std, aw3, actor[5], d_ha, d_act, False)
+    _check_reward_done(reward, done, obs)
+
+
+def _check_reward_done(reward, done, obs) -> None:
+    """A TD or DQN target's reward and done: fp32 [M] or [M, 1] of one shape, contiguous, on the device of obs [M,
+    d_in]."""
+    M = obs.shape[0]
     for name, t in (("reward", reward), ("done", done)):
         if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or tuple(t.shape) not in ((M,), (M, 1)):
             raise ValueError(f"{name} must be a float32 tensor of shape ({M},) or ({M}, 1), got "
@@ -285,23 +294,25 @@ def _check_td_target(w1, w2, w3, biases, obs, twin, log_std, actor, reward, done
 
 
 _ARGUMENTS = ("seed", "log_std", "mask", "value", "nvec", "log_std_bounds", "squash", "epsilon", "taken", "noise",
-              "noise_clip", "action", "twin") + TD_OPTIONS   # _check_policy's options, td's last
+              "noise_clip", "action", "twin") + TD_OPTIONS + ("online",)   # _check_policy's options, td's, online
 
 
 def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, obs=None, value=None,
                   nvec=None, log_std_bounds=None, squash=None, epsilon=None, taken=None, noise=None,
-                  noise_clip=None, action=None, twin=None, w2=None, td=(None,) * 6) -> None:
-    """Raise ValueError for a call the kernels do not take, td = (actor, policy, reward, done, gamma, alpha) and None
-    an option not given.  The options each output takes and requires are those of the table mapped.MLP_TAKES
-    (check_mlp_options, check_mlp_rules), and a constant's value is checked as mapped() checks it (CONSTANT_CHECKS).
-    Then the tensors: a TD target's (_check_td_target) and a critic's (_check_critic); a head 1 to 256 wide; nvec
+                  noise_clip=None, action=None, twin=None, w2=None, td=(None,) * 6, online=None) -> None:
+    """Raise ValueError for a call the kernels do not take, td = (actor, policy, reward, done, gamma, alpha) (a DQN
+    target's reward, done and gamma there too) and None an option not given.  The options each output takes and
+    requires are those of the table mapped.MLP_TAKES (check_mlp_options, check_mlp_rules), and a constant's value is
+    checked as mapped() checks it (CONSTANT_CHECKS).  Then the tensors: a TD target's (_check_td_target), a critic's
+    (_check_critic) and a DQN target's (its online network as a twin, _check_twin, then reward and done); a head 1 to 256
+    wide; nvec
     summing to d_out; taken (_check_taken); an epsilon tensor (_check_epsilon); log_std, a 1-D contiguous CUDA float32
     tensor of length d_out or a state-dependent head (w_ls, b_ls) (_check_state_std); a mask, a contiguous CUDA
     torch.bool tensor [M, d_out] on the device of obs [M, d_in]; a value head (_check_value); the biases."""
     if output not in OUTPUTS:
         raise ValueError(f"output must be one of {OUTPUTS}, got {output!r}")
     values = (seed, log_std, mask, value, nvec, log_std_bounds, squash, epsilon, taken, noise, noise_clip, action, twin,
-              *td)
+              *td, online)
     given = {name: v for name, v in zip(_ARGUMENTS, values) if v is not None}
     actor, policy, reward, done = td[:4]
     row = check_mlp_options(output, policy, given, argument=True)
@@ -315,6 +326,12 @@ def _check_policy(w1, w3, biases, output, seed=None, log_std=None, mask=None, ob
         return
     if output == "critic":
         _check_critic(w1, w2, w3, biases, obs, action, twin)
+    if output == "dqn_target":
+        if online is not None:
+            _check_twin(online, w1, w2, w3, biases, "online", ("the online network", "the target network's"))
+        if not isinstance(obs, torch.Tensor):
+            raise ValueError("a DQN target is checked against obs: pass the next observations [M, d_in] it goes with")
+        _check_reward_done(reward, done, obs)
     if len(biases) != 3:
         raise ValueError("biases must be (b1, b2, b3), each a tensor or None")
     d_hidden, d_out = w1.shape[0], w3.shape[0]
@@ -531,7 +548,7 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
                 actor: Optional[Sequence[Optional[torch.Tensor]]] = None, policy: Optional[str] = None,
                 reward: Optional[torch.Tensor] = None, done: Optional[torch.Tensor] = None,
                 gamma: Optional[float] = None, alpha: Optional[float] = None, target: Optional[torch.Tensor] = None,
-                _stacked: bool = False):
+                online: Optional[Sequence[Optional[torch.Tensor]]] = None, _stacked: bool = False):
     """logits[M, d_out] = W3·relu(W2·relu(W1·obsᵀ + b1) + b2) + b3; bf16 storage, fp32 accumulation in registers,
     each bias added to the fp32 accumulator (nn.Linear).  `biases` = (b1, b2, b3), each optional.  `output` is
     "logits" (returns the logits), "actions" (returns int64 argmax actions[M]; no logits are written), "both"
@@ -598,6 +615,14 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
     fp32 as torch evaluates that expression; `reward` and `done` are fp32 [M] or [M, 1] on the device of obs, and gamma
     and alpha finite numbers (alpha required with "gaussian" and refused with "deterministic").  Per row chunk the
     actor's actions stay in scratch and feed the critics' action tile; nothing M-sized but y is written.
+    output="dqn_target" (the Bellman target of DQN and Double DQN, forward only) returns fp32 y of the shape of
+    `reward`, into `target` when given: obs are the next observations, w1, w2, w3 and biases the target Q-network's and
+    `online` = (w1, b1, w2, b2, w3, b3) an optional online Q-network of the same shapes (biases given exactly when the
+    target's are).  The next action a* is the argmax of the online network's logits (Double DQN) or of the target's
+    (DQN), masked with `mask` (bool [M, d_out] legal actions of the next states) when given, with output="actions"'s
+    rules; q = the target's logit at a*, UNMASKED, widened to fp32; and y = reward + gamma * (1 - done) * q evaluated
+    as torch evaluates it (so a terminal row with no legal action gives y = reward at done = 1).  `reward`, `done` and
+    `gamma` as with "td_target".  Per row chunk a* stays in scratch; nothing M-sized but y is written.
     `_stacked` (internal, from
     mlp_scatter_gather, which checked the call): w3 and biases[2] are
     already the head the C entry takes (stacked with a value head, interleaved with a log-std head), and a critic's
@@ -617,11 +642,14 @@ def mlp_forward(obs: torch.Tensor, w1: torch.Tensor, w2: torch.Tensor, w3: torch
         raise ValueError("weight shapes must be W1[d_h,d_in], W2[d_h,d_h], W3[d_out,d_h] (nn.Linear layout)")
     if not _stacked:
         _check_policy(w1, w3, biases, output, seed, log_std, mask, obs, value, nvec, log_std_bounds, squash, epsilon,
-                      taken, noise, noise_clip, action, twin, w2, td)
+                      taken, noise, noise_clip, action, twin, w2, td, online)
     if output == "td_target":
         return _td_target(obs, w1, w2, w3, biases, twin, td, seed, log_std, log_std_bounds, squash, noise, noise_clip,
                           row_offset, target, dev, stream if stream is not None else torch.cuda.current_stream(dev),
                           staged, _stacked)
+    if output == "dqn_target":
+        return _dqn_target(obs, w1, w2, w3, biases, online, mask, reward, done, gamma, target, dev,
+                           stream if stream is not None else torch.cuda.current_stream(dev), staged)
     std = _std(log_std, log_std_bounds, squash) if output == "gaussian" else None
     valued = value is not None or (_stacked and values is not None)
     if _stacked:
@@ -711,6 +739,25 @@ def _td_target(obs, w1, w2, w3, biases, twin, td, seed, log_std, log_std_bounds,
     return target
 
 
+def _dqn_target(obs, w1, w2, w3, biases, online, mask, reward, done, gamma, target, dev, s, staged):
+    """mlp_forward's output="dqn_target" on `dev` and stream `s`: y of the shape of reward, into `target` when given."""
+    M, d_in = obs.shape
+    if target is None:
+        target = torch.empty(reward.shape, dtype=torch.float32, device=f"cuda:{dev}")
+    else:
+        ops.ensure_init({target.device.index})
+    if staged is None:
+        staged = obs.device.index != dev
+    ptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+    scratch = _cached_buffer(_scratch, dev, dev, L.load().ktb_mlp_dqn_target_scratch_bytes(M, w1.shape[0]))
+    L.call("ktb_mlp_bf16_dqn_target" + ("" if mask is None else "_masked"), dev, obs.data_ptr(), M, d_in, w1.shape[0],
+           w3.shape[0], w1.data_ptr(), ptr(biases[0]), w2.data_ptr(), ptr(biases[1]), w3.data_ptr(), ptr(biases[2]),
+           *(ptr(t) for t in (online or (None,) * 6)), *(() if mask is None else (mask.data_ptr(),)), reward.data_ptr(),
+           done.data_ptr(), float(gamma), target.data_ptr(), scratch.data_ptr(),
+           _stage_for(dev, M, d_in).data_ptr() if staged else 0, int(s.cuda_stream))
+    return target
+
+
 def _weights_on(dev: int, ws: Sequence[torch.Tensor]) -> List[torch.Tensor]:
     """Weights are shared by all ranks: broadcast once per (weights, device) and kept resident
     (excluded from per-call bytes, SURVEY.md §8(d) C4)."""
@@ -763,6 +810,11 @@ def _forward_rows(obs_root, b, e, dev, stream, staged, ws, bufs, output, seed, l
     the arguments of _mlp_scatter_gather_pushed, with ws, log_std and twin those on `dev`."""
     logits, actions, log_probs, values = _rows(bufs, b, e)
     valued = values is not None and epsilon is None   # an ε-greedy head's values slot is its q_max
+    target = {}   # a TD or DQN target's options, its y in the logits slot
+    if td is not None:
+        target = dict(reward=td[2][b:e], done=td[3][b:e], gamma=td[4], target=logits)
+        target.update(dict(online=None if td[0] is None else td[0][dev]) if output == "dqn_target" else
+                      dict(actor=td[0][dev], policy=td[1], alpha=td[5], twin=twin))
     mlp_forward(obs_root[b:e], ws[0], ws[1], ws[2], out=logits, device=dev, stream=stream, staged=staged,
                 biases=ws[3:], output=output, actions=actions, seed=seed, row_offset=b, log_probs=log_probs,
                 log_std=log_std, mask=None if mask is None else mask[b:e], values=values, nvec=nvec,
@@ -772,8 +824,7 @@ def _forward_rows(obs_root, b, e, dev, stream, staged, ws, bufs, output, seed, l
                 **({} if taken is None else dict(taken=taken[b:e], entropy=actions)),
                 **({} if output != "critic" else dict(action=action[b:e], twin=twin, q=logits, q2=actions,
                                                        q_min=log_probs)),
-                **({} if td is None else dict(actor=td[0][dev], policy=td[1], reward=td[2][b:e], done=td[3][b:e],
-                                              gamma=td[4], alpha=td[5], twin=twin, target=logits)),
+                **target,
                 _stacked=valued or std is not None or output == "critic" or td is not None)
 
 
@@ -801,13 +852,19 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
     (actors, policy, reward, done, gamma, alpha): actors[dev] is the actor's six weights and biases on that device (its
     head interleaved with the log-std head for policy="gaussian", picked by `std`; "deterministic" by `det`), reward and
     done (on the root) are pushed with the rows, weights[dev] and twin[dev] are the target critics as with "critic", and
-    out_root is y."""
+    out_root is y.  With output="dqn_target", td = (onlines, None, reward, done, gamma, None): onlines[dev] (None for
+    DQN) is the online network's six weights and biases on that device, the mask (unless None) and one side of
+    interleaved (reward, done) pairs, stacked on the root, are pushed with the rows, and out_root is y."""
     root, n, key = devs[0], len(devs), tuple(devs)
     critic = output == "critic"
     valued = values_root is not None and epsilon is None   # an ε-greedy head's values_root is its q_max
     d_in, d_hidden = obs_root.shape[1], weights[root][0].shape[0]
     actors, policy, reward, done, gamma, alpha = td or (None,) * 6
-    if td is not None:   # the entry's d_act
+    dqn = output == "dqn_target"
+    rd = None
+    if dqn:   # one side of (reward, done) pairs: the pushed entries take at most two sides, the mask one of them
+        rd, reward, done = torch.stack((reward.reshape(-1), done.reshape(-1)), 1), None, None
+    if td is not None and not dqn:   # the entry's d_act
         d_out = actors[root][4].shape[0] // (2 if std is not None else 1)
     else:
         d_out = action.shape[1] if critic else (weights[root][2].shape[0] - valued) // (2 if std is not None else 1)
@@ -816,7 +873,7 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         taken.element_size()
     sides = [(name, t, row_bytes) for name, t, row_bytes in
              (("mask", mask, d_out), ("epsilon", epsilon, 4), ("taken", taken, taken_row), ("act", action, 4 * d_out),
-              ("reward", reward, 4), ("done", done, 4)) if t is not None]
+              ("reward", reward, 4), ("done", done, 4), ("rd", rd, 8)) if t is not None]
     offsets, stage_bytes = _stage_layout(rows, d_in, [(name, row_bytes) for name, _, row_bytes in sides])
     sess = _push_sessions.get(key)
     if sess is None or sess.stride < stage_bytes:
@@ -828,7 +885,9 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         raise
     # scratch per rank, not per device: ranks sharing a device must not share one, nor the root's own shard on the
     # side stream
-    if td is not None:
+    if dqn:   # the chunk's int64 actions after the hidden activations
+        scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS) + min(PUSH_CHUNK_ROWS, rows) * 8
+    elif td is not None:
         scratch_bytes = pushed_td_scratch_bytes(rows, actors[root][0].shape[0], d_hidden, d_out, PUSH_CHUNK_ROWS)
     else:
         scratch_bytes = pushed_scratch_bytes(rows, d_hidden, PUSH_CHUNK_ROWS, critic)
@@ -860,8 +919,12 @@ def _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, out_root
         ws = weights[devs[r]]
         ptr = lambda t: 0 if t is None or e == b else t.data_ptr()   # noqa: E731
         logits, actions, log_probs, values = _rows(bufs, b, e)
-        if td is not None:   # y rides in the logits slot
-            wptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+        wptr = lambda t: 0 if t is None else t.data_ptr()   # noqa: E731
+        if dqn:   # y rides in the logits slot
+            entry = "ktb_mlp_bf16_dqn_target" + ("" if mask is None else "_masked") + "_pushed"
+            head = (*(wptr(t) for t in (actors[devs[r]] if actors is not None else (None,) * 6)),
+                    *(() if mask is None else (offsets["mask"],)), offsets["rd"], float(gamma), ptr(logits))
+        elif td is not None:   # y rides in the logits slot
             entry = "ktb_mlp_bf16_td_target_" + policy + "_pushed"
             head = (*(wptr(t) for t in (twin[devs[r]] if twin is not None else (None,) * 6)),
                     actors[root][0].shape[0], *(wptr(t) for t in actors[devs[r]]),
@@ -901,7 +964,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                        actor: Optional[Sequence[Optional[torch.Tensor]]] = None, policy: Optional[str] = None,
                        reward: Optional[torch.Tensor] = None, done: Optional[torch.Tensor] = None,
                        gamma: Optional[float] = None, alpha: Optional[float] = None,
-                       target_root: Optional[torch.Tensor] = None) -> list:
+                       target_root: Optional[torch.Tensor] = None,
+                       online: Optional[Sequence[Optional[torch.Tensor]]] = None) -> list:
     """Rank r runs the MLP on `obs.chunk(world)[r]`: its first GEMM's TMA loads read the rows straight
     from the root GPU (scatter) and its last epilogue stores the logits straight into the root's
     result buffer (gather). Returns rank-ordered views of the root result: logits views for output="logits",
@@ -928,17 +992,21 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     like the other weights, again after an in-place update of w1.  output="td_target" with `actor`, `policy`, its
     options, `twin`, `reward`, `done` (on the root), `gamma` and `alpha` as in mlp_forward returns fp32 y views of
     `target_root` (of reward's shape, allocated on the root when None); each rank draws the noise of its shard's global
-    rows, reads its rows of reward and done in place on the pull form, and the push form pushes them with the rows."""
+    rows, reads its rows of reward and done in place on the pull form, and the push form pushes them with the rows.
+    output="dqn_target" with `online`, `mask`, `reward`, `done` (on the root) and `gamma` as in mlp_forward returns fp32
+    y views of `target_root` likewise; the online network is copied to the other devices like the other weights, each
+    rank reads its rows of mask, reward and done in place on the pull form, and the push form pushes them with the
+    rows, reward and done as one side of interleaved pairs."""
     root = obs_root.device.index
     devs = [int(d) for d in devices]
     if devs[0] != root:
         raise ValueError("obs must live on the root GPU (devices[0])")
     td = (actor, policy, reward, done, gamma, alpha)
     _check_policy(w1, w3, biases, output, seed, log_std, mask, obs_root, value, nvec, log_std_bounds, squash, epsilon,
-                  taken, noise, noise_clip, action, twin, w2, td)
+                  taken, noise, noise_clip, action, twin, w2, td, online)
     if transfer not in ("auto", "pull", "push"):
         raise ValueError("transfer must be 'auto', 'pull' or 'push'")
-    critic, target = output == "critic", output == "td_target"
+    critic, target, dqn = output == "critic", output == "td_target", output == "dqn_target"
     if critic:   # q (or q1), q2 and q_min ride in the logits, actions and log_probs slots
         out_root, actions_root, log_probs_root = q_root, q2_root, q_min_root
     det = dict(noise=noise, noise_clip=noise_clip, squash=squash) \
@@ -950,7 +1018,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     valued = value is not None
     if taken is not None:   # the entropy rides in the actions slot
         actions_root = entropy_root
-    if target:   # y, of reward's shape, rides in the logits slot
+    if target or dqn:   # y, of reward's shape, rides in the logits slot
         if target_root is None:
             target_root = torch.empty(reward.shape, dtype=torch.float32, device=obs_root.device)
         else:
@@ -975,7 +1043,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
     ready = torch.cuda.Event()
     ready.record(root_stream)
     bounds = [ops.shard_bounds(M, len(devs), r) for r in range(len(devs))]
-    views = [target_root[b:e] if target else _result(output, *_rows(bufs, b, e)) for b, e in bounds]
+    views = [target_root[b:e] if target or dqn else _result(output, *_rows(bufs, b, e)) for b, e in bounds]
     weights = {dev: _weights_on(dev, (w1, w2, w3)) + _weights_on(dev, biases) for dev in set(devs)}
     if std is not None:   # the pair only marks the form on each rank: its rows are in the interleaved head
         log_stds = {dev: log_std for dev in set(devs)}
@@ -983,9 +1051,11 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
         log_stds = None if log_std is None else {dev: _weights_on(dev, (log_std,))[0] for dev in set(devs)}
     if target:
         td = ({dev: tuple(_weights_on(dev, actor)) for dev in set(devs)}, *td[1:])
+    if dqn:   # the online network where td holds a TD target's actors
+        td = (None if online is None else {dev: tuple(_weights_on(dev, online)) for dev in set(devs)}, *td[1:])
     if _use_push(devs, bounds, transfer):
         _mlp_scatter_gather_pushed(obs_root, devs, bounds, weights, output, *bufs[:3], seed, log_stds, mask, bufs[3],
-                                   nvec, std, epsilon, taken, det, action, twins, td if target else None)
+                                   nvec, std, epsilon, taken, det, action, twins, td if target or dqn else None)
         return views
     rows = max(e - b for b, e in bounds)
     for dev in set(devs):       # allocate scratch/staging on the calling thread (allocator + first use)
@@ -993,6 +1063,8 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
             d_act = actor[4].shape[0] // (2 if std is not None else 1)
             _cached_buffer(_scratch, dev, dev,
                            L.load().ktb_mlp_td_target_scratch_bytes(rows, actor[0].shape[0], w1.shape[0], d_act))
+        elif dqn:
+            _cached_buffer(_scratch, dev, dev, L.load().ktb_mlp_dqn_target_scratch_bytes(rows, w1.shape[0]))
         else:
             _scratch_for(dev, rows, w1.shape[0], critic)
         if dev != root:
@@ -1011,7 +1083,7 @@ def mlp_scatter_gather(obs_root: torch.Tensor, w1, w2, w3, devices: Sequence[int
                 st.wait_event(ready)
             _forward_rows(obs_root, b, e, dev, st, None, weights[dev], bufs, output, seed,
                           None if log_stds is None else log_stds[dev], mask, nvec, std, epsilon, taken, det, action,
-                          None if twins is None else twins[dev], td if target else None)
+                          None if twins is None else twins[dev], td if target or dqn else None)
             if dev != root:
                 ev = torch.cuda.Event()
                 ev.record(st)

@@ -27,9 +27,12 @@ MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
 ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
-               "gaussian_evaluate", "deterministic", "critic", "td_target")   # also device.mlp.OUTPUTS
+               "gaussian_evaluate", "deterministic", "critic", "td_target", "dqn_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
-TD_OPTIONS = ("actor", "policy", "reward", "done", "gamma", "alpha")   # the options of output="td_target" alone
+# The options of output="td_target" and of output="dqn_target" that no other output takes: the supervisor passes them
+# to mlp_scatter_gather with their output only
+TD_OPTIONS = ("actor", "policy", "reward", "done", "gamma", "alpha")
+DQN_OPTIONS = ("online", "reward", "done", "gamma")
 
 # The options each MLP output takes beside bias= and output=, True for those it requires, keyed by (output, policy):
 # a TD target's depend on its policy=, and every other output has none.  mapped() and device.mlp._check_policy refuse
@@ -49,6 +52,7 @@ MLP_TAKES = {
                                          noise=False, noise_clip=False, seed=False, squash=False),
     ("td_target", "gaussian"): dict(actor=True, policy=True, reward=True, done=True, gamma=True, twin=False, seed=True,
                                     alpha=True, log_std=True, log_std_bounds=False, squash=False),
+    ("dqn_target", None): dict(reward=True, done=True, gamma=True, online=False, mask=False),
 }
 
 # Each MLP option's form at decoration: "name", the name of a call argument; "names", a tuple of such names
@@ -57,11 +61,13 @@ MLP_TAKES = {
 MLP_FORMS = dict(seed="name or constant", log_std="names", mask="name", value="names", nvec="constant",
                  log_std_bounds="constant", squash="constant", epsilon="name or constant", taken="name",
                  noise="name or constant", noise_clip="constant", action="name", twin="names", actor="names",
-                 policy="constant", reward="name", done="name", gamma="constant", alpha="name or constant")
+                 policy="constant", reward="name", done="name", gamma="constant", alpha="name or constant",
+                 online="names")
 
 # What each "names" option names, for the message that refuses a wrong count (log_std may also be one name)
 _NAMES =dict(log_std="one call argument or two (w_ls, b_ls)", value="two call arguments (wv, bv)",
-              twin="the second critic's {n} call arguments {what}", actor="the actor's {n} call arguments {what}")
+              twin="the second critic's {n} call arguments {what}", actor="the actor's {n} call arguments {what}",
+              online="the online network's {n} call arguments {what}")
 
 
 def check_mlp_options(output: str, policy, given, argument: bool = False) -> dict:
@@ -272,7 +278,15 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
     ``"gaussian"`` only, required there) a finite number or the name of a call argument that holds a number or a
     one-element tensor; a CUDA tensor is read with ``float()``, one host synchronisation per call.  ``mask=``,
     ``value=``, ``nvec=``, ``epsilon=``, ``taken=`` and ``action=`` are refused, and these options with every other
-    output."""
+    output.
+    ``output="dqn_target"`` is the Bellman target of DQN and Double DQN (forward only): the callable is ``(next_obs, w1,
+    b1, w2, b2, w3, b3, ...)``, the target Q-network, and each rank returns the fp32 ``y`` of its rows, ``reward + gamma
+    * (1 - done) * q``.  ``online=`` names the online Q-network's six arguments (three without ``bias=True``) for Double
+    DQN, which picks the greedy next action with the online network; without it the target network picks it (DQN).
+    ``mask=`` names the bool ``[M, d_out]`` legal actions of the next states, which mask the ranking only: ``q`` is the
+    target network's unmasked Q-value at the chosen action, so a terminal row with no legal action gets ``y = reward``
+    at ``done = 1``.  ``reward=``, ``done=`` and ``gamma=`` as with ``"td_target"``.  Every other option is refused,
+    and ``online=`` with every other output."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
@@ -299,7 +313,7 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
             if form == "name" and not isinstance(v, str):
                 raise ValueError(f"{name} must be the name of a call argument, got {v!r}")
             if form == "names" and not (name == "log_std" and isinstance(v, str)):
-                n = (6 if bias else 3) if name in ("twin", "actor") else 2
+                n = (6 if bias else 3) if name in ("twin", "actor", "online") else 2
                 if not isinstance(v, (tuple, list)) or len(v) != n or not all(isinstance(x, str) for x in v):
                     what = "(w1, b1, w2, b2, w3, b3)" if n == 6 else "(w1, w2, w3) (bias=False)"
                     raise ValueError(f"{name} must name {_NAMES[name].format(n=n, what=what)}, got {v!r}")

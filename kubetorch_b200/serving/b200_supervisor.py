@@ -50,7 +50,7 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import ELEMENTWISE_OPS, MLP_FORMS, TD_OPTIONS, mapped_spec, names_arguments
+from ..mapped import DQN_OPTIONS, ELEMENTWISE_OPS, MLP_FORMS, TD_OPTIONS, mapped_spec, names_arguments
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -572,14 +572,15 @@ class B200Supervisor:
         else:
             obs, w1, w2, w3 = (bound[n] for n in names[:4])
             biases = (None, None, None)
-        # every option mlp_scatter_gather takes, a TD target's only with output="td_target"; None unless given
-        args = {name: None for name in MLP_FORMS if name not in TD_OPTIONS or output == "td_target"}
+        # every option mlp_scatter_gather takes, a TD or DQN target's only with its output; None unless given
+        own = {"td_target": TD_OPTIONS, "dqn_target": DQN_OPTIONS}.get(output, ())
+        args = {name: None for name in MLP_FORMS if name not in TD_OPTIONS + DQN_OPTIONS or name in own}
         for option, v in spec.extra.items():
             if option not in MLP_FORMS:
                 continue
             if names_arguments(option, v):   # resolved per call: mapped() checked that each names an argument
                 v = bound[v] if isinstance(v, str) else tuple(bound[name] for name in v)
-                if option in ("twin", "actor") and len(v) == 3:   # (w1, w2, w3) of a bias-free network
+                if option in ("twin", "actor", "online") and len(v) == 3:   # (w1, w2, w3) of a bias-free network
                     v = (v[0], None, v[1], None, v[2], None)
                 elif option == "alpha":
                     v = float(v)   # a number or a one-element tensor (on a GPU: one host synchronisation)

@@ -55,6 +55,11 @@ Variants, timed alternately (one sample = the mean of --calls back-to-back calls
      actor's head, the padded concatenation and the minimum in torch).  Before timing, the fused y equals the two-call
      arm's bit for bit on every row, and is within rtol 2^-7, atol 1e-2 of the eager arm's on at least 99 % of the rows
      (the eager arm's tanh and log rounding move some bf16 actions by an ulp).
+  r  DQN targets (output="dqn_target") over the C4 trunk, d_out 6, 18 and 64 and d_out 18 under a random legal-action
+     mask, DQN (the target network selects) and Double DQN (an online network of its own selects), each beside the
+     two-call arm (output="actions" on the selector, output="logits" on the target, then the gather and reward + 0.99 *
+     (1 - done) * q in eager torch) and the eager arm (the logits entry on each network, then the mask, argmax, gather
+     and the target in torch).  Before timing, the fused y equals both arms' bit for bit on every row.
 Parity: 2048 sampled rows against an fp32 evaluation (rtol 2^-7, atol 1e-2; actions wherever the fp32 top-2 gap
 exceeds 2^-6), and the actions equal torch.argmax of the kernel's logits on every row.  Sampled rows: on 2048
 consecutive rows, the action is the argmax of the kernel's logits plus the fp64 Gumbel noise wherever the top-2 gap
@@ -492,6 +497,50 @@ def main():
                                             "target_eq_eager_bits_frac": round(float(
                                                 (got.view(torch.int32) == eager.view(torch.int32)).float().mean()), 6)}
             del got, two, eager
+    # r: DQN targets; the online network has weights of its own
+    gr = torch.Generator(device="cuda:0").manual_seed(17)
+    rr = lambda *s, scale=1.0: (torch.randn(*s, device="cuda:0", generator=gr) * scale).bfloat16()   # noqa: E731
+    q_nets = {(d, k): (rr(d_hidden, d_in, scale=0.02), rr(d_hidden, scale=0.1), rr(d_hidden, d_hidden, scale=0.02),
+                       rr(d_hidden, scale=0.1), rr(d, d_hidden, scale=0.02), rr(d, scale=0.1))
+              for d in (6, 18, 64) for k in ("target", "online")}
+    q_legal = torch.rand(M, 18, device="cuda:0", generator=gr) < 0.5
+
+    def dqn_fused(d, double, mask):
+        t = q_nets[(d, "target")]
+        return mlp.mlp_forward(obs, t[0], t[2], t[4], biases=t[1::2], output="dqn_target", reward=reward, done=done,
+                               gamma=0.99, online=q_nets[(d, "online")] if double else None, mask=mask)
+
+    def dqn_two_call(d, double, mask):
+        """The actions entry on the selector, the logits entry on the target, then the gather and y in eager torch."""
+        t, s = q_nets[(d, "target")], q_nets[(d, "online" if double else "target")]
+        a = mlp.mlp_forward(obs, s[0], s[2], s[4], biases=s[1::2], output="actions", mask=mask)
+        qt = mlp.mlp_forward(obs, t[0], t[2], t[4], biases=t[1::2], output="logits")
+        return reward + 0.99 * (1 - done) * qt.float().gather(1, a[:, None]).squeeze(1)
+
+    def dqn_eager(d, double, mask):
+        """The logits entry on each network, then the mask, argmax, gather and y in torch."""
+        t, s = q_nets[(d, "target")], q_nets[(d, "online")]
+        qt = mlp.mlp_forward(obs, t[0], t[2], t[4], biases=t[1::2])
+        sel = mlp.mlp_forward(obs, s[0], s[2], s[4], biases=s[1::2]) if double else qt
+        if mask is not None:
+            sel = sel.masked_fill(~mask, float("-inf"))
+        return reward + 0.99 * (1 - done) * qt.float().gather(1, sel.argmax(-1, keepdim=True)).squeeze(1)
+
+    dqn_cases = [(6, None), (18, None), (18, q_legal), (64, None)]
+    for d, mask in dqn_cases:
+        for double in (False, True):
+            tag = ("double" if double else "dqn") + ("_masked" if mask is not None else "")
+            for arm, fn in (("target", dqn_fused), ("two_call", dqn_two_call), ("eager", dqn_eager)):
+                variants[f"r_bias_{tag}_{arm}_d{d}"] = (d, lambda d=d, double=double, mask=mask, fn=fn: fn(d, double,
+                                                                                                         mask))
+    for d, mask in dqn_cases:   # parity before timing: the fused target equals both arms bit for bit
+        for double in (False, True):
+            tag = ("double" if double else "dqn") + ("_masked" if mask is not None else "")
+            got = dqn_fused(d, double, mask)
+            for arm in (dqn_two_call, dqn_eager):
+                assert torch.equal(got.view(torch.int32), arm(d, double, mask).view(torch.int32)), (tag, d, arm)
+            parity[f"r_bias_{tag}_d{d}"] = {"target_eq_two_call_all_rows": "ok", "target_eq_eager_all_rows": "ok"}
+            del got
     for _, fn in variants.values():   # warm-up: tensor maps, smem attributes, allocations
         fn()
         fn()
