@@ -1053,6 +1053,34 @@ int ktb_mlp_bf16_dqn_target_masked_pushed(int dev, const void* stage_local, size
                                           void* scratch, void* ctrl_local, void* ctrl_root_peer, int rank,
                                           size_t chunk_rows, unsigned long long seq, uintptr_t stream);
 
+/* ---- generalized advantage estimation (PPO's learner target) --------------------------------------------------------
+ *
+ * Env-major fp32 [N, T]: row i is environment i's trajectory and column t is step t.  dones[i, t] is the done flag of
+ * transition t (the episode ended after the action at step t); last_values[i] is V(s_T), which bootstraps step T - 1.
+ * CleanRL's and SB3's `dones[t]` / `episode_starts[t]` mark that observation t STARTS an episode: their transition-t
+ * flag is dones[t + 1] (next_done at the last step).
+ *
+ * Per row, as fp32 operations each rounded to nearest even, with no FMA contraction, starting from acc = 0 and
+ * nv = last_values[i], for t = T - 1 down to 0 (r, v, d = rewards, values, dones at [i, t]):
+ *     nt    = 1 - d
+ *     delta = (r + (gamma * nv) * nt) - v
+ *     acc   = delta + (gamma_lam * nt) * acc
+ *     adv[i, t] = acc
+ *     ret[i, t] = acc + v
+ *     nv    = v
+ * which is bit for bit the torch loop of tests/policy_gae_cases.py (CleanRL's expression order) when gamma is the
+ * fp32 rounding of γ and gamma_lam the fp32 rounding of the double product γ·λ.  A done step multiplies by nt = 0, it
+ * does not select: an infinite value or advantage after an episode boundary makes the advantages before it NaN, as in
+ * the torch loop.  Rows are independent; the recurrence along a row is evaluated sequentially (no parallel-in-time
+ * scan, which would change the bits).
+ *
+ * Checks, in this order: an unregistered dev is KTB_ERR_STATE; a non-finite gamma or gamma_lam is KTB_ERR_ARG;
+ * N·T == 0 is KTB_OK with nothing enqueued (the pointers may then be NULL); otherwise a NULL or not 4-byte-aligned
+ * pointer, N·T·4 past SIZE_MAX, or an adv or ret range that overlaps an input range or the other output is
+ * KTB_ERR_ARG.  The kernel reads each input element once and writes adv[0, N·T) and ret[0, N·T) once each. */
+int ktb_gae_f32(int dev, const float* rewards, const float* values, const float* dones, const float* last_values,
+                size_t N, size_t T, float gamma, float gamma_lam, float* adv, float* ret, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -234,6 +234,8 @@ for _masked in ("", "_masked"):
         _args = _SIGNATURES["ktb_mlp_bf16_policy" + _form][1]
         _SIGNATURES["ktb_mlp_bf16_dqn_target" + _masked + _form] = (
             c_int, _args[:_at] + [c_void_p] * 6 + [_in] * bool(_masked) + _rd + [c_float, c_void_p] + _args[_at + 2:])
+_SIGNATURES["ktb_gae_f32"] = (c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_size_t, c_float, c_float,
+                                      c_void_p, c_void_p, c_uintptr])
 _SIGNATURES["ktb_push_scatter_ce_sides"] = (
     c_int, _SIGNATURES["ktb_push_scatter_ce"][1][:13] + [c_int, POINTER(c_void_p), POINTER(c_size_t), POINTER(c_size_t),
                                                          ctypes.c_ulonglong, c_uintptr])

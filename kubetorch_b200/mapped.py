@@ -1,6 +1,6 @@
 """Registry of *mapped callables*: user functions whose body is one of the closed set of ops that
-libktb200 executes as sm_90a kernels (identity / scale / affine, their sum-reduced forms, and the
-bf16 MLP policy).
+libktb200 executes as sm_90a kernels (identity / scale / affine, their sum-reduced forms, the
+bf16 MLP policy, and generalized advantage estimation).
 
 Arbitrary Python cannot become a CUDA kernel, so the device route is opt-in by declaration:
 
@@ -25,7 +25,10 @@ from .sampling import _check_seed
 
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
-ALL_OPS = ELEMENTWISE_OPS + ("mlp",)
+ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae")
+# The options of op="gae": gamma and lam, each required (a finite number or the name of a call argument holding one),
+# and self_check
+GAE_OPTIONS = ("gamma", "lam")
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
                "gaussian_evaluate", "deterministic", "critic", "td_target", "dqn_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
@@ -207,7 +210,7 @@ class MappedSpec:
 _UNSET = object()   # mapped()'s alpha when not given: 1.0, and no entropy coefficient of a TD target
 
 
-def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] = None, arg: str = None, **extra):
+def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[str] = None, arg: str = None, **extra):
     """Declare that the decorated function is computed by device op `op` (see module docstring).
 
     The "mlp" op takes more options.  ``bias=True``: the callable is ``(obs, w1, b1, w2, b2, w3, b3, ...)``, an
@@ -286,19 +289,36 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
     ``mask=`` names the bool ``[M, d_out]`` legal actions of the next states, which mask the ranking only: ``q`` is the
     target network's unmasked Q-value at the chosen action, so a terminal row with no legal action gets ``y = reward``
     at ``done = 1``.  ``reward=``, ``done=`` and ``gamma=`` as with ``"td_target"``.  Every other option is refused,
-    and ``online=`` with every other output."""
+    and ``online=`` with every other output.
+
+    The "gae" op is generalized advantage estimation, PPO's learner target: the callable is ``(rewards, values, dones,
+    last_values, ...)`` with fp32 ``[N, T]`` rewards, values and dones in env-major layout (row i is environment i's
+    trajectory, column t its step t) and fp32 ``[N]`` last_values, V(s_T), all CUDA tensors on the root GPU.  Each rank
+    returns ``(advantages, returns)`` of its rows, ``x.chunk(WORLD_SIZE)[RANK]``: the backward loop ``delta = r[:, t] +
+    gamma * next_v * (1 - d[:, t]) - v[:, t]``, ``acc = delta + gamma * lam * (1 - d[:, t]) * acc``, ``adv[:, t] =
+    acc``, returns ``adv + values``, bit for bit as torch computes it in that order.  ``dones[:, t]`` is the done flag of
+    transition t: the episode ended after the action at step t.  CleanRL's ``dones[t]`` (and SB3's
+    ``episode_starts[t]``) say that observation t starts an episode, so their transition-t flag is ``dones[t + 1]``, or
+    ``next_done`` at the last step: from time-major CleanRL buffers, ``torch.cat([dones[1:], next_done[None]]).T
+    .contiguous()``.  For truncated episodes add ``gamma * V(final_obs)`` to the reward, as SB3 does.  ``gamma=`` and
+    ``lam=`` are required, each a finite number or the name of a call argument that holds one (checked per call);
+    ``self_check=False`` skips the deployment's check of a constant γ and λ against the body.  Every other option is
+    refused."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
+    if op == "gae":
+        _check_gae_options(alpha, beta, reduce, arg, extra)
+    beta = 0.0 if beta is _UNSET else beta
     if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
         extra["alpha"] = alpha
     alpha = 1.0 if alpha is _UNSET or op == "mlp" and "alpha" in extra else alpha
     if reduce not in (None, "sum"):
         raise ValueError("reduce must be None or 'sum'")
-    if op != "mlp":
+    if op in ELEMENTWISE_OPS:
         if any(k in extra for k in ("bias", "output", *MLP_FORMS)):
             raise ValueError(f"{', '.join(k + '=' for k in ('bias', 'output', *MLP_FORMS))} are options of the 'mlp' "
                              f"op, not of '{op}'")
-    else:
+    elif op == "mlp":
         bias = extra.get("bias", False)
         if not isinstance(bias, bool):
             raise ValueError(f"bias must be True or False, got {bias!r}")
@@ -326,8 +346,11 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
 
     def deco(fn):
         params = inspect.signature(fn).parameters
+        if op == "gae" and len(params) < 4:
+            raise ValueError(f"a 'gae' callable takes (rewards, values, dones, last_values, ...) positionally, "
+                             f"{getattr(fn, '__name__', fn)!r} has {len(params)} parameters")
         for option, names in extra.items():
-            if not names_arguments(option, names):
+            if not (isinstance(names, str) if op == "gae" else names_arguments(option, names)):
                 continue
             for name in (names,) if isinstance(names, str) else names:
                 if name not in params:
@@ -337,6 +360,25 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = 0.0, reduce: Optional[str] 
         return fn
 
     return deco
+
+
+def _check_gae_options(alpha, beta, reduce, arg, extra) -> None:
+    """The options of op="gae", or ValueError naming the first it does not take or the first it lacks; a constant gamma
+    or lam must be a finite number (extra keeps it)."""
+    refused = dict(alpha=alpha is not _UNSET, beta=beta is not _UNSET, reduce=reduce is not None, arg=arg is not None)
+    refused.update((k, True) for k in extra if k not in GAE_OPTIONS + ("self_check",))
+    for name, given in refused.items():
+        if given:
+            raise ValueError(f"{name}= is not an option of the 'gae' op, which takes gamma=, lam= and self_check=: its "
+                             f"callable is (rewards, values, dones, last_values) and it returns (advantages, returns)")
+    for name in GAE_OPTIONS:
+        if name not in extra:
+            raise ValueError(f"{name}= is required with the 'gae' op: a finite number or the name of a call argument "
+                             f"that holds one")
+        if not isinstance(extra[name], str):
+            check_finite(name, extra[name])
+    if not isinstance(extra.get("self_check", False), bool):
+        raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
 
 
 def names_arguments(option: str, v) -> bool:

@@ -36,6 +36,8 @@ One controller process drives N local H100s.  For a @kt.mapped callable a remote
         (ktb_map_host_multi: chunked H2D / kernel / D2H), ranks in parallel.
     reduce="sum"
         ktb_scatter_map_reduce: per-rank warp-shuffle reduction, scalar peer-stored to the root.
+    "gae"
+        ktb_gae_f32: one launch on the root GPU over every selected rank's rows.
 
 There is NO CPU fallback here: a missing library or GPU raises.
 """
@@ -50,7 +52,8 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import DQN_OPTIONS, ELEMENTWISE_OPS, MLP_FORMS, TD_OPTIONS, mapped_spec, names_arguments
+from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, TD_OPTIONS, check_finite, mapped_spec,
+                      names_arguments)
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -194,6 +197,8 @@ class B200Supervisor:
                     targets.append(m)
         for method in targets:
             spec = mapped_spec(method)
+            if spec.op == "gae" and spec.extra.get("self_check") is not False:
+                self._self_check_gae(spec, method)
             if spec.op not in ELEMENTWISE_OPS or spec.extra.get("self_check") is False:
                 continue
             if not (isinstance(spec.alpha, (int, float)) and isinstance(spec.beta, (int, float))):
@@ -244,6 +249,54 @@ class B200Supervisor:
                         f"'{spec.op}' (alpha={spec.alpha}, beta={spec.beta}, reduce={spec.reduce}) does not reproduce "
                         f"the Python body on a seeded {dtype} tensor; refusing to deploy"
                     )
+
+    def _self_check_gae(self, spec, method):
+        """A "gae" callable with a constant gamma and lam: its body on CPU, rank by rank, against the kernel on seeded
+        (4·world + 3, 9) rollouts with some done = 1; refuse the deployment on any bit difference.  This catches a body
+        that reads dones as episode starts (CleanRL's buffers, shifted by one step) and a γ or λ other than declared."""
+        import inspect
+
+        import torch
+
+        if any(isinstance(spec.extra[k], str) for k in GAE_OPTIONS) or len(inspect.signature(method).parameters) != 4:
+            return   # gamma or lam is a call argument: nothing constant to check at deploy time
+        world, dev0 = self.world_size, self.devices[0]
+        gen = torch.Generator().manual_seed(1234)
+        n, t = 4 * world + 3, 9
+        rewards, values = torch.randn(n, t, generator=gen), torch.randn(n, t, generator=gen)
+        dones = (torch.rand(n, t, generator=gen) < 0.25).float()
+        dones[::3, t // 2] = 1.0
+        last_values = torch.randn(n, generator=gen)
+        args = (rewards, values, dones, last_values)
+        saved = {k: os.environ.get(k) for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK")}
+        want = []
+        try:
+            for r in range(world):
+                os.environ.update({"RANK": str(r), "WORLD_SIZE": str(world), "LOCAL_RANK": str(r)})
+                want.append(method(*(a.clone() for a in args)))
+        except Exception:  # noqa: BLE001 - a body that cannot run here (needs a GPU arg, a group, ...) is skipped
+            return
+        finally:
+            for k, v in saved.items():
+                if v is None:
+                    os.environ.pop(k, None)
+                else:
+                    os.environ[k] = v
+        got = self._run_mapped(spec, method, [a.to(f"cuda:{dev0}") for a in args], {}, list(range(world)))
+        self.ops.synchronize(dev0)
+
+        def same(g, w):
+            return isinstance(w, torch.Tensor) and w.dtype == torch.float32 and tuple(g.shape) == tuple(w.shape) \
+                and torch.equal(g.cpu().view(torch.int32), w.contiguous().view(torch.int32))
+
+        if not all(isinstance(w, (tuple, list)) and len(w) == 2 and all(same(*p) for p in zip(g, w))
+                   for g, w in zip(got, want)):
+            raise ValueError(
+                f"@kt.mapped self-check failed for '{getattr(method, '__name__', method)}': the 'gae' op (gamma="
+                f"{spec.extra['gamma']}, lam={spec.extra['lam']}) does not reproduce the Python body's (advantages, "
+                f"returns) bit for bit on seeded rollouts; refusing to deploy.  The op reads dones[:, t] as the done "
+                f"flag of transition t (the episode ended after the action at step t): CleanRL's dones[t] marks that "
+                f"observation t starts an episode, so pass torch.cat([dones[1:], next_done[None]]).T.contiguous()")
 
     # ---- small-call lane (the local CUDA-stream scheduler for launch-bound calls) ----------------------------
     SMALL_CALL_BYTES = 4 << 20
@@ -415,6 +468,8 @@ class B200Supervisor:
         x, alpha, beta, bound = spec.bind(method, args, kwargs)
         if spec.op == "mlp":
             return self._call_mlp(spec, bound, ranks)
+        if spec.op == "gae":
+            return self._call_gae(spec, bound, ranks)
         if spec.op not in ELEMENTWISE_OPS:
             raise TypeError(f"unsupported mapped op '{spec.op}'")
         if not isinstance(x, torch.Tensor):
@@ -591,3 +646,37 @@ class B200Supervisor:
         except self.ops.PushTimeout as e:
             self._raise_device_timeout(e)
         return out if self._all_ranks(ranks) else [out[r] for r in ranks]
+
+    def _call_gae(self, spec, bound, ranks=None):
+        """(advantages, returns) per selected rank: one ktb_gae_f32 launch on the root over the rows of every run of
+        consecutive selected ranks (all rows when every rank is selected).  The rows stay on the root: the op does a
+        few flops per byte, and spreading them over the ranks' GPUs would move every byte over NVLink twice."""
+        import torch
+
+        from ..device import returns
+
+        rewards, values, dones, last_values = (bound[n] for n in list(bound)[:4])
+        root = self.devices[0]
+        for name, t in (("rewards", rewards), ("values", values), ("dones", dones), ("last_values", last_values)):
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != root:
+                where = t.device if isinstance(t, torch.Tensor) else type(t).__name__
+                raise ValueError(f"the 'gae' op takes CUDA tensors on the root GPU cuda:{root}: {name} is on {where} "
+                                 f"(host tensors are not staged for this op)")
+        gamma, lam = (bound[v] if isinstance(v, str) else v for v in (spec.extra["gamma"], spec.extra["lam"]))
+        check_finite("gamma", gamma)
+        check_finite("lam", lam)
+        if rewards.dim() != 2:
+            raise ValueError(f"rewards must be a 2-D [N, T] tensor, got {list(rewards.shape)}")
+        ranks = list(range(self.world_size)) if ranks is None else list(ranks)
+        bounds = [self.ops.shard_bounds(rewards.shape[0], self.world_size, r) for r in ranks]
+        out = []
+        i = 0
+        while i < len(ranks):   # one launch per run of consecutive ranks
+            j = i
+            while j + 1 < len(ranks) and ranks[j + 1] == ranks[j] + 1:
+                j += 1
+            b, e = bounds[i][0], bounds[j][1]
+            adv, ret = returns.gae(rewards[b:e], values[b:e], dones[b:e], last_values[b:e], gamma, lam)
+            out += [(adv[rb - b:re - b], ret[rb - b:re - b]) for rb, re in bounds[i:j + 1]]
+            i = j + 1
+        return out
