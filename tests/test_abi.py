@@ -27,6 +27,55 @@ def test_library_exports_every_declared_symbol():
     assert lib.ktb_version() == 100
 
 
+def test_ctypes_prototypes_are_read_from_the_header():
+    """lib.py reads every prototype from ktb200.h: known answers for entries that together take every C type the header
+    uses, an error that names a parameter whose type has no rule (never a guess), and one prototype per declared entry
+    plus the ktb_set_tuning knob, which the header does not declare."""
+    from ctypes import (POINTER, c_char_p, c_double, c_float, c_int, c_int32, c_size_t, c_uint, c_uint64, c_ulonglong,
+                        c_void_p)
+
+    ptr, stream = c_void_p, L.c_uintptr
+    layers = [ptr] * 6                                           # W1, b1, W2, b2, W3, b3
+    push = [ptr, ptr, c_int, c_size_t, c_ulonglong, stream]      # ctrl_local, ctrl_root_peer, rank, chunk_rows, seq
+    want = {
+        "ktb_init": (c_int, [c_int, POINTER(c_int)]),
+        "ktb_last_error": (c_char_p, []),
+        "ktb_ipc_export": (c_int, [c_int, ptr, ptr]),
+        "ktb_ipc_open": (c_int, [c_int, ptr, POINTER(ptr)]),
+        "ktb_shard_bounds": (c_int, [c_size_t, c_int, c_int, POINTER(c_size_t), POINTER(c_size_t)]),
+        "ktb_push_status": (c_int, [c_int, ptr, POINTER(c_uint)]),
+        "ktb_scatter_map_reduce": (c_int, [c_int, c_int, ptr, c_size_t, c_size_t, c_double, c_double, c_int,
+                                           POINTER(c_int), c_int, ptr, ptr, POINTER(ptr), POINTER(stream)]),
+        "ktb_push_scatter_ce_sides": (c_int, [c_int, ptr, c_size_t, c_size_t, c_int, c_int, c_int, POINTER(c_int),
+                                              POINTER(ptr), c_size_t, POINTER(ptr), ptr, c_size_t, c_int, POINTER(ptr),
+                                              POINTER(c_size_t), POINTER(c_size_t), c_ulonglong, stream]),
+        # obs, M, d_in, d_hidden, d_out, the layers, mask, logits, actions, scratch, stage, stream
+        "ktb_mlp_bf16_policy_masked": (c_int, [c_int, ptr, c_size_t, c_int, c_int, c_int] + layers
+                                       + [ptr, ptr, ptr, ptr, ptr, stream]),
+        # stage_local, stage_stride, M, d_in, d_hidden, d_out, the layers, nvec, n_groups, mask_offset, seed, row_base,
+        # actions, log_probs, scratch, then the push arguments
+        "ktb_mlp_bf16_policy_sample_multidiscrete_masked_pushed": (
+            c_int, [c_int, ptr, c_size_t, c_size_t, c_int, c_int, c_int] + layers
+            + [POINTER(c_int32), c_int, c_size_t, c_uint64, c_uint64, ptr, ptr, ptr] + push),
+        # the two critics, d_hidden_actor and the actor, log_std_min, log_std_max, squash, seed, row_base, reward, done,
+        # gamma, alpha, y, scratch, stage, stream
+        "ktb_mlp_bf16_td_target_gaussian": (
+            c_int, [c_int, ptr, c_size_t, c_int, c_int, c_int] + layers + layers + [c_int] + layers
+            + [c_float, c_float, c_int, c_uint64, c_uint64, ptr, ptr, c_float, c_float, ptr, ptr, ptr, stream]),
+        "ktb_gae_f32": (c_int, [c_int, ptr, ptr, ptr, ptr, c_size_t, c_size_t, c_float, c_float, ptr, ptr, stream]),
+    }
+    for name, prototype in want.items():
+        assert L._SIGNATURES[name] == prototype, name
+
+    assert L._parse_header("size_t ktb_ok(int n,\n    const float* x); /* int ktb_gone(int); */") == \
+        {"ktb_ok": (c_size_t, [c_int, ptr])}
+    with pytest.raises(TypeError, match=r"ktb_bad: .*parameter 'const struct opts\* o'"):
+        L._parse_header("int ktb_bad(int dev, const struct opts* o, uintptr_t stream);")
+
+    names = _declared_symbols()
+    assert len(L._SIGNATURES) == len(names) + 1 and set(L._SIGNATURES) == set(names) | {"ktb_set_tuning"}
+
+
 def test_library_is_sm90a_only():
     import subprocess
 
