@@ -1081,6 +1081,42 @@ int ktb_mlp_bf16_dqn_target_masked_pushed(int dev, const void* stage_local, size
 int ktb_gae_f32(int dev, const float* rewards, const float* values, const float* dones, const float* last_values,
                 size_t N, size_t T, float gamma, float gamma_lam, float* adv, float* ret, uintptr_t stream);
 
+/* ---- V-trace (IMPALA's off-policy learner target) -------------------------------------------------------------------
+ *
+ * Env-major fp32 [N, T] as for ktb_gae_f32: log_rhos[i, t] = log π(a_t|s_t) − log μ(a_t|s_t), the target policy's
+ * log-probability of the taken action less the behaviour policy's; dones[i, t] the done flag of transition t;
+ * bootstrap[i] = V(s_T).  rho_bar, c_bar and pg_rho_bar are the clipping thresholds ρ̄, c̄ and the policy gradient's
+ * ρ̄; +inf means no clip.
+ *
+ * Per row, as fp32 operations each rounded to nearest even, with no FMA contraction, starting from acc = 0 and
+ * nv = nvs = bootstrap[i], for t = T - 1 down to 0 (lr, r, v, d = log_rhos, rewards, values, dones at [i, t]):
+ *     rho   = expf(lr)
+ *     disc  = gamma * (1 - d)
+ *     cr    = rho > rho_bar ? rho_bar : rho
+ *     c     = lam * (rho > c_bar ? c_bar : rho)
+ *     pr    = rho > pg_rho_bar ? pg_rho_bar : rho
+ *     delta = cr * ((r + disc * nv) - v)
+ *     acc   = delta + (disc * c) * acc
+ *     vs[i, t]     = acc + v
+ *     pg_adv[i, t] = pr * ((r + disc * nvs) - v)
+ *     nv    = v
+ *     nvs   = vs[i, t]
+ * which is bit for bit TorchBeast's from_importance_weights made env-major (tests/policy_vtrace_cases.py) when every
+ * scalar is the fp32 rounding of its Python value, expf is CUDA's correctly-rounded-to-2-ulp expf without fast math
+ * (torch's exp of an fp32 CUDA tensor), and λ = 1 gives TorchBeast's bits.  The clips are compares, so a NaN ρ stays
+ * NaN as under torch.clamp.  A done multiplies by 1 - d = 0, it does not select: an infinite value after an episode
+ * boundary makes the targets before it NaN, as in the torch loop.  vs[i, t + 1] is the scan's previous result, so one
+ * backward pass produces both outputs.
+ *
+ * Checks, in this order: an unregistered dev is KTB_ERR_STATE; a non-finite gamma or lam, or a NaN or non-positive
+ * rho_bar, c_bar or pg_rho_bar (+inf is allowed) is KTB_ERR_ARG; N·T == 0 is KTB_OK with nothing enqueued (the pointers
+ * may then be NULL); otherwise a NULL or not 4-byte-aligned pointer, N·T·4 past SIZE_MAX, or a vs or pg_adv range that
+ * overlaps an input range or the other output is KTB_ERR_ARG.  The kernel reads each input element once and writes
+ * vs[0, N·T) and pg_adv[0, N·T) once each: 24·N·T + 4·N bytes. */
+int ktb_vtrace_f32(int dev, const float* log_rhos, const float* rewards, const float* values, const float* dones,
+                   const float* bootstrap, size_t N, size_t T, float gamma, float lam, float rho_bar, float c_bar,
+                   float pg_rho_bar, float* vs, float* pg_adv, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

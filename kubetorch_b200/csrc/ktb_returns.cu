@@ -1,26 +1,37 @@
-// ktb_returns.cu — generalized advantage estimation (ktb_gae_f32): PPO's advantages and λ-returns of env-major
-// [N, T] rollouts, the reverse linear recurrence of include/ktb200.h evaluated exactly as written there.
+// ktb_returns.cu — the learner targets of env-major [N, T] rollouts, the reverse linear recurrences of include/ktb200.h
+// evaluated exactly as written there:
+//   ktb_gae_f32     generalized advantage estimation: PPO's advantages and λ-returns;
+//   ktb_vtrace_f32  V-trace (IMPALA): off-policy value targets and policy-gradient advantages.
 //
-// HBM-bound: 20·N·T + 4·N bytes, a handful of flops per element.  The recurrence runs along a row, but the rows are
-// stored env-major, so one thread per row would read with a stride of T elements.  Instead each warp owns 32 rows
-// and walks T backwards in 32-step tiles:
-//   loads  for each of its rows the 32 lanes copy 32 consecutive steps of rewards, values and dones into shared
-//          tiles (cp.async, 4 bytes per lane: any T and any 4-byte alignment take the same path, and each row's
-//          32 words are one coalesced access), rows padded to 33 words so that the scan's column reads hit 32 banks;
+// HBM-bound: (4·inputs + 8)·N·T + 4·N bytes, a handful of flops per element.  The recurrence runs along a row, but the
+// rows are stored env-major, so one thread per row would read with a stride of T elements.  Instead each warp owns 32
+// rows and walks T backwards in 32-step tiles:
+//   loads  for each of its rows the 32 lanes copy 32 consecutive steps of every input into shared tiles (cp.async, 4
+//          bytes per lane: any T and any 4-byte alignment take the same path, and each row's 32 words are one
+//          coalesced access), rows padded to 33 words so that the scan's column reads hit 32 banks;
 //   scan   lane i runs row i's recurrence over the tile, right to left, with __fadd_rn / __fmul_rn / __fsub_rn so that
-//          nothing is contracted into an FMA, and writes adv over the rewards and ret over the values;
-//   stores the lanes write the tile's rows of adv and ret back as consecutive steps.
-// kStages tiles are in flight per warp: the loads of the next two (earlier) tiles are issued before the current one
-// is scanned.  A tile shorter than 32 steps (T % 32 at the end of the row, or T < 32) is copied by flat index over
-// its rows, so that small T still moves whole segments.
+//          nothing is contracted into an FMA, and writes the two outputs over the tile's first two input planes;
+//   stores the lanes write the tile's rows of both outputs back as consecutive steps.
+// kStages tiles are in flight per warp: the loads of the next kStages - 1 (earlier) tiles are issued before the current
+// one is scanned.  A tile shorter than 32 steps (T % 32 at the end of the row, or T < 32) is copied by flat index over
+// its rows, so that small T still moves whole segments.  The tile walk is scan_rows(); each op is a per-step functor.
 #include "ktb_common.cuh"
 
 #include <cmath>
 
 namespace ktb {
 
-constexpr int kGaeStages = 3;   // 3 x 12.4 KiB of shared tiles per warp
-constexpr int kGaePad = 33;
+constexpr int kPad = 33;
+constexpr int kGaeStages = 3;      // 3 x 12.4 KiB of shared tiles per warp (3 planes)
+// 2 x 16.5 KiB per warp (4 planes), 6 blocks per SM, in dynamic shared memory.  Three stages (49.5 KiB, past the static
+// limit) measured 0.4-2.5 % slower at every shape of tools/bench_vtrace.py: the per-step exp, not the loads, bounds long
+// rows.  The same two stages as a static array compile to 114 registers instead of 80 and measured 1.8-4.1 % slower
+// (DESIGN.md §4b).
+constexpr int kVtraceStages = 2;
+constexpr int kVtraceSmem = kVtraceStages * 4 * 32 * kPad * 4;   // 33 792 B: under 48 KiB, so no opt-in attribute
+
+template <int P>
+using Tile = float[P][32][kPad];   // [input plane][row][step]
 
 __device__ __forceinline__ void cp_async4(float* smem, const float* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem)), "l"(gmem) : "memory");
@@ -43,12 +54,12 @@ __device__ __forceinline__ void for_tile(int nr, int len, int lane, F&& f) {
   }
 }
 
-// One warp per block and per 32 rows.
-__global__ void __launch_bounds__(32)
-    gae_kernel(const float* __restrict__ rewards, const float* __restrict__ values, const float* __restrict__ dones,
-               const float* __restrict__ last_values, size_t N, size_t T, float gamma, float gamma_lam,
-               float* __restrict__ adv, float* __restrict__ ret) {
-  __shared__ float tile[kGaeStages][3][32][kGaePad];   // [stage][rewards → adv, values → ret, dones][row][step]
+// The tile walk of one warp over its 32 rows: P input planes in[] staged through tile[kStages], step.start(boot[row])
+// once per lane, then step(s, lane, c) for c = len - 1 … 0 of every tile, right to left; step leaves its two outputs
+// in planes 0 and 1, which go to out0 and out1.
+template <int P, int kStages, class Step>
+__device__ __forceinline__ void scan_rows(Tile<P>* tile, const float* const (&in)[P], const float* boot, size_t N,
+                                          size_t T, float* out0, float* out1, Step& step) {
   const int lane = threadIdx.x;
   const size_t row0 = (size_t)blockIdx.x * 32;
   const int nr = (int)(N - row0 < 32 ? N - row0 : 32);
@@ -61,54 +72,128 @@ __global__ void __launch_bounds__(32)
   auto issue = [&](size_t k) {
     if (k < n_tiles) {
       const size_t t0 = t0_of(k);
-      float(*s)[32][kGaePad] = tile[k % kGaeStages];
+      Tile<P>& s = tile[k % kStages];
       for_tile(nr, len_of(t0), lane, [&](int j, int c) {
         const size_t g = base + (size_t)j * T + t0 + c;
-        cp_async4(&s[0][j][c], rewards + g);
-        cp_async4(&s[1][j][c], values + g);
-        cp_async4(&s[2][j][c], dones + g);
+#pragma unroll
+        for (int p = 0; p < P; ++p) cp_async4(&s[p][j][c], in[p] + g);
       });
     }
     cp_async_commit();   // one group per tile, empty past the first step: wait_group counts stay uniform
   };
 
-  for (int k = 0; k < kGaeStages - 1; ++k) issue(k);
-  float acc = 0.0f;
-  float nv = lane < nr ? last_values[row0 + lane] : 0.0f;
+  for (int k = 0; k < kStages - 1; ++k) issue(k);
+  step.start(lane < nr ? boot[row0 + lane] : 0.0f);
   for (size_t k = 0; k < n_tiles; ++k) {
-    issue(k + kGaeStages - 1);
-    cp_async_wait<kGaeStages - 1>();   // this lane's copies of tile k have landed
-    __syncwarp();                      // ... and every other lane's
-    float(*s)[32][kGaePad] = tile[k % kGaeStages];
+    issue(k + kStages - 1);
+    cp_async_wait<kStages - 1>();   // this lane's copies of tile k have landed
+    __syncwarp();                   // ... and every other lane's
+    Tile<P>& s = tile[k % kStages];
     const size_t t0 = t0_of(k);
     const int len = len_of(t0);
     if (lane < nr) {
-      float* rw = s[0][lane];
-      float* vl = s[1][lane];
-      const float* dn = s[2][lane];
-      for (int c = len - 1; c >= 0; --c) {
-        const float v = vl[c];
-        const float nt = __fsub_rn(1.0f, dn[c]);
-        const float delta = __fsub_rn(__fadd_rn(rw[c], __fmul_rn(__fmul_rn(gamma, nv), nt)), v);
-        acc = __fadd_rn(delta, __fmul_rn(__fmul_rn(gamma_lam, nt), acc));
-        rw[c] = acc;
-        vl[c] = __fadd_rn(acc, v);
-        nv = v;
-      }
+      for (int c = len - 1; c >= 0; --c) step(s, lane, c);
     }
     __syncwarp();
     for_tile(nr, len, lane, [&](int j, int c) {
       const size_t g = base + (size_t)j * T + t0 + c;
-      adv[g] = s[0][j][c];
-      ret[g] = s[1][j][c];
+      out0[g] = s[0][j][c];
+      out1[g] = s[1][j][c];
     });
     __syncwarp();   // the stage is reloaded by the next iteration's issue()
   }
 }
 
+// GAE over planes [rewards → adv, values → ret, dones].
+struct GaeStep {
+  float gamma, gamma_lam, acc, nv;
+  __device__ __forceinline__ void start(float last_value) {
+    acc = 0.0f;
+    nv = last_value;
+  }
+  __device__ __forceinline__ void operator()(Tile<3>& s, int j, int c) {
+    const float v = s[1][j][c];
+    const float nt = __fsub_rn(1.0f, s[2][j][c]);
+    const float delta = __fsub_rn(__fadd_rn(s[0][j][c], __fmul_rn(__fmul_rn(gamma, nv), nt)), v);
+    acc = __fadd_rn(delta, __fmul_rn(__fmul_rn(gamma_lam, nt), acc));
+    s[0][j][c] = acc;
+    s[1][j][c] = __fadd_rn(acc, v);
+    nv = v;
+  }
+};
+
+// V-trace over planes [log_rhos → vs, rewards → pg_adv, values, dones].  The clips are compares, so that a NaN ρ stays
+// NaN as under torch.clamp (fminf would return the threshold); a threshold of +inf never clips.
+struct VtraceStep {
+  float gamma, lam, rho_bar, c_bar, pg_rho_bar, acc, nv, nvs;
+  __device__ __forceinline__ void start(float bootstrap) {
+    acc = 0.0f;
+    nv = nvs = bootstrap;
+  }
+  __device__ __forceinline__ void operator()(Tile<4>& s, int j, int c) {
+    const float rho = expf(s[0][j][c]);
+    const float r = s[1][j][c], v = s[2][j][c];
+    const float disc = __fmul_rn(gamma, __fsub_rn(1.0f, s[3][j][c]));
+    const float cr = rho > rho_bar ? rho_bar : rho;
+    const float cc = __fmul_rn(lam, rho > c_bar ? c_bar : rho);
+    const float pr = rho > pg_rho_bar ? pg_rho_bar : rho;
+    const float delta = __fmul_rn(cr, __fsub_rn(__fadd_rn(r, __fmul_rn(disc, nv)), v));
+    acc = __fadd_rn(delta, __fmul_rn(__fmul_rn(disc, cc), acc));
+    const float vs = __fadd_rn(acc, v);
+    s[0][j][c] = vs;
+    s[1][j][c] = __fmul_rn(pr, __fsub_rn(__fadd_rn(r, __fmul_rn(disc, nvs)), v));
+    nv = v;
+    nvs = vs;
+  }
+};
+
+// One warp per block and per 32 rows.
+__global__ void __launch_bounds__(32)
+    gae_kernel(const float* __restrict__ rewards, const float* __restrict__ values, const float* __restrict__ dones,
+               const float* __restrict__ last_values, size_t N, size_t T, float gamma, float gamma_lam,
+               float* __restrict__ adv, float* __restrict__ ret) {
+  __shared__ Tile<3> tile[kGaeStages];
+  const float* const in[3] = {rewards, values, dones};
+  GaeStep step{gamma, gamma_lam};
+  scan_rows<3, kGaeStages>(tile, in, last_values, N, T, adv, ret, step);
+}
+
+__global__ void __launch_bounds__(32)
+    vtrace_kernel(const float* __restrict__ log_rhos, const float* __restrict__ rewards,
+                  const float* __restrict__ values, const float* __restrict__ dones,
+                  const float* __restrict__ bootstrap, size_t N, size_t T, float gamma, float lam, float rho_bar,
+                  float c_bar, float pg_rho_bar, float* __restrict__ vs, float* __restrict__ pg_adv) {
+  extern __shared__ __align__(16) float smem[];
+  const float* const in[4] = {log_rhos, rewards, values, dones};
+  VtraceStep step{gamma, lam, rho_bar, c_bar, pg_rho_bar};
+  scan_rows<4, kVtraceStages>(reinterpret_cast<Tile<4>*>(smem), in, bootstrap, N, T, vs, pg_adv, step);
+}
+
 static bool overlaps(const void* a, size_t an, const void* b, size_t bn) {
   const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
   return x < y + bn && y < x + an;
+}
+
+// The pointer, size and overlap checks of a returns entry, in the header's order: NI inputs (the last one [N], the
+// others [N, T]) then two [N, T] outputs, all fp32.  KTB_OK or KTB_ERR_ARG with the message set.
+template <int NI>
+static int check_buffers(const char* who, const void* const (&ptrs)[NI + 2], const char* const (&names)[NI + 2],
+                         size_t N, size_t T) {
+  for (int i = 0; i < NI + 2; ++i) {
+    KTB_REQUIRE(ptrs[i] != nullptr, KTB_ERR_ARG, "%s: %s is NULL with N*T = %zu*%zu", who, names[i], N, T);
+    KTB_REQUIRE(((uintptr_t)ptrs[i] & 3) == 0, KTB_ERR_ARG, "%s: %s is not 4-byte aligned", who, names[i]);
+  }
+  KTB_REQUIRE(T <= SIZE_MAX / 4 / N, KTB_ERR_ARG, "%s: N*T = %zu*%zu elements is too large", who, N, T);
+  const size_t bytes = N * T * 4;
+  for (int o = NI; o < NI + 2; ++o) {
+    for (int i = 0; i < NI; ++i)
+      KTB_REQUIRE(!overlaps(ptrs[o], bytes, ptrs[i], i == NI - 1 ? N * 4 : bytes), KTB_ERR_ARG, "%s: %s overlaps %s",
+                  who, names[o], names[i]);
+  }
+  KTB_REQUIRE(!overlaps(ptrs[NI], bytes, ptrs[NI + 1], bytes), KTB_ERR_ARG, "%s: %s overlaps %s", who, names[NI],
+              names[NI + 1]);
+  KTB_REQUIRE((N + 31) / 32 <= 0x7fffffffULL, KTB_ERR_ARG, "%s: N = %zu rows is too many", who, N);
+  return KTB_OK;
 }
 
 }  // namespace ktb
@@ -124,26 +209,33 @@ int ktb_gae_f32(int dev, const float* rewards, const float* values, const float*
   KTB_REQUIRE(std::isfinite(gamma) && std::isfinite(gamma_lam), KTB_ERR_ARG,
               "ktb_gae_f32: gamma (%g) and gamma_lam (%g) must be finite", (double)gamma, (double)gamma_lam);
   if (N == 0 || T == 0) return KTB_OK;
-  const void* ptrs[6] = {rewards, values, dones, last_values, adv, ret};
-  const char* names[6] = {"rewards", "values", "dones", "last_values", "adv", "ret"};
-  for (int i = 0; i < 6; ++i) {
-    KTB_REQUIRE(ptrs[i] != nullptr, KTB_ERR_ARG, "ktb_gae_f32: %s is NULL with N*T = %zu*%zu", names[i], N, T);
-    KTB_REQUIRE(((uintptr_t)ptrs[i] & 3) == 0, KTB_ERR_ARG, "ktb_gae_f32: %s is not 4-byte aligned", names[i]);
-  }
-  KTB_REQUIRE(T <= SIZE_MAX / 4 / N, KTB_ERR_ARG, "ktb_gae_f32: N*T = %zu*%zu elements is too large", N, T);
-  const size_t bytes = N * T * 4;
-  const size_t in_bytes[4] = {bytes, bytes, bytes, N * 4};
-  for (int o = 4; o < 6; ++o) {
-    for (int i = 0; i < 4; ++i)
-      KTB_REQUIRE(!overlaps(ptrs[o], bytes, ptrs[i], in_bytes[i]), KTB_ERR_ARG, "ktb_gae_f32: %s overlaps %s",
-                  names[o], names[i]);
-  }
-  KTB_REQUIRE(!overlaps(adv, bytes, ret, bytes), KTB_ERR_ARG, "ktb_gae_f32: adv overlaps ret");
+  if ((rc = check_buffers<4>("ktb_gae_f32", {rewards, values, dones, last_values, adv, ret},
+                             {"rewards", "values", "dones", "last_values", "adv", "ret"}, N, T)))
+    return rc;
   KTB_GUARD(dev);
-  const size_t grid = (N + 31) / 32;
-  KTB_REQUIRE(grid <= 0x7fffffffULL, KTB_ERR_ARG, "ktb_gae_f32: N = %zu rows is too many", N);
-  gae_kernel<<<(unsigned)grid, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(rewards, values, dones, last_values,
-                                                                                   N, T, gamma, gamma_lam, adv, ret);
+  gae_kernel<<<(unsigned)((N + 31) / 32), 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+      rewards, values, dones, last_values, N, T, gamma, gamma_lam, adv, ret);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
+}
+
+int ktb_vtrace_f32(int dev, const float* log_rhos, const float* rewards, const float* values, const float* dones,
+                   const float* bootstrap, size_t N, size_t T, float gamma, float lam, float rho_bar, float c_bar,
+                   float pg_rho_bar, float* vs, float* pg_adv, uintptr_t stream) {
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(std::isfinite(gamma) && std::isfinite(lam), KTB_ERR_ARG,
+              "ktb_vtrace_f32: gamma (%g) and lam (%g) must be finite", (double)gamma, (double)lam);
+  KTB_REQUIRE(rho_bar > 0.0f && c_bar > 0.0f && pg_rho_bar > 0.0f, KTB_ERR_ARG,
+              "ktb_vtrace_f32: rho_bar (%g), c_bar (%g) and pg_rho_bar (%g) must be > 0 (+inf: no clip)",
+              (double)rho_bar, (double)c_bar, (double)pg_rho_bar);
+  if (N == 0 || T == 0) return KTB_OK;
+  if ((rc = check_buffers<5>("ktb_vtrace_f32", {log_rhos, rewards, values, dones, bootstrap, vs, pg_adv},
+                             {"log_rhos", "rewards", "values", "dones", "bootstrap", "vs", "pg_adv"}, N, T)))
+    return rc;
+  KTB_GUARD(dev);
+  vtrace_kernel<<<(unsigned)((N + 31) / 32), 32, kVtraceSmem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      log_rhos, rewards, values, dones, bootstrap, N, T, gamma, lam, rho_bar, c_bar, pg_rho_bar, vs, pg_adv);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }

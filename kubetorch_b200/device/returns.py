@@ -1,7 +1,9 @@
-"""Generalized advantage estimation on the device: ktb_gae_f32 (include/ktb200.h) over torch tensors.
-
-The advantages and λ-returns of env-major fp32 rollouts [N, T], bit for bit the per-step torch loop of CleanRL
-(tests/policy_gae_cases.py), in one kernel launch on the caller's current stream."""
+"""The learner targets of env-major fp32 rollouts [N, T] on the device, each in one kernel launch on the caller's
+current stream (include/ktb200.h):
+  gae     ktb_gae_f32: PPO's advantages and λ-returns, bit for bit CleanRL's per-step torch loop
+          (tests/policy_gae_cases.py);
+  vtrace  ktb_vtrace_f32: IMPALA's V-trace targets and policy-gradient advantages, bit for bit TorchBeast's
+          from_importance_weights made env-major (tests/policy_vtrace_cases.py)."""
 from __future__ import annotations
 
 import math
@@ -9,7 +11,7 @@ from typing import Optional, Tuple
 
 import torch
 
-from ..mapped import check_finite
+from ..mapped import check_finite, check_threshold
 from . import lib as L
 from . import ops
 
@@ -63,3 +65,58 @@ def gae(rewards: torch.Tensor, values: torch.Tensor, dones: torch.Tensor, last_v
     L.call("ktb_gae_f32", dev, rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), last_values.data_ptr(),
            shape[0], shape[1], g, gl, adv.data_ptr(), ret.data_ptr(), ops._stream(dev, stream))
     return adv, ret
+
+
+def _fp32(v) -> float:
+    return torch.tensor(float(v), dtype=torch.float32).item()
+
+
+def vtrace_scalars(gamma, lam, rho_bar, c_bar, pg_rho_bar) -> Tuple[float, float, float, float, float]:
+    """(gamma, lam, rho_bar, c_bar, pg_rho_bar) as the fp32 values ktb_vtrace_f32 takes, each rounded as torch rounds a
+    Python scalar that meets an fp32 tensor, a threshold of None as +inf (no clip); ValueError naming the first bad
+    argument: gamma and lam must be finite numbers, finite in float32, and each threshold a number > 0 in float32."""
+    check_finite("gamma", gamma)
+    check_finite("lam", lam)
+    out = []
+    for name, v in (("gamma", gamma), ("lam", lam)):
+        out.append(_fp32(v))
+        if not math.isfinite(out[-1]):
+            raise ValueError(f"{name}={v!r} must be finite in float32")
+    for name, v in (("rho_bar", rho_bar), ("c_bar", c_bar), ("pg_rho_bar", pg_rho_bar)):
+        check_threshold(name, v)
+        out.append(math.inf if v is None else _fp32(v))
+        if not out[-1] > 0:
+            raise ValueError(f"{name}={v!r} must be > 0 in float32")
+    return tuple(out)
+
+
+def vtrace(log_rhos: torch.Tensor, rewards: torch.Tensor, values: torch.Tensor, dones: torch.Tensor,
+           bootstrap_value: torch.Tensor, gamma, lam=1.0, rho_bar=1.0, c_bar=1.0, pg_rho_bar=1.0,
+           vs: Optional[torch.Tensor] = None, pg_adv: Optional[torch.Tensor] = None,
+           stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(vs, pg_advantages) of env-major rollouts: log_rhos (target less behaviour log-probabilities of the taken
+    actions), rewards, values and dones fp32 [N, T] (row i is environment i's trajectory; dones[i, t] = 1 when the
+    episode ended after the action at step t), bootstrap_value fp32 [N] = V(s_T).  rho_bar, c_bar and pg_rho_bar clip
+    ρ in the TD errors, the traces and the policy gradient (None: no clip); lam is seed_rl's lambda_.  Every tensor is
+    contiguous and on one CUDA device.  vs and pg_adv are fresh fp32 [N, T] tensors unless given; given ones must not
+    overlap the inputs or each other.  Enqueued on `stream` (default: the current stream of that device)."""
+    if not isinstance(rewards, torch.Tensor) or rewards.dim() != 2:
+        raise ValueError(f"rewards must be a 2-D [N, T] tensor, got "
+                         f"{list(rewards.shape) if isinstance(rewards, torch.Tensor) else type(rewards).__name__}")
+    shape, device = tuple(rewards.shape), rewards.device
+    _check("rewards", rewards, shape, device)
+    _check("log_rhos", log_rhos, shape, device)
+    _check("values", values, shape, device)
+    _check("dones", dones, shape, device)
+    _check("bootstrap_value", bootstrap_value, shape[:1], device)
+    scalars = vtrace_scalars(gamma, lam, rho_bar, c_bar, pg_rho_bar)
+    vs = torch.empty(shape, dtype=torch.float32, device=device) if vs is None else vs
+    pg_adv = torch.empty(shape, dtype=torch.float32, device=device) if pg_adv is None else pg_adv
+    _check("vs", vs, shape, device)
+    _check("pg_adv", pg_adv, shape, device)
+    dev = device.index
+    ops.ensure_init([dev])
+    L.call("ktb_vtrace_f32", dev, log_rhos.data_ptr(), rewards.data_ptr(), values.data_ptr(), dones.data_ptr(),
+           bootstrap_value.data_ptr(), shape[0], shape[1], *scalars, vs.data_ptr(), pg_adv.data_ptr(),
+           ops._stream(dev, stream))
+    return vs, pg_adv

@@ -1,6 +1,6 @@
 """Registry of *mapped callables*: user functions whose body is one of the closed set of ops that
 libktb200 executes as sm_90a kernels (identity / scale / affine, their sum-reduced forms, the
-bf16 MLP policy, and generalized advantage estimation).
+bf16 MLP policy, generalized advantage estimation and V-trace).
 
 Arbitrary Python cannot become a CUDA kernel, so the device route is opt-in by declaration:
 
@@ -25,10 +25,15 @@ from .sampling import _check_seed
 
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
-ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae")
+ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace")
 # The options of op="gae": gamma and lam, each required (a finite number or the name of a call argument holding one),
 # and self_check
 GAE_OPTIONS = ("gamma", "lam")
+# The options of op="vtrace" and their defaults (None: required) beside self_check: gamma and lam a finite number or the
+# name of a call argument holding one (VTRACE_ARGUMENTS); rho_bar, c_bar and pg_rho_bar constants, a number > 0 or None
+# (no clip).  mapped() stores every default it fills in into MappedSpec.extra.
+VTRACE_OPTIONS = dict(gamma=None, lam=1.0, rho_bar=1.0, c_bar=1.0, pg_rho_bar=1.0)
+VTRACE_ARGUMENTS = ("gamma", "lam")
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
                "gaussian_evaluate", "deterministic", "critic", "td_target", "dqn_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
@@ -303,11 +308,30 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
     .contiguous()``.  For truncated episodes add ``gamma * V(final_obs)`` to the reward, as SB3 does.  ``gamma=`` and
     ``lam=`` are required, each a finite number or the name of a call argument that holds one (checked per call);
     ``self_check=False`` skips the deployment's check of a constant γ and λ against the body.  Every other option is
+    refused.
+
+    The "vtrace" op is V-trace, IMPALA's off-policy learner target: the callable is ``(log_rhos, rewards, values, dones,
+    bootstrap_value, ...)`` with fp32 ``[N, T]`` log_rhos, rewards, values and dones in the env-major layout of "gae"
+    and fp32 ``[N]`` bootstrap_value, V(s_T), all CUDA tensors on the root GPU.  Each rank returns ``(vs,
+    pg_advantages)`` of its rows, ``x.chunk(WORLD_SIZE)[RANK]``: TorchBeast's ``from_importance_weights`` with
+    ``discounts = gamma * (1 - dones)``, ``rhos = exp(log_rhos)`` clipped at ``rho_bar`` in the TD errors, ``lam *
+    clamp(rhos, max=c_bar)`` as the traces and ``clamp(rhos, max=pg_rho_bar)`` in the advantages, bit for bit as torch
+    computes it on the GPU (tests/policy_vtrace_cases.py).  ``dones[:, t]`` is the done flag of transition t, which is
+    TorchBeast's ``batch["done"][1:]``.  From TorchBeast's time-major ``[T, B]`` tensors pass ``x.T.contiguous()`` and
+    ``bootstrap_value = baseline[-1]``; from the evaluate head, ``log_rhos = (target_lp - behaviour_lp).view(N, T)``
+    with ``behaviour_lp`` the log-probabilities of ``output="sample"`` (or ``"gaussian"``) at rollout and ``target_lp``
+    those of ``output="evaluate"`` (or ``"gaussian_evaluate"``) under the learner's weights.  ``gamma=`` is required and
+    ``lam=`` (seed_rl's ``lambda_``) defaults to 1.0, each a finite number or the name of a call argument that holds one
+    (checked per call); ``rho_bar=``, ``c_bar=`` and ``pg_rho_bar=`` are constants, a number > 0 or None for no clip,
+    each 1.0 by default (TorchBeast clamps the traces at 1.0 whatever ``c_bar``: declare ``c_bar=1.0`` for its bits).
+    ``self_check=False`` skips the deployment's check of constant options against the body.  Every other option is
     refused."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if op == "gae":
         _check_gae_options(alpha, beta, reduce, arg, extra)
+    if op == "vtrace":
+        _check_vtrace_options(alpha, beta, reduce, arg, extra)
     beta = 0.0 if beta is _UNSET else beta
     if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
         extra["alpha"] = alpha
@@ -349,8 +373,11 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
         if op == "gae" and len(params) < 4:
             raise ValueError(f"a 'gae' callable takes (rewards, values, dones, last_values, ...) positionally, "
                              f"{getattr(fn, '__name__', fn)!r} has {len(params)} parameters")
+        if op == "vtrace" and len(params) < 5:
+            raise ValueError(f"a 'vtrace' callable takes (log_rhos, rewards, values, dones, bootstrap_value, ...) "
+                             f"positionally, {getattr(fn, '__name__', fn)!r} has {len(params)} parameters")
         for option, names in extra.items():
-            if not (isinstance(names, str) if op == "gae" else names_arguments(option, names)):
+            if not (isinstance(names, str) if op in ("gae", "vtrace") else names_arguments(option, names)):
                 continue
             for name in (names,) if isinstance(names, str) else names:
                 if name not in params:
@@ -379,6 +406,39 @@ def _check_gae_options(alpha, beta, reduce, arg, extra) -> None:
             check_finite(name, extra[name])
     if not isinstance(extra.get("self_check", False), bool):
         raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
+
+
+def _check_vtrace_options(alpha, beta, reduce, arg, extra) -> None:
+    """The options of op="vtrace", or ValueError naming the first it does not take or the first it lacks; a constant
+    gamma or lam must be a finite number and each threshold a number > 0 or None.  Fills in the defaults of the options
+    not given (extra keeps them)."""
+    refused = dict(alpha=alpha is not _UNSET, beta=beta is not _UNSET, reduce=reduce is not None, arg=arg is not None)
+    refused.update((k, True) for k in extra if k not in (*VTRACE_OPTIONS, "self_check"))
+    for name, given in refused.items():
+        if given:
+            raise ValueError(f"{name}= is not an option of the 'vtrace' op, which takes gamma=, lam=, rho_bar=, c_bar=, "
+                             f"pg_rho_bar= and self_check=: its callable is (log_rhos, rewards, values, dones, "
+                             f"bootstrap_value) and it returns (vs, pg_advantages)")
+    for name, default in VTRACE_OPTIONS.items():
+        if name not in extra:
+            if default is None:
+                raise ValueError(f"{name}= is required with the 'vtrace' op: a finite number or the name of a call "
+                                 f"argument that holds one")
+            extra[name] = default
+        elif name in VTRACE_ARGUMENTS:
+            if not isinstance(extra[name], str):
+                check_finite(name, extra[name])
+        else:
+            check_threshold(name, extra[name])
+    if not isinstance(extra.get("self_check", False), bool):
+        raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
+
+
+def check_threshold(name: str, v):
+    """rho_bar, c_bar or pg_rho_bar of V-trace: a number (not a bool) > 0, or None for no clip."""
+    if v is not None and (isinstance(v, bool) or not isinstance(v, (int, float)) or not v > 0):
+        raise ValueError(f"{name} must be a number > 0 or None (no clip), got {v!r}")
+    return v
 
 
 def names_arguments(option: str, v) -> bool:

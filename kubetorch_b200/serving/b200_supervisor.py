@@ -38,6 +38,8 @@ One controller process drives N local H100s.  For a @kt.mapped callable a remote
         ktb_scatter_map_reduce: per-rank warp-shuffle reduction, scalar peer-stored to the root.
     "gae"
         ktb_gae_f32: one launch on the root GPU over every selected rank's rows.
+    "vtrace"
+        ktb_vtrace_f32: the same, one launch on the root GPU.
 
 There is NO CPU fallback here: a missing library or GPU raises.
 """
@@ -52,8 +54,8 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, TD_OPTIONS, check_finite, mapped_spec,
-                      names_arguments)
+from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, TD_OPTIONS, VTRACE_ARGUMENTS,
+                      VTRACE_OPTIONS, check_finite, mapped_spec, names_arguments)
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -199,6 +201,8 @@ class B200Supervisor:
             spec = mapped_spec(method)
             if spec.op == "gae" and spec.extra.get("self_check") is not False:
                 self._self_check_gae(spec, method)
+            if spec.op == "vtrace" and spec.extra.get("self_check") is not False:
+                self._self_check_vtrace(spec, method)
             if spec.op not in ELEMENTWISE_OPS or spec.extra.get("self_check") is False:
                 continue
             if not (isinstance(spec.alpha, (int, float)) and isinstance(spec.beta, (int, float))):
@@ -297,6 +301,62 @@ class B200Supervisor:
                 f"returns) bit for bit on seeded rollouts; refusing to deploy.  The op reads dones[:, t] as the done "
                 f"flag of transition t (the episode ended after the action at step t): CleanRL's dones[t] marks that "
                 f"observation t starts an episode, so pass torch.cat([dones[1:], next_done[None]]).T.contiguous()")
+
+    def _self_check_vtrace(self, spec, method):
+        """A "vtrace" callable with a constant gamma and lam: its body on the root GPU, rank by rank, against the kernel
+        on seeded (4·world + 3, 9) rollouts whose log-ratios fall on both sides of every threshold, with some done = 1;
+        refuse the deployment on any bit difference.  The body runs on the GPU because ρ = exp(log_rhos) is CUDA's expf
+        there, which torch's CPU exp does not reproduce.  This catches a body that reads dones as episode starts, a γ,
+        λ or threshold other than declared (TorchBeast's traces clamped at 1.0 under another c_bar=)."""
+        import inspect
+
+        import torch
+
+        if any(isinstance(spec.extra[k], str) for k in VTRACE_ARGUMENTS) or \
+                len(inspect.signature(method).parameters) != 5:
+            return   # gamma or lam is a call argument: nothing constant to check at deploy time
+        world, dev0 = self.world_size, self.devices[0]
+        gen = torch.Generator().manual_seed(1234)
+        n, t = 4 * world + 3, 9
+        # log-ratios spread over ±2.3: ρ from 0.1 to 10, across any threshold a deployment would declare
+        log_rhos = (torch.rand(n, t, generator=gen) * 4.6 - 2.3)
+        rewards, values = torch.randn(n, t, generator=gen), torch.randn(n, t, generator=gen)
+        dones = (torch.rand(n, t, generator=gen) < 0.25).float()
+        dones[::3, t // 2] = 1.0
+        bootstrap = torch.randn(n, generator=gen)
+        args = [a.to(f"cuda:{dev0}") for a in (log_rhos, rewards, values, dones, bootstrap)]
+        saved = {k: os.environ.get(k) for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK")}
+        want = []
+        try:
+            with torch.cuda.device(dev0):
+                for r in range(world):
+                    os.environ.update({"RANK": str(r), "WORLD_SIZE": str(world), "LOCAL_RANK": str(r)})
+                    want.append(method(*(a.clone() for a in args)))
+        except Exception:  # noqa: BLE001 - a body that cannot run here (needs an argument, a group, ...) is skipped
+            return
+        finally:
+            for k, v in saved.items():
+                if v is None:
+                    os.environ.pop(k, None)
+                else:
+                    os.environ[k] = v
+        got = self._run_mapped(spec, method, args, {}, list(range(world)))
+        self.ops.synchronize(dev0)
+
+        def same(g, w):
+            return isinstance(w, torch.Tensor) and w.dtype == torch.float32 and tuple(g.shape) == tuple(w.shape) \
+                and torch.equal(g.cpu().view(torch.int32), w.cpu().contiguous().view(torch.int32))
+
+        if not all(isinstance(w, (tuple, list)) and len(w) == 2 and all(same(*p) for p in zip(g, w))
+                   for g, w in zip(got, want)):
+            declared = ", ".join(f"{k}={spec.extra[k]}" for k in VTRACE_OPTIONS)
+            raise ValueError(
+                f"@kt.mapped self-check failed for '{getattr(method, '__name__', method)}': the 'vtrace' op ({declared}) "
+                f"does not reproduce the Python body's (vs, pg_advantages) bit for bit on seeded rollouts; refusing to "
+                f"deploy.  The op computes TorchBeast's from_importance_weights with the declared gamma, lam (seed_rl's "
+                f"lambda_) and thresholds, clamping the traces at c_bar (TorchBeast clamps them at 1.0: declare "
+                f"c_bar=1.0), and reads dones[:, t] as the done flag of transition t, TorchBeast's batch['done'][1:] "
+                f"(not a flag that observation t starts an episode)")
 
     # ---- small-call lane (the local CUDA-stream scheduler for launch-bound calls) ----------------------------
     SMALL_CALL_BYTES = 4 << 20
@@ -470,6 +530,8 @@ class B200Supervisor:
             return self._call_mlp(spec, bound, ranks)
         if spec.op == "gae":
             return self._call_gae(spec, bound, ranks)
+        if spec.op == "vtrace":
+            return self._call_vtrace(spec, bound, ranks)
         if spec.op not in ELEMENTWISE_OPS:
             raise TypeError(f"unsupported mapped op '{spec.op}'")
         if not isinstance(x, torch.Tensor):
@@ -651,20 +713,36 @@ class B200Supervisor:
         """(advantages, returns) per selected rank: one ktb_gae_f32 launch on the root over the rows of every run of
         consecutive selected ranks (all rows when every rank is selected).  The rows stay on the root: the op does a
         few flops per byte, and spreading them over the ranks' GPUs would move every byte over NVLink twice."""
-        import torch
-
         from ..device import returns
 
-        rewards, values, dones, last_values = (bound[n] for n in list(bound)[:4])
+        return self._call_returns(spec, bound, ranks, ("rewards", "values", "dones", "last_values"), returns.gae)
+
+    def _call_vtrace(self, spec, bound, ranks=None):
+        """(vs, pg_advantages) per selected rank: one ktb_vtrace_f32 launch on the root per run of consecutive selected
+        ranks, as _call_gae."""
+        from ..device import returns
+
+        bars = {k: spec.extra[k] for k in ("rho_bar", "c_bar", "pg_rho_bar")}
+        return self._call_returns(spec, bound, ranks, ("log_rhos", "rewards", "values", "dones", "bootstrap_value"),
+                                  lambda *xs: returns.vtrace(*xs, **bars))
+
+    def _call_returns(self, spec, bound, ranks, names, launch):
+        """The first len(names) call arguments, checked to be CUDA tensors on the root GPU, and gamma and lam (constants
+        or call arguments) checked to be finite: launch(*rows, gamma, lam) over the rows of every run of consecutive
+        selected ranks, its pair of [rows, T] outputs split into one pair of views per rank."""
+        import torch
+
+        tensors = [bound[n] for n in list(bound)[:len(names)]]
         root = self.devices[0]
-        for name, t in (("rewards", rewards), ("values", values), ("dones", dones), ("last_values", last_values)):
+        for name, t in zip(names, tensors):
             if not isinstance(t, torch.Tensor) or not t.is_cuda or t.device.index != root:
                 where = t.device if isinstance(t, torch.Tensor) else type(t).__name__
-                raise ValueError(f"the 'gae' op takes CUDA tensors on the root GPU cuda:{root}: {name} is on {where} "
-                                 f"(host tensors are not staged for this op)")
+                raise ValueError(f"the '{spec.op}' op takes CUDA tensors on the root GPU cuda:{root}: {name} is on "
+                                 f"{where} (host tensors are not staged for this op)")
         gamma, lam = (bound[v] if isinstance(v, str) else v for v in (spec.extra["gamma"], spec.extra["lam"]))
         check_finite("gamma", gamma)
         check_finite("lam", lam)
+        rewards = tensors[names.index("rewards")]
         if rewards.dim() != 2:
             raise ValueError(f"rewards must be a 2-D [N, T] tensor, got {list(rewards.shape)}")
         ranks = list(range(self.world_size)) if ranks is None else list(ranks)
@@ -676,7 +754,7 @@ class B200Supervisor:
             while j + 1 < len(ranks) and ranks[j + 1] == ranks[j] + 1:
                 j += 1
             b, e = bounds[i][0], bounds[j][1]
-            adv, ret = returns.gae(rewards[b:e], values[b:e], dones[b:e], last_values[b:e], gamma, lam)
-            out += [(adv[rb - b:re - b], ret[rb - b:re - b]) for rb, re in bounds[i:j + 1]]
+            first, second = launch(*(x[b:e] for x in tensors), gamma, lam)
+            out += [(first[rb - b:re - b], second[rb - b:re - b]) for rb, re in bounds[i:j + 1]]
             i = j + 1
         return out
