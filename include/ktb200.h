@@ -1117,6 +1117,37 @@ int ktb_vtrace_f32(int dev, const float* log_rhos, const float* rewards, const f
                    const float* bootstrap, size_t N, size_t T, float gamma, float lam, float rho_bar, float c_bar,
                    float pg_rho_bar, float* vs, float* pg_adv, uintptr_t stream);
 
+/* ---- n-step bootstrapped returns (Ape-X's, R2D2's and A3C's learner targets) ----------------------------------------
+ *
+ * Env-major fp32 [N, T] as for ktb_gae_f32: dones[i, t] the done flag of transition t; values[i, t] the bootstrap
+ * value of state s_t (V(s_t), max_a Q(s_t, a) or a Double-DQN value); baseline[i, t] what the TD error is taken
+ * against (Q(s_t, a_t) for Ape-X priorities, values itself for A3C's advantages); last_values[i] = V(s_T).
+ *
+ * Per element (i, t), as fp32 operations each rounded to nearest even, with no FMA contraction:
+ *     acc = t + n < T ? values[i, t + n] : last_values[i]
+ *     for k = n - 1 down to 0:
+ *         (r, disc) = t + k < T ? (rewards[i, t + k], gamma * (1 - dones[i, t + k])) : (0, 1)
+ *         acc = r + disc * acc
+ *     ret[i, t] = acc
+ *     td[i, t]  = acc - baseline[i, t]
+ * which is bit for bit rlax's n_step_bootstrapped_returns at lambda_t = 1 made env-major (tests/policy_nstep_cases.py,
+ * the body pads the rollout's end with n - 1 steps of reward 0, discount 1 and value V(s_T)) when gamma is the fp32
+ * rounding of γ, as torch rounds a Python scalar that meets an fp32 tensor.  The padded steps past T are real
+ * operations, 0 + 1·acc: a −0 becomes +0 there and a NaN stays NaN, as in the padded torch loop.  A done multiplies by
+ * 1 - d = 0, it does not select: an infinite bootstrap value after an episode boundary makes the returns before it NaN,
+ * as in GAE.  n is at most 32, so every window lies inside the current 32-step tile and the next one; n >= T is
+ * allowed, and then every return bootstraps from last_values.  Inputs may alias one another.
+ *
+ * Checks, in this order: an unregistered dev is KTB_ERR_STATE; n outside [1, 32] or a non-finite gamma is KTB_ERR_ARG;
+ * N·T == 0 is KTB_OK with nothing enqueued (the pointers may then be NULL); otherwise a NULL or not 4-byte-aligned
+ * pointer, N·T·4 past SIZE_MAX, a ret or td range that overlaps an input range or the other output, or more than
+ * 32·(2³¹ − 1) rows is KTB_ERR_ARG.  The kernel reads each input element once (the halo of the last 32-step tile of
+ * each warp's span, at most n steps per row, once more) and writes ret[0, N·T) and td[0, N·T) once each: 24·N·T + 4·N
+ * bytes. */
+int ktb_nstep_f32(int dev, const float* rewards, const float* values, const float* dones, const float* baseline,
+                  const float* last_values, size_t N, size_t T, int n, float gamma, float* ret, float* td,
+                  uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,7 +1,9 @@
 // ktb_returns.cu — the learner targets of env-major [N, T] rollouts, the reverse linear recurrences of include/ktb200.h
 // evaluated exactly as written there:
 //   ktb_gae_f32     generalized advantage estimation: PPO's advantages and λ-returns;
-//   ktb_vtrace_f32  V-trace (IMPALA): off-policy value targets and policy-gradient advantages.
+//   ktb_vtrace_f32  V-trace (IMPALA): off-policy value targets and policy-gradient advantages;
+// and the n-step bootstrapped returns that are no recurrence along the row (nstep_kernel, after the first two):
+//   ktb_nstep_f32   Ape-X's, R2D2's and A3C's n-step targets and their TD errors.
 //
 // HBM-bound: (4·inputs + 8)·N·T + 4·N bytes, a handful of flops per element.  The recurrence runs along a row, but the
 // rows are stored env-major, so one thread per row would read with a stride of T elements.  Instead each warp owns 32
@@ -169,6 +171,105 @@ __global__ void __launch_bounds__(32)
   scan_rows<4, kVtraceStages>(reinterpret_cast<Tile<4>*>(smem), in, bootstrap, N, T, vs, pg_adv, step);
 }
 
+// n-step bootstrapped returns.  Unlike the two recurrences above, output (i, t) depends only on the window of steps
+// [t, t + n] of its row, so the grid splits T as well as N: block (x, y) is one warp over rows [32x, 32x + 32) and the
+// span of kNstepSpan consecutive 32-step tiles starting at tile y·span.  The warp walks its span forwards with a ring of
+// two tiles per row in shared memory, the current one and the next (the windows' halo), so a tile copied as the halo is
+// the next iteration's current tile and is read from global memory once; only the span's last halo is cut to the n
+// steps the windows reach.  Steps past T hold the header's padding (reward 0, discount 1, value V(s_T)), so every
+// window runs its n operations with no branch.  Lane c computes step t0 + c of kNstepRows rows at a time: its reads of
+// ring position (c + k) & 63 are consecutive across the lanes (no bank conflicts), and the rows' chains interleave.
+// One tile per warp and eight rows at a time measured fastest at three of the four shapes of tools/bench_nstep.py (one
+// tile and four rows: 1-17 % slower; two tiles: up to 86 % slower, 2-8 % faster at (16384, 128); four: slower at
+// every shape): the warp waits for its copies once per tile, so more warps beat a longer span (DESIGN.md §4b).  The
+// span is larger only where T has more than 65535 tiles, the grid's y limit.
+constexpr int kNstepSpan = 1;
+constexpr int kNstepRows = 8;
+
+__global__ void __launch_bounds__(32)
+    nstep_kernel(const float* __restrict__ rewards, const float* __restrict__ values, const float* __restrict__ dones,
+                 const float* __restrict__ baseline, const float* __restrict__ last_values, size_t N, size_t T, int n,
+                 float gamma, size_t span, float* __restrict__ ret, float* __restrict__ td) {
+  __shared__ __align__(16) float2 rd[32][64];   // [row][ring position]: (reward, gamma·(1 − done)), 16 KiB
+  __shared__ float vv[32][64];                  // [row][ring position]: value, 8 KiB
+  const int lane = threadIdx.x;
+  const size_t row0 = (size_t)blockIdx.x * 32;
+  const int nr = (int)(N - row0 < 32 ? N - row0 : 32);
+  const size_t n_tiles = (T + 31) / 32;
+  const size_t k0 = (size_t)blockIdx.y * span;
+  const size_t k1 = k0 + span < n_tiles ? k0 + span : n_tiles;
+  const size_t base = row0 * T;
+  const float lv = lane < nr ? last_values[row0 + lane] : 0.0f;   // V(s_T) of row `lane`
+
+  auto len_of = [&](size_t k) { return k < n_tiles ? (int)(T - k * 32 < 32 ? T - k * 32 : 32) : 0; };
+  // the steps of tile k to copy: all of them inside the span, the n that the last windows reach past it
+  auto count = [&](size_t k) { return k < k1 ? len_of(k) : min(len_of(k), n); };
+  auto issue = [&](size_t k, int cnt) {
+    const int p0 = (int)(k & 1) * 32;
+    for_tile(nr, cnt, lane, [&](int j, int c) {
+      const size_t g = base + (size_t)j * T + k * 32 + c;
+      cp_async4(&rd[j][p0 + c].x, rewards + g);
+      cp_async4(&rd[j][p0 + c].y, dones + g);
+      cp_async4(&vv[j][p0 + c], values + g);
+    });
+  };
+  // once tile k's copies have landed: the discount of each copied step, and the padding at every other position
+  auto convert = [&](size_t k, int cnt) {
+    const int p = (int)(k & 1) * 32 + lane;
+    for (int j = 0; j < nr; ++j) {
+      const float lvj = __shfl_sync(0xffffffffu, lv, j);
+      if (lane < cnt) {
+        rd[j][p].y = __fmul_rn(gamma, __fsub_rn(1.0f, rd[j][p].y));
+      } else {
+        rd[j][p] = make_float2(0.0f, 1.0f);
+        vv[j][p] = lvj;
+      }
+    }
+  };
+
+  issue(k0, len_of(k0));
+  for (size_t k = k0; k < k1; ++k) {
+    issue(k + 1, count(k + 1));
+    cp_async_commit();
+    const bool live = lane < len_of(k);
+    const size_t g0 = base + k * 32 + lane;
+    float b[32];   // the tile's baseline, read while the copies are in flight: one memory latency per tile
+#pragma unroll
+    for (int j = 0; j < 32; ++j) b[j] = live && j < nr ? baseline[g0 + (size_t)j * T] : 0.0f;
+    cp_async_wait<0>();
+    __syncwarp();
+    if (k == k0) convert(k0, len_of(k0));
+    convert(k + 1, count(k + 1));
+    __syncwarp();
+    const int p = (int)(k & 1) * 32 + lane;
+#pragma unroll
+    for (int j0 = 0; j0 < 32; j0 += kNstepRows) {   // rows past nr are computed from stale tiles and never stored
+      if (j0 >= nr) break;
+      float acc[kNstepRows];
+#pragma unroll
+      for (int r = 0; r < kNstepRows; ++r) acc[r] = vv[j0 + r][(p + n) & 63];
+#pragma unroll 2
+      for (int i = n - 1; i >= 0; --i) {
+        const int q = (p + i) & 63;
+#pragma unroll
+        for (int r = 0; r < kNstepRows; ++r) {
+          const float2 x = rd[j0 + r][q];
+          acc[r] = __fadd_rn(x.x, __fmul_rn(x.y, acc[r]));
+        }
+      }
+#pragma unroll
+      for (int r = 0; r < kNstepRows; ++r) {
+        if (live && j0 + r < nr) {
+          const size_t g = g0 + (size_t)(j0 + r) * T;
+          ret[g] = acc[r];
+          td[g] = __fsub_rn(acc[r], b[j0 + r]);
+        }
+      }
+    }
+    __syncwarp();   // slot k & 1 is reloaded by the next iteration's issue()
+  }
+}
+
 static bool overlaps(const void* a, size_t an, const void* b, size_t bn) {
   const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
   return x < y + bn && y < x + an;
@@ -236,6 +337,28 @@ int ktb_vtrace_f32(int dev, const float* log_rhos, const float* rewards, const f
   KTB_GUARD(dev);
   vtrace_kernel<<<(unsigned)((N + 31) / 32), 32, kVtraceSmem, reinterpret_cast<cudaStream_t>(stream)>>>(
       log_rhos, rewards, values, dones, bootstrap, N, T, gamma, lam, rho_bar, c_bar, pg_rho_bar, vs, pg_adv);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
+}
+
+int ktb_nstep_f32(int dev, const float* rewards, const float* values, const float* dones, const float* baseline,
+                  const float* last_values, size_t N, size_t T, int n, float gamma, float* ret, float* td,
+                  uintptr_t stream) {
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(n >= 1 && n <= 32, KTB_ERR_ARG, "ktb_nstep_f32: n = %d must be in [1, 32]", n);
+  KTB_REQUIRE(std::isfinite(gamma), KTB_ERR_ARG, "ktb_nstep_f32: gamma (%g) must be finite", (double)gamma);
+  if (N == 0 || T == 0) return KTB_OK;
+  if ((rc = check_buffers<5>("ktb_nstep_f32", {rewards, values, dones, baseline, last_values, ret, td},
+                             {"rewards", "values", "dones", "baseline", "last_values", "ret", "td"}, N, T)))
+    return rc;
+  KTB_GUARD(dev);
+  const size_t n_tiles = (T + 31) / 32;
+  size_t span = (n_tiles + 65534) / 65535;   // gridDim.y is at most 65535
+  span = span > (size_t)kNstepSpan ? span : (size_t)kNstepSpan;
+  const dim3 grid((unsigned)((N + 31) / 32), (unsigned)((n_tiles + span - 1) / span));
+  nstep_kernel<<<grid, 32, 0, reinterpret_cast<cudaStream_t>(stream)>>>(rewards, values, dones, baseline, last_values,
+                                                                         N, T, n, gamma, span, ret, td);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }

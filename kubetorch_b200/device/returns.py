@@ -3,7 +3,9 @@ current stream (include/ktb200.h):
   gae     ktb_gae_f32: PPO's advantages and λ-returns, bit for bit CleanRL's per-step torch loop
           (tests/policy_gae_cases.py);
   vtrace  ktb_vtrace_f32: IMPALA's V-trace targets and policy-gradient advantages, bit for bit TorchBeast's
-          from_importance_weights made env-major (tests/policy_vtrace_cases.py)."""
+          from_importance_weights made env-major (tests/policy_vtrace_cases.py);
+  nstep   ktb_nstep_f32: Ape-X's, R2D2's and A3C's n-step bootstrapped returns and their TD errors, bit for bit rlax's
+          n_step_bootstrapped_returns at lambda_t = 1 made env-major (tests/policy_nstep_cases.py)."""
 from __future__ import annotations
 
 import math
@@ -120,3 +122,47 @@ def vtrace(log_rhos: torch.Tensor, rewards: torch.Tensor, values: torch.Tensor, 
            bootstrap_value.data_ptr(), shape[0], shape[1], *scalars, vs.data_ptr(), pg_adv.data_ptr(),
            ops._stream(dev, stream))
     return vs, pg_adv
+
+
+def nstep_scalars(n, gamma) -> Tuple[int, float]:
+    """(n, gamma) as ktb_nstep_f32 takes them: n an int (not a bool) in [1, 32], gamma rounded to fp32 as torch rounds
+    a Python scalar that meets an fp32 tensor; ValueError naming the first bad argument: gamma must be a finite number,
+    finite in float32."""
+    if isinstance(n, bool) or not isinstance(n, int) or not 1 <= n <= 32:
+        raise ValueError(f"n must be an int in [1, 32], got {n!r}")
+    check_finite("gamma", gamma)
+    g = _fp32(gamma)
+    if not math.isfinite(g):
+        raise ValueError(f"gamma={gamma!r} must be finite in float32")
+    return n, g
+
+
+def nstep(rewards: torch.Tensor, values: torch.Tensor, dones: torch.Tensor, baseline: torch.Tensor,
+          last_values: torch.Tensor, n, gamma, ret: Optional[torch.Tensor] = None, td: Optional[torch.Tensor] = None,
+          stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(returns, td_errors) of env-major rollouts: the n-step bootstrapped returns G_t = r_t + γ r_{t+1} + … +
+    γ^{n−1} r_{t+n−1} + γ^n values[:, t + n], cut at episode ends and bootstrapped from last_values past the rollout's
+    end, and G_t − baseline[:, t].  rewards, values (the bootstrap value of each state), dones (dones[i, t] = 1 when the
+    episode ended after the action at step t) and baseline (Q(s_t, a_t), or values for A3C) are fp32 [N, T];
+    last_values fp32 [N] = V(s_T).  Every tensor is contiguous and on one CUDA device; inputs may alias one another.
+    ret and td are fresh fp32 [N, T] tensors unless given; given ones must not overlap the inputs or each other.
+    Enqueued on `stream` (default: the current stream of that device)."""
+    if not isinstance(rewards, torch.Tensor) or rewards.dim() != 2:
+        raise ValueError(f"rewards must be a 2-D [N, T] tensor, got "
+                         f"{list(rewards.shape) if isinstance(rewards, torch.Tensor) else type(rewards).__name__}")
+    shape, device = tuple(rewards.shape), rewards.device
+    _check("rewards", rewards, shape, device)
+    _check("values", values, shape, device)
+    _check("dones", dones, shape, device)
+    _check("baseline", baseline, shape, device)
+    _check("last_values", last_values, shape[:1], device)
+    n, g = nstep_scalars(n, gamma)
+    ret = torch.empty(shape, dtype=torch.float32, device=device) if ret is None else ret
+    td = torch.empty(shape, dtype=torch.float32, device=device) if td is None else td
+    _check("ret", ret, shape, device)
+    _check("td", td, shape, device)
+    dev = device.index
+    ops.ensure_init([dev])
+    L.call("ktb_nstep_f32", dev, rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), baseline.data_ptr(),
+           last_values.data_ptr(), shape[0], shape[1], n, g, ret.data_ptr(), td.data_ptr(), ops._stream(dev, stream))
+    return ret, td

@@ -1,6 +1,6 @@
 """Registry of *mapped callables*: user functions whose body is one of the closed set of ops that
 libktb200 executes as sm_90a kernels (identity / scale / affine, their sum-reduced forms, the
-bf16 MLP policy, generalized advantage estimation and V-trace).
+bf16 MLP policy, generalized advantage estimation, V-trace and n-step bootstrapped returns).
 
 Arbitrary Python cannot become a CUDA kernel, so the device route is opt-in by declaration:
 
@@ -25,7 +25,7 @@ from .sampling import _check_seed
 
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
-ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace")
+ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace", "nstep")
 # The options of op="gae": gamma and lam, each required (a finite number or the name of a call argument holding one),
 # and self_check
 GAE_OPTIONS = ("gamma", "lam")
@@ -34,6 +34,10 @@ GAE_OPTIONS = ("gamma", "lam")
 # (no clip).  mapped() stores every default it fills in into MappedSpec.extra.
 VTRACE_OPTIONS = dict(gamma=None, lam=1.0, rho_bar=1.0, c_bar=1.0, pg_rho_bar=1.0)
 VTRACE_ARGUMENTS = ("gamma", "lam")
+# The options of op="nstep" beside self_check, both required (None): n an int constant in [1, 32], gamma a finite number
+# or the name of a call argument holding one (NSTEP_ARGUMENTS)
+NSTEP_OPTIONS = dict(n=None, gamma=None)
+NSTEP_ARGUMENTS = ("gamma",)
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
                "gaussian_evaluate", "deterministic", "critic", "td_target", "dqn_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
@@ -325,13 +329,31 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
     (checked per call); ``rho_bar=``, ``c_bar=`` and ``pg_rho_bar=`` are constants, a number > 0 or None for no clip,
     each 1.0 by default (TorchBeast clamps the traces at 1.0 whatever ``c_bar``: declare ``c_bar=1.0`` for its bits).
     ``self_check=False`` skips the deployment's check of constant options against the body.  Every other option is
-    refused."""
+    refused.
+
+    The "nstep" op is the n-step bootstrapped return of Ape-X, R2D2, Rainbow and A3C: the callable is ``(rewards,
+    values, dones, baseline, last_values, ...)`` with fp32 ``[N, T]`` rewards, values, dones and baseline in the
+    env-major layout of "gae" and fp32 ``[N]`` last_values, V(s_T), all CUDA tensors on the root GPU.  Each rank
+    returns ``(returns, td)`` of its rows, ``x.chunk(WORLD_SIZE)[RANK]``: ``G_t = r_t + γ r_{t+1} + … + γ^{n−1}
+    r_{t+n−1} + γ^n values[:, t + n]`` with ``γ(1 − dones)`` as each step's discount, so the sum is cut at episode
+    ends, and past the rollout's end padded with reward 0, discount 1 and ``last_values``; ``td = G − baseline``.  It
+    is rlax's ``n_step_bootstrapped_returns`` at ``lambda_t = 1`` made env-major, bit for bit as torch computes the
+    padded loop (tests/policy_nstep_cases.py).  ``values[:, t]`` is the bootstrap value of state s_t and ``baseline[:,
+    t]`` what the TD error is taken against: for Ape-X's priorities ``values = q_max`` and ``baseline = q`` of
+    ``output="epsilon_greedy"`` over the rollout's observations, ``.view(N, T)``; for A3C's n-step advantages ``values``
+    from the value head and ``baseline = values``.  ``dones[:, t]`` is the done flag of transition t, so CleanRL-style
+    episode-start flags become ``torch.cat([dones[1:], next_done[None]]).T.contiguous()`` as for "gae".  ``n=`` is a
+    required int constant in [1, 32] and ``gamma=`` a required finite number or the name of a call argument that holds
+    one (checked per call).  ``self_check=False`` skips the deployment's check of a constant γ against the body.  Every
+    other option is refused."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if op == "gae":
         _check_gae_options(alpha, beta, reduce, arg, extra)
     if op == "vtrace":
         _check_vtrace_options(alpha, beta, reduce, arg, extra)
+    if op == "nstep":
+        _check_nstep_options(alpha, beta, reduce, arg, extra)
     beta = 0.0 if beta is _UNSET else beta
     if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
         extra["alpha"] = alpha
@@ -376,8 +398,11 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
         if op == "vtrace" and len(params) < 5:
             raise ValueError(f"a 'vtrace' callable takes (log_rhos, rewards, values, dones, bootstrap_value, ...) "
                              f"positionally, {getattr(fn, '__name__', fn)!r} has {len(params)} parameters")
+        if op == "nstep" and len(params) < 5:
+            raise ValueError(f"a 'nstep' callable takes (rewards, values, dones, baseline, last_values, ...) "
+                             f"positionally, {getattr(fn, '__name__', fn)!r} has {len(params)} parameters")
         for option, names in extra.items():
-            if not (isinstance(names, str) if op in ("gae", "vtrace") else names_arguments(option, names)):
+            if not (isinstance(names, str) if op in ("gae", "vtrace", "nstep") else names_arguments(option, names)):
                 continue
             for name in (names,) if isinstance(names, str) else names:
                 if name not in params:
@@ -430,6 +455,29 @@ def _check_vtrace_options(alpha, beta, reduce, arg, extra) -> None:
                 check_finite(name, extra[name])
         else:
             check_threshold(name, extra[name])
+    if not isinstance(extra.get("self_check", False), bool):
+        raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
+
+
+def _check_nstep_options(alpha, beta, reduce, arg, extra) -> None:
+    """The options of op="nstep", or ValueError naming the first it does not take or the first it lacks; n must be an
+    int constant in [1, 32] and a constant gamma a finite number (extra keeps them)."""
+    refused = dict(alpha=alpha is not _UNSET, beta=beta is not _UNSET, reduce=reduce is not None, arg=arg is not None)
+    refused.update((k, True) for k in extra if k not in (*NSTEP_OPTIONS, "self_check"))
+    for name, given in refused.items():
+        if given:
+            raise ValueError(f"{name}= is not an option of the 'nstep' op, which takes n=, gamma= and self_check=: its "
+                             f"callable is (rewards, values, dones, baseline, last_values) and it returns (returns, td)")
+    if "n" not in extra:
+        raise ValueError("n= is required with the 'nstep' op: an int constant in [1, 32]")
+    n = extra["n"]
+    if isinstance(n, bool) or not isinstance(n, int) or not 1 <= n <= 32:
+        raise ValueError(f"n must be an int constant in [1, 32] (not the name of a call argument), got {n!r}")
+    if "gamma" not in extra:
+        raise ValueError("gamma= is required with the 'nstep' op: a finite number or the name of a call argument that "
+                         "holds one")
+    if not isinstance(extra["gamma"], str):
+        check_finite("gamma", extra["gamma"])
     if not isinstance(extra.get("self_check", False), bool):
         raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
 

@@ -40,6 +40,8 @@ One controller process drives N local H100s.  For a @kt.mapped callable a remote
         ktb_gae_f32: one launch on the root GPU over every selected rank's rows.
     "vtrace"
         ktb_vtrace_f32: the same, one launch on the root GPU.
+    "nstep"
+        ktb_nstep_f32: the same, one launch on the root GPU.
 
 There is NO CPU fallback here: a missing library or GPU raises.
 """
@@ -54,8 +56,8 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, TD_OPTIONS, VTRACE_ARGUMENTS,
-                      VTRACE_OPTIONS, check_finite, mapped_spec, names_arguments)
+from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, NSTEP_ARGUMENTS, TD_OPTIONS,
+                      VTRACE_ARGUMENTS, VTRACE_OPTIONS, check_finite, mapped_spec, names_arguments)
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -203,6 +205,8 @@ class B200Supervisor:
                 self._self_check_gae(spec, method)
             if spec.op == "vtrace" and spec.extra.get("self_check") is not False:
                 self._self_check_vtrace(spec, method)
+            if spec.op == "nstep" and spec.extra.get("self_check") is not False:
+                self._self_check_nstep(spec, method)
             if spec.op not in ELEMENTWISE_OPS or spec.extra.get("self_check") is False:
                 continue
             if not (isinstance(spec.alpha, (int, float)) and isinstance(spec.beta, (int, float))):
@@ -357,6 +361,59 @@ class B200Supervisor:
                 f"lambda_) and thresholds, clamping the traces at c_bar (TorchBeast clamps them at 1.0: declare "
                 f"c_bar=1.0), and reads dones[:, t] as the done flag of transition t, TorchBeast's batch['done'][1:] "
                 f"(not a flag that observation t starts an episode)")
+
+    def _self_check_nstep(self, spec, method):
+        """An "nstep" callable with a constant gamma: its body on CPU, rank by rank, against the kernel on seeded
+        (4·world + 3, n + 8) rollouts with some done = 1, so that both full windows and the padded end are exercised;
+        refuse the deployment on any bit difference (the op has no exp, so the CPU's bits are the GPU's).  This catches
+        a body that reads dones as episode starts, a γ or n other than declared, and one that bootstraps 0 past the
+        rollout's end instead of V(s_T)."""
+        import inspect
+
+        import torch
+
+        if any(isinstance(spec.extra[k], str) for k in NSTEP_ARGUMENTS) or \
+                len(inspect.signature(method).parameters) != 5:
+            return   # gamma is a call argument: nothing constant to check at deploy time
+        world, dev0 = self.world_size, self.devices[0]
+        gen = torch.Generator().manual_seed(1234)
+        n, t = 4 * world + 3, spec.extra["n"] + 8
+        rewards, values = torch.randn(n, t, generator=gen), torch.randn(n, t, generator=gen)
+        dones = (torch.rand(n, t, generator=gen) < 0.25).float()
+        dones[::3, t // 2] = 1.0
+        baseline, last_values = torch.randn(n, t, generator=gen), torch.randn(n, generator=gen)
+        args = (rewards, values, dones, baseline, last_values)
+        saved = {k: os.environ.get(k) for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK")}
+        want = []
+        try:
+            for r in range(world):
+                os.environ.update({"RANK": str(r), "WORLD_SIZE": str(world), "LOCAL_RANK": str(r)})
+                want.append(method(*(a.clone() for a in args)))
+        except Exception:  # noqa: BLE001 - a body that cannot run here (needs a GPU arg, a group, ...) is skipped
+            return
+        finally:
+            for k, v in saved.items():
+                if v is None:
+                    os.environ.pop(k, None)
+                else:
+                    os.environ[k] = v
+        got = self._run_mapped(spec, method, [a.to(f"cuda:{dev0}") for a in args], {}, list(range(world)))
+        self.ops.synchronize(dev0)
+
+        def same(g, w):
+            return isinstance(w, torch.Tensor) and w.dtype == torch.float32 and tuple(g.shape) == tuple(w.shape) \
+                and torch.equal(g.cpu().view(torch.int32), w.cpu().contiguous().view(torch.int32))
+
+        if not all(isinstance(w, (tuple, list)) and len(w) == 2 and all(same(*p) for p in zip(g, w))
+                   for g, w in zip(got, want)):
+            raise ValueError(
+                f"@kt.mapped self-check failed for '{getattr(method, '__name__', method)}': the 'nstep' op (n="
+                f"{spec.extra['n']}, gamma={spec.extra['gamma']}) does not reproduce the Python body's (returns, td) "
+                f"bit for bit on seeded rollouts; refusing to deploy.  The op sums n={spec.extra['n']} discounted "
+                f"rewards with gamma={spec.extra['gamma']}, reads dones[:, t] as the done flag of transition t (not a "
+                f"flag that observation t starts an episode: CleanRL's dones become torch.cat([dones[1:], "
+                f"next_done[None]]).T.contiguous()), and past the rollout's end bootstraps from last_values, V(s_T), "
+                f"not from 0")
 
     # ---- small-call lane (the local CUDA-stream scheduler for launch-bound calls) ----------------------------
     SMALL_CALL_BYTES = 4 << 20
@@ -532,6 +589,8 @@ class B200Supervisor:
             return self._call_gae(spec, bound, ranks)
         if spec.op == "vtrace":
             return self._call_vtrace(spec, bound, ranks)
+        if spec.op == "nstep":
+            return self._call_nstep(spec, bound, ranks)
         if spec.op not in ELEMENTWISE_OPS:
             raise TypeError(f"unsupported mapped op '{spec.op}'")
         if not isinstance(x, torch.Tensor):
@@ -715,7 +774,8 @@ class B200Supervisor:
         few flops per byte, and spreading them over the ranks' GPUs would move every byte over NVLink twice."""
         from ..device import returns
 
-        return self._call_returns(spec, bound, ranks, ("rewards", "values", "dones", "last_values"), returns.gae)
+        return self._call_returns(spec, bound, ranks, ("rewards", "values", "dones", "last_values"), returns.gae,
+                                  GAE_OPTIONS)
 
     def _call_vtrace(self, spec, bound, ranks=None):
         """(vs, pg_advantages) per selected rank: one ktb_vtrace_f32 launch on the root per run of consecutive selected
@@ -724,12 +784,22 @@ class B200Supervisor:
 
         bars = {k: spec.extra[k] for k in ("rho_bar", "c_bar", "pg_rho_bar")}
         return self._call_returns(spec, bound, ranks, ("log_rhos", "rewards", "values", "dones", "bootstrap_value"),
-                                  lambda *xs: returns.vtrace(*xs, **bars))
+                                  lambda *xs: returns.vtrace(*xs, **bars), VTRACE_ARGUMENTS)
 
-    def _call_returns(self, spec, bound, ranks, names, launch):
-        """The first len(names) call arguments, checked to be CUDA tensors on the root GPU, and gamma and lam (constants
-        or call arguments) checked to be finite: launch(*rows, gamma, lam) over the rows of every run of consecutive
-        selected ranks, its pair of [rows, T] outputs split into one pair of views per rank."""
+    def _call_nstep(self, spec, bound, ranks=None):
+        """(returns, td) per selected rank: one ktb_nstep_f32 launch on the root per run of consecutive selected ranks,
+        as _call_gae."""
+        from ..device import returns
+
+        n = spec.extra["n"]
+        return self._call_returns(spec, bound, ranks, ("rewards", "values", "dones", "baseline", "last_values"),
+                                  lambda *xs: returns.nstep(*xs[:5], n, *xs[5:]), NSTEP_ARGUMENTS)
+
+    def _call_returns(self, spec, bound, ranks, names, launch, arguments):
+        """The first len(names) call arguments, checked to be CUDA tensors on the root GPU, and the options named in
+        `arguments` (constants or call arguments, such as gamma and lam) checked to be finite: launch(*rows,
+        *those options) over the rows of every run of consecutive selected ranks, its pair of [rows, T] outputs split
+        into one pair of views per rank."""
         import torch
 
         tensors = [bound[n] for n in list(bound)[:len(names)]]
@@ -739,9 +809,9 @@ class B200Supervisor:
                 where = t.device if isinstance(t, torch.Tensor) else type(t).__name__
                 raise ValueError(f"the '{spec.op}' op takes CUDA tensors on the root GPU cuda:{root}: {name} is on "
                                  f"{where} (host tensors are not staged for this op)")
-        gamma, lam = (bound[v] if isinstance(v, str) else v for v in (spec.extra["gamma"], spec.extra["lam"]))
-        check_finite("gamma", gamma)
-        check_finite("lam", lam)
+        scalars = [bound[v] if isinstance(v, str) else v for v in (spec.extra[k] for k in arguments)]
+        for name, v in zip(arguments, scalars):
+            check_finite(name, v)
         rewards = tensors[names.index("rewards")]
         if rewards.dim() != 2:
             raise ValueError(f"rewards must be a 2-D [N, T] tensor, got {list(rewards.shape)}")
@@ -754,7 +824,7 @@ class B200Supervisor:
             while j + 1 < len(ranks) and ranks[j + 1] == ranks[j] + 1:
                 j += 1
             b, e = bounds[i][0], bounds[j][1]
-            first, second = launch(*(x[b:e] for x in tensors), gamma, lam)
+            first, second = launch(*(x[b:e] for x in tensors), *scalars)
             out += [(first[rb - b:re - b], second[rb - b:re - b]) for rb, re in bounds[i:j + 1]]
             i = j + 1
         return out
