@@ -1148,6 +1148,42 @@ int ktb_nstep_f32(int dev, const float* rewards, const float* values, const floa
                   const float* last_values, size_t N, size_t T, int n, float gamma, float* ret, float* td,
                   uintptr_t stream);
 
+/* ---- Retrace(λ) (the off-policy Q-value target of ACER, Reactor, MPO and Q(λ)) --------------------------------------
+ *
+ * Env-major fp32 [N, T] as for ktb_gae_f32: log_rhos[i, t] = log π(a_t|s_t) − log μ(a_t|s_t), the target policy's
+ * log-probability of the taken action less the behaviour policy's; q[i, t] = Q_target(s_t, a_t); values[i, t] =
+ * E_{a~π} Q_target(s_t, a) (max_a Q_target(s_t, a) for a greedy π); dones[i, t] the done flag of transition t;
+ * baseline[i, t] what the TD error is taken against, Q_online(s_t, a_t) (it may be q itself); bootstrap[i] =
+ * E_π Q_target(s_T, ·).  Columns 0 of log_rhos, q and values are never read.
+ *
+ * Per row, as fp32 operations each rounded to nearest even, with no FMA contraction, starting from acc = +0, nv =
+ * bootstrap[i], nq = −0 and nc = −0, for t = T - 1 down to 0 (lr, r, q, v, d, b = log_rhos, rewards, q, values, dones,
+ * baseline at [i, t]):
+ *     disc     = gamma * (1 - d)
+ *     acc      = r + disc * ((nv - nc * nq) + nc * acc)
+ *     ret[i, t] = acc
+ *     td[i, t]  = acc - b
+ *     nc       = lam * (expf(lr) > 1 ? 1 : expf(lr))
+ *     nv       = v
+ *     nq       = q
+ * which is bit for bit rlax's retrace_continuous made env-major (tests/policy_retrace_cases.py) when gamma and lam are
+ * the fp32 roundings of γ and λ, as torch rounds a Python scalar that meets an fp32 tensor, and expf is CUDA's expf
+ * without fast math (torch's exp of an fp32 CUDA tensor).  The −0 start values make the general step at t = T − 1 the
+ * body's first step, r + disc · bootstrap, bit for bit, a −0 bootstrap included; +0 would give +0 there.  The clip is a
+ * compare, so a NaN ρ stays NaN, as under torch.clamp.  A done multiplies by 1 - d = 0, it does not select: an infinite
+ * value after an episode boundary makes the targets before it NaN, as in the torch loop.  log_rhos = 0 is Harutyunyan's
+ * Q(λ) (c = λ); log_rhos = −inf on the actions a greedy π does not take is Watkins' Q(λ) (c = 0 cuts the trace there).
+ * Inputs may alias one another.
+ *
+ * Checks, in this order: an unregistered dev is KTB_ERR_STATE; a non-finite gamma or lam is KTB_ERR_ARG; N·T == 0 is
+ * KTB_OK with nothing enqueued (the pointers may then be NULL); otherwise a NULL or not 4-byte-aligned pointer, N·T·4
+ * past SIZE_MAX, a ret or td range that overlaps an input range or the other output, or more than 32·(2³¹ − 1) rows is
+ * KTB_ERR_ARG.  The kernel reads each input element once and writes ret[0, N·T) and td[0, N·T) once each: 32·N·T + 4·N
+ * bytes. */
+int ktb_retrace_f32(int dev, const float* log_rhos, const float* rewards, const float* q, const float* values,
+                    const float* dones, const float* baseline, const float* bootstrap, size_t N, size_t T, float gamma,
+                    float lam, float* ret, float* td, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,7 +2,8 @@
 // evaluated exactly as written there:
 //   ktb_gae_f32     generalized advantage estimation: PPO's advantages and λ-returns;
 //   ktb_vtrace_f32  V-trace (IMPALA): off-policy value targets and policy-gradient advantages;
-// and the n-step bootstrapped returns that are no recurrence along the row (nstep_kernel, after the first two):
+//   ktb_retrace_f32 Retrace(λ) (ACER, Reactor, MPO, Q(λ)): off-policy Q-value targets and their TD errors;
+// and the n-step bootstrapped returns that are no recurrence along the row (nstep_kernel, after the first three):
 //   ktb_nstep_f32   Ape-X's, R2D2's and A3C's n-step targets and their TD errors.
 //
 // HBM-bound: (4·inputs + 8)·N·T + 4·N bytes, a handful of flops per element.  The recurrence runs along a row, but the
@@ -19,6 +20,7 @@
 // its rows, so that small T still moves whole segments.  The tile walk is scan_rows(); each op is a per-step functor.
 #include "ktb_common.cuh"
 
+#include <atomic>
 #include <cmath>
 
 namespace ktb {
@@ -31,6 +33,13 @@ constexpr int kGaeStages = 3;      // 3 x 12.4 KiB of shared tiles per warp (3 p
 // (DESIGN.md §4b).
 constexpr int kVtraceStages = 2;
 constexpr int kVtraceSmem = kVtraceStages * 4 * 32 * kPad * 4;   // 33 792 B: under 48 KiB, so no opt-in attribute
+// 2 x 24.8 KiB per warp (6 planes), 4 blocks per SM: past 48 KiB, so the launch opts in to the larger dynamic size.
+// Five planes under 48 KiB (42 240 B, 5 blocks per SM), td formed at store time from a coalesced read of baseline,
+// measured 3.5 % and 8.8 % slower at (16384, 128) and (4096, 256) and at most 3 % faster at the latency-bound shapes of
+// tools/bench_retrace.py; the same with the tile's baseline read into registers before the scan was 6-21 % slower at
+// every shape (DESIGN.md §4b).
+constexpr int kRetraceStages = 2;
+constexpr int kRetraceSmem = kRetraceStages * 6 * 32 * kPad * 4;   // 50 688 B
 
 template <int P>
 using Tile = float[P][32][kPad];   // [input plane][row][step]
@@ -149,6 +158,28 @@ struct VtraceStep {
   }
 };
 
+// Retrace(λ) over planes [log_rhos → ret, rewards → td, q, values, dones, baseline].  The step carries the next step's
+// value, Q and trace (nv, nq, nc); starting from nq = nc = −0 makes the general step reproduce the first one, r + disc ·
+// bootstrap, bit for bit (−0 included).  The clip is a compare, so that a NaN ρ stays NaN as under torch.clamp.
+struct RetraceStep {
+  float gamma, lam, acc, nv, nq, nc;
+  __device__ __forceinline__ void start(float bootstrap) {
+    acc = 0.0f;
+    nv = bootstrap;
+    nq = nc = -0.0f;
+  }
+  __device__ __forceinline__ void operator()(Tile<6>& s, int j, int c) {
+    const float rho = expf(s[0][j][c]);
+    const float disc = __fmul_rn(gamma, __fsub_rn(1.0f, s[4][j][c]));
+    acc = __fadd_rn(s[1][j][c], __fmul_rn(disc, __fadd_rn(__fsub_rn(nv, __fmul_rn(nc, nq)), __fmul_rn(nc, acc))));
+    s[0][j][c] = acc;
+    s[1][j][c] = __fsub_rn(acc, s[5][j][c]);
+    nc = __fmul_rn(lam, rho > 1.0f ? 1.0f : rho);
+    nv = s[3][j][c];
+    nq = s[2][j][c];
+  }
+};
+
 // One warp per block and per 32 rows.
 __global__ void __launch_bounds__(32)
     gae_kernel(const float* __restrict__ rewards, const float* __restrict__ values, const float* __restrict__ dones,
@@ -171,7 +202,18 @@ __global__ void __launch_bounds__(32)
   scan_rows<4, kVtraceStages>(reinterpret_cast<Tile<4>*>(smem), in, bootstrap, N, T, vs, pg_adv, step);
 }
 
-// n-step bootstrapped returns.  Unlike the two recurrences above, output (i, t) depends only on the window of steps
+__global__ void __launch_bounds__(32)
+    retrace_kernel(const float* __restrict__ log_rhos, const float* __restrict__ rewards, const float* __restrict__ q,
+                   const float* __restrict__ values, const float* __restrict__ dones,
+                   const float* __restrict__ baseline, const float* __restrict__ bootstrap, size_t N, size_t T,
+                   float gamma, float lam, float* __restrict__ ret, float* __restrict__ td) {
+  extern __shared__ __align__(16) float smem[];
+  const float* const in[6] = {log_rhos, rewards, q, values, dones, baseline};
+  RetraceStep step{gamma, lam};
+  scan_rows<6, kRetraceStages>(reinterpret_cast<Tile<6>*>(smem), in, bootstrap, N, T, ret, td, step);
+}
+
+// n-step bootstrapped returns.  Unlike the recurrences above, output (i, t) depends only on the window of steps
 // [t, t + n] of its row, so the grid splits T as well as N: block (x, y) is one warp over rows [32x, 32x + 32) and the
 // span of kNstepSpan consecutive 32-step tiles starting at tile y·span.  The warp walks its span forwards with a ring of
 // two tiles per row in shared memory, the current one and the next (the windows' halo), so a tile copied as the halo is
@@ -337,6 +379,30 @@ int ktb_vtrace_f32(int dev, const float* log_rhos, const float* rewards, const f
   KTB_GUARD(dev);
   vtrace_kernel<<<(unsigned)((N + 31) / 32), 32, kVtraceSmem, reinterpret_cast<cudaStream_t>(stream)>>>(
       log_rhos, rewards, values, dones, bootstrap, N, T, gamma, lam, rho_bar, c_bar, pg_rho_bar, vs, pg_adv);
+  KTB_CK(cudaGetLastError());
+  return KTB_OK;
+}
+
+int ktb_retrace_f32(int dev, const float* log_rhos, const float* rewards, const float* q, const float* values,
+                    const float* dones, const float* baseline, const float* bootstrap, size_t N, size_t T, float gamma,
+                    float lam, float* ret, float* td, uintptr_t stream) {
+  static std::atomic<unsigned> smem_set{0};   // the devices whose retrace_kernel has opted in to kRetraceSmem
+  int rc = require_device(dev);
+  if (rc) return rc;
+  KTB_REQUIRE(std::isfinite(gamma) && std::isfinite(lam), KTB_ERR_ARG,
+              "ktb_retrace_f32: gamma (%g) and lam (%g) must be finite", (double)gamma, (double)lam);
+  if (N == 0 || T == 0) return KTB_OK;
+  if ((rc = check_buffers<7>("ktb_retrace_f32", {log_rhos, rewards, q, values, dones, baseline, bootstrap, ret, td},
+                             {"log_rhos", "rewards", "q", "values", "dones", "baseline", "bootstrap", "ret", "td"}, N,
+                             T)))
+    return rc;
+  KTB_GUARD(dev);
+  if (!(smem_set.load(std::memory_order_acquire) & (1u << dev))) {   // dev < kMaxDevices: require_device checked it
+    KTB_CK(cudaFuncSetAttribute(retrace_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRetraceSmem));
+    smem_set.fetch_or(1u << dev, std::memory_order_release);
+  }
+  retrace_kernel<<<(unsigned)((N + 31) / 32), 32, kRetraceSmem, reinterpret_cast<cudaStream_t>(stream)>>>(
+      log_rhos, rewards, q, values, dones, baseline, bootstrap, N, T, gamma, lam, ret, td);
   KTB_CK(cudaGetLastError());
   return KTB_OK;
 }

@@ -5,7 +5,9 @@ current stream (include/ktb200.h):
   vtrace  ktb_vtrace_f32: IMPALA's V-trace targets and policy-gradient advantages, bit for bit TorchBeast's
           from_importance_weights made env-major (tests/policy_vtrace_cases.py);
   nstep   ktb_nstep_f32: Ape-X's, R2D2's and A3C's n-step bootstrapped returns and their TD errors, bit for bit rlax's
-          n_step_bootstrapped_returns at lambda_t = 1 made env-major (tests/policy_nstep_cases.py)."""
+          n_step_bootstrapped_returns at lambda_t = 1 made env-major (tests/policy_nstep_cases.py);
+  retrace ktb_retrace_f32: Retrace(λ), the off-policy Q-value targets of ACER, Reactor, MPO and Q(λ), and their TD
+          errors, bit for bit rlax's retrace_continuous made env-major (tests/policy_retrace_cases.py)."""
 from __future__ import annotations
 
 import math
@@ -165,4 +167,51 @@ def nstep(rewards: torch.Tensor, values: torch.Tensor, dones: torch.Tensor, base
     ops.ensure_init([dev])
     L.call("ktb_nstep_f32", dev, rewards.data_ptr(), values.data_ptr(), dones.data_ptr(), baseline.data_ptr(),
            last_values.data_ptr(), shape[0], shape[1], n, g, ret.data_ptr(), td.data_ptr(), ops._stream(dev, stream))
+    return ret, td
+
+
+def retrace_scalars(gamma, lam) -> Tuple[float, float]:
+    """(gamma, lam) as the fp32 values ktb_retrace_f32 takes, each rounded as torch rounds a Python scalar that meets an
+    fp32 tensor; ValueError naming the first bad argument: each must be a finite number, finite in float32."""
+    out = []
+    for name, v in (("gamma", gamma), ("lam", lam)):
+        out.append(_fp32(check_finite(name, v)))
+        if not math.isfinite(out[-1]):
+            raise ValueError(f"{name}={v!r} must be finite in float32")
+    return tuple(out)
+
+
+def retrace(log_rhos: torch.Tensor, rewards: torch.Tensor, q: torch.Tensor, values: torch.Tensor, dones: torch.Tensor,
+            baseline: torch.Tensor, bootstrap_value: torch.Tensor, gamma, lam, ret: Optional[torch.Tensor] = None,
+            td: Optional[torch.Tensor] = None,
+            stream: Optional[torch.cuda.Stream] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(returns, td_errors) of env-major rollouts under Retrace(λ): G_t = r_t + γ(1 − d_t)·(values[:, t + 1] −
+    c_{t+1}·q[:, t + 1] + c_{t+1}·G_{t+1}) with traces c = λ·min(1, exp(log_rhos)), bootstrapped from bootstrap_value at
+    the rollout's end, and G_t − baseline[:, t].  log_rhos (target less behaviour log-probabilities of the taken
+    actions), rewards, q (Q_target(s_t, a_t)), values (E_π Q_target(s_t, ·)), dones (dones[i, t] = 1 when the episode
+    ended after the action at step t) and baseline (Q_online(s_t, a_t), or q itself) are fp32 [N, T]; bootstrap_value
+    fp32 [N] = E_π Q_target(s_T, ·).  Columns 0 of log_rhos, q and values are not read.  Every tensor is contiguous and
+    on one CUDA device; inputs may alias one another.  ret and td are fresh fp32 [N, T] tensors unless given; given ones
+    must not overlap the inputs or each other.  Enqueued on `stream` (default: the current stream of that device)."""
+    if not isinstance(rewards, torch.Tensor) or rewards.dim() != 2:
+        raise ValueError(f"rewards must be a 2-D [N, T] tensor, got "
+                         f"{list(rewards.shape) if isinstance(rewards, torch.Tensor) else type(rewards).__name__}")
+    shape, device = tuple(rewards.shape), rewards.device
+    _check("rewards", rewards, shape, device)
+    _check("log_rhos", log_rhos, shape, device)
+    _check("q", q, shape, device)
+    _check("values", values, shape, device)
+    _check("dones", dones, shape, device)
+    _check("baseline", baseline, shape, device)
+    _check("bootstrap_value", bootstrap_value, shape[:1], device)
+    g, lm = retrace_scalars(gamma, lam)
+    ret = torch.empty(shape, dtype=torch.float32, device=device) if ret is None else ret
+    td = torch.empty(shape, dtype=torch.float32, device=device) if td is None else td
+    _check("ret", ret, shape, device)
+    _check("td", td, shape, device)
+    dev = device.index
+    ops.ensure_init([dev])
+    L.call("ktb_retrace_f32", dev, log_rhos.data_ptr(), rewards.data_ptr(), q.data_ptr(), values.data_ptr(),
+           dones.data_ptr(), baseline.data_ptr(), bootstrap_value.data_ptr(), shape[0], shape[1], g, lm, ret.data_ptr(),
+           td.data_ptr(), ops._stream(dev, stream))
     return ret, td

@@ -25,7 +25,7 @@ from .sampling import _check_seed
 
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
-ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace", "nstep")
+ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace", "nstep", "retrace")
 # The options of op="gae": gamma and lam, each required (a finite number or the name of a call argument holding one),
 # and self_check
 GAE_OPTIONS = ("gamma", "lam")
@@ -38,6 +38,9 @@ VTRACE_ARGUMENTS = ("gamma", "lam")
 # or the name of a call argument holding one (NSTEP_ARGUMENTS)
 NSTEP_OPTIONS = dict(n=None, gamma=None)
 NSTEP_ARGUMENTS = ("gamma",)
+# The options of op="retrace": gamma and lam, each required (a finite number or the name of a call argument holding
+# one), and self_check
+RETRACE_OPTIONS = ("gamma", "lam")
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
                "gaussian_evaluate", "deterministic", "critic", "td_target", "dqn_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
@@ -345,7 +348,32 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
     episode-start flags become ``torch.cat([dones[1:], next_done[None]]).T.contiguous()`` as for "gae".  ``n=`` is a
     required int constant in [1, 32] and ``gamma=`` a required finite number or the name of a call argument that holds
     one (checked per call).  ``self_check=False`` skips the deployment's check of a constant γ against the body.  Every
-    other option is refused."""
+    other option is refused.
+
+    The "retrace" op is Retrace(λ) (Munos et al. 2016), the off-policy Q-value target of ACER, Reactor, MPO and Q(λ)
+    agents: the callable is ``(log_rhos, rewards, q, values, dones, baseline, bootstrap_value, ...)`` with fp32 ``[N,
+    T]`` log_rhos, rewards, q, values, dones and baseline in the env-major layout of "gae" and fp32 ``[N]``
+    bootstrap_value, all CUDA tensors on the root GPU.  Each rank returns ``(returns, td)`` of its rows,
+    ``x.chunk(WORLD_SIZE)[RANK]``: from ``g = r[:, T-1] + discounts[:, T-1] * bootstrap_value`` backwards, ``g = r[:, t]
+    + discounts[:, t] * (values[:, t+1] - c[:, t+1] * q[:, t+1] + c[:, t+1] * g)`` with ``discounts = gamma * (1 -
+    dones)`` and traces ``c = clamp(exp(log_rhos), max=1) * lam``, and ``td = returns - baseline``: rlax's
+    ``retrace_continuous`` made env-major, bit for bit as torch computes it on the GPU (tests/policy_retrace_cases.py).
+    ``log_rhos[:, t]`` is ``log π(a_t|s_t) − log μ(a_t|s_t)`` of the taken action: for stochastic policies ``(target_lp
+    - behaviour_lp).view(N, T)`` with ``behaviour_lp`` from ``output="sample"`` (or ``"gaussian"``) at rollout and
+    ``target_lp`` from ``output="evaluate"`` (or ``"gaussian_evaluate"``) under the target weights; for Watkins' Q(λ)
+    over ε-greedy data, 0 where the taken action is the target network's greedy one and ``-inf`` elsewhere (the trace
+    is cut there), and for Harutyunyan's Q(λ) 0 everywhere.  ``q`` is ``Q_target(s_t, a_t)`` and ``values`` is
+    ``E_π Q_target(s_t, ·)``: for a greedy target policy, ``q_max`` of ``output="epsilon_greedy"`` at ``epsilon=0.0``
+    on the target network over the rollout's N·(T + 1) observations, ``.view(N, T + 1)``, gives ``values = q_max[:,
+    :T]`` and ``bootstrap_value = q_max[:, T]``; under Watkins' log-ratios ``q = values`` is exact, because ``q`` only
+    enters multiplied by the trace, which is 0 wherever the taken action is not the greedy one.  ``baseline`` is what
+    the TD error is taken against, ``Q_online(s_t, a_t)`` (rlax's ``q_tm1``: ``q`` of the behaviour's
+    ``output="epsilon_greedy"`` on the online network), and may be ``q`` itself.  Columns 0 of log_rhos, q and values
+    are never read.  ``dones[:, t]`` is the done flag of transition t; from time-major ``[T, N]`` buffers pass
+    ``x.T.contiguous()``, and CleanRL-style episode-start flags become ``torch.cat([dones[1:],
+    next_done[None]]).T.contiguous()`` as for "gae".  ``gamma=`` and ``lam=`` are required, each a finite number or the
+    name of a call argument that holds one (checked per call); ``self_check=False`` skips the deployment's check of a
+    constant γ and λ against the body.  Every other option is refused."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if op == "gae":
@@ -354,6 +382,8 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
         _check_vtrace_options(alpha, beta, reduce, arg, extra)
     if op == "nstep":
         _check_nstep_options(alpha, beta, reduce, arg, extra)
+    if op == "retrace":
+        _check_retrace_options(alpha, beta, reduce, arg, extra)
     beta = 0.0 if beta is _UNSET else beta
     if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
         extra["alpha"] = alpha
@@ -401,8 +431,13 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
         if op == "nstep" and len(params) < 5:
             raise ValueError(f"a 'nstep' callable takes (rewards, values, dones, baseline, last_values, ...) "
                              f"positionally, {getattr(fn, '__name__', fn)!r} has {len(params)} parameters")
+        if op == "retrace" and len(params) < 7:
+            raise ValueError(f"a 'retrace' callable takes (log_rhos, rewards, q, values, dones, baseline, "
+                             f"bootstrap_value, ...) positionally, {getattr(fn, '__name__', fn)!r} has {len(params)} "
+                             f"parameters")
         for option, names in extra.items():
-            if not (isinstance(names, str) if op in ("gae", "vtrace", "nstep") else names_arguments(option, names)):
+            if not (isinstance(names, str) if op in ("gae", "vtrace", "nstep", "retrace")
+                    else names_arguments(option, names)):
                 continue
             for name in (names,) if isinstance(names, str) else names:
                 if name not in params:
@@ -478,6 +513,26 @@ def _check_nstep_options(alpha, beta, reduce, arg, extra) -> None:
                          "holds one")
     if not isinstance(extra["gamma"], str):
         check_finite("gamma", extra["gamma"])
+    if not isinstance(extra.get("self_check", False), bool):
+        raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
+
+
+def _check_retrace_options(alpha, beta, reduce, arg, extra) -> None:
+    """The options of op="retrace", or ValueError naming the first it does not take or the first it lacks; a constant
+    gamma or lam must be a finite number (extra keeps it)."""
+    refused = dict(alpha=alpha is not _UNSET, beta=beta is not _UNSET, reduce=reduce is not None, arg=arg is not None)
+    refused.update((k, True) for k in extra if k not in RETRACE_OPTIONS + ("self_check",))
+    for name, given in refused.items():
+        if given:
+            raise ValueError(f"{name}= is not an option of the 'retrace' op, which takes gamma=, lam= and self_check=: "
+                             f"its callable is (log_rhos, rewards, q, values, dones, baseline, bootstrap_value) and it "
+                             f"returns (returns, td)")
+    for name in RETRACE_OPTIONS:
+        if name not in extra:
+            raise ValueError(f"{name}= is required with the 'retrace' op: a finite number or the name of a call "
+                             f"argument that holds one")
+        if not isinstance(extra[name], str):
+            check_finite(name, extra[name])
     if not isinstance(extra.get("self_check", False), bool):
         raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
 

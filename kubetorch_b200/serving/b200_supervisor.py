@@ -42,6 +42,8 @@ One controller process drives N local H100s.  For a @kt.mapped callable a remote
         ktb_vtrace_f32: the same, one launch on the root GPU.
     "nstep"
         ktb_nstep_f32: the same, one launch on the root GPU.
+    "retrace"
+        ktb_retrace_f32: the same, one launch on the root GPU.
 
 There is NO CPU fallback here: a missing library or GPU raises.
 """
@@ -56,8 +58,8 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, NSTEP_ARGUMENTS, TD_OPTIONS,
-                      VTRACE_ARGUMENTS, VTRACE_OPTIONS, check_finite, mapped_spec, names_arguments)
+from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, NSTEP_ARGUMENTS, RETRACE_OPTIONS,
+                      TD_OPTIONS, VTRACE_ARGUMENTS, VTRACE_OPTIONS, check_finite, mapped_spec, names_arguments)
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -207,6 +209,8 @@ class B200Supervisor:
                 self._self_check_vtrace(spec, method)
             if spec.op == "nstep" and spec.extra.get("self_check") is not False:
                 self._self_check_nstep(spec, method)
+            if spec.op == "retrace" and spec.extra.get("self_check") is not False:
+                self._self_check_retrace(spec, method)
             if spec.op not in ELEMENTWISE_OPS or spec.extra.get("self_check") is False:
                 continue
             if not (isinstance(spec.alpha, (int, float)) and isinstance(spec.beta, (int, float))):
@@ -415,6 +419,63 @@ class B200Supervisor:
                 f"next_done[None]]).T.contiguous()), and past the rollout's end bootstraps from last_values, V(s_T), "
                 f"not from 0")
 
+    def _self_check_retrace(self, spec, method):
+        """A "retrace" callable with a constant gamma and lam: its body on the root GPU, rank by rank, against the
+        kernel on seeded (4·world + 3, 9) rollouts whose log-ratios fall on both sides of 0, so that the min(1, ρ) clip
+        binds at some steps and not at others, with some done = 1; refuse the deployment on any bit difference.  The
+        body runs on the GPU because ρ = exp(log_rhos) is CUDA's expf there, which torch's CPU exp does not reproduce.
+        This catches a body that reads dones as episode starts, a γ or λ other than declared, unclipped traces λ·ρ, and
+        one that reads the current step's values where the target reads the next step's."""
+        import inspect
+
+        import torch
+
+        if any(isinstance(spec.extra[k], str) for k in RETRACE_OPTIONS) or \
+                len(inspect.signature(method).parameters) != 7:
+            return   # gamma or lam is a call argument: nothing constant to check at deploy time
+        world, dev0 = self.world_size, self.devices[0]
+        gen = torch.Generator().manual_seed(1234)
+        n, t = 4 * world + 3, 9
+        log_rhos = torch.rand(n, t, generator=gen) * 4.6 - 2.3   # ρ from 0.1 to 10: the clip at 1 binds about half
+        rewards, q, values, baseline = (torch.randn(n, t, generator=gen) for _ in range(4))
+        dones = (torch.rand(n, t, generator=gen) < 0.25).float()
+        dones[::3, t // 2] = 1.0
+        bootstrap = torch.randn(n, generator=gen)
+        args = [a.to(f"cuda:{dev0}") for a in (log_rhos, rewards, q, values, dones, baseline, bootstrap)]
+        saved = {k: os.environ.get(k) for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK")}
+        want = []
+        try:
+            with torch.cuda.device(dev0):
+                for r in range(world):
+                    os.environ.update({"RANK": str(r), "WORLD_SIZE": str(world), "LOCAL_RANK": str(r)})
+                    want.append(method(*(a.clone() for a in args)))
+        except Exception:  # noqa: BLE001 - a body that cannot run here (needs an argument, a group, ...) is skipped
+            return
+        finally:
+            for k, v in saved.items():
+                if v is None:
+                    os.environ.pop(k, None)
+                else:
+                    os.environ[k] = v
+        got = self._run_mapped(spec, method, args, {}, list(range(world)))
+        self.ops.synchronize(dev0)
+
+        def same(g, w):
+            return isinstance(w, torch.Tensor) and w.dtype == torch.float32 and tuple(g.shape) == tuple(w.shape) \
+                and torch.equal(g.cpu().view(torch.int32), w.cpu().contiguous().view(torch.int32))
+
+        if not all(isinstance(w, (tuple, list)) and len(w) == 2 and all(same(*p) for p in zip(g, w))
+                   for g, w in zip(got, want)):
+            raise ValueError(
+                f"@kt.mapped self-check failed for '{getattr(method, '__name__', method)}': the 'retrace' op (gamma="
+                f"{spec.extra['gamma']}, lam={spec.extra['lam']}) does not reproduce the Python body's (returns, td) "
+                f"bit for bit on seeded rollouts; refusing to deploy.  The op computes rlax's retrace_continuous with "
+                f"the declared gamma and lam: traces c = lam * min(1, exp(log_rhos)), the target r[:, t] + "
+                f"gamma * (1 - dones[:, t]) * (values[:, t + 1] - c[:, t + 1] * q[:, t + 1] + c[:, t + 1] * g), "
+                f"bootstrapped from bootstrap_value at the rollout's end, and td = returns - baseline.  It reads "
+                f"dones[:, t] as the done flag of transition t (not a flag that observation t starts an episode: "
+                f"CleanRL's dones become torch.cat([dones[1:], next_done[None]]).T.contiguous())")
+
     # ---- small-call lane (the local CUDA-stream scheduler for launch-bound calls) ----------------------------
     SMALL_CALL_BYTES = 4 << 20
 
@@ -591,6 +652,8 @@ class B200Supervisor:
             return self._call_vtrace(spec, bound, ranks)
         if spec.op == "nstep":
             return self._call_nstep(spec, bound, ranks)
+        if spec.op == "retrace":
+            return self._call_retrace(spec, bound, ranks)
         if spec.op not in ELEMENTWISE_OPS:
             raise TypeError(f"unsupported mapped op '{spec.op}'")
         if not isinstance(x, torch.Tensor):
@@ -794,6 +857,14 @@ class B200Supervisor:
         n = spec.extra["n"]
         return self._call_returns(spec, bound, ranks, ("rewards", "values", "dones", "baseline", "last_values"),
                                   lambda *xs: returns.nstep(*xs[:5], n, *xs[5:]), NSTEP_ARGUMENTS)
+
+    def _call_retrace(self, spec, bound, ranks=None):
+        """(returns, td) per selected rank: one ktb_retrace_f32 launch on the root per run of consecutive selected
+        ranks, as _call_gae."""
+        from ..device import returns
+
+        return self._call_returns(spec, bound, ranks, ("log_rhos", "rewards", "q", "values", "dones", "baseline",
+                                                       "bootstrap_value"), returns.retrace, RETRACE_OPTIONS)
 
     def _call_returns(self, spec, bound, ranks, names, launch, arguments):
         """The first len(names) call arguments, checked to be CUDA tensors on the root GPU, and the options named in
