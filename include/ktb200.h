@@ -1184,6 +1184,47 @@ int ktb_retrace_f32(int dev, const float* log_rhos, const float* rewards, const 
                     const float* dones, const float* baseline, const float* bootstrap, size_t N, size_t T, float gamma,
                     float lam, float* ret, float* td, uintptr_t stream);
 
+/* ---- Prioritized experience replay (the proportional sampler of Ape-X, R2D2 and Rainbow) ----------------------------
+ *
+ * priorities[C] fp32 holds the stored priorities p_i^α of a replay buffer (usually its filled prefix).  Every call is
+ * stateless: it builds the sum tree of the priorities and draws from it.
+ *
+ * ktb_per_sample_f32 draws strata [j0, j0 + rows) of `batch`.  With P = the least power of two >= C and the leaves
+ * priorities[0, C) padded with +0 to P, every node is ONE fp32 add of its two children, left + right, in heap order
+ * (node 1 the root, node n's children 2n and 2n + 1, leaf i node P + i).  tree[max(P, 2)] is fp32 scratch of the
+ * caller's, left holding: tree[0] = min(priorities) (NaN if any is NaN), tree[1] = total (the root; priorities[0] when
+ * C = 1), and tree[n] for 2 <= n < P the internal node n.  Leaves are not copied.  For stratum j, as fp32 operations each
+ * rounded to nearest even, with no FMA contraction (value(n) = tree[n] for n < P, else the padded leaf n − P):
+ *     u     = (2·(x >> 9) + 1)·2^-24, x = word 0 of Philox4x32-10(counter = (j mod 2^32, j >> 32, 0, 4),
+ *             key = (seed mod 2^32, seed >> 32))                     (kubetorch_b200.sampling.replay_noise)
+ *     mass  = ((float)j + u) * (total * (1 / (float)batch))           (1 / batch rounded once to fp32)
+ *     n     = 1;  while n < P:  go = mass >= value(2n) && value(2n + 1) > 0
+ *                               if go: mass = mass - value(2n);   n = 2n + go
+ *     i     = n − P;  indices[j − j0] = i
+ *     weights[j − j0] = pw(priorities[i] / total * (float)C, −beta) / pw(tree[0] / total * (float)C, −beta)
+ * where pw(x, s) is torch's pow of an fp32 CUDA tensor by a scalar: 1 at s = 0, sqrtf(x) at 0.5, rsqrtf(x) at −0.5,
+ * 1 / x at −1, x·x at 2, x·x·x at 3, (float)(1.0 / (double)(x·x)) at −2, powf(x, s) otherwise.  This is bit for bit
+ * the body of tests/policy_per_cases.py run on the GPU when beta is the fp32 rounding of β and β is exactly 0.5, 1 or 2
+ * wherever its rounding is.  A right child is never entered unless its value is > 0 (a NaN never is), so every index
+ * lies in [0, C) whatever the priorities hold; with finite priorities >= 0 and a positive total no zero-priority item
+ * is drawn, and indices never decrease from one stratum to the next.  The noise depends on (seed, j) only: every split
+ * of the strata into calls gives the same bits.
+ *
+ * ktb_per_update_f32 writes priorities[indices[b]] = pw(|td[b]| + eps, alpha) in place for b in [0, B), where an index
+ * repeated in indices takes its LAST occurrence, deterministically.  An index outside [0, C) is skipped: nothing is
+ * written for it (the torch body would raise).  No scratch is needed.
+ *
+ * Checks, in this order: an unregistered dev is KTB_ERR_STATE; a negative or non-finite beta, or a non-finite alpha or
+ * eps, is KTB_ERR_ARG; C outside [1, 2^30], batch or B of 0 or j0 + rows > batch is KTB_ERR_ARG, and batch or B above
+ * 8192 KTB_ERR_UNSUPPORTED; rows == 0 is then KTB_OK with nothing enqueued; otherwise a NULL pointer, or one not 4-byte
+ * aligned (indices: 8-byte), is KTB_ERR_ARG, and so is any overlap of an output (tree, indices, weights; priorities for
+ * the update) with an input or another output.  The draw moves about 4·C + 4·P bytes for the tree and, per stratum,
+ * log2(P) dependent pairs of loads, mostly from L2. */
+int ktb_per_sample_f32(int dev, const float* priorities, size_t C, size_t batch, size_t j0, size_t rows, uint64_t seed,
+                       float beta, float* tree, int64_t* indices, float* weights, uintptr_t stream);
+int ktb_per_update_f32(int dev, float* priorities, size_t C, const int64_t* indices, const float* td, size_t B,
+                       float alpha, float eps, uintptr_t stream);
+
 #ifdef __cplusplus
 }
 #endif

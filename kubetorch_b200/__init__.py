@@ -27,7 +27,7 @@ from .exceptions import (  # noqa: F401
     WorkerMembershipChanged,
 )
 from .mapped import mapped, mapped_spec  # noqa: F401
-from .sampling import explore_noise, gumbel_noise, normal_noise  # noqa: F401
+from .sampling import explore_noise, gumbel_noise, normal_noise, replay_noise  # noqa: F401
 from .resources.callables import Cls, Fn, Module, cls, fn  # noqa: F401
 from .resources.compute import Compute  # noqa: F401
 from .resources.decorators import async_, autoscale, compute, distribute  # noqa: F401

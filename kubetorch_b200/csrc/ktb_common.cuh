@@ -100,6 +100,12 @@ constexpr size_t acc_size(int dtype) {
                                                                      : 0;
 }
 
+// Whether the byte ranges [a, a + an) and [b, b + bn) overlap.
+inline bool overlaps(const void* a, size_t an, const void* b, size_t bn) {
+  const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+  return x < y + bn && y < x + an;
+}
+
 // ---- argument checks of the element-wise entry points (KTB_ERR_ARG with a message naming `who`) ----------------
 inline int check_dtype(const char* who, int dtype) {
   KTB_REQUIRE(dtype_size(dtype) != 0, KTB_ERR_ARG, "%s: unknown dtype %d", who, dtype);
@@ -280,6 +286,20 @@ __device__ __forceinline__ void apply_elem(const uint8_t* src, uint8_t* dst, con
     *reinterpret_cast<unsigned long long*>(dst) =
         apply_i64<OP>(*reinterpret_cast<const unsigned long long*>(src), p);
   }
+}
+
+// Philox4x32-10 (Random123; the round of curand_philox4x32_x.h): the four words of counter c under key k.  The noise
+// of the MLP heads (ktb_mlp.cu) and of the replay sampler (ktb_replay.cu); kubetorch_b200/sampling.py is its twin.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int i = 0; i < 10; ++i) {
+    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
+    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+    k.x += 0x9E3779B9u;
+    k.y += 0xBB67AE85u;
+  }
+  return c;
 }
 
 // ---- PTX: streaming vector loads/stores (no L1 allocation; data is touched once) -------------

@@ -222,19 +222,6 @@ __device__ __forceinline__ bool argmax_before(float v, int col, float best, int 
   return v > best || (v == best && col < best_col);
 }
 
-// Philox4x32-10 (Random123; the round of curand_philox4x32_x.h): the four words of counter c under key k.
-__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
-#pragma unroll
-  for (int i = 0; i < 10; ++i) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c.x), lo0 = 0xD2511F53u * c.x;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c.z), lo1 = 0xCD9E8D57u * c.z;
-    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-    k.x += 0x9E3779B9u;
-    k.y += 0xBB67AE85u;
-  }
-  return c;
-}
-
 // Gumbel noise of one random word: u = (2·(x >> 9) + 1)·2^-24 is exact and strictly inside (0, 1), g = -log(-log u).
 __device__ __forceinline__ float gumbel_of(uint32_t x) {
   const float u = (float)(2u * (x >> 9) + 1u) * 5.9604644775390625e-8f;

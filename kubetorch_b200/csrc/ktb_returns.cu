@@ -312,11 +312,6 @@ __global__ void __launch_bounds__(32)
   }
 }
 
-static bool overlaps(const void* a, size_t an, const void* b, size_t bn) {
-  const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
-  return x < y + bn && y < x + an;
-}
-
 // The pointer, size and overlap checks of a returns entry, in the header's order: NI inputs (the last one [N], the
 // others [N, T]) then two [N, T] outputs, all fp32.  KTB_OK or KTB_ERR_ARG with the message set.
 template <int NI>

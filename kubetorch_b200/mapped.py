@@ -1,6 +1,7 @@
 """Registry of *mapped callables*: user functions whose body is one of the closed set of ops that
 libktb200 executes as sm_90a kernels (identity / scale / affine, their sum-reduced forms, the
-bf16 MLP policy, generalized advantage estimation, V-trace and n-step bootstrapped returns).
+bf16 MLP policy, generalized advantage estimation, V-trace, n-step bootstrapped returns, Retrace(λ) and prioritized
+replay sampling).
 
 Arbitrary Python cannot become a CUDA kernel, so the device route is opt-in by declaration:
 
@@ -25,7 +26,7 @@ from .sampling import _check_seed
 
 MAPPED_ATTR = "__ktb_mapped__"
 ELEMENTWISE_OPS = ("identity", "scale", "affine")
-ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace", "nstep", "retrace")
+ALL_OPS = ELEMENTWISE_OPS + ("mlp", "gae", "vtrace", "nstep", "retrace", "per")
 # The options of op="gae": gamma and lam, each required (a finite number or the name of a call argument holding one),
 # and self_check
 GAE_OPTIONS = ("gamma", "lam")
@@ -41,6 +42,10 @@ NSTEP_ARGUMENTS = ("gamma",)
 # The options of op="retrace": gamma and lam, each required (a finite number or the name of a call argument holding
 # one), and self_check
 RETRACE_OPTIONS = ("gamma", "lam")
+# The options of op="per" beside self_check, all required: batch an int constant in [1, 8192], beta a finite number >= 0
+# and seed an int in [0, 2**64), each of the last two or the name of a call argument holding one (PER_ARGUMENTS)
+PER_OPTIONS = ("batch", "beta", "seed")
+PER_ARGUMENTS = ("beta", "seed")
 MLP_OUTPUTS = ("logits", "actions", "both", "sample", "gaussian", "epsilon_greedy", "evaluate",
                "gaussian_evaluate", "deterministic", "critic", "td_target", "dqn_target")   # also device.mlp.OUTPUTS
 EVALUATE_OUTPUTS = ("evaluate", "gaussian_evaluate")
@@ -373,7 +378,24 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
     ``x.T.contiguous()``, and CleanRL-style episode-start flags become ``torch.cat([dones[1:],
     next_done[None]]).T.contiguous()`` as for "gae".  ``gamma=`` and ``lam=`` are required, each a finite number or the
     name of a call argument that holds one (checked per call); ``self_check=False`` skips the deployment's check of a
-    constant γ and λ against the body.  Every other option is refused."""
+    constant γ and λ against the body.  Every other option is refused.
+
+    The "per" op is prioritized experience replay's proportional sampler (Schaul et al. 2016; Ape-X, R2D2, Rainbow):
+    the callable is ``(priorities, ...)`` with fp32 ``[C]`` priorities, the stored ``p_i^α`` of a replay buffer
+    (usually its filled prefix ``prio[:size]``), a CUDA tensor on the root GPU.  Each rank returns ``(indices,
+    weights)`` for its strata ``torch.arange(batch).chunk(WORLD_SIZE)[RANK]``: the body builds the sum tree of the
+    priorities, each node one fp32 add of its two children over the leaves padded with +0 to a power of two, and
+    stratum j descends it from the mass ``(j + u) * (total / batch)``, ``u = kubetorch_b200.sampling.replay_noise(seed,
+    j, 1)``, stepping right where ``mass >= left`` and the right child is > 0; int64 ``indices`` and fp32 importance
+    weights ``(p_i / total * C) ** -beta / (min p / total * C) ** -beta``, bit for bit as torch computes them on the GPU
+    (tests/policy_per_cases.py).  Every index lies in [0, C), no zero-priority item is drawn while the total is
+    positive and finite, and the noise depends on (seed, j) only, so every rank count draws the same batch.
+    ``batch=`` is a required int constant in [1, 8192]; ``beta=`` a required number >= 0 or the name of a call
+    argument that holds one (PER's annealed β), and ``seed=`` a required int in [0, 2**64) or the name of a call
+    argument that holds one (a new seed for every batch).  ``self_check=False`` skips the deployment's check of the
+    body.  Every other option is refused.  The priority update that follows the learner step is
+    ``kubetorch_b200.device.replay.per_update(priorities, indices, td, alpha, eps)``, a device call rather than a
+    mapped op: it writes the caller's tensor in place."""
     if op not in ALL_OPS:
         raise ValueError(f"unknown mapped op '{op}'; expected one of {ALL_OPS}")
     if op == "gae":
@@ -384,6 +406,9 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
         _check_nstep_options(alpha, beta, reduce, arg, extra)
     if op == "retrace":
         _check_retrace_options(alpha, beta, reduce, arg, extra)
+    if op == "per":
+        _check_per_options(alpha, beta, reduce, arg, extra)
+        beta = _UNSET   # extra keeps it
     beta = 0.0 if beta is _UNSET else beta
     if op == "mlp" and extra.get("output") == "td_target" and alpha is not _UNSET:   # SAC's α, an option of the head
         extra["alpha"] = alpha
@@ -435,8 +460,11 @@ def mapped(op: str, alpha: Any = _UNSET, beta: Any = _UNSET, reduce: Optional[st
             raise ValueError(f"a 'retrace' callable takes (log_rhos, rewards, q, values, dones, baseline, "
                              f"bootstrap_value, ...) positionally, {getattr(fn, '__name__', fn)!r} has {len(params)} "
                              f"parameters")
+        if op == "per" and len(params) < 1:
+            raise ValueError(f"a 'per' callable takes (priorities, ...) positionally, {getattr(fn, '__name__', fn)!r} "
+                             f"has no parameters")
         for option, names in extra.items():
-            if not (isinstance(names, str) if op in ("gae", "vtrace", "nstep", "retrace")
+            if not (isinstance(names, str) if op in ("gae", "vtrace", "nstep", "retrace", "per")
                     else names_arguments(option, names)):
                 continue
             for name in (names,) if isinstance(names, str) else names:
@@ -535,6 +563,41 @@ def _check_retrace_options(alpha, beta, reduce, arg, extra) -> None:
             check_finite(name, extra[name])
     if not isinstance(extra.get("self_check", False), bool):
         raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
+
+
+def _check_per_options(alpha, beta, reduce, arg, extra) -> None:
+    """The options of op="per", or ValueError naming the first it does not take or the first it lacks: batch an int
+    constant in [1, 8192], a constant beta a finite number >= 0 and a constant seed an int in [0, 2**64).  Moves beta
+    into extra, which keeps every option."""
+    refused = dict(alpha=alpha is not _UNSET, reduce=reduce is not None, arg=arg is not None)
+    refused.update((k, True) for k in extra if k not in PER_OPTIONS + ("self_check",))
+    for name, given in refused.items():
+        if given:
+            raise ValueError(f"{name}= is not an option of the 'per' op, which takes batch=, beta=, seed= and "
+                             f"self_check=: its callable is (priorities, ...) and it returns (indices, weights)")
+    if beta is not _UNSET:
+        extra["beta"] = beta
+    for name in PER_OPTIONS:
+        if name not in extra:
+            raise ValueError(f"{name}= is required with the 'per' op: " + (
+                "an int constant in [1, 8192]" if name == "batch" else "a constant or the name of a call argument"))
+    n = extra["batch"]
+    if isinstance(n, bool) or not isinstance(n, int) or not 1 <= n <= 8192:
+        raise ValueError(f"batch must be an int constant in [1, 8192] (not the name of a call argument), got {n!r}")
+    if not isinstance(extra["beta"], str):
+        check_beta(extra["beta"])
+    if not isinstance(extra["seed"], str):
+        _check_seed(extra["seed"])
+    if not isinstance(extra.get("self_check", False), bool):
+        raise ValueError(f"self_check must be True or False, got {extra['self_check']!r}")
+
+
+def check_beta(v):
+    """PER's β: a finite number (not a bool) >= 0."""
+    check_finite("beta", v)
+    if not v >= 0:
+        raise ValueError(f"beta must be >= 0, got {v!r}")
+    return v
 
 
 def check_threshold(name: str, v):

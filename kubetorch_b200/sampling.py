@@ -1,5 +1,5 @@
-"""The Gumbel noise of @kt.mapped("mlp", output="sample"), the Gaussian noise of output="gaussian" and the exploration
-draws of output="epsilon_greedy", in plain torch (no GPU, no library).
+"""The Gumbel noise of @kt.mapped("mlp", output="sample"), the Gaussian noise of output="gaussian", the exploration
+draws of output="epsilon_greedy" and the stratum offsets of @kt.mapped("per"), in plain torch (no GPU, no library).
 
 A sampled policy body adds ``gumbel_noise(seed, row0, rows, d_out)`` to its fp32 logits, takes the argmax and gathers
 the log_softmax; a Gaussian policy body adds ``exp(log_std)·normal_noise(seed, row0, rows, d_out)`` to its mean; an
@@ -16,6 +16,8 @@ legal column with the largest word ``w``.  The device kernel draws the very same
                 "deterministic", scaled by σ and clipped)
     explore 2   the word x itself (a uint32): ranks the legal columns of an exploring row of output="epsilon_greedy"
     coin    3   u of column 0 only (one draw per row): the row explores iff u < ε in fp32
+    replay  4   u of column 0 only, with i the global stratum of a prioritized replay batch (replay_noise): the
+                stratum's draw lands at mass (i + u)·(total / batch) of the sum tree
 
 The noise depends on (seed, i, j) only, so every sharding of the rows draws the same noise for the same row.
 """
@@ -58,7 +60,8 @@ def _check_seed(seed) -> int:
 
 def random_words(seed: int, row_offset: int, rows: int, cols: int, device="cpu", word3: int = 0) -> torch.Tensor:
     """int64 [rows, cols]: the 32-bit Philox word of global row row_offset + r and column j.  `word3` is the fourth
-    counter word: 0 for the Gumbel noise, 1 for the Gaussian noise, 2 for the exploration words, 3 for the coin."""
+    counter word: 0 for the Gumbel noise, 1 for the Gaussian noise, 2 for the exploration words, 3 for the coin, 4 for
+    the replay strata."""
     seed = _check_seed(seed)
     if row_offset < 0 or rows < 0 or cols < 0:
         raise ValueError("row_offset, rows and cols must be non-negative")
@@ -101,3 +104,10 @@ def explore_noise(seed: int, row_offset: int, rows: int, cols: int, device="cpu"
     ties to the lower column).  Neither stream reuses the Gumbel (0) or Gaussian (1) draws of the same seed."""
     u = gumbel_uniform(seed, row_offset, rows, 1, device, word3=3)[:, 0]
     return u, random_words(seed, row_offset, rows, cols, device, word3=2)
+
+
+def replay_noise(seed: int, row0: int, rows: int, device="cpu") -> torch.Tensor:
+    """float32 [rows]: the offsets u of strata row0 .. row0 + rows - 1 of @kt.mapped("per"), the exact uniform of word 0
+    of counter (j, 0, 4), strictly inside (0, 1).  Stratum j draws at mass (j + u)·(total / batch) of the sum tree.  The
+    stream reuses none of the Gumbel (0), Gaussian (1), exploration (2) or coin (3) draws of the same seed."""
+    return gumbel_uniform(seed, row0, rows, 1, device, word3=4)[:, 0]

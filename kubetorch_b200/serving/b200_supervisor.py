@@ -44,6 +44,8 @@ One controller process drives N local H100s.  For a @kt.mapped callable a remote
         ktb_nstep_f32: the same, one launch on the root GPU.
     "retrace"
         ktb_retrace_f32: the same, one launch on the root GPU.
+    "per"
+        ktb_per_sample_f32: one launch on the root GPU over every selected rank's strata.
 
 There is NO CPU fallback here: a missing library or GPU raises.
 """
@@ -58,8 +60,9 @@ from typing import List, Optional
 
 from ..distributed import local_pod_ips
 from ..exceptions import PodTerminatedError, SerializationError
-from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, NSTEP_ARGUMENTS, RETRACE_OPTIONS,
-                      TD_OPTIONS, VTRACE_ARGUMENTS, VTRACE_OPTIONS, check_finite, mapped_spec, names_arguments)
+from ..mapped import (DQN_OPTIONS, ELEMENTWISE_OPS, GAE_OPTIONS, MLP_FORMS, NSTEP_ARGUMENTS, PER_ARGUMENTS,
+                      RETRACE_OPTIONS, TD_OPTIONS, VTRACE_ARGUMENTS, VTRACE_OPTIONS, check_finite, mapped_spec,
+                      names_arguments)
 from .codec import HTTPException, check_allowed
 from .process_worker import instantiate, load_callable, load_callable_from_env, resolve_method
 from .supervisors import check_callable_name, select_worker_nodes
@@ -211,6 +214,8 @@ class B200Supervisor:
                 self._self_check_nstep(spec, method)
             if spec.op == "retrace" and spec.extra.get("self_check") is not False:
                 self._self_check_retrace(spec, method)
+            if spec.op == "per" and spec.extra.get("self_check") is not False:
+                self._self_check_per(spec, method)
             if spec.op not in ELEMENTWISE_OPS or spec.extra.get("self_check") is False:
                 continue
             if not (isinstance(spec.alpha, (int, float)) and isinstance(spec.beta, (int, float))):
@@ -476,6 +481,70 @@ class B200Supervisor:
                 f"dones[:, t] as the done flag of transition t (not a flag that observation t starts an episode: "
                 f"CleanRL's dones become torch.cat([dones[1:], next_done[None]]).T.contiguous())")
 
+    def _self_check_per(self, spec, method):
+        """A "per" callable: its body on the root GPU, rank by rank, against the kernel, refusing the deployment on any
+        bit difference.  The body runs on the GPU because its pow is CUDA's there.  The check passes its own seed and
+        its own β where those name call arguments, and calls the body with the priorities and those arguments only (a
+        body that needs more is not checked).  Two priority vectors of C = 1000, not a power of two: seeded values with
+        30 % zeros, index 0 among them, and one dominant item; and the same zeros with every other item the least
+        subnormal, where every mass and every partial sum is a whole number of that subnormal, so that masses equal
+        left sums and `mass >= left` decides the descent.  This catches uniform in place of stratified draws, rank-local strata, `mass > left`,
+        weights not divided by the largest one, and another noise stream."""
+        import inspect
+
+        import torch
+
+        params = list(inspect.signature(method).parameters)
+        given = {v: 8675309 if k == "seed" else 0.6 for k, v in spec.extra.items() if k in PER_ARGUMENTS
+                 and isinstance(v, str)}
+        if len(params) != 1 + len(given):
+            return   # the body takes arguments the check cannot supply
+        world, dev0 = self.world_size, self.devices[0]
+        gen = torch.Generator().manual_seed(1234)
+        c = 1000
+        prio = torch.rand(c, generator=gen) * 2
+        prio[torch.rand(c, generator=gen) < 0.3] = 0.0
+        prio[0] = 0.0
+        prio[617] = 500.0
+        tiny = torch.where(prio > 0, torch.tensor(1e-45), torch.tensor(0.0))
+        for p in (prio, tiny):
+            p = p.to(f"cuda:{dev0}")
+            kwargs = {params[0]: p, **given}
+            saved = {k: os.environ.get(k) for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK")}
+            want = []
+            try:
+                with torch.cuda.device(dev0):
+                    for r in range(world):
+                        os.environ.update({"RANK": str(r), "WORLD_SIZE": str(world), "LOCAL_RANK": str(r)})
+                        want.append(method(**{k: v.clone() if isinstance(v, torch.Tensor) else v
+                                              for k, v in kwargs.items()}))
+            except Exception:  # noqa: BLE001 - a body that cannot run here (needs a group, ...) is skipped
+                return
+            finally:
+                for k, v in saved.items():
+                    if v is None:
+                        os.environ.pop(k, None)
+                    else:
+                        os.environ[k] = v
+            got = self._run_mapped(spec, method, [], kwargs, list(range(world)))
+            self.ops.synchronize(dev0)
+
+            def same(g, w, dtype):
+                return isinstance(w, torch.Tensor) and w.dtype == dtype and tuple(g.shape) == tuple(w.shape) \
+                    and torch.equal(g.cpu().view(torch.int32 if dtype == torch.float32 else dtype),
+                                    w.cpu().contiguous().view(torch.int32 if dtype == torch.float32 else dtype))
+
+            if not all(isinstance(w, (tuple, list)) and len(w) == 2 and same(g[0], w[0], torch.int64)
+                       and same(g[1], w[1], torch.float32) for g, w in zip(got, want)):
+                raise ValueError(
+                    f"@kt.mapped self-check failed for '{getattr(method, '__name__', method)}': the 'per' op (batch="
+                    f"{spec.extra['batch']}, beta={spec.extra['beta']}, seed={spec.extra['seed']}) does not reproduce "
+                    f"the Python body's (indices, weights) bit for bit on seeded priorities; refusing to deploy.  The "
+                    f"op draws stratum j of torch.arange(batch).chunk(WORLD_SIZE)[RANK] (the global j) from the sum "
+                    f"tree at mass (j + u) * (total / batch) with u = kubetorch_b200.sampling.replay_noise(seed, j, 1), "
+                    f"steps right where mass >= left and the right child is > 0, and weights each draw by "
+                    f"(p / total * C) ** -beta / (min p / total * C) ** -beta")
+
     # ---- small-call lane (the local CUDA-stream scheduler for launch-bound calls) ----------------------------
     SMALL_CALL_BYTES = 4 << 20
 
@@ -654,6 +723,8 @@ class B200Supervisor:
             return self._call_nstep(spec, bound, ranks)
         if spec.op == "retrace":
             return self._call_retrace(spec, bound, ranks)
+        if spec.op == "per":
+            return self._call_per(spec, bound, ranks)
         if spec.op not in ELEMENTWISE_OPS:
             raise TypeError(f"unsupported mapped op '{spec.op}'")
         if not isinstance(x, torch.Tensor):
@@ -865,6 +936,37 @@ class B200Supervisor:
 
         return self._call_returns(spec, bound, ranks, ("log_rhos", "rewards", "q", "values", "dones", "baseline",
                                                        "bootstrap_value"), returns.retrace, RETRACE_OPTIONS)
+
+    def _call_per(self, spec, bound, ranks=None):
+        """(indices, weights) per selected rank: one ktb_per_sample_f32 launch on the root over the strata of every run
+        of consecutive selected ranks (all `batch` strata when every rank is selected), each launch building the tree
+        of the priorities, the first call argument, a CUDA tensor on the root GPU.  beta and seed are the constants
+        declared or the call arguments they name."""
+        import torch
+
+        from ..device import replay
+
+        prio = bound[next(iter(bound))]
+        root = self.devices[0]
+        if not isinstance(prio, torch.Tensor) or not prio.is_cuda or prio.device.index != root:
+            where = prio.device if isinstance(prio, torch.Tensor) else type(prio).__name__
+            raise ValueError(f"the 'per' op takes CUDA tensors on the root GPU cuda:{root}: priorities is on {where} "
+                             f"(host tensors are not staged for this op)")
+        batch = spec.extra["batch"]
+        beta, seed = (bound[v] if isinstance(v, str) else v for v in (spec.extra[k] for k in PER_ARGUMENTS))
+        ranks = list(range(self.world_size)) if ranks is None else list(ranks)
+        bounds = [self.ops.shard_bounds(batch, self.world_size, r) for r in ranks]
+        out = []
+        i = 0
+        while i < len(ranks):   # one launch per run of consecutive ranks
+            j = i
+            while j + 1 < len(ranks) and ranks[j + 1] == ranks[j] + 1:
+                j += 1
+            b, e = bounds[i][0], bounds[j][1]
+            idx, w = replay.per_sample(prio, batch, seed, beta, j0=b, rows=e - b)
+            out += [(idx[rb - b:re - b], w[rb - b:re - b]) for rb, re in bounds[i:j + 1]]
+            i = j + 1
+        return out
 
     def _call_returns(self, spec, bound, ranks, names, launch, arguments):
         """The first len(names) call arguments, checked to be CUDA tensors on the root GPU, and the options named in
