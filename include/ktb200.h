@@ -1206,8 +1206,9 @@ int ktb_retrace_f32(int dev, const float* log_rhos, const float* rewards, const 
  * 1 / x at −1, x·x at 2, x·x·x at 3, (float)(1.0 / (double)(x·x)) at −2, powf(x, s) otherwise.  This is bit for bit
  * the body of tests/policy_per_cases.py run on the GPU when beta is the fp32 rounding of β and β is exactly 0.5, 1 or 2
  * wherever its rounding is.  A right child is never entered unless its value is > 0 (a NaN never is), so every index
- * lies in [0, C) whatever the priorities hold; with finite priorities >= 0 and a positive total no zero-priority item
- * is drawn, and indices never decrease from one stratum to the next.  The noise depends on (seed, j) only: every split
+ * lies in [0, C) whatever the priorities hold; with finite priorities >= 0 and a positive, finite total no zero-priority
+ * item is drawn (a total that overflows to inf makes mass inf - inf = NaN wherever a left child is inf, and a NaN mass
+ * steps left, into zero priorities too), and indices never decrease from one stratum to the next.  The noise depends on (seed, j) only: every split
  * of the strata into calls gives the same bits.
  *
  * ktb_per_update_f32 writes priorities[indices[b]] = pw(|td[b]| + eps, alpha) in place for b in [0, B), where an index
